@@ -36,7 +36,7 @@
 extern "C" {
 #endif
 
-#define NR_B200_ABI_VERSION 3
+#define NR_B200_ABI_VERSION 4
 
 #if defined(__GNUC__)
 #define NR_B200_API __attribute__((visibility("default")))
@@ -83,6 +83,20 @@ extern "C" {
                                        /* (DESIGN.md section 4), hence opt-in.  Ignored when the cube size is not a multiple of   */
                                        /* 16 bytes or `textures` is not 16-byte aligned.                                           */
 
+/* ABI 4: UV-mapped texture image instead of per-face cubes.
+ *   `textures` / `grad_textures` are the image [Bt,Ht,Wt,3] float32, HWC, row 0 = TOP row (as a PNG is read); Bt = B, or
+ *   1 with NR_TEX_SHARED (one image for every item; its gradient is the sum over the items).  `face_uvs` holds the UV of
+ *   every face corner, OBJ convention (v = 0 is the BOTTOM of the image).  texture_size is ignored.
+ *   Covered pixel with winner weights w_k, depth zp and the winner's OWN vertex depths z_k (NR_TEX_Z_BATCH0 has no
+ *   effect on this sampler):  l_k = w_k * (zp / z_k)  (div.rn),  uv = l_0 uv_0 + l_1 uv_1 + l_2 uv_2  (not renormalised).
+ *   Addressing as nr_b200_bake_textures: u, v clamped into [0,1] (NaN -> 0), pos_x = u (Wt-1), pos_y = v (Ht-1); taps
+ *   ix, ix+1 / iy, iy+1 (clamped into the image; tap row iy is image row Ht-1-iy); bilinear weights products of frac and
+ *   1 - frac; fp32, round-to-nearest; clamp to edge only (no wrap, no mipmaps).  face_light multiplies every tap first.
+ *   With NR_TEX_FILL_BACK face f >= F/2 uses the UV corners of face f - F/2 in reverse order (`face_uvs` holds F/2 faces).
+ *   The backward fills grad_textures (the image gradient) and grad_face_light; there is NO gradient for face_uvs. */
+#define NR_TEX_UV 0x20000u    /* sample a texture image through per-corner UVs (fields face_uvs / texture_height / _width) */
+#define NR_UV_SHARED 0x40000u /* face_uvs is [F,3,2] and serves every batch item (else [B,F,3,2])                        */
+
 typedef struct nr_b200_forward_args {
     uint32_t struct_size; /* sizeof(nr_b200_forward_args), for ABI evolution */
     uint32_t flags;
@@ -121,6 +135,10 @@ typedef struct nr_b200_forward_args {
     const int32_t *face_indices; /* [B,F,3], or [F,3] with NR_INDICES_SHARED */
     int32_t num_vertices;        /* Nv */
     int32_t _pad1;
+    /* ABI 4: texture image, only with NR_TEX_UV (then `textures` is the image [Bt,Ht,Wt,3]) */
+    const float *face_uvs;  /* [B,F,3,2], or [F,3,2] with NR_UV_SHARED (F/2 faces with NR_TEX_FILL_BACK) */
+    int32_t texture_height; /* Ht >= 1 */
+    int32_t texture_width;  /* Wt >= 1 */
 } nr_b200_forward_args;
 
 typedef struct nr_b200_backward_args {
@@ -154,6 +172,10 @@ typedef struct nr_b200_backward_args {
     float *grad_vertices; /* [B,Nv,3] */
     int32_t num_vertices;
     int32_t _pad1;
+    /* ABI 4: as in the forward call; with NR_TEX_UV grad_textures is the image gradient [Bt,Ht,Wt,3] */
+    const float *face_uvs;
+    int32_t texture_height;
+    int32_t texture_width;
 } nr_b200_backward_args;
 
 /* ABI version of the loaded library (== NR_B200_ABI_VERSION it was built with). */

@@ -28,8 +28,10 @@ NR_TEX_SHARED = 0x2000
 NR_BWD_PART_TEXTURES = 0x4000
 NR_BWD_PART_FACES = 0x8000
 NR_FWD_STAGE_TEXTURES = 0x10000
+NR_TEX_UV = 0x20000
+NR_UV_SHARED = 0x40000
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 
 # every symbol include/nr_b200.h declares
 EXPORTED_SYMBOLS = (
@@ -67,6 +69,7 @@ class ForwardArgs(ctypes.Structure):
         ("face_light", ctypes.c_void_p),
         ("vertices", ctypes.c_void_p), ("face_indices", ctypes.c_void_p),
         ("num_vertices", ctypes.c_int32), ("_pad1", ctypes.c_int32),
+        ("face_uvs", ctypes.c_void_p), ("texture_height", ctypes.c_int32), ("texture_width", ctypes.c_int32),
     ]
 
 
@@ -85,6 +88,7 @@ class BackwardArgs(ctypes.Structure):
         ("face_light", ctypes.c_void_p), ("grad_face_light", ctypes.c_void_p),
         ("vertices", ctypes.c_void_p), ("face_indices", ctypes.c_void_p), ("grad_vertices", ctypes.c_void_p),
         ("num_vertices", ctypes.c_int32), ("_pad1", ctypes.c_int32),
+        ("face_uvs", ctypes.c_void_p), ("texture_height", ctypes.c_int32), ("texture_width", ctypes.c_int32),
     ]
 
 

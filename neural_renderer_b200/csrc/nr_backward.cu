@@ -25,6 +25,8 @@
 //                     per-face light factor / fill_back cube sharing of the forward sampler and reduces d loss /
 //                     d face_light per run of lanes; neighbouring lanes that blend the same eight texels merge their
 //                     contributions with shuffles before the reductions.
+//   k_image_grad      K6 for a texture image sampled through per-corner UVs (NR_TEX_UV): four bilinear taps per pixel,
+//                     two 6-float horizontal pairs scattered the same way.
 //   k_depth_grad      K7 (rasterize.py:805-847): analytic d zp / d(x, y, z) of the winning face, summed per run of
 //                     neighbouring lanes that show the same face before the atomics.
 //
@@ -65,6 +67,9 @@
 #endif
 #ifndef NR_TG_MIN_CTAS
 #define NR_TG_MIN_CTAS 6
+#endif
+#ifndef NR_IG_MIN_CTAS
+#define NR_IG_MIN_CTAS 4        // k_image_grad CTAs of 256 threads per SM (64 registers; see DESIGN.md section 4)
 #endif
 
 namespace {
@@ -116,6 +121,10 @@ struct BwdParams {
 #endif
     uint32_t flags;
     float eps, two_over_S, tex_cmp, tex_val;
+    // NR_TEX_UV (appended, so the cube variants keep their parameter offsets): textures / grad_textures = image [Bt,Ht,Wt,3]
+    const float* uvs;
+    uint32_t uv_bstride, img_bstride;  // floats per item (0 = shared)
+    int Ht, Wt;
 };
 
 //@phase helpers: rcp / vector RED / load_grad (inlined)
@@ -1042,6 +1051,143 @@ __global__ void __launch_bounds__(256, kTgCombine ? 4 : NR_TG_MIN_CTAS) k_textur
     }
 }
 
+// ----------------------------------------------------------------------------------------------- k_image_grad
+// NR_TEX_UV counterpart of K6, one thread per raster pixel in the same row-major map.  The pixel's uv and its four
+// bilinear taps are recomputed from the saved weight / depth maps and the winner's own vertex depths with the forward's
+// helpers (nr_math.cuh), and w_xy * light * grad_rgb goes to the taps: per tap row one horizontal pair = 6 consecutive
+// floats, scattered with vector reductions by alignment as in K6.  A shared image receives from every item, so lanes
+// next to each other that hit the same (image, cell) first merge their contributions (kTgCombine shuffle steps).
+__device__ __forceinline__ void red_add_6(float* t, const float v[6]) {
+    switch ((reinterpret_cast<uintptr_t>(t) >> 2) & 3) {
+        case 0: red_add_v4(t, v[0], v[1], v[2], v[3]); red_add_v2(t + 4, v[4], v[5]); break;
+        case 2: red_add_v2(t, v[0], v[1]); red_add_v4(t + 2, v[2], v[3], v[4], v[5]); break;
+        case 3: atomicAdd(t, v[0]); red_add_v4(t + 1, v[1], v[2], v[3], v[4]); atomicAdd(t + 5, v[5]); break;
+        default: atomicAdd(t, v[0]); red_add_v2(t + 1, v[1], v[2]); red_add_v2(t + 3, v[3], v[4]); atomicAdd(t + 5, v[5]); break;
+    }
+}
+
+template <int kTgCombine>
+__global__ void __launch_bounds__(256, NR_IG_MIN_CTAS) k_image_grad(const __grid_constant__ BwdParams p) {
+    const int S = p.S;
+    const size_t plane = (size_t)S * S;
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;  // pixel within the image (image orientation)
+    const int b = blockIdx.y;
+    const int lane = threadIdx.x & 31;
+    const int fn = (i < plane) ? __ldg(p.fim + (size_t)b * plane + i) : -1;
+    const bool want_light = p.grad_face_light != nullptr;  // uniform
+    if (!want_light && !__any_sync(0xffffffffu, fn >= 0)) return;  // warp-uniform
+    float gl0 = 0.0f, gl1 = 0.0f, gl2 = 0.0f;  // d loss / d face_light of this pixel
+    float val[2][6];                           // tap row 0 / 1: taps (x0, x1) x 3 channels
+    float* tp[2] = {nullptr, nullptr};
+    bool adjacent = true;                      // x1 == x0 + 1 (else both taps of a row are the same texel, weight 0 on x1)
+    long long key = -1 - (long long)lane;      // (image, cell): equal keys <=> the same four texels
+#pragma unroll
+    for (int r = 0; r < 2; r++)
+#pragma unroll
+        for (int k = 0; k < 6; k++) val[r][k] = 0.0f;
+    if (fn >= 0) {
+        const int row = (int)(i / S), col = (int)(i % S);
+        const bool aa = (p.flags & NR_ANTI_ALIASING) != 0;
+        float g0 = load_grad(p.g_rgb, aa, S, (size_t)b * 3 + 0, row, col);
+        float g1 = load_grad(p.g_rgb, aa, S, (size_t)b * 3 + 1, row, col);
+        float g2 = load_grad(p.g_rgb, aa, S, (size_t)b * 3 + 2, row, col);
+        const float* wm = p.wmap + (size_t)b * 3 * plane + i;
+        const float w[3] = {__ldg(wm), __ldg(wm + plane), __ldg(wm + 2 * plane)};
+        const float zp = __ldg(p.dmap + (size_t)b * plane + i);
+        float z0, z1, z2;  // the item's own vertex depths, as in the forward sampler
+        if (p.src.idx == nullptr) {
+            const float* v = p.src.faces + ((size_t)b * p.F + fn) * 9;
+            z0 = __ldg(v + 2); z1 = __ldg(v + 5); z2 = __ldg(v + 8);
+        } else {
+            z0 = __ldg(nr::face_vertex_t<true>(p.src, b, fn, 0) + 2);
+            z1 = __ldg(nr::face_vertex_t<true>(p.src, b, fn, 1) + 2);
+            z2 = __ldg(nr::face_vertex_t<true>(p.src, b, fn, 2) + 2);
+        }
+        int uf = fn;
+        bool rev = false;
+        if (p.flags & NR_TEX_FILL_BACK) {
+            const int half = p.F >> 1;
+            if (fn >= half) { uf = fn - half; rev = true; }
+        }
+        float uv[6], u, v;
+        nr::load_face_uvs(p.uvs + ((uint32_t)b * p.uv_bstride + (uint32_t)uf * 6u), rev, uv);
+        nr::pixel_uv(w, zp, z0, z1, z2, uv, u, v);
+        const nr::UvTaps t = nr::uv_taps(u, v, p.Ht, p.Wt);
+        const uint32_t img_off = (uint32_t)b * p.img_bstride;
+        if (want_light) {  // unlit sample (same blend as the forward pass) times the upstream gradient
+            float c[3];
+            nr::uv_blend<false>(p.textures + img_off, p.Wt, t, 1.0f, 1.0f, 1.0f, c);
+            gl0 = c[0] * g0; gl1 = c[1] * g1; gl2 = c[2] * g2;
+        }
+        if (p.face_light) {  // d rgb / d texel = weight * light
+            const float* lp = p.face_light + ((size_t)b * p.F + fn) * 3;
+            g0 *= __ldg(lp); g1 *= __ldg(lp + 1); g2 *= __ldg(lp + 2);
+        }
+        const uint32_t row3 = (uint32_t)p.Wt * 3u;
+        float* gi = p.grad_textures + img_off;
+        tp[0] = gi + (uint32_t)t.r0 * row3 + (uint32_t)t.x0 * 3u;
+        tp[1] = gi + (uint32_t)t.r1 * row3 + (uint32_t)t.x0 * 3u;
+        adjacent = t.x1 != t.x0;
+        key = (long long)(img_off / 3u) + t.cell;
+        val[0][0] = t.w00 * g0; val[0][1] = t.w00 * g1; val[0][2] = t.w00 * g2;
+        val[0][3] = t.w10 * g0; val[0][4] = t.w10 * g1; val[0][5] = t.w10 * g2;
+        val[1][0] = t.w01 * g0; val[1][1] = t.w01 * g1; val[1][2] = t.w01 * g2;
+        val[1][3] = t.w11 * g0; val[1][4] = t.w11 * g1; val[1][5] = t.w11 * g2;
+    }
+    bool issue = fn >= 0;
+    if (kTgCombine) {
+        // runs of neighbouring lanes with the same key (segmented shuffle of k_texture_grad)
+        const long long key_prev = __shfl_up_sync(0xffffffffu, key, 1);
+        const uint32_t heads = __ballot_sync(0xffffffffu, lane == 0 || key != key_prev);
+        const uint32_t later = heads & ~((2u << lane) - 1u);
+        const int run_end = (lane == 31 || later == 0) ? 31 : (__ffs(later) - 2);
+        const int run_start = 31 - __clz(heads & ((2u << lane) - 1u));
+        if (heads != 0xffffffffu) {  // warp-uniform: somebody has a neighbour to merge with
+#pragma unroll
+            for (int step = 0; step < kTgCombine; step++) {
+                const int off = 1 << step;
+                const bool take = lane + off <= run_end;
+#pragma unroll
+                for (int r = 0; r < 2; r++)
+#pragma unroll
+                    for (int k = 0; k < 6; k++) {
+                        const float x = __shfl_down_sync(0xffffffffu, val[r][k], off);
+                        if (take) val[r][k] += x;
+                    }
+            }
+            issue = issue && (((lane - run_start) & ((1 << kTgCombine) - 1)) == 0);
+        }
+    }
+    if (issue) {
+#pragma unroll
+        for (int r = 0; r < 2; r++) {
+            if (adjacent) {
+                red_add_6(tp[r], val[r]);
+            } else {
+                float* q = tp[r];
+                atomicAdd(q, val[r][0] + val[r][3]); atomicAdd(q + 1, val[r][1] + val[r][4]); atomicAdd(q + 2, val[r][2] + val[r][5]);
+            }
+        }
+    }
+    if (!want_light) return;
+    // warp-aggregated scatter of the light gradient: runs of neighbouring lanes that show the same face
+    const int fn_prev = __shfl_up_sync(0xffffffffu, fn, 1);
+    const uint32_t heads = __ballot_sync(0xffffffffu, lane == 0 || fn != fn_prev);
+    const uint32_t later = heads & ~((2u << lane) - 1u);
+    const int run_end = (lane == 31 || later == 0) ? 31 : (__ffs(later) - 2);
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+        const bool take = lane + off <= run_end;
+        const float t0 = __shfl_down_sync(0xffffffffu, gl0, off), t1 = __shfl_down_sync(0xffffffffu, gl1, off),
+                    t2 = __shfl_down_sync(0xffffffffu, gl2, off);
+        if (take) { gl0 += t0; gl1 += t1; gl2 += t2; }
+    }
+    if (fn >= 0 && ((heads >> lane) & 1u)) {
+        float* gl = p.grad_face_light + ((size_t)b * p.F + fn) * 3;
+        atomicAdd(gl, gl0); atomicAdd(gl + 1, gl1); atomicAdd(gl + 2, gl2);
+    }
+}
+
 // ----------------------------------------------------------------------------------------------- k_depth_grad
 __global__ void __launch_bounds__(256) k_depth_grad(const __grid_constant__ BwdParams p) {
     const int S = p.S;
@@ -1211,20 +1357,27 @@ extern "C" int nr_b200_backward(const nr_b200_backward_args* a, void* cuda_strea
     if (part_faces && !nr_internal::make_face_grad(flags, a->grad_faces, a->grad_vertices, a->face_indices, F, a->num_vertices, &dst))
         return NR_ERR_INVALID_ARG;
     const bool rgb = (flags & NR_RETURN_RGB) != 0, alpha = (flags & NR_RETURN_ALPHA) != 0, depth = (flags & NR_RETURN_DEPTH) != 0;
-    if (rgb && (!a->rgb_map || ts < 2)) return NR_ERR_INVALID_ARG;
+    const bool uv = (flags & NR_TEX_UV) != 0;
+    if (uv && (!rgb || !a->face_uvs || a->texture_height < 1 || a->texture_width < 1)) return NR_ERR_INVALID_ARG;
+    if (rgb && (!a->rgb_map || (!uv && ts < 2))) return NR_ERR_INVALID_ARG;
     if (rgb && part_tex && !a->grad_textures) return NR_ERR_INVALID_ARG;
     if (rgb && (flags & NR_TEX_FILL_BACK) && (F & 1)) return NR_ERR_INVALID_ARG;
     if (rgb && a->grad_face_light && !a->textures) return NR_ERR_INVALID_ARG;
     if ((flags & NR_ANTI_ALIASING) && (S & 1)) return NR_ERR_INVALID_ARG;
     if (S > 32767 || B > 65535) return NR_ERR_UNSUPPORTED;
     if ((size_t)B * F * 2 * kWideStrips >= (size_t)0x7FFFFFFF) return NR_ERR_UNSUPPORTED;  // 32-bit list offsets
+    const size_t ncubes = (flags & NR_TEX_FILL_BACK) ? (size_t)F / 2 : (size_t)F;
+    const size_t tex_items = (flags & NR_TEX_SHARED) ? 1 : (size_t)B;
+    // NR_TEX_UV: the image gradient [Bt,Ht,Wt,3] (the zero-fill below and the edge scan's side fill are sized from it)
+    const size_t img_floats = uv ? (size_t)a->texture_height * (size_t)a->texture_width * 3 : 0;
+    const size_t uv_floats = ncubes * 6;
+    if (uv && (tex_items * img_floats > 0x7FFFFFFFull || uv_floats * ((flags & NR_UV_SHARED) ? 1 : (size_t)B) > 0x7FFFFFFFull))
+        return NR_ERR_UNSUPPORTED;  // 32-bit image / UV offsets in the kernels
     const size_t need = nr_b200_backward_workspace_bytes(B, F, S, ts, flags);
     if (!a->workspace || a->workspace_bytes < need || ((uintptr_t)a->workspace & 15)) return NR_ERR_WORKSPACE;
     cudaStream_t stream = (cudaStream_t)cuda_stream;
 
-    const size_t ncubes = (flags & NR_TEX_FILL_BACK) ? (size_t)F / 2 : (size_t)F;
-    const size_t tex_items = (flags & NR_TEX_SHARED) ? 1 : (size_t)B;
-    const size_t tex_floats = tex_items * ncubes * ts * ts * ts * 3;
+    const size_t tex_floats = uv ? tex_items * img_floats : tex_items * ncubes * ts * ts * ts * 3;
     // When one call runs both halves, grad_textures is zero-filled by the CTAs of the edge scan (a side job of an
     // issue-bound kernel instead of a memset of its own) and K6 runs after the edge scan.  Separate halves (the caller wants
     // the texture gradient first, for a collective) and unaligned buffers keep the memset.
@@ -1263,9 +1416,20 @@ extern "C" int nr_b200_backward(const nr_b200_backward_args* a, void* cuda_strea
     const double tmax = (double)(ts - 1) - a->eps;
     p.tex_cmp = float_le(tmax);
     p.tex_val = (float)tmax;
+    if (uv) {
+        p.uvs = a->face_uvs;
+        p.uv_bstride = (flags & NR_UV_SHARED) ? 0u : (uint32_t)uv_floats;
+        p.img_bstride = (flags & NR_TEX_SHARED) ? 0u : (uint32_t)img_floats;
+        p.Ht = a->texture_height; p.Wt = a->texture_width;
+    }
 
     const dim3 pgrid((unsigned)(((size_t)S * S + 255) / 256), B);
     auto launch_texture_grad = [&]() {
+        if (uv) {
+            nr_internal::LaunchScope ls("k_image_grad", stream);
+            k_image_grad<NR_TG_COMBINE><<<pgrid, 256, 0, stream>>>(p);
+            return;
+        }
         nr_internal::LaunchScope ls("k_texture_grad", stream);
         k_texture_grad<NR_TG_COMBINE><<<pgrid, 256, 0, stream>>>(p);
     };

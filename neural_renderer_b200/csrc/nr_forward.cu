@@ -90,6 +90,11 @@ struct FwdParams {
     uint32_t flags;
     float near_lo, far_cmp, far_val, tex_cmp, tex_val;
     float bg[3];
+    // NR_TEX_UV (appended, so the cube variants keep their parameter offsets): `textures` is the image [Bt,Ht,Wt,3]
+    const float* uvs;      // face_uvs [B,F,3,2] / [F,3,2] (F/2 faces with NR_TEX_FILL_BACK)
+    uint32_t uv_bstride;   // floats per item in face_uvs (0 with NR_UV_SHARED)
+    uint32_t img_bstride;  // floats per item in the image (0 with NR_TEX_SHARED)
+    int Ht, Wt;
 };
 
 // rasterize.py:291-292  xp = (2 * xi + 1 - is) / is evaluated in double and rounded to float.  Both operands are
@@ -420,7 +425,8 @@ __device__ __forceinline__ void sampler_depths(const FwdParams& p, int fn, const
     }
 }
 
-// cube of face fn (NR_TEX_FILL_BACK: the reversed copy of face f - F/2 samples that face's cube with reversed axes)
+// cube of face fn (NR_TEX_FILL_BACK: the reversed copy of face f - F/2 samples that face's cube with reversed axes; with
+// NR_TEX_UV the same index picks the face's UV corners, reversed)
 __device__ __forceinline__ int face_cube(const FwdParams& p, int fn, bool& rev) {
     rev = false;
     if (p.flags & NR_TEX_FILL_BACK) {
@@ -430,8 +436,9 @@ __device__ __forceinline__ int face_cube(const FwdParams& p, int fn, bool& rev) 
     return fn;
 }
 
-// one pixel, every texel straight from global memory (anti-aliased quads, texture sizes the bulk copy cannot stage)
-template <bool kLit>
+// one pixel, every texel straight from global memory (anti-aliased quads, texture sizes the bulk copy cannot stage);
+// kUV: bilinear sample of the texture image at the pixel's perspective-correct UV instead of the ts^3 cube
+template <bool kLit, bool kUV = false>
 __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigned long long key, int xi, int yi, float bgr,
                                               float bgg, float bgb) {
     Shaded o;
@@ -449,14 +456,32 @@ __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigne
     o.fim = fn; o.w0 = w[0]; o.w1 = w[1]; o.w2 = w[2]; o.depth = zp; o.alpha = 1.0f;
     o.r = o.g = o.b = 0.0f;
     if (p.flags & NR_RETURN_RGB) {
-        float z0, z1, z2;
-        sampler_depths(p, fn, cc, z0, z1, z2);
-        const int ts = p.ts;
-        const nr::TexCoord tc = nr::texture_coords(w, zp, z0, z1, z2, ts, p.tex_cmp, p.tex_val);
-        bool rev;
-        const int cube = face_cube(p, fn, rev);
-        const float* tex = p.textures + ((size_t)b * p.tex_bstride + cube) * (size_t)(ts * ts * ts) * 3;
-        blend_corners<kLit>(p, tc, tex, rev, b, fn, o.r, o.g, o.b);
+        if constexpr (kUV) {
+            // the winner's own vertex depths (no batch-0 quirk); fill_back copies read face fn - F/2's corners reversed
+            bool rev;
+            const int uf = face_cube(p, fn, rev);
+            float uv[6], u, v;
+            nr::load_face_uvs(p.uvs + ((uint32_t)b * p.uv_bstride + (uint32_t)uf * 6u), rev, uv);
+            nr::pixel_uv(w, zp, cc.y, cc.z, cc.w, uv, u, v);
+            const nr::UvTaps t = nr::uv_taps(u, v, p.Ht, p.Wt);
+            float l0 = 1.0f, l1 = 1.0f, l2 = 1.0f;
+            if (kLit) {
+                const float* lp = p.face_light + ((size_t)b * p.F + fn) * 3;
+                l0 = __ldg(lp); l1 = __ldg(lp + 1); l2 = __ldg(lp + 2);
+            }
+            float c[3];
+            nr::uv_blend<kLit>(p.textures + (uint32_t)b * p.img_bstride, p.Wt, t, l0, l1, l2, c);
+            o.r = c[0]; o.g = c[1]; o.b = c[2];
+        } else {
+            float z0, z1, z2;
+            sampler_depths(p, fn, cc, z0, z1, z2);
+            const int ts = p.ts;
+            const nr::TexCoord tc = nr::texture_coords(w, zp, z0, z1, z2, ts, p.tex_cmp, p.tex_val);
+            bool rev;
+            const int cube = face_cube(p, fn, rev);
+            const float* tex = p.textures + ((size_t)b * p.tex_bstride + cube) * (size_t)(ts * ts * ts) * 3;
+            blend_corners<kLit>(p, tc, tex, rev, b, fn, o.r, o.g, o.b);
+        }
     }
     return o;
 }
@@ -475,9 +500,12 @@ __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigne
 // 119 us for the direct gather (ts = 4; 92.5 vs 90.8 us at ts = 2) -- a whole 768-byte cube (ts = 4) is copied for the 8 texels a pixel blends, and the L1 data stage pays
 // for the shared-memory writes of the copy plus the bank conflicts of the 24 scattered reads.  The direct gather is
 // therefore the default.
+//
+// kTex == 2 (NR_TEX_UV): the direct variants with the texture-image sampler (shade_pixel<kLit, true>), same tile map.
 template <bool kAA, int kTex, bool kLit>
 __global__ void __launch_bounds__(256, kAA ? 5 : NR_RESOLVE_MIN_CTAS) k_resolve(const __grid_constant__ FwdParams p, int nslots) {
     constexpr bool kStage = kTex == 1;  // kTex: 0 = every texel straight from global memory, 1 = cubes staged with cp.async.bulk
+    constexpr bool kUV = kTex == 2;     //       2 = texture image through per-corner UVs
     extern __shared__ __align__(16) unsigned char stage_raw[];
     __shared__ uint64_t s_bar;
     __shared__ int s_runs[8];
@@ -572,7 +600,7 @@ __global__ void __launch_bounds__(256, kAA ? 5 : NR_RESOLVE_MIN_CTAS) k_resolve(
         // thread = one pixel of the IMAGE (row 0 = top): raster row yi = S - 1 - row
         const int row = row2, yi = S - 1 - row;
         if (col >= S || row >= S) return;
-        const Shaded s = shade_pixel<kLit>(p, b, __ldg(zb + (uint32_t)yi * S + col), col, yi, bgr, bgg, bgb);
+        const Shaded s = shade_pixel<kLit, kUV>(p, b, __ldg(zb + (uint32_t)yi * S + col), col, yi, bgr, bgg, bgb);
         const uint32_t o = (uint32_t)row * S + col;
         // streaming stores: 134 MB of maps that nothing reads again before the backward pass should not push the
         // z-buffer, the face records and the texture cubes out of the L2
@@ -594,7 +622,7 @@ __global__ void __launch_bounds__(256, kAA ? 5 : NR_RESOLVE_MIN_CTAS) k_resolve(
         for (int k = 0; k < 4; k++) {
             const int row = 2 * orow + (k >> 1), xi = 2 * col + (k & 1);
             const int yi = S - 1 - row;
-            const Shaded s = shade_pixel<kLit>(p, b, __ldg(zb + (uint32_t)yi * S + xi), xi, yi, bgr, bgg, bgb);
+            const Shaded s = shade_pixel<kLit, kUV>(p, b, __ldg(zb + (uint32_t)yi * S + xi), xi, yi, bgr, bgg, bgb);
             const uint32_t o = (uint32_t)row * S + xi;
             __stcs(fim + o, s.fim);
             __stcs(dmap + o, s.depth);
@@ -657,13 +685,21 @@ extern "C" int nr_b200_forward(const nr_b200_forward_args* a, void* cuda_stream)
     if (!a->face_index_map || !a->weight_map || !a->depth_map) return NR_ERR_INVALID_ARG;
     nr::FaceSrc src{};
     if (!nr_internal::make_face_src(flags, a->faces, a->vertices, a->face_indices, F, a->num_vertices, &src)) return NR_ERR_INVALID_ARG;
+    const bool uv = (flags & NR_TEX_UV) != 0;
     if (flags & NR_RETURN_RGB) {
-        if (!a->textures || !a->rgb_map || ts < 2) return NR_ERR_INVALID_ARG;
+        if (!a->textures || !a->rgb_map || (!uv && ts < 2)) return NR_ERR_INVALID_ARG;
         if ((flags & NR_TEX_FILL_BACK) && (F & 1)) return NR_ERR_INVALID_ARG;
         if ((flags & NR_BG_PER_BATCH) && !a->background_batch) return NR_ERR_INVALID_ARG;
     }
+    if (uv && (!(flags & NR_RETURN_RGB) || !a->face_uvs || a->texture_height < 1 || a->texture_width < 1)) return NR_ERR_INVALID_ARG;
     if ((flags & NR_ANTI_ALIASING) && (S & 1)) return NR_ERR_INVALID_ARG;
     if (S > 32767 || B > 65535) return NR_ERR_UNSUPPORTED;  // 32-bit pixel offsets; batch = grid.z of the resolve pass
+    // NR_TEX_UV: image and UV offsets are 32-bit in the kernels
+    const size_t img_floats = uv ? (size_t)a->texture_height * (size_t)a->texture_width * 3 : 0;
+    const size_t uv_floats = (size_t)((flags & NR_TEX_FILL_BACK) ? F / 2 : F) * 6;
+    if (uv && (img_floats * ((flags & NR_TEX_SHARED) ? 1 : B) > 0x7FFFFFFFull ||
+               uv_floats * ((flags & NR_UV_SHARED) ? 1 : B) > 0x7FFFFFFFull))
+        return NR_ERR_UNSUPPORTED;
     const size_t need = nr_b200_forward_workspace_bytes(B, F, S, ts, flags);
     if (!a->workspace || a->workspace_bytes < need || ((uintptr_t)a->workspace & 15)) return NR_ERR_WORKSPACE;
     cudaStream_t stream = (cudaStream_t)cuda_stream;
@@ -681,7 +717,13 @@ extern "C" int nr_b200_forward(const nr_b200_forward_args* a, void* cuda_stream)
     p.zbuf = (unsigned long long*)(wsb + L.off_zbuf);
     p.tab = (float4*)(wsb + L.off_tab);
     p.big_list = (int*)(wsb + L.off_list);
-    p.z0tab = ((flags & NR_RETURN_RGB) && (flags & NR_TEX_Z_BATCH0)) ? (float4*)(wsb + L.off_z0) : nullptr;
+    p.z0tab = ((flags & NR_RETURN_RGB) && (flags & NR_TEX_Z_BATCH0) && !uv) ? (float4*)(wsb + L.off_z0) : nullptr;
+    if (uv) {
+        p.uvs = a->face_uvs;
+        p.uv_bstride = (flags & NR_UV_SHARED) ? 0u : (uint32_t)uv_floats;
+        p.img_bstride = (flags & NR_TEX_SHARED) ? 0u : (uint32_t)img_floats;
+        p.Ht = a->texture_height; p.Wt = a->texture_width;
+    }
     p.fim = a->face_index_map; p.wmap = a->weight_map; p.dmap = a->depth_map; p.rgb = a->rgb_map; p.alpha = a->alpha_map;
     p.out_rgb = a->out_rgb; p.out_alpha = a->out_alpha; p.out_depth = a->out_depth;
     p.B = B; p.F = F; p.S = S; p.ts = ts; p.ngroups = (F + 31) / 32;
@@ -735,7 +777,7 @@ extern "C" int nr_b200_forward(const nr_b200_forward_args* a, void* cuda_stream)
         const bool aa = (flags & NR_ANTI_ALIASING) != 0;
         const bool lit = p.face_light != nullptr;
         const uint32_t cube_bytes = (flags & NR_RETURN_RGB) ? (uint32_t)(ts * ts * ts) * 12u : 0u;
-        const bool stage = (flags & NR_FWD_STAGE_TEXTURES) && !aa && (flags & NR_RETURN_RGB) && (cube_bytes % 16u) == 0 &&
+        const bool stage = !uv && (flags & NR_FWD_STAGE_TEXTURES) && !aa && (flags & NR_RETURN_RGB) && (cube_bytes % 16u) == 0 &&
                            cube_bytes <= kStageBytes / 8 && ((uintptr_t)a->textures & 15) == 0;
         int nslots = 0;
         size_t smem = 0;
@@ -754,7 +796,9 @@ extern "C" int nr_b200_forward(const nr_b200_forward_args* a, void* cuda_stream)
             bx = 256;
             grid = dim3((width + kResolveTileW - 1) / kResolveTileW, (width + kResolveTileH - 1) / kResolveTileH, B);
         }
-        if (aa) NR_RESOLVE_LIT(true, 0);
+        if (uv && aa) NR_RESOLVE_LIT(true, 2);
+        else if (uv) NR_RESOLVE_LIT(false, 2);
+        else if (aa) NR_RESOLVE_LIT(true, 0);
         else if (stage) NR_RESOLVE_LIT(false, 1);
         else NR_RESOLVE_LIT(false, 0);
 #undef NR_RESOLVE_LIT

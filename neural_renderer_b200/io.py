@@ -108,9 +108,64 @@ def load_textures(filename_obj, filename_mtl, texture_size):
     return textures
 
 
-def load_obj(filename_obj, normalization=True, texture_size=4, load_texture=False):
-    """Load vertices (v x y z), faces (f ...; n-gons are fan-triangulated) and optionally the baked per-face textures
-    of a Wavefront .obj file (load_obj.py:147-197)."""
+def load_texture_image(filename_obj, filename_mtl):
+    """The OBJ's materials as ONE texture image plus per-corner UVs, for the rasterizer's texture-image mode:
+    (face_uvs [F,3,2] float32, OBJ convention; image [H,W,3] float32, row 0 = top).
+
+    A model whose faces all use one map_Kd image gets that image, unpadded, and its UVs unchanged.  Otherwise every
+    map_Kd image used by a face becomes a tile of an atlas with a 1-texel replicated border, faces of materials without
+    an image get a 1x1 tile of their Kd colour (0.5 grey without a material, as the cube loader), and the UVs (clamped
+    into [0, 1] first) are remapped so that the sample position inside the tile is x0 + u (w - 1), y0 + v (h - 1): a
+    bilinear sample of the atlas equals the sample of the material's own image up to the float32 rounding of the UV."""
+    uv_faces, material_names = parse_texture_faces(filename_obj)
+    colors, texture_filenames = load_mtl(filename_mtl)
+    names = np.array(material_names)
+    used = list(dict.fromkeys(material_names))  # materials in order of first use
+    image_of = {m: texture_filenames[m] for m in used if m in texture_filenames}
+    images = {}
+    for fn in dict.fromkeys(image_of.values()):
+        images[fn] = _read_image(os.path.join(os.path.dirname(filename_obj), fn))
+    if len(images) == 1 and len(image_of) == len(used):
+        return uv_faces, next(iter(images.values()))
+    # tiles: one per image file, one per colour-only material; laid out left to right, top-aligned
+    tiles, tile_of = [], {}
+    for fn, img in images.items():
+        tile_of[fn] = len(tiles)
+        tiles.append(img)
+    for m in used:
+        if m not in image_of:
+            color = colors.get(m, np.full(3, 0.5, np.float32))
+            tile_of[('color', m)] = len(tiles)
+            tiles.append(np.asarray(color, np.float32).reshape(1, 1, 3))
+    width = sum(t.shape[1] + 2 for t in tiles)
+    height = max(t.shape[0] + 2 for t in tiles)
+    atlas = np.zeros((height, width, 3), np.float32)
+    placed, x = [], 0
+    for t in tiles:
+        h, w = t.shape[:2]
+        atlas[:h + 2, x:x + w + 2] = np.pad(t, ((1, 1), (1, 1), (0, 0)), mode='edge')
+        placed.append((x + 1, h, w))  # first interior column, interior size
+        x += w + 2
+    uv = np.nan_to_num(np.clip(uv_faces.astype(np.float64), 0.0, 1.0), nan=0.0)
+    out = np.empty_like(uv)
+    for m in used:
+        sel = names == m
+        x0, h, w = placed[tile_of[image_of[m]] if m in image_of else tile_of[('color', m)]]
+        y0 = height - 1 - h  # tap row (v axis, from the bottom) of the tile's bottom interior row
+        out[sel, :, 0] = (x0 + uv[sel, :, 0] * (w - 1)) / (width - 1)
+        out[sel, :, 1] = (y0 + uv[sel, :, 1] * (h - 1)) / (height - 1)
+    return np.ascontiguousarray(out, dtype=np.float32), atlas
+
+
+def load_obj(filename_obj, normalization=True, texture_size=4, load_texture=False, texture_mode='cubes'):
+    """Load vertices (v x y z), faces (f ...; n-gons are fan-triangulated) and optionally the textures of a Wavefront
+    .obj file (load_obj.py:147-197).
+
+    texture_mode='cubes' (the reference's behaviour): returns vertices, faces, textures [F,ts,ts,ts,3] baked from the
+    material images.  texture_mode='uv': returns vertices, faces, face_uvs [F,3,2], texture_image [H,W,3] (see
+    load_texture_image) for `Renderer.render(vertices, faces, texture_image, face_uvs=face_uvs)`."""
+    if texture_mode not in ('cubes', 'uv'):
+        raise ValueError("texture_mode must be 'cubes' or 'uv', got %r" % (texture_mode,))
     vertices, faces = [], []
     with open(filename_obj) as f:
         lines = f.readlines()
@@ -131,7 +186,10 @@ def load_obj(filename_obj, normalization=True, texture_size=4, load_texture=Fals
         for line in lines:
             if line.startswith('mtllib'):
                 filename_mtl = os.path.join(os.path.dirname(filename_obj), line.split()[1])
-                textures = load_textures(filename_obj, filename_mtl, texture_size)
+                if texture_mode == 'uv':
+                    textures = load_texture_image(filename_obj, filename_mtl)
+                else:
+                    textures = load_textures(filename_obj, filename_mtl, texture_size)
         if textures is None:
             raise Exception('Failed to load textures.')  # load_obj.py:185
     if normalization:  # unit cube centred at zero, load_obj.py:188-192
@@ -139,6 +197,8 @@ def load_obj(filename_obj, normalization=True, texture_size=4, load_texture=Fals
         vertices /= np.abs(vertices).max()
         vertices *= 2
         vertices -= vertices.max(0)[None, :] / 2
+    if load_texture and texture_mode == 'uv':
+        return (vertices, faces) + textures
     if load_texture:
         return vertices, faces, textures
     return vertices, faces

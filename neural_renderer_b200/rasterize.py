@@ -60,7 +60,7 @@ def _ptr(t):
     return None if t is None else ctypes.c_void_p(t.data_ptr())
 
 
-def _check_inputs(faces, textures, return_rgb, face_light=None, textures_fill_back=False, vertices=None):
+def _check_inputs(faces, textures, return_rgb, face_light=None, textures_fill_back=False, vertices=None, face_uvs=None):
     # rasterize.py:66-90 (chainer type_check) -> TypeError / ValueError with the same conditions
     if not isinstance(faces, torch.Tensor):
         raise TypeError("faces must be a torch.Tensor")
@@ -93,6 +93,9 @@ def _check_inputs(faces, textures, return_rgb, face_light=None, textures_fill_ba
         num_cubes = num_faces // 2 if textures_fill_back else num_faces
         if textures_fill_back and num_faces % 2:
             raise ValueError("textures_fill_back needs an even number of faces (front faces, then their reversed copies)")
+    if return_rgb and face_uvs is not None:
+        _check_uv_inputs(textures, face_uvs, batch_size, num_cubes)
+    elif return_rgb:
         # batch size 1 with a larger geometry batch = ONE set of cubes shared by every item (a mesh seen from B viewpoints)
         if (textures.dim() != 6 or textures.shape[2] < 2 or textures.shape[2] != textures.shape[3]
                 or textures.shape[3] != textures.shape[4] or textures.shape[5] != 3
@@ -104,8 +107,26 @@ def _check_inputs(faces, textures, return_rgb, face_light=None, textures_fill_ba
             raise ValueError("face_light must have shape [batch size, num faces, 3]")
         if not face_light.is_cuda:
             raise NotImplementedError("neural_renderer_b200 has no CPU implementation (inputs must be CUDA tensors)")
-    if not faces.is_cuda or (return_rgb and not textures.is_cuda):
+    if not faces.is_cuda or (return_rgb and not textures.is_cuda) or (return_rgb and face_uvs is not None and not face_uvs.is_cuda):
         raise NotImplementedError("neural_renderer_b200 has no CPU implementation (inputs must be CUDA tensors)")
+
+
+def _check_uv_inputs(image, face_uvs, batch_size, num_uv_faces):
+    # texture image [Ht,Wt,3] / [1|B,Ht,Wt,3] and per-corner UVs [F,3,2] / [1|B,F,3,2] (F/2 faces with textures_fill_back)
+    if not isinstance(face_uvs, torch.Tensor) or not face_uvs.is_floating_point():
+        raise TypeError("face_uvs must be a floating point torch.Tensor")
+    if not ((face_uvs.dim() == 3 or (face_uvs.dim() == 4 and face_uvs.shape[0] in (1, batch_size)))
+            and tuple(face_uvs.shape[-3:]) == (num_uv_faces, 3, 2)):
+        raise ValueError("face_uvs must have shape [num faces, 3, 2] or [batch size, num faces, 3, 2] with num faces = %d "
+                         "(half the faces with textures_fill_back), got %s" % (num_uv_faces, tuple(face_uvs.shape)))
+    if not isinstance(image, torch.Tensor):
+        raise TypeError("with face_uvs, textures must be the texture image (a torch.Tensor)")
+    if not image.is_floating_point():
+        raise TypeError("the texture image must be floating point")
+    if not ((image.dim() == 3 or (image.dim() == 4 and image.shape[0] in (1, batch_size)))
+            and image.shape[-1] == 3 and image.shape[-2] >= 1 and image.shape[-3] >= 1):
+        raise ValueError("with face_uvs, textures must be an image of shape [height, width, 3] or [batch size, height, "
+                         "width, 3], got %s" % (tuple(image.shape),))
 
 
 # Optional hook between the two halves of the backward pass (neural_renderer_b200.distributed.overlap_texture_allreduce):
@@ -177,7 +198,7 @@ class _RasterizeFunction(torch.autograd.Function):
     the `Rasterize` object can look at them)."""
 
     @staticmethod
-    def forward(ctx, geom, textures, face_light, cfg, indices):
+    def forward(ctx, geom, textures, face_light, cfg, indices, face_uvs=None):
         lib = _lib.load()
         dev = geom.device
         geom_c = geom.detach().contiguous()
@@ -197,6 +218,14 @@ class _RasterizeFunction(torch.autograd.Function):
             flags |= _lib.NR_TEX_SHARED
         S = cfg.S
         ts = int(tex_c.shape[2]) if tex_c is not None else 0
+        uv_c = None
+        if face_uvs is not None:  # texture image [Bt,Ht,Wt,3] sampled through face_uvs (NR_TEX_UV)
+            uv_c = face_uvs.detach().contiguous()
+            flags |= _lib.NR_TEX_UV
+            if uv_c.shape[0] == 1 and B > 1:
+                flags |= _lib.NR_UV_SHARED
+            ts = 0
+        tex_hw = (int(tex_c.shape[1]), int(tex_c.shape[2])) if uv_c is not None else (0, 0)
         want_rgb = bool(flags & _lib.NR_RETURN_RGB)
         want_alpha = bool(flags & _lib.NR_RETURN_ALPHA)
         want_depth = bool(flags & _lib.NR_RETURN_DEPTH)
@@ -233,15 +262,17 @@ class _RasterizeFunction(torch.autograd.Function):
             a.out_rgb, a.out_alpha, a.out_depth = _ptr(out_rgb), _ptr(out_alpha), _ptr(out_depth)
             a.workspace, a.workspace_bytes = _ptr(ws), ws_bytes
             a.face_light = _ptr(light_c)
+            a.face_uvs, (a.texture_height, a.texture_width) = _ptr(uv_c), tex_hw
             _lib.check(lib.nr_b200_forward(ctypes.byref(a), _stream_ptr(dev)))
         ctx.cfg = cfg
         ctx.flags = flags
         ctx.ts = ts
         ctx.F = F
         ctx.tex_shape = tuple(textures.shape) if textures is not None else None
+        ctx.tex_hw = tex_hw
         # the unlit textures are only needed again for d loss / d face_light
         need_light_grad = light_c is not None and ctx.needs_input_grad[2]
-        ctx.save_for_backward(geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c if need_light_grad else None, indices)
+        ctx.save_for_backward(geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c if need_light_grad else None, indices, uv_c)
         if cfg.aa:
             rgb_o, alpha_o, depth_o = out_rgb, out_alpha, out_depth
         else:
@@ -254,7 +285,7 @@ class _RasterizeFunction(torch.autograd.Function):
         lib = _lib.load()
         cfg = ctx.cfg
         flags = ctx.flags
-        geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c, indices = ctx.saved_tensors
+        geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c, indices, uv_c = ctx.saved_tensors
         dev = geom_c.device
         B, F = geom_c.shape[0], ctx.F
         want_rgb = bool(flags & _lib.NR_RETURN_RGB)
@@ -283,6 +314,7 @@ class _RasterizeFunction(torch.autograd.Function):
             else:
                 a.faces, a.grad_faces = _ptr(geom_c), _ptr(grad_geom)
             a.textures = _ptr(tex_c)
+            a.face_uvs, (a.texture_height, a.texture_width) = _ptr(uv_c), ctx.tex_hw
             a.face_light, a.grad_face_light = _ptr(light_c), _ptr(grad_light)
             a.face_index_map, a.weight_map, a.depth_map, a.rgb_map = _ptr(fim), _ptr(wmap), _ptr(dmap), _ptr(rgb_map)
             a.grad_rgb, a.grad_alpha, a.grad_depth = _ptr(g_rgb), _ptr(g_alpha), _ptr(g_depth)
@@ -302,12 +334,13 @@ class _RasterizeFunction(torch.autograd.Function):
                 _lib.check(lib.nr_b200_backward(ctypes.byref(a), _stream_ptr(dev)))
                 if pending is not None:
                     pending.wait()
-        return grad_geom, grad_textures, grad_light, None, None
+        # no gradient for face_uvs (the sampler's UV derivative is not implemented)
+        return grad_geom, grad_textures, grad_light, None, None, None
 
 
 def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_color, return_rgb, return_alpha,
-         return_depth, face_light=None, textures_fill_back=False, vertices=None, reference_exact=None):
-    _check_inputs(faces, textures, return_rgb, face_light, textures_fill_back, vertices)
+         return_depth, face_light=None, textures_fill_back=False, vertices=None, reference_exact=None, face_uvs=None):
+    _check_inputs(faces, textures, return_rgb, face_light, textures_fill_back, vertices, face_uvs)
     indices = None
     if vertices is not None:
         geom = vertices if vertices.dtype == torch.float32 else vertices.float()
@@ -318,9 +351,19 @@ def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_
     else:
         geom = faces if faces.dtype == torch.float32 else faces.float()
     batch_size = geom.shape[0]
+    if not return_rgb:
+        face_uvs = None
     if return_rgb:
         if textures.dtype != torch.float32:
             textures = textures.float()
+        if face_uvs is not None:
+            if textures.dim() == 3:
+                textures = textures[None]  # one image for every item
+            face_uvs = face_uvs.float() if face_uvs.dtype != torch.float32 else face_uvs
+            if face_uvs.dim() == 3:
+                face_uvs = face_uvs[None]
+            if face_uvs.shape[0] == batch_size > 1 and face_uvs.stride(0) == 0:
+                face_uvs = face_uvs[:1]  # an expanded shared UV set (NR_UV_SHARED)
         if textures.shape[0] == batch_size > 1 and textures.stride(0) == 0:
             textures = textures[:1]  # an expanded shared texture set: sample it in place (NR_TEX_SHARED)
     cfg = _make_config(image_size, anti_aliasing, near, far, eps, background_color, return_rgb, return_alpha,
@@ -330,7 +373,7 @@ def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_
     if return_rgb and _STAGE_TEXTURES:
         cfg.flags |= _lib.NR_FWD_STAGE_TEXTURES
     return _RasterizeFunction.apply(geom, textures if return_rgb else None, face_light if return_rgb else None, cfg,
-                                    indices)
+                                    indices, face_uvs)
 
 
 def rasterize_rgbad(
@@ -350,6 +393,7 @@ def rasterize_rgbad(
         textures_fill_back=False,
         vertices=None,
         reference_exact=None,
+        face_uvs=None,
 ):
     """Generate RGB, alpha channel, and depth images from faces and textures (for RGB).  rasterize.py:900-977.
 
@@ -369,11 +413,16 @@ def rasterize_rgbad(
                               (rasterize.py:389).  True reproduces that bit for bit; False samples every item with its own
                               depths -- what one wants for batches of different meshes or cameras (the images of items
                               b > 0 and grad_textures differ, item 0 and all silhouettes / depths do not)
+      face_uvs [F,3,2] / [B,F,3,2]  texture-image mode: `textures` is then an image [Ht,Wt,3] or [1|B,Ht,Wt,3] (row 0 =
+                              top, as read from a PNG) and face_uvs the UV of every face corner (OBJ convention, v = 0 at
+                              the bottom; F/2 faces with textures_fill_back).  Sampled bilinearly (clamp to edge) at the
+                              perspective-correct UV, with every item's own vertex depths (`reference_exact` has no
+                              effect).  The image receives a gradient, face_uvs does not.
     `textures` with batch size 1 (or an expanded stride-0 batch) while the geometry batch is larger = one texture set
     shared by every item (a mesh seen from B viewpoints, mesh.py:29-34); its gradient is the sum over the items."""
     rgb, alpha, depth, _, _ = _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_color,
                                    return_rgb, return_alpha, return_depth, face_light, textures_fill_back, vertices,
-                                   reference_exact)
+                                   reference_exact, face_uvs)
     return {
         'rgb': rgb if return_rgb else None,
         'alpha': alpha if return_alpha else None,
@@ -395,12 +444,13 @@ def rasterize(
         textures_fill_back=False,
         vertices=None,
         reference_exact=None,
+        face_uvs=None,
 ):
     """RGB images [B,3,H,W] from faces and textures.  rasterize.py:980-1008 (keyword-only extras: rasterize_rgbad)."""
     return rasterize_rgbad(
         faces, textures, image_size, anti_aliasing, near, far, eps, background_color, True, False, False,
         face_light=face_light, textures_fill_back=textures_fill_back, vertices=vertices,
-        reference_exact=reference_exact)['rgb']
+        reference_exact=reference_exact, face_uvs=face_uvs)['rgb']
 
 
 def rasterize_silhouettes(

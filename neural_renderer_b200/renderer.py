@@ -83,7 +83,10 @@ class Renderer(object):
         faces = F.vertices_to_faces(vertices, faces)
         return rasterize_depth(faces, self.image_size, self.anti_aliasing)  # renderer.py:72
 
-    def render(self, vertices, faces, textures):
+    def render(self, vertices, faces, textures, face_uvs=None):
+        """RGB images [B,3,H,W].  `textures` are per-face cubes [B,F,ts,ts,ts,3], or -- with `face_uvs` [F,3,2] /
+        [B,F,3,2] (UV of every face corner, OBJ convention) -- a texture image [Ht,Wt,3] / [1|B,Ht,Wt,3] (row 0 = top),
+        sampled bilinearly at the perspective-correct UV (neural_renderer_b200.rasterize_rgbad)."""
         fused = (self.fused and self._fusable(vertices, faces) and textures.is_cuda and textures.dtype == torch.float32)
         light_args = (self.light_intensity_ambient, self.light_intensity_directional, self.light_color_ambient,
                       self.light_color_directional, self.light_direction)
@@ -96,7 +99,17 @@ class Renderer(object):
             return rasterize(
                 indices, textures, self.image_size, self.anti_aliasing, self.near, self.far, self.rasterizer_eps,
                 self.background_color, face_light=light, textures_fill_back=self.fill_back,
-                vertices=self._transform(vertices), reference_exact=self.reference_exact)
+                vertices=self._transform(vertices), reference_exact=self.reference_exact, face_uvs=face_uvs)
+        if face_uvs is not None:
+            # op by op: materialised faces, the light factor of those faces (F.face_light), doubled UV corners for fill_back
+            if self.fill_back:
+                faces = torch.cat((faces, faces.flip(2)), dim=1)
+                face_uvs = torch.cat((face_uvs, face_uvs.flip(-2)), dim=-3)
+            light = F.face_light(F.vertices_to_faces(vertices, faces), *light_args)
+            faces = F.vertices_to_faces(self._transform(vertices), faces)
+            return rasterize(
+                faces, textures, self.image_size, self.anti_aliasing, self.near, self.far, self.rasterizer_eps,
+                self.background_color, face_light=light, reference_exact=self.reference_exact, face_uvs=face_uvs)
         if self.fill_back:
             faces = torch.cat((faces, faces.flip(2)), dim=1)
             textures = torch.cat((textures, textures.permute(0, 1, 4, 3, 2, 5)), dim=1)

@@ -56,6 +56,28 @@ def sphere_faces(batch_size, num_faces=5000, radius=0.8, jitter=0.01, z_center=2
     return out
 
 
+def sphere_uvs(num_faces=5000):
+    """[num_faces,3,2] float32 spherical UVs of sphere_mesh's face corners (same faces as sphere_faces): u = longitude /
+    2 pi, v = 1 - colatitude / pi (OBJ convention, v = 1 at the top pole); the corners past the seam get u = 1."""
+    n = max(2, int(math.ceil(math.sqrt(num_faces / 2.0))))
+    delta = 0.01
+    i, j = np.meshgrid(np.arange(n), np.arange(n), indexing="ij")
+
+    def corner(ii, jj):
+        theta = (ii * (1 - 2 * delta) / n + delta)  # colatitude / pi, as in sphere_mesh
+        return np.stack([jj / n, 1.0 - theta], axis=-1)
+
+    a, b, c, d = corner(i, j), corner(i + 1, j), corner(i + 1, j + 1), corner(i, j + 1)
+    uv = np.stack([np.stack([a, b, c], axis=-2), np.stack([a, c, d], axis=-2)], axis=2).reshape(-1, 3, 2)
+    return np.ascontiguousarray(uv[:num_faces], dtype=np.float32)
+
+
+def random_image(batch_size, height, width, seed=4322):
+    """[batch_size,height,width,3] float32 texture images, uniform in [0, 1)."""
+    rng = np.random.default_rng(seed)
+    return rng.random((batch_size, height, width, 3), dtype=np.float32)
+
+
 def random_textures(batch_size, num_faces, texture_size=4, seed=4321):
     rng = np.random.default_rng(seed)
     return rng.random((batch_size, num_faces, texture_size, texture_size, texture_size, 3), dtype=np.float32)

@@ -1,0 +1,123 @@
+#!/usr/bin/env python
+"""Texture image vs texture cubes at the headline geometry: one JSON object.
+
+Geometry: B 64 seeded spheres (synthetic.sphere_faces), F 5000, 256 x 256, no anti-aliasing, `rasterize()` forward +
+backward with a dense N(0,1) upstream gradient (bench.py's headline step).  Textures:
+  uv_shared_1024   one 1024 x 1024 image shared by every item (NR_TEX_SHARED), spherical UVs shared (NR_UV_SHARED)
+  uv_item_256      one 256 x 256 image per item, spherical UVs shared
+  cubes_ts4        the per-item ts = 4 cubes of bench.py
+Whole step: CUDA events around `steps` steps after `warmup` warm-up steps, median over `reps` repetitions.  Per kernel:
+the library's own CUDA-event profiler over `steps` further steps (ms per step).  Bytes held = texture + its gradient.
+The roofline fraction of the image-gradient kernel and of the zero-fill uses bench.py's HBM figure.
+
+    python tools/bench_uv.py [--steps 20] [--warmup 3] [--reps 5]
+"""
+import argparse
+import collections
+import json
+import os
+import sys
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+import neural_renderer as nr  # noqa: E402
+from neural_renderer_b200 import _lib, synthetic  # noqa: E402
+
+
+def hbm_gbs():
+    path = os.path.join(ROOT, "MEASURED_PEAKS.json")  # as bench.py: measured figure if present, else the data sheet
+    if os.path.exists(path):
+        with open(path) as f:
+            return float(json.load(f)["hbm_gbs"])
+    return 3350.0
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--batch", type=int, default=64)
+    ap.add_argument("--faces", type=int, default=5000)
+    ap.add_argument("--size", type=int, default=256)
+    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--reps", type=int, default=5)
+    a = ap.parse_args()
+    dev = torch.device("cuda")
+    B, F, S = a.batch, a.faces, a.size
+    faces = torch.from_numpy(synthetic.sphere_faces(B, F)).to(dev).requires_grad_(True)
+    uvs = torch.from_numpy(synthetic.sphere_uvs(F)).to(dev)
+    g = torch.randn((B, 3, S, S), generator=torch.Generator().manual_seed(0)).to(dev)
+    variants = collections.OrderedDict([
+        ("uv_shared_1024", (torch.from_numpy(synthetic.random_image(1, 1024, 1024)[0]).to(dev), uvs)),
+        ("uv_item_256", (torch.from_numpy(synthetic.random_image(B, 256, 256)).to(dev), uvs)),
+        ("cubes_ts4", (torch.from_numpy(synthetic.random_textures(B, F, 4)).to(dev), None)),
+    ])
+    lib = _lib.load()
+    out = {"gpu": torch.cuda.get_device_name(dev), "shape": {"batch": B, "faces": F, "size": S, "anti_aliasing": False},
+           "hbm_gbs": hbm_gbs(), "variants": {}}
+    for name, (tex0, fuv) in variants.items():
+        tex = tex0.clone().requires_grad_(True)
+
+        def step():
+            faces.grad = None
+            tex.grad = None
+            img = nr.rasterize(faces, tex, S, False, face_uvs=fuv)
+            img.backward(g)
+
+        for _ in range(a.warmup):
+            step()
+        torch.cuda.synchronize()
+        reps = []
+        for _ in range(a.reps):
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for _ in range(a.steps):
+                step()
+            e1.record()
+            torch.cuda.synchronize()
+            reps.append(e0.elapsed_time(e1) / a.steps)
+        lib.nr_b200_set_profiling(1)
+        _lib.read_profile()
+        for _ in range(a.steps):
+            step()
+        torch.cuda.synchronize()
+        prof = _lib.read_profile()
+        lib.nr_b200_set_profiling(0)
+        kern = collections.OrderedDict()
+        for k, ms in prof:
+            kern[k] = kern.get(k, 0.0) + ms / a.steps
+        tex_bytes = tex.numel() * 4
+        rec = {"step_ms_median": float(np.median(reps)), "step_ms_reps": reps,
+               "kernels_ms_per_step": kern, "texture_bytes": tex_bytes, "texture_plus_grad_bytes": 2 * tex_bytes}
+        grad_kernel = "k_image_grad" if fuv is not None else "k_texture_grad"
+        if grad_kernel in kern:
+            rec["grad_kernel"] = grad_kernel
+        # The zero-fill of the texture gradient rides in k_edge_scan's CTAs when one call runs both halves of the
+        # backward.  Timed on its own here: with a (no-op) texture hook the backward runs as two calls and the texture
+        # half zero-fills with a memset of its own, the first "memset_grads" of every step.
+        R = sys.modules["neural_renderer_b200.rasterize"]
+        prev = R.set_texture_grad_hook(lambda grad: None)
+        try:
+            lib.nr_b200_set_profiling(1)
+            _lib.read_profile()
+            for _ in range(a.steps):
+                step()
+            torch.cuda.synchronize()
+            prof2 = _lib.read_profile()
+            lib.nr_b200_set_profiling(0)
+        finally:
+            R.set_texture_grad_hook(prev)
+        fills = [ms for k, ms in prof2 if k == "memset_grads"][0::2]
+        rec["zero_fill_bytes"] = tex_bytes
+        rec["zero_fill_ms_separate_memset"] = float(np.median(fills)) if fills else None
+        rec["zero_fill_ms_at_hbm_peak"] = tex_bytes / (out["hbm_gbs"] * 1e6)
+        rec["split_backward_kernels_ms_per_step"] = {k: sum(ms for kk, ms in prof2 if kk == k) / a.steps
+                                                     for k in dict.fromkeys(k for k, _ in prof2)}
+        out["variants"][name] = rec
+    print(json.dumps(out))
+
+
+if __name__ == "__main__":
+    main()
