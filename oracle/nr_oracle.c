@@ -238,9 +238,18 @@ static inline float k5_dist(float ratio, int d1, float d1_cross, int is, double 
     return dist;
 }
 
+#define K5_ADD(j, term)                               \
+    do {                                              \
+        const float t_ = (term);                      \
+        if (sum_fp64) grad_face64[j] -= (double)t_;   \
+        else grad_face[j] -= t_;                      \
+    } while (0)
 NRO_API void nro_pixel_bwd(const float *faces, const int *face_index_map, const float *rgb_map, const float *alpha_map,
                            const float *grad_rgb_map, const float *grad_alpha_map, int bs, int nf, int is, double eps,
-                           int return_rgb, int return_alpha, float *grad_faces) {
+                           int return_rgb, int return_alpha, int sum_fp64, float *grad_faces) {
+    /* sum_fp64: each term is the reference's fp32 diff_grad / dist, but the nine sums are kept in double.  The
+     * reference adds up to ~S terms per crossing pixel in fp32, one after the other; at rasters of 2048 its own
+     * rounding reaches 4e-4 of the tensor maximum, so a product that sums in another order is compared with this. */
     if (!return_rgb && !return_alpha) return;
     const int64_t n = (int64_t)bs * nf;
 #pragma omp parallel for schedule(dynamic, 16)
@@ -248,6 +257,7 @@ NRO_API void nro_pixel_bwd(const float *faces, const int *face_index_map, const 
         const int bn = (int)(i / nf), fn = (int)(i % nf);
         const float *face = faces + 9 * i;
         float grad_face[9] = {0};
+        double grad_face64[9] = {0};
         if (backside(face)) continue; /* `return`: grad_faces[i] keeps its zero initialisation */
         const int64_t base = (int64_t)bn * is * is;
         for (int edge_num = 0; edge_num < 3; edge_num++) {
@@ -312,11 +322,11 @@ NRO_API void nro_pixel_bwd(const float *faces, const int *face_index_map, const 
                             if (diff_grad <= 0) continue;
                             if (p[1][0] != fd0) {
                                 float dist = k5_dist(ratio0, d1, d1_cross, is, eps);
-                                grad_face[pi[0] * 3 + (1 - axis)] -= diff_grad / dist;
+                                K5_ADD(pi[0] * 3 + (1 - axis), diff_grad / dist);
                             }
                             if (p[0][0] != fd0) {
                                 float dist = k5_dist(ratio1, d1, d1_cross, is, eps);
-                                grad_face[pi[1] * 3 + (1 - axis)] -= diff_grad / dist;
+                                K5_ADD(pi[1] * 3 + (1 - axis), diff_grad / dist);
                             }
                         }
                     }
@@ -345,18 +355,18 @@ NRO_API void nro_pixel_bwd(const float *faces, const int *face_index_map, const 
                             if (diff_grad <= 0) continue;
                             if (p[1][0] != fd0) {
                                 float dist = k5_dist(ratio0, d1, d1_cross, is, eps);
-                                grad_face[pi[0] * 3 + (1 - axis)] -= diff_grad / dist;
+                                K5_ADD(pi[0] * 3 + (1 - axis), diff_grad / dist);
                             }
                             if (p[0][0] != fd0) {
                                 float dist = k5_dist(ratio1, d1, d1_cross, is, eps);
-                                grad_face[pi[1] * 3 + (1 - axis)] -= diff_grad / dist;
+                                K5_ADD(pi[1] * 3 + (1 - axis), diff_grad / dist);
                             }
                         }
                     }
                 }
             }
         }
-        for (int k = 0; k < 9; k++) grad_faces[i * 9 + k] = grad_face[k];
+        for (int k = 0; k < 9; k++) grad_faces[i * 9 + k] = sum_fp64 ? (float)grad_face64[k] : grad_face[k];
     }
 }
 

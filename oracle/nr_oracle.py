@@ -97,6 +97,7 @@ class OracleRasterize:
         self.background_color = background_color
         self.return_rgb, self.return_alpha, self.return_depth = bool(return_rgb), bool(return_alpha), bool(return_depth)
         self.tex_z_batch0 = bool(tex_z_batch0)
+        self.k5_sum_fp64 = False  # True: K5 keeps its sums in double (nr_oracle.c nro_pixel_bwd)
 
     # ---- forward (rasterize.py:467-513)
     def forward(self, faces, textures=None):
@@ -159,7 +160,7 @@ class OracleRasterize:
             g_depth = _f32(grad_depth) if grad_depth is not None else np.zeros_like(self.depth_map)
         L.nro_pixel_bwd(_fp(self.faces), _ip(self.face_index_map), _fp(self.rgb_map), _fp(self.alpha_map), _fp(g_rgb),
                         _fp(g_alpha), bs, nf, S, ctypes.c_double(self.eps), int(self.return_rgb),
-                        int(self.return_alpha), _fp(grad_faces))
+                        int(self.return_alpha), int(self.k5_sum_fp64), _fp(grad_faces))
         if self.return_rgb:
             L.nro_texture_bwd(_ip(self.face_index_map), _fp(self.sampling_weight_map), _ip(self.sampling_index_map),
                               _fp(g_rgb), bs, nf, S, self.texture_size, _fp(grad_textures))

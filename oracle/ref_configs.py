@@ -8,6 +8,7 @@ anti-aliasing); near/far/eps keep their Python type because the reference pastes
 from build_ref import normalize_config as cfg
 
 NEAR, FAR = 0.1, 100  # module defaults rasterize.py:9-10 (far is an int literal in the reference)
+SIZES, SIZES_F, SIZES_TS = (255, 257, 700, 1024, 2048, 2051), 300, 2
 
 
 def all_configs():
@@ -39,4 +40,10 @@ def all_configs():
     c.append(cfg(512, 70000, 2, NEAR, FAR, 1e-4, 1, 0, 1))
     # config 5 of BASELINE.json at reduced size: one shared 100k-face mesh, 512x512, RGB through Renderer.render (eps 1e-3)
     c.append(cfg(512, 100000, 2, NEAR, FAR, 1e-3, 1, 0, 0))
+    # raster sizes that select other code paths of the product (tests/test_gpu_sizes.py, tests/test_gpu_uv.py): odd
+    # sizes with a one-line last strip (255, 257), one-line strips (700, 1024), global-atomics binning (2048, 2051),
+    # no pixel-centre table and a strip above 48 KB of shared memory (2051).  One (1, 1, 1) binary serves every
+    # backward mode: the missing upstream gradients are zeros.
+    for S in SIZES:
+        c.append(cfg(S, SIZES_F, SIZES_TS, NEAR, FAR, 1e-4, 1, 1, 1))
     return c

@@ -188,6 +188,12 @@ MORE = [
     ("behind_camera", 64, False, 120, 2, (1, 1, 1), 0.1, 100, 1e-4, "soup", 2, (-1.0, 3.0)),
     ("depth_aa", 32, True, 60, 2, (0, 0, 1), 0.5, 2.5, 1e-4, "soup", 2, (1.0, 3.0)),
     ("alpha_aa_big", 96, True, 12, 2, (0, 1, 0), 0.1, 100, 1e-4, "big", 2, (1.0, 3.0)),
+    # a one-pixel raster (item 0 empty, item 1 covered) and rasters with fewer lines than one edge-scan strip
+    ("raster1", 1, False, 24, 2, (1, 1, 1), 0.1, 100, 1e-4, "big", 2, (1.0, 3.0)),
+    ("raster3", 3, False, 40, 2, (1, 1, 1), 0.1, 100, 1e-4, "big", 2, (1.0, 3.0)),
+    ("raster5", 5, False, 24, 3, (1, 1, 1), 0.1, 100, 1e-4, "big", 2, (1.0, 3.0)),
+    ("odd63_all", 63, False, 120, 2, (1, 1, 1), 0.1, 100, 1e-4, "soup", 2, (1.0, 3.0)),
+    ("odd_aa51", 51, True, 100, 2, (1, 1, 1), 0.1, 100, 1e-4, "soup", 2, (1.0, 3.0)),  # raster 102
 ]
 
 

@@ -79,24 +79,29 @@ def _render(faces, image, uvs, S, aa, light=None, fill_back=False, reference_exa
 
 
 CASES = [
-    # aa, lit, fill_back, shared image, shared uvs, (Ht, Wt), uv range
-    (False, False, False, True, True, (32, 32), (0, 1)),
-    (True, False, False, True, True, (32, 32), (0, 1)),
-    (False, True, False, False, True, (17, 40), (0, 1)),
-    (True, True, True, True, False, (40, 17), (0, 1)),
-    (False, False, True, False, False, (16, 16), (0, 1)),
-    (False, True, True, True, True, (1, 9), (0, 1)),
-    (True, False, False, False, True, (12, 1), (0, 1)),
-    (False, False, False, True, False, (1, 1), (0, 1)),
-    (False, True, False, True, True, (24, 20), (-0.6, 1.7)),
-    (True, True, True, False, False, (9, 30), (-0.6, 1.7)),
+    # aa, lit, fill_back, shared image, shared uvs, (Ht, Wt), uv range, API image size H, F
+    (False, False, False, True, True, (32, 32), (0, 1), 48, 200),
+    (True, False, False, True, True, (32, 32), (0, 1), 48, 200),
+    (False, True, False, False, True, (17, 40), (0, 1), 48, 200),
+    (True, True, True, True, False, (40, 17), (0, 1), 48, 200),
+    (False, False, True, False, False, (16, 16), (0, 1), 48, 200),
+    (False, True, True, True, True, (1, 9), (0, 1), 48, 200),
+    (True, False, False, False, True, (12, 1), (0, 1), 48, 200),
+    (False, False, False, True, False, (1, 1), (0, 1), 48, 200),
+    (False, True, False, True, True, (24, 20), (-0.6, 1.7), 48, 200),
+    (True, True, True, False, False, (9, 30), (-0.6, 1.7), 48, 200),
+    # raster 257: odd, the edge scan keeps only the face index in its strip; 700 (image 350, odd) and 102 (image 51):
+    # anti-aliasing with an odd pooled size, one-line strips at 700
+    (False, True, False, True, True, (24, 20), (0, 1), 257, 300),
+    (True, False, True, False, True, (33, 47), (-0.6, 1.7), 350, 300),
+    (True, True, False, True, False, (16, 9), (0, 1), 51, 200),
 ]
 
 
 @pytest.mark.parametrize("case", CASES)
 def test_forward_and_gradients_vs_oracle(case):
-    aa, lit, fill_back, shared_img, shared_uv, (Ht, Wt), (lo, hi) = case
-    B, F, H = 2, 200, 48
+    aa, lit, fill_back, shared_img, shared_uv, (Ht, Wt), (lo, hi), H, F = case
+    B = 2
     S = 2 * H if aa else H
     faces = _case(B, F, seed=3)
     if fill_back:
@@ -205,10 +210,9 @@ def test_two_part_backward_with_texture_hook():
     assert rel_err(np_(gf1), np_(gf0)) <= 1e-5
 
 
-def test_vertex_gradient_vs_reference_k5():
+def _vertex_gradient_vs_reference_k5(S, F, ts, flags):
     import refhost
-    S, F = 64, 200
-    if not refhost.available(S, F, 4, 0.1, 100, 1e-4, 1, 0, 0):
+    if not refhost.available(S, F, ts, 0.1, 100, 1e-4, *flags):
         pytest.skip("reference kernels not built (oracle/_ref)")
     B = 2
     faces = _case(B, F, seed=12)
@@ -216,13 +220,25 @@ def test_vertex_gradient_vs_reference_k5():
     bg = (0.2, 0.4, 0.6)
     g = torch.randn((B, 3, S, S), generator=torch.Generator().manual_seed(3)).to(DEV)
     f = faces.clone().requires_grad_(True)
-    rgb = _R()._run(f, img, S, False, 0.1, 100, 1e-4, bg, True, False, False, face_uvs=uvs)[0]
+    rgb = _R()._run(f, img, S, False, 0.1, 100, 1e-4, bg, *flags, face_uvs=uvs)[0]
     (rgb * g).sum().backward()
-    placeholder = torch.zeros((B, F, 4, 4, 4, 3), device=DEV)  # K5 reads only the rgb map
-    ref = refhost.rasterize_rgbad(faces, placeholder, S, False, 0.1, 100, 1e-4, bg, True, False, False)
+    placeholder = torch.zeros((B, F, ts, ts, ts, 3), device=DEV)  # K5 reads only the rgb map
+    ref = refhost.rasterize_rgbad(faces, placeholder, S, False, 0.1, 100, 1e-4, bg, *flags)
     ref.fn.rgb_map = rgb.detach().permute(0, 2, 3, 1).flip(1).contiguous()  # API image -> the reference's NHWC, unflipped
     gf_ref, _ = ref.backward(g, None, None)
     assert rel_err(np_(f.grad), np_(gf_ref)) <= 1e-4
+
+
+def test_vertex_gradient_vs_reference_k5():
+    _vertex_gradient_vs_reference_k5(64, 200, 4, (1, 0, 0))
+
+
+@pytest.mark.parametrize("S", [257, 1024])
+def test_vertex_gradient_vs_reference_k5_at_other_raster_sizes(S):
+    """257 (odd, face index only in the strip) and 1024 (one-line strips): the (1, 1, 1) binaries of
+    oracle/ref_configs.py SIZES, with the product run with the same return flags (same strip width)"""
+    from ref_configs import SIZES_F, SIZES_TS
+    _vertex_gradient_vs_reference_k5(S, SIZES_F, SIZES_TS, (1, 1, 1))
 
 
 @pytest.mark.parametrize("fill_back", [True, False])
