@@ -2,7 +2,11 @@
 renders from random viewpoints match renders of the model's own texture.  The model is tests/golden/display, loaded
 with load_obj(texture_mode='uv'): its 7 materials (2 images) arrive as one atlas image plus per-corner UVs.
 
-    python examples/example5_optimize_texture_image.py [--iters 50]
+    python examples/example5_optimize_texture_image.py [--iters 50] [--size 256] [--texture-filter bilinear|trilinear]
+
+A parameter image much larger than its footprint on screen (--size 1024 at the 256 x 256 renders) is minified: bilinear
+sampling then aliases and gives most texels no gradient from a view; --texture-filter trilinear samples a mip pyramid of
+it instead, so every texel receives gradient through the coarser levels.
 """
 import argparse
 import os
@@ -16,7 +20,7 @@ import neural_renderer  # noqa: E402
 from neural_renderer_b200 import io  # noqa: E402
 
 
-def run(iters=50, device="cuda", seed=0, size=256):
+def run(iters=50, device="cuda", seed=0, size=256, texture_filter="bilinear"):
     path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests", "golden", "display", "model.obj")
     v, f, uv, image = io.load_obj(path, load_texture=True, texture_mode="uv")
     vertices = torch.from_numpy(v).to(device)[None]
@@ -26,6 +30,7 @@ def run(iters=50, device="cuda", seed=0, size=256):
     param = torch.zeros((size, size, 3), device=device, requires_grad=True)
     renderer = neural_renderer.Renderer()
     renderer.perspective = False
+    renderer.texture_filter = texture_filter
     optimizer = neural_renderer.Adam([param], lr=0.1, betas=(0.5, 0.999))
     rng = np.random.default_rng(seed)
     losses = []
@@ -45,5 +50,8 @@ def run(iters=50, device="cuda", seed=0, size=256):
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=50)
-    ls = run(ap.parse_args().iters)
+    ap.add_argument("--size", type=int, default=256)
+    ap.add_argument("--texture-filter", default="bilinear", choices=("bilinear", "trilinear"))
+    args = ap.parse_args()
+    ls = run(args.iters, size=args.size, texture_filter=args.texture_filter)
     print("loss: first %.1f -> last %.1f" % (ls[0], ls[-1]))

@@ -91,11 +91,34 @@ extern "C" {
  *   effect on this sampler):  l_k = w_k * (zp / z_k)  (div.rn),  uv = l_0 uv_0 + l_1 uv_1 + l_2 uv_2  (not renormalised).
  *   Addressing as nr_b200_bake_textures: u, v clamped into [0,1] (NaN -> 0), pos_x = u (Wt-1), pos_y = v (Ht-1); taps
  *   ix, ix+1 / iy, iy+1 (clamped into the image; tap row iy is image row Ht-1-iy); bilinear weights products of frac and
- *   1 - frac; fp32, round-to-nearest; clamp to edge only (no wrap, no mipmaps).  face_light multiplies every tap first.
+ *   1 - frac; fp32, round-to-nearest; clamp to edge only (no wrap; NR_TEX_MIPMAP below samples a mip pyramid
+ *   trilinearly instead).  face_light multiplies every tap first.
  *   With NR_TEX_FILL_BACK face f >= F/2 uses the UV corners of face f - F/2 in reverse order (`face_uvs` holds F/2 faces).
  *   The backward fills grad_textures (the image gradient) and grad_face_light; there is NO gradient for face_uvs. */
 #define NR_TEX_UV 0x20000u    /* sample a texture image through per-corner UVs (fields face_uvs / texture_height / _width) */
 #define NR_UV_SHARED 0x40000u /* face_uvs is [F,3,2] and serves every batch item (else [B,F,3,2])                        */
+
+/* Trilinear sampling through a mip pyramid (additive to ABI 4: a flag bit and three entry points, no struct field).
+ *   Only together with NR_TEX_UV.  `textures` is then the PACKED PYRAMID [Bt,P,3]: level 0 (the image, Ht x Wt), then
+ *   level 1, 2, ... in order, each HWC with row 0 = top; `grad_textures` is the gradient of that pyramid (collapse it into
+ *   the image with nr_b200_mip_collapse).  texture_height / texture_width stay the level-0 size.
+ *   Level sizes: H_{l+1} = max(1, (H_l + 1) >> 1), the same for W, until both are 1: L = 1 + ceil(log2(max(Ht, Wt)))
+ *   levels, P = sum_l H_l W_l texels (nr_b200_mip_texels).  A 1x1 image has one level (trilinear = bilinear).
+ *   Building (nr_b200_mip_build), in tap coordinates (x right, y up from the bottom row, row r = H_l-1-y): texel (x, y)
+ *   of level l+1 = ((a + b) + (c + d)) * 0.25 (fp32, round-to-nearest) with a, b = level-l taps (2x, 2y), (2x+1, 2y) and
+ *   c, d = (2x, 2y+1), (2x+1, 2y+1), each clamped into level l (the edge texel of an odd or 1-texel axis counts twice).
+ *   Level of detail per covered raster pixel (raster pixels; anti-aliasing pools on top): with the winner's K1 inverse
+ *   inv[9], weights w, depth zp and own vertex depths z_k,  l_k = w_k zp / z_k,
+ *   d l_k / dx = zp (inv[3k] / z_k - l_k sum_j inv[3j] / z_j)  (y: inv[3k+1]),  du/dx = sum_k u_k d l_k / dx (v, y alike;
+ *   evaluated as sum_{k=1,2} (u_k - u_0) d l_k / dx, equal because sum_k d l_k / dx = 0, without the fp32 cancellation
+ *   of UV corners that lie close together far from 0),
+ *   rho^2 = max(((Wt-1) du/dx)^2 + ((Ht-1) dv/dx)^2, the same in y),  lod = 0.5 log2(rho^2) clamped into [0, L-1]
+ *   (NaN and -inf -> 0).  The derivative ignores the [0,1] clamp of u, v and the clamping of the weights.
+ *   Sample: l0 = floor(lod), l1 = min(l0+1, L-1), f = lod - l0; rgb = (1-f) bilinear_l0 + f bilinear_l1, each level with
+ *   the NR_TEX_UV addressing at its own size; face_light multiplies every tap first; level l1 is not read when f == 0.
+ *   The backward sends (1-f or f) * tap weight * light * grad_rgb to each tap of the pyramid and grad_face_light gets the
+ *   unlit trilinear sample times the upstream gradient.  NO gradient flows through the LOD or into face_uvs. */
+#define NR_TEX_MIPMAP 0x80000u /* textures = packed mip pyramid of the image, sampled trilinearly (needs NR_TEX_UV)        */
 
 typedef struct nr_b200_forward_args {
     uint32_t struct_size; /* sizeof(nr_b200_forward_args), for ABI evolution */
@@ -241,6 +264,21 @@ NR_B200_API int nr_b200_face_lighting_backward(const float *vertices, const int3
 NR_B200_API int nr_b200_bake_textures(const float *image, const float *uv_faces, const int32_t *is_update,
                                       int32_t num_faces, int32_t texture_size, int32_t image_height,
                                       int32_t image_width, float *textures, void *cuda_stream);
+
+/* Mip pyramid of a texture image for NR_TEX_MIPMAP (layout and arithmetic above).
+ *   nr_b200_mip_texels    P for an Ht x Wt image (0 for sizes < 1).  Pure host arithmetic; safe without a GPU.
+ *   nr_b200_mip_build     image [Bt,Ht,Wt,3] -> pyramid [Bt,P,3] (level 0 is a copy).  At most two kernel launches.
+ *   nr_b200_mip_collapse  the exact transpose of the build: grad_pyramid [Bt,P,3] -> grad_image [Bt,Ht,Wt,3]; a child
+ *                         texel receives m_x m_y / 4 of its parent's gradient (m = 2 where the edge clamp counts it
+ *                         twice, else 1).  Writes grad_image, or adds into it with NR_GRAD_ACCUMULATE.  Deterministic
+ *                         (one gather per level-0 texel, no atomics).
+ * Null pointers and sizes < 1 give NR_ERR_INVALID_ARG, pyramids beyond 32-bit offsets NR_ERR_UNSUPPORTED, before any
+ * launch. */
+NR_B200_API size_t nr_b200_mip_texels(int32_t texture_height, int32_t texture_width);
+NR_B200_API int nr_b200_mip_build(const float *image, int32_t batch_size, int32_t texture_height, int32_t texture_width,
+                                  float *pyramid, void *cuda_stream);
+NR_B200_API int nr_b200_mip_collapse(const float *grad_pyramid, int32_t batch_size, int32_t texture_height,
+                                     int32_t texture_width, float *grad_image, uint32_t flags, void *cuda_stream);
 
 /* Number of kernels the last forward/backward call on this thread launched (for launch accounting). */
 NR_B200_API int nr_b200_last_launch_count(void);

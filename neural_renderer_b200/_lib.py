@@ -30,6 +30,7 @@ NR_BWD_PART_FACES = 0x8000
 NR_FWD_STAGE_TEXTURES = 0x10000
 NR_TEX_UV = 0x20000
 NR_UV_SHARED = 0x40000
+NR_TEX_MIPMAP = 0x80000
 
 ABI_VERSION = 4
 
@@ -48,6 +49,9 @@ EXPORTED_SYMBOLS = (
     "nr_b200_face_lighting",
     "nr_b200_face_lighting_backward",
     "nr_b200_bake_textures",
+    "nr_b200_mip_texels",
+    "nr_b200_mip_build",
+    "nr_b200_mip_collapse",
     "nr_b200_last_launch_count",
     "nr_b200_set_profiling",
     "nr_b200_read_profile",
@@ -140,6 +144,13 @@ def load():
                                                                                                 ctypes.c_void_p]
     lib.nr_b200_bake_textures.restype = ctypes.c_int
     lib.nr_b200_bake_textures.argtypes = [ctypes.c_void_p] * 3 + [ctypes.c_int32] * 4 + [ctypes.c_void_p, ctypes.c_void_p]
+    lib.nr_b200_mip_texels.restype = ctypes.c_size_t
+    lib.nr_b200_mip_texels.argtypes = [ctypes.c_int32, ctypes.c_int32]
+    lib.nr_b200_mip_build.restype = ctypes.c_int
+    lib.nr_b200_mip_build.argtypes = [ctypes.c_void_p] + [ctypes.c_int32] * 3 + [ctypes.c_void_p, ctypes.c_void_p]
+    lib.nr_b200_mip_collapse.restype = ctypes.c_int
+    lib.nr_b200_mip_collapse.argtypes = [ctypes.c_void_p] + [ctypes.c_int32] * 3 + [ctypes.c_void_p, ctypes.c_uint32,
+                                                                                   ctypes.c_void_p]
     lib.nr_b200_last_launch_count.restype = ctypes.c_int
     lib.nr_b200_set_profiling.restype = None
     lib.nr_b200_set_profiling.argtypes = [ctypes.c_int]

@@ -26,7 +26,8 @@
 //                     d face_light per run of lanes; neighbouring lanes that blend the same eight texels merge their
 //                     contributions with shuffles before the reductions.
 //   k_image_grad      K6 for a texture image sampled through per-corner UVs (NR_TEX_UV): four bilinear taps per pixel,
-//                     two 6-float horizontal pairs scattered the same way.
+//                     two 6-float horizontal pairs scattered the same way.  k_image_grad_mip: the trilinear variant
+//                     (NR_TEX_MIPMAP), up to four pairs on two levels of the packed pyramid.
 //   k_depth_grad      K7 (rasterize.py:805-847): analytic d zp / d(x, y, z) of the winning face, summed per run of
 //                     neighbouring lanes that show the same face before the atomics.
 //
@@ -70,6 +71,9 @@
 #endif
 #ifndef NR_IG_MIN_CTAS
 #define NR_IG_MIN_CTAS 4        // k_image_grad CTAs of 256 threads per SM (64 registers; see DESIGN.md section 4)
+#endif
+#ifndef NR_IGM_MIN_CTAS
+#define NR_IGM_MIN_CTAS 3       // k_image_grad_mip (trilinear): chosen with -Xptxas -v, see DESIGN.md section 4c
 #endif
 
 namespace {
@@ -125,6 +129,8 @@ struct BwdParams {
     const float* uvs;
     uint32_t uv_bstride, img_bstride;  // floats per item (0 = shared)
     int Ht, Wt;
+    // NR_TEX_MIPMAP (appended likewise): textures / grad_textures = the packed pyramid [Bt,P,3]
+    nr::MipTable mip;
 };
 
 //@phase helpers: rcp / vector RED / load_grad (inlined)
@@ -1066,8 +1072,13 @@ __device__ __forceinline__ void red_add_6(float* t, const float v[6]) {
     }
 }
 
-template <int kTgCombine>
-__global__ void __launch_bounds__(256, NR_IG_MIN_CTAS) k_image_grad(const __grid_constant__ BwdParams p) {
+// kMip (NR_TEX_MIPMAP): trilinear variant.  The pixel's level of detail is recomputed with the forward's nr::mip_lod from
+// the K1 inverse of the same pixel-space vertices (face_inverse(to_pixel(...)), as k_depth_grad) and the saved weight /
+// depth maps, so the taps and level weights are the forward's.  Up to four 6-float pairs (two rows on each of the two
+// levels) go to the packed pyramid; lanes merge only when they hit the same cells on both levels.
+template <int kTgCombine, bool kMip>
+__device__ __forceinline__ void image_grad(const BwdParams& p) {
+    constexpr int kPairs = kMip ? 4 : 2;
     const int S = p.S;
     const size_t plane = (size_t)S * S;
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;  // pixel within the image (image orientation)
@@ -1077,14 +1088,19 @@ __global__ void __launch_bounds__(256, NR_IG_MIN_CTAS) k_image_grad(const __grid
     const bool want_light = p.grad_face_light != nullptr;  // uniform
     if (!want_light && !__any_sync(0xffffffffu, fn >= 0)) return;  // warp-uniform
     float gl0 = 0.0f, gl1 = 0.0f, gl2 = 0.0f;  // d loss / d face_light of this pixel
-    float val[2][6];                           // tap row 0 / 1: taps (x0, x1) x 3 channels
-    float* tp[2] = {nullptr, nullptr};
-    bool adjacent = true;                      // x1 == x0 + 1 (else both taps of a row are the same texel, weight 0 on x1)
+    float val[kPairs][6];                      // tap row 0 / 1 (of level l0, then l1): taps (x0, x1) x 3 channels
+    float* tp[kPairs];
+    bool adjacent[kPairs / 2];                 // x1 == x0 + 1 (else both taps of a row are the same texel, weight 0 on x1)
     long long key = -1 - (long long)lane;      // (image, cell): equal keys <=> the same four texels
+    long long key1 = -1;                       // kMip: the cell on level l1 (-1 when f == 0)
 #pragma unroll
-    for (int r = 0; r < 2; r++)
+    for (int r = 0; r < kPairs; r++) {
+        tp[r] = nullptr;
 #pragma unroll
         for (int k = 0; k < 6; k++) val[r][k] = 0.0f;
+    }
+#pragma unroll
+    for (int r = 0; r < kPairs / 2; r++) adjacent[r] = true;
     if (fn >= 0) {
         const int row = (int)(i / S), col = (int)(i % S);
         const bool aa = (p.flags & NR_ANTI_ALIASING) != 0;
@@ -1095,7 +1111,15 @@ __global__ void __launch_bounds__(256, NR_IG_MIN_CTAS) k_image_grad(const __grid
         const float w[3] = {__ldg(wm), __ldg(wm + plane), __ldg(wm + 2 * plane)};
         const float zp = __ldg(p.dmap + (size_t)b * plane + i);
         float z0, z1, z2;  // the item's own vertex depths, as in the forward sampler
-        if (p.src.idx == nullptr) {
+        float inv[9];
+        if constexpr (kMip) {
+            float c[9];
+            nr::load_face(p.src, b, fn, c);
+            const float fS = (float)S;
+            nr::face_inverse(nr::to_pixel(c[0], fS), nr::to_pixel(c[1], fS), nr::to_pixel(c[3], fS), nr::to_pixel(c[4], fS),
+                             nr::to_pixel(c[6], fS), nr::to_pixel(c[7], fS), inv);
+            z0 = c[2]; z1 = c[5]; z2 = c[8];
+        } else if (p.src.idx == nullptr) {
             const float* v = p.src.faces + ((size_t)b * p.F + fn) * 9;
             z0 = __ldg(v + 2); z1 = __ldg(v + 5); z2 = __ldg(v + 8);
         } else {
@@ -1112,33 +1136,66 @@ __global__ void __launch_bounds__(256, NR_IG_MIN_CTAS) k_image_grad(const __grid
         float uv[6], u, v;
         nr::load_face_uvs(p.uvs + ((uint32_t)b * p.uv_bstride + (uint32_t)uf * 6u), rev, uv);
         nr::pixel_uv(w, zp, z0, z1, z2, uv, u, v);
-        const nr::UvTaps t = nr::uv_taps(u, v, p.Ht, p.Wt);
         const uint32_t img_off = (uint32_t)b * p.img_bstride;
+        // level(s) and their weights: the bilinear variant is level 0 of an image with weight 1
+        int lv[2] = {0, 0};
+        float lw[2] = {1.0f, 0.0f};
+        int nlev = 1;
+        if constexpr (kMip) {
+            const nr::MipLevels m = nr::mip_levels(nr::mip_lod(inv, w, zp, z0, z1, z2, uv, p.Ht, p.Wt, p.mip.levels), p.mip.levels);
+            lv[0] = m.l0; lv[1] = m.l1;
+            lw[0] = __fsub_rn(1.0f, m.f); lw[1] = m.f;
+            nlev = m.f != 0.0f ? 2 : 1;
+        }
+        const nr::UvTaps t0 = nr::uv_taps(u, v, kMip ? p.mip.h[lv[0]] : p.Ht, kMip ? p.mip.w[lv[0]] : p.Wt);
         if (want_light) {  // unlit sample (same blend as the forward pass) times the upstream gradient
             float c[3];
-            nr::uv_blend<false>(p.textures + img_off, p.Wt, t, 1.0f, 1.0f, 1.0f, c);
+            if constexpr (kMip) {
+                nr::MipLevels m;
+                m.l0 = lv[0]; m.l1 = lv[1]; m.f = lw[1];
+                nr::mip_blend<false>(p.textures + img_off, p.mip, m, u, v, 1.0f, 1.0f, 1.0f, c);
+            } else {
+                nr::uv_blend<false>(p.textures + img_off, p.Wt, t0, 1.0f, 1.0f, 1.0f, c);
+            }
             gl0 = c[0] * g0; gl1 = c[1] * g1; gl2 = c[2] * g2;
         }
         if (p.face_light) {  // d rgb / d texel = weight * light
             const float* lp = p.face_light + ((size_t)b * p.F + fn) * 3;
             g0 *= __ldg(lp); g1 *= __ldg(lp + 1); g2 *= __ldg(lp + 2);
         }
-        const uint32_t row3 = (uint32_t)p.Wt * 3u;
         float* gi = p.grad_textures + img_off;
-        tp[0] = gi + (uint32_t)t.r0 * row3 + (uint32_t)t.x0 * 3u;
-        tp[1] = gi + (uint32_t)t.r1 * row3 + (uint32_t)t.x0 * 3u;
-        adjacent = t.x1 != t.x0;
-        key = (long long)(img_off / 3u) + t.cell;
-        val[0][0] = t.w00 * g0; val[0][1] = t.w00 * g1; val[0][2] = t.w00 * g2;
-        val[0][3] = t.w10 * g0; val[0][4] = t.w10 * g1; val[0][5] = t.w10 * g2;
-        val[1][0] = t.w01 * g0; val[1][1] = t.w01 * g1; val[1][2] = t.w01 * g2;
-        val[1][3] = t.w11 * g0; val[1][4] = t.w11 * g1; val[1][5] = t.w11 * g2;
+#pragma unroll
+        for (int q = 0; q < kPairs / 2; q++) {
+            if (q >= nlev) break;
+            const int Hl = kMip ? p.mip.h[lv[q]] : p.Ht, Wl = kMip ? p.mip.w[lv[q]] : p.Wt;
+            const uint32_t loff = kMip ? p.mip.off[lv[q]] : 0u;
+            const nr::UvTaps t = q == 0 ? t0 : nr::uv_taps(u, v, Hl, Wl);
+            const uint32_t row3 = (uint32_t)Wl * 3u;
+            tp[2 * q] = gi + loff + (uint32_t)t.r0 * row3 + (uint32_t)t.x0 * 3u;
+            tp[2 * q + 1] = gi + loff + (uint32_t)t.r1 * row3 + (uint32_t)t.x0 * 3u;
+            adjacent[q] = t.x1 != t.x0;
+            const long long k = (long long)((img_off + loff) / 3u) + t.cell;
+            if (q == 0) key = k; else key1 = k;
+            const float h0 = kMip ? __fmul_rn(lw[q], g0) : g0, h1 = kMip ? __fmul_rn(lw[q], g1) : g1,
+                        h2 = kMip ? __fmul_rn(lw[q], g2) : g2;
+            float* v0 = val[2 * q];
+            float* v1 = val[2 * q + 1];
+            v0[0] = t.w00 * h0; v0[1] = t.w00 * h1; v0[2] = t.w00 * h2;
+            v0[3] = t.w10 * h0; v0[4] = t.w10 * h1; v0[5] = t.w10 * h2;
+            v1[0] = t.w01 * h0; v1[1] = t.w01 * h1; v1[2] = t.w01 * h2;
+            v1[3] = t.w11 * h0; v1[4] = t.w11 * h1; v1[5] = t.w11 * h2;
+        }
     }
     bool issue = fn >= 0;
     if (kTgCombine) {
         // runs of neighbouring lanes with the same key (segmented shuffle of k_texture_grad)
         const long long key_prev = __shfl_up_sync(0xffffffffu, key, 1);
-        const uint32_t heads = __ballot_sync(0xffffffffu, lane == 0 || key != key_prev);
+        bool differs = key != key_prev;
+        if constexpr (kMip) {
+            const long long key1_prev = __shfl_up_sync(0xffffffffu, key1, 1);  // every lane takes part in the shuffle
+            differs = differs || key1 != key1_prev;
+        }
+        const uint32_t heads = __ballot_sync(0xffffffffu, lane == 0 || differs);
         const uint32_t later = heads & ~((2u << lane) - 1u);
         const int run_end = (lane == 31 || later == 0) ? 31 : (__ffs(later) - 2);
         const int run_start = 31 - __clz(heads & ((2u << lane) - 1u));
@@ -1148,7 +1205,7 @@ __global__ void __launch_bounds__(256, NR_IG_MIN_CTAS) k_image_grad(const __grid
                 const int off = 1 << step;
                 const bool take = lane + off <= run_end;
 #pragma unroll
-                for (int r = 0; r < 2; r++)
+                for (int r = 0; r < kPairs; r++)
 #pragma unroll
                     for (int k = 0; k < 6; k++) {
                         const float x = __shfl_down_sync(0xffffffffu, val[r][k], off);
@@ -1160,8 +1217,9 @@ __global__ void __launch_bounds__(256, NR_IG_MIN_CTAS) k_image_grad(const __grid
     }
     if (issue) {
 #pragma unroll
-        for (int r = 0; r < 2; r++) {
-            if (adjacent) {
+        for (int r = 0; r < kPairs; r++) {
+            if (kMip && tp[r] == nullptr) break;  // level l1 has no taps when f == 0
+            if (adjacent[r >> 1]) {
                 red_add_6(tp[r], val[r]);
             } else {
                 float* q = tp[r];
@@ -1186,6 +1244,15 @@ __global__ void __launch_bounds__(256, NR_IG_MIN_CTAS) k_image_grad(const __grid
         float* gl = p.grad_face_light + ((size_t)b * p.F + fn) * 3;
         atomicAdd(gl, gl0); atomicAdd(gl + 1, gl1); atomicAdd(gl + 2, gl2);
     }
+}
+
+template <int kTgCombine>
+__global__ void __launch_bounds__(256, NR_IG_MIN_CTAS) k_image_grad(const __grid_constant__ BwdParams p) {
+    image_grad<kTgCombine, false>(p);
+}
+template <int kTgCombine>
+__global__ void __launch_bounds__(256, NR_IGM_MIN_CTAS) k_image_grad_mip(const __grid_constant__ BwdParams p) {
+    image_grad<kTgCombine, true>(p);
 }
 
 // ----------------------------------------------------------------------------------------------- k_depth_grad
@@ -1359,6 +1426,8 @@ extern "C" int nr_b200_backward(const nr_b200_backward_args* a, void* cuda_strea
     const bool rgb = (flags & NR_RETURN_RGB) != 0, alpha = (flags & NR_RETURN_ALPHA) != 0, depth = (flags & NR_RETURN_DEPTH) != 0;
     const bool uv = (flags & NR_TEX_UV) != 0;
     if (uv && (!rgb || !a->face_uvs || a->texture_height < 1 || a->texture_width < 1)) return NR_ERR_INVALID_ARG;
+    const bool mip = (flags & NR_TEX_MIPMAP) != 0;
+    if (mip && !uv) return NR_ERR_INVALID_ARG;
     if (rgb && (!a->rgb_map || (!uv && ts < 2))) return NR_ERR_INVALID_ARG;
     if (rgb && part_tex && !a->grad_textures) return NR_ERR_INVALID_ARG;
     if (rgb && (flags & NR_TEX_FILL_BACK) && (F & 1)) return NR_ERR_INVALID_ARG;
@@ -1368,8 +1437,11 @@ extern "C" int nr_b200_backward(const nr_b200_backward_args* a, void* cuda_strea
     if ((size_t)B * F * 2 * kWideStrips >= (size_t)0x7FFFFFFF) return NR_ERR_UNSUPPORTED;  // 32-bit list offsets
     const size_t ncubes = (flags & NR_TEX_FILL_BACK) ? (size_t)F / 2 : (size_t)F;
     const size_t tex_items = (flags & NR_TEX_SHARED) ? 1 : (size_t)B;
-    // NR_TEX_UV: the image gradient [Bt,Ht,Wt,3] (the zero-fill below and the edge scan's side fill are sized from it)
-    const size_t img_floats = uv ? (size_t)a->texture_height * (size_t)a->texture_width * 3 : 0;
+    // NR_TEX_UV: the image gradient [Bt,Ht,Wt,3], NR_TEX_MIPMAP: the pyramid gradient [Bt,P,3] (the zero-fill below and the
+    // edge scan's side fill are sized from it)
+    nr::MipTable mt{};
+    const size_t img_floats = mip ? nr::mip_table(a->texture_height, a->texture_width, &mt) * 3
+                                  : (uv ? (size_t)a->texture_height * (size_t)a->texture_width * 3 : 0);
     const size_t uv_floats = ncubes * 6;
     if (uv && (tex_items * img_floats > 0x7FFFFFFFull || uv_floats * ((flags & NR_UV_SHARED) ? 1 : (size_t)B) > 0x7FFFFFFFull))
         return NR_ERR_UNSUPPORTED;  // 32-bit image / UV offsets in the kernels
@@ -1421,10 +1493,16 @@ extern "C" int nr_b200_backward(const nr_b200_backward_args* a, void* cuda_strea
         p.uv_bstride = (flags & NR_UV_SHARED) ? 0u : (uint32_t)uv_floats;
         p.img_bstride = (flags & NR_TEX_SHARED) ? 0u : (uint32_t)img_floats;
         p.Ht = a->texture_height; p.Wt = a->texture_width;
+        if (mip) p.mip = mt;
     }
 
     const dim3 pgrid((unsigned)(((size_t)S * S + 255) / 256), B);
     auto launch_texture_grad = [&]() {
+        if (mip) {
+            nr_internal::LaunchScope ls("k_image_grad", stream);
+            k_image_grad_mip<NR_TG_COMBINE><<<pgrid, 256, 0, stream>>>(p);
+            return;
+        }
         if (uv) {
             nr_internal::LaunchScope ls("k_image_grad", stream);
             k_image_grad<NR_TG_COMBINE><<<pgrid, 256, 0, stream>>>(p);

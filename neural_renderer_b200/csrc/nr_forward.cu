@@ -61,6 +61,10 @@ constexpr int kOwnTable = 256;         // rows / fragments per pass whose owner 
                                // latency-bound on its dependent gathers; 8 CTAs = 32 registers spill on sm_90 and were
                                // measured slower on H100: 121 vs 114 us at the headline shape)
 #endif
+#ifndef NR_RESOLVE_MIP_MIN_CTAS
+#define NR_RESOLVE_MIP_MIN_CTAS 4  // the trilinear variants (kTex == 3): 64 registers; at 5 or 6 CTAs (48 / 40 registers)
+                                   // they spill (-Xptxas -v)
+#endif
 constexpr int kResolveTileW = 32, kResolveTileH = 8;  // API pixels per k_resolve CTA (256 threads, 8 x 4 per warp)
 constexpr uint32_t kStageBytes = 32 * 1024;  // shared memory of a k_resolve CTA for staged texture cubes
 
@@ -95,6 +99,8 @@ struct FwdParams {
     uint32_t uv_bstride;   // floats per item in face_uvs (0 with NR_UV_SHARED)
     uint32_t img_bstride;  // floats per item in the image (0 with NR_TEX_SHARED)
     int Ht, Wt;
+    // NR_TEX_MIPMAP (appended likewise): `textures` is the packed pyramid, img_bstride its floats per item
+    nr::MipTable mip;
 };
 
 // rasterize.py:291-292  xp = (2 * xi + 1 - is) / is evaluated in double and rounded to float.  Both operands are
@@ -437,8 +443,9 @@ __device__ __forceinline__ int face_cube(const FwdParams& p, int fn, bool& rev) 
 }
 
 // one pixel, every texel straight from global memory (anti-aliased quads, texture sizes the bulk copy cannot stage);
-// kUV: bilinear sample of the texture image at the pixel's perspective-correct UV instead of the ts^3 cube
-template <bool kLit, bool kUV = false>
+// kUV: bilinear sample of the texture image at the pixel's perspective-correct UV instead of the ts^3 cube; kMip:
+// trilinear sample of its mip pyramid at the pixel's level of detail
+template <bool kLit, bool kUV = false, bool kMip = false>
 __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigned long long key, int xi, int yi, float bgr,
                                               float bgg, float bgb) {
     Shaded o;
@@ -463,14 +470,20 @@ __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigne
             float uv[6], u, v;
             nr::load_face_uvs(p.uvs + ((uint32_t)b * p.uv_bstride + (uint32_t)uf * 6u), rev, uv);
             nr::pixel_uv(w, zp, cc.y, cc.z, cc.w, uv, u, v);
-            const nr::UvTaps t = nr::uv_taps(u, v, p.Ht, p.Wt);
             float l0 = 1.0f, l1 = 1.0f, l2 = 1.0f;
             if (kLit) {
                 const float* lp = p.face_light + ((size_t)b * p.F + fn) * 3;
                 l0 = __ldg(lp); l1 = __ldg(lp + 1); l2 = __ldg(lp + 2);
             }
             float c[3];
-            nr::uv_blend<kLit>(p.textures + (uint32_t)b * p.img_bstride, p.Wt, t, l0, l1, l2, c);
+            if constexpr (kMip) {
+                const float lod = nr::mip_lod(inv, w, zp, cc.y, cc.z, cc.w, uv, p.Ht, p.Wt, p.mip.levels);
+                nr::mip_blend<kLit>(p.textures + (uint32_t)b * p.img_bstride, p.mip, nr::mip_levels(lod, p.mip.levels), u, v,
+                                    l0, l1, l2, c);
+            } else {
+                const nr::UvTaps t = nr::uv_taps(u, v, p.Ht, p.Wt);
+                nr::uv_blend<kLit>(p.textures + (uint32_t)b * p.img_bstride, p.Wt, t, l0, l1, l2, c);
+            }
             o.r = c[0]; o.g = c[1]; o.b = c[2];
         } else {
             float z0, z1, z2;
@@ -502,10 +515,12 @@ __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigne
 // therefore the default.
 //
 // kTex == 2 (NR_TEX_UV): the direct variants with the texture-image sampler (shade_pixel<kLit, true>), same tile map.
+// kTex == 3 (NR_TEX_UV | NR_TEX_MIPMAP): the same with the trilinear pyramid sampler (shade_pixel<kLit, true, true>).
 template <bool kAA, int kTex, bool kLit>
-__global__ void __launch_bounds__(256, kAA ? 5 : NR_RESOLVE_MIN_CTAS) k_resolve(const __grid_constant__ FwdParams p, int nslots) {
+__global__ void __launch_bounds__(256, kTex == 3 ? NR_RESOLVE_MIP_MIN_CTAS : (kAA ? 5 : NR_RESOLVE_MIN_CTAS)) k_resolve(const __grid_constant__ FwdParams p, int nslots) {
     constexpr bool kStage = kTex == 1;  // kTex: 0 = every texel straight from global memory, 1 = cubes staged with cp.async.bulk
-    constexpr bool kUV = kTex == 2;     //       2 = texture image through per-corner UVs
+    constexpr bool kUV = kTex >= 2;     //       2 = texture image through per-corner UVs, 3 = its mip pyramid
+    constexpr bool kMip = kTex == 3;
     extern __shared__ __align__(16) unsigned char stage_raw[];
     __shared__ uint64_t s_bar;
     __shared__ int s_runs[8];
@@ -600,7 +615,7 @@ __global__ void __launch_bounds__(256, kAA ? 5 : NR_RESOLVE_MIN_CTAS) k_resolve(
         // thread = one pixel of the IMAGE (row 0 = top): raster row yi = S - 1 - row
         const int row = row2, yi = S - 1 - row;
         if (col >= S || row >= S) return;
-        const Shaded s = shade_pixel<kLit, kUV>(p, b, __ldg(zb + (uint32_t)yi * S + col), col, yi, bgr, bgg, bgb);
+        const Shaded s = shade_pixel<kLit, kUV, kMip>(p, b, __ldg(zb + (uint32_t)yi * S + col), col, yi, bgr, bgg, bgb);
         const uint32_t o = (uint32_t)row * S + col;
         // streaming stores: 134 MB of maps that nothing reads again before the backward pass should not push the
         // z-buffer, the face records and the texture cubes out of the L2
@@ -622,7 +637,7 @@ __global__ void __launch_bounds__(256, kAA ? 5 : NR_RESOLVE_MIN_CTAS) k_resolve(
         for (int k = 0; k < 4; k++) {
             const int row = 2 * orow + (k >> 1), xi = 2 * col + (k & 1);
             const int yi = S - 1 - row;
-            const Shaded s = shade_pixel<kLit, kUV>(p, b, __ldg(zb + (uint32_t)yi * S + xi), xi, yi, bgr, bgg, bgb);
+            const Shaded s = shade_pixel<kLit, kUV, kMip>(p, b, __ldg(zb + (uint32_t)yi * S + xi), xi, yi, bgr, bgg, bgb);
             const uint32_t o = (uint32_t)row * S + xi;
             __stcs(fim + o, s.fim);
             __stcs(dmap + o, s.depth);
@@ -692,10 +707,14 @@ extern "C" int nr_b200_forward(const nr_b200_forward_args* a, void* cuda_stream)
         if ((flags & NR_BG_PER_BATCH) && !a->background_batch) return NR_ERR_INVALID_ARG;
     }
     if (uv && (!(flags & NR_RETURN_RGB) || !a->face_uvs || a->texture_height < 1 || a->texture_width < 1)) return NR_ERR_INVALID_ARG;
+    const bool mip = (flags & NR_TEX_MIPMAP) != 0;
+    if (mip && !uv) return NR_ERR_INVALID_ARG;
     if ((flags & NR_ANTI_ALIASING) && (S & 1)) return NR_ERR_INVALID_ARG;
     if (S > 32767 || B > 65535) return NR_ERR_UNSUPPORTED;  // 32-bit pixel offsets; batch = grid.z of the resolve pass
-    // NR_TEX_UV: image and UV offsets are 32-bit in the kernels
-    const size_t img_floats = uv ? (size_t)a->texture_height * (size_t)a->texture_width * 3 : 0;
+    // NR_TEX_UV: image (NR_TEX_MIPMAP: pyramid) and UV offsets are 32-bit in the kernels
+    nr::MipTable mt{};
+    const size_t img_floats = mip ? nr::mip_table(a->texture_height, a->texture_width, &mt) * 3
+                                  : (uv ? (size_t)a->texture_height * (size_t)a->texture_width * 3 : 0);
     const size_t uv_floats = (size_t)((flags & NR_TEX_FILL_BACK) ? F / 2 : F) * 6;
     if (uv && (img_floats * ((flags & NR_TEX_SHARED) ? 1 : B) > 0x7FFFFFFFull ||
                uv_floats * ((flags & NR_UV_SHARED) ? 1 : B) > 0x7FFFFFFFull))
@@ -723,6 +742,7 @@ extern "C" int nr_b200_forward(const nr_b200_forward_args* a, void* cuda_stream)
         p.uv_bstride = (flags & NR_UV_SHARED) ? 0u : (uint32_t)uv_floats;
         p.img_bstride = (flags & NR_TEX_SHARED) ? 0u : (uint32_t)img_floats;
         p.Ht = a->texture_height; p.Wt = a->texture_width;
+        if (mip) p.mip = mt;
     }
     p.fim = a->face_index_map; p.wmap = a->weight_map; p.dmap = a->depth_map; p.rgb = a->rgb_map; p.alpha = a->alpha_map;
     p.out_rgb = a->out_rgb; p.out_alpha = a->out_alpha; p.out_depth = a->out_depth;
@@ -796,7 +816,9 @@ extern "C" int nr_b200_forward(const nr_b200_forward_args* a, void* cuda_stream)
             bx = 256;
             grid = dim3((width + kResolveTileW - 1) / kResolveTileW, (width + kResolveTileH - 1) / kResolveTileH, B);
         }
-        if (uv && aa) NR_RESOLVE_LIT(true, 2);
+        if (mip && aa) NR_RESOLVE_LIT(true, 3);
+        else if (mip) NR_RESOLVE_LIT(false, 3);
+        else if (uv && aa) NR_RESOLVE_LIT(true, 2);
         else if (uv) NR_RESOLVE_LIT(false, 2);
         else if (aa) NR_RESOLVE_LIT(true, 0);
         else if (stage) NR_RESOLVE_LIT(false, 1);

@@ -58,6 +58,8 @@ class overlap_texture_allreduce:
     the collective; after the second half is enqueued the compute stream waits for the collective, so what autograd
     accumulates into `textures.grad` is already the global sum.  The collective is linear, so this is correct for a
     shared texture set ([1,F,...], NR_TEX_SHARED: 96 MB at 1 M faces / ts 2) and for per-item textures alike.
+    With texture_filter='trilinear' the hook receives the gradient of the mip pyramid (about 4/3 of the image); the
+    collapse into the image runs afterwards on every rank and is linear too, so the image gradient is the same global sum.
     With one rank, or outside an initialised process group, the hook does nothing.
     """
 

@@ -143,7 +143,7 @@ def set_texture_grad_hook(hook):
 
 
 class _Config:
-    __slots__ = ("S", "aa", "near", "far", "eps", "bg", "bg_batch", "flags", "reference_exact")
+    __slots__ = ("S", "aa", "near", "far", "eps", "bg", "bg_batch", "flags", "reference_exact", "mip_hw")
 
 
 def _make_config(image_size, anti_aliasing, near, far, eps, background_color, return_rgb, return_alpha, return_depth,
@@ -154,6 +154,7 @@ def _make_config(image_size, anti_aliasing, near, far, eps, background_color, re
     cfg.aa = bool(anti_aliasing)
     cfg.S = int(image_size) * 2 if cfg.aa else int(image_size)
     cfg.near, cfg.far, cfg.eps = float(near), float(far), float(eps)
+    cfg.mip_hw = None  # (Ht, Wt) of level 0 when `textures` is a packed mip pyramid (NR_TEX_MIPMAP)
     flags = 0
     if return_rgb:
         flags |= _lib.NR_RETURN_RGB
@@ -226,6 +227,8 @@ class _RasterizeFunction(torch.autograd.Function):
                 flags |= _lib.NR_UV_SHARED
             ts = 0
         tex_hw = (int(tex_c.shape[1]), int(tex_c.shape[2])) if uv_c is not None else (0, 0)
+        if uv_c is not None and cfg.mip_hw is not None:
+            tex_hw = cfg.mip_hw  # `textures` is the packed pyramid [Bt,P,3] of an Ht x Wt image
         want_rgb = bool(flags & _lib.NR_RETURN_RGB)
         want_alpha = bool(flags & _lib.NR_RETURN_ALPHA)
         want_depth = bool(flags & _lib.NR_RETURN_DEPTH)
@@ -338,8 +341,45 @@ class _RasterizeFunction(torch.autograd.Function):
         return grad_geom, grad_textures, grad_light, None, None, None
 
 
+class _MipPyramid(torch.autograd.Function):
+    """image [Bt,Ht,Wt,3] -> packed mip pyramid [Bt,P,3] (nr_b200_mip_build); the backward collapses the pyramid gradient
+    into the image gradient (nr_b200_mip_collapse, the exact transpose of the build)."""
+
+    @staticmethod
+    def forward(ctx, image):
+        lib = _lib.load()
+        img = image.detach().contiguous()
+        Bt, H, W = (int(n) for n in img.shape[:3])
+        P = int(lib.nr_b200_mip_texels(H, W))
+        dev = img.device
+        with torch.cuda.device(dev):
+            pyr = torch.empty((Bt, P, 3), dtype=torch.float32, device=dev)
+            _lib.check(lib.nr_b200_mip_build(_ptr(img), Bt, H, W, _ptr(pyr), _stream_ptr(dev)))
+        ctx.shape = (Bt, H, W)
+        return pyr
+
+    @staticmethod
+    def backward(ctx, grad_pyr):
+        lib = _lib.load()
+        Bt, H, W = ctx.shape
+        g = grad_pyr.detach().to(torch.float32).contiguous()
+        dev = g.device
+        with torch.cuda.device(dev):
+            grad_image = torch.empty((Bt, H, W, 3), dtype=torch.float32, device=dev)
+            _lib.check(lib.nr_b200_mip_collapse(_ptr(g), Bt, H, W, _ptr(grad_image), 0, _stream_ptr(dev)))
+        return grad_image
+
+
+TEXTURE_FILTERS = ('bilinear', 'trilinear')
+
+
 def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_color, return_rgb, return_alpha,
-         return_depth, face_light=None, textures_fill_back=False, vertices=None, reference_exact=None, face_uvs=None):
+         return_depth, face_light=None, textures_fill_back=False, vertices=None, reference_exact=None, face_uvs=None,
+         texture_filter='bilinear'):
+    if texture_filter not in TEXTURE_FILTERS:
+        raise ValueError("texture_filter must be one of %s, got %r" % (TEXTURE_FILTERS, texture_filter))
+    if texture_filter == 'trilinear' and face_uvs is None:
+        raise ValueError("texture_filter='trilinear' samples a texture image: it needs face_uvs")
     _check_inputs(faces, textures, return_rgb, face_light, textures_fill_back, vertices, face_uvs)
     indices = None
     if vertices is not None:
@@ -372,6 +412,12 @@ def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_
         cfg.flags |= _lib.NR_TEX_FILL_BACK
     if return_rgb and _STAGE_TEXTURES:
         cfg.flags |= _lib.NR_FWD_STAGE_TEXTURES
+    if return_rgb and texture_filter == 'trilinear':
+        # the pyramid is built from the image (shared or per item, as the image is) and autograd chains its gradient
+        # back into the image
+        cfg.mip_hw = (int(textures.shape[1]), int(textures.shape[2]))
+        cfg.flags |= _lib.NR_TEX_MIPMAP
+        textures = _MipPyramid.apply(textures)
     return _RasterizeFunction.apply(geom, textures if return_rgb else None, face_light if return_rgb else None, cfg,
                                     indices, face_uvs)
 
@@ -394,6 +440,7 @@ def rasterize_rgbad(
         vertices=None,
         reference_exact=None,
         face_uvs=None,
+        texture_filter='bilinear',
 ):
     """Generate RGB, alpha channel, and depth images from faces and textures (for RGB).  rasterize.py:900-977.
 
@@ -418,11 +465,15 @@ def rasterize_rgbad(
                               the bottom; F/2 faces with textures_fill_back).  Sampled bilinearly (clamp to edge) at the
                               perspective-correct UV, with every item's own vertex depths (`reference_exact` has no
                               effect).  The image receives a gradient, face_uvs does not.
+      texture_filter          'bilinear' (default) or 'trilinear' (texture-image mode only): sample a mip pyramid of the
+                              image at each pixel's level of detail, so minified images neither alias nor leave most
+                              texels without gradient.  The pyramid is rebuilt from the image on every call and its
+                              gradient collapsed back into the image; no gradient flows through the level of detail.
     `textures` with batch size 1 (or an expanded stride-0 batch) while the geometry batch is larger = one texture set
     shared by every item (a mesh seen from B viewpoints, mesh.py:29-34); its gradient is the sum over the items."""
     rgb, alpha, depth, _, _ = _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_color,
                                    return_rgb, return_alpha, return_depth, face_light, textures_fill_back, vertices,
-                                   reference_exact, face_uvs)
+                                   reference_exact, face_uvs, texture_filter)
     return {
         'rgb': rgb if return_rgb else None,
         'alpha': alpha if return_alpha else None,
@@ -445,12 +496,13 @@ def rasterize(
         vertices=None,
         reference_exact=None,
         face_uvs=None,
+        texture_filter='bilinear',
 ):
     """RGB images [B,3,H,W] from faces and textures.  rasterize.py:980-1008 (keyword-only extras: rasterize_rgbad)."""
     return rasterize_rgbad(
         faces, textures, image_size, anti_aliasing, near, far, eps, background_color, True, False, False,
         face_light=face_light, textures_fill_back=textures_fill_back, vertices=vertices,
-        reference_exact=reference_exact, face_uvs=face_uvs)['rgb']
+        reference_exact=reference_exact, face_uvs=face_uvs, texture_filter=texture_filter)['rgb']
 
 
 def rasterize_silhouettes(

@@ -42,6 +42,9 @@ class Renderer(object):
         # None = module default (reference-exact, see neural_renderer_b200.set_reference_exact); False = every item with
         # its own depths (batches of different meshes / cameras, viewpoint shards of a multi-GPU run)
         self.reference_exact = None
+        # sampler of a texture image (render(..., face_uvs=...)): 'bilinear', or 'trilinear' through a mip pyramid of the
+        # image (minified images neither alias nor leave texels without gradient); per-face cubes ignore it
+        self.texture_filter = 'bilinear'
 
     def _transform(self, vertices):
         # renderer.py:41-50 (look_at / look, then perspective), fused into one kernel on CUDA
@@ -86,7 +89,8 @@ class Renderer(object):
     def render(self, vertices, faces, textures, face_uvs=None):
         """RGB images [B,3,H,W].  `textures` are per-face cubes [B,F,ts,ts,ts,3], or -- with `face_uvs` [F,3,2] /
         [B,F,3,2] (UV of every face corner, OBJ convention) -- a texture image [Ht,Wt,3] / [1|B,Ht,Wt,3] (row 0 = top),
-        sampled bilinearly at the perspective-correct UV (neural_renderer_b200.rasterize_rgbad)."""
+        sampled at the perspective-correct UV with `self.texture_filter` (neural_renderer_b200.rasterize_rgbad)."""
+        texture_filter = self.texture_filter if face_uvs is not None else 'bilinear'
         fused = (self.fused and self._fusable(vertices, faces) and textures.is_cuda and textures.dtype == torch.float32)
         light_args = (self.light_intensity_ambient, self.light_intensity_directional, self.light_color_ambient,
                       self.light_color_directional, self.light_direction)
@@ -99,7 +103,8 @@ class Renderer(object):
             return rasterize(
                 indices, textures, self.image_size, self.anti_aliasing, self.near, self.far, self.rasterizer_eps,
                 self.background_color, face_light=light, textures_fill_back=self.fill_back,
-                vertices=self._transform(vertices), reference_exact=self.reference_exact, face_uvs=face_uvs)
+                vertices=self._transform(vertices), reference_exact=self.reference_exact, face_uvs=face_uvs,
+                texture_filter=texture_filter)
         if face_uvs is not None:
             # op by op: materialised faces, the light factor of those faces (F.face_light), doubled UV corners for fill_back
             if self.fill_back:
@@ -109,7 +114,8 @@ class Renderer(object):
             faces = F.vertices_to_faces(self._transform(vertices), faces)
             return rasterize(
                 faces, textures, self.image_size, self.anti_aliasing, self.near, self.far, self.rasterizer_eps,
-                self.background_color, face_light=light, reference_exact=self.reference_exact, face_uvs=face_uvs)
+                self.background_color, face_light=light, reference_exact=self.reference_exact, face_uvs=face_uvs,
+                texture_filter=texture_filter)
         if self.fill_back:
             faces = torch.cat((faces, faces.flip(2)), dim=1)
             textures = torch.cat((textures, textures.permute(0, 1, 4, 3, 2, 5)), dim=1)

@@ -6,9 +6,13 @@ backward with a dense N(0,1) upstream gradient (bench.py's headline step).  Text
   uv_shared_1024   one 1024 x 1024 image shared by every item (NR_TEX_SHARED), spherical UVs shared (NR_UV_SHARED)
   uv_item_256      one 256 x 256 image per item, spherical UVs shared
   cubes_ts4        the per-item ts = 4 cubes of bench.py
+  uv_shared_1024_trilinear, uv_item_256_trilinear   the two image variants with texture_filter='trilinear': the mip
+                   pyramid is built (k_mip_build) and its gradient collapsed (k_mip_collapse) on every step
 Whole step: CUDA events around `steps` steps after `warmup` warm-up steps, median over `reps` repetitions.  Per kernel:
 the library's own CUDA-event profiler over `steps` further steps (ms per step).  Bytes held = texture + its gradient.
-The roofline fraction of the image-gradient kernel and of the zero-fill uses bench.py's HBM figure.
+The roofline fraction of the image-gradient kernel and of the zero-fill uses bench.py's HBM figure.  For every image
+variant, `lod_above_0` is the share of covered pixels whose trilinear level of detail is above 0 (how much the geometry
+minifies the image), computed once with torch from the saved maps and not timed.
 
     python tools/bench_uv.py [--steps 20] [--warmup 3] [--reps 5]
 """
@@ -20,6 +24,7 @@ import sys
 
 import numpy as np
 import torch
+import torch.nn.functional
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -33,6 +38,33 @@ def hbm_gbs():
         with open(path) as f:
             return float(json.load(f)["hbm_gbs"])
     return 3350.0
+
+
+def lod_above_0(faces, uvs, Ht, Wt, S):
+    """share of covered pixels with a level of detail above 0 (include/nr_b200.h, NR_TEX_MIPMAP), float64 from the faces
+    and the product's own face_index_map / weight_map / depth map"""
+    R = sys.modules["neural_renderer_b200.rasterize"]
+    with torch.no_grad():
+        _, _, dmap, fim, wmap = R._run(faces, None, S, False, 0.1, 100, 1e-4, None, False, False, True)
+        B = faces.shape[0]
+        f64 = faces.double()
+        px, py = 0.5 * (f64[..., 0] * S + S - 1), 0.5 * (f64[..., 1] * S + S - 1)
+        M = torch.linalg.inv_ex(torch.stack((px, py, torch.ones_like(px)), dim=-2)).inverse
+        cov = fim >= 0
+        fi = fim.clamp(min=0).long()
+        bidx = torch.arange(B, device=faces.device)[:, None, None].expand_as(fi)
+        Mp, z = M[bidx, fi], f64[..., 2][bidx, fi]
+        uvk = uvs.double().expand(B, -1, -1, -1)[bidx, fi]
+        zp = dmap.double()[..., None]
+        lam = wmap.double().permute(0, 2, 3, 1) * (zp / z)
+        rho2 = []
+        for d in (0, 1):
+            q = Mp[..., d] / z
+            dl = zp * (q - lam * q.sum(-1, keepdim=True))
+            du, dv = (uvk[..., 0] * dl).sum(-1) * (Wt - 1), (uvk[..., 1] * dl).sum(-1) * (Ht - 1)
+            rho2.append(du * du + dv * dv)
+        lod = torch.nan_to_num(0.5 * torch.log2(torch.maximum(*rho2)), nan=0.0, neginf=0.0)
+        return float((lod[cov] > 0).double().mean())
 
 
 def main():
@@ -49,21 +81,26 @@ def main():
     faces = torch.from_numpy(synthetic.sphere_faces(B, F)).to(dev).requires_grad_(True)
     uvs = torch.from_numpy(synthetic.sphere_uvs(F)).to(dev)
     g = torch.randn((B, 3, S, S), generator=torch.Generator().manual_seed(0)).to(dev)
+    img1024 = torch.from_numpy(synthetic.random_image(1, 1024, 1024)[0]).to(dev)
+    img256 = torch.from_numpy(synthetic.random_image(B, 256, 256)).to(dev)
     variants = collections.OrderedDict([
-        ("uv_shared_1024", (torch.from_numpy(synthetic.random_image(1, 1024, 1024)[0]).to(dev), uvs)),
-        ("uv_item_256", (torch.from_numpy(synthetic.random_image(B, 256, 256)).to(dev), uvs)),
-        ("cubes_ts4", (torch.from_numpy(synthetic.random_textures(B, F, 4)).to(dev), None)),
+        ("uv_shared_1024", (img1024, uvs, "bilinear")),
+        ("uv_item_256", (img256, uvs, "bilinear")),
+        ("cubes_ts4", (torch.from_numpy(synthetic.random_textures(B, F, 4)).to(dev), None, "bilinear")),
+        ("uv_shared_1024_trilinear", (img1024, uvs, "trilinear")),
+        ("uv_item_256_trilinear", (img256, uvs, "trilinear")),
     ])
     lib = _lib.load()
-    out = {"gpu": torch.cuda.get_device_name(dev), "shape": {"batch": B, "faces": F, "size": S, "anti_aliasing": False},
+    props = torch.cuda.get_device_properties(dev)
+    out = {"gpu": torch.cuda.get_device_name(dev), "sm_count": props.multi_processor_count, "shape": {"batch": B, "faces": F, "size": S, "anti_aliasing": False},
            "hbm_gbs": hbm_gbs(), "variants": {}}
-    for name, (tex0, fuv) in variants.items():
+    for name, (tex0, fuv, tf) in variants.items():
         tex = tex0.clone().requires_grad_(True)
 
         def step():
             faces.grad = None
             tex.grad = None
-            img = nr.rasterize(faces, tex, S, False, face_uvs=fuv)
+            img = nr.rasterize(faces, tex, S, False, face_uvs=fuv, texture_filter=tf)
             img.backward(g)
 
         for _ in range(a.warmup):
@@ -89,8 +126,12 @@ def main():
         for k, ms in prof:
             kern[k] = kern.get(k, 0.0) + ms / a.steps
         tex_bytes = tex.numel() * 4
-        rec = {"step_ms_median": float(np.median(reps)), "step_ms_reps": reps,
+        if tf == "trilinear":  # the rasterizer samples (and its gradient is) the pyramid
+            tex_bytes = tex.numel() // (tex.shape[-3] * tex.shape[-2]) * lib.nr_b200_mip_texels(*tex.shape[-3:-1]) * 4
+        rec = {"texture_filter": tf, "step_ms_median": float(np.median(reps)), "step_ms_reps": reps,
                "kernels_ms_per_step": kern, "texture_bytes": tex_bytes, "texture_plus_grad_bytes": 2 * tex_bytes}
+        if fuv is not None:
+            rec["lod_above_0"] = lod_above_0(faces.detach(), fuv[None], tex.shape[-3], tex.shape[-2], S)
         grad_kernel = "k_image_grad" if fuv is not None else "k_texture_grad"
         if grad_kernel in kern:
             rec["grad_kernel"] = grad_kernel
