@@ -59,7 +59,8 @@ extern "C" {
 #define NR_BG_PER_BATCH 16u   /* background_color given as [B,3] (rasterize.py:464-465) in `background_batch`  */
 #define NR_TEX_Z_BATCH0 32u   /* reproduce rasterize.py:389: the texture sampler reads vertex depths of batch  */
                               /* item 0 (reference-exact; clear it for per-item depths)                        */
-#define NR_GRAD_ACCUMULATE 64u /* backward: add into grad_faces / grad_textures instead of zero-filling first */
+#define NR_GRAD_ACCUMULATE 64u /* backward: add into grad_faces | grad_vertices, grad_textures, grad_face_light    */
+                               /* instead of zero-filling them first (also for each call of a two-part backward) */
 #define NR_TEX_FILL_BACK 0x400u /* Renderer.fill_back without materialising the doubled texture tensor            */
                                 /* (renderer.py:78-80): F is even, faces [F/2, F) are the reversed copies of      */
                                 /* [0, F/2); `textures` / `grad_textures` hold F/2 cubes and face f >= F/2 samples */
@@ -134,7 +135,7 @@ typedef struct nr_b200_forward_args {
     float _pad0;
     const float *faces;            /* [B,F,3,3]  x,y in NDC [-1,1], z = camera depth                            */
     const float *textures;         /* [B,F,ts,ts,ts,3] ([F,...] with NR_TEX_SHARED) or NULL                     */
-    const float *background_batch; /* [B,3] device, only with NR_BG_PER_BATCH                                   */
+    const float *background_batch; /* [B,3] device, only with NR_BG_PER_BATCH; read only with NR_RETURN_RGB     */
     /* raster-resolution maps, saved for the backward pass (all required unless noted) */
     int32_t *face_index_map; /* [B,S,S]   -1 where empty                                                      */
     float *weight_map;       /* [B,3,S,S] barycentric weights of the winning face, 0 where empty              */
@@ -189,7 +190,8 @@ typedef struct nr_b200_backward_args {
     const float *face_light; /* [B,F,3] as given to the forward call, or NULL */
     float *grad_face_light;  /* [B,F,3] or NULL */
     /* ABI 3: indexed geometry as in the forward call; with NR_FACES_INDEXED the face gradient is reduced into
-     * grad_vertices [B,Nv,3] (zero-filled first unless NR_GRAD_ACCUMULATE) and grad_faces may be NULL. */
+     * grad_vertices [B,Nv,3] (zero-filled first unless NR_GRAD_ACCUMULATE); grad_faces is then neither read nor written
+     * and may be NULL. */
     const float *vertices;
     const int32_t *face_indices;
     float *grad_vertices; /* [B,Nv,3] */
@@ -229,8 +231,9 @@ NR_B200_API int nr_b200_vertices_to_faces_backward(const float *grad_faces, cons
  *   d = vertices[b,v,:] - eye[b];   o = rot[b] * d   (rows of rot = camera x, y, z axes; rot NULL = identity,
  *   eye NULL = origin);   with NR_CAM_PERSPECTIVE:  out = (o.x / o.z / width[b], o.y / o.z / width[b], o.z)
  * rot [B,9], eye [B,3], width [B] are device arrays; with NR_CAM_SHARED they hold ONE camera used by every item.
- * The backward writes grad_vertices [B,Nv,3] (may be NULL) and accumulates, per camera, grad_rot [.,9], grad_eye
- * [.,3], grad_width [.] (each may be NULL; zero-filled first unless NR_GRAD_ACCUMULATE). */
+ * The backward stores grad_vertices [B,Nv,3] (may be NULL; overwritten, with or without NR_GRAD_ACCUMULATE) and
+ * accumulates, per camera, grad_rot [.,9], grad_eye [.,3], grad_width [.] (each may be NULL; zero-filled first unless
+ * NR_GRAD_ACCUMULATE, which adds into them). */
 #define NR_CAM_PERSPECTIVE 0x100u
 #define NR_CAM_SHARED 0x200u
 NR_B200_API int nr_b200_camera_transform(const float *vertices, const float *rot, const float *eye, const float *width,

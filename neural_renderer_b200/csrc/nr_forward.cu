@@ -748,7 +748,9 @@ extern "C" int nr_b200_forward(const nr_b200_forward_args* a, void* cuda_stream)
     p.out_rgb = a->out_rgb; p.out_alpha = a->out_alpha; p.out_depth = a->out_depth;
     p.B = B; p.F = F; p.S = S; p.ts = ts; p.ngroups = (F + 31) / 32;
     p.big_area = S > 256 ? 4 * kBigArea : kBigArea;
-    p.flags = flags;
+    // the background only colours the RGB image: without NR_RETURN_RGB, background_batch is neither checked above nor
+    // read (it may be NULL), so the resolve pass must not see NR_BG_PER_BATCH either
+    p.flags = (flags & NR_RETURN_RGB) ? flags : (flags & ~NR_BG_PER_BATCH);
     p.near_lo = float_le(a->near_);
     p.far_cmp = fminf(float_ge(a->far_), (float)a->far_);
     p.far_val = (float)a->far_;

@@ -1,0 +1,278 @@
+"""Direct C-ABI harness for nr_b200_forward / nr_b200_backward (test infrastructure).
+
+It fills _lib.ForwardArgs / BackwardArgs itself -- no Python wrapper in between -- from a case of abi_cases.py, so that
+each case controls the exact flag word, which optional pointers are NULL, where every user buffer sits (fresh, or 4
+bytes into a slightly larger allocation; grad_textures also 8 bytes in: 2-float but not 4-float aligned) and what every
+output buffer holds before the call: NaN in each float output and a sentinel in face_index_map, so an element the
+kernels fail to write shows, or seeded values for NR_GRAD_ACCUMULATE.  Guard words around every buffer show a
+store just outside it.
+
+The alignment cases stay inside the ABI's promise (float alignment).  Every vector access of a user buffer in csrc/ is
+behind a host check on its address: the edge scan's side fill of grad_textures (16 bytes, else a memset), the staged
+strips of the edge scan (8 bytes on face_index_map, rgb_map, grad_rgb, grad_alpha), the TMA staging of texture cubes
+(16 bytes), and the v4 / v2 reductions of k_texture_grad / k_image_grad, which pick their width from the address."""
+import ctypes
+
+import numpy as np
+
+NEAR, FAR, EPS = 0.1, 100.0, 1e-4
+UNIFORM_BG = (0.1, 0.2, 0.3)
+FIM_SENTINEL = -7  # never a face index, never the -1 of an empty pixel
+RASTER = {"even": (64, 64), "odd": (57, 57), "aa": (66, 33)}  # raster S, API image H (anti-aliased: odd pooled size)
+F_FRONT = {False: 201, True: 101}  # front faces; fill_back appends the reversed copies: F = 201 or 202 (odd / even)
+UV_SIZES = [(17, 41), (32, 32), (9, 30), (1, 9), (24, 13)]
+MIP_SIZES = [(37, 29), (64, 48), (17, 41), (1, 9)]
+
+
+def _lib():
+    from neural_renderer_b200 import _lib as L
+    return L
+
+
+class Plan:
+    """shapes, flags and pointer layout of one case (pure host data: no device needed)"""
+
+    def __init__(self, c):
+        L = _lib()
+        self.case = c
+        self.kind = c["kind"]
+        self.B = 3 if c["batch"] == "B3" else 1
+        shared_flags = c["batch"] != "B1"  # B1: shared data at batch 1 without the flag bits; else the bits are set
+        self.fill_back = c["fill_back"]
+        self.F_front = F_FRONT[self.fill_back]
+        self.F = 2 * self.F_front if self.fill_back else self.F_front
+        self.S, self.H = RASTER[c["raster"]]
+        self.aa = c["raster"] == "aa"
+        self.rgb, self.alpha, self.depth = ("r" in c["outputs"]), ("a" in c["outputs"]), ("d" in c["outputs"])
+        self.indexed = c["geometry"] != "faces"
+        self.idx_shared = c["geometry"] in ("idx_shared", "idx_shared_oor")
+        from neural_renderer_b200 import synthetic
+        self.Nv = synthetic.sphere_mesh(self.F_front)[0].shape[0]
+        self.ts = c["ts"] or 0
+        self.uv = self.kind in ("uv", "mip")
+        self.mip = self.kind == "mip"
+        self.tex_shared = self.kind == "cube_shared" or (self.uv and c["image"] == "shared")
+        self.uv_shared = self.uv and c["uvs"] == "shared"
+        self.Ht = self.Wt = 0
+        if self.uv:
+            sizes = MIP_SIZES if self.mip else UV_SIZES
+            self.Ht, self.Wt = sizes[c["id"] % len(sizes)]
+        self.P = int(L.load().nr_b200_mip_texels(self.Ht, self.Wt)) if self.mip else 0
+        self.lit = bool(c["light"])
+        self.bg_batch = c["bg"] == "per_batch"
+        self.given = c["optional"] == "given"
+        f = 0
+        f |= L.NR_RETURN_RGB if self.rgb else 0
+        f |= L.NR_RETURN_ALPHA if self.alpha else 0
+        f |= L.NR_RETURN_DEPTH if self.depth else 0
+        f |= L.NR_ANTI_ALIASING if self.aa else 0
+        f |= L.NR_BG_PER_BATCH if self.bg_batch else 0
+        f |= L.NR_TEX_Z_BATCH0 if c["z_batch0"] else 0
+        f |= L.NR_TEX_FILL_BACK if self.fill_back else 0
+        f |= L.NR_FACES_INDEXED if self.indexed else 0
+        f |= L.NR_INDICES_SHARED if (self.idx_shared and shared_flags) else 0
+        f |= L.NR_TEX_SHARED if (self.tex_shared and shared_flags) else 0
+        f |= L.NR_TEX_UV if self.uv else 0
+        f |= L.NR_UV_SHARED if (self.uv_shared and shared_flags) else 0
+        f |= L.NR_TEX_MIPMAP if self.mip else 0
+        self.flags = f
+        up = c["upstream"]
+        self.g_rgb = self.rgb and up in ("all", "only_rgb")
+        self.g_alpha = self.alpha and up in ("all", "no_rgb")
+        self.g_depth = self.depth and up in ("all", "no_rgb")
+        self.n_cubes = self.F_front if self.fill_back else self.F
+        Bt = 1 if self.tex_shared else self.B
+        if self.kind in ("cube", "cube_shared"):
+            tex_shape = (Bt, self.n_cubes, self.ts, self.ts, self.ts, 3)
+        elif self.mip:
+            tex_shape = (Bt, self.P, 3)
+        elif self.uv:
+            tex_shape = (Bt, self.Ht, self.Wt, 3)
+        else:
+            tex_shape = None
+        B, F, S, H, Nv = self.B, self.F, self.S, self.H, self.Nv
+        f32, i32 = np.float32, np.int32
+        # name -> (shape, dtype) of every user buffer the case passes; a name that is missing is NULL
+        bufs = {}
+        if self.indexed:
+            bufs["vertices"] = ((B, Nv, 3), f32)
+            bufs["face_indices"] = (((F, 3) if self.idx_shared else (B, F, 3)), i32)
+            if self.given:  # ignored with NR_FACES_INDEXED: NaN faces in, grad_faces left as it was
+                bufs["faces"] = ((B, F, 3, 3), f32)
+        else:
+            bufs["faces"] = ((B, F, 3, 3), f32)
+        if self.rgb:
+            bufs["textures"] = (tex_shape, f32)
+            if self.lit:
+                bufs["face_light"] = ((B, F, 3), f32)
+            if self.uv:
+                nu = self.F_front if self.fill_back else F
+                bufs["face_uvs"] = (((nu, 3, 2) if self.uv_shared else (B, nu, 3, 2)), f32)
+        if self.bg_batch and (self.rgb or self.given):
+            bufs["background_batch"] = ((B, 3), f32)
+        bufs["face_index_map"] = ((B, S, S), i32)
+        bufs["weight_map"] = ((B, 3, S, S), f32)
+        bufs["depth_map"] = ((B, S, S), f32)
+        if self.rgb:
+            bufs["rgb_map"] = ((B, 3, S, S), f32)
+        if self.alpha and self.given:
+            bufs["alpha_map"] = ((B, S, S), f32)
+        if self.aa and self.given:
+            for k, want, shape in (("out_rgb", self.rgb, (B, 3, H, H)), ("out_alpha", self.alpha, (B, H, H)),
+                                   ("out_depth", self.depth, (B, H, H))):
+                if want:
+                    bufs[k] = (shape, f32)
+        if self.g_rgb:
+            bufs["grad_rgb"] = ((B, 3, H, H), f32)
+        if self.g_alpha:
+            bufs["grad_alpha"] = ((B, H, H), f32)
+        if self.g_depth:
+            bufs["grad_depth"] = ((B, H, H), f32)
+        if self.indexed:
+            bufs["grad_vertices"] = ((B, Nv, 3), f32)
+            if self.given:
+                bufs["grad_faces"] = ((B, F, 3, 3), f32)
+        else:
+            bufs["grad_faces"] = ((B, F, 3, 3), f32)
+        if self.rgb:
+            bufs["grad_textures"] = (tex_shape, f32)
+            if self.lit and self.given:
+                bufs["grad_face_light"] = ((B, F, 3), f32)
+        self.bufs = bufs
+        self.bwd_textures = self.rgb and (self.given or "grad_face_light" in bufs)  # textures may be NULL in the backward
+        p = c["pointers"]
+        self.offsets = {k: (0 if p == "fresh" else 4) for k in bufs}
+        if "grad_textures" in bufs and p == "off8":
+            self.offsets["grad_textures"] = 8
+        self.fwd_outputs = [k for k in ("face_index_map", "weight_map", "depth_map", "rgb_map", "alpha_map", "out_rgb",
+                                        "out_alpha", "out_depth") if k in bufs]
+        self.grad_outputs = [k for k in ("grad_faces", "grad_vertices", "grad_textures", "grad_face_light") if k in bufs]
+
+    # ---- the argument structs, from name -> address (int) of each buffer the case passes
+    def forward_args(self, ptr, workspace, workspace_bytes):
+        L = _lib()
+        a = L.ForwardArgs()
+        a.struct_size = ctypes.sizeof(L.ForwardArgs)
+        a.flags = self.flags
+        a.batch_size, a.num_faces, a.raster_size, a.texture_size = self.B, self.F, self.S, self.ts
+        a.near_, a.far_, a.eps = NEAR, FAR, EPS
+        a.background[0], a.background[1], a.background[2] = UNIFORM_BG
+        for k in ("faces", "textures", "background_batch", "face_index_map", "weight_map", "depth_map", "rgb_map",
+                  "alpha_map", "out_rgb", "out_alpha", "out_depth", "face_light", "vertices", "face_indices", "face_uvs"):
+            setattr(a, k, ptr.get(k))
+        a.num_vertices = self.Nv if self.indexed else 0
+        a.texture_height, a.texture_width = self.Ht, self.Wt
+        a.workspace, a.workspace_bytes = workspace, workspace_bytes
+        return a
+
+    def backward_args(self, ptr, flags, workspace, workspace_bytes):
+        L = _lib()
+        a = L.BackwardArgs()
+        a.struct_size = ctypes.sizeof(L.BackwardArgs)
+        a.flags = flags
+        a.batch_size, a.num_faces, a.raster_size, a.texture_size = self.B, self.F, self.S, self.ts
+        a.eps = EPS
+        for k in ("faces", "face_index_map", "weight_map", "depth_map", "rgb_map", "grad_rgb", "grad_alpha",
+                  "grad_depth", "grad_faces", "grad_textures", "face_light", "grad_face_light", "vertices",
+                  "face_indices", "grad_vertices", "face_uvs"):
+            setattr(a, k, ptr.get(k))
+        a.textures = ptr.get("textures") if self.bwd_textures else None
+        a.num_vertices = self.Nv if self.indexed else 0
+        a.texture_height, a.texture_width = self.Ht, self.Wt
+        a.workspace, a.workspace_bytes = workspace, workspace_bytes
+        return a
+
+    def backward_calls(self):
+        """[(flag word, accumulate?)] of the case's backward mode, in call order"""
+        L = _lib()
+        base = self.flags
+        acc = L.NR_GRAD_ACCUMULATE
+        tex, faces = L.NR_BWD_PART_TEXTURES, L.NR_BWD_PART_FACES
+        return {"one": [base], "tex_faces": [base | tex, base | faces], "faces_tex": [base | faces, base | tex],
+                "acc_one": [base | acc], "acc_halves": [base | acc | tex, base | acc | faces]}[self.case["backward"]]
+
+    @property
+    def accumulate(self):
+        return self.case["backward"].startswith("acc")
+
+    def fake_pointers(self):
+        """distinct non-NULL addresses with the case's offsets (host argument checks only: never dereferenced)"""
+        return {k: 0x10000000 * (i + 1) + self.offsets[k] for i, k in enumerate(sorted(self.bufs))}
+
+
+# ---- device side
+GUARD_WORDS = 4          # 16 bytes of guard before (keeps the data's 16-byte phase) and at least 16 after every buffer
+GUARD_BITS = 0x7FBADBAD  # a NaN payload no kernel stores (and no face index)
+
+
+def alloc(shape, dtype, offset_bytes, dev):
+    """a tensor of `shape` whose data starts `offset_bytes` past a 16-byte boundary inside a fresh allocation (the
+    allocator's blocks are 512-byte aligned), between guard words that guards_intact() checks after the calls: a store
+    just before or past a buffer -- a tail store of the side fill, an overrunning vector reduction -- fails the case.
+    The view keeps the allocation alive (it is t._base)."""
+    import torch
+    tdt = {np.float32: torch.float32, np.int32: torch.int32}[dtype]
+    n = int(np.prod(shape))
+    assert offset_bytes % 4 == 0 and offset_bytes < 16
+    lo = GUARD_WORDS + offset_bytes // 4
+    base = torch.empty(lo + n + GUARD_WORDS, dtype=tdt, device=dev)
+    base.view(torch.int32).fill_(GUARD_BITS)
+    assert base.data_ptr() % 16 == 0
+    t = base[lo:lo + n].view(shape)
+    assert t.data_ptr() % 16 == offset_bytes % 16
+    return t
+
+
+def guards_intact(t):
+    """whether the guard words around a buffer from alloc() still hold their pattern"""
+    import torch
+    base = t._base
+    lo = (t.data_ptr() - base.data_ptr()) // t.element_size()
+    bits = base.view(torch.int32)
+    return bool((bits[:lo] == GUARD_BITS).all()) and bool((bits[lo + t.numel():] == GUARD_BITS).all())
+
+
+def poison(t):
+    import torch
+    if t.dtype == torch.int32:
+        t.fill_(FIM_SENTINEL)
+    else:
+        t.fill_(float("nan"))
+
+
+def workspace(nbytes, dev):
+    import torch
+    ws = torch.empty((max(int(nbytes), 16),), dtype=torch.uint8, device=dev)
+    assert ws.data_ptr() % 16 == 0
+    return ws
+
+
+def forward(plan, buf, dev):
+    """poison the forward outputs, call nr_b200_forward on the current stream, return the return code"""
+    import torch
+    L = _lib()
+    lib = L.load()
+    for k in plan.fwd_outputs:
+        poison(buf[k])
+    nbytes = lib.nr_b200_forward_workspace_bytes(plan.B, plan.F, plan.S, plan.ts, plan.flags)
+    ws = workspace(nbytes, dev)
+    a = plan.forward_args({k: t.data_ptr() for k, t in buf.items()}, ws.data_ptr(), ws.numel())
+    rc = lib.nr_b200_forward(ctypes.byref(a), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+    torch.cuda.synchronize(dev)
+    return rc
+
+
+def backward(plan, buf, dev):
+    """the case's backward calls in order; [return codes].  The caller prepares the gradient buffers: poisoned, or
+    prefilled when the mode accumulates."""
+    import torch
+    L = _lib()
+    lib = L.load()
+    out = []
+    for flags in plan.backward_calls():
+        nbytes = lib.nr_b200_backward_workspace_bytes(plan.B, plan.F, plan.S, plan.ts, flags)
+        ws = workspace(nbytes, dev)
+        a = plan.backward_args({k: t.data_ptr() for k, t in buf.items()}, flags, ws.data_ptr(), ws.numel())
+        out.append(lib.nr_b200_backward(ctypes.byref(a), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+    torch.cuda.synchronize(dev)
+    return out

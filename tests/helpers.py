@@ -23,5 +23,22 @@ def rel_err(x, ref):
     return float(np.abs(x - ref).max() / den)
 
 
+def elem_err(x, ref, floor=1e-3):
+    """per-element gate: max over the elements of |x - ref| / max(|ref|, floor * max|ref|).  `elem_err(x, ref) <= tol`
+    holds every component to tol of its own size, and components below floor x the tensor maximum to tol x floor x
+    the maximum, so a wrong contribution to a small component cannot hide behind the largest one (rel_err can).  NaN
+    anywhere in x gives NaN, which fails every `<=` gate."""
+    x = np.asarray(x, np.float64)
+    ref = np.asarray(ref, np.float64)
+    if x.size == 0:
+        return 0.0
+    m = np.abs(ref).max()
+    if m == 0:
+        return float(np.abs(x).max()) if np.isfinite(x).all() else float("nan")
+    den = np.maximum(np.abs(ref), floor * m)
+    d = np.abs(x - ref) / den
+    return float("nan") if np.isnan(d).any() else float(d.max())
+
+
 def np_(t):
     return t.detach().cpu().numpy()

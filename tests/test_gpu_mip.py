@@ -3,7 +3,7 @@
 The pyramid build is checked against a float64 numpy restatement and the collapse as its adjoint; the forward and the
 image / light gradients against a float64 torch oracle of the documented sampler (include/nr_b200.h) that computes its
 level of detail from the faces, built on the product's own face_index_map / weight_map / depth_map like oracle_rgb of
-test_gpu_uv.py."""
+test_gpu_uv.py (both in oracles.py)."""
 import ctypes
 import os
 
@@ -12,6 +12,7 @@ import pytest
 import torch
 
 from helpers import np_, rel_err
+from oracles import oracle_trilinear, pyramid64
 from test_gpu_uv import CASES as UV_CASES
 
 pytestmark = pytest.mark.gpu
@@ -37,35 +38,6 @@ def _spread_uvs(shape, lo, hi, seed):
     centre = lo + (hi - lo) * torch.rand(shape[:-2] + (1, 2), generator=g, dtype=torch.float64)
     spread = 10.0 ** (-3 + 5 * torch.rand(shape[:-2] + (1, 1), generator=g, dtype=torch.float64))
     return (centre + spread * (torch.rand(shape, generator=g, dtype=torch.float64) - 0.5)).float().to(DEV)
-
-
-def _levels(H, W):
-    out = [(H, W)]
-    while out[-1] != (1, 1):
-        h, w = out[-1]
-        out.append((max(1, (h + 1) >> 1), max(1, (w + 1) >> 1)))
-    return out
-
-
-def pyramid64(image):
-    """float64 (numpy or torch, differentiable) restatement of the build: list of levels [Bt,H_l,W_l,3], row 0 = top."""
-    xp = torch if isinstance(image, torch.Tensor) else np
-    up = image[:, ::-1] if xp is np else image.flip(1)  # tap coordinates: y up from the bottom row
-    out = [up]
-    H, W = image.shape[1:3]
-    for h, w in _levels(H, W)[1:]:
-        Hs, Ws = out[-1].shape[1:3]
-        x0 = np.arange(w) * 2
-        x1 = np.minimum(x0 + 1, Ws - 1)
-        y0 = np.arange(h) * 2
-        y1 = np.minimum(y0 + 1, Hs - 1)
-        if xp is torch:
-            x0, x1, y0, y1 = (torch.as_tensor(a, device=image.device) for a in (x0, x1, y0, y1))
-        s = out[-1]
-        a, b = s[:, y0][:, :, x0], s[:, y0][:, :, x1]
-        c, d = s[:, y1][:, :, x0], s[:, y1][:, :, x1]
-        out.append(((a + b) + (c + d)) * 0.25)
-    return [t[:, ::-1] if xp is np else t.flip(1) for t in out]
 
 
 def _pack(levels):
@@ -119,88 +91,6 @@ def test_build_and_collapse(hw, Bt):
     acc = torch.ones_like(img)
     _collapse(G, H, W, out=acc, flags=_lib()[0].NR_GRAD_ACCUMULATE)
     assert rel_err(np_(acc), np_(_collapse(G, H, W) + 1)) <= 1e-6
-
-
-def _lod64(faces, fim, wmap, dmap, uvk, S, Ht, Wt, L):
-    """float64 level of detail of every raster pixel from the faces (inverse of the pixel-space vertex matrix)."""
-    B = faces.shape[0]
-    f64 = faces.double()
-    px = 0.5 * (f64[..., 0] * S + S - 1)
-    py = 0.5 * (f64[..., 1] * S + S - 1)
-    T = torch.stack((px, py, torch.ones_like(px)), dim=-2)           # [B,F,3,3] columns = vertices
-    M = torch.linalg.inv_ex(T).inverse                                # rows k: d a_k / dx, d a_k / dy, constant
-    fi = fim.clamp(min=0).long()
-    bidx = torch.arange(B, device=DEV)[:, None, None].expand_as(fi)
-    Mp = M[bidx, fi]                                                  # [B,S,S,3,3]
-    z = f64[..., 2][bidx, fi]                                         # [B,S,S,3]
-    w = wmap.double().permute(0, 2, 3, 1)
-    zp = dmap.double()[..., None]
-    lam = w * (zp / z)
-    out = []
-    for d in (0, 1):
-        q = Mp[..., d] / z
-        dl = zp * (q - lam * q.sum(-1, keepdim=True))                 # [B,S,S,3]
-        du = (uvk[..., 0] * dl).sum(-1) * (Wt - 1)
-        dv = (uvk[..., 1] * dl).sum(-1) * (Ht - 1)
-        out.append(du * du + dv * dv)
-    lod = 0.5 * torch.log2(torch.maximum(*out))
-    return torch.nan_to_num(lod, nan=0.0, neginf=0.0).clamp(0, L - 1)
-
-
-def oracle_trilinear(faces, fim, wmap, dmap, uvs, image, light, bg, fill_back, aa):
-    """float64 trilinear sample on the product's maps; image [1|B,Ht,Wt,3] (differentiable through the float64 pyramid),
-    light [B,F,3] or None.  Returns (API rgb [B,3,H,W], raster LOD [B,S,S], L)."""
-    B = faces.shape[0]
-    S = fim.shape[-1]
-    uvs = uvs.double().expand(B, -1, -1, -1)
-    if fill_back:
-        uvs = torch.cat((uvs, uvs.flip(2)), dim=1)
-    Ht, Wt = image.shape[1:3]
-    levels = [l.expand(B, -1, -1, -1) for l in pyramid64(image.double())]
-    L = len(levels)
-    cov = fim >= 0
-    fi = fim.clamp(min=0).long()
-    bidx = torch.arange(B, device=DEV)[:, None, None].expand(B, S, S)
-    z = faces.double()[..., 2][bidx, fi]
-    w = wmap.double().permute(0, 2, 3, 1)
-    zp = dmap.double()[..., None]
-    uvk = uvs[bidx, fi]                                                # [B,S,S,3,2]
-    # the pixel's uv and texel positions in fp32 with the sampler's pinned operation order (include/nr_b200.h): at 1024
-    # texels one ulp of u is 6e-5 texel, which would otherwise dominate the comparison of the large images
-    lam32 = w.float() * (zp.float() / z.float())
-    u32 = uvk.float()
-    uv = (lam32[..., 0, None] * u32[..., 0, :] + lam32[..., 1, None] * u32[..., 1, :]) + lam32[..., 2, None] * u32[..., 2, :]
-    uv = torch.nan_to_num(uv.clamp(0, 1))
-    lod = _lod64(faces, fim, wmap, dmap, uvk, S, Ht, Wt, L)
-    lt = light.double()[bidx, fi] if light is not None else None
-
-    def bilinear(img):
-        h, wd = img.shape[1:3]
-        px, py = (uv[..., 0] * (wd - 1)).double(), (uv[..., 1] * (h - 1)).double()  # fp32 positions, as pinned
-        ix, iy = px.floor().long().clamp(max=wd - 1), py.floor().long().clamp(max=h - 1)
-        wx1, wy1 = px - ix, py - iy
-        wx0, wy0 = 1 - wx1, 1 - wy1
-        x1, y1 = (ix + 1).clamp(max=wd - 1), (iy + 1).clamp(max=h - 1)
-        r0, r1 = h - 1 - iy, h - 1 - y1
-
-        def tap(r, c):
-            t = img[bidx, r, c]
-            return t * lt if lt is not None else t
-        return ((wx0 * wy0)[..., None] * tap(r0, ix) + (wx0 * wy1)[..., None] * tap(r1, ix)
-                + (wx1 * wy0)[..., None] * tap(r0, x1) + (wx1 * wy1)[..., None] * tap(r1, x1))
-
-    samples = torch.stack([bilinear(l) for l in levels], dim=0)      # [L,B,S,S,3]
-    l0 = lod.floor()
-    f = (lod - l0)[..., None]
-    l0 = l0.long()
-    l1 = (l0 + 1).clamp(max=L - 1)
-    pick = lambda l: samples.gather(0, l[None, ..., None].expand(1, B, S, S, 3))[0]
-    rgb = (1 - f) * pick(l0) + f * pick(l1)
-    bgt = torch.as_tensor(bg, dtype=torch.float64, device=DEV)
-    rgb = torch.where(cov[..., None], rgb, bgt).permute(0, 3, 1, 2)
-    if aa:
-        rgb = torch.nn.functional.avg_pool2d(rgb, 2, 2)
-    return rgb, torch.where(cov, lod, torch.full_like(lod, -1.0)), L
 
 
 def _render(faces, image, uvs, H, aa, light=None, fill_back=False, bg=(0.1, 0.2, 0.3), texture_filter="trilinear"):

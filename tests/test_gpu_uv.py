@@ -1,8 +1,11 @@
 """GPU: the texture-image mode (face_uvs + texture image, NR_TEX_UV).
 
 The forward and the image / light gradients are checked against an op-by-op float64 torch oracle of the documented
-sampler (include/nr_b200.h), built on the product's own face_index_map / weight_map / depth_map; coverage against the
-cube mode; the vertex gradient against the reference's own K5 (oracle/refhost.py) fed with the UV-mode rgb map."""
+sampler (include/nr_b200.h; oracles.oracle_rgb), built on the product's own face_index_map / weight_map / depth_map;
+coverage against the cube mode; the vertex gradient against the reference's own K5 (oracle/refhost.py) fed with the
+UV-mode rgb map.  The oracle forms the pixel's uv and texel positions in fp32 in the sampler's pinned operation order
+(the header specifies fp32 there) and everything after that in float64: less independent of the kernel than a float64
+uv, but one fp32 ulp of u would otherwise dominate the comparison."""
 import os
 
 import numpy as np
@@ -10,6 +13,7 @@ import pytest
 import torch
 
 from helpers import np_, rel_err
+from oracles import oracle_rgb
 
 pytestmark = pytest.mark.gpu
 
@@ -30,47 +34,6 @@ def _case(B=2, F=200, seed=0):
 def _uvs(shape, lo=0.0, hi=1.0, seed=1):
     g = torch.Generator().manual_seed(seed)
     return (lo + (hi - lo) * torch.rand(shape, generator=g, dtype=torch.float32)).to(DEV)
-
-
-def oracle_rgb(faces, fim, wmap, dmap, uvs, image, light, bg, fill_back, aa):
-    """float64 torch restatement of the UV sampler on the product's maps.  faces [B,F,3,3]; uvs [1|B,F',3,2];
-    image [1|B,Ht,Wt,3] (differentiable); light [B,F,3] or None (differentiable); returns the API rgb [B,3,H,W]."""
-    B, F = faces.shape[:2]
-    S = fim.shape[-1]
-    uvs = uvs.double().expand(B, -1, -1, -1)
-    if fill_back:
-        uvs = torch.cat((uvs, uvs.flip(2)), dim=1)
-    img = image.double().expand(B, -1, -1, -1)
-    Ht, Wt = img.shape[1:3]
-    cov = fim >= 0
-    fi = fim.clamp(min=0).long()                                       # [B,S,S]
-    bidx = torch.arange(B, device=DEV)[:, None, None].expand(B, S, S)
-    z = faces.double()[..., 2][bidx, fi]                               # [B,S,S,3] winner's own vertex depths
-    w = wmap.double().permute(0, 2, 3, 1)
-    zp = dmap.double()[..., None]
-    lam = w * (zp / z)
-    uvk = uvs[bidx, fi]                                                # [B,S,S,3,2]
-    uv = (lam[..., None] * uvk).sum(-2)
-    uv = torch.nan_to_num(uv.clamp(0, 1))
-    px, py = uv[..., 0] * (Wt - 1), uv[..., 1] * (Ht - 1)
-    ix, iy = px.floor().long().clamp(max=Wt - 1), py.floor().long().clamp(max=Ht - 1)
-    wx1, wy1 = px - ix, py - iy
-    wx0, wy0 = 1 - wx1, 1 - wy1
-    x1, y1 = (ix + 1).clamp(max=Wt - 1), (iy + 1).clamp(max=Ht - 1)
-    r0, r1 = Ht - 1 - iy, Ht - 1 - y1
-
-    def tap(r, c):
-        t = img[bidx, r, c]                                            # [B,S,S,3]
-        if light is not None:
-            t = t * light.double()[bidx, fi]
-        return t
-    rgb = ((wx0 * wy0)[..., None] * tap(r0, ix) + (wx0 * wy1)[..., None] * tap(r1, ix)
-           + (wx1 * wy0)[..., None] * tap(r0, x1) + (wx1 * wy1)[..., None] * tap(r1, x1))
-    bgt = torch.as_tensor(bg, dtype=torch.float64, device=DEV)
-    rgb = torch.where(cov[..., None], rgb, bgt).permute(0, 3, 1, 2)
-    if aa:
-        rgb = torch.nn.functional.avg_pool2d(rgb, 2, 2)
-    return rgb
 
 
 def _render(faces, image, uvs, S, aa, light=None, fill_back=False, reference_exact=None, bg=(0.1, 0.2, 0.3)):
