@@ -95,14 +95,26 @@ extern "C" {
  *   1 - frac; fp32, round-to-nearest; clamp to edge only (no wrap; NR_TEX_MIPMAP below samples a mip pyramid
  *   trilinearly instead).  face_light multiplies every tap first.
  *   With NR_TEX_FILL_BACK face f >= F/2 uses the UV corners of face f - F/2 in reverse order (`face_uvs` holds F/2 faces).
- *   The backward fills grad_textures (the image gradient) and grad_face_light; there is NO gradient for face_uvs. */
+ *   The backward fills grad_textures (the image gradient), grad_face_light and, when given, grad_face_uvs:
+ *   d loss / d face_uvs (nr_b200_backward_args.grad_face_uvs).  For a covered raster pixel with the winner's UV corners
+ *   uv_k (reversed for a fill_back copy, as above), l_k as above, fp32 uv = (u, v) and upstream rgb gradient g_c (the
+ *   pooled gradient / 4 with NR_ANTI_ALIASING): per sampled level l with weight a_l (bilinear: level 0, a = 1; NR_TEX_MIPMAP:
+ *   l0 with 1 - f and, only when f != 0, l1 with f) and the taps T_xy of that level's addressing (tap (x, y), y up, so T_01
+ *   is image row r1), each times face_light:
+ *     Dx_c = (W_l - 1) (wy0 (T10 - T00) + wy1 (T11 - T01)),   Dy_c = (H_l - 1) (wx0 (T01 - T00) + wx1 (T11 - T10)),
+ *     gu = [0 <= u <= 1] sum_l a_l sum_c g_c Dx_c,   gv = [0 <= v <= 1] sum_l a_l sum_c g_c Dy_c   (NaN u / v: 0),
+ *     grad_face_uvs[corner k] += (l_k gu, l_k gv)
+ *   (a fill_back copy f >= F/2 adds into face f - F/2, its corner k being that face's corner 2 - k; with NR_UV_SHARED the
+ *   sum over the items).  This is the derivative of the bilinear sample within the cell the forward picked: the level of
+ *   detail, l_k and the clamp are held fixed, a 1-texel axis gets 0.  fp32, not bit-pinned (unordered atomics). */
 #define NR_TEX_UV 0x20000u    /* sample a texture image through per-corner UVs (fields face_uvs / texture_height / _width) */
 #define NR_UV_SHARED 0x40000u /* face_uvs is [F,3,2] and serves every batch item (else [B,F,3,2])                        */
 
 /* Trilinear sampling through a mip pyramid (additive to ABI 4: a flag bit and three entry points, no struct field).
  *   Only together with NR_TEX_UV.  `textures` is then the PACKED PYRAMID [Bt,P,3]: level 0 (the image, Ht x Wt), then
  *   level 1, 2, ... in order, each HWC with row 0 = top; `grad_textures` is the gradient of that pyramid (collapse it into
- *   the image with nr_b200_mip_collapse).  texture_height / texture_width stay the level-0 size.
+ *   the image with nr_b200_mip_collapse); grad_face_uvs is the face_uvs gradient (NR_TEX_UV above, through both
+ *   levels).  texture_height / texture_width stay the level-0 size.
  *   Level sizes: H_{l+1} = max(1, (H_l + 1) >> 1), the same for W, until both are 1: L = 1 + ceil(log2(max(Ht, Wt)))
  *   levels, P = sum_l H_l W_l texels (nr_b200_mip_texels).  A 1x1 image has one level (trilinear = bilinear).
  *   Building (nr_b200_mip_build), in tap coordinates (x right, y up from the bottom row, row r = H_l-1-y): texel (x, y)
@@ -118,7 +130,7 @@ extern "C" {
  *   Sample: l0 = floor(lod), l1 = min(l0+1, L-1), f = lod - l0; rgb = (1-f) bilinear_l0 + f bilinear_l1, each level with
  *   the NR_TEX_UV addressing at its own size; face_light multiplies every tap first; level l1 is not read when f == 0.
  *   The backward sends (1-f or f) * tap weight * light * grad_rgb to each tap of the pyramid and grad_face_light gets the
- *   unlit trilinear sample times the upstream gradient.  NO gradient flows through the LOD or into face_uvs. */
+ *   unlit trilinear sample times the upstream gradient.  NO gradient flows through the LOD. */
 #define NR_TEX_MIPMAP 0x80000u /* textures = packed mip pyramid of the image, sampled trilinearly (needs NR_TEX_UV)        */
 
 typedef struct nr_b200_forward_args {
@@ -166,7 +178,8 @@ typedef struct nr_b200_forward_args {
 } nr_b200_forward_args;
 
 typedef struct nr_b200_backward_args {
-    uint32_t struct_size;
+    uint32_t struct_size; /* sizeof(nr_b200_backward_args), or offsetof(nr_b200_backward_args, grad_face_uvs): the ABI-4
+                             layout before that field, which then reads as NULL.  Only struct_size bytes are read. */
     uint32_t flags; /* same flag set as the forward call that produced the maps */
     int32_t batch_size, num_faces, raster_size, texture_size;
     double eps; /* edge-distance epsilon (rasterize.py:650) and texture clamp epsilon -- the reference uses one value */
@@ -201,6 +214,10 @@ typedef struct nr_b200_backward_args {
     const float *face_uvs;
     int32_t texture_height;
     int32_t texture_width;
+    /* ABI 4, appended: d loss / d face_uvs [B,F',3,2], or [F',3,2] with NR_UV_SHARED (F' = F/2 with NR_TEX_FILL_BACK), or
+     * NULL = not wanted.  Needs NR_TEX_UV, NR_RETURN_RGB and `textures`.  Part of the texture half
+     * (NR_BWD_PART_TEXTURES): zero-filled first unless NR_GRAD_ACCUMULATE; stays zero without grad_rgb. */
+    float *grad_face_uvs;
 } nr_b200_backward_args;
 
 /* ABI version of the loaded library (== NR_B200_ABI_VERSION it was built with). */

@@ -93,6 +93,7 @@ class BackwardArgs(ctypes.Structure):
         ("vertices", ctypes.c_void_p), ("face_indices", ctypes.c_void_p), ("grad_vertices", ctypes.c_void_p),
         ("num_vertices", ctypes.c_int32), ("_pad1", ctypes.c_int32),
         ("face_uvs", ctypes.c_void_p), ("texture_height", ctypes.c_int32), ("texture_width", ctypes.c_int32),
+        ("grad_face_uvs", ctypes.c_void_p),  # appended within ABI 4; struct_size = BackwardArgs.grad_face_uvs.offset omits it
     ]
 
 

@@ -37,6 +37,7 @@
 #include <math.h>
 #include <stdint.h>
 #include <stdlib.h>
+#include <string.h>
 
 #include <type_traits>
 
@@ -74,6 +75,12 @@
 #endif
 #ifndef NR_IGM_MIN_CTAS
 #define NR_IGM_MIN_CTAS 3       // k_image_grad_mip (trilinear): chosen with -Xptxas -v, see DESIGN.md section 4c
+#endif
+#ifndef NR_IGU_MIN_CTAS
+#define NR_IGU_MIN_CTAS 4       // k_image_grad with the face_uvs gradient: 56 registers, no spills (DESIGN.md section 4c)
+#endif
+#ifndef NR_IGMU_MIN_CTAS
+#define NR_IGMU_MIN_CTAS 3      // k_image_grad_mip with the face_uvs gradient: 79 registers, no spills
 #endif
 
 namespace {
@@ -131,6 +138,8 @@ struct BwdParams {
     int Ht, Wt;
     // NR_TEX_MIPMAP (appended likewise): textures / grad_textures = the packed pyramid [Bt,P,3]
     nr::MipTable mip;
+    // d loss / d face_uvs (appended likewise): the layout of `uvs` (uv_bstride floats per item), or nullptr
+    float* grad_uvs;
 };
 
 //@phase helpers: rcp / vector RED / load_grad (inlined)
@@ -1076,7 +1085,13 @@ __device__ __forceinline__ void red_add_6(float* t, const float v[6]) {
 // the K1 inverse of the same pixel-space vertices (face_inverse(to_pixel(...)), as k_depth_grad) and the saved weight /
 // depth maps, so the taps and level weights are the forward's.  Up to four 6-float pairs (two rows on each of the two
 // levels) go to the packed pyramid; lanes merge only when they hit the same cells on both levels.
-template <int kTgCombine, bool kMip>
+//
+// kUvGrad (grad_face_uvs given): the same pass also sends d loss / d face_uvs.  Per sampled level, nr::uv_blend_grad reads
+// the four unlit taps once and returns d sample / d (u, v) per channel together with the unlit blend (which the light
+// gradient then takes instead of reading the taps again); gu = sum_l a_l sum_c g_c light_c du_c (v alike, a_l = the level
+// weight) goes to UV corner k as l_k (gu, gv), corners reversed back for a fill_back copy.  Runs of neighbouring lanes
+// that show the same face sum their 6 floats with shuffles and the run's first lane adds them.
+template <int kTgCombine, bool kMip, bool kUvGrad>
 __device__ __forceinline__ void image_grad(const BwdParams& p) {
     constexpr int kPairs = kMip ? 4 : 2;
     const int S = p.S;
@@ -1093,6 +1108,8 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
     bool adjacent[kPairs / 2];                 // x1 == x0 + 1 (else both taps of a row are the same texel, weight 0 on x1)
     long long key = -1 - (long long)lane;      // (image, cell): equal keys <=> the same four texels
     long long key1 = -1;                       // kMip: the cell on level l1 (-1 when f == 0)
+    float uvg[6] = {0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f};  // kUvGrad: d loss / d face_uvs, corners of the stored face
+    uint32_t uv_at = 0;                        // kUvGrad: offset of the face's corners in face_uvs / grad_face_uvs
 #pragma unroll
     for (int r = 0; r < kPairs; r++) {
         tp[r] = nullptr;
@@ -1148,7 +1165,39 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
             nlev = m.f != 0.0f ? 2 : 1;
         }
         const nr::UvTaps t0 = nr::uv_taps(u, v, kMip ? p.mip.h[lv[0]] : p.Ht, kMip ? p.mip.w[lv[0]] : p.Wt);
-        if (want_light) {  // unlit sample (same blend as the forward pass) times the upstream gradient
+        if constexpr (kUvGrad) {
+            float lt[3] = {1.0f, 1.0f, 1.0f};
+            if (p.face_light) {
+                const float* lp = p.face_light + ((size_t)b * p.F + fn) * 3;
+                lt[0] = __ldg(lp); lt[1] = __ldg(lp + 1); lt[2] = __ldg(lp + 2);
+            }
+            const float h[3] = {g0 * lt[0], g1 * lt[1], g2 * lt[2]};  // d loss / d unlit tap value, per unit weight
+            float c[3], gu = 0.0f, gv = 0.0f;
+#pragma unroll
+            for (int q = 0; q < 2; q++) {
+                if (q >= nlev) break;
+                const int Hl = kMip ? p.mip.h[lv[q]] : p.Ht, Wl = kMip ? p.mip.w[lv[q]] : p.Wt;
+                const nr::UvTaps t = q == 0 ? t0 : nr::uv_taps(u, v, Hl, Wl);
+                float bl[3], du[3], dv[3];
+                nr::uv_blend_grad(p.textures + img_off + (kMip ? p.mip.off[lv[q]] : 0u), Hl, Wl, t, bl, du, dv);
+#pragma unroll
+                for (int k = 0; k < 3; k++) c[k] = q == 0 ? bl[k] : __fmaf_rn(lw[1], bl[k], __fmul_rn(lw[0], c[k]));  // mip_blend
+                const float eu = __fmaf_rn(h[2], du[2], __fmaf_rn(h[1], du[1], __fmul_rn(h[0], du[0])));
+                const float ev = __fmaf_rn(h[2], dv[2], __fmaf_rn(h[1], dv[1], __fmul_rn(h[0], dv[0])));
+                gu = __fmaf_rn(lw[q], eu, gu);
+                gv = __fmaf_rn(lw[q], ev, gv);
+            }
+            if (want_light) { gl0 = c[0] * g0; gl1 = c[1] * g1; gl2 = c[2] * g2; }
+            // uv = sum_k l_k uv_k (pixel_uv); a fill_back copy's corner k is corner 2 - k of the stored face
+            const float l0 = __fmul_rn(w[0], __fdiv_rn(zp, z0)), l1 = __fmul_rn(w[1], __fdiv_rn(zp, z1)),
+                        l2 = __fmul_rn(w[2], __fdiv_rn(zp, z2));
+            const float s0 = rev ? l2 : l0, s2 = rev ? l0 : l2;  // l of the stored face's corners 0 and 2
+            uvg[0] = __fmul_rn(s0, gu); uvg[1] = __fmul_rn(s0, gv);
+            uvg[2] = __fmul_rn(l1, gu); uvg[3] = __fmul_rn(l1, gv);
+            uvg[4] = __fmul_rn(s2, gu); uvg[5] = __fmul_rn(s2, gv);
+            uv_at = (uint32_t)b * p.uv_bstride + (uint32_t)uf * 6u;
+        }
+        if (!kUvGrad && want_light) {  // unlit sample (same blend as the forward pass) times the upstream gradient
             float c[3];
             if constexpr (kMip) {
                 nr::MipLevels m;
@@ -1227,6 +1276,24 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
             }
         }
     }
+    if constexpr (kUvGrad) {
+        // warp-aggregated scatter of d loss / d face_uvs: runs of neighbouring lanes that show the same face (the same fn
+        // is the same UV face with the same corner order)
+        const int fn_prev = __shfl_up_sync(0xffffffffu, fn, 1);
+        const uint32_t heads = __ballot_sync(0xffffffffu, lane == 0 || fn != fn_prev);
+        const uint32_t later = heads & ~((2u << lane) - 1u);
+        const int run_end = (lane == 31 || later == 0) ? 31 : (__ffs(later) - 2);
+#pragma unroll
+        for (int off = 1; off < 32; off <<= 1) {
+            const bool take = lane + off <= run_end;
+#pragma unroll
+            for (int k = 0; k < 6; k++) {
+                const float x = __shfl_down_sync(0xffffffffu, uvg[k], off);
+                if (take) uvg[k] += x;
+            }
+        }
+        if (fn >= 0 && ((heads >> lane) & 1u)) red_add_6(p.grad_uvs + uv_at, uvg);
+    }
     if (!want_light) return;
     // warp-aggregated scatter of the light gradient: runs of neighbouring lanes that show the same face
     const int fn_prev = __shfl_up_sync(0xffffffffu, fn, 1);
@@ -1246,13 +1313,13 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
     }
 }
 
-template <int kTgCombine>
-__global__ void __launch_bounds__(256, NR_IG_MIN_CTAS) k_image_grad(const __grid_constant__ BwdParams p) {
-    image_grad<kTgCombine, false>(p);
+template <int kTgCombine, bool kUvGrad>
+__global__ void __launch_bounds__(256, kUvGrad ? NR_IGU_MIN_CTAS : NR_IG_MIN_CTAS) k_image_grad(const __grid_constant__ BwdParams p) {
+    image_grad<kTgCombine, false, kUvGrad>(p);
 }
-template <int kTgCombine>
-__global__ void __launch_bounds__(256, NR_IGM_MIN_CTAS) k_image_grad_mip(const __grid_constant__ BwdParams p) {
-    image_grad<kTgCombine, true>(p);
+template <int kTgCombine, bool kUvGrad>
+__global__ void __launch_bounds__(256, kUvGrad ? NR_IGMU_MIN_CTAS : NR_IGM_MIN_CTAS) k_image_grad_mip(const __grid_constant__ BwdParams p) {
+    image_grad<kTgCombine, true, kUvGrad>(p);
 }
 
 // ----------------------------------------------------------------------------------------------- k_depth_grad
@@ -1407,9 +1474,17 @@ extern "C" size_t nr_b200_backward_workspace_bytes(int32_t B, int32_t F, int32_t
     return bin_layout(B, F, S, strip_rec_bytes(S, both)).total;
 }
 
-extern "C" int nr_b200_backward(const nr_b200_backward_args* a, void* cuda_stream) {
+extern "C" int nr_b200_backward(const nr_b200_backward_args* args, void* cuda_stream) {
     nr_internal::launch_count() = 0;
-    if (!a || a->struct_size != sizeof(nr_b200_backward_args)) return NR_ERR_INVALID_ARG;
+    // Two layouts: the full struct, and the ABI-4 struct from before grad_face_uvs (which then reads as NULL).  Only the
+    // caller's struct_size bytes are read.
+    if (!args) return NR_ERR_INVALID_ARG;
+    const uint32_t size = args->struct_size;
+    if (size != sizeof(nr_b200_backward_args) && size != offsetof(nr_b200_backward_args, grad_face_uvs)) return NR_ERR_INVALID_ARG;
+    nr_b200_backward_args args_copy;
+    memset(&args_copy, 0, sizeof(args_copy));
+    memcpy(&args_copy, args, size);
+    const nr_b200_backward_args* a = &args_copy;
     const int B = a->batch_size, F = a->num_faces, S = a->raster_size, ts = a->texture_size;
     const uint32_t flags = a->flags;
     if (B <= 0 || F <= 0 || S <= 0) return NR_ERR_INVALID_ARG;
@@ -1428,6 +1503,10 @@ extern "C" int nr_b200_backward(const nr_b200_backward_args* a, void* cuda_strea
     if (uv && (!rgb || !a->face_uvs || a->texture_height < 1 || a->texture_width < 1)) return NR_ERR_INVALID_ARG;
     const bool mip = (flags & NR_TEX_MIPMAP) != 0;
     if (mip && !uv) return NR_ERR_INVALID_ARG;
+    // d loss / d face_uvs: only for the texture-image sampler, and it reads the image (pyramid).  It has the layout of
+    // face_uvs, so the 32-bit UV offset check below covers it.
+    const bool uv_grad = a->grad_face_uvs != nullptr;
+    if (uv_grad && (!uv || !rgb || !a->textures)) return NR_ERR_INVALID_ARG;
     if (rgb && (!a->rgb_map || (!uv && ts < 2))) return NR_ERR_INVALID_ARG;
     if (rgb && part_tex && !a->grad_textures) return NR_ERR_INVALID_ARG;
     if (rgb && (flags & NR_TEX_FILL_BACK) && (F & 1)) return NR_ERR_INVALID_ARG;
@@ -1443,7 +1522,8 @@ extern "C" int nr_b200_backward(const nr_b200_backward_args* a, void* cuda_strea
     const size_t img_floats = mip ? nr::mip_table(a->texture_height, a->texture_width, &mt) * 3
                                   : (uv ? (size_t)a->texture_height * (size_t)a->texture_width * 3 : 0);
     const size_t uv_floats = ncubes * 6;
-    if (uv && (tex_items * img_floats > 0x7FFFFFFFull || uv_floats * ((flags & NR_UV_SHARED) ? 1 : (size_t)B) > 0x7FFFFFFFull))
+    const size_t uv_items = (flags & NR_UV_SHARED) ? 1 : (size_t)B;
+    if (uv && (tex_items * img_floats > 0x7FFFFFFFull || uv_floats * uv_items > 0x7FFFFFFFull))
         return NR_ERR_UNSUPPORTED;  // 32-bit image / UV offsets in the kernels
     const size_t need = nr_b200_backward_workspace_bytes(B, F, S, ts, flags);
     if (!a->workspace || a->workspace_bytes < need || ((uintptr_t)a->workspace & 15)) return NR_ERR_WORKSPACE;
@@ -1471,6 +1551,8 @@ extern "C" int nr_b200_backward(const nr_b200_backward_args* a, void* cuda_strea
             return NR_ERR_CUDA;
         if (part_tex && rgb && a->grad_face_light && cudaMemsetAsync(a->grad_face_light, 0, (size_t)B * F * 3 * sizeof(float), stream) != cudaSuccess)
             return NR_ERR_CUDA;
+        if (part_tex && uv_grad && cudaMemsetAsync(a->grad_face_uvs, 0, uv_items * uv_floats * sizeof(float), stream) != cudaSuccess)
+            return NR_ERR_CUDA;
         nr_internal::prof_end(stream);
     }
 
@@ -1494,18 +1576,21 @@ extern "C" int nr_b200_backward(const nr_b200_backward_args* a, void* cuda_strea
         p.img_bstride = (flags & NR_TEX_SHARED) ? 0u : (uint32_t)img_floats;
         p.Ht = a->texture_height; p.Wt = a->texture_width;
         if (mip) p.mip = mt;
+        p.grad_uvs = a->grad_face_uvs;
     }
 
     const dim3 pgrid((unsigned)(((size_t)S * S + 255) / 256), B);
     auto launch_texture_grad = [&]() {
         if (mip) {
             nr_internal::LaunchScope ls("k_image_grad", stream);
-            k_image_grad_mip<NR_TG_COMBINE><<<pgrid, 256, 0, stream>>>(p);
+            if (uv_grad) k_image_grad_mip<NR_TG_COMBINE, true><<<pgrid, 256, 0, stream>>>(p);
+            else k_image_grad_mip<NR_TG_COMBINE, false><<<pgrid, 256, 0, stream>>>(p);
             return;
         }
         if (uv) {
             nr_internal::LaunchScope ls("k_image_grad", stream);
-            k_image_grad<NR_TG_COMBINE><<<pgrid, 256, 0, stream>>>(p);
+            if (uv_grad) k_image_grad<NR_TG_COMBINE, true><<<pgrid, 256, 0, stream>>>(p);
+            else k_image_grad<NR_TG_COMBINE, false><<<pgrid, 256, 0, stream>>>(p);
             return;
         }
         nr_internal::LaunchScope ls("k_texture_grad", stream);

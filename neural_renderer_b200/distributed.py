@@ -5,7 +5,9 @@ dimension, so one process per GPU renders its own contiguous slice and no data-p
 (`shard_range`).  The only exchange the path ever has is the gradient of a mesh SHARED by all viewpoints
 (`Mesh.get_batch` broadcasts one mesh, mesh.py:29-34 of the reference): each rank reduces its own views locally
 (autograd sums over the expanded batch axis) and the per-rank sums of `vertices.grad` / `textures.grad` are combined
-with one sum-all-reduce each (`allreduce_shared_grads`; NCCL over NVLink on GPUs, gloo in the CPU tests).
+with one sum-all-reduce each (`allreduce_shared_grads`; NCCL over NVLink on GPUs, gloo in the CPU tests).  A shared
+learnable texture image and its `face_uvs` ([F,3,2]: the rasterizer sums its gradient over the rank's items) are
+combined the same way: pass them to `allreduce_shared_grads` with the vertices.
 """
 from __future__ import annotations
 

@@ -273,9 +273,11 @@ class _RasterizeFunction(torch.autograd.Function):
         ctx.F = F
         ctx.tex_shape = tuple(textures.shape) if textures is not None else None
         ctx.tex_hw = tex_hw
-        # the unlit textures are only needed again for d loss / d face_light
+        # the unlit textures are only needed again for d loss / d face_light and d loss / d face_uvs
         need_light_grad = light_c is not None and ctx.needs_input_grad[2]
-        ctx.save_for_backward(geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c if need_light_grad else None, indices, uv_c)
+        ctx.need_uv_grad = uv_c is not None and want_rgb and ctx.needs_input_grad[5]
+        need_tex = need_light_grad or ctx.need_uv_grad
+        ctx.save_for_backward(geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c if need_tex else None, indices, uv_c)
         if cfg.aa:
             rgb_o, alpha_o, depth_o = out_rgb, out_alpha, out_depth
         else:
@@ -304,7 +306,8 @@ class _RasterizeFunction(torch.autograd.Function):
         with torch.cuda.device(dev):
             grad_geom = torch.empty_like(geom_c)  # grad_faces [B,F,3,3], or grad_vertices [B,Nv,3] when indexed
             grad_textures = torch.empty(ctx.tex_shape, dtype=torch.float32, device=dev) if want_rgb else None
-            grad_light = torch.empty_like(light_c) if (want_rgb and tex_c is not None) else None
+            grad_light = torch.empty_like(light_c) if (want_rgb and light_c is not None and ctx.needs_input_grad[2]) else None
+            grad_uvs = torch.empty_like(uv_c) if ctx.need_uv_grad else None  # same layout as face_uvs: [1|B,F',3,2]
             ws_bytes = lib.nr_b200_backward_workspace_bytes(B, F, cfg.S, ctx.ts, flags)
             ws = torch.empty((max(ws_bytes, 16),), dtype=torch.uint8, device=dev)
             a = _lib.BackwardArgs()
@@ -322,6 +325,7 @@ class _RasterizeFunction(torch.autograd.Function):
             a.face_index_map, a.weight_map, a.depth_map, a.rgb_map = _ptr(fim), _ptr(wmap), _ptr(dmap), _ptr(rgb_map)
             a.grad_rgb, a.grad_alpha, a.grad_depth = _ptr(g_rgb), _ptr(g_alpha), _ptr(g_depth)
             a.grad_textures = _ptr(grad_textures)
+            a.grad_face_uvs = _ptr(grad_uvs)  # filled by the texture half
             a.workspace, a.workspace_bytes = _ptr(ws), ws.numel()
             hook = _TEXTURE_GRAD_HOOK if (want_rgb and g_rgb is not None) else None
             if hook is None:
@@ -337,8 +341,7 @@ class _RasterizeFunction(torch.autograd.Function):
                 _lib.check(lib.nr_b200_backward(ctypes.byref(a), _stream_ptr(dev)))
                 if pending is not None:
                     pending.wait()
-        # no gradient for face_uvs (the sampler's UV derivative is not implemented)
-        return grad_geom, grad_textures, grad_light, None, None, None
+        return grad_geom, grad_textures, grad_light, None, None, grad_uvs
 
 
 class _MipPyramid(torch.autograd.Function):
@@ -464,11 +467,16 @@ def rasterize_rgbad(
                               top, as read from a PNG) and face_uvs the UV of every face corner (OBJ convention, v = 0 at
                               the bottom; F/2 faces with textures_fill_back).  Sampled bilinearly (clamp to edge) at the
                               perspective-correct UV, with every item's own vertex depths (`reference_exact` has no
-                              effect).  The image receives a gradient, face_uvs does not.
+                              effect).  The image and face_uvs receive gradients: d / d face_uvs is the derivative of
+                              the bilinear sample within the texel cell the forward picked (include/nr_b200.h), with
+                              the level of detail, the perspective weights and the [0,1] clamp held fixed (0 where a
+                              UV is clamped).  A shared face_uvs ([F,3,2], [1,F,3,2] or expanded) gets the sum over
+                              the items; with textures_fill_back the copies' gradient is folded into the F/2 faces.
       texture_filter          'bilinear' (default) or 'trilinear' (texture-image mode only): sample a mip pyramid of the
                               image at each pixel's level of detail, so minified images neither alias nor leave most
                               texels without gradient.  The pyramid is rebuilt from the image on every call and its
-                              gradient collapsed back into the image; no gradient flows through the level of detail.
+                              gradient collapsed back into the image; no gradient flows through the level of detail
+                              (face_uvs gets the level-weighted sum of both levels' derivatives).
     `textures` with batch size 1 (or an expanded stride-0 batch) while the geometry batch is larger = one texture set
     shared by every item (a mesh seen from B viewpoints, mesh.py:29-34); its gradient is the sum over the items."""
     rgb, alpha, depth, _, _ = _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_color,
@@ -498,7 +506,8 @@ def rasterize(
         face_uvs=None,
         texture_filter='bilinear',
 ):
-    """RGB images [B,3,H,W] from faces and textures.  rasterize.py:980-1008 (keyword-only extras: rasterize_rgbad)."""
+    """RGB images [B,3,H,W] from faces and textures.  rasterize.py:980-1008 (keyword-only extras: rasterize_rgbad; in
+    texture-image mode both the image and face_uvs receive gradients)."""
     return rasterize_rgbad(
         faces, textures, image_size, anti_aliasing, near, far, eps, background_color, True, False, False,
         face_light=face_light, textures_fill_back=textures_fill_back, vertices=vertices,

@@ -89,7 +89,9 @@ class Renderer(object):
     def render(self, vertices, faces, textures, face_uvs=None):
         """RGB images [B,3,H,W].  `textures` are per-face cubes [B,F,ts,ts,ts,3], or -- with `face_uvs` [F,3,2] /
         [B,F,3,2] (UV of every face corner, OBJ convention) -- a texture image [Ht,Wt,3] / [1|B,Ht,Wt,3] (row 0 = top),
-        sampled at the perspective-correct UV with `self.texture_filter` (neural_renderer_b200.rasterize_rgbad)."""
+        sampled at the perspective-correct UV with `self.texture_filter` (neural_renderer_b200.rasterize_rgbad).  Both
+        the image and a `face_uvs` with requires_grad receive gradients (fused: the fill_back copies' UV gradient is
+        folded into the original faces in the kernel; op by op: through the cat / flip of the doubled corners)."""
         texture_filter = self.texture_filter if face_uvs is not None else 'bilinear'
         fused = (self.fused and self._fusable(vertices, faces) and textures.is_cuda and textures.dtype == torch.float32)
         light_args = (self.light_intensity_ambient, self.light_intensity_directional, self.light_color_ambient,

@@ -8,13 +8,18 @@ backward with a dense N(0,1) upstream gradient (bench.py's headline step).  Text
   cubes_ts4        the per-item ts = 4 cubes of bench.py
   uv_shared_1024_trilinear, uv_item_256_trilinear   the two image variants with texture_filter='trilinear': the mip
                    pyramid is built (k_mip_build) and its gradient collapsed (k_mip_collapse) on every step
+  uv_shared_1024_uvgrad, uv_shared_1024_trilinear_uvgrad   uv_shared_1024 (bilinear / trilinear) with
+                   face_uvs.requires_grad_(True): k_image_grad also returns d loss / d face_uvs
 Whole step: CUDA events around `steps` steps after `warmup` warm-up steps, median over `reps` repetitions.  Per kernel:
 the library's own CUDA-event profiler over `steps` further steps (ms per step).  Bytes held = texture + its gradient.
 The roofline fraction of the image-gradient kernel and of the zero-fill uses bench.py's HBM figure.  For every image
 variant, `lod_above_0` is the share of covered pixels whose trilinear level of detail is above 0 (how much the geometry
 minifies the image), computed once with torch from the saved maps and not timed.
 
-    python tools/bench_uv.py [--steps 20] [--warmup 3] [--reps 5]
+    python tools/bench_uv.py [--steps 20] [--warmup 3] [--reps 5] [--only name,name,...]
+
+--only runs the named variants in the given order (e.g. a variant before and after its counterpart, to see how much of
+a difference is the order of the run).
 """
 import argparse
 import collections
@@ -75,6 +80,7 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--only", default=None, help="comma-separated variant names, run in this order")
     a = ap.parse_args()
     dev = torch.device("cuda")
     B, F, S = a.batch, a.faces, a.size
@@ -84,22 +90,29 @@ def main():
     img1024 = torch.from_numpy(synthetic.random_image(1, 1024, 1024)[0]).to(dev)
     img256 = torch.from_numpy(synthetic.random_image(B, 256, 256)).to(dev)
     variants = collections.OrderedDict([
-        ("uv_shared_1024", (img1024, uvs, "bilinear")),
-        ("uv_item_256", (img256, uvs, "bilinear")),
-        ("cubes_ts4", (torch.from_numpy(synthetic.random_textures(B, F, 4)).to(dev), None, "bilinear")),
-        ("uv_shared_1024_trilinear", (img1024, uvs, "trilinear")),
-        ("uv_item_256_trilinear", (img256, uvs, "trilinear")),
+        ("uv_shared_1024", (img1024, uvs, "bilinear", False)),
+        ("uv_item_256", (img256, uvs, "bilinear", False)),
+        ("cubes_ts4", (torch.from_numpy(synthetic.random_textures(B, F, 4)).to(dev), None, "bilinear", False)),
+        ("uv_shared_1024_trilinear", (img1024, uvs, "trilinear", False)),
+        ("uv_item_256_trilinear", (img256, uvs, "trilinear", False)),
+        ("uv_shared_1024_uvgrad", (img1024, uvs, "bilinear", True)),
+        ("uv_shared_1024_trilinear_uvgrad", (img1024, uvs, "trilinear", True)),
     ])
+    if a.only:
+        variants = collections.OrderedDict((k, variants[k]) for k in a.only.split(","))
     lib = _lib.load()
     props = torch.cuda.get_device_properties(dev)
     out = {"gpu": torch.cuda.get_device_name(dev), "sm_count": props.multi_processor_count, "shape": {"batch": B, "faces": F, "size": S, "anti_aliasing": False},
            "hbm_gbs": hbm_gbs(), "variants": {}}
-    for name, (tex0, fuv, tf) in variants.items():
+    for name, (tex0, fuv0, tf, uv_grad) in variants.items():
         tex = tex0.clone().requires_grad_(True)
+        fuv = fuv0.clone().requires_grad_(True) if uv_grad else fuv0
 
         def step():
             faces.grad = None
             tex.grad = None
+            if uv_grad:
+                fuv.grad = None
             img = nr.rasterize(faces, tex, S, False, face_uvs=fuv, texture_filter=tf)
             img.backward(g)
 
@@ -128,10 +141,10 @@ def main():
         tex_bytes = tex.numel() * 4
         if tf == "trilinear":  # the rasterizer samples (and its gradient is) the pyramid
             tex_bytes = tex.numel() // (tex.shape[-3] * tex.shape[-2]) * lib.nr_b200_mip_texels(*tex.shape[-3:-1]) * 4
-        rec = {"texture_filter": tf, "step_ms_median": float(np.median(reps)), "step_ms_reps": reps,
+        rec = {"texture_filter": tf, "uv_grad": uv_grad, "step_ms_median": float(np.median(reps)), "step_ms_reps": reps,
                "kernels_ms_per_step": kern, "texture_bytes": tex_bytes, "texture_plus_grad_bytes": 2 * tex_bytes}
         if fuv is not None:
-            rec["lod_above_0"] = lod_above_0(faces.detach(), fuv[None], tex.shape[-3], tex.shape[-2], S)
+            rec["lod_above_0"] = lod_above_0(faces.detach(), fuv.detach()[None], tex.shape[-3], tex.shape[-2], S)
         grad_kernel = "k_image_grad" if fuv is not None else "k_texture_grad"
         if grad_kernel in kern:
             rec["grad_kernel"] = grad_kernel
