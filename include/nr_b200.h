@@ -133,8 +133,24 @@ extern "C" {
  *   unlit trilinear sample times the upstream gradient.  NO gradient flows through the LOD. */
 #define NR_TEX_MIPMAP 0x80000u /* textures = packed mip pyramid of the image, sampled trilinearly (needs NR_TEX_UV)        */
 
+/* Smooth (Gouraud) shading, additive to ABI 4: the field corner_light appended to nr_b200_forward_args, and the backward
+ * entry point nr_b200_backward_corner_light, which takes the same corner_light (the backward struct is unchanged).
+ *   corner_light [B,F,3,3] is an RGB light factor at each corner k of face f, corners in the face's own order (the order
+ *   of `faces` / `face_indices`); as with face_light, F counts the fill_back copies as faces of their own.  Per item only.
+ *   A non-NULL corner_light needs NR_RETURN_RGB and excludes face_light (else NR_ERR_INVALID_ARG).
+ *   Covered raster pixel with winner weights w_k, depth zp and the winner's OWN vertex depths z_k (NR_TEX_Z_BATCH0 has no
+ *   effect on this):  l_k = w_k * (zp / z_k)  (div.rn, the l_k of NR_TEX_UV), and per channel c
+ *     L_c = fma(l_2, C_2c, fma(l_1, C_1c, l_0 * C_0c)),   rgb_c = L_c * s_c  (fp32, round-to-nearest)
+ *   where s is the UNLIT sample exactly as the unlit path computes it (ts^3 cube, bilinear image or trilinear pyramid):
+ *   the light multiplies after the blend, not per tap.  The background is not lit; anti-aliasing pools on top as before.
+ *   NR_FWD_STAGE_TEXTURES is ignored with corner_light.
+ *   Backward (nr_b200_backward_corner_light), texture half: grad_textures as without light, with d rgb_c / d s_c = L_c in place of face_light; grad_face_uvs
+ *   likewise uses L_c; grad_corner_light[b,f,k,c] += l_k * g_c * s_c (zero-filled first unless NR_GRAD_ACCUMULATE; needs
+ *   corner_light and `textures`).  No vertex gradient flows through l_k: grad_faces / grad_vertices are those of the
+ *   unchanged edge scan (which reads the smooth-shaded rgb map) and depth gradient.  fp32 atomics, not bit-pinned. */
+
 typedef struct nr_b200_forward_args {
-    uint32_t struct_size; /* sizeof(nr_b200_forward_args), for ABI evolution */
+    uint32_t struct_size; /* sizeof(nr_b200_forward_args), or offsetof(.., corner_light) (see there) */
     uint32_t flags;
     int32_t batch_size;   /* B */
     int32_t num_faces;    /* F */
@@ -175,6 +191,9 @@ typedef struct nr_b200_forward_args {
     const float *face_uvs;  /* [B,F,3,2], or [F,3,2] with NR_UV_SHARED (F/2 faces with NR_TEX_FILL_BACK) */
     int32_t texture_height; /* Ht >= 1 */
     int32_t texture_width;  /* Wt >= 1 */
+    /* ABI 4, appended: smooth shading (above).  struct_size may also be offsetof(nr_b200_forward_args, corner_light), the
+     * layout before this field, which then reads as NULL.  Only struct_size bytes are read. */
+    const float *corner_light; /* [B,F,3,3] or NULL */
 } nr_b200_forward_args;
 
 typedef struct nr_b200_backward_args {
@@ -232,6 +251,11 @@ NR_B200_API size_t nr_b200_backward_workspace_bytes(int32_t batch_size, int32_t 
 
 NR_B200_API int nr_b200_forward(const nr_b200_forward_args *args, void *cuda_stream);
 NR_B200_API int nr_b200_backward(const nr_b200_backward_args *args, void *cuda_stream);
+/* The backward of a forward call that had corner_light (smooth shading, above): `args` as for nr_b200_backward (with
+ * face_light NULL), corner_light [B,F,3,3] as given to the forward call (required), grad_corner_light [B,F,3,3] or NULL =
+ * not wanted (part of the texture half, NR_BWD_PART_TEXTURES).  nr_b200_backward is this call with corner_light NULL. */
+NR_B200_API int nr_b200_backward_corner_light(const nr_b200_backward_args *args, const float *corner_light,
+                                              float *grad_corner_light, void *cuda_stream);
 
 /* vertices_to_faces (reference vertices_to_faces.py:4-21), the step either side of the rasterizer:
  *   forward   out_faces[b,f,k,:] = vertices[b, faces[b,f,k], :]           ([B,Nv,3] x [B,Nf,3] int32 -> [B,Nf,3,3])
@@ -275,6 +299,40 @@ NR_B200_API int nr_b200_face_lighting(const float *vertices, const int32_t *face
 NR_B200_API int nr_b200_face_lighting_backward(const float *vertices, const int32_t *faces, const float *light_params,
                                                const float *grad_face_light, int32_t batch_size, int32_t num_vertices,
                                                int32_t num_faces, uint32_t flags, float *grad_vertices, void *cuda_stream);
+
+/* Smooth shading glue (feeds nr_b200_forward_args.corner_light).
+ * Vertex normals, area weighted, from vertices [B,Nv,3] and the index set `faces` [B,Nf,3] ([Nf,3] with NR_INDICES_SHARED):
+ *   c_f = cross(v0 - v1, v2 - v1) (unnormalised, the face-normal direction of lighting.py:40-43; 0 for a face with an index
+ *   outside [0, Nv)),  s_v = sum of c_f over every corner (f, k) with faces[f,k] == v, added in ascending (f, k) order,
+ *   n_v = s_v / (|s_v| + 1e-5)  (an unreferenced vertex gets 0).  Pass the original faces, not a fill_back-doubled set
+ *   (whose copies would cancel the sums).  The forward is deterministic (no float atomics): a stable radix sort of the
+ *   corners by vertex, then one ordered gather per vertex, with scratch in the caller's workspace of
+ *   nr_b200_vertex_normals_workspace_bytes (it asks the current device for the sort's tuning, so it needs a CUDA device;
+ *   0 = unsupported sizes).  The same workspace serves the backward, which turns d loss / d vertex_normals into
+ *   d loss / d vertices (zero-filled first unless NR_GRAD_ACCUMULATE; fp32 atomics).
+ *   NR_ERR_UNSUPPORTED when (items of the index set) * (Nv + 1) or 3 Nf exceeds 2^31 - 1. */
+NR_B200_API size_t nr_b200_vertex_normals_workspace_bytes(int32_t batch_size, int32_t num_vertices, int32_t num_faces,
+                                                         uint32_t flags);
+NR_B200_API int nr_b200_vertex_normals(const float *vertices, const int32_t *faces, int32_t batch_size, int32_t num_vertices,
+                                       int32_t num_faces, uint32_t flags, float *vertex_normals, void *workspace,
+                                       size_t workspace_bytes, void *cuda_stream);
+NR_B200_API int nr_b200_vertex_normals_backward(const float *vertices, const int32_t *faces, const float *grad_vertex_normals,
+                                                int32_t batch_size, int32_t num_vertices, int32_t num_faces, uint32_t flags,
+                                                float *grad_vertices, void *workspace, size_t workspace_bytes,
+                                                void *cuda_stream);
+/* Per-corner Lambertian light from vertex normals [B,Nv,3], `faces` the index set the rasterizer receives ([B,Nf,3] or
+ * [Nf,3] with NR_INDICES_SHARED) and light_params [B,9] ([1,9] with NR_CAM_SHARED, layout of nr_b200_face_lighting):
+ *   corner_light[b,f,k,:] = ambient + directional * max(sgn * (n . direction), 0),   n = vertex_normals[b, faces[f,k]]
+ *   (0 for an index outside [0, Nv)), dot as (n0 d0 + n1 d1) + n2 d2, sgn = -1 for the reversed copies f >= Nf/2 with
+ *   NR_TEX_FILL_BACK (Nf even; their face normal is reversed, as in face_light), else 1.  The backward scatters
+ *   d loss / d corner_light into grad_vertex_normals [B,Nv,3] (zero-filled first unless NR_GRAD_ACCUMULATE; atomics). */
+NR_B200_API int nr_b200_corner_lighting(const float *vertex_normals, const int32_t *faces, const float *light_params,
+                                        int32_t batch_size, int32_t num_vertices, int32_t num_faces, uint32_t flags,
+                                        float *corner_light, void *cuda_stream);
+NR_B200_API int nr_b200_corner_lighting_backward(const float *vertex_normals, const int32_t *faces, const float *light_params,
+                                                 const float *grad_corner_light, int32_t batch_size, int32_t num_vertices,
+                                                 int32_t num_faces, uint32_t flags, float *grad_vertex_normals,
+                                                 void *cuda_stream);
 
 /* Texture baking of load_obj (reference load_obj.py:88-137): every texel (a, b, c) of the ts^3 cube of face f is the
  * bilinear sample of `image` [H,W,3] (rows already flipped, load_obj.py:82) at the UV position with barycentric

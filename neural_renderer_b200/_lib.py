@@ -42,12 +42,18 @@ EXPORTED_SYMBOLS = (
     "nr_b200_backward_workspace_bytes",
     "nr_b200_forward",
     "nr_b200_backward",
+    "nr_b200_backward_corner_light",
     "nr_b200_vertices_to_faces",
     "nr_b200_vertices_to_faces_backward",
     "nr_b200_camera_transform",
     "nr_b200_camera_transform_backward",
     "nr_b200_face_lighting",
     "nr_b200_face_lighting_backward",
+    "nr_b200_vertex_normals_workspace_bytes",
+    "nr_b200_vertex_normals",
+    "nr_b200_vertex_normals_backward",
+    "nr_b200_corner_lighting",
+    "nr_b200_corner_lighting_backward",
     "nr_b200_bake_textures",
     "nr_b200_mip_texels",
     "nr_b200_mip_build",
@@ -74,6 +80,7 @@ class ForwardArgs(ctypes.Structure):
         ("vertices", ctypes.c_void_p), ("face_indices", ctypes.c_void_p),
         ("num_vertices", ctypes.c_int32), ("_pad1", ctypes.c_int32),
         ("face_uvs", ctypes.c_void_p), ("texture_height", ctypes.c_int32), ("texture_width", ctypes.c_int32),
+        ("corner_light", ctypes.c_void_p),  # appended within ABI 4; struct_size = ForwardArgs.corner_light.offset omits it
     ]
 
 
@@ -125,6 +132,9 @@ def load():
     lib.nr_b200_forward.argtypes = [ctypes.POINTER(ForwardArgs), ctypes.c_void_p]
     lib.nr_b200_backward.restype = ctypes.c_int
     lib.nr_b200_backward.argtypes = [ctypes.POINTER(BackwardArgs), ctypes.c_void_p]
+    lib.nr_b200_backward_corner_light.restype = ctypes.c_int
+    lib.nr_b200_backward_corner_light.argtypes = [ctypes.POINTER(BackwardArgs), ctypes.c_void_p, ctypes.c_void_p,
+                                                  ctypes.c_void_p]
     lib.nr_b200_vertices_to_faces.restype = ctypes.c_int
     lib.nr_b200_vertices_to_faces.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
                                               ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p]
@@ -143,6 +153,20 @@ def load():
     lib.nr_b200_face_lighting_backward.restype = ctypes.c_int
     lib.nr_b200_face_lighting_backward.argtypes = [ctypes.c_void_p] * 4 + [ctypes.c_int32] * 3 + [ctypes.c_uint32, ctypes.c_void_p,
                                                                                                 ctypes.c_void_p]
+    lib.nr_b200_vertex_normals_workspace_bytes.restype = ctypes.c_size_t
+    lib.nr_b200_vertex_normals_workspace_bytes.argtypes = [ctypes.c_int32] * 3 + [ctypes.c_uint32]
+    lib.nr_b200_vertex_normals.restype = ctypes.c_int
+    lib.nr_b200_vertex_normals.argtypes = [ctypes.c_void_p] * 2 + [ctypes.c_int32] * 3 + [ctypes.c_uint32] + \
+        [ctypes.c_void_p] * 2 + [ctypes.c_size_t, ctypes.c_void_p]
+    lib.nr_b200_vertex_normals_backward.restype = ctypes.c_int
+    lib.nr_b200_vertex_normals_backward.argtypes = [ctypes.c_void_p] * 3 + [ctypes.c_int32] * 3 + [ctypes.c_uint32] + \
+        [ctypes.c_void_p] * 2 + [ctypes.c_size_t, ctypes.c_void_p]
+    lib.nr_b200_corner_lighting.restype = ctypes.c_int
+    lib.nr_b200_corner_lighting.argtypes = [ctypes.c_void_p] * 3 + [ctypes.c_int32] * 3 + [ctypes.c_uint32, ctypes.c_void_p,
+                                                                                         ctypes.c_void_p]
+    lib.nr_b200_corner_lighting_backward.restype = ctypes.c_int
+    lib.nr_b200_corner_lighting_backward.argtypes = [ctypes.c_void_p] * 4 + [ctypes.c_int32] * 3 + [ctypes.c_uint32,
+                                                                                                  ctypes.c_void_p, ctypes.c_void_p]
     lib.nr_b200_bake_textures.restype = ctypes.c_int
     lib.nr_b200_bake_textures.argtypes = [ctypes.c_void_p] * 3 + [ctypes.c_int32] * 4 + [ctypes.c_void_p, ctypes.c_void_p]
     lib.nr_b200_mip_texels.restype = ctypes.c_size_t

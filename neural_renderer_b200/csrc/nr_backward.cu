@@ -70,6 +70,9 @@
 #ifndef NR_TG_MIN_CTAS
 #define NR_TG_MIN_CTAS 6
 #endif
+#ifndef NR_TGC_MIN_CTAS
+#define NR_TGC_MIN_CTAS 3       // k_texture_grad with corner_light: spills at 4 CTAs (64 registers)
+#endif
 #ifndef NR_IG_MIN_CTAS
 #define NR_IG_MIN_CTAS 4        // k_image_grad CTAs of 256 threads per SM (64 registers; see DESIGN.md section 4)
 #endif
@@ -140,6 +143,9 @@ struct BwdParams {
     nr::MipTable mip;
     // d loss / d face_uvs (appended likewise): the layout of `uvs` (uv_bstride floats per item), or nullptr
     float* grad_uvs;
+    // smooth shading (appended likewise): corner_light [B,F,3,3] (the kCorner variants) and its gradient, or nullptr
+    const float* corner_light;
+    float* grad_corner_light;
 };
 
 //@phase helpers: rcp / vector RED / load_grad (inlined)
@@ -919,26 +925,71 @@ __global__ void __launch_bounds__(kThreads, NR_ES_CTAS_PER_1024 * 1024 / kThread
 #endif
 }
 
+// ---------------------------------------------------------------------------------------- corner-light gradient
+// d loss / d corner_light of one pixel from its unlit sample s, upstream gradient g and perspective weights l:
+// [k][c] = l_k (g_c s_c), the face_light term g_c s_c spread over the corners
+__device__ __forceinline__ void corner_light_grad(const float s[3], float g0, float g1, float g2, const float l[3], float (&gl)[9]) {
+    const float gs[3] = {s[0] * g0, s[1] * g1, s[2] * g2};
+#pragma unroll
+    for (int k = 0; k < 3; k++)
+#pragma unroll
+        for (int c = 0; c < 3; c++) gl[3 * k + c] = l[k] * gs[c];
+}
+
+// warp-aggregated scatter of a light gradient into dst [B,F,N]: runs of neighbouring lanes that show the same face sum
+// their N floats with a segmented shuffle and the run's first lane adds them -- the face_light tail of k_texture_grad /
+// image_grad widened to N floats (the corner_light variants, N = 9; the face_light variants keep their own 3-float copy,
+// whose SASS this form would change)
+template <int N>
+__device__ __forceinline__ void light_grad_scatter(float (&gl)[N], int fn, int lane, float* dst, int b, int F) {
+    const int fn_prev = __shfl_up_sync(0xffffffffu, fn, 1);
+    const uint32_t heads = __ballot_sync(0xffffffffu, lane == 0 || fn != fn_prev);
+    const uint32_t later = heads & ~((2u << lane) - 1u);
+    const int run_end = (lane == 31 || later == 0) ? 31 : (__ffs(later) - 2);
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+        const bool take = lane + off <= run_end;
+        float t[N];
+#pragma unroll
+        for (int k = 0; k < N; k++) t[k] = __shfl_down_sync(0xffffffffu, gl[k], off);
+        if (take) {
+#pragma unroll
+            for (int k = 0; k < N; k++) gl[k] += t[k];
+        }
+    }
+    if (fn >= 0 && ((heads >> lane) & 1u)) {
+        float* g = dst + ((size_t)b * F + fn) * N;
+#pragma unroll
+        for (int k = 0; k < N; k++) atomicAdd(g + k, gl[k]);
+    }
+}
+
 // --------------------------------------------------------------------------------------------- k_texture_grad
 // Neighbouring pixels of a face often blend the SAME eight texels (the same cell of the texture cube: 31 % of the
 // covered pixels at the headline shape, 57 % at raster 512), and the L2 pays per reduction it receives.  Lanes of a warp
 // that sit next to each other with the same (cube, cell) therefore add their 8 x 3 contributions together with
 // kTgCombine shuffle steps first (runs of up to 2^kTgCombine lanes collapse into one lane's reductions).
-template <int kTgCombine>
-__global__ void __launch_bounds__(256, kTgCombine ? 4 : NR_TG_MIN_CTAS) k_texture_grad(const __grid_constant__ BwdParams p) {
+//
+// kCorner (corner_light): the pixel's light L_c = the corner factors interpolated with its perspective weights l_k (own
+// vertex depths) takes face_light's place, and d loss / d corner_light = l_k g_c s_c goes through the same run reduction.
+template <int kTgCombine, bool kCorner>
+__global__ void __launch_bounds__(256, kTgCombine ? (kCorner ? NR_TGC_MIN_CTAS : 4) : NR_TG_MIN_CTAS) k_texture_grad(const __grid_constant__ BwdParams p) {
     const int S = p.S;
     const size_t plane = (size_t)S * S;
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;  // pixel within the image (image orientation)
     const int b = blockIdx.y;
     const int lane = threadIdx.x & 31;
     const int fn = (i < plane) ? __ldg(p.fim + (size_t)b * plane + i) : -1;
-    const bool want_light = p.grad_face_light != nullptr;  // uniform
+    const bool want_light = (kCorner ? p.grad_corner_light : p.grad_face_light) != nullptr;  // uniform
     if (kTgCombine) {
         if (!want_light && !__any_sync(0xffffffffu, fn >= 0)) return;  // warp-uniform
     } else {
         if (fn < 0 && !want_light) return;
     }
     float gl0 = 0.0f, gl1 = 0.0f, gl2 = 0.0f;  // d loss / d face_light of this pixel
+    float glc[kCorner ? 9 : 1];                // kCorner: d loss / d corner_light of this pixel
+#pragma unroll
+    for (int k = 0; k < (kCorner ? 9 : 1); k++) glc[k] = 0.0f;
     float val[4][6];                           // contributions to the four corner pairs (6 consecutive floats each)
     float* tp[4] = {nullptr, nullptr, nullptr, nullptr};
     long long key = -1 - (long long)lane;      // (cube, cell, orientation): equal keys <=> the same eight texels
@@ -967,6 +1018,16 @@ __global__ void __launch_bounds__(256, kTgCombine ? 4 : NR_TG_MIN_CTAS) k_textur
             z2 = __ldg(nr::face_vertex_t<true>(p.src, zb, fn, 2) + 2);
         }
         const nr::TexCoord tc = nr::texture_coords(w, zp, z0, z1, z2, ts, p.tex_cmp, p.tex_val);
+        float lam[3] = {0.0f, 0.0f, 0.0f}, L[3];  // kCorner: perspective weights (own depths) and light of the pixel
+        if constexpr (kCorner) {  // l_k with the item's own depths (NR_TEX_Z_BATCH0 only moves the cube coordinates)
+            float oz[3] = {z0, z1, z2};
+            if (zb != b) {
+#pragma unroll
+                for (int k = 0; k < 3; k++) oz[k] = __ldg(nr::face_vertex(p.src, b, fn, k) + 2);
+            }
+            nr::perspective_weights(w, zp, oz[0], oz[1], oz[2], lam);
+            nr::corner_light_at(p.corner_light + ((size_t)b * p.F + fn) * 9, lam, L);
+        }
         // NR_TEX_FILL_BACK: the reversed copy of face f - F/2 shares that face's cube, axes reversed
         int cube = fn, ncubes = p.F;
         bool rev = false;
@@ -986,9 +1047,16 @@ __global__ void __launch_bounds__(256, kTgCombine ? 4 : NR_TG_MIN_CTAS) k_textur
                 g = __fmaf_rn(cw, __ldg(t + 1), g);
                 bl = __fmaf_rn(cw, __ldg(t + 2), bl);
             }
-            gl0 = r * g0; gl1 = g * g1; gl2 = bl * g2;
+            if constexpr (kCorner) {
+                const float s3[3] = {r, g, bl};
+                corner_light_grad(s3, g0, g1, g2, lam, glc);
+            } else {
+                gl0 = r * g0; gl1 = g * g1; gl2 = bl * g2;
+            }
         }
-        if (p.face_light) {  // d rgb / d texel = weight * light
+        if constexpr (kCorner) {  // d rgb / d texel = weight * interpolated light
+            g0 *= L[0]; g1 *= L[1]; g2 *= L[2];
+        } else if (p.face_light) {  // d rgb / d texel = weight * light
             const float* lp = p.face_light + ((size_t)b * p.F + fn) * 3;
             g0 *= __ldg(lp); g1 *= __ldg(lp + 1); g2 *= __ldg(lp + 2);
         }
@@ -1048,6 +1116,10 @@ __global__ void __launch_bounds__(256, kTgCombine ? 4 : NR_TG_MIN_CTAS) k_textur
         }
     }
     if (!want_light) return;
+    if constexpr (kCorner) {
+        light_grad_scatter(glc, fn, lane, p.grad_corner_light, b, p.F);
+        return;
+    }
     // warp-aggregated scatter of the light gradient: runs of neighbouring lanes that show the same face
     const int fn_prev = __shfl_up_sync(0xffffffffu, fn, 1);
     const uint32_t heads = __ballot_sync(0xffffffffu, lane == 0 || fn != fn_prev);
@@ -1091,7 +1163,10 @@ __device__ __forceinline__ void red_add_6(float* t, const float v[6]) {
 // gradient then takes instead of reading the taps again); gu = sum_l a_l sum_c g_c light_c du_c (v alike, a_l = the level
 // weight) goes to UV corner k as l_k (gu, gv), corners reversed back for a fill_back copy.  Runs of neighbouring lanes
 // that show the same face sum their 6 floats with shuffles and the run's first lane adds them.
-template <int kTgCombine, bool kMip, bool kUvGrad>
+//
+// kCorner (corner_light): as in k_texture_grad, the interpolated light L_c replaces face_light (also in the face_uvs
+// gradient) and the 9-float corner-light gradient goes through the run reduction.
+template <int kTgCombine, bool kMip, bool kUvGrad, bool kCorner>
 __device__ __forceinline__ void image_grad(const BwdParams& p) {
     constexpr int kPairs = kMip ? 4 : 2;
     const int S = p.S;
@@ -1100,9 +1175,12 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
     const int b = blockIdx.y;
     const int lane = threadIdx.x & 31;
     const int fn = (i < plane) ? __ldg(p.fim + (size_t)b * plane + i) : -1;
-    const bool want_light = p.grad_face_light != nullptr;  // uniform
+    const bool want_light = (kCorner ? p.grad_corner_light : p.grad_face_light) != nullptr;  // uniform
     if (!want_light && !__any_sync(0xffffffffu, fn >= 0)) return;  // warp-uniform
     float gl0 = 0.0f, gl1 = 0.0f, gl2 = 0.0f;  // d loss / d face_light of this pixel
+    float glc[kCorner ? 9 : 1];                // kCorner: d loss / d corner_light of this pixel
+#pragma unroll
+    for (int k = 0; k < (kCorner ? 9 : 1); k++) glc[k] = 0.0f;
     float val[kPairs][6];                      // tap row 0 / 1 (of level l0, then l1): taps (x0, x1) x 3 channels
     float* tp[kPairs];
     bool adjacent[kPairs / 2];                 // x1 == x0 + 1 (else both taps of a row are the same texel, weight 0 on x1)
@@ -1153,6 +1231,11 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
         float uv[6], u, v;
         nr::load_face_uvs(p.uvs + ((uint32_t)b * p.uv_bstride + (uint32_t)uf * 6u), rev, uv);
         nr::pixel_uv(w, zp, z0, z1, z2, uv, u, v);
+        float lam[3] = {0.0f, 0.0f, 0.0f}, L[3];  // kCorner: perspective weights and light of the pixel
+        if constexpr (kCorner) {
+            nr::perspective_weights(w, zp, z0, z1, z2, lam);
+            nr::corner_light_at(p.corner_light + ((size_t)b * p.F + fn) * 9, lam, L);
+        }
         const uint32_t img_off = (uint32_t)b * p.img_bstride;
         // level(s) and their weights: the bilinear variant is level 0 of an image with weight 1
         int lv[2] = {0, 0};
@@ -1167,7 +1250,9 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
         const nr::UvTaps t0 = nr::uv_taps(u, v, kMip ? p.mip.h[lv[0]] : p.Ht, kMip ? p.mip.w[lv[0]] : p.Wt);
         if constexpr (kUvGrad) {
             float lt[3] = {1.0f, 1.0f, 1.0f};
-            if (p.face_light) {
+            if constexpr (kCorner) {
+                lt[0] = L[0]; lt[1] = L[1]; lt[2] = L[2];
+            } else if (p.face_light) {
                 const float* lp = p.face_light + ((size_t)b * p.F + fn) * 3;
                 lt[0] = __ldg(lp); lt[1] = __ldg(lp + 1); lt[2] = __ldg(lp + 2);
             }
@@ -1187,7 +1272,11 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
                 gu = __fmaf_rn(lw[q], eu, gu);
                 gv = __fmaf_rn(lw[q], ev, gv);
             }
-            if (want_light) { gl0 = c[0] * g0; gl1 = c[1] * g1; gl2 = c[2] * g2; }
+            if constexpr (kCorner) {
+                if (want_light) corner_light_grad(c, g0, g1, g2, lam, glc);
+            } else {
+                if (want_light) { gl0 = c[0] * g0; gl1 = c[1] * g1; gl2 = c[2] * g2; }
+            }
             // uv = sum_k l_k uv_k (pixel_uv); a fill_back copy's corner k is corner 2 - k of the stored face
             const float l0 = __fmul_rn(w[0], __fdiv_rn(zp, z0)), l1 = __fmul_rn(w[1], __fdiv_rn(zp, z1)),
                         l2 = __fmul_rn(w[2], __fdiv_rn(zp, z2));
@@ -1206,9 +1295,12 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
             } else {
                 nr::uv_blend<false>(p.textures + img_off, p.Wt, t0, 1.0f, 1.0f, 1.0f, c);
             }
-            gl0 = c[0] * g0; gl1 = c[1] * g1; gl2 = c[2] * g2;
+            if constexpr (kCorner) corner_light_grad(c, g0, g1, g2, lam, glc);
+            else { gl0 = c[0] * g0; gl1 = c[1] * g1; gl2 = c[2] * g2; }
         }
-        if (p.face_light) {  // d rgb / d texel = weight * light
+        if constexpr (kCorner) {  // d rgb / d texel = weight * interpolated light
+            g0 *= L[0]; g1 *= L[1]; g2 *= L[2];
+        } else if (p.face_light) {  // d rgb / d texel = weight * light
             const float* lp = p.face_light + ((size_t)b * p.F + fn) * 3;
             g0 *= __ldg(lp); g1 *= __ldg(lp + 1); g2 *= __ldg(lp + 2);
         }
@@ -1295,6 +1387,10 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
         if (fn >= 0 && ((heads >> lane) & 1u)) red_add_6(p.grad_uvs + uv_at, uvg);
     }
     if (!want_light) return;
+    if constexpr (kCorner) {
+        light_grad_scatter(glc, fn, lane, p.grad_corner_light, b, p.F);
+        return;
+    }
     // warp-aggregated scatter of the light gradient: runs of neighbouring lanes that show the same face
     const int fn_prev = __shfl_up_sync(0xffffffffu, fn, 1);
     const uint32_t heads = __ballot_sync(0xffffffffu, lane == 0 || fn != fn_prev);
@@ -1313,13 +1409,13 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
     }
 }
 
-template <int kTgCombine, bool kUvGrad>
+template <int kTgCombine, bool kUvGrad, bool kCorner>
 __global__ void __launch_bounds__(256, kUvGrad ? NR_IGU_MIN_CTAS : NR_IG_MIN_CTAS) k_image_grad(const __grid_constant__ BwdParams p) {
-    image_grad<kTgCombine, false, kUvGrad>(p);
+    image_grad<kTgCombine, false, kUvGrad, kCorner>(p);
 }
-template <int kTgCombine, bool kUvGrad>
+template <int kTgCombine, bool kUvGrad, bool kCorner>
 __global__ void __launch_bounds__(256, kUvGrad ? NR_IGMU_MIN_CTAS : NR_IGM_MIN_CTAS) k_image_grad_mip(const __grid_constant__ BwdParams p) {
-    image_grad<kTgCombine, true, kUvGrad>(p);
+    image_grad<kTgCombine, true, kUvGrad, kCorner>(p);
 }
 
 // ----------------------------------------------------------------------------------------------- k_depth_grad
@@ -1474,7 +1570,9 @@ extern "C" size_t nr_b200_backward_workspace_bytes(int32_t B, int32_t F, int32_t
     return bin_layout(B, F, S, strip_rec_bytes(S, both)).total;
 }
 
-extern "C" int nr_b200_backward(const nr_b200_backward_args* args, void* cuda_stream) {
+// nr_b200_backward (corner_light NULL) and nr_b200_backward_corner_light (smooth shading)
+static int backward_impl(const nr_b200_backward_args* args, const float* corner_light, float* grad_corner_light,
+                         void* cuda_stream) {
     nr_internal::launch_count() = 0;
     // Two layouts: the full struct, and the ABI-4 struct from before grad_face_uvs (which then reads as NULL).  Only the
     // caller's struct_size bytes are read.
@@ -1511,6 +1609,10 @@ extern "C" int nr_b200_backward(const nr_b200_backward_args* args, void* cuda_st
     if (rgb && part_tex && !a->grad_textures) return NR_ERR_INVALID_ARG;
     if (rgb && (flags & NR_TEX_FILL_BACK) && (F & 1)) return NR_ERR_INVALID_ARG;
     if (rgb && a->grad_face_light && !a->textures) return NR_ERR_INVALID_ARG;
+    // smooth shading: corner_light only for RGB and instead of face_light; its gradient reads the (unlit) textures
+    const bool smooth = corner_light != nullptr;
+    if (smooth && (!rgb || a->face_light)) return NR_ERR_INVALID_ARG;
+    if (grad_corner_light && (!smooth || !a->textures)) return NR_ERR_INVALID_ARG;
     if ((flags & NR_ANTI_ALIASING) && (S & 1)) return NR_ERR_INVALID_ARG;
     if (S > 32767 || B > 65535) return NR_ERR_UNSUPPORTED;
     if ((size_t)B * F * 2 * kWideStrips >= (size_t)0x7FFFFFFF) return NR_ERR_UNSUPPORTED;  // 32-bit list offsets
@@ -1553,6 +1655,9 @@ extern "C" int nr_b200_backward(const nr_b200_backward_args* args, void* cuda_st
             return NR_ERR_CUDA;
         if (part_tex && uv_grad && cudaMemsetAsync(a->grad_face_uvs, 0, uv_items * uv_floats * sizeof(float), stream) != cudaSuccess)
             return NR_ERR_CUDA;
+        if (part_tex && grad_corner_light &&
+            cudaMemsetAsync(grad_corner_light, 0, (size_t)B * F * 9 * sizeof(float), stream) != cudaSuccess)
+            return NR_ERR_CUDA;
         nr_internal::prof_end(stream);
     }
 
@@ -1578,23 +1683,29 @@ extern "C" int nr_b200_backward(const nr_b200_backward_args* args, void* cuda_st
         if (mip) p.mip = mt;
         p.grad_uvs = a->grad_face_uvs;
     }
+    p.corner_light = corner_light; p.grad_corner_light = grad_corner_light;
 
     const dim3 pgrid((unsigned)(((size_t)S * S + 255) / 256), B);
     auto launch_texture_grad = [&]() {
         if (mip) {
             nr_internal::LaunchScope ls("k_image_grad", stream);
-            if (uv_grad) k_image_grad_mip<NR_TG_COMBINE, true><<<pgrid, 256, 0, stream>>>(p);
-            else k_image_grad_mip<NR_TG_COMBINE, false><<<pgrid, 256, 0, stream>>>(p);
+            if (smooth && uv_grad) k_image_grad_mip<NR_TG_COMBINE, true, true><<<pgrid, 256, 0, stream>>>(p);
+            else if (smooth) k_image_grad_mip<NR_TG_COMBINE, false, true><<<pgrid, 256, 0, stream>>>(p);
+            else if (uv_grad) k_image_grad_mip<NR_TG_COMBINE, true, false><<<pgrid, 256, 0, stream>>>(p);
+            else k_image_grad_mip<NR_TG_COMBINE, false, false><<<pgrid, 256, 0, stream>>>(p);
             return;
         }
         if (uv) {
             nr_internal::LaunchScope ls("k_image_grad", stream);
-            if (uv_grad) k_image_grad<NR_TG_COMBINE, true><<<pgrid, 256, 0, stream>>>(p);
-            else k_image_grad<NR_TG_COMBINE, false><<<pgrid, 256, 0, stream>>>(p);
+            if (smooth && uv_grad) k_image_grad<NR_TG_COMBINE, true, true><<<pgrid, 256, 0, stream>>>(p);
+            else if (smooth) k_image_grad<NR_TG_COMBINE, false, true><<<pgrid, 256, 0, stream>>>(p);
+            else if (uv_grad) k_image_grad<NR_TG_COMBINE, true, false><<<pgrid, 256, 0, stream>>>(p);
+            else k_image_grad<NR_TG_COMBINE, false, false><<<pgrid, 256, 0, stream>>>(p);
             return;
         }
         nr_internal::LaunchScope ls("k_texture_grad", stream);
-        k_texture_grad<NR_TG_COMBINE><<<pgrid, 256, 0, stream>>>(p);
+        if (smooth) k_texture_grad<NR_TG_COMBINE, true><<<pgrid, 256, 0, stream>>>(p);
+        else k_texture_grad<NR_TG_COMBINE, false><<<pgrid, 256, 0, stream>>>(p);
     };
     // K6 first, unless its output buffer is zero-filled by the edge scan
     if (part_tex && rgb && p.g_rgb && !fill_in_scan) launch_texture_grad();
@@ -1685,4 +1796,17 @@ extern "C" int nr_b200_backward(const nr_b200_backward_args* args, void* cuda_st
         k_depth_grad<<<pgrid, 256, 0, stream>>>(p);
     }
     return cudaGetLastError() == cudaSuccess ? NR_OK : NR_ERR_CUDA;
+}
+
+extern "C" int nr_b200_backward(const nr_b200_backward_args* args, void* cuda_stream) {
+    return backward_impl(args, nullptr, nullptr, cuda_stream);
+}
+
+extern "C" int nr_b200_backward_corner_light(const nr_b200_backward_args* args, const float* corner_light,
+                                             float* grad_corner_light, void* cuda_stream) {
+    if (!corner_light) {
+        nr_internal::launch_count() = 0;
+        return NR_ERR_INVALID_ARG;
+    }
+    return backward_impl(args, corner_light, grad_corner_light, cuda_stream);
 }

@@ -34,6 +34,7 @@
 #include <math.h>
 #include <stdint.h>
 #include <stdlib.h>
+#include <string.h>
 
 #include <algorithm>
 
@@ -64,6 +65,12 @@ constexpr int kOwnTable = 256;         // rows / fragments per pass whose owner 
 #ifndef NR_RESOLVE_MIP_MIN_CTAS
 #define NR_RESOLVE_MIP_MIN_CTAS 4  // the trilinear variants (kTex == 3): 64 registers; at 5 or 6 CTAs (48 / 40 registers)
                                    // they spill (-Xptxas -v)
+#endif
+#ifndef NR_RESOLVE_SMOOTH_MIN_CTAS
+#define NR_RESOLVE_SMOOTH_MIN_CTAS 6     // smooth-shaded (kLight == 2) cube / bilinear variants: 40 registers, no spills
+#endif
+#ifndef NR_RESOLVE_SMOOTH_AA_MIN_CTAS
+#define NR_RESOLVE_SMOOTH_AA_MIN_CTAS 4  // the same with anti-aliasing: the cube variant spills at 5 CTAs (48 registers)
 #endif
 constexpr int kResolveTileW = 32, kResolveTileH = 8;  // API pixels per k_resolve CTA (256 threads, 8 x 4 per warp)
 constexpr uint32_t kStageBytes = 32 * 1024;  // shared memory of a k_resolve CTA for staged texture cubes
@@ -101,6 +108,8 @@ struct FwdParams {
     int Ht, Wt;
     // NR_TEX_MIPMAP (appended likewise): `textures` is the packed pyramid, img_bstride its floats per item
     nr::MipTable mip;
+    // smooth shading (appended likewise): corner_light [B,F,3,3], or nullptr
+    const float* corner_light;
 };
 
 // rasterize.py:291-292  xp = (2 * xi + 1 - is) / is evaluated in double and rounded to float.  Both operands are
@@ -444,8 +453,9 @@ __device__ __forceinline__ int face_cube(const FwdParams& p, int fn, bool& rev) 
 
 // one pixel, every texel straight from global memory (anti-aliased quads, texture sizes the bulk copy cannot stage);
 // kUV: bilinear sample of the texture image at the pixel's perspective-correct UV instead of the ts^3 cube; kMip:
-// trilinear sample of its mip pyramid at the pixel's level of detail
-template <bool kLit, bool kUV = false, bool kMip = false>
+// trilinear sample of its mip pyramid at the pixel's level of detail.  kLight: 0 = unlit, 1 = face_light multiplies every
+// texel, 2 = corner_light interpolated to the pixel multiplies the unlit sample
+template <int kLight, bool kUV = false, bool kMip = false>
 __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigned long long key, int xi, int yi, float bgr,
                                               float bgg, float bgb) {
     Shaded o;
@@ -471,18 +481,18 @@ __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigne
             nr::load_face_uvs(p.uvs + ((uint32_t)b * p.uv_bstride + (uint32_t)uf * 6u), rev, uv);
             nr::pixel_uv(w, zp, cc.y, cc.z, cc.w, uv, u, v);
             float l0 = 1.0f, l1 = 1.0f, l2 = 1.0f;
-            if (kLit) {
+            if (kLight == 1) {
                 const float* lp = p.face_light + ((size_t)b * p.F + fn) * 3;
                 l0 = __ldg(lp); l1 = __ldg(lp + 1); l2 = __ldg(lp + 2);
             }
             float c[3];
             if constexpr (kMip) {
                 const float lod = nr::mip_lod(inv, w, zp, cc.y, cc.z, cc.w, uv, p.Ht, p.Wt, p.mip.levels);
-                nr::mip_blend<kLit>(p.textures + (uint32_t)b * p.img_bstride, p.mip, nr::mip_levels(lod, p.mip.levels), u, v,
-                                    l0, l1, l2, c);
+                nr::mip_blend<kLight == 1>(p.textures + (uint32_t)b * p.img_bstride, p.mip, nr::mip_levels(lod, p.mip.levels), u,
+                                           v, l0, l1, l2, c);
             } else {
                 const nr::UvTaps t = nr::uv_taps(u, v, p.Ht, p.Wt);
-                nr::uv_blend<kLit>(p.textures + (uint32_t)b * p.img_bstride, p.Wt, t, l0, l1, l2, c);
+                nr::uv_blend<kLight == 1>(p.textures + (uint32_t)b * p.img_bstride, p.Wt, t, l0, l1, l2, c);
             }
             o.r = c[0]; o.g = c[1]; o.b = c[2];
         } else {
@@ -493,7 +503,13 @@ __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigne
             bool rev;
             const int cube = face_cube(p, fn, rev);
             const float* tex = p.textures + ((size_t)b * p.tex_bstride + cube) * (size_t)(ts * ts * ts) * 3;
-            blend_corners<kLit>(p, tc, tex, rev, b, fn, o.r, o.g, o.b);
+            blend_corners<kLight == 1>(p, tc, tex, rev, b, fn, o.r, o.g, o.b);
+        }
+        if constexpr (kLight == 2) {  // smooth shading: the light interpolated with the pixel's l_k times the unlit sample
+            float l[3], L[3];
+            nr::perspective_weights(w, zp, cc.y, cc.z, cc.w, l);
+            nr::corner_light_at(p.corner_light + ((size_t)b * p.F + fn) * 9, l, L);
+            o.r = __fmul_rn(L[0], o.r); o.g = __fmul_rn(L[1], o.g); o.b = __fmul_rn(L[2], o.b);
         }
     }
     return o;
@@ -516,8 +532,8 @@ __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigne
 //
 // kTex == 2 (NR_TEX_UV): the direct variants with the texture-image sampler (shade_pixel<kLit, true>), same tile map.
 // kTex == 3 (NR_TEX_UV | NR_TEX_MIPMAP): the same with the trilinear pyramid sampler (shade_pixel<kLit, true, true>).
-template <bool kAA, int kTex, bool kLit>
-__global__ void __launch_bounds__(256, kTex == 3 ? NR_RESOLVE_MIP_MIN_CTAS : (kAA ? 5 : NR_RESOLVE_MIN_CTAS)) k_resolve(const __grid_constant__ FwdParams p, int nslots) {
+template <bool kAA, int kTex, int kLight>
+__global__ void __launch_bounds__(256, kTex == 3 ? NR_RESOLVE_MIP_MIN_CTAS : (kLight == 2 ? (kAA ? NR_RESOLVE_SMOOTH_AA_MIN_CTAS : NR_RESOLVE_SMOOTH_MIN_CTAS) : (kAA ? 5 : NR_RESOLVE_MIN_CTAS))) k_resolve(const __grid_constant__ FwdParams p, int nslots) {
     constexpr bool kStage = kTex == 1;  // kTex: 0 = every texel straight from global memory, 1 = cubes staged with cp.async.bulk
     constexpr bool kUV = kTex >= 2;     //       2 = texture image through per-corner UVs, 3 = its mip pyramid
     constexpr bool kMip = kTex == 3;
@@ -606,16 +622,16 @@ __global__ void __launch_bounds__(256, kTex == 3 ? NR_RESOLVE_MIP_MIN_CTAS : (kA
         float r, g, bl;
         if (staged) {
             mbar_wait(&s_bar, 0);
-            blend_corners<kLit>(p, tc, stex, rev, b, fn, r, g, bl);
+            blend_corners<kLight == 1>(p, tc, stex, rev, b, fn, r, g, bl);
         } else {
-            blend_corners<kLit>(p, tc, gtex, rev, b, fn, r, g, bl);
+            blend_corners<kLight == 1>(p, tc, gtex, rev, b, fn, r, g, bl);
         }
         rgb[o] = r; rgb[o + plane] = g; rgb[o + 2 * plane] = bl;
     } else if (!kAA) {
         // thread = one pixel of the IMAGE (row 0 = top): raster row yi = S - 1 - row
         const int row = row2, yi = S - 1 - row;
         if (col >= S || row >= S) return;
-        const Shaded s = shade_pixel<kLit, kUV, kMip>(p, b, __ldg(zb + (uint32_t)yi * S + col), col, yi, bgr, bgg, bgb);
+        const Shaded s = shade_pixel<kLight, kUV, kMip>(p, b, __ldg(zb + (uint32_t)yi * S + col), col, yi, bgr, bgg, bgb);
         const uint32_t o = (uint32_t)row * S + col;
         // streaming stores: 134 MB of maps that nothing reads again before the backward pass should not push the
         // z-buffer, the face records and the texture cubes out of the L2
@@ -637,7 +653,7 @@ __global__ void __launch_bounds__(256, kTex == 3 ? NR_RESOLVE_MIP_MIN_CTAS : (kA
         for (int k = 0; k < 4; k++) {
             const int row = 2 * orow + (k >> 1), xi = 2 * col + (k & 1);
             const int yi = S - 1 - row;
-            const Shaded s = shade_pixel<kLit, kUV, kMip>(p, b, __ldg(zb + (uint32_t)yi * S + xi), xi, yi, bgr, bgg, bgb);
+            const Shaded s = shade_pixel<kLight, kUV, kMip>(p, b, __ldg(zb + (uint32_t)yi * S + xi), xi, yi, bgr, bgg, bgb);
             const uint32_t o = (uint32_t)row * S + xi;
             __stcs(fim + o, s.fim);
             __stcs(dmap + o, s.depth);
@@ -690,9 +706,17 @@ extern "C" size_t nr_b200_forward_workspace_bytes(int32_t B, int32_t F, int32_t 
     return fwd_layout(B, F, S).total;
 }
 
-extern "C" int nr_b200_forward(const nr_b200_forward_args* a, void* cuda_stream) {
+extern "C" int nr_b200_forward(const nr_b200_forward_args* args, void* cuda_stream) {
     nr_internal::launch_count() = 0;
-    if (!a || a->struct_size != sizeof(nr_b200_forward_args)) return NR_ERR_INVALID_ARG;
+    // Two layouts: the full struct, and the ABI-4 struct from before corner_light (which then reads as NULL).  Only the
+    // caller's struct_size bytes are read.
+    if (!args) return NR_ERR_INVALID_ARG;
+    const uint32_t size = args->struct_size;
+    if (size != sizeof(nr_b200_forward_args) && size != offsetof(nr_b200_forward_args, corner_light)) return NR_ERR_INVALID_ARG;
+    nr_b200_forward_args args_copy;
+    memset(&args_copy, 0, sizeof(args_copy));
+    memcpy(&args_copy, args, size);
+    const nr_b200_forward_args* a = &args_copy;
     const int B = a->batch_size, F = a->num_faces, S = a->raster_size, ts = a->texture_size;
     const uint32_t flags = a->flags;
     if (B <= 0 || F <= 0 || S <= 0) return NR_ERR_INVALID_ARG;
@@ -709,6 +733,8 @@ extern "C" int nr_b200_forward(const nr_b200_forward_args* a, void* cuda_stream)
     if (uv && (!(flags & NR_RETURN_RGB) || !a->face_uvs || a->texture_height < 1 || a->texture_width < 1)) return NR_ERR_INVALID_ARG;
     const bool mip = (flags & NR_TEX_MIPMAP) != 0;
     if (mip && !uv) return NR_ERR_INVALID_ARG;
+    const bool smooth = a->corner_light != nullptr;  // per-corner light: only for RGB, and instead of face_light
+    if (smooth && (!(flags & NR_RETURN_RGB) || a->face_light)) return NR_ERR_INVALID_ARG;
     if ((flags & NR_ANTI_ALIASING) && (S & 1)) return NR_ERR_INVALID_ARG;
     if (S > 32767 || B > 65535) return NR_ERR_UNSUPPORTED;  // 32-bit pixel offsets; batch = grid.z of the resolve pass
     // NR_TEX_UV: image (NR_TEX_MIPMAP: pyramid) and UV offsets are 32-bit in the kernels
@@ -730,6 +756,7 @@ extern "C" int nr_b200_forward(const nr_b200_forward_args* a, void* cuda_stream)
     p.tex_bstride = (flags & NR_TEX_SHARED) ? 0 : ((flags & NR_TEX_FILL_BACK) ? (size_t)F / 2 : (size_t)F);
     p.textures = a->textures; p.bg_batch = a->background_batch;
     p.face_light = (flags & NR_RETURN_RGB) ? a->face_light : nullptr;
+    p.corner_light = a->corner_light;
     p.big_cnt = (int*)(wsb + L.off_cnt);
     p.work_next = p.big_cnt + B;
     p.any_big = p.big_cnt + B + 1;
@@ -797,9 +824,9 @@ extern "C" int nr_b200_forward(const nr_b200_forward_args* a, void* cuda_stream)
         // Staging whole cubes with cp.async.bulk needs 16-byte aligned, 16-byte sized cubes; up to kStageBytes of
         // shared memory per CTA hold the cubes of the row's runs (the rest of the runs read global memory)
         const bool aa = (flags & NR_ANTI_ALIASING) != 0;
-        const bool lit = p.face_light != nullptr;
+        const int light = smooth ? 2 : (p.face_light != nullptr ? 1 : 0);
         const uint32_t cube_bytes = (flags & NR_RETURN_RGB) ? (uint32_t)(ts * ts * ts) * 12u : 0u;
-        const bool stage = !uv && (flags & NR_FWD_STAGE_TEXTURES) && !aa && (flags & NR_RETURN_RGB) && (cube_bytes % 16u) == 0 &&
+        const bool stage = !uv && !smooth && (flags & NR_FWD_STAGE_TEXTURES) && !aa && (flags & NR_RETURN_RGB) && (cube_bytes % 16u) == 0 &&
                            cube_bytes <= kStageBytes / 8 && ((uintptr_t)a->textures & 15) == 0;
         int nslots = 0;
         size_t smem = 0;
@@ -813,7 +840,12 @@ extern "C" int nr_b200_forward(const nr_b200_forward_args* a, void* cuda_stream)
         if (optin.ensure(k_resolve<AA, TEX, LIT>, smem) != cudaSuccess) return NR_ERR_CUDA;         \
         k_resolve<AA, TEX, LIT><<<grid, bx, smem, stream>>>(p, nslots);                             \
     } while (0)
-#define NR_RESOLVE_LIT(AA, TEX) do { if (lit) NR_RESOLVE(AA, TEX, true); else NR_RESOLVE(AA, TEX, false); } while (0)
+#define NR_RESOLVE_LIT(AA, TEX)                                                                    \
+    do {                                                                                            \
+        if (light == 2) NR_RESOLVE(AA, TEX, 2);                                                     \
+        else if (light == 1) NR_RESOLVE(AA, TEX, 1);                                                \
+        else NR_RESOLVE(AA, TEX, 0);                                                                \
+    } while (0)
         if (!stage && !aa) {  // direct variant: 32 x 8 pixel tiles
             bx = 256;
             grid = dim3((width + kResolveTileW - 1) / kResolveTileW, (width + kResolveTileH - 1) / kResolveTileH, B);
@@ -823,7 +855,8 @@ extern "C" int nr_b200_forward(const nr_b200_forward_args* a, void* cuda_stream)
         else if (uv && aa) NR_RESOLVE_LIT(true, 2);
         else if (uv) NR_RESOLVE_LIT(false, 2);
         else if (aa) NR_RESOLVE_LIT(true, 0);
-        else if (stage) NR_RESOLVE_LIT(false, 1);
+        else if (stage && light == 1) NR_RESOLVE(false, 1, 1);
+        else if (stage) NR_RESOLVE(false, 1, 0);
         else NR_RESOLVE_LIT(false, 0);
 #undef NR_RESOLVE_LIT
 #undef NR_RESOLVE

@@ -14,11 +14,17 @@
 // face indices (no gathered [B,F,3,3] tensor), and its backward as a scatter-add into the vertex gradient.  The
 // factor itself is applied inside the rasterizer's sampler (nr_b200_forward_args.face_light).
 //
+// Smooth shading (include/nr_b200.h): area-weighted vertex normals and the per-corner Lambertian light the rasterizer
+// interpolates (nr_b200_forward_args.corner_light).  The normal sums are deterministic: the corners are stable-sorted by
+// vertex (cub radix sort) and every vertex adds its corners' face normals in ascending (face, corner) order.
+//
 // Texture baking (SURVEY.md section 8(f), rank 4): the bilinear image -> per-face ts^3 cube resampling kernel of
 // load_obj.py:88-137, operation for operation (including its NaN at texel (0,0,0), where the three barycentric
 // coordinates are 0/0).
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include <cub/device/device_radix_sort.cuh>
 
 #include "nr_b200.h"
 #include "nr_internal.h"
@@ -250,6 +256,180 @@ __global__ void __launch_bounds__(256) k_face_light_bwd(const float* __restrict_
 }
 
 
+// ------------------------------------------------------------------------------------------- smooth shading
+// sort keys of the vertex-normal adjacency: corner i = f*3 + k of index-set item `item` -> key item * (Nv + 1) + vertex
+// (Nv for an index outside [0, Nv): sorted past every vertex, never gathered), value = i
+__global__ void __launch_bounds__(256) k_vn_keys(const int32_t* __restrict__ faces, int Nv, long long n_corners_per_item,
+                                                 uint32_t* __restrict__ keys, int32_t* __restrict__ vals) {
+    const int item = blockIdx.y;
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_corners_per_item) return;
+    const size_t o = (size_t)item * n_corners_per_item + i;
+    const int idx = __ldg(faces + o);
+    keys[o] = (uint32_t)item * (uint32_t)(Nv + 1) + ((unsigned)idx < (unsigned)Nv ? (uint32_t)idx : (uint32_t)Nv);
+    vals[o] = (int32_t)i;
+}
+
+__device__ __forceinline__ uint32_t lower_bound_u32(const uint32_t* a, uint32_t n, uint32_t key) {
+    uint32_t lo = 0, hi = n;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (__ldg(a + mid) < key) lo = mid + 1; else hi = mid;
+    }
+    return lo;
+}
+
+// n_v = s_v / (|s_v| + 1e-5), s_v = sum of the face normals c_f (face_geom) of v's corners in the sorted (= ascending
+// corner) order: one thread per vertex of every batch item
+__global__ void __launch_bounds__(256) k_vn_gather(const float* __restrict__ vertices, const int32_t* __restrict__ faces,
+                                                   const uint32_t* __restrict__ keys, const int32_t* __restrict__ vals,
+                                                   uint32_t n_keys, int Nv, int Nf, uint32_t flags, float* __restrict__ normals) {
+    const int b = blockIdx.y;
+    const int v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= Nv) return;
+    const uint32_t key = (uint32_t)((flags & NR_INDICES_SHARED) ? 0 : b) * (uint32_t)(Nv + 1) + (uint32_t)v;
+    const uint32_t lo = lower_bound_u32(keys, n_keys, key), hi = lower_bound_u32(keys, n_keys, key + 1);
+    float s0 = 0.0f, s1 = 0.0f, s2 = 0.0f;
+    for (uint32_t j = lo; j < hi; j++) {
+        const FaceGeom G = face_geom(vertices, faces, b, Nv, Nf, __ldg(vals + j) / 3, flags);
+        s0 += G.c[0]; s1 += G.c[1]; s2 += G.c[2];
+    }
+    const float inv = 1.0f / (sqrtf((s0 * s0 + s1 * s1) + s2 * s2) + 1e-5f);
+    float* o = normals + ((size_t)b * Nv + v) * 3;
+    o[0] = s0 * inv; o[1] = s1 * inv; o[2] = s2 * inv;
+}
+
+// backward, step 1: s_v again, with atomics (the backward is not bit-pinned)
+__global__ void __launch_bounds__(256) k_vn_sums(const float* __restrict__ vertices, const int32_t* __restrict__ faces, int Nv,
+                                                 int Nf, uint32_t flags, float* __restrict__ sums) {
+    const int b = blockIdx.y;
+    const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= Nf) return;
+    const FaceGeom G = face_geom(vertices, faces, b, Nv, Nf, f, flags);
+    if (!G.ok) return;
+    const int idx[3] = {G.i0, G.i1, G.i2};
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        float* q = sums + ((size_t)b * Nv + idx[k]) * 3;
+        atomicAdd(q, G.c[0]); atomicAdd(q + 1, G.c[1]); atomicAdd(q + 2, G.c[2]);
+    }
+}
+
+// step 2, per face: g_c = sum over its corners of d n / d s (at s_v) applied to d loss / d n_v, then through c = a x b
+// as in k_face_light_bwd
+__global__ void __launch_bounds__(256) k_vn_bwd(const float* __restrict__ vertices, const int32_t* __restrict__ faces,
+                                                const float* __restrict__ sums, const float* __restrict__ grad_normals, int Nv,
+                                                int Nf, uint32_t flags, float* __restrict__ grad_vertices) {
+    const int b = blockIdx.y;
+    const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= Nf) return;
+    const FaceGeom G = face_geom(vertices, faces, b, Nv, Nf, f, flags);
+    if (!G.ok) return;
+    const int idx[3] = {G.i0, G.i1, G.i2};
+    float gc[3] = {0.0f, 0.0f, 0.0f};
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        const float* q = sums + ((size_t)b * Nv + idx[k]) * 3;
+        const float* g = grad_normals + ((size_t)b * Nv + idx[k]) * 3;
+        const float sv[3] = {q[0], q[1], q[2]}, gn[3] = {__ldg(g), __ldg(g + 1), __ldg(g + 2)};
+        // n = s / (len + eps):  g_s = g_n / (len + eps) - s (s . g_n) / (len (len + eps)^2)
+        const float len = sqrtf((sv[0] * sv[0] + sv[1] * sv[1]) + sv[2] * sv[2]);
+        const float inv = 1.0f / (len + 1e-5f);
+        const float sg = (sv[0] * gn[0] + sv[1] * gn[1]) + sv[2] * gn[2];
+        const float k2 = len > 0.0f ? sg * inv * inv / len : 0.0f;
+#pragma unroll
+        for (int j = 0; j < 3; j++) gc[j] += gn[j] * inv - sv[j] * k2;
+    }
+    const float ga[3] = {G.b[1] * gc[2] - G.b[2] * gc[1], G.b[2] * gc[0] - G.b[0] * gc[2], G.b[0] * gc[1] - G.b[1] * gc[0]};
+    const float gb[3] = {gc[1] * G.a[2] - gc[2] * G.a[1], gc[2] * G.a[0] - gc[0] * G.a[2], gc[0] * G.a[1] - gc[1] * G.a[0]};
+    float* g0 = grad_vertices + ((size_t)b * Nv + G.i0) * 3;
+    float* g1 = grad_vertices + ((size_t)b * Nv + G.i1) * 3;
+    float* g2 = grad_vertices + ((size_t)b * Nv + G.i2) * 3;
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        atomicAdd(g0 + k, ga[k]);
+        atomicAdd(g2 + k, gb[k]);
+        atomicAdd(g1 + k, -(ga[k] + gb[k]));
+    }
+}
+
+// corner_light[b,f,k,:] = ambient + directional * max(sgn * (n . direction), 0), n = the corner's vertex normal
+__global__ void __launch_bounds__(256) k_corner_light_fwd(const float* __restrict__ normals, const int32_t* __restrict__ faces,
+                                                          const float* __restrict__ params, int Nv, int Nf, uint32_t flags,
+                                                          float* __restrict__ light) {
+    const int b = blockIdx.y;
+    const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= Nf) return;
+    const LightItem L = load_light(params, (flags & NR_CAM_SHARED) ? 0 : b);
+    const int32_t* fi = faces + ((size_t)((flags & NR_INDICES_SHARED) ? 0 : b) * Nf + f) * 3;
+    const bool rev = (flags & NR_TEX_FILL_BACK) && f >= (Nf >> 1);  // reversed copy: its face normal is -n
+    float* o = light + ((size_t)b * Nf + f) * 9;
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        const int idx = __ldg(fi + k);
+        float n[3] = {0.0f, 0.0f, 0.0f};
+        if ((unsigned)idx < (unsigned)Nv) {
+            const float* q = normals + ((size_t)b * Nv + idx) * 3;
+            n[0] = __ldg(q); n[1] = __ldg(q + 1); n[2] = __ldg(q + 2);
+        }
+        const float dot = (n[0] * L.dir[0] + n[1] * L.dir[1]) + n[2] * L.dir[2];
+        const float cosv = fmaxf(rev ? -dot : dot, 0.0f);
+#pragma unroll
+        for (int c = 0; c < 3; c++) o[3 * k + c] = L.amb[c] + L.dir_rgb[c] * cosv;
+    }
+}
+
+__global__ void __launch_bounds__(256) k_corner_light_bwd(const float* __restrict__ normals, const int32_t* __restrict__ faces,
+                                                          const float* __restrict__ params, const float* __restrict__ grad_light,
+                                                          int Nv, int Nf, uint32_t flags, float* __restrict__ grad_normals) {
+    const int b = blockIdx.y;
+    const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= Nf) return;
+    const LightItem L = load_light(params, (flags & NR_CAM_SHARED) ? 0 : b);
+    const int32_t* fi = faces + ((size_t)((flags & NR_INDICES_SHARED) ? 0 : b) * Nf + f) * 3;
+    const float sgn = ((flags & NR_TEX_FILL_BACK) && f >= (Nf >> 1)) ? -1.0f : 1.0f;
+    const float* g = grad_light + ((size_t)b * Nf + f) * 9;
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        const int idx = __ldg(fi + k);
+        if ((unsigned)idx >= (unsigned)Nv) continue;
+        const float* q = normals + ((size_t)b * Nv + idx) * 3;
+        const float dot = (__ldg(q) * L.dir[0] + __ldg(q + 1) * L.dir[1]) + __ldg(q + 2) * L.dir[2];
+        if (!(sgn * dot > 0.0f)) continue;  // relu
+        const float gcos = (__ldg(g + 3 * k) * L.dir_rgb[0] + __ldg(g + 3 * k + 1) * L.dir_rgb[1]) + __ldg(g + 3 * k + 2) * L.dir_rgb[2];
+        if (gcos == 0.0f) continue;
+        float* o = grad_normals + ((size_t)b * Nv + idx) * 3;
+        atomicAdd(o, sgn * gcos * L.dir[0]); atomicAdd(o + 1, sgn * gcos * L.dir[1]); atomicAdd(o + 2, sgn * gcos * L.dir[2]);
+    }
+}
+
+struct VnLayout {
+    size_t n;  // corners of the index set (items x 3 Nf)
+    int end_bit;
+    size_t off_keys_out, off_vals_in, off_vals_out, off_temp, temp_bytes, total;
+};
+inline size_t align256(size_t x) { return (x + 255) / 256 * 256; }
+// workspace = sort keys in | keys out | values in | values out | cub scratch; the backward uses the first B Nv 3 floats
+bool vn_layout(int B, int Nv, int Nf, uint32_t flags, VnLayout* L) {
+    if (B <= 0 || Nv <= 0 || Nf <= 0 || B > 65535) return false;
+    const long long items = (flags & NR_INDICES_SHARED) ? 1 : B;
+    if (items * ((long long)Nv + 1) > 0x7FFFFFFFll || 3ll * Nf > 0x7FFFFFFFll || items * 3ll * Nf > 0x7FFFFFFFll) return false;
+    L->n = (size_t)(items * 3ll * Nf);
+    const uint32_t max_key = (uint32_t)(items * ((long long)Nv + 1) - 1);
+    L->end_bit = 1;
+    while (L->end_bit < 32 && (max_key >> L->end_bit) != 0) L->end_bit++;
+    L->temp_bytes = 0;
+    if (cub::DeviceRadixSort::SortPairs(nullptr, L->temp_bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr,
+                                        (const int32_t*)nullptr, (int32_t*)nullptr, (int)L->n, 0, L->end_bit) != cudaSuccess)
+        return false;
+    const size_t a = align256(L->n * 4);
+    L->off_keys_out = a; L->off_vals_in = 2 * a; L->off_vals_out = 3 * a; L->off_temp = 4 * a;
+    L->total = L->off_temp + align256(L->temp_bytes);
+    const size_t bwd = align256((size_t)B * Nv * 3 * sizeof(float));
+    if (bwd > L->total) L->total = bwd;
+    return true;
+}
+
 // load_obj.py:97-131.  One thread per texel of every face.  Arithmetic as the reference build evaluates it (read from
 // its SASS): dims = (float)((double)k / (ts - 1.)), normalised by IEEE division with sum = (d0 + d1) + d2;
 // pos = fma(f2, d2, fma(f0, d0, f1 * d1)) * (size - 1); taps blended as fma chains in source order.
@@ -388,6 +568,107 @@ extern "C" int nr_b200_face_lighting_backward(const float* vertices, const int32
         nr_internal::LaunchScope ls("k_face_light_bwd", stream);
         k_face_light_bwd<<<dim3((unsigned)((Nf + 255) / 256), B), 256, 0, stream>>>(vertices, faces, light_params, grad_face_light,
                                                                                    Nv, Nf, flags, grad_vertices);
+    }
+    return cudaGetLastError() == cudaSuccess ? NR_OK : NR_ERR_CUDA;
+}
+
+extern "C" size_t nr_b200_vertex_normals_workspace_bytes(int32_t B, int32_t Nv, int32_t Nf, uint32_t flags) {
+    VnLayout L;
+    return vn_layout(B, Nv, Nf, flags, &L) ? L.total : 0;
+}
+
+extern "C" int nr_b200_vertex_normals(const float* vertices, const int32_t* faces, int32_t B, int32_t Nv, int32_t Nf,
+                                      uint32_t flags, float* normals, void* workspace, size_t workspace_bytes,
+                                      void* cuda_stream) {
+    nr_internal::launch_count() = 0;
+    if (!vertices || !faces || !normals || B <= 0 || Nv <= 0 || Nf <= 0 || B > 65535) return NR_ERR_INVALID_ARG;
+    VnLayout L;
+    if (!vn_layout(B, Nv, Nf, flags, &L)) return NR_ERR_UNSUPPORTED;
+    if (!workspace || workspace_bytes < L.total || ((uintptr_t)workspace & 15)) return NR_ERR_WORKSPACE;
+    cudaStream_t stream = (cudaStream_t)cuda_stream;
+    char* w = (char*)workspace;
+    uint32_t* keys_in = (uint32_t*)w;
+    uint32_t* keys_out = (uint32_t*)(w + L.off_keys_out);
+    int32_t* vals_in = (int32_t*)(w + L.off_vals_in);
+    int32_t* vals_out = (int32_t*)(w + L.off_vals_out);
+    const int items = (flags & NR_INDICES_SHARED) ? 1 : B;
+    const long long n = 3ll * Nf;
+    {
+        nr_internal::LaunchScope ls("k_vn_keys", stream);
+        k_vn_keys<<<dim3((unsigned)((n + 255) / 256), items), 256, 0, stream>>>(faces, Nv, n, keys_in, vals_in);
+    }
+    {
+        nr_internal::LaunchScope ls("vn_sort", stream);  // stable: equal vertices keep ascending corner order
+        size_t temp = L.temp_bytes;
+        if (cub::DeviceRadixSort::SortPairs(w + L.off_temp, temp, keys_in, keys_out, vals_in, vals_out, (int)L.n, 0, L.end_bit,
+                                            stream) != cudaSuccess)
+            return NR_ERR_CUDA;
+    }
+    {
+        nr_internal::LaunchScope ls("k_vn_gather", stream);
+        k_vn_gather<<<dim3((unsigned)((Nv + 255) / 256), B), 256, 0, stream>>>(vertices, faces, keys_out, vals_out, (uint32_t)L.n,
+                                                                             Nv, Nf, flags, normals);
+    }
+    return cudaGetLastError() == cudaSuccess ? NR_OK : NR_ERR_CUDA;
+}
+
+extern "C" int nr_b200_vertex_normals_backward(const float* vertices, const int32_t* faces, const float* grad_normals, int32_t B,
+                                               int32_t Nv, int32_t Nf, uint32_t flags, float* grad_vertices, void* workspace,
+                                               size_t workspace_bytes, void* cuda_stream) {
+    nr_internal::launch_count() = 0;
+    if (!vertices || !faces || !grad_normals || !grad_vertices || B <= 0 || Nv <= 0 || Nf <= 0 || B > 65535)
+        return NR_ERR_INVALID_ARG;
+    VnLayout L;
+    if (!vn_layout(B, Nv, Nf, flags, &L)) return NR_ERR_UNSUPPORTED;
+    if (!workspace || workspace_bytes < L.total || ((uintptr_t)workspace & 15)) return NR_ERR_WORKSPACE;
+    cudaStream_t stream = (cudaStream_t)cuda_stream;
+    float* sums = (float*)workspace;
+    if (cudaMemsetAsync(sums, 0, (size_t)B * Nv * 3 * sizeof(float), stream) != cudaSuccess) return NR_ERR_CUDA;
+    if (!(flags & NR_GRAD_ACCUMULATE) &&
+        cudaMemsetAsync(grad_vertices, 0, (size_t)B * Nv * 3 * sizeof(float), stream) != cudaSuccess)
+        return NR_ERR_CUDA;
+    const dim3 grid((unsigned)((Nf + 255) / 256), B);
+    {
+        nr_internal::LaunchScope ls("k_vn_sums", stream);
+        k_vn_sums<<<grid, 256, 0, stream>>>(vertices, faces, Nv, Nf, flags, sums);
+    }
+    {
+        nr_internal::LaunchScope ls("k_vn_bwd", stream);
+        k_vn_bwd<<<grid, 256, 0, stream>>>(vertices, faces, sums, grad_normals, Nv, Nf, flags, grad_vertices);
+    }
+    return cudaGetLastError() == cudaSuccess ? NR_OK : NR_ERR_CUDA;
+}
+
+extern "C" int nr_b200_corner_lighting(const float* normals, const int32_t* faces, const float* light_params, int32_t B,
+                                       int32_t Nv, int32_t Nf, uint32_t flags, float* corner_light, void* cuda_stream) {
+    nr_internal::launch_count() = 0;
+    if (!normals || !faces || !light_params || !corner_light || B <= 0 || Nv <= 0 || Nf <= 0 || B > 65535) return NR_ERR_INVALID_ARG;
+    if ((flags & NR_TEX_FILL_BACK) && (Nf & 1)) return NR_ERR_INVALID_ARG;
+    cudaStream_t stream = (cudaStream_t)cuda_stream;
+    {
+        nr_internal::LaunchScope ls("k_corner_light_fwd", stream);
+        k_corner_light_fwd<<<dim3((unsigned)((Nf + 255) / 256), B), 256, 0, stream>>>(normals, faces, light_params, Nv, Nf, flags,
+                                                                                     corner_light);
+    }
+    return cudaGetLastError() == cudaSuccess ? NR_OK : NR_ERR_CUDA;
+}
+
+extern "C" int nr_b200_corner_lighting_backward(const float* normals, const int32_t* faces, const float* light_params,
+                                                const float* grad_corner_light, int32_t B, int32_t Nv, int32_t Nf,
+                                                uint32_t flags, float* grad_normals, void* cuda_stream) {
+    nr_internal::launch_count() = 0;
+    if (!normals || !faces || !light_params || !grad_corner_light || !grad_normals || B <= 0 || Nv <= 0 || Nf <= 0 || B > 65535)
+        return NR_ERR_INVALID_ARG;
+    if ((flags & NR_TEX_FILL_BACK) && (Nf & 1)) return NR_ERR_INVALID_ARG;
+    cudaStream_t stream = (cudaStream_t)cuda_stream;
+    if (!(flags & NR_GRAD_ACCUMULATE) &&
+        cudaMemsetAsync(grad_normals, 0, (size_t)B * Nv * 3 * sizeof(float), stream) != cudaSuccess)
+        return NR_ERR_CUDA;
+    {
+        nr_internal::LaunchScope ls("k_corner_light_bwd", stream);
+        k_corner_light_bwd<<<dim3((unsigned)((Nf + 255) / 256), B), 256, 0, stream>>>(normals, faces, light_params,
+                                                                                     grad_corner_light, Nv, Nf, flags,
+                                                                                     grad_normals);
     }
     return cudaGetLastError() == cudaSuccess ? NR_OK : NR_ERR_CUDA;
 }

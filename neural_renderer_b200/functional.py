@@ -11,6 +11,10 @@ test oracle of those kernels.  `Renderer` goes one step further and hands vertic
   perspective             perspective.py:5-19   (pi is 3.1416 there, kept)
   lighting                lighting.py:8-52
   vertices_to_faces       vertices_to_faces.py:4-21
+
+Not in the reference: smooth (Gouraud) shading -- `vertex_normals` (area weighted) and `corner_light`, the Lambertian
+light of lighting.py evaluated at every face corner with its vertex normal, which the rasterizer interpolates across the
+face (rasterize(..., corner_light=...)).
 """
 from __future__ import annotations
 
@@ -431,3 +435,193 @@ def vertices_to_faces(vertices, faces):
         return _VerticesToFaces.apply(vertices, faces.to(torch.int32).contiguous())
     idx = faces.long() + (torch.arange(bs, device=faces.device, dtype=torch.long) * nv)[:, None, None]
     return vertices.reshape(bs * nv, 3)[idx]
+
+
+def _light_params(intensity_ambient, intensity_directional, color_ambient, color_directional, direction, device):
+    """light_params [1,9] of the CUDA light kernels (cached per value), or None for tensor-valued / batched parameters."""
+    if not _is_plain(intensity_ambient, intensity_directional, color_ambient, color_directional, direction):
+        return None
+    import numpy as np
+    ca, cd, d = (np.asarray(x, dtype=np.float32) for x in (color_ambient, color_directional, direction))
+    if ca.ndim != 1 or cd.ndim != 1 or d.ndim != 1:
+        return None
+    key = ("light", float(intensity_ambient), float(intensity_directional), tuple(ca.tolist()), tuple(cd.tolist()),
+           tuple(d.tolist()), str(device))
+    params = _CAMERA_CACHE.get(key)
+    if params is None:
+        row = np.concatenate([np.float32(intensity_ambient) * ca, np.float32(intensity_directional) * cd, d]).astype(np.float32)
+        params = _cache_put(key, torch.from_numpy(row[None]).to(device))
+    return params
+
+
+def _index_set(faces, batch_size):
+    """faces [F,3] / [1|B,F,3] (an expanded shared set stays shared) -> (int32 [1|B,F,3], shared)"""
+    if faces.dim() == 2:
+        faces = faces[None]
+    if faces.shape[0] > 1 and faces.stride(0) == 0:
+        faces = faces[:1]
+    if faces.shape[0] not in (1, batch_size):
+        raise ValueError("faces must have shape [num faces, 3] or [batch size, num faces, 3]")
+    return faces.to(torch.int32).contiguous(), faces.shape[0] == 1 and batch_size != 1
+
+
+def _gather_vertices(values, faces):
+    """values [B,Nv,3], faces [1|B,F,3] -> [B,F,3,3] (zeros for indices outside [0, Nv)) and the in-range mask [B,F,3]"""
+    bs, nv = values.shape[:2]
+    idx = faces.long().expand(bs, -1, -1)
+    ok = (idx >= 0) & (idx < nv)
+    flat = (idx.clamp(0, nv - 1) + (torch.arange(bs, device=values.device) * nv)[:, None, None])
+    return values.reshape(bs * nv, 3)[flat] * ok[..., None].to(values.dtype), ok
+
+
+def _vertex_normals_torch(vertices, faces):
+    bs, nv = vertices.shape[:2]
+    faces = faces[None] if faces.dim() == 2 else faces
+    v, ok = _gather_vertices(vertices, faces)
+    face_ok = ok.all(dim=2)
+    c = torch.linalg.cross(v[:, :, 0] - v[:, :, 1], v[:, :, 2] - v[:, :, 1], dim=2) * face_ok[..., None].to(v.dtype)
+    idx = faces.long().expand(bs, -1, -1)
+    corner_ok = (idx >= 0) & (idx < nv)
+    target = (idx.clamp(0, nv - 1) + (torch.arange(bs, device=vertices.device) * nv)[:, None, None])
+    contrib = c[:, :, None, :].expand(-1, -1, 3, -1) * corner_ok[..., None].to(c.dtype)
+    s = torch.zeros((bs * nv, 3), dtype=vertices.dtype, device=vertices.device)
+    s = s.index_add(0, target.reshape(-1), contrib.reshape(-1, 3)).reshape(bs, nv, 3)
+    return s / (s.norm(dim=2, keepdim=True) + 1e-5)
+
+
+class _VertexNormals(torch.autograd.Function):
+    """vertex normals [B,Nv,3] from vertices and an index set (nr_b200_vertex_normals*); faces_i32 [1|B,F,3]."""
+
+    @staticmethod
+    def forward(ctx, vertices, faces_i32, shared):
+        import ctypes
+        from . import _lib
+        lib = _lib.load()
+        v = vertices.detach().contiguous()
+        bs, nv = v.shape[:2]
+        nf = faces_i32.shape[1]
+        flags = _lib.NR_INDICES_SHARED if shared else 0
+        out = torch.empty_like(v)
+        with torch.cuda.device(v.device):
+            ws_bytes = lib.nr_b200_vertex_normals_workspace_bytes(bs, nv, nf, flags)
+            if ws_bytes == 0:
+                raise RuntimeError("nr_b200: vertex normals of this size are not supported")
+            ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=v.device)
+            stream = ctypes.c_void_p(torch.cuda.current_stream(v.device).cuda_stream)
+            _lib.check(lib.nr_b200_vertex_normals(v.data_ptr(), faces_i32.data_ptr(), bs, nv, nf, flags, out.data_ptr(),
+                                                  ws.data_ptr(), ws_bytes, stream))
+        ctx.save_for_backward(v, faces_i32)
+        ctx.flags = flags
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_normals):
+        import ctypes
+        from . import _lib
+        lib = _lib.load()
+        v, faces_i32 = ctx.saved_tensors
+        g = grad_normals.detach().to(torch.float32).contiguous()
+        bs, nv = v.shape[:2]
+        nf = faces_i32.shape[1]
+        grad_v = torch.empty_like(v)
+        with torch.cuda.device(v.device):
+            ws_bytes = lib.nr_b200_vertex_normals_workspace_bytes(bs, nv, nf, ctx.flags)
+            ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=v.device)
+            stream = ctypes.c_void_p(torch.cuda.current_stream(v.device).cuda_stream)
+            _lib.check(lib.nr_b200_vertex_normals_backward(v.data_ptr(), faces_i32.data_ptr(), g.data_ptr(), bs, nv, nf,
+                                                           ctx.flags, grad_v.data_ptr(), ws.data_ptr(), ws_bytes, stream))
+        return grad_v, None, None
+
+
+def vertex_normals(vertices, faces):
+    """Area-weighted vertex normals [B,Nv,3] of vertices [B,Nv,3] and faces [F,3] / [1|B,F,3] (integer indices):
+    s_v = sum of cross(v0 - v1, v2 - v1) over the faces at v (the face-normal direction of `face_light`), n_v = s_v /
+    (|s_v| + 1e-5).  A face with an index outside [0, Nv) contributes nothing; an unreferenced vertex gets 0.  Pass the
+    original faces, not the fill_back-doubled set.  One deterministic CUDA kernel pair for CUDA float32 tensors."""
+    assert vertices.dim() == 3 and vertices.shape[2] == 3
+    if _fused_camera_ok(vertices) and faces.is_cuda:
+        faces_i32, shared = _index_set(faces, vertices.shape[0])
+        return _VertexNormals.apply(vertices, faces_i32, shared)
+    return _vertex_normals_torch(vertices, faces)
+
+
+def _corner_light_torch(vertex_normals, faces, intensity_ambient, intensity_directional, color_ambient, color_directional,
+                        direction, fill_back):
+    bs, nv = vertex_normals.shape[:2]
+    faces = faces[None] if faces.dim() == 2 else faces
+    nf = faces.shape[1]
+    color_ambient, color_directional, direction = (_as_vec(x, vertex_normals) for x in (color_ambient, color_directional,
+                                                                                        direction))
+    color_ambient, color_directional, direction = (x[None, :].expand(bs, 3) if x.dim() == 1 else x
+                                                   for x in (color_ambient, color_directional, direction))
+    n, _ = _gather_vertices(vertex_normals, faces)  # [B,F,3 corners,3]
+    light = torch.zeros((bs, nf, 3, 3), dtype=vertex_normals.dtype, device=vertex_normals.device)
+    if intensity_ambient != 0:
+        light = light + (intensity_ambient * color_ambient)[:, None, None, :]
+    if intensity_directional != 0:
+        dot = (n * direction[:, None, None, :]).sum(dim=3)
+        if fill_back:
+            sign = torch.ones(nf, dtype=dot.dtype, device=dot.device)
+            sign[nf // 2:] = -1
+            dot = dot * sign[None, :, None]
+        light = light + (intensity_directional * color_directional)[:, None, None, :] * torch.relu(dot)[..., None]
+    return light
+
+
+class _CornerLighting(torch.autograd.Function):
+    """corner_light [B,F,3,3] from vertex normals (nr_b200_corner_lighting*); params [1,9]."""
+
+    @staticmethod
+    def forward(ctx, normals, faces_i32, params, flags):
+        import ctypes
+        from . import _lib
+        lib = _lib.load()
+        n = normals.detach().to(torch.float32).contiguous()
+        bs, nv = n.shape[:2]
+        nf = faces_i32.shape[1]
+        out = torch.empty((bs, nf, 3, 3), dtype=torch.float32, device=n.device)
+        with torch.cuda.device(n.device):
+            stream = ctypes.c_void_p(torch.cuda.current_stream(n.device).cuda_stream)
+            _lib.check(lib.nr_b200_corner_lighting(n.data_ptr(), faces_i32.data_ptr(), params.data_ptr(), bs, nv, nf, flags,
+                                                   out.data_ptr(), stream))
+        ctx.save_for_backward(n, faces_i32, params)
+        ctx.flags = flags
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_light):
+        import ctypes
+        from . import _lib
+        lib = _lib.load()
+        n, faces_i32, params = ctx.saved_tensors
+        g = grad_light.detach().to(torch.float32).contiguous()
+        bs, nv = n.shape[:2]
+        grad_n = torch.empty_like(n)
+        with torch.cuda.device(n.device):
+            stream = ctypes.c_void_p(torch.cuda.current_stream(n.device).cuda_stream)
+            _lib.check(lib.nr_b200_corner_lighting_backward(n.data_ptr(), faces_i32.data_ptr(), params.data_ptr(), g.data_ptr(),
+                                                            bs, nv, faces_i32.shape[1], ctx.flags, grad_n.data_ptr(), stream))
+        return grad_n, None, None, None
+
+
+def corner_light(vertex_normals, faces, intensity_ambient=0.5, intensity_directional=0.5, color_ambient=(1, 1, 1),
+                 color_directional=(1, 1, 1), direction=(0, 1, 0), fill_back=False):
+    """Per-corner RGB light factor [B,F,3,3] for rasterize(..., corner_light=...): the Lambertian light of `face_light`
+    with the normal of each corner's vertex, ambient + directional * relu(n . direction).  `faces` [F,3] / [1|B,F,3] is
+    the index set the rasterizer receives; with fill_back=True faces [F/2, F) are the reversed copies and use -n.  An
+    index outside [0, Nv) gets n = 0.  No gradient flows into the light parameters.  One CUDA kernel pair for CUDA float32
+    tensors with plain-number light parameters, the torch formulation otherwise."""
+    assert vertex_normals.dim() == 3 and vertex_normals.shape[2] == 3
+    nf = faces.shape[-2]
+    if fill_back and nf % 2:
+        raise ValueError("fill_back needs an even number of faces (front faces, then their reversed copies)")
+    params = _light_params(intensity_ambient, intensity_directional, color_ambient, color_directional, direction,
+                           vertex_normals.device) if (_fused_camera_ok(vertex_normals) and faces.is_cuda) else None
+    if params is None:
+        return _corner_light_torch(vertex_normals, faces, intensity_ambient, intensity_directional, color_ambient,
+                                   color_directional, direction, fill_back)
+    from . import _lib
+    faces_i32, shared = _index_set(faces, vertex_normals.shape[0])
+    flags = (_lib.NR_CAM_SHARED if vertex_normals.shape[0] != 1 else 0) | (_lib.NR_INDICES_SHARED if shared else 0) | \
+        (_lib.NR_TEX_FILL_BACK if fill_back else 0)
+    return _CornerLighting.apply(vertex_normals, faces_i32, params, flags)

@@ -60,7 +60,8 @@ def _ptr(t):
     return None if t is None else ctypes.c_void_p(t.data_ptr())
 
 
-def _check_inputs(faces, textures, return_rgb, face_light=None, textures_fill_back=False, vertices=None, face_uvs=None):
+def _check_inputs(faces, textures, return_rgb, face_light=None, textures_fill_back=False, vertices=None, face_uvs=None,
+                  corner_light=None):
     # rasterize.py:66-90 (chainer type_check) -> TypeError / ValueError with the same conditions
     if not isinstance(faces, torch.Tensor):
         raise TypeError("faces must be a torch.Tensor")
@@ -106,6 +107,17 @@ def _check_inputs(faces, textures, return_rgb, face_light=None, textures_fill_ba
         if not isinstance(face_light, torch.Tensor) or tuple(face_light.shape) != (batch_size, num_faces, 3):
             raise ValueError("face_light must have shape [batch size, num faces, 3]")
         if not face_light.is_cuda:
+            raise NotImplementedError("neural_renderer_b200 has no CPU implementation (inputs must be CUDA tensors)")
+    if corner_light is not None:
+        if face_light is not None:
+            raise ValueError("face_light and corner_light are exclusive: give one light factor")
+        if not return_rgb:
+            raise ValueError("corner_light lights the RGB image: it needs return_rgb")
+        if not isinstance(corner_light, torch.Tensor) or not corner_light.is_floating_point():
+            raise TypeError("corner_light must be a floating point torch.Tensor")
+        if tuple(corner_light.shape) != (batch_size, num_faces, 3, 3):
+            raise ValueError("corner_light must have shape [batch size, num faces, 3, 3], got %s" % (tuple(corner_light.shape),))
+        if not corner_light.is_cuda:
             raise NotImplementedError("neural_renderer_b200 has no CPU implementation (inputs must be CUDA tensors)")
     if not faces.is_cuda or (return_rgb and not textures.is_cuda) or (return_rgb and face_uvs is not None and not face_uvs.is_cuda):
         raise NotImplementedError("neural_renderer_b200 has no CPU implementation (inputs must be CUDA tensors)")
@@ -199,12 +211,13 @@ class _RasterizeFunction(torch.autograd.Function):
     the `Rasterize` object can look at them)."""
 
     @staticmethod
-    def forward(ctx, geom, textures, face_light, cfg, indices, face_uvs=None):
+    def forward(ctx, geom, textures, face_light, cfg, indices, face_uvs=None, corner_light=None):
         lib = _lib.load()
         dev = geom.device
         geom_c = geom.detach().contiguous()
         tex_c = textures.detach().contiguous() if textures is not None else None
         light_c = face_light.detach().to(torch.float32).contiguous() if face_light is not None else None
+        corner_c = corner_light.detach().to(torch.float32).contiguous() if corner_light is not None else None
         flags = cfg.flags
         if indices is not None:
             B, Nv = geom_c.shape[:2]
@@ -266,6 +279,7 @@ class _RasterizeFunction(torch.autograd.Function):
             a.workspace, a.workspace_bytes = _ptr(ws), ws_bytes
             a.face_light = _ptr(light_c)
             a.face_uvs, (a.texture_height, a.texture_width) = _ptr(uv_c), tex_hw
+            a.corner_light = _ptr(corner_c)
             _lib.check(lib.nr_b200_forward(ctypes.byref(a), _stream_ptr(dev)))
         ctx.cfg = cfg
         ctx.flags = flags
@@ -273,11 +287,12 @@ class _RasterizeFunction(torch.autograd.Function):
         ctx.F = F
         ctx.tex_shape = tuple(textures.shape) if textures is not None else None
         ctx.tex_hw = tex_hw
-        # the unlit textures are only needed again for d loss / d face_light and d loss / d face_uvs
+        # the unlit textures are only needed again for d loss / d face_light (corner_light) and d loss / d face_uvs
         need_light_grad = light_c is not None and ctx.needs_input_grad[2]
+        ctx.need_corner_grad = corner_c is not None and ctx.needs_input_grad[6]
         ctx.need_uv_grad = uv_c is not None and want_rgb and ctx.needs_input_grad[5]
-        need_tex = need_light_grad or ctx.need_uv_grad
-        ctx.save_for_backward(geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c if need_tex else None, indices, uv_c)
+        need_tex = need_light_grad or ctx.need_uv_grad or ctx.need_corner_grad
+        ctx.save_for_backward(geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c if need_tex else None, indices, uv_c, corner_c)
         if cfg.aa:
             rgb_o, alpha_o, depth_o = out_rgb, out_alpha, out_depth
         else:
@@ -290,7 +305,7 @@ class _RasterizeFunction(torch.autograd.Function):
         lib = _lib.load()
         cfg = ctx.cfg
         flags = ctx.flags
-        geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c, indices, uv_c = ctx.saved_tensors
+        geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c, indices, uv_c, corner_c = ctx.saved_tensors
         dev = geom_c.device
         B, F = geom_c.shape[0], ctx.F
         want_rgb = bool(flags & _lib.NR_RETURN_RGB)
@@ -308,6 +323,7 @@ class _RasterizeFunction(torch.autograd.Function):
             grad_textures = torch.empty(ctx.tex_shape, dtype=torch.float32, device=dev) if want_rgb else None
             grad_light = torch.empty_like(light_c) if (want_rgb and light_c is not None and ctx.needs_input_grad[2]) else None
             grad_uvs = torch.empty_like(uv_c) if ctx.need_uv_grad else None  # same layout as face_uvs: [1|B,F',3,2]
+            grad_corner = torch.empty_like(corner_c) if ctx.need_corner_grad else None
             ws_bytes = lib.nr_b200_backward_workspace_bytes(B, F, cfg.S, ctx.ts, flags)
             ws = torch.empty((max(ws_bytes, 16),), dtype=torch.uint8, device=dev)
             a = _lib.BackwardArgs()
@@ -328,20 +344,27 @@ class _RasterizeFunction(torch.autograd.Function):
             a.grad_face_uvs = _ptr(grad_uvs)  # filled by the texture half
             a.workspace, a.workspace_bytes = _ptr(ws), ws.numel()
             hook = _TEXTURE_GRAD_HOOK if (want_rgb and g_rgb is not None) else None
+
+            def call():
+                if corner_c is None:
+                    return lib.nr_b200_backward(ctypes.byref(a), _stream_ptr(dev))
+                # smooth shading: grad_corner_light is filled by the texture half
+                return lib.nr_b200_backward_corner_light(ctypes.byref(a), _ptr(corner_c), _ptr(grad_corner),
+                                                         _stream_ptr(dev))
             if hook is None:
                 a.flags = flags
-                _lib.check(lib.nr_b200_backward(ctypes.byref(a), _stream_ptr(dev)))
+                _lib.check(call())
             else:
                 # two halves: the texture gradient is complete (and may start its all-reduce on another stream)
                 # before the edge scan is even enqueued
                 a.flags = flags | _lib.NR_BWD_PART_TEXTURES
-                _lib.check(lib.nr_b200_backward(ctypes.byref(a), _stream_ptr(dev)))
+                _lib.check(call())
                 pending = hook(grad_textures)
                 a.flags = flags | _lib.NR_BWD_PART_FACES
-                _lib.check(lib.nr_b200_backward(ctypes.byref(a), _stream_ptr(dev)))
+                _lib.check(call())
                 if pending is not None:
                     pending.wait()
-        return grad_geom, grad_textures, grad_light, None, None, grad_uvs
+        return grad_geom, grad_textures, grad_light, None, None, grad_uvs, grad_corner
 
 
 class _MipPyramid(torch.autograd.Function):
@@ -378,12 +401,12 @@ TEXTURE_FILTERS = ('bilinear', 'trilinear')
 
 def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_color, return_rgb, return_alpha,
          return_depth, face_light=None, textures_fill_back=False, vertices=None, reference_exact=None, face_uvs=None,
-         texture_filter='bilinear'):
+         texture_filter='bilinear', corner_light=None):
     if texture_filter not in TEXTURE_FILTERS:
         raise ValueError("texture_filter must be one of %s, got %r" % (TEXTURE_FILTERS, texture_filter))
     if texture_filter == 'trilinear' and face_uvs is None:
         raise ValueError("texture_filter='trilinear' samples a texture image: it needs face_uvs")
-    _check_inputs(faces, textures, return_rgb, face_light, textures_fill_back, vertices, face_uvs)
+    _check_inputs(faces, textures, return_rgb, face_light, textures_fill_back, vertices, face_uvs, corner_light)
     indices = None
     if vertices is not None:
         geom = vertices if vertices.dtype == torch.float32 else vertices.float()
@@ -422,7 +445,7 @@ def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_
         cfg.flags |= _lib.NR_TEX_MIPMAP
         textures = _MipPyramid.apply(textures)
     return _RasterizeFunction.apply(geom, textures if return_rgb else None, face_light if return_rgb else None, cfg,
-                                    indices, face_uvs)
+                                    indices, face_uvs, corner_light)
 
 
 def rasterize_rgbad(
@@ -444,6 +467,7 @@ def rasterize_rgbad(
         reference_exact=None,
         face_uvs=None,
         texture_filter='bilinear',
+        corner_light=None,
 ):
     """Generate RGB, alpha channel, and depth images from faces and textures (for RGB).  rasterize.py:900-977.
 
@@ -477,11 +501,17 @@ def rasterize_rgbad(
                               texels without gradient.  The pyramid is rebuilt from the image on every call and its
                               gradient collapsed back into the image; no gradient flows through the level of detail
                               (face_uvs gets the level-weighted sum of both levels' derivatives).
+      corner_light [B,F,3,3]  smooth shading: an RGB light factor at each corner of every face (corners in the order of
+                              `faces`; F counts fill_back copies), interpolated with the pixel's perspective-correct
+                              weights and multiplied onto the unlit sample (include/nr_b200.h).  Exclusive with
+                              face_light; needs return_rgb.  F.vertex_normals / F.corner_light compute the Lambertian
+                              factor, but any per-corner factor works.  It receives d loss / d corner_light; no vertex
+                              gradient flows through the interpolation weights.
     `textures` with batch size 1 (or an expanded stride-0 batch) while the geometry batch is larger = one texture set
     shared by every item (a mesh seen from B viewpoints, mesh.py:29-34); its gradient is the sum over the items."""
     rgb, alpha, depth, _, _ = _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_color,
                                    return_rgb, return_alpha, return_depth, face_light, textures_fill_back, vertices,
-                                   reference_exact, face_uvs, texture_filter)
+                                   reference_exact, face_uvs, texture_filter, corner_light)
     return {
         'rgb': rgb if return_rgb else None,
         'alpha': alpha if return_alpha else None,
@@ -505,13 +535,14 @@ def rasterize(
         reference_exact=None,
         face_uvs=None,
         texture_filter='bilinear',
+        corner_light=None,
 ):
     """RGB images [B,3,H,W] from faces and textures.  rasterize.py:980-1008 (keyword-only extras: rasterize_rgbad; in
     texture-image mode both the image and face_uvs receive gradients)."""
     return rasterize_rgbad(
         faces, textures, image_size, anti_aliasing, near, far, eps, background_color, True, False, False,
         face_light=face_light, textures_fill_back=textures_fill_back, vertices=vertices,
-        reference_exact=reference_exact, face_uvs=face_uvs, texture_filter=texture_filter)['rgb']
+        reference_exact=reference_exact, face_uvs=face_uvs, texture_filter=texture_filter, corner_light=corner_light)['rgb']
 
 
 def rasterize_silhouettes(

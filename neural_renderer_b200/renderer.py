@@ -45,6 +45,10 @@ class Renderer(object):
         # sampler of a texture image (render(..., face_uvs=...)): 'bilinear', or 'trilinear' through a mip pyramid of the
         # image (minified images neither alias nor leave texels without gradient); per-face cubes ignore it
         self.texture_filter = 'bilinear'
+        # 'flat': the reference's one light factor per face; 'smooth': the light evaluated at every vertex from its
+        # area-weighted normal and interpolated across the face (Gouraud), with vertex gradients through the normals.
+        # Silhouettes and depth ignore it
+        self.shading = 'flat'
 
     def _transform(self, vertices):
         # renderer.py:41-50 (look_at / look, then perspective), fused into one kernel on CUDA
@@ -93,9 +97,13 @@ class Renderer(object):
         the image and a `face_uvs` with requires_grad receive gradients (fused: the fill_back copies' UV gradient is
         folded into the original faces in the kernel; op by op: through the cat / flip of the doubled corners)."""
         texture_filter = self.texture_filter if face_uvs is not None else 'bilinear'
+        if self.shading not in ('flat', 'smooth'):
+            raise ValueError("shading must be 'flat' or 'smooth', got %r" % (self.shading,))
         fused = (self.fused and self._fusable(vertices, faces) and textures.is_cuda and textures.dtype == torch.float32)
         light_args = (self.light_intensity_ambient, self.light_intensity_directional, self.light_color_ambient,
                       self.light_color_directional, self.light_direction)
+        if self.shading == 'smooth':
+            return self._render_smooth(vertices, faces, textures, face_uvs, texture_filter, fused, light_args)
         if fused:
             # lighting.py:29-52, renderer.py:78-80 and vertices_to_faces (renderer.py:103) folded into the rasterizer:
             # neither `textures * light`, nor the doubled texture tensor, nor faces [B,F,3,3] exist; pixel values are
@@ -127,3 +135,29 @@ class Renderer(object):
         return rasterize(
             faces, textures, self.image_size, self.anti_aliasing, self.near, self.far, self.rasterizer_eps,
             self.background_color, reference_exact=self.reference_exact)
+
+    def _render_smooth(self, vertices, faces, textures, face_uvs, texture_filter, fused, light_args):
+        # vertex normals of the original faces (the fill_back copies would cancel them), light at every corner of the
+        # faces the rasterizer draws (copies: reversed normal), interpolated per pixel and applied to the unlit sample
+        if fused:
+            indices = self._indices(faces)
+            corner = F.corner_light(F.vertex_normals(vertices, faces), indices, *light_args, fill_back=self.fill_back)
+            return rasterize(
+                indices, textures, self.image_size, self.anti_aliasing, self.near, self.far, self.rasterizer_eps,
+                self.background_color, textures_fill_back=self.fill_back, vertices=self._transform(vertices),
+                reference_exact=self.reference_exact, face_uvs=face_uvs, texture_filter=texture_filter,
+                corner_light=corner)
+        # op by op: torch normals and light, materialised faces, doubled textures / UV corners for fill_back
+        normals = F._vertex_normals_torch(vertices, faces)
+        if self.fill_back:
+            faces = torch.cat((faces, faces.flip(2)), dim=1)
+            if face_uvs is not None:
+                face_uvs = torch.cat((face_uvs, face_uvs.flip(-2)), dim=-3)
+            else:
+                textures = torch.cat((textures, textures.permute(0, 1, 4, 3, 2, 5)), dim=1)
+        corner = F._corner_light_torch(normals, faces, *light_args, fill_back=self.fill_back)
+        faces = F.vertices_to_faces(self._transform(vertices), faces)
+        return rasterize(
+            faces, textures, self.image_size, self.anti_aliasing, self.near, self.far, self.rasterizer_eps,
+            self.background_color, reference_exact=self.reference_exact, face_uvs=face_uvs,
+            texture_filter=texture_filter, corner_light=corner)

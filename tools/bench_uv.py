@@ -10,6 +10,11 @@ backward with a dense N(0,1) upstream gradient (bench.py's headline step).  Text
                    pyramid is built (k_mip_build) and its gradient collapsed (k_mip_collapse) on every step
   uv_shared_1024_uvgrad, uv_shared_1024_trilinear_uvgrad   uv_shared_1024 (bilinear / trilinear) with
                    face_uvs.requires_grad_(True): k_image_grad also returns d loss / d face_uvs
+  cubes_ts4_smooth, uv_shared_1024_smooth, uv_shared_1024_trilinear_smooth   the same with smooth shading: every step
+                   computes vertex normals (every corner its own vertex: faces viewed as [B,3F,3] vertices) and the
+                   per-corner light with the glue kernels and passes corner_light to rasterize()
+  teapot_render_flat, teapot_render_smooth   Renderer.render fwd + bwd (fused), the teapot at 256 x 256 with
+                   anti-aliasing, batch 8, ts 4 cubes, flat vs smooth shading (README's Renderer row)
 Whole step: CUDA events around `steps` steps after `warmup` warm-up steps, median over `reps` repetitions.  Per kernel:
 the library's own CUDA-event profiler over `steps` further steps (ms per step).  Bytes held = texture + its gradient.
 The roofline fraction of the image-gradient kernel and of the zero-fill uses bench.py's HBM figure.  For every image
@@ -34,7 +39,8 @@ import torch.nn.functional
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import neural_renderer as nr  # noqa: E402
-from neural_renderer_b200 import _lib, synthetic  # noqa: E402
+import neural_renderer_b200 as nb  # noqa: E402
+from neural_renderer_b200 import _lib, functional as NF, synthetic  # noqa: E402
 
 
 def hbm_gbs():
@@ -72,6 +78,48 @@ def lod_above_0(faces, uvs, Ht, Wt, S):
         return float((lod[cov] > 0).double().mean())
 
 
+def teapot_render(smooth, a, lib, dev):
+    """Renderer.render fwd + bwd (fused), teapot 256 x 256 anti-aliased, batch 8, ts 4 cubes: step time and kernels"""
+    B = 8
+    d = np.load(os.path.join(ROOT, "tests", "golden", "teapot.npz"))
+    v = torch.from_numpy(np.stack([d["vertices"]] * B)).to(dev).requires_grad_(True)
+    f = torch.from_numpy(np.stack([d["faces"]] * B)).to(dev)
+    tex = torch.rand((B, f.shape[1], 4, 4, 4, 3), generator=torch.Generator().manual_seed(1)).to(dev).requires_grad_(True)
+    g = torch.randn((B, 3, 256, 256), generator=torch.Generator().manual_seed(2)).to(dev)
+    r = nb.Renderer()
+    r.eye = nb.get_points_from_angles(2.732, 30, 40)
+    r.shading = "smooth" if smooth else "flat"
+
+    def step():
+        v.grad = None
+        tex.grad = None
+        r.render(v, f, tex).backward(g)
+
+    for _ in range(a.warmup):
+        step()
+    torch.cuda.synchronize()
+    reps = []
+    for _ in range(a.reps):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(a.steps):
+            step()
+        e1.record()
+        torch.cuda.synchronize()
+        reps.append(e0.elapsed_time(e1) / a.steps)
+    lib.nr_b200_set_profiling(1)
+    _lib.read_profile()
+    for _ in range(a.steps):
+        step()
+    torch.cuda.synchronize()
+    kern = collections.OrderedDict()
+    for k, ms in _lib.read_profile():
+        kern[k] = kern.get(k, 0.0) + ms / a.steps
+    lib.nr_b200_set_profiling(0)
+    return {"shading": r.shading, "step_ms_median": float(np.median(reps)), "step_ms_min_max": [min(reps), max(reps)],
+            "step_ms_reps": reps, "kernels_ms_per_step": kern}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=64)
@@ -89,22 +137,34 @@ def main():
     g = torch.randn((B, 3, S, S), generator=torch.Generator().manual_seed(0)).to(dev)
     img1024 = torch.from_numpy(synthetic.random_image(1, 1024, 1024)[0]).to(dev)
     img256 = torch.from_numpy(synthetic.random_image(B, 256, 256)).to(dev)
+    cubes = torch.from_numpy(synthetic.random_textures(B, F, 4)).to(dev)
     variants = collections.OrderedDict([
         ("uv_shared_1024", (img1024, uvs, "bilinear", False)),
         ("uv_item_256", (img256, uvs, "bilinear", False)),
-        ("cubes_ts4", (torch.from_numpy(synthetic.random_textures(B, F, 4)).to(dev), None, "bilinear", False)),
+        ("cubes_ts4", (cubes, None, "bilinear", False)),
         ("uv_shared_1024_trilinear", (img1024, uvs, "trilinear", False)),
         ("uv_item_256_trilinear", (img256, uvs, "trilinear", False)),
         ("uv_shared_1024_uvgrad", (img1024, uvs, "bilinear", True)),
         ("uv_shared_1024_trilinear_uvgrad", (img1024, uvs, "trilinear", True)),
+        ("cubes_ts4_smooth", (cubes, None, "bilinear", False)),
+        ("uv_shared_1024_smooth", (img1024, uvs, "bilinear", False)),
+        ("uv_shared_1024_trilinear_smooth", (img1024, uvs, "trilinear", False)),
+        ("teapot_render_flat", None),
+        ("teapot_render_smooth", None),
     ])
+    corner_idx = torch.arange(3 * F, device=dev, dtype=torch.int32).reshape(F, 3)
     if a.only:
         variants = collections.OrderedDict((k, variants[k]) for k in a.only.split(","))
     lib = _lib.load()
     props = torch.cuda.get_device_properties(dev)
     out = {"gpu": torch.cuda.get_device_name(dev), "sm_count": props.multi_processor_count, "shape": {"batch": B, "faces": F, "size": S, "anti_aliasing": False},
            "hbm_gbs": hbm_gbs(), "variants": {}}
-    for name, (tex0, fuv0, tf, uv_grad) in variants.items():
+    for name, spec in variants.items():
+        if spec is None:
+            out["variants"][name] = teapot_render(name.endswith("smooth"), a, lib, dev)
+            continue
+        tex0, fuv0, tf, uv_grad = spec
+        smooth = name.endswith("_smooth")
         tex = tex0.clone().requires_grad_(True)
         fuv = fuv0.clone().requires_grad_(True) if uv_grad else fuv0
 
@@ -113,7 +173,11 @@ def main():
             tex.grad = None
             if uv_grad:
                 fuv.grad = None
-            img = nr.rasterize(faces, tex, S, False, face_uvs=fuv, texture_filter=tf)
+            corner = None
+            if smooth:
+                verts = faces.reshape(B, 3 * F, 3)
+                corner = NF.corner_light(NF.vertex_normals(verts, corner_idx), corner_idx)
+            img = nb.rasterize(faces, tex, S, False, face_uvs=fuv, texture_filter=tf, corner_light=corner)
             img.backward(g)
 
         for _ in range(a.warmup):
@@ -141,7 +205,8 @@ def main():
         tex_bytes = tex.numel() * 4
         if tf == "trilinear":  # the rasterizer samples (and its gradient is) the pyramid
             tex_bytes = tex.numel() // (tex.shape[-3] * tex.shape[-2]) * lib.nr_b200_mip_texels(*tex.shape[-3:-1]) * 4
-        rec = {"texture_filter": tf, "uv_grad": uv_grad, "step_ms_median": float(np.median(reps)), "step_ms_reps": reps,
+        rec = {"texture_filter": tf, "uv_grad": uv_grad, "smooth": smooth, "step_ms_median": float(np.median(reps)),
+               "step_ms_min_max": [min(reps), max(reps)], "step_ms_reps": reps,
                "kernels_ms_per_step": kern, "texture_bytes": tex_bytes, "texture_plus_grad_bytes": 2 * tex_bytes}
         if fuv is not None:
             rec["lod_above_0"] = lod_above_0(faces.detach(), fuv.detach()[None], tex.shape[-3], tex.shape[-2], S)
