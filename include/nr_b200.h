@@ -239,6 +239,67 @@ typedef struct nr_b200_backward_args {
     float *grad_face_uvs;
 } nr_b200_backward_args;
 
+/* Attribute interpolation, additive to ABI 4: two flag bits, one struct and two entry points.  Renders C >= 1 arbitrary
+ * channels (normals, positions, UVs, labels, features) through the maps an ordinary forward call wrote (face_index_map,
+ * weight_map; a silhouette-only forward suffices), with gradients into the attributes and, through the perspective
+ * weights, into the vertices.
+ *   Attributes are per corner [B,F,3,C] (corners in the face's own order), or with NR_ATTR_PER_VERTEX per vertex [B,Nv,C]
+ *   (needs NR_FACES_INDEXED: corner k of face f reads vertex face_indices[f,k], an index outside [0, Nv) reads zeros, as
+ *   the geometry does).  NR_ATTR_SHARED: one set [F,3,C] / [Nv,C] serves every item; its gradient is the sum over the
+ *   items.  F counts the fill_back copies as faces of their own (give the copies their corners; no fill_back fold).
+ *   Forward, covered raster pixel (fn = face_index_map >= 0) with saved weights w_k and the winner's OWN camera depths z_k
+ *   (NR_TEX_Z_BATCH0 has no effect):
+ *     zp = rcp.rn((w0/z0 + w1/z1) + w2/z2)  (div.rn; the expression of the forward, so zp == depth_map bit for bit),
+ *     l_k = w_k * (zp / z_k)  (the l_k of NR_TEX_UV),   out_c = fma(l_2, a_2c, fma(l_1, a_1c, l_0 * a_0c))
+ *   (the chain of corner_light: interpolating corner_light as a C = 3 corner attribute gives smooth shading's L_c bit for
+ *   bit).  Uncovered pixels are 0.  `out` is planar [B,C,H,W] in image orientation; with NR_ANTI_ALIASING it is the 2x2
+ *   mean, summed top-left, top-right, bottom-left, bottom-right, then * 0.25f (only the pooled image is written).
+ *   Backward, covered raster pixel with upstream g_c (the pooled gradient / 4 with NR_ANTI_ALIASING):
+ *     grad_attributes[corner k (or vertex face_indices[fn,k]), c] += l_k g_c;
+ *     interior vertex gradient (grad_faces [B,F,3,3], or grad_vertices [B,Nv,3] with NR_FACES_INDEXED): inv = the K1 inverse
+ *     of the winner's pixel-space vertices (face_inverse(to_pixel(.)), as the depth gradient K7 recomputes it),
+ *       qx_k = inv[3k] / z_k,  sx = sum_k qx_k,  lx_k = zp (qx_k - l_k sx)  (= d l_k / dx in raster pixels; y alike with
+ *       inv[3k+1]),  Gx = sum_c g_c sum_{k=1,2} (a_kc - a_0c) lx_k  (differences against corner 0: no fp32 cancellation
+ *       for attributes close together far from 0; sum_k lx_k = 0),  Gy alike,
+ *       Gz_m = (l_m / z_m) sum_c g_c (out_c - a_mc)  (out_c the raster-resolution interpolant),
+ *       grad x_m += -w_m Gx S/2,   grad y_m += -w_m Gy S/2,   grad z_m += Gz_m.
+ *     Derivation: the unclamped barycentrics a_k are affine in the pixel and d a_k / d x_m = -a_m inv[3k] (pixel units), so
+ *     d l_k / d x_m = -w_m d l_k / dx_screen; l_k = (w_k / z_k) / sum_j (w_j / z_j) gives d l_k / d z_m = -delta_km l_k / z_k
+ *     + l_k l_m / z_m; S/2 takes pixel to NDC units.  This is the derivative at the saved w: the clamp / renormalisation of
+ *     the weights is held fixed, as in K7.  No edge or occlusion gradient flows from the attribute image: those come from
+ *     the rasterizer's backward (K5) through the alpha image.
+ *   Either gradient output may be NULL (not wanted); each is zero-filled first unless NR_GRAD_ACCUMULATE.  grad_out NULL =
+ *   zeros.  fp32 atomics, not bit-pinned.
+ *   Host rejections (NR_ERR_INVALID_ARG, before any launch): struct_size != sizeof(nr_b200_interpolate_args), B, F or S < 1,
+ *   C < 1, a NULL face_index_map / weight_map / attributes (or `out` in the forward), missing geometry for the chosen form,
+ *   NR_ATTR_PER_VERTEX without NR_FACES_INDEXED, an odd S with NR_ANTI_ALIASING, grad_vertices without / grad_faces with
+ *   NR_FACES_INDEXED, and S > 32767 or B > 65535 (the kernels' grid and 32-bit plane offsets).  No workspace. */
+#define NR_ATTR_PER_VERTEX 0x100000u /* attributes [B,Nv,C] per vertex (needs NR_FACES_INDEXED), else [B,F,3,C] per corner */
+#define NR_ATTR_SHARED 0x200000u     /* one attribute set [F,3,C] / [Nv,C] for every item                                */
+
+typedef struct nr_b200_interpolate_args {
+    uint32_t struct_size; /* sizeof(nr_b200_interpolate_args) */
+    uint32_t flags;       /* NR_ANTI_ALIASING as the forward call, NR_FACES_INDEXED / NR_INDICES_SHARED, NR_ATTR_*,
+                             NR_GRAD_ACCUMULATE (backward) */
+    int32_t batch_size;   /* B */
+    int32_t num_faces;    /* F */
+    int32_t raster_size;  /* S (doubled with NR_ANTI_ALIASING), as the forward call */
+    int32_t channels;     /* C >= 1 */
+    const float *faces;          /* [B,F,3,3] as given to the forward call, or NULL with NR_FACES_INDEXED */
+    const float *vertices;       /* [B,Nv,3], NR_FACES_INDEXED only */
+    const int32_t *face_indices; /* [B,F,3], or [F,3] with NR_INDICES_SHARED */
+    int32_t num_vertices;        /* Nv */
+    int32_t _pad0;
+    const int32_t *face_index_map; /* [B,S,S] saved by nr_b200_forward */
+    const float *weight_map;       /* [B,3,S,S] saved by nr_b200_forward */
+    const float *attributes;       /* [B,F,3,C] / [B,Nv,C] (no B with NR_ATTR_SHARED) */
+    float *out;                    /* forward: [B,C,H,W], H = S or S/2 */
+    const float *grad_out;         /* backward: [B,C,H,W] or NULL (zeros) */
+    float *grad_attributes;        /* backward: layout of attributes, or NULL */
+    float *grad_faces;             /* backward: [B,F,3,3] or NULL; not with NR_FACES_INDEXED */
+    float *grad_vertices;          /* backward: [B,Nv,3] or NULL; only with NR_FACES_INDEXED */
+} nr_b200_interpolate_args;
+
 /* ABI version of the loaded library (== NR_B200_ABI_VERSION it was built with). */
 NR_B200_API int nr_b200_abi_version(void);
 NR_B200_API const char *nr_b200_error_string(int code);
@@ -256,6 +317,10 @@ NR_B200_API int nr_b200_backward(const nr_b200_backward_args *args, void *cuda_s
  * not wanted (part of the texture half, NR_BWD_PART_TEXTURES).  nr_b200_backward is this call with corner_light NULL. */
 NR_B200_API int nr_b200_backward_corner_light(const nr_b200_backward_args *args, const float *corner_light,
                                               float *grad_corner_light, void *cuda_stream);
+/* Attribute interpolation (nr_b200_interpolate_args above): the image `out`, and its backward into grad_attributes and the
+ * interior vertex gradient.  One kernel launch each (plus the zero-fill of the backward). */
+NR_B200_API int nr_b200_interpolate(const nr_b200_interpolate_args *args, void *cuda_stream);
+NR_B200_API int nr_b200_interpolate_backward(const nr_b200_interpolate_args *args, void *cuda_stream);
 
 /* vertices_to_faces (reference vertices_to_faces.py:4-21), the step either side of the rasterizer:
  *   forward   out_faces[b,f,k,:] = vertices[b, faces[b,f,k], :]           ([B,Nv,3] x [B,Nf,3] int32 -> [B,Nf,3,3])

@@ -8,7 +8,7 @@ with torch tensors in place of chainer Variables.
 from .functional import cross, get_points_from_angles, lighting, look, look_at, perspective, vertices_to_faces
 from .rasterize import (
     rasterize_rgbad, rasterize, rasterize_silhouettes, rasterize_depth, use_unsafe_rasterizer, Rasterize,
-    set_reference_exact)
+    set_reference_exact, rasterize_attributes)
 from .renderer import Renderer
 from .io import load_obj, save_obj
 from .mesh import Mesh

@@ -31,6 +31,8 @@ NR_FWD_STAGE_TEXTURES = 0x10000
 NR_TEX_UV = 0x20000
 NR_UV_SHARED = 0x40000
 NR_TEX_MIPMAP = 0x80000
+NR_ATTR_PER_VERTEX = 0x100000
+NR_ATTR_SHARED = 0x200000
 
 ABI_VERSION = 4
 
@@ -43,6 +45,8 @@ EXPORTED_SYMBOLS = (
     "nr_b200_forward",
     "nr_b200_backward",
     "nr_b200_backward_corner_light",
+    "nr_b200_interpolate",
+    "nr_b200_interpolate_backward",
     "nr_b200_vertices_to_faces",
     "nr_b200_vertices_to_faces_backward",
     "nr_b200_camera_transform",
@@ -104,6 +108,20 @@ class BackwardArgs(ctypes.Structure):
     ]
 
 
+class InterpolateArgs(ctypes.Structure):
+    _fields_ = [
+        ("struct_size", ctypes.c_uint32), ("flags", ctypes.c_uint32),
+        ("batch_size", ctypes.c_int32), ("num_faces", ctypes.c_int32),
+        ("raster_size", ctypes.c_int32), ("channels", ctypes.c_int32),
+        ("faces", ctypes.c_void_p), ("vertices", ctypes.c_void_p), ("face_indices", ctypes.c_void_p),
+        ("num_vertices", ctypes.c_int32), ("_pad0", ctypes.c_int32),
+        ("face_index_map", ctypes.c_void_p), ("weight_map", ctypes.c_void_p),
+        ("attributes", ctypes.c_void_p), ("out", ctypes.c_void_p),
+        ("grad_out", ctypes.c_void_p), ("grad_attributes", ctypes.c_void_p),
+        ("grad_faces", ctypes.c_void_p), ("grad_vertices", ctypes.c_void_p),
+    ]
+
+
 _LIB = None
 
 
@@ -135,6 +153,10 @@ def load():
     lib.nr_b200_backward_corner_light.restype = ctypes.c_int
     lib.nr_b200_backward_corner_light.argtypes = [ctypes.POINTER(BackwardArgs), ctypes.c_void_p, ctypes.c_void_p,
                                                   ctypes.c_void_p]
+    for name in ("nr_b200_interpolate", "nr_b200_interpolate_backward"):
+        fn = getattr(lib, name)
+        fn.restype = ctypes.c_int
+        fn.argtypes = [ctypes.POINTER(InterpolateArgs), ctypes.c_void_p]
     lib.nr_b200_vertices_to_faces.restype = ctypes.c_int
     lib.nr_b200_vertices_to_faces.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
                                               ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p]

@@ -575,6 +575,159 @@ def rasterize_depth(
                            vertices=vertices)['depth']
 
 
+class _InterpolateFunction(torch.autograd.Function):
+    """autograd node of attribute interpolation: forward = nr_b200_interpolate on the maps of a forward call, backward =
+    nr_b200_interpolate_backward (d loss / d attributes, and the interior vertex gradient through the perspective weights).
+
+    `geom` / `indices` are the geometry exactly as the forward call that produced `fim` / `wmap` got it; `flags` holds the
+    anti-aliasing and attribute-layout bits, `S` the raster size."""
+
+    @staticmethod
+    def forward(ctx, geom, attributes, fim, wmap, indices, flags, S):
+        lib = _lib.load()
+        dev = geom.device
+        geom_c = geom.detach().contiguous()
+        attr_c = attributes.detach().contiguous()
+        B, C = geom_c.shape[0], attr_c.shape[-1]
+        H = S // 2 if flags & _lib.NR_ANTI_ALIASING else S
+        with torch.cuda.device(dev):
+            out = torch.empty((B, C, H, H), dtype=torch.float32, device=dev)
+            a = _interpolate_args(geom_c, attr_c, fim, wmap, indices, flags, S)
+            a.out = _ptr(out)
+            _lib.check(lib.nr_b200_interpolate(ctypes.byref(a), _stream_ptr(dev)))
+        ctx.flags, ctx.S = flags, S
+        ctx.save_for_backward(geom_c, attr_c, fim, wmap, indices)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        want_geom, want_attr = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        if g is None or not (want_geom or want_attr):
+            return None, None, None, None, None, None, None
+        lib = _lib.load()
+        geom_c, attr_c, fim, wmap, indices = ctx.saved_tensors
+        dev = geom_c.device
+        g = g.detach().to(torch.float32).contiguous()
+        with torch.cuda.device(dev):
+            grad_geom = torch.empty_like(geom_c) if want_geom else None
+            grad_attr = torch.empty_like(attr_c) if want_attr else None
+            a = _interpolate_args(geom_c, attr_c, fim, wmap, indices, ctx.flags, ctx.S)
+            a.grad_out, a.grad_attributes = _ptr(g), _ptr(grad_attr)
+            if indices is not None:
+                a.grad_vertices = _ptr(grad_geom)
+            else:
+                a.grad_faces = _ptr(grad_geom)
+            _lib.check(lib.nr_b200_interpolate_backward(ctypes.byref(a), _stream_ptr(dev)))
+        return grad_geom, grad_attr, None, None, None, None, None
+
+
+def _interpolate_args(geom_c, attr_c, fim, wmap, indices, flags, S):
+    a = _lib.InterpolateArgs()
+    a.struct_size = ctypes.sizeof(_lib.InterpolateArgs)
+    B = geom_c.shape[0]
+    if indices is not None:
+        flags |= _lib.NR_FACES_INDEXED
+        if indices.dim() == 2 or (indices.shape[0] == 1 and B > 1):
+            flags |= _lib.NR_INDICES_SHARED
+        a.vertices, a.face_indices, a.num_vertices = _ptr(geom_c), _ptr(indices), geom_c.shape[1]
+        a.num_faces = indices.shape[-2]
+    else:
+        a.faces, a.num_faces = _ptr(geom_c), geom_c.shape[1]
+    if attr_c.shape[0] == 1 and B > 1:
+        flags |= _lib.NR_ATTR_SHARED
+    a.flags = flags
+    a.batch_size, a.raster_size, a.channels = B, S, attr_c.shape[-1]
+    a.face_index_map, a.weight_map, a.attributes = _ptr(fim), _ptr(wmap), _ptr(attr_c)
+    return a
+
+
+def _check_attribute_inputs(faces, vertices, vertex_attributes, face_attributes):
+    """argument errors of rasterize_attributes, all raised before any device check"""
+    if (vertex_attributes is None) == (face_attributes is None):
+        raise TypeError("give exactly one of vertex_attributes= and face_attributes=")
+    per_vertex = vertex_attributes is not None
+    attrs = vertex_attributes if per_vertex else face_attributes
+    name = "vertex_attributes" if per_vertex else "face_attributes"
+    if not isinstance(attrs, torch.Tensor) or not attrs.is_floating_point():
+        raise TypeError("%s must be a floating point torch.Tensor" % name)
+    if per_vertex and vertices is None:
+        raise ValueError("vertex_attributes need indexed geometry: vertices= and integer faces")
+    # the attribute shapes against the geometry's, when the geometry's own shape is valid (else _check_inputs says why)
+    B = F = Nv = None
+    if isinstance(faces, torch.Tensor) and faces.dim() >= 2:
+        if isinstance(vertices, torch.Tensor) and vertices.dim() == 3:
+            B, F, Nv = vertices.shape[0], faces.shape[-2], vertices.shape[1]
+        elif vertices is None and faces.dim() == 4:
+            B, F = faces.shape[0], faces.shape[1]
+    if B is not None:
+        rows = (Nv,) if per_vertex else (F, 3)
+        nd = len(rows) + 1
+        ok = attrs.dim() in (nd, nd + 1) and tuple(attrs.shape[-nd:-1]) == rows and attrs.shape[-1] >= 1
+        if ok and attrs.dim() == nd + 1:
+            ok = attrs.shape[0] in (1, B)
+        if not ok:
+            want = "[num vertices, C] or [batch size, num vertices, C]" if per_vertex else \
+                "[num faces, 3, C] or [batch size, num faces, 3, C]"
+            raise ValueError("%s must have shape %s with C >= 1 matching the geometry (num faces counts fill_back "
+                             "copies), got %s" % (name, want, tuple(attrs.shape)))
+    _check_inputs(faces, None, False, vertices=vertices)  # the geometry, then the device check
+    if not attrs.is_cuda:
+        raise NotImplementedError("neural_renderer_b200 has no CPU implementation (inputs must be CUDA tensors)")
+    return attrs, per_vertex
+
+
+def rasterize_attributes(
+        faces,
+        image_size=DEFAULT_IMAGE_SIZE,
+        anti_aliasing=DEFAULT_ANTI_ALIASING,
+        near=DEFAULT_NEAR,
+        far=DEFAULT_FAR,
+        eps=DEFAULT_EPS,
+        *,
+        vertices=None,
+        vertex_attributes=None,
+        face_attributes=None,
+        return_alpha=False,
+):
+    """Images [B,C,H,W] of arbitrary per-vertex or per-corner attributes: normal maps, position maps, UV G-buffers,
+    part labels, feature images.  Not in the reference (PyTorch3D: interpolate_face_attributes, nvdiffrast: interpolate).
+
+    Exactly one of (keywords, because [B,Nv,C] and [F,3,C] cannot be told apart by shape):
+      vertex_attributes [Nv,C] / [1|B,Nv,C]     one row per vertex; needs indexed geometry (`vertices`, integer faces)
+      face_attributes [F,3,C] / [1|B,F,3,C]     one row per face corner, corners in the order of `faces` (F counts any
+                                                fill_back copies: give them their corners, e.g. cat((a, a.flip(-2)), -3))
+    A batch of 1 (or an expanded stride-0 batch) with a larger geometry batch is one set shared by every item; its
+    gradient is the sum over the items.  Every covered pixel gets sum_k l_k a_k with the perspective-correct weights l_k
+    of the winning face (include/nr_b200.h), uncovered pixels 0; with anti-aliasing the 2x2 mean.  No lighting.
+
+    Gradients flow into the attributes and, through the interpolation weights, into the vertices (the interior
+    derivative, with the weights' clamp held fixed).  The image has no edge or occlusion gradient: for that, use the
+    alpha image of `return_alpha=True`, which is the rasterizer's and carries its usual silhouette gradient.  Returns
+    the image, or (image, alpha)."""
+    attrs, per_vertex = _check_attribute_inputs(faces, vertices, vertex_attributes, face_attributes)
+    indices = None
+    if vertices is not None:
+        geom = vertices if vertices.dtype == torch.float32 else vertices.float()
+        indices = faces
+        if indices.dim() == 3 and indices.shape[0] > 1 and indices.stride(0) == 0:
+            indices = indices[:1]
+        indices = indices.to(torch.int32).contiguous()
+    else:
+        geom = faces if faces.dtype == torch.float32 else faces.float()
+    batch_size = geom.shape[0]
+    attrs = attrs if attrs.dtype == torch.float32 else attrs.float()
+    if attrs.dim() == (2 if per_vertex else 3):
+        attrs = attrs[None]
+    if attrs.shape[0] == batch_size > 1 and attrs.stride(0) == 0:
+        attrs = attrs[:1]  # an expanded shared set (NR_ATTR_SHARED)
+    _, alpha, _, fim, wmap = _run(indices if indices is not None else geom, None, image_size, anti_aliasing, near, far,
+                                  eps, None, False, True, False, vertices=geom if indices is not None else None)
+    flags = (_lib.NR_ANTI_ALIASING if anti_aliasing else 0) | (_lib.NR_ATTR_PER_VERTEX if per_vertex else 0)
+    S = int(image_size) * 2 if anti_aliasing else int(image_size)
+    image = _InterpolateFunction.apply(geom, attrs, fim, wmap, indices, flags, S)
+    return (image, alpha) if return_alpha else image
+
+
 class Rasterize(object):
     """The reference's function object (rasterize.py:19-64): `Rasterize(image_size, near, far, eps,
     background_color, return_rgb, return_alpha, return_depth)(faces[, textures]) -> (rgb, alpha, depth)` with the

@@ -6,7 +6,7 @@ import math
 import torch
 
 from . import functional as F
-from .rasterize import rasterize, rasterize_depth, rasterize_silhouettes
+from .rasterize import rasterize, rasterize_attributes, rasterize_depth, rasterize_silhouettes
 
 
 class Renderer(object):
@@ -135,6 +135,33 @@ class Renderer(object):
         return rasterize(
             faces, textures, self.image_size, self.anti_aliasing, self.near, self.far, self.rasterizer_eps,
             self.background_color, reference_exact=self.reference_exact)
+
+    def render_attributes(self, vertices, faces, vertex_attributes=None, face_attributes=None):
+        """Attribute images [B,C,H,W] (neural_renderer_b200.rasterize_attributes) seen through this renderer's camera:
+        e.g. a normal map, `render_attributes(v, f, vertex_attributes=F.vertex_normals(v, f))`.  Exactly one of
+        vertex_attributes [Nv,C] / [1|B,Nv,C] and face_attributes [F,3,C] / [1|B,F,3,C] (F = the faces given, without
+        fill_back copies: those get the corners reversed).  No lighting, no texture.  Gradients flow into the attributes
+        and the vertices (interior derivative; render_silhouettes gives the edge gradient)."""
+        if (vertex_attributes is None) == (face_attributes is None):
+            raise TypeError("give exactly one of vertex_attributes= and face_attributes=")
+        if face_attributes is not None and self.fill_back:
+            face_attributes = torch.cat((face_attributes, face_attributes.flip(-2)), dim=-3)
+        if self.fused and self._fusable(vertices, faces):
+            # per-vertex attributes follow the doubled index set of fill_back as the vertices do
+            return rasterize_attributes(self._indices(faces), self.image_size, self.anti_aliasing, self.near, self.far,
+                                        self.rasterizer_eps, vertices=self._transform(vertices),
+                                        vertex_attributes=vertex_attributes, face_attributes=face_attributes)
+        # op by op: materialised faces, per-vertex attributes gathered to the corners in torch
+        if self.fill_back:
+            faces = torch.cat((faces, faces.flip(2)), dim=1)
+        if vertex_attributes is not None:
+            va = vertex_attributes[None] if vertex_attributes.dim() == 2 else vertex_attributes
+            B, C = vertices.shape[0], va.shape[-1]
+            idx = faces.long().expand(B, -1, -1).reshape(B, -1, 1).expand(-1, -1, C)
+            face_attributes = torch.gather(va.expand(B, -1, -1), 1, idx).reshape(B, -1, 3, C)
+        faces = F.vertices_to_faces(self._transform(vertices), faces)
+        return rasterize_attributes(faces, self.image_size, self.anti_aliasing, self.near, self.far, self.rasterizer_eps,
+                                    face_attributes=face_attributes)
 
     def _render_smooth(self, vertices, faces, textures, face_uvs, texture_filter, fused, light_args):
         # vertex normals of the original faces (the fill_back copies would cancel them), light at every corner of the
