@@ -1,14 +1,21 @@
-"""Deterministic covering array over the flag dimensions of nr_b200_forward / nr_b200_backward (test infrastructure).
+"""Deterministic covering array over the flag dimensions of nr_b200_forward / nr_b200_backward /
+nr_b200_backward_corner_light and of the attribute interpolation that reads their maps, nr_b200_interpolate /
+nr_b200_interpolate_backward (test infrastructure).
 
 `cases()` returns the case list of tests/test_gpu_abi_matrix.py: the full product of texture kind x fill_back x
 anti-aliasing x backward mode, with every other dimension filled in greedily so that every compatible pair of levels of
 any two dimensions appears in at least one case; rows are added until no pair is missing.  No randomness: the same list
-on every machine.
+on every machine.  The cases of the matrix as it stood before smooth shading, the face_uvs gradient, texture staging,
+the short layouts and interpolation joined it (BASE) come first and are generated as they were, so their ids, inputs and
+oracle stay the same; the rows and pairs of the newer levels follow.
 
-A level that has no meaning for a case (ts without texture cubes, image / UV sharing without a texture image) is None and
-takes part in no pair.  Combinations the ABI rejects are never generated: texture kinds other than "none" always draw
-RGB and "none" never does, light needs RGB; fill_back doubles the faces (F even) and anti-aliasing doubles the raster
-(even) by construction of the geometry, so no case is skipped."""
+A level that has no meaning for a case (ts without texture cubes, image / UV sharing and the face_uvs gradient without a
+texture image, staging without RGB) is None and takes part in no pair.  Combinations the ABI rejects are never
+generated: texture kinds other than "none" always draw RGB and "none" never does, light (per face or per corner) needs
+RGB, the short struct layouts (ending before corner_light / grad_face_uvs) carry neither field, per-vertex attributes
+need indexed geometry; fill_back doubles the faces (F even) and anti-aliasing doubles the raster (even) by construction
+of the geometry, so no case is skipped.  The attribute channel count C is not a dimension: it rotates over
+ATTR_CHANNELS with the case id (abi_harness.Plan)."""
 import itertools
 
 DIMS = [
@@ -17,10 +24,10 @@ DIMS = [
     ("raster", ["even", "odd", "aa"]),
     ("backward", ["one", "tex_faces", "faces_tex", "acc_one", "acc_halves"]),
     ("geometry", ["faces", "idx_item", "idx_shared", "idx_shared_oor"]),
-    ("ts", [2, 3, 5]),
+    ("ts", [2, 3, 4, 5, 6]),
     ("image", ["item", "shared"]),
     ("uvs", ["item", "shared"]),
-    ("light", [False, True]),
+    ("light", ["none", "face", "corner"]),
     ("bg", ["uniform", "per_batch"]),
     ("outputs", ["r", "a", "d", "ra", "rd", "ad", "rad"]),
     ("z_batch0", [False, True]),
@@ -28,6 +35,10 @@ DIMS = [
     ("upstream", ["all", "no_rgb", "only_rgb"]),
     ("pointers", ["fresh", "off4", "off8"]),
     ("optional", ["given", "null"]),
+    ("uv_grad", ["given", "null"]),
+    ("stage", [False, True]),
+    ("layout", ["full", "short"]),
+    ("attr", ["off", "corner", "corner_shared", "vertex", "vertex_shared"]),
 ]
 NAMES = [n for n, _ in DIMS]
 LEVELS = dict(DIMS)
@@ -37,8 +48,10 @@ def active(dim, kind):
     """whether `dim` means anything for texture kind `kind`"""
     if dim == "ts":
         return kind in ("cube", "cube_shared")
-    if dim in ("image", "uvs"):
+    if dim in ("image", "uvs", "uv_grad"):
         return kind in ("uv", "mip")
+    if dim == "stage":
+        return kind != "none"
     return True
 
 
@@ -48,17 +61,21 @@ def compatible(a):
     out = a.get("outputs")
     if kind is not None and out is not None and (kind == "none") == ("r" in out):
         return False  # the texture models draw RGB, "none" draws no RGB
-    if kind == "none" and a.get("light"):
+    if kind == "none" and a.get("light") not in (None, "none"):
         return False
+    if a.get("layout") == "short" and (a.get("light") == "corner" or a.get("uv_grad") == "given"):
+        return False  # the short forward struct ends before corner_light, the short backward before grad_face_uvs
+    if a.get("geometry") == "faces" and str(a.get("attr")).startswith("vertex"):
+        return False  # per-vertex attributes need NR_FACES_INDEXED
     return True
 
 
-def required_pairs():
-    """every pair ((dim1, level1), (dim2, level2)) some valid case can hold"""
+def required_pairs(levels=LEVELS):
+    """every pair ((dim1, level1), (dim2, level2)) some valid case can hold, over the dimensions and levels of `levels`"""
     out = set()
-    for (i, (d1, l1s)), (j, (d2, l2s)) in itertools.combinations(enumerate(DIMS), 2):
-        for l1 in l1s:
-            for l2 in l2s:
+    for d1, d2 in itertools.combinations([n for n in NAMES if n in levels], 2):
+        for l1 in levels[d1]:
+            for l2 in levels[d2]:
                 a = {d1: l1, d2: l2}
                 if not compatible(a):
                     continue
@@ -73,16 +90,16 @@ def pairs_of(case):
     return set(itertools.combinations(ks, 2))
 
 
-def _fill(case, covered, order):
-    """assign the unassigned dimensions one after the other, each to the level that covers most new pairs (ties: the
-    level that comes first in `order`, a rotation of the level list that changes from row to row)"""
+def _fill(case, covered, order, choices=LEVELS):
+    """assign the unassigned dimensions one after the other, each to the level of `choices` that covers most new pairs
+    (ties: the level that comes first in `order`, a rotation of the level list that changes from row to row)"""
     for name in NAMES:
         if name in case:
             continue
         if not active(name, case["kind"]):
             case[name] = None
             continue
-        levels = LEVELS[name]
+        levels = choices[name]
         r = order % len(levels)
         best, best_gain = None, -1
         for lv in levels[r:] + levels[:r]:
@@ -104,6 +121,13 @@ def _key(d1, l1, d2, l2):
     return ((d1, l1), (d2, l2)) if NAMES.index(d1) < NAMES.index(d2) else ((d2, l2), (d1, l1))
 
 
+# The matrix as it stood before smooth shading, the face_uvs gradient, texture staging, the short struct layouts and
+# attribute interpolation joined it: its dimensions and levels, the others held at the level that leaves the call as it
+# was.  Its cases are generated first, exactly as before, so their ids and inputs stay what they were.
+BASE = {**{n: LEVELS[n] for n in NAMES[:NAMES.index("optional") + 1]}, "ts": [2, 3, 5], "light": ["none", "face"],
+        "uv_grad": ["null"], "stage": [False], "layout": ["full"], "attr": ["off"]}
+BASE_PAIRS = {n: BASE[n] for n in NAMES[:NAMES.index("optional") + 1]}
+
 # rows the pairs alone would not force: the edge scan zero-fills grad_textures on the side (one call, both halves, rgb
 # upstream gradient, 16-byte aligned buffer) with a float count that is not a multiple of 4 (ts 3 and an odd cube count:
 # the scalar tail of the fill)
@@ -114,35 +138,71 @@ MUST = [{"kind": "cube", "ts": 3, "fill_back": False, "_aa": False, "backward": 
 # rgb upstream gradient -- a conjunction the pairs do not force.  Every texture kind gets it in a fresh and an
 # accumulating backward, one call and two halves, with and without fill_back and anti-aliasing.
 LIGHT_ROWS = [(False, False, "one"), (True, True, "acc_halves"), (True, False, "tex_faces"), (False, True, "acc_one")]
-MUST += [{"kind": kind, "fill_back": fb, "_aa": aa, "backward": bwd, "light": True, "optional": "given",
+MUST += [{"kind": kind, "fill_back": fb, "_aa": aa, "backward": bwd, "light": "face", "optional": "given",
           "upstream": ("all", "only_rgb")[i % 2]}
          for kind in ("cube", "cube_shared", "uv", "mip") for i, (fb, aa, bwd) in enumerate(LIGHT_ROWS)]
+# the same for smooth shading: grad_corner_light (nr_b200_backward_corner_light) with the same spread of backward modes
+CORNER_ROWS = [(False, False, "faces_tex"), (True, True, "acc_halves"), (True, False, "one"), (False, True, "acc_one")]
+MUST_NEW = [{"kind": kind, "fill_back": fb, "_aa": aa, "backward": bwd, "light": "corner", "optional": "given",
+          "upstream": ("all", "only_rgb")[i % 2]}
+         for kind in ("cube", "cube_shared", "uv", "mip") for i, (fb, aa, bwd) in enumerate(CORNER_ROWS)]
+# corner light with NR_TEX_Z_BATCH0 on indexed geometry, three items: the cube texture gradient reloads each item's own
+# depths for the perspective weights (the cube coordinates keep item 0's)
+MUST_NEW += [{"kind": kind, "light": "corner", "z_batch0": True, "batch": "B3", "geometry": geom, "optional": "given",
+          "upstream": "all"}
+         for kind, geom in (("cube", "idx_item"), ("cube_shared", "idx_shared"))]
+# grad_face_uvs at every phase of the 6-float reduction (4 bytes in: phases 1 / 3; fresh and 8 bytes in: 0 / 2), for both
+# samplers, and once each with corner light (the kUvGrad && kCorner variants)
+MUST_NEW += [{"kind": kind, "uv_grad": "given", "upstream": up, "pointers": ptr, "light": light}
+         for kind in ("uv", "mip")
+         for up, ptr, light in (("all", "off4", "none"), ("only_rgb", "fresh", "face"), ("all", "off8", "none"),
+                                ("all", "off4", "corner"))]
+# NR_FWD_STAGE_TEXTURES where it really stages (cube kinds, no anti-aliasing, 16-byte aligned textures, 16-byte cubes:
+# ts even), and once with ts = 6 (2592-byte cubes, 12 slots per row segment) where a pixel row shows more runs of
+# distinct faces than there are slots, so the runs beyond the capacity read global memory
+MUST_NEW += [{"kind": "cube", "stage": True, "_aa": False, "pointers": "fresh", "ts": 2, "light": "face", "upstream": "all",
+              "batch": "B3"},
+         {"kind": "cube_shared", "stage": True, "_aa": False, "pointers": "fresh", "ts": 4, "light": "none"},
+         {"kind": "cube", "stage": True, "_aa": False, "pointers": "fresh", "ts": 6, "light": "none", "fill_back": False,
+          "batch": "B3", "raster": "even"}]
 
 
-def cases():
-    covered = set()
-    out = []
-    for n, seed in enumerate(MUST):
-        c = _fill(dict(seed), covered, n)
-        covered |= pairs_of(c)
-        out.append(c)
-    for n, (kind, fb, aa, bwd) in enumerate(itertools.product(LEVELS["kind"], LEVELS["fill_back"], (False, True),
-                                                             LEVELS["backward"])):
-        c = _fill({"kind": kind, "fill_back": fb, "_aa": aa, "backward": bwd}, covered, n)
-        covered |= pairs_of(c)
-        out.append(c)
-    missing = sorted(required_pairs() - covered, key=repr)
+def _complete(out, covered, choices, pairs):
+    """append rows until every pair of `pairs` (required_pairs of some levels) is covered"""
+    missing = sorted(pairs - covered, key=repr)
     n = len(out)
     while missing:
         (d1, l1), (d2, l2) = missing[0]
         seed = {d1: l1, d2: l2}
         if "kind" not in seed:  # a kind under which both levels mean something
             seed["kind"] = next(k for k in LEVELS["kind"] if active(d1, k) and active(d2, k) and compatible({**seed, "kind": k}))
-        c = _fill(seed, covered, n)
+        c = _fill(seed, covered, n, choices)
         covered |= pairs_of(c)
         out.append(c)
-        missing = sorted(required_pairs() - covered, key=repr)
+        missing = sorted(pairs - covered, key=repr)
         n += 1
+
+
+def cases():
+    covered = set()
+    out = []
+    # the earlier matrix, first
+    for n, seed in enumerate(MUST):
+        c = _fill(dict(seed), covered, n, BASE)
+        covered |= pairs_of(c)
+        out.append(c)
+    for n, (kind, fb, aa, bwd) in enumerate(itertools.product(LEVELS["kind"], LEVELS["fill_back"], (False, True),
+                                                             LEVELS["backward"])):
+        c = _fill({"kind": kind, "fill_back": fb, "_aa": aa, "backward": bwd}, covered, n, BASE)
+        covered |= pairs_of(c)
+        out.append(c)
+    _complete(out, covered, BASE, required_pairs(BASE_PAIRS))
+    # then the rows and pairs of every level
+    for seed in MUST_NEW:
+        c = _fill(dict(seed), covered, len(out))
+        covered |= pairs_of(c)
+        out.append(c)
+    _complete(out, covered, LEVELS, required_pairs())
     for i, c in enumerate(out):
         c["id"] = i
     return out
@@ -150,7 +210,10 @@ def cases():
 
 def case_id(c):
     parts = [c["kind"] + ("%d" % c["ts"] if c["ts"] else ""), "fb" if c["fill_back"] else "", c["raster"], c["backward"],
-             c["geometry"], ("img-" + c["image"] + ",uv-" + c["uvs"]) if c["image"] else "", "lit" if c["light"] else "",
-             "bgB" if c["bg"] == "per_batch" else "", c["outputs"], "z0" if c["z_batch0"] else "", c["batch"],
-             "up-" + c["upstream"], c["pointers"], "nulls" if c["optional"] == "null" else ""]
+             c["geometry"], ("img-" + c["image"] + ",uv-" + c["uvs"]) if c["image"] else "",
+             "uvgrad" if c["uv_grad"] == "given" else "", {"none": "", "face": "lit", "corner": "smooth"}[c["light"]],
+             "stage" if c["stage"] else "", "bgB" if c["bg"] == "per_batch" else "", c["outputs"],
+             "z0" if c["z_batch0"] else "", c["batch"], "up-" + c["upstream"], c["pointers"],
+             "nulls" if c["optional"] == "null" else "", "short" if c["layout"] == "short" else "",
+             "" if c["attr"] == "off" else "attr-" + c["attr"]]
     return "%03d-" % c["id"] + "-".join(p for p in parts if p)

@@ -1,16 +1,21 @@
-"""Direct C-ABI harness for nr_b200_forward / nr_b200_backward (test infrastructure).
+"""Direct C-ABI harness for nr_b200_forward, nr_b200_backward / nr_b200_backward_corner_light and nr_b200_interpolate /
+nr_b200_interpolate_backward (test infrastructure).
 
-It fills _lib.ForwardArgs / BackwardArgs itself -- no Python wrapper in between -- from a case of abi_cases.py, so that
-each case controls the exact flag word, which optional pointers are NULL, where every user buffer sits (fresh, or 4
-bytes into a slightly larger allocation; grad_textures also 8 bytes in: 2-float but not 4-float aligned) and what every
-output buffer holds before the call: NaN in each float output and a sentinel in face_index_map, so an element the
-kernels fail to write shows, or seeded values for NR_GRAD_ACCUMULATE.  Guard words around every buffer show a
-store just outside it.
+It fills _lib.ForwardArgs / BackwardArgs / InterpolateArgs itself -- no Python wrapper in between -- from a case of
+abi_cases.py, so that each case controls the exact flag word, the struct size (the full layouts, or the short ones that
+end before corner_light / grad_face_uvs), which optional pointers are NULL, where every user buffer sits (fresh, or 4
+bytes into a slightly larger allocation; grad_textures, grad_face_uvs and grad_corner_light also 8 bytes in: 2-float but
+not 4-float aligned) and what every output buffer holds before the call: NaN in each float output and a sentinel in
+face_index_map, so an element the kernels fail to write shows, or seeded values for NR_GRAD_ACCUMULATE.  Guard words
+around every buffer show a store just outside it.  With a short layout the field just past struct_size points at a real,
+NaN-filled, guarded buffer: the forward would light the image with NaN if it read it, and the backward must leave it
+as it was, bit for bit.
 
 The alignment cases stay inside the ABI's promise (float alignment).  Every vector access of a user buffer in csrc/ is
 behind a host check on its address: the edge scan's side fill of grad_textures (16 bytes, else a memset), the staged
 strips of the edge scan (8 bytes on face_index_map, rgb_map, grad_rgb, grad_alpha), the TMA staging of texture cubes
-(16 bytes), and the v4 / v2 reductions of k_texture_grad / k_image_grad, which pick their width from the address."""
+(16 bytes), and the v4 / v2 reductions of k_texture_grad / k_image_grad (grad_textures, grad_face_uvs), which pick their
+width from the address."""
 import ctypes
 
 import numpy as np
@@ -22,6 +27,8 @@ RASTER = {"even": (64, 64), "odd": (57, 57), "aa": (66, 33)}  # raster S, API im
 F_FRONT = {False: 201, True: 101}  # front faces; fill_back appends the reversed copies: F = 201 or 202 (odd / even)
 UV_SIZES = [(17, 41), (32, 32), (9, 30), (1, 9), (24, 13)]
 MIP_SIZES = [(37, 29), (64, 48), (17, 41), (1, 9)]
+ATTR_CHANNELS = [1, 3, 4, 16]
+K_STAGE_BYTES = 32 * 1024  # shared memory of a staged k_resolve CTA (csrc/nr_forward.cu kStageBytes)
 
 
 def _lib():
@@ -58,9 +65,16 @@ class Plan:
             sizes = MIP_SIZES if self.mip else UV_SIZES
             self.Ht, self.Wt = sizes[c["id"] % len(sizes)]
         self.P = int(L.load().nr_b200_mip_texels(self.Ht, self.Wt)) if self.mip else 0
-        self.lit = bool(c["light"])
+        self.lit = c["light"] == "face"
+        self.corner = c["light"] == "corner"
+        self.uv_grad = c["uv_grad"] == "given"
+        self.short = c["layout"] == "short"
         self.bg_batch = c["bg"] == "per_batch"
         self.given = c["optional"] == "given"
+        self.attr = c["attr"] != "off"
+        self.attr_pv = c["attr"].startswith("vertex")
+        self.attr_shared = c["attr"].endswith("_shared")
+        self.C = ATTR_CHANNELS[c["id"] % len(ATTR_CHANNELS)] if self.attr else 0
         f = 0
         f |= L.NR_RETURN_RGB if self.rgb else 0
         f |= L.NR_RETURN_ALPHA if self.alpha else 0
@@ -76,6 +90,11 @@ class Plan:
         f |= L.NR_UV_SHARED if (self.uv_shared and shared_flags) else 0
         f |= L.NR_TEX_MIPMAP if self.mip else 0
         self.flags = f
+        self.fwd_flags = f | (L.NR_FWD_STAGE_TEXTURES if c["stage"] else 0)  # a forward-only bit
+        af = f & (L.NR_ANTI_ALIASING | L.NR_FACES_INDEXED | L.NR_INDICES_SHARED)
+        af |= L.NR_ATTR_PER_VERTEX if self.attr_pv else 0
+        af |= L.NR_ATTR_SHARED if (self.attr_shared and shared_flags) else 0
+        self.attr_flags = af
         up = c["upstream"]
         self.g_rgb = self.rgb and up in ("all", "only_rgb")
         self.g_alpha = self.alpha and up in ("all", "no_rgb")
@@ -101,13 +120,19 @@ class Plan:
                 bufs["faces"] = ((B, F, 3, 3), f32)
         else:
             bufs["faces"] = ((B, F, 3, 3), f32)
+        nu = self.F_front if self.fill_back else F
+        uv_shape = (nu, 3, 2) if self.uv_shared else (B, nu, 3, 2)
         if self.rgb:
             bufs["textures"] = (tex_shape, f32)
             if self.lit:
                 bufs["face_light"] = ((B, F, 3), f32)
+            if self.corner:
+                bufs["corner_light"] = ((B, F, 3, 3), f32)
             if self.uv:
-                nu = self.F_front if self.fill_back else F
-                bufs["face_uvs"] = (((nu, 3, 2) if self.uv_shared else (B, nu, 3, 2)), f32)
+                bufs["face_uvs"] = (uv_shape, f32)
+        if self.short:  # what the fields past the short layouts point at: never to be read
+            bufs["past_end_fwd"] = ((B, F, 3, 3), f32)
+            bufs["past_end_bwd"] = ((uv_shape if self.uv else (B, F, 3, 2)), f32)
         if self.bg_batch and (self.rgb or self.given):
             bufs["background_batch"] = ((B, 3), f32)
         bufs["face_index_map"] = ((B, S, S), i32)
@@ -138,28 +163,49 @@ class Plan:
             bufs["grad_textures"] = (tex_shape, f32)
             if self.lit and self.given:
                 bufs["grad_face_light"] = ((B, F, 3), f32)
+            if self.corner and self.given:
+                bufs["grad_corner_light"] = ((B, F, 3, 3), f32)
+            if self.uv_grad:
+                bufs["grad_face_uvs"] = (uv_shape, f32)
+        if self.attr:  # attribute interpolation on the forward's maps, with gradient buffers of its own
+            C, Ba = self.C, (1 if self.attr_shared else B)
+            bufs["attributes"] = (((Ba, Nv, C) if self.attr_pv else (Ba, F, 3, C)), f32)
+            bufs["attr_out"] = ((B, C, H, H), f32)
+            bufs["attr_grad_out"] = ((B, C, H, H), f32)
+            bufs["attr_grad_attributes"] = (bufs["attributes"][0], f32)
+            if self.given:  # the interior vertex gradient is optional (NULL = not wanted)
+                bufs["attr_grad_vertices" if self.indexed else "attr_grad_faces"] = (((B, Nv, 3) if self.indexed
+                                                                                      else (B, F, 3, 3)), f32)
         self.bufs = bufs
-        self.bwd_textures = self.rgb and (self.given or "grad_face_light" in bufs)  # textures may be NULL in the backward
+        # textures may be NULL in the backward unless a gradient that reads them is wanted
+        self.bwd_textures = self.rgb and (self.given or self.uv_grad or "grad_face_light" in bufs)
         p = c["pointers"]
         self.offsets = {k: (0 if p == "fresh" else 4) for k in bufs}
-        if "grad_textures" in bufs and p == "off8":
-            self.offsets["grad_textures"] = 8
+        if p == "off8":
+            for k in ("grad_textures", "grad_face_uvs", "grad_corner_light"):
+                if k in bufs:
+                    self.offsets[k] = 8
         self.fwd_outputs = [k for k in ("face_index_map", "weight_map", "depth_map", "rgb_map", "alpha_map", "out_rgb",
                                         "out_alpha", "out_depth") if k in bufs]
-        self.grad_outputs = [k for k in ("grad_faces", "grad_vertices", "grad_textures", "grad_face_light") if k in bufs]
+        self.grad_outputs = [k for k in ("grad_faces", "grad_vertices", "grad_textures", "grad_face_light",
+                                         "grad_corner_light", "grad_face_uvs", "attr_grad_attributes",
+                                         "attr_grad_faces", "attr_grad_vertices") if k in bufs]
 
     # ---- the argument structs, from name -> address (int) of each buffer the case passes
     def forward_args(self, ptr, workspace, workspace_bytes):
         L = _lib()
         a = L.ForwardArgs()
-        a.struct_size = ctypes.sizeof(L.ForwardArgs)
-        a.flags = self.flags
+        a.struct_size = L.ForwardArgs.corner_light.offset if self.short else ctypes.sizeof(L.ForwardArgs)
+        a.flags = self.fwd_flags
         a.batch_size, a.num_faces, a.raster_size, a.texture_size = self.B, self.F, self.S, self.ts
         a.near_, a.far_, a.eps = NEAR, FAR, EPS
         a.background[0], a.background[1], a.background[2] = UNIFORM_BG
         for k in ("faces", "textures", "background_batch", "face_index_map", "weight_map", "depth_map", "rgb_map",
-                  "alpha_map", "out_rgb", "out_alpha", "out_depth", "face_light", "vertices", "face_indices", "face_uvs"):
+                  "alpha_map", "out_rgb", "out_alpha", "out_depth", "face_light", "vertices", "face_indices", "face_uvs",
+                  "corner_light"):
             setattr(a, k, ptr.get(k))
+        if self.short:
+            a.corner_light = ptr.get("past_end_fwd")
         a.num_vertices = self.Nv if self.indexed else 0
         a.texture_height, a.texture_width = self.Ht, self.Wt
         a.workspace, a.workspace_bytes = workspace, workspace_bytes
@@ -168,18 +214,44 @@ class Plan:
     def backward_args(self, ptr, flags, workspace, workspace_bytes):
         L = _lib()
         a = L.BackwardArgs()
-        a.struct_size = ctypes.sizeof(L.BackwardArgs)
+        a.struct_size = L.BackwardArgs.grad_face_uvs.offset if self.short else ctypes.sizeof(L.BackwardArgs)
         a.flags = flags
         a.batch_size, a.num_faces, a.raster_size, a.texture_size = self.B, self.F, self.S, self.ts
         a.eps = EPS
         for k in ("faces", "face_index_map", "weight_map", "depth_map", "rgb_map", "grad_rgb", "grad_alpha",
                   "grad_depth", "grad_faces", "grad_textures", "face_light", "grad_face_light", "vertices",
-                  "face_indices", "grad_vertices", "face_uvs"):
+                  "face_indices", "grad_vertices", "face_uvs", "grad_face_uvs"):
             setattr(a, k, ptr.get(k))
+        if self.short:
+            a.grad_face_uvs = ptr.get("past_end_bwd")
         a.textures = ptr.get("textures") if self.bwd_textures else None
         a.num_vertices = self.Nv if self.indexed else 0
         a.texture_height, a.texture_width = self.Ht, self.Wt
         a.workspace, a.workspace_bytes = workspace, workspace_bytes
+        return a
+
+    def call_backward(self, lib, a, ptr, stream):
+        """nr_b200_backward_corner_light for a smooth-shaded case, else nr_b200_backward"""
+        if self.corner:
+            return lib.nr_b200_backward_corner_light(ctypes.byref(a), ptr.get("corner_light"),
+                                                     ptr.get("grad_corner_light"), stream)
+        return lib.nr_b200_backward(ctypes.byref(a), stream)
+
+    def interpolate_args(self, ptr, backward):
+        """InterpolateArgs of the case's attribute interpolation (forward, or backward with its gradient buffers)"""
+        L = _lib()
+        a = L.InterpolateArgs()
+        a.struct_size = ctypes.sizeof(L.InterpolateArgs)
+        a.flags = self.attr_flags | (L.NR_GRAD_ACCUMULATE if (backward and self.accumulate) else 0)
+        a.batch_size, a.num_faces, a.raster_size, a.channels = self.B, self.F, self.S, self.C
+        a.faces, a.vertices, a.face_indices = ptr.get("faces"), ptr.get("vertices"), ptr.get("face_indices")
+        a.num_vertices = self.Nv if self.indexed else 0
+        a.face_index_map, a.weight_map, a.attributes = ptr.get("face_index_map"), ptr.get("weight_map"), ptr.get("attributes")
+        if backward:
+            a.grad_out, a.grad_attributes = ptr.get("attr_grad_out"), ptr.get("attr_grad_attributes")
+            a.grad_faces, a.grad_vertices = ptr.get("attr_grad_faces"), ptr.get("attr_grad_vertices")
+        else:
+            a.out = ptr.get("attr_out")
         return a
 
     def backward_calls(self):
@@ -198,6 +270,83 @@ class Plan:
     def fake_pointers(self):
         """distinct non-NULL addresses with the case's offsets (host argument checks only: never dereferenced)"""
         return {k: 0x10000000 * (i + 1) + self.offsets[k] for i, k in enumerate(sorted(self.bufs))}
+
+
+def make_inputs(plan, seed):
+    """seeded numpy inputs of a case: the arrays the ABI calls read, plus `faces_mat` (the materialised fp32 faces)"""
+    from neural_renderer_b200 import synthetic
+    rng = np.random.default_rng(1000 + seed)
+    B, F, Nv = plan.B, plan.F, plan.Nv
+    verts, idx = synthetic.sphere_mesh(plan.F_front)
+    if plan.fill_back:
+        idx = np.concatenate((idx, idx[:, ::-1]), axis=0)
+    v = np.empty((B, Nv, 3), np.float32)
+    for b in range(B):
+        vb = (verts * 0.8) @ synthetic._rotation(rng).T + rng.normal(scale=0.01, size=verts.shape)
+        vb[:, 2] += 2.75
+        v[b] = vb.astype(np.float32)
+    d = {}
+    if plan.indexed:
+        if plan.idx_shared:
+            ind = idx.astype(np.int32)
+            if plan.case["geometry"] == "idx_shared_oor":  # about 3 % of the indices out of range, both sides
+                sel = rng.random(ind.shape) < 0.03
+                ind = np.where(sel, rng.choice(np.array([-1, -5, Nv, Nv + 7, 1 << 30], np.int32), size=ind.shape), ind)
+            d["face_indices"] = np.ascontiguousarray(ind, np.int32)
+            d["vertices"] = v
+            full = np.broadcast_to(ind, (B,) + ind.shape)
+        else:  # every item lists its vertices in its own order
+            vv = np.empty_like(v)
+            ind = np.empty((B,) + idx.shape, np.int32)
+            for b in range(B):
+                perm = rng.permutation(Nv)
+                vv[b, perm] = v[b]
+                ind[b] = perm[idx]
+            d["vertices"], d["face_indices"] = vv, ind
+            full = ind
+        valid = (full >= 0) & (full < Nv)
+        vsrc = d["vertices"]
+        d["faces_mat"] = np.where(valid[..., None], vsrc[np.arange(B)[:, None, None], np.clip(full, 0, Nv - 1)], 0).astype(np.float32)
+        if "faces" in plan.bufs:
+            d["faces"] = np.full((B, F, 3, 3), np.nan, np.float32)  # must be ignored
+    else:
+        d["faces"] = np.ascontiguousarray(v[:, idx])
+        d["faces_mat"] = d["faces"]
+    if "textures" in plan.bufs:
+        d["textures"] = rng.random(plan.bufs["textures"][0], dtype=np.float32)
+    if "face_light" in plan.bufs:
+        d["face_light"] = (0.5 + rng.random((B, F, 3))).astype(np.float32)
+    if "corner_light" in plan.bufs:
+        d["corner_light"] = (0.3 + 0.9 * rng.random((B, F, 3, 3))).astype(np.float32)
+    if "face_uvs" in plan.bufs:
+        shape = plan.bufs["face_uvs"][0]
+        if plan.mip:  # per-face spread from 1e-3 to 100: magnified, fractional and last-level LODs
+            centre = rng.random(shape[:-2] + (1, 2))
+            spread = 10.0 ** (-3 + 5 * rng.random(shape[:-2] + (1, 1)))
+            d["face_uvs"] = (centre + spread * (rng.random(shape) - 0.5)).astype(np.float32)
+        else:
+            d["face_uvs"] = (-0.2 + 1.4 * rng.random(shape)).astype(np.float32)
+    if "background_batch" in plan.bufs:
+        d["background_batch"] = rng.random((B, 3), dtype=np.float32)
+    for k in ("grad_rgb", "grad_alpha", "grad_depth", "attr_grad_out"):
+        if k in plan.bufs:
+            d[k] = rng.standard_normal(plan.bufs[k][0]).astype(np.float32)
+    if "attributes" in plan.bufs:
+        d["attributes"] = (2.0 + rng.standard_normal(plan.bufs["attributes"][0])).astype(np.float32)
+    for k in ("past_end_fwd", "past_end_bwd"):
+        if k in plan.bufs:
+            d[k] = np.full(plan.bufs[k][0], np.nan, np.float32)
+    return d
+
+
+def stage_runs(plan):
+    """whether the forward stages texture cubes (the predicate of nr_b200_forward), and the slots per row segment"""
+    if not (plan.rgb and plan.case["stage"] and not plan.uv and not plan.corner and not plan.aa):
+        return False, 0
+    cube_bytes = plan.ts ** 3 * 12
+    ok = cube_bytes % 16 == 0 and cube_bytes <= K_STAGE_BYTES // 8 and plan.offsets["textures"] % 16 == 0
+    bx = 256 if plan.S >= 256 else (plan.S + 31) // 32 * 32
+    return ok, min(K_STAGE_BYTES // cube_bytes, bx)
 
 
 # ---- device side
@@ -254,7 +403,7 @@ def forward(plan, buf, dev):
     lib = L.load()
     for k in plan.fwd_outputs:
         poison(buf[k])
-    nbytes = lib.nr_b200_forward_workspace_bytes(plan.B, plan.F, plan.S, plan.ts, plan.flags)
+    nbytes = lib.nr_b200_forward_workspace_bytes(plan.B, plan.F, plan.S, plan.ts, plan.fwd_flags)
     ws = workspace(nbytes, dev)
     a = plan.forward_args({k: t.data_ptr() for k, t in buf.items()}, ws.data_ptr(), ws.numel())
     rc = lib.nr_b200_forward(ctypes.byref(a), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
@@ -269,10 +418,34 @@ def backward(plan, buf, dev):
     L = _lib()
     lib = L.load()
     out = []
+    ptr = {k: t.data_ptr() for k, t in buf.items()}
+    stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
     for flags in plan.backward_calls():
         nbytes = lib.nr_b200_backward_workspace_bytes(plan.B, plan.F, plan.S, plan.ts, flags)
         ws = workspace(nbytes, dev)
-        a = plan.backward_args({k: t.data_ptr() for k, t in buf.items()}, flags, ws.data_ptr(), ws.numel())
-        out.append(lib.nr_b200_backward(ctypes.byref(a), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+        a = plan.backward_args(ptr, flags, ws.data_ptr(), ws.numel())
+        out.append(plan.call_backward(lib, a, ptr, stream))
     torch.cuda.synchronize(dev)
     return out
+
+
+def interpolate(plan, buf, dev):
+    """poison the attribute image, call nr_b200_interpolate on the saved maps, return the return code"""
+    import torch
+    lib = _lib().load()
+    poison(buf["attr_out"])
+    a = plan.interpolate_args({k: t.data_ptr() for k, t in buf.items()}, False)
+    rc = lib.nr_b200_interpolate(ctypes.byref(a), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+    torch.cuda.synchronize(dev)
+    return rc
+
+
+def interpolate_backward(plan, buf, dev):
+    """nr_b200_interpolate_backward (NR_GRAD_ACCUMULATE when the case's backward mode accumulates); the caller prepares
+    the gradient buffers as for backward()"""
+    import torch
+    lib = _lib().load()
+    a = plan.interpolate_args({k: t.data_ptr() for k, t in buf.items()}, True)
+    rc = lib.nr_b200_interpolate_backward(ctypes.byref(a), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+    torch.cuda.synchronize(dev)
+    return rc

@@ -15,6 +15,8 @@ def smooth_light64(faces, fim, wmap, dmap, corner_light):
     fi = fim.clamp(min=0).long()
     bidx = torch.arange(B, device=dev)[:, None, None].expand(B, S, S)
     z = faces.double()[..., 2][bidx, fi]
+    # an uncovered pixel reads face 0, which may have a zero depth (an out-of-range index): keep 0 * inf out of autograd
+    z = torch.where((fim >= 0)[..., None], z, torch.ones_like(z))
     lam = wmap.double().permute(0, 2, 3, 1) * (dmap.double()[..., None] / z)   # [B,S,S,3]
     C = corner_light.double()[bidx, fi]                                         # [B,S,S,3 corners,3]
     return (lam[..., None] * C).sum(dim=3)

@@ -30,6 +30,8 @@ def _pixel_uvs(faces, fim, wmap, dmap, uvs, fill_back, z64):
     fi = fim.clamp(min=0).long()
     bidx = torch.arange(B, device=dev)[:, None, None].expand(B, S, S)
     z = (faces.double() if z64 else faces)[..., 2][bidx, fi]
+    # an uncovered pixel reads face 0, which may have a zero depth (an out-of-range index): keep 0 * inf out of autograd
+    z = torch.where((fim >= 0)[..., None], z, torch.ones_like(z))
     w = wmap.permute(0, 2, 3, 1)
     zp = dmap[..., None]
     uvk = uvs[bidx, fi]
@@ -71,10 +73,17 @@ def oracle_rgb_uv_grad(faces, fim, wmap, dmap, uvs, image, light, bg, fill_back,
 def oracle_trilinear_uv_grad(faces, fim, wmap, dmap, uvs, image, light, bg, fill_back, aa):
     """trilinear sampler (oracles.oracle_trilinear: float64 pyramid and level of detail), differentiable in `uvs`; the
     level of detail is a constant.  Returns the API rgb [B,3,H,W]."""
+    Ht, Wt = image.shape[1:3]
+    return oracle_trilinear_levels_uv_grad(faces, fim, wmap, dmap, uvs, pyramid64(image.double()), Ht, Wt, light, bg,
+                                           fill_back, aa)
+
+
+def oracle_trilinear_levels_uv_grad(faces, fim, wmap, dmap, uvs, levels, Ht, Wt, light, bg, fill_back, aa):
+    """oracle_trilinear_uv_grad on given pyramid levels [1|B,H_l,W_l,3] (e.g. oracles.unpack_pyramid of the packed
+    `textures`)"""
     B = faces.shape[0]
     S = fim.shape[-1]
-    Ht, Wt = image.shape[1:3]
-    levels = [l.expand(B, -1, -1, -1) for l in pyramid64(image.double())]
+    levels = [l.double().expand(B, -1, -1, -1) for l in levels]
     L = len(levels)
     bidx, fi, uvk, uv_raw, st = _pixel_uvs(faces, fim, wmap, dmap, uvs, fill_back, z64=True)
     lod = lod64(faces, fim, wmap, dmap, uvk.detach(), S, Ht, Wt, L)

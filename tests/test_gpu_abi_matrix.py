@@ -1,4 +1,5 @@
-"""GPU: every pair of the rasterizer's C-ABI flags, called directly (tests/abi_harness.py), held to an unfused oracle.
+"""GPU: every pair of the C-ABI flag levels of the rasterizer (forward, backward, smooth-shading backward) and of the
+attribute interpolation on its maps, called directly (tests/abi_harness.py), held to an unfused oracle.
 
 The cases come from the covering array of tests/abi_cases.py.  The oracle never runs the product's fused paths:
   cubes       the inputs are materialised as a float64 torch function of (vertices | faces, textures, light) -- faces by
@@ -6,17 +7,41 @@ The cases come from the covering array of tests/abi_cases.py.  The oracle never 
               cat(t, t.permute(0,1,4,3,2,5)), the light multiplied in (in fp32 for the forward: the header pins the fused
               light as bit-identical to sampling the product) -- and rendered by the CPU oracle (oracle/nr_oracle.py,
               with per-item background and the batch-0 depth quirk as flagged; K5 summed in float64).  Its face /
-              texture gradients are chained back to vertices, textures and light by float64 autograd.
+              texture gradients are chained back to vertices, textures and light by float64 autograd.  NR_FWD_STAGE_TEXTURES
+              changes nothing here: a staged render is held bit-exact like any other.
   images      the float64 samplers of tests/oracles.py on the materialised geometry (bilinear, or trilinear on the
               packed pyramid passed as `textures`); the face / vertex gradient from the CPU oracle's K5 fed with the
-              product's own raster rgb map.
-Gates: face_index_map, weight_map and depth_map bit-exact; images bit-exact in non-anti-aliased cube mode, 1e-5 relative
-elsewhere; every gradient tensor 1e-4 per tensor (helpers.rel_err) and per element (helpers.elem_err); the mip sampler's
-image and pyramid gradient are the two exceptions, with their cause and measured maxima below.  Every output is poisoned
-before a call (NaN, face-index sentinel), so an element the kernels do not write fails, and guard words around every
-buffer must survive both calls, so a store just outside one fails; with
-NR_GRAD_ACCUMULATE the gradients are prefilled with seeded values and must come back as prefill + fresh gradient, the
-prefill untouched bit for bit wherever the oracle's fresh gradient is exactly 0."""
+              product's own raster rgb map.  grad_face_uvs from the straight-through samplers of tests/oracles_uv_grad.py,
+              the fill_back fold and the sum over items of shared UVs by autograd.
+  smooth      corner_light: the light oracles_smooth.smooth_light64 (each item's own depths, on the maps) times the unlit
+              sample -- for cubes the CPU oracle's unlit render (bit-exact, NR_TEX_Z_BATCH0 honoured), for images the
+              samplers above; grad_corner_light by float64 autograd of that image, the cube texture gradient from the
+              CPU oracle's K6 sampling maps fed the raster upstream gradient times the light (summed in float64: the
+              fp32 sums of the oracle's own K6 are up to 3e-5 per element off there), K5 fed the product's lit rgb map.
+  attributes  oracles_attr.interp64 on the float64 materialised faces (fill_back copies included) and corner
+              attributes gathered in float64 (out-of-range indices read zeros), at the product's weights; the attribute
+              and interior vertex gradients by autograd back through the gathers.  A face with an out-of-range corner
+              (a zero vertex: z = 0 puts zp below near) must never win a pixel, and that is checked.
+Gates: face_index_map, weight_map and depth_map bit-exact; images bit-exact in non-anti-aliased, unlit or flat-lit cube
+mode, 1e-5 relative elsewhere; every gradient tensor 1e-4 per tensor (helpers.rel_err) and per element (helpers.elem_err),
+with the exceptions of the feature tests (test_gpu_smooth.py, test_gpu_uv_grad.py, test_gpu_attr.py, with their causes
+there): the trilinear sampler's image and per-element gradients, the attribute image (1e-6), the attribute gradient per
+tensor (1e-5) and the interpolation's interior vertex gradient per element (2.5e-3).
+Measured maxima over this matrix (177 cases) on an H100 80GB HBM3 at 400 W, per gate:
+  raster / anti-aliased image, trilinear   4.4e-5 / 5.1e-6 (cases 101, 116)    gate 6e-5
+  raster / anti-aliased image, smooth      1.6e-7 / 1.4e-7                      gate 1e-5
+  pyramid gradient per element             3.6e-4 (case 101)                    gate 5e-4
+  grad_corner_light per tensor / element   4.2e-7 / 2.9e-5; trilinear 5.4e-5   gates 1e-4 / 1e-4, 5e-4
+  grad_face_uvs per tensor / element       2.9e-7 / 4.1e-5; trilinear 5.3e-5   gates 1e-4 / 1e-4, 1.5e-3
+  attribute image                          2.0e-7                               gate 1e-6
+  attribute gradient per tensor / element  9.8e-7 / 5.4e-5                      gates 1e-5 / 1e-4
+  interior vertex gradient tensor / elem   6.1e-5 / 1.5e-3 (case 129)           gates 1e-4 / 2.5e-3
+  every other gradient per element         9.5e-5 (case 136; with NR_GRAD_ACCUMULATE 7.5e-5)
+Every output is poisoned before a call (NaN, face-index sentinel), so an element the kernels do not write fails, and
+guard words around every buffer must survive the calls, so a store just outside one fails; with NR_GRAD_ACCUMULATE the
+gradients are prefilled with seeded values and must come back as prefill + fresh gradient, the prefill untouched bit for
+bit wherever the oracle's fresh gradient is exactly 0.  With a short struct layout the field past its end points at a
+NaN-filled buffer that must come back bit for bit (and would light the forward image with NaN if read)."""
 import numpy as np
 import pytest
 import torch
@@ -33,78 +58,18 @@ TOL_IMAGE = 1e-5
 # NR_TEX_MIPMAP relaxes two gates.  The product evaluates the level of detail in fp32 (include/nr_b200.h), the oracle in
 # float64 (oracles.lod64), and the pyramid here is random data, so neighbouring levels differ by O(1) and a pixel's colour
 # moves by about its LOD difference; a texel whose gradient comes only through a small blend weight f (or 1 - f) sees
-# the same absolute difference relative to its own size.  Measured maxima over the matrix on an H100: raster image
-# 4.4e-5, anti-aliased image 5.1e-6, pyramid gradient per element 3.6e-4 (both in case 101), light gradient per element
-# 7.5e-5 (inside TOL_GRAD).  Every other gate holds at its nominal value (largest per-element gradient error 5.9e-5,
-# with NR_GRAD_ACCUMULATE 4.0e-5).
+# the same absolute difference relative to its own size (measured maxima in the module docstring).
 TOL_IMAGE_MIP = 6e-5
 TOL_GRAD_ELEM_MIP = 5e-4
+# the gates of the smooth-shading, face_uvs-gradient and attribute tests (test_gpu_smooth.py, test_gpu_uv_grad.py,
+# test_gpu_attr.py, with their causes there); measured maxima over this matrix in the module docstring
+TOL_CORNER_ELEM_MIP = 5e-4   # grad_corner_light per element with NR_TEX_MIPMAP
+TOL_UV_ELEM_MIP = 1.5e-3     # grad_face_uvs per element with NR_TEX_MIPMAP
+TOL_ATTR_IMAGE = 1e-6        # interpolated attribute image
+TOL_ATTR = 1e-5              # attribute gradient per tensor (per element TOL_GRAD)
+TOL_INTERIOR = 1e-4          # interior vertex gradient of the interpolation per tensor
+TOL_INTERIOR_ELEM = 2.5e-3   # and per element
 CASES = abi_cases.cases()
-
-
-def _rotation(rng):
-    from neural_renderer_b200 import synthetic
-    return synthetic._rotation(rng)
-
-
-def make_inputs(plan, seed):
-    """seeded numpy inputs of a case: the arrays the ABI call reads, plus `faces_mat` (the materialised fp32 faces)"""
-    from neural_renderer_b200 import synthetic
-    rng = np.random.default_rng(1000 + seed)
-    B, F, Nv = plan.B, plan.F, plan.Nv
-    verts, idx = synthetic.sphere_mesh(plan.F_front)
-    if plan.fill_back:
-        idx = np.concatenate((idx, idx[:, ::-1]), axis=0)
-    v = np.empty((B, Nv, 3), np.float32)
-    for b in range(B):
-        vb = (verts * 0.8) @ _rotation(rng).T + rng.normal(scale=0.01, size=verts.shape)
-        vb[:, 2] += 2.75
-        v[b] = vb.astype(np.float32)
-    d = {}
-    if plan.indexed:
-        if plan.idx_shared:
-            ind = idx.astype(np.int32)
-            if plan.case["geometry"] == "idx_shared_oor":  # about 3 % of the indices out of range, both sides
-                sel = rng.random(ind.shape) < 0.03
-                ind = np.where(sel, rng.choice(np.array([-1, -5, Nv, Nv + 7, 1 << 30], np.int32), size=ind.shape), ind)
-            d["face_indices"] = np.ascontiguousarray(ind, np.int32)
-            d["vertices"] = v
-            full = np.broadcast_to(ind, (B,) + ind.shape)
-        else:  # every item lists its vertices in its own order
-            vv = np.empty_like(v)
-            ind = np.empty((B,) + idx.shape, np.int32)
-            for b in range(B):
-                perm = rng.permutation(Nv)
-                vv[b, perm] = v[b]
-                ind[b] = perm[idx]
-            d["vertices"], d["face_indices"] = vv, ind
-            full = ind
-        valid = (full >= 0) & (full < Nv)
-        vsrc = d["vertices"]
-        d["faces_mat"] = np.where(valid[..., None], vsrc[np.arange(B)[:, None, None], np.clip(full, 0, Nv - 1)], 0).astype(np.float32)
-        if "faces" in plan.bufs:
-            d["faces"] = np.full((B, F, 3, 3), np.nan, np.float32)  # must be ignored
-    else:
-        d["faces"] = np.ascontiguousarray(v[:, idx])
-        d["faces_mat"] = d["faces"]
-    if "textures" in plan.bufs:
-        d["textures"] = rng.random(plan.bufs["textures"][0], dtype=np.float32)
-    if "face_light" in plan.bufs:
-        d["face_light"] = (0.5 + rng.random((B, F, 3))).astype(np.float32)
-    if "face_uvs" in plan.bufs:
-        shape = plan.bufs["face_uvs"][0]
-        if plan.mip:  # per-face spread from 1e-3 to 100: magnified, fractional and last-level LODs
-            centre = rng.random(shape[:-2] + (1, 2))
-            spread = 10.0 ** (-3 + 5 * rng.random(shape[:-2] + (1, 1)))
-            d["face_uvs"] = (centre + spread * (rng.random(shape) - 0.5)).astype(np.float32)
-        else:
-            d["face_uvs"] = (-0.2 + 1.4 * rng.random(shape)).astype(np.float32)
-    if "background_batch" in plan.bufs:
-        d["background_batch"] = rng.random((B, 3), dtype=np.float32)
-    for k in ("grad_rgb", "grad_alpha", "grad_depth"):
-        if k in plan.bufs:
-            d[k] = rng.standard_normal(plan.bufs[k][0]).astype(np.float32)
-    return d
 
 
 def materialise(plan, d, geom, tex, light):
@@ -128,10 +93,33 @@ def materialise(plan, d, geom, tex, light):
     return faces, cubes
 
 
+def _upsample(g, aa):
+    """API-layout upstream gradient -> the raster gradient the backward sees (pooling: each raster pixel gets g / 4)"""
+    return g.repeat_interleave(2, -1).repeat_interleave(2, -2) * 0.25 if aa else g
+
+
+def _k6_64(fn, G):
+    """the CPU oracle's texture backward (K6: each covered raster pixel sends weight x upstream gradient to the 8 texels
+    its sample blended, through the oracle's sampling maps), summed in float64; G [B,S,S,3] raster layout, float64"""
+    B, F, ts = fn.batch_size, fn.num_faces, fn.texture_size
+    out = np.zeros((B, F, ts ** 3, 3))
+    fim = fn.face_index_map.reshape(B, -1)
+    w = fn.sampling_weight_map.reshape(B, -1, 8).astype(np.float64)
+    idx = fn.sampling_index_map.reshape(B, -1, 8)
+    g = np.asarray(G, np.float64).reshape(B, -1, 3)
+    for b in range(B):
+        cov = fim[b] >= 0
+        np.add.at(out[b], (np.repeat(fim[b][cov], 8), idx[b][cov].reshape(-1)),
+                  (w[b][cov][..., None] * g[b][cov][:, None, :]).reshape(-1, 3))
+    return out.reshape(fn.textures.shape)
+
+
 def oracle(plan, d, got):
     """(forward reference {name: tensor in the product's layout}, fresh gradients {buffer name: float64 numpy})"""
     import nr_oracle
     from oracles import oracle_rgb, oracle_trilinear_levels, unpack_pyramid
+    from oracles_smooth import smooth_light64, smooth_rgb
+    from oracles_uv_grad import oracle_rgb_uv_grad, oracle_trilinear_levels_uv_grad
     B, S = plan.B, plan.S
     t = lambda k, dt=torch.float32: torch.from_numpy(np.ascontiguousarray(d[k])).to(dt) if k in d else None
     geom_key = "vertices" if plan.indexed else "faces"
@@ -148,46 +136,89 @@ def oracle(plan, d, got):
     if plan.alpha:
         ref["alpha_map"] = torch.from_numpy(fn.alpha_map).flip(1)
     if plan.aa:
-        for k in ("alpha", "depth") + (("rgb",) if cube else ()):
+        for k in ("alpha", "depth") + (("rgb",) if cube and not plan.corner else ()):
             if res[k] is not None:
                 ref["out_" + k] = torch.from_numpy(res[k])
     grads = {}
     g = lambda k: d.get(k)
-    if cube:
+    # the product's maps (held bit-exact to the oracle's above) for the float64 samplers, light and interpolation
+    fim, wmap, dmap = (got[k] for k in ("face_index_map", "weight_map", "depth_map"))
+    fm = torch.from_numpy(d["faces_mat"]).to(DEV)
+    bgd = torch.from_numpy(np.asarray(bg)).to(DEV)
+    g_rgb = torch.from_numpy(d["grad_rgb"]).to(DEV).double() if "grad_rgb" in d else None
+    c64 = L64 = None
+    if plan.corner:  # smooth shading: float64 light from each item's own depths, times the unlit sample
+        c64 = torch.from_numpy(d["corner_light"]).to(DEV).double().requires_grad_(True)
+        L64 = smooth_light64(fm, fim, wmap, dmap, c64)
+
+    def grad_of(out, ins):
+        if g_rgb is None:
+            return [torch.zeros_like(x) for x in ins]
+        return torch.autograd.grad((out * g_rgb).sum(), ins)
+    gt_corner = None
+    if cube and plan.corner:
+        # the CPU oracle's unlit raster sample (bit-exact, NR_TEX_Z_BATCH0 honoured) lit by the float64 light
+        unlit = torch.from_numpy(fn.rgb_map).permute(0, 3, 1, 2).flip(2).to(DEV)
+        ref["rgb_map"] = smooth_rgb(unlit, L64, fim, bgd, False).detach()
+        out = smooth_rgb(unlit, L64, fim, bgd, plan.aa)
+        if plan.aa:
+            ref["out_rgb"] = out.detach()
+        grads["grad_corner_light"] = grad_of(out, [c64])[0].detach().cpu().numpy()
+        # K6 of the oracle fed the raster upstream gradient times the light, in float64
+        if g_rgb is not None:
+            G = (_upsample(g_rgb, plan.aa) * L64.detach().permute(0, 3, 1, 2)).flip(2).permute(0, 2, 3, 1)
+            gt_corner = _k6_64(fn, G.cpu().numpy())
+        else:
+            gt_corner = np.zeros_like(fn.textures)
+        fn.rgb_map = np.ascontiguousarray(got["rgb_map"].permute(0, 2, 3, 1).flip(1).cpu().numpy())
+    elif cube:
         ref["rgb_map"] = torch.from_numpy(fn.rgb_map).permute(0, 3, 1, 2).flip(2)
     elif plan.rgb:
-        # the texture-image sampler on the product's maps (held bit-exact to the oracle's above), in float64
-        fim, wmap, dmap = (got[k] for k in ("face_index_map", "weight_map", "depth_map"))
-        fm = torch.from_numpy(d["faces_mat"]).to(DEV)
+        # the texture-image sampler on the product's maps, in float64
         uvs = torch.from_numpy(d["face_uvs"]).to(DEV)
         uvs = uvs[None] if uvs.dim() == 3 else uvs
         tex64 = torch.from_numpy(d["textures"]).to(DEV).double().requires_grad_(True)
         light64 = torch.from_numpy(d["face_light"]).to(DEV).double().requires_grad_(True) if plan.lit else None
-        bgd = torch.from_numpy(np.asarray(bg)).to(DEV)
+        zero_bg = torch.zeros(3, dtype=torch.float64, device=DEV)
 
-        def sample(aa):
+        def sample(aa, bg_, light, uv, uv_grad):
             if plan.mip:
-                return oracle_trilinear_levels(fm, fim, wmap, dmap, uvs, unpack_pyramid(tex64, plan.Ht, plan.Wt),
-                                               plan.Ht, plan.Wt, light64, bgd, plan.fill_back, aa)[0]
-            return oracle_rgb(fm, fim, wmap, dmap, uvs, tex64, light64, bgd, plan.fill_back, aa)
-        ref["rgb_map"] = sample(False).detach()
-        api = sample(True) if plan.aa else None
+                levels = unpack_pyramid(tex64, plan.Ht, plan.Wt)
+                if uv_grad:
+                    return oracle_trilinear_levels_uv_grad(fm, fim, wmap, dmap, uv, levels, plan.Ht, plan.Wt, light, bg_,
+                                                           plan.fill_back, aa)
+                return oracle_trilinear_levels(fm, fim, wmap, dmap, uv, levels, plan.Ht, plan.Wt, light, bg_,
+                                               plan.fill_back, aa)[0]
+            if uv_grad:
+                return oracle_rgb_uv_grad(fm, fim, wmap, dmap, uv, tex64, light, bg_, plan.fill_back, aa)
+            return oracle_rgb(fm, fim, wmap, dmap, uv, tex64, light, bg_, plan.fill_back, aa)
+
+        def image(aa, uv=uvs, uv_grad=False, L=None):
+            if plan.corner:  # the unlit sample times the interpolated light
+                return smooth_rgb(sample(False, zero_bg, None, uv, uv_grad), L, fim, bgd, aa)
+            return sample(aa, bgd, light64, uv, uv_grad)
+        ref["rgb_map"] = image(False, L=L64).detach()
+        out = image(plan.aa, L=L64)
         if plan.aa:
-            ref["out_rgb"] = api.detach()
-        out = api if plan.aa else sample(False)
-        ins = [tex64] + ([light64] if plan.lit else [])
-        if "grad_rgb" in d:
-            gi = torch.autograd.grad((out * torch.from_numpy(d["grad_rgb"]).to(DEV).double()).sum(), ins)
-        else:
-            gi = [torch.zeros_like(x) for x in ins]
+            ref["out_rgb"] = out.detach()
+        ins = [tex64] + ([light64] if plan.lit else []) + ([c64] if plan.corner else [])
+        gi = grad_of(out, ins)
         grads["grad_textures"] = gi[0].detach().cpu().numpy()
         if "grad_face_light" in plan.bufs:
             grads["grad_face_light"] = gi[1].detach().cpu().numpy()
+        if "grad_corner_light" in plan.bufs:
+            grads["grad_corner_light"] = gi[-1].detach().cpu().numpy()
+        if plan.uv_grad:  # through the straight-through UV oracles; autograd folds fill_back and sums shared UVs
+            uv64 = torch.from_numpy(d["face_uvs"]).to(DEV).double().requires_grad_(True)
+            img = image(plan.aa, uv64[None] if uv64.dim() == 3 else uv64, True, L64.detach() if plan.corner else None)
+            grads["grad_face_uvs"] = grad_of(img, [uv64])[0].detach().cpu().numpy()
         # K5 reads the rgb map: feed the oracle's edge scan the product's own (held to the float64 sampler above)
         fn.rgb_map = np.ascontiguousarray(got["rgb_map"].permute(0, 2, 3, 1).flip(1).cpu().numpy())
     fn.k5_sum_fp64 = True
     gf, gt = res.backward(g("grad_rgb") if plan.rgb else None, g("grad_alpha") if plan.alpha else None,
                           g("grad_depth") if plan.depth else None)
+    if gt_corner is not None:
+        gt = gt_corner
     # float64 chain of the oracle's face / cube gradients back to the inputs of the case
     geom64 = t(geom_key, torch.float64).requires_grad_(True)
     tex64 = t("textures", torch.float64).requires_grad_(True) if cube else None
@@ -205,11 +236,48 @@ def oracle(plan, d, got):
         grads["grad_textures"] = chained[1].numpy()
         if "grad_face_light" in plan.bufs:
             grads["grad_face_light"] = chained[2].numpy()
+    if plan.attr:
+        interp_oracle(plan, d, got, ref, grads)
     return ref, grads
+
+
+def interp_oracle(plan, d, got, ref, grads):
+    """attribute interpolation: oracles_attr.interp64 on the float64 materialised faces (fill_back copies included) and
+    corner attributes gathered in float64 (an out-of-range index reads zeros), at the product's weights; both gradients
+    by autograd back through the gathers"""
+    from oracles_attr import interp64
+    B, F, Nv = plan.B, plan.F, plan.Nv
+    fim, wmap = got["face_index_map"].cpu(), got["weight_map"].cpu()
+    geom64 = torch.from_numpy(d["vertices" if plan.indexed else "faces"]).double().requires_grad_(True)
+    f64 = materialise(plan, d, geom64, None, None)[0]
+    a64 = torch.from_numpy(d["attributes"]).double().requires_grad_(True)
+    if plan.attr_pv:
+        ind = torch.from_numpy(d["face_indices"].astype(np.int64)).expand(B, F, 3)
+        valid = ((ind >= 0) & (ind < Nv))[..., None]
+        ga = a64.expand(B, -1, -1)[torch.arange(B)[:, None, None], ind.clamp(0, Nv - 1)]
+        corner = torch.where(valid, ga, torch.zeros((), dtype=torch.float64))
+    else:
+        corner = a64.expand(B, -1, -1, -1)
+    img = interp64(f64, fim, corner, plan.S, plan.aa, wmap=wmap)
+    ref["attr_out"] = img.detach()
+    ga, gg = torch.autograd.grad((img * torch.from_numpy(d["attr_grad_out"]).double()).sum(), [a64, geom64])
+    grads["attr_grad_attributes"] = ga.numpy()
+    for k in ("attr_grad_faces", "attr_grad_vertices"):
+        if k in plan.bufs:
+            grads[k] = gg.numpy()
 
 
 def _bits(t):
     return t.contiguous().view(torch.int32)
+
+
+# gates of the gradients: (per tensor, per element, per element with NR_TEX_MIPMAP), measured maxima in the docstring
+GRAD_GATES = {"grad_corner_light": (TOL_GRAD, TOL_GRAD, TOL_CORNER_ELEM_MIP),
+              "grad_face_uvs": (TOL_GRAD, TOL_GRAD, TOL_UV_ELEM_MIP),
+              "attr_grad_attributes": (TOL_ATTR, TOL_GRAD, TOL_GRAD),
+              "attr_grad_faces": (TOL_INTERIOR, TOL_INTERIOR_ELEM, TOL_INTERIOR_ELEM),
+              "attr_grad_vertices": (TOL_INTERIOR, TOL_INTERIOR_ELEM, TOL_INTERIOR_ELEM),
+              "grad_textures": (TOL_GRAD, TOL_GRAD, TOL_GRAD_ELEM_MIP)}
 
 
 def run_case(c, metrics=None):
@@ -217,7 +285,7 @@ def run_case(c, metrics=None):
     value) of every gated comparison"""
     note = (lambda *m: metrics.append((c["id"],) + m)) if metrics is not None else (lambda *m: None)
     plan = H.Plan(c)
-    d = make_inputs(plan, c["id"])
+    d = H.make_inputs(plan, c["id"])
     buf = {k: H.alloc(shape, dt, plan.offsets[k], DEV) for k, (shape, dt) in plan.bufs.items()}
     for k, a in d.items():
         if k in buf:
@@ -226,26 +294,42 @@ def run_case(c, metrics=None):
     rc = H.forward(plan, buf, DEV)
     if rc != 0:
         return ["forward returned %d" % rc]
+    if plan.attr:
+        rc = H.interpolate(plan, buf, DEV)
+        if rc != 0:
+            return ["nr_b200_interpolate returned %d" % rc]
     fails += ["%s: a guard word next to the buffer changed in the forward" % k for k in buf if not H.guards_intact(buf[k])]
     got = {k: buf[k] for k in plan.fwd_outputs}
+    if plan.indexed:  # a face with an out-of-range corner has a zero vertex (z = 0): it must never win a pixel
+        ind = np.broadcast_to(d["face_indices"], (plan.B, plan.F, 3))
+        bad = ((ind < 0) | (ind >= plan.Nv)).any(-1)
+        fimn = got["face_index_map"].cpu().numpy()
+        won = bad[np.arange(plan.B)[:, None, None], np.clip(fimn, 0, plan.F - 1)] & (fimn >= 0)
+        if won.any():
+            fails.append("%d pixels won by a face with an out-of-range index" % int(won.sum()))
     ref, grads = oracle(plan, d, got)
     cov = int((got["face_index_map"] >= 0).sum())
     if cov < 300:
         fails.append("only %d covered pixels" % cov)
     cube = plan.kind in ("cube", "cube_shared")
-    for k in plan.fwd_outputs:
+    if plan.attr:
+        got["attr_out"] = buf["attr_out"]
+    for k in got:
         x, r = got[k].cpu(), ref[k].cpu()
-        if k in ("face_index_map", "weight_map", "depth_map", "alpha_map") or (k == "rgb_map" and cube):
+        if k in ("face_index_map", "weight_map", "depth_map", "alpha_map") or (k == "rgb_map" and cube and not plan.corner):
             if not torch.equal(x, r.to(x.dtype)):
                 fails.append("%s: %d elements differ" % (k, int((x != r.to(x.dtype)).sum())))
         else:
             e = rel_err(x.numpy(), r.numpy()) if torch.isfinite(x).all() else float("nan")
-            note(k, "mip" if plan.mip else "image", e)
-            if not e <= (TOL_IMAGE_MIP if plan.mip else TOL_IMAGE):
+            kind = "attr" if k == "attr_out" else ("mip" if plan.mip else ("smooth" if plan.corner else "image"))
+            note(k, kind, e)
+            if not e <= {"attr": TOL_ATTR_IMAGE, "mip": TOL_IMAGE_MIP}.get(kind, TOL_IMAGE):
                 fails.append("%s: rel_err %.3g" % (k, e))
     # ---- backward
     rng = np.random.default_rng(2000 + c["id"])
-    untouched = [k for k in ("grad_faces",) if plan.indexed and k in buf]  # ignored with NR_FACES_INDEXED
+    # ignored with NR_FACES_INDEXED; the field past the short backward struct
+    untouched = [k for k in ("grad_faces", "past_end_fwd", "past_end_bwd")
+                 if k in buf and (k != "grad_faces" or plan.indexed)]
     prefill = {}
     if plan.accumulate:  # per element about the size of the fresh gradient; where that is 0, a value of its scale
         for k in plan.grad_outputs:
@@ -262,10 +346,15 @@ def run_case(c, metrics=None):
     rcs = H.backward(plan, buf, DEV)
     if any(rcs):
         return fails + ["backward returned %s" % rcs]
+    if plan.attr:
+        rc = H.interpolate_backward(plan, buf, DEV)
+        if rc != 0:
+            return fails + ["nr_b200_interpolate_backward returned %d" % rc]
     fails += ["%s: a guard word next to the buffer changed in the backward" % k for k in buf if not H.guards_intact(buf[k])]
     for k in untouched:
         if not torch.equal(_bits(buf[k]), before[k]):
-            fails.append("%s written although the geometry is indexed" % k)
+            fails.append("%s written although %s" % (k, "the geometry is indexed" if k == "grad_faces"
+                                                     else "it lies past struct_size"))
     for k in plan.grad_outputs:
         if k in untouched:
             continue
@@ -282,11 +371,11 @@ def run_case(c, metrics=None):
                              % (k, int((x[zero] != p[zero]).sum()), int(zero.sum())))
             x = x - p.astype(np.float64)
         e1, e2 = rel_err(x, r), elem_err(x, r)
-        mip_tex = plan.mip and k == "grad_textures"
-        tol_elem = TOL_GRAD_ELEM_MIP if mip_tex else TOL_GRAD
+        tol_t, tol_e, tol_e_mip = GRAD_GATES.get(k, (TOL_GRAD, TOL_GRAD, TOL_GRAD))
+        tol_elem = tol_e_mip if plan.mip else tol_e
         note(k, "tensor", e1)
-        note(k, "elem_mip" if mip_tex else ("elem_acc" if plan.accumulate else "elem"), e2)
-        if not (e1 <= TOL_GRAD and e2 <= tol_elem):
+        note(k, ("elem_mip" if plan.mip and tol_e_mip != tol_e else ("elem_acc" if plan.accumulate else "elem")), e2)
+        if not (e1 <= tol_t and e2 <= tol_elem):
             fails.append("%s: rel_err %.3g elem_err %.3g (max |ref| %.3g)" % (k, e1, e2, float(np.abs(r).max())))
     return fails
 
