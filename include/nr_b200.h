@@ -106,7 +106,8 @@ extern "C" {
  *     grad_face_uvs[corner k] += (l_k gu, l_k gv)
  *   (a fill_back copy f >= F/2 adds into face f - F/2, its corner k being that face's corner 2 - k; with NR_UV_SHARED the
  *   sum over the items).  This is the derivative of the bilinear sample within the cell the forward picked: the level of
- *   detail, l_k and the clamp are held fixed, a 1-texel axis gets 0.  fp32, not bit-pinned (unordered atomics). */
+ *   detail, l_k and the clamp are held fixed, a 1-texel axis gets 0.  fp32, not bit-pinned (unordered atomics).
+ *   No vertex gradient flows through l_k unless NR_GRAD_INTERIOR (below). */
 #define NR_TEX_UV 0x20000u    /* sample a texture image through per-corner UVs (fields face_uvs / texture_height / _width) */
 #define NR_UV_SHARED 0x40000u /* face_uvs is [F,3,2] and serves every batch item (else [B,F,3,2])                        */
 
@@ -146,8 +147,36 @@ extern "C" {
  *   NR_FWD_STAGE_TEXTURES is ignored with corner_light.
  *   Backward (nr_b200_backward_corner_light), texture half: grad_textures as without light, with d rgb_c / d s_c = L_c in place of face_light; grad_face_uvs
  *   likewise uses L_c; grad_corner_light[b,f,k,c] += l_k * g_c * s_c (zero-filled first unless NR_GRAD_ACCUMULATE; needs
- *   corner_light and `textures`).  No vertex gradient flows through l_k: grad_faces / grad_vertices are those of the
- *   unchanged edge scan (which reads the smooth-shaded rgb map) and depth gradient.  fp32 atomics, not bit-pinned. */
+ *   corner_light and `textures`).  No vertex gradient flows through l_k unless NR_GRAD_INTERIOR (below): without it
+ *   grad_faces / grad_vertices are those of the unchanged edge scan (which reads the smooth-shaded rgb map) and depth
+ *   gradient.  fp32 atomics, not bit-pinned. */
+
+/* Interior vertex gradient of the RGB image, additive to ABI 4: one backward flag, honoured by nr_b200_backward and
+ * nr_b200_backward_corner_light (no struct field, no entry point, no workspace).  Without it the face / vertex gradient is
+ * the reference's (edge scan K5 + depth K7), bit for bit as before.  With it, the faces half (NR_BWD_PART_FACES) also adds
+ * the derivative of the colour INSIDE each face through the perspective weights: K5 covers the coverage changes, this term
+ * the colour changes at fixed coverage, so nothing is counted twice.
+ *   Covered raster pixel: winner fn, saved weights w_k, the winner's OWN camera depths z_k (also for cubes), zp recomputed
+ *   as the forward does, l_k = w_k (zp / z_k) (nr::perspective_weights), upstream g_c (the pooled gradient / 4 with
+ *   NR_ANTI_ALIASING).  L_c = face_light_c, 1 when unlit, or the corner_light interpolant (smooth shading).  s_c = the unlit
+ *   sample.  E_kc = d s_c / d l_k with the cell, the level of detail and the clamps held fixed:
+ *     cubes:     E_kc = [0 <= t_k <= ts-1-eps] (ts-1) dS_c/dt_k, t_k the unclamped texture coordinate of the sampler, and
+ *                dS_c/dt_k = sum over the 4 corner pairs along axis k of (T_hi - T_lo) times the other two axes' weights,
+ *                in the cell the forward picked (addressing as the forward, reversed axes for a NR_TEX_FILL_BACK copy);
+ *     bilinear:  E_kc = Du_c u_k + Dv_c v_k with Du, Dv the d sample / d (u, v) of NR_TEX_UV above (clamp gates in_u / in_v
+ *                and the (W-1) / (H-1) scales included), uv_k the (for a fill_back copy reversed) UV corners;
+ *     trilinear: sum_l a_l (Du_c^l u_k + Dv_c^l v_k) over the one or two levels the forward read (none through the LOD).
+ *   G_k = sum_c g_c (L_c E_kc + [smooth] C_kc s_c) = d loss / d l_k, and the chain of nr_b200_interpolate_backward:
+ *     D_k = G_k - G_0 (k = 1, 2; images and corner light from corner differences (uv_k - uv_0), (C_k - C_0)),
+ *     Gx = D_1 lx_1 + D_2 lx_2, Gy alike (lx_k, ly_k = d l_k / d (x, y) in raster pixels, as there),
+ *     P_m = sum_k l_k G_k - G_m (images: gu (u - u_m) + gv (v - v_m) with the pixel's uv; light: sum_c g_c s_c (L_c - C_mc)),
+ *     grad x_m += -w_m Gx S/2,   grad y_m += -w_m Gy S/2,   grad z_m += (l_m / z_m) P_m,
+ *   with the weights' clamp and renormalisation held fixed, as K7.  fp32 atomics, not bit-pinned.
+ *   Needs NR_RETURN_RGB and `textures` (the image / pyramid for NR_TEX_UV); per-face cubes with NR_TEX_Z_BATCH0 at B > 1
+ *   (whose sampler reads the depths of item 0, so the derivative would cross items) are refused: NR_ERR_INVALID_ARG
+ *   before any launch.  It runs only when grad_rgb is given; the texture half and its outputs are unchanged.
+ *   NR_GRAD_ACCUMULATE and the short struct layouts behave as without it. */
+#define NR_GRAD_INTERIOR 0x400000u
 
 typedef struct nr_b200_forward_args {
     uint32_t struct_size; /* sizeof(nr_b200_forward_args), or offsetof(.., corner_light) (see there) */

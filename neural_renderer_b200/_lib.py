@@ -33,6 +33,7 @@ NR_UV_SHARED = 0x40000
 NR_TEX_MIPMAP = 0x80000
 NR_ATTR_PER_VERTEX = 0x100000
 NR_ATTR_SHARED = 0x200000
+NR_GRAD_INTERIOR = 0x400000
 
 ABI_VERSION = 4
 

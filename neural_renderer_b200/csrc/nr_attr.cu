@@ -51,11 +51,6 @@ __device__ __forceinline__ long long attr_row(const AttrParams& p, int b, int f,
 
 __device__ __forceinline__ float ld_or0(const float* a, long long row, int c) { return row >= 0 ? __ldg(a + row + c) : 0.0f; }
 
-// zp = rcp.rn((w0/z0 + w1/z1) + w2/z2) -- the expression of nr::weights_and_depth, so it equals depth_map bit for bit
-__device__ __forceinline__ float pixel_depth(const float w[3], float z0, float z1, float z2) {
-    return __frcp_rn(__fadd_rn(__fadd_rn(__fdiv_rn(w[0], z0), __fdiv_rn(w[1], z1)), __fdiv_rn(w[2], z2)));
-}
-
 // out_c = fma(l2, a_2c, fma(l1, a_1c, l0 a_0c)): the chain of nr::corner_light_at
 __device__ __forceinline__ float interp(const float l[3], float a0, float a1, float a2) {
     return __fmaf_rn(l[2], a2, __fmaf_rn(l[1], a1, __fmul_rn(l[0], a0)));
@@ -88,7 +83,7 @@ __global__ void __launch_bounds__(256) k_interp(const __grid_constant__ AttrPara
             const float z0 = __ldg(nr::face_vertex_t<kIdx>(p.src, b, fn, 0) + 2);
             const float z1 = __ldg(nr::face_vertex_t<kIdx>(p.src, b, fn, 1) + 2);
             const float z2 = __ldg(nr::face_vertex_t<kIdx>(p.src, b, fn, 2) + 2);
-            nr::perspective_weights(w, pixel_depth(w, z0, z1, z2), z0, z1, z2, lam[q]);
+            nr::perspective_weights(w, nr::pixel_depth(w, z0, z1, z2), z0, z1, z2, lam[q]);
 #pragma unroll
             for (int k = 0; k < 3; k++) row[q][k] = attr_row<kPV>(p, b, fn, k);
         }
@@ -136,7 +131,7 @@ __global__ void __launch_bounds__(256) k_interp_grad(const __grid_constant__ Att
             float v[9];
             nr::load_face(p.src, b, fn, v);
             const float z[3] = {v[2], v[5], v[8]};
-            const float zp = pixel_depth(w, z[0], z[1], z[2]);
+            const float zp = nr::pixel_depth(w, z[0], z[1], z[2]);
             nr::perspective_weights(w, zp, z[0], z[1], z[2], lam);
             const float fS = (float)S;
             float inv[9];
@@ -172,7 +167,7 @@ __global__ void __launch_bounds__(256) k_interp_grad(const __grid_constant__ Att
             const float z0 = __ldg(nr::face_vertex_t<kIdx>(p.src, b, fn, 0) + 2);
             const float z1 = __ldg(nr::face_vertex_t<kIdx>(p.src, b, fn, 1) + 2);
             const float z2 = __ldg(nr::face_vertex_t<kIdx>(p.src, b, fn, 2) + 2);
-            nr::perspective_weights(w, pixel_depth(w, z0, z1, z2), z0, z1, z2, lam);
+            nr::perspective_weights(w, nr::pixel_depth(w, z0, z1, z2), z0, z1, z2, lam);
         }
     }
     // runs of neighbouring lanes that show the same face (a warp = 32 consecutive pixels of a row)

@@ -43,6 +43,7 @@
 
 #include "nr_b200.h"
 #include "nr_bbox.cuh"
+#include "nr_interior.h"
 #include "nr_internal.h"
 #include "nr_math.cuh"
 
@@ -1613,6 +1614,11 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
     const bool smooth = corner_light != nullptr;
     if (smooth && (!rgb || a->face_light)) return NR_ERR_INVALID_ARG;
     if (grad_corner_light && (!smooth || !a->textures)) return NR_ERR_INVALID_ARG;
+    // NR_GRAD_INTERIOR: the sampler's derivative reads the textures; the cubes of NR_TEX_Z_BATCH0 sample item b with the
+    // depths of item 0, so their derivative would cross items (B = 1 is the plain sampler)
+    const bool interior = (flags & NR_GRAD_INTERIOR) != 0;
+    if (interior && (!rgb || !a->textures)) return NR_ERR_INVALID_ARG;
+    if (interior && !uv && (flags & NR_TEX_Z_BATCH0) && B > 1) return NR_ERR_INVALID_ARG;
     if ((flags & NR_ANTI_ALIASING) && (S & 1)) return NR_ERR_INVALID_ARG;
     if (S > 32767 || B > 65535) return NR_ERR_UNSUPPORTED;
     if ((size_t)B * F * 2 * kWideStrips >= (size_t)0x7FFFFFFF) return NR_ERR_UNSUPPORTED;  // 32-bit list offsets
@@ -1794,6 +1800,15 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
     if (depth && p.g_depth) {
         nr_internal::LaunchScope ls("k_depth_grad", stream);
         k_depth_grad<<<pgrid, 256, 0, stream>>>(p);
+    }
+    if (interior && p.g_rgb) {  // the interior term of the rgb image (nr_interior.cu), into the same face / vertex gradient
+        nr_internal::InteriorLaunch il{};
+        il.args = a; il.src = src; il.dst = dst; il.corner_light = corner_light;
+        il.tex_bstride = (flags & NR_TEX_SHARED) ? 0 : (uv ? img_floats : ncubes * (size_t)ts * ts * ts * 3);
+        il.uv_bstride = p.uv_bstride;
+        il.tex_cmp = p.tex_cmp; il.tex_val = p.tex_val;
+        il.mip = mip ? &mt : nullptr;
+        nr_internal::launch_interior_grad(il, stream);
     }
     return cudaGetLastError() == cudaSuccess ? NR_OK : NR_ERR_CUDA;
 }

@@ -1,0 +1,28 @@
+// nr_interior.h -- host interface of the NR_GRAD_INTERIOR kernel (nr_interior.cu) for nr_b200_backward (not part of the ABI).
+#pragma once
+#include <cuda_runtime.h>
+#include <stddef.h>
+#include <stdint.h>
+
+#include "nr_b200.h"
+#include "nr_geom.cuh"
+#include "nr_math.cuh"
+
+namespace nr_internal {
+
+struct InteriorLaunch {
+    const nr_b200_backward_args* args;  // the checked call (flags, maps, grad_rgb, textures, face_uvs, face_light)
+    nr::FaceSrc src;
+    nr::FaceGrad dst;
+    const float* corner_light;  // smooth shading, or nullptr
+    size_t tex_bstride;         // floats per item in `textures` (0 = shared)
+    uint32_t uv_bstride;        // floats per item in face_uvs (0 = shared)
+    float tex_cmp, tex_val;     // the cube clamp thresholds of the forward
+    const nr::MipTable* mip;    // NR_TEX_MIPMAP: the pyramid's level table, else nullptr
+};
+
+// one launch of k_interior_grad, adding d loss / d vertices through l_k into src / dst's gradient (faces half); launch
+// errors surface through the caller's cudaGetLastError
+void launch_interior_grad(const InteriorLaunch& L, cudaStream_t stream);
+
+}  // namespace nr_internal

@@ -155,7 +155,7 @@ def set_texture_grad_hook(hook):
 
 
 class _Config:
-    __slots__ = ("S", "aa", "near", "far", "eps", "bg", "bg_batch", "flags", "reference_exact", "mip_hw")
+    __slots__ = ("S", "aa", "near", "far", "eps", "bg", "bg_batch", "flags", "reference_exact", "mip_hw", "interior")
 
 
 def _make_config(image_size, anti_aliasing, near, far, eps, background_color, return_rgb, return_alpha, return_depth,
@@ -167,6 +167,7 @@ def _make_config(image_size, anti_aliasing, near, far, eps, background_color, re
     cfg.S = int(image_size) * 2 if cfg.aa else int(image_size)
     cfg.near, cfg.far, cfg.eps = float(near), float(far), float(eps)
     cfg.mip_hw = None  # (Ht, Wt) of level 0 when `textures` is a packed mip pyramid (NR_TEX_MIPMAP)
+    cfg.interior = False  # NR_GRAD_INTERIOR on the backward call (interior_gradient=True)
     flags = 0
     if return_rgb:
         flags |= _lib.NR_RETURN_RGB
@@ -291,7 +292,9 @@ class _RasterizeFunction(torch.autograd.Function):
         need_light_grad = light_c is not None and ctx.needs_input_grad[2]
         ctx.need_corner_grad = corner_c is not None and ctx.needs_input_grad[6]
         ctx.need_uv_grad = uv_c is not None and want_rgb and ctx.needs_input_grad[5]
-        need_tex = need_light_grad or ctx.need_uv_grad or ctx.need_corner_grad
+        # interior_gradient: the backward differentiates the sampler, so it reads the textures (and face_uvs / corner_light)
+        ctx.interior = cfg.interior and want_rgb and ctx.needs_input_grad[0]
+        need_tex = need_light_grad or ctx.need_uv_grad or ctx.need_corner_grad or ctx.interior
         ctx.save_for_backward(geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c if need_tex else None, indices, uv_c, corner_c)
         if cfg.aa:
             rgb_o, alpha_o, depth_o = out_rgb, out_alpha, out_depth
@@ -304,7 +307,7 @@ class _RasterizeFunction(torch.autograd.Function):
     def backward(ctx, g_rgb, g_alpha, g_depth, _g_fim, _g_wmap):
         lib = _lib.load()
         cfg = ctx.cfg
-        flags = ctx.flags
+        flags = ctx.flags | (_lib.NR_GRAD_INTERIOR if ctx.interior else 0)
         geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c, indices, uv_c, corner_c = ctx.saved_tensors
         dev = geom_c.device
         B, F = geom_c.shape[0], ctx.F
@@ -401,11 +404,17 @@ TEXTURE_FILTERS = ('bilinear', 'trilinear')
 
 def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_color, return_rgb, return_alpha,
          return_depth, face_light=None, textures_fill_back=False, vertices=None, reference_exact=None, face_uvs=None,
-         texture_filter='bilinear', corner_light=None):
+         texture_filter='bilinear', corner_light=None, interior_gradient=False):
     if texture_filter not in TEXTURE_FILTERS:
         raise ValueError("texture_filter must be one of %s, got %r" % (TEXTURE_FILTERS, texture_filter))
     if texture_filter == 'trilinear' and face_uvs is None:
         raise ValueError("texture_filter='trilinear' samples a texture image: it needs face_uvs")
+    geom_in = vertices if vertices is not None else faces
+    if (return_rgb and interior_gradient and face_uvs is None and isinstance(geom_in, torch.Tensor) and geom_in.dim() >= 1
+            and geom_in.shape[0] > 1 and (_REFERENCE_EXACT if reference_exact is None else reference_exact)):
+        raise ValueError("interior_gradient=True with per-face cubes needs every item's own depths when the batch has more "
+                         "than one item: the reference-exact sampler reads the depths of item 0 for every item, so its "
+                         "derivative would cross items.  Pass reference_exact=False (or set_reference_exact(False))")
     _check_inputs(faces, textures, return_rgb, face_light, textures_fill_back, vertices, face_uvs, corner_light)
     indices = None
     if vertices is not None:
@@ -438,6 +447,7 @@ def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_
         cfg.flags |= _lib.NR_TEX_FILL_BACK
     if return_rgb and _STAGE_TEXTURES:
         cfg.flags |= _lib.NR_FWD_STAGE_TEXTURES
+    cfg.interior = bool(return_rgb and interior_gradient)
     if return_rgb and texture_filter == 'trilinear':
         # the pyramid is built from the image (shared or per item, as the image is) and autograd chains its gradient
         # back into the image
@@ -468,6 +478,7 @@ def rasterize_rgbad(
         face_uvs=None,
         texture_filter='bilinear',
         corner_light=None,
+        interior_gradient=False,
 ):
     """Generate RGB, alpha channel, and depth images from faces and textures (for RGB).  rasterize.py:900-977.
 
@@ -506,12 +517,18 @@ def rasterize_rgbad(
                               weights and multiplied onto the unlit sample (include/nr_b200.h).  Exclusive with
                               face_light; needs return_rgb.  F.vertex_normals / F.corner_light compute the Lambertian
                               factor, but any per-corner factor works.  It receives d loss / d corner_light; no vertex
-                              gradient flows through the interpolation weights.
+                              gradient flows through the interpolation weights unless interior_gradient=True.
+      interior_gradient       False (default): the vertices receive the reference's gradient (edges through the rgb / alpha
+                              images, depth).  True: also the derivative of the colour INSIDE each face through the
+                              perspective weights -- the texture sampled at a moving position and the smooth light
+                              (include/nr_b200.h, NR_GRAD_INTERIOR), with the cell, level of detail and clamps held fixed.
+                              What photometric alignment of a textured mesh needs.  Per-face cubes with a batch > 1 need
+                              reference_exact=False.
     `textures` with batch size 1 (or an expanded stride-0 batch) while the geometry batch is larger = one texture set
     shared by every item (a mesh seen from B viewpoints, mesh.py:29-34); its gradient is the sum over the items."""
     rgb, alpha, depth, _, _ = _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_color,
                                    return_rgb, return_alpha, return_depth, face_light, textures_fill_back, vertices,
-                                   reference_exact, face_uvs, texture_filter, corner_light)
+                                   reference_exact, face_uvs, texture_filter, corner_light, interior_gradient)
     return {
         'rgb': rgb if return_rgb else None,
         'alpha': alpha if return_alpha else None,
@@ -536,13 +553,15 @@ def rasterize(
         face_uvs=None,
         texture_filter='bilinear',
         corner_light=None,
+        interior_gradient=False,
 ):
     """RGB images [B,3,H,W] from faces and textures.  rasterize.py:980-1008 (keyword-only extras: rasterize_rgbad; in
     texture-image mode both the image and face_uvs receive gradients)."""
     return rasterize_rgbad(
         faces, textures, image_size, anti_aliasing, near, far, eps, background_color, True, False, False,
         face_light=face_light, textures_fill_back=textures_fill_back, vertices=vertices,
-        reference_exact=reference_exact, face_uvs=face_uvs, texture_filter=texture_filter, corner_light=corner_light)['rgb']
+        reference_exact=reference_exact, face_uvs=face_uvs, texture_filter=texture_filter, corner_light=corner_light,
+        interior_gradient=interior_gradient)['rgb']
 
 
 def rasterize_silhouettes(

@@ -49,6 +49,9 @@ class Renderer(object):
         # area-weighted normal and interpolated across the face (Gouraud), with vertex gradients through the normals.
         # Silhouettes and depth ignore it
         self.shading = 'flat'
+        # True: render() also sends the vertices the derivative of the colour inside each face (texture moving under the
+        # face, smooth light) -- photometric alignment; per-face cubes with a batch > 1 need reference_exact=False
+        self.interior_gradient = False
 
     def _transform(self, vertices):
         # renderer.py:41-50 (look_at / look, then perspective), fused into one kernel on CUDA
@@ -114,7 +117,7 @@ class Renderer(object):
                 indices, textures, self.image_size, self.anti_aliasing, self.near, self.far, self.rasterizer_eps,
                 self.background_color, face_light=light, textures_fill_back=self.fill_back,
                 vertices=self._transform(vertices), reference_exact=self.reference_exact, face_uvs=face_uvs,
-                texture_filter=texture_filter)
+                texture_filter=texture_filter, interior_gradient=self.interior_gradient)
         if face_uvs is not None:
             # op by op: materialised faces, the light factor of those faces (F.face_light), doubled UV corners for fill_back
             if self.fill_back:
@@ -125,7 +128,7 @@ class Renderer(object):
             return rasterize(
                 faces, textures, self.image_size, self.anti_aliasing, self.near, self.far, self.rasterizer_eps,
                 self.background_color, face_light=light, reference_exact=self.reference_exact, face_uvs=face_uvs,
-                texture_filter=texture_filter)
+                texture_filter=texture_filter, interior_gradient=self.interior_gradient)
         if self.fill_back:
             faces = torch.cat((faces, faces.flip(2)), dim=1)
             textures = torch.cat((textures, textures.permute(0, 1, 4, 3, 2, 5)), dim=1)
@@ -134,7 +137,7 @@ class Renderer(object):
         faces = F.vertices_to_faces(vertices, faces)
         return rasterize(
             faces, textures, self.image_size, self.anti_aliasing, self.near, self.far, self.rasterizer_eps,
-            self.background_color, reference_exact=self.reference_exact)
+            self.background_color, reference_exact=self.reference_exact, interior_gradient=self.interior_gradient)
 
     def render_attributes(self, vertices, faces, vertex_attributes=None, face_attributes=None):
         """Attribute images [B,C,H,W] (neural_renderer_b200.rasterize_attributes) seen through this renderer's camera:
@@ -173,7 +176,7 @@ class Renderer(object):
                 indices, textures, self.image_size, self.anti_aliasing, self.near, self.far, self.rasterizer_eps,
                 self.background_color, textures_fill_back=self.fill_back, vertices=self._transform(vertices),
                 reference_exact=self.reference_exact, face_uvs=face_uvs, texture_filter=texture_filter,
-                corner_light=corner)
+                corner_light=corner, interior_gradient=self.interior_gradient)
         # op by op: torch normals and light, materialised faces, doubled textures / UV corners for fill_back
         normals = F._vertex_normals_torch(vertices, faces)
         if self.fill_back:
@@ -187,4 +190,4 @@ class Renderer(object):
         return rasterize(
             faces, textures, self.image_size, self.anti_aliasing, self.near, self.far, self.rasterizer_eps,
             self.background_color, reference_exact=self.reference_exact, face_uvs=face_uvs,
-            texture_filter=texture_filter, corner_light=corner)
+            texture_filter=texture_filter, corner_light=corner, interior_gradient=self.interior_gradient)
