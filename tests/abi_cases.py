@@ -5,16 +5,18 @@ nr_b200_interpolate_backward (test infrastructure).
 `cases()` returns the case list of tests/test_gpu_abi_matrix.py: the full product of texture kind x fill_back x
 anti-aliasing x backward mode, with every other dimension filled in greedily so that every compatible pair of levels of
 any two dimensions appears in at least one case; rows are added until no pair is missing.  No randomness: the same list
-on every machine.  The cases of the matrix as it stood before smooth shading, the face_uvs gradient, texture staging,
-the short layouts and interpolation joined it (BASE) come first and are generated as they were, so their ids, inputs and
-oracle stay the same; the rows and pairs of the newer levels follow.
+on every machine.  The cases are generated in three frozen stages, each one exactly as it was when the next joined, so
+the ids, inputs and oracle of every earlier case stay the same: the matrix as it stood before smooth shading, the
+face_uvs gradient, texture staging, the short layouts and interpolation joined it (BASE); then the rows and pairs of
+those levels, with the interior vertex gradient off (FROZEN); then the interior rows and the pairs of every level.
 
 A level that has no meaning for a case (ts without texture cubes, image / UV sharing and the face_uvs gradient without a
-texture image, staging without RGB) is None and takes part in no pair.  Combinations the ABI rejects are never
-generated: texture kinds other than "none" always draw RGB and "none" never does, light (per face or per corner) needs
-RGB, the short struct layouts (ending before corner_light / grad_face_uvs) carry neither field, per-vertex attributes
-need indexed geometry; fill_back doubles the faces (F even) and anti-aliasing doubles the raster (even) by construction
-of the geometry, so no case is skipped.  The attribute channel count C is not a dimension: it rotates over
+texture image, staging and the interior gradient without RGB) is None and takes part in no pair.  Combinations the ABI
+rejects are never generated: texture kinds other than "none" always draw RGB and "none" never does, light (per face or
+per corner) needs RGB, the short struct layouts (ending before corner_light / grad_face_uvs) carry neither field,
+per-vertex attributes need indexed geometry, and the interior gradient refuses per-face cubes sampled with the depths of
+item 0 (NR_TEX_Z_BATCH0) at B > 1; fill_back doubles the faces (F even) and anti-aliasing doubles the raster (even) by
+construction of the geometry, so no case is skipped.  The attribute channel count C is not a dimension: it rotates over
 ATTR_CHANNELS with the case id (abi_harness.Plan)."""
 import itertools
 
@@ -39,6 +41,7 @@ DIMS = [
     ("stage", [False, True]),
     ("layout", ["full", "short"]),
     ("attr", ["off", "corner", "corner_shared", "vertex", "vertex_shared"]),
+    ("interior", ["off", "on"]),
 ]
 NAMES = [n for n, _ in DIMS]
 LEVELS = dict(DIMS)
@@ -50,13 +53,14 @@ def active(dim, kind):
         return kind in ("cube", "cube_shared")
     if dim in ("image", "uvs", "uv_grad"):
         return kind in ("uv", "mip")
-    if dim == "stage":
+    if dim in ("stage", "interior"):
         return kind != "none"
     return True
 
 
 def compatible(a):
-    """partial assignment {dim: level} -> False if it violates a rule (rules involve at most two dimensions)"""
+    """partial assignment {dim: level} -> False if it violates a rule (rules involve at most two dimensions, except the
+    interior gradient's refusal of z_batch0 cubes at three items, which involves four)"""
     kind = a.get("kind")
     out = a.get("outputs")
     if kind is not None and out is not None and (kind == "none") == ("r" in out):
@@ -67,6 +71,9 @@ def compatible(a):
         return False  # the short forward struct ends before corner_light, the short backward before grad_face_uvs
     if a.get("geometry") == "faces" and str(a.get("attr")).startswith("vertex"):
         return False  # per-vertex attributes need NR_FACES_INDEXED
+    if (a.get("interior") == "on" and kind in ("cube", "cube_shared") and a.get("z_batch0") is True
+            and a.get("batch") == "B3"):
+        return False  # the cubes would be sampled with item 0's depths: the derivative would cross items (refused)
     return True
 
 
@@ -125,7 +132,7 @@ def _key(d1, l1, d2, l2):
 # attribute interpolation joined it: its dimensions and levels, the others held at the level that leaves the call as it
 # was.  Its cases are generated first, exactly as before, so their ids and inputs stay what they were.
 BASE = {**{n: LEVELS[n] for n in NAMES[:NAMES.index("optional") + 1]}, "ts": [2, 3, 5], "light": ["none", "face"],
-        "uv_grad": ["null"], "stage": [False], "layout": ["full"], "attr": ["off"]}
+        "uv_grad": ["null"], "stage": [False], "layout": ["full"], "attr": ["off"], "interior": ["off"]}
 BASE_PAIRS = {n: BASE[n] for n in NAMES[:NAMES.index("optional") + 1]}
 
 # rows the pairs alone would not force: the edge scan zero-fills grad_textures on the side (one call, both halves, rgb
@@ -165,6 +172,38 @@ MUST_NEW += [{"kind": "cube", "stage": True, "_aa": False, "pointers": "fresh", 
          {"kind": "cube_shared", "stage": True, "_aa": False, "pointers": "fresh", "ts": 4, "light": "none"},
          {"kind": "cube", "stage": True, "_aa": False, "pointers": "fresh", "ts": 6, "light": "none", "fill_back": False,
           "batch": "B3", "raster": "even"}]
+# the matrix as it stood before the interior vertex gradient joined it: every level but that flag, held off
+FROZEN = {**LEVELS, "interior": ["off"]}
+FROZEN_PAIRS = {n: LEVELS[n] for n in NAMES if n != "interior"}
+
+# the interior vertex gradient (NR_GRAD_INTERIOR) with an rgb upstream gradient, for every texture kind: every light, a
+# fresh and an accumulating backward, one call and two halves, with and without fill_back and anti-aliasing, spread over
+# the four geometries and the three batch levels.  Per-item index sets and per-item light at three items (the scatter and
+# the light reads address item b), ts 3 / 5 / 6, z_batch0 cubes at B = 1 and z_batch0 images at B = 3 (no effect there),
+# K5 with rgb + alpha and K7 adding into the same buffer (outputs "rad"), NULL optional pointers.  The image size follows
+# the case id (abi_harness.Plan): the rows sit so that the last uv row (id 188) and the third mip row (id 191) get the
+# one-texel-high (1, 9) image.
+_I = [  # kind, light, fill_back, aa, backward, geometry, batch, extra levels
+    ("cube", "none", False, False, "one", "idx_item", "B3", {"ts": 3, "outputs": "rad", "upstream": "all"}),
+    ("cube", "face", True, True, "acc_halves", "faces", "B3", {"ts": 5, "optional": "given"}),
+    ("cube", "corner", True, False, "faces_tex", "idx_shared_oor", "B3", {"ts": 6, "optional": "given"}),
+    ("cube", "face", False, True, "acc_one", "idx_shared", "B1", {"ts": 4, "z_batch0": True}),
+    ("cube_shared", "corner", False, False, "one", "idx_item", "B3", {"ts": 5, "optional": "null"}),
+    ("cube_shared", "none", True, True, "acc_halves", "idx_shared", "B1_shared_flags", {"ts": 3, "z_batch0": True}),
+    ("cube_shared", "face", True, False, "tex_faces", "idx_item", "B3", {"ts": 6, "outputs": "rad", "upstream": "all"}),
+    ("cube_shared", "corner", False, True, "acc_one", "faces", "B3", {"ts": 2}),
+    ("uv", "face", False, False, "one", "idx_item", "B3", {"uv_grad": "given", "outputs": "rad", "upstream": "all"}),
+    ("uv", "corner", True, True, "acc_halves", "idx_shared_oor", "B3", {"z_batch0": True}),
+    ("uv", "none", True, False, "faces_tex", "faces", "B1", {"optional": "null"}),
+    ("uv", "corner", False, True, "acc_one", "idx_item", "B3", {"image": "item", "uvs": "shared"}),
+    ("mip", "corner", False, False, "one", "idx_item", "B3", {"outputs": "rad", "upstream": "all"}),
+    ("mip", "face", True, True, "acc_halves", "faces", "B3", {"uv_grad": "given", "z_batch0": True}),
+    ("mip", "none", True, False, "tex_faces", "idx_shared", "B1", {"image": "shared", "uvs": "item"}),
+    ("mip", "face", False, True, "acc_one", "idx_item", "B3", {"optional": "null"}),
+]
+MUST_INTERIOR = [{"kind": kind, "light": light, "fill_back": fb, "_aa": aa, "backward": bwd, "geometry": geom, "batch": batch,
+                  "interior": "on", "upstream": ("all", "only_rgb")[i % 2], **extra}
+                 for i, (kind, light, fb, aa, bwd, geom, batch, extra) in enumerate(_I)]
 
 
 def _complete(out, covered, choices, pairs):
@@ -197,8 +236,14 @@ def cases():
         covered |= pairs_of(c)
         out.append(c)
     _complete(out, covered, BASE, required_pairs(BASE_PAIRS))
-    # then the rows and pairs of every level
+    # then the rows and pairs of every level but the interior gradient
     for seed in MUST_NEW:
+        c = _fill(dict(seed), covered, len(out), FROZEN)
+        covered |= pairs_of(c)
+        out.append(c)
+    _complete(out, covered, FROZEN, required_pairs(FROZEN_PAIRS))
+    # then the interior rows and the pairs of every level
+    for seed in MUST_INTERIOR:
         c = _fill(dict(seed), covered, len(out))
         covered |= pairs_of(c)
         out.append(c)
@@ -215,5 +260,5 @@ def case_id(c):
              "stage" if c["stage"] else "", "bgB" if c["bg"] == "per_batch" else "", c["outputs"],
              "z0" if c["z_batch0"] else "", c["batch"], "up-" + c["upstream"], c["pointers"],
              "nulls" if c["optional"] == "null" else "", "short" if c["layout"] == "short" else "",
-             "" if c["attr"] == "off" else "attr-" + c["attr"]]
+             "" if c["attr"] == "off" else "attr-" + c["attr"], "interior" if c["interior"] == "on" else ""]
     return "%03d-" % c["id"] + "-".join(p for p in parts if p)

@@ -75,6 +75,7 @@ class Plan:
         self.attr_pv = c["attr"].startswith("vertex")
         self.attr_shared = c["attr"].endswith("_shared")
         self.C = ATTR_CHANNELS[c["id"] % len(ATTR_CHANNELS)] if self.attr else 0
+        self.interior = c["interior"] == "on"  # NR_GRAD_INTERIOR: a backward-only bit (backward_calls)
         f = 0
         f |= L.NR_RETURN_RGB if self.rgb else 0
         f |= L.NR_RETURN_ALPHA if self.alpha else 0
@@ -177,8 +178,9 @@ class Plan:
                 bufs["attr_grad_vertices" if self.indexed else "attr_grad_faces"] = (((B, Nv, 3) if self.indexed
                                                                                       else (B, F, 3, 3)), f32)
         self.bufs = bufs
-        # textures may be NULL in the backward unless a gradient that reads them is wanted
-        self.bwd_textures = self.rgb and (self.given or self.uv_grad or "grad_face_light" in bufs)
+        # textures may be NULL in the backward unless a gradient that reads them is wanted (the interior gradient reads
+        # the sampler's derivative from them)
+        self.bwd_textures = self.rgb and (self.given or self.uv_grad or "grad_face_light" in bufs or self.interior)
         p = c["pointers"]
         self.offsets = {k: (0 if p == "fresh" else 4) for k in bufs}
         if p == "off8":
@@ -257,7 +259,7 @@ class Plan:
     def backward_calls(self):
         """[(flag word, accumulate?)] of the case's backward mode, in call order"""
         L = _lib()
-        base = self.flags
+        base = self.flags | (L.NR_GRAD_INTERIOR if self.interior else 0)
         acc = L.NR_GRAD_ACCUMULATE
         tex, faces = L.NR_BWD_PART_TEXTURES, L.NR_BWD_PART_FACES
         return {"one": [base], "tex_faces": [base | tex, base | faces], "faces_tex": [base | faces, base | tex],

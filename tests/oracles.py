@@ -126,6 +126,44 @@ def lod64(faces, fim, wmap, dmap, uvk, S, Ht, Wt, L):
     return torch.nan_to_num(lod, nan=0.0, neginf=0.0).clamp(0, L - 1)
 
 
+def lod32(faces, fim, wmap, dmap, uvk, S, Ht, Wt, L):
+    """the level of detail as include/nr_b200.h pins it in fp32 (the arguments of lod64; returns float64 holding fp32
+    values): the K1 inverse of the pixel-space vertices, d l_k / dx from corner differences, each operation rounded to
+    fp32 in the header's order.  Every operation is evaluated in float64 and rounded once more, so a result can differ
+    from the product's by an ulp where that double rounding or log2 (log2f is not correctly rounded) lands differently.
+    It shows how far the fp32 LOD lies from lod64 -- up to 7e-5 in the C-ABI matrix, from the cancellation in
+    qx_k - l_k sx -- and so what of a trilinear comparison comes from the LOD alone."""
+    r = lambda t: t.float().double()  # round to fp32
+    fma = lambda a, b, c: r(a * b + c)  # a * b of two fp32 values is exact in float64
+    B = faces.shape[0]
+    fi = fim.clamp(min=0).long()
+    bidx = torch.arange(B, device=fim.device)[:, None, None].expand_as(fi)
+    f = r(faces.detach().double())[bidx, fi]  # [B,S,S,3 corners,3]
+    fS = float(S)
+    px = [r(r(fma(f[..., k, 0], fS, fS) - 1.0) * 0.5) for k in range(3)]  # to_pixel
+    py = [r(r(fma(f[..., k, 1], fS, fS) - 1.0) * 0.5) for k in range(3)]
+    n = [r(py[1] - py[2]), r(px[2] - px[1]), r(py[2] - py[0]), r(px[0] - px[2]), r(py[0] - py[1]), r(px[1] - px[0])]
+    det = fma(px[1], n[2], fma(px[2], n[4], r(px[0] * n[0])))  # face_inverse
+    inv = [r(n[2 * k + d] / det) for k in range(3) for d in (0, 1)]  # inv[3k], inv[3k+1]
+    z = [f[..., k, 2] for k in range(3)]
+    w = r(wmap.double()).permute(0, 2, 3, 1)
+    zp = r(dmap.double())
+    lam = [r(w[..., k] * r(zp / z[k])) for k in range(3)]
+    out = []
+    for d in (0, 1):
+        q = [r(inv[2 * k + d] / z[k]) for k in range(3)]
+        s = r(r(q[0] + q[1]) + q[2])
+        dl = [r(zp * r(q[k] - r(lam[k] * s))) for k in (1, 2)]
+        u = [uvk[..., k, 0].double() for k in range(3)]
+        v = [uvk[..., k, 1].double() for k in range(3)]
+        du = fma(r(u[2] - u[0]), dl[1], r(r(u[1] - u[0]) * dl[0]))
+        dv = fma(r(v[2] - v[0]), dl[1], r(r(v[1] - v[0]) * dl[0]))
+        a, b = r(float(Wt - 1) * du), r(float(Ht - 1) * dv)
+        out.append(r(r(a * a) + r(b * b)))
+    lod = r(0.5 * r(torch.log2(torch.fmax(*out))))  # fmaxf: a NaN loses to a number
+    return torch.nan_to_num(lod, nan=0.0, neginf=0.0).clamp(0, L - 1)
+
+
 def oracle_trilinear(faces, fim, wmap, dmap, uvs, image, light, bg, fill_back, aa):
     """float64 trilinear sample on the product's maps; image [1|B,Ht,Wt,3] (differentiable through the float64 pyramid),
     light [B,F,3] or None.  Returns (API rgb [B,3,H,W], raster LOD [B,S,S], L)."""
@@ -133,8 +171,9 @@ def oracle_trilinear(faces, fim, wmap, dmap, uvs, image, light, bg, fill_back, a
     return oracle_trilinear_levels(faces, fim, wmap, dmap, uvs, pyramid64(image.double()), Ht, Wt, light, bg, fill_back, aa)
 
 
-def oracle_trilinear_levels(faces, fim, wmap, dmap, uvs, levels, Ht, Wt, light, bg, fill_back, aa):
-    """oracle_trilinear on given pyramid levels [1|B,H_l,W_l,3] (e.g. unpack_pyramid of the packed `textures`)"""
+def oracle_trilinear_levels(faces, fim, wmap, dmap, uvs, levels, Ht, Wt, light, bg, fill_back, aa, lod_fn=None):
+    """oracle_trilinear on given pyramid levels [1|B,H_l,W_l,3] (e.g. unpack_pyramid of the packed `textures`); the level
+    of detail from `lod_fn` (default lod64)"""
     dev = fim.device
     B = faces.shape[0]
     S = fim.shape[-1]
@@ -156,7 +195,7 @@ def oracle_trilinear_levels(faces, fim, wmap, dmap, uvs, levels, Ht, Wt, light, 
     u32 = uvk.float()
     uv = (lam32[..., 0, None] * u32[..., 0, :] + lam32[..., 1, None] * u32[..., 1, :]) + lam32[..., 2, None] * u32[..., 2, :]
     uv = torch.nan_to_num(uv.clamp(0, 1))
-    lod = lod64(faces, fim, wmap, dmap, uvk, S, Ht, Wt, L)
+    lod = (lod_fn or lod64)(faces, fim, wmap, dmap, uvk, S, Ht, Wt, L)
     lt = light.double()[bidx, fi] if light is not None else None
 
     def bilinear(img):

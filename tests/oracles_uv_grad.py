@@ -78,15 +78,15 @@ def oracle_trilinear_uv_grad(faces, fim, wmap, dmap, uvs, image, light, bg, fill
                                            fill_back, aa)
 
 
-def oracle_trilinear_levels_uv_grad(faces, fim, wmap, dmap, uvs, levels, Ht, Wt, light, bg, fill_back, aa):
+def oracle_trilinear_levels_uv_grad(faces, fim, wmap, dmap, uvs, levels, Ht, Wt, light, bg, fill_back, aa, lod_fn=None):
     """oracle_trilinear_uv_grad on given pyramid levels [1|B,H_l,W_l,3] (e.g. oracles.unpack_pyramid of the packed
-    `textures`)"""
+    `textures`); the level of detail from `lod_fn` (default oracles.lod64)"""
     B = faces.shape[0]
     S = fim.shape[-1]
     levels = [l.double().expand(B, -1, -1, -1) for l in levels]
     L = len(levels)
     bidx, fi, uvk, uv_raw, st = _pixel_uvs(faces, fim, wmap, dmap, uvs, fill_back, z64=True)
-    lod = lod64(faces, fim, wmap, dmap, uvk.detach(), S, Ht, Wt, L)
+    lod = (lod_fn or lod64)(faces, fim, wmap, dmap, uvk.detach(), S, Ht, Wt, L)
     lt = light.double()[bidx, fi] if light is not None else None
     uv = torch.nan_to_num(uv_raw.clamp(0, 1))
     samples = torch.stack([_bilinear(l, uv, st, bidx, lt) for l in levels], dim=0)  # [L,B,S,S,3]

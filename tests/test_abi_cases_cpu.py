@@ -1,10 +1,12 @@
 """CPU: the covering array of the C-ABI matrix (tests/abi_cases.py) -- every compatible pair of levels appears, the full
 product of texture kind x fill_back x anti-aliasing x backward mode is there, the conjunctions the pairs do not force are
 reached (the side fill's tail, the light and corner-light gradients, the own-depth reload of the corner-light cube
-gradient, every phase of the face_uvs reduction, texture staging and its overflow), and every case passes the library's
-host argument checks (forward and backward called with a NULL workspace, so the call stops at the workspace check before
-touching a device; the interpolation, which has no workspace, only with arguments it rejects before any launch)."""
+gradient, every phase of the face_uvs reduction, texture staging and its overflow, the interior vertex gradient), the
+cases from before the interior gradient joined are unchanged, and every case passes the library's host argument checks
+(forward and backward called with a NULL workspace, so the call stops at the workspace check before touching a device;
+the interpolation, which has no workspace, only with arguments it rejects before any launch)."""
 import ctypes
+import hashlib
 import itertools
 
 import numpy as np
@@ -26,6 +28,15 @@ def test_generator_is_deterministic():
     assert abi_cases.cases() == abi_cases.cases()
 
 
+def test_cases_before_the_interior_gradient_are_frozen():
+    """the 177 cases the matrix held before the interior gradient joined it keep their ids, levels and seeded inputs:
+    without the `interior` key (always "off" there) they hash to the list as it was"""
+    old = [{k: v for k, v in c.items() if k != "interior"} for c in abi_cases.cases()[:177]]
+    assert all(c["interior"] in (None, "off") for c in abi_cases.cases()[:177])
+    assert hashlib.sha256(repr(old).encode()).hexdigest() == \
+        "cde6f0825f0973a0dfd6be5efe813401024db41c1de100869a3a5c23bd7ed758"
+
+
 def test_every_pair_of_levels_appears():
     cases = abi_cases.cases()
     covered = set().union(*(abi_cases.pairs_of(c) for c in cases))
@@ -34,7 +45,7 @@ def test_every_pair_of_levels_appears():
     # every level of every dimension is reachable, and the rules exclude nothing else
     for name, levels in abi_cases.DIMS:
         assert {c[name] for c in cases if c[name] is not None} == set(levels), name
-    assert len(cases) <= 180
+    assert len(cases) <= 200
 
 
 def test_full_product_of_the_fused_paths():
@@ -85,6 +96,54 @@ def test_corner_light_gradient_is_held_to_the_oracle():
     want = {(k, v) for k in ("acc", "halves", "fill_back", "aa") for v in (False, True)}
     for kind in ("cube", "cube_shared", "uv", "mip"):
         assert seen.get(kind, set()) >= want, (kind, want - seen.get(kind, set()))
+
+
+def test_interior_gradient_is_held_to_the_oracle():
+    """NR_GRAD_INTERIOR with an rgb upstream gradient, for every texture kind: every light, fresh and accumulating,
+    one-call and two-half backward passes, with and without fill_back and anti-aliasing; and over all interior cases
+    every geometry (per-item and shared index sets, out-of-range indices), every batch level, the odd cube sizes and a
+    one-texel-high image for both samplers"""
+    import abi_harness
+    seen, every = {}, set()
+    for c in abi_cases.cases():
+        p = abi_harness.Plan(c)
+        if not p.interior:
+            continue
+        every |= {("geometry", c["geometry"]), ("batch", c["batch"]), ("ts", p.ts), ("one_texel", p.kind, p.Ht == 1)}
+        if p.g_rgb:
+            s = seen.setdefault(p.kind, set())
+            s |= {("light", c["light"]), ("acc", p.accumulate), ("halves", len(p.backward_calls()) == 2),
+                  ("fill_back", p.fill_back), ("aa", p.aa)}
+    want = {(k, v) for k in ("acc", "halves", "fill_back", "aa") for v in (False, True)}
+    want |= {("light", v) for v in abi_cases.LEVELS["light"]}
+    for kind in ("cube", "cube_shared", "uv", "mip"):
+        assert seen.get(kind, set()) >= want, (kind, want - seen.get(kind, set()))
+    want_every = {("geometry", v) for v in abi_cases.LEVELS["geometry"]} | {("batch", v) for v in abi_cases.LEVELS["batch"]}
+    want_every |= {("ts", 3), ("ts", 5), ("ts", 6), ("one_texel", "uv", True), ("one_texel", "mip", True)}
+    assert every >= want_every, want_every - every
+
+
+def test_interior_gradient_next_to_other_outputs_is_reached():
+    """interior cases at three items with per-item index sets and with per-item face and corner light (the scatter and
+    the light reads address item b), z_batch0 cubes at B = 1 and z_batch0 images at B = 3, the rgb + alpha edge scan
+    and the depth gradient in the same call, and the flag without an rgb upstream gradient"""
+    import abi_harness
+    seen = set()
+    for c in abi_cases.cases():
+        p = abi_harness.Plan(c)
+        if not p.interior:
+            continue
+        cube = p.kind in ("cube", "cube_shared")
+        if p.g_rgb and p.B == 3:
+            seen |= {k for k, on in (("idx_item_B3", c["geometry"] == "idx_item"), ("lit_B3", p.lit),
+                                     ("corner_B3", p.corner)) if on}
+        if c["z_batch0"] and p.g_rgb and p.B == (1 if cube else 3):
+            seen.add("z0_cube_B1" if cube else "z0_image_B3")
+        if p.g_rgb and p.g_alpha and p.g_depth:
+            seen.add("rgb_alpha_depth")
+        if not p.g_rgb:
+            seen.add("no_rgb")
+    assert seen >= {"idx_item_B3", "lit_B3", "corner_B3", "z0_cube_B1", "z0_image_B3", "rgb_alpha_depth", "no_rgb"}, seen
 
 
 def test_corner_light_own_depth_reload_is_reached():
@@ -155,7 +214,8 @@ def test_cases_hold_the_rules():
 
 def test_every_case_passes_the_host_argument_checks(lib):
     import abi_harness
-    n_offset = n_short = n_corner = n_attr = 0
+    from neural_renderer_b200 import _lib as lib_flags
+    n_offset = n_short = n_corner = n_attr = n_interior = 0
     for c in abi_cases.cases():
         plan = abi_harness.Plan(c)
         ptr = plan.fake_pointers()
@@ -167,6 +227,22 @@ def test_every_case_passes_the_host_argument_checks(lib):
             b = plan.backward_args(ptr, flags, None, 0)
             assert plan.call_backward(lib, b, ptr, None) == NR_ERR_WORKSPACE, (abi_cases.case_id(c), hex(flags))
             n_corner += plan.corner
+            if plan.interior:
+                # the interior gradient reads the textures: NULL textures are refused for the flag alone -- without the
+                # other gradients that read them, the same call without the flag passes the host checks
+                n_interior += 1
+                I = lib_flags.NR_GRAD_INTERIOR
+                bare = {k: v for k, v in ptr.items() if k not in ("grad_face_light", "grad_face_uvs", "grad_corner_light")}
+                for fl, want in ((flags & ~I, NR_ERR_WORKSPACE), (flags, NR_ERR_INVALID_ARG)):
+                    b = plan.backward_args(bare, fl, None, 0)
+                    b.textures = None
+                    assert plan.call_backward(lib, b, bare, None) == want, (abi_cases.case_id(c), hex(fl))
+                # z_batch0 at three items: refused for cubes with the flag only; images ignore z_batch0
+                cube = plan.kind in ("cube", "cube_shared")
+                for fl, want in ((flags & ~I, NR_ERR_WORKSPACE), (flags, NR_ERR_INVALID_ARG if cube else NR_ERR_WORKSPACE)):
+                    b = plan.backward_args(ptr, fl | lib_flags.NR_TEX_Z_BATCH0, None, 0)
+                    b.batch_size = 3
+                    assert plan.call_backward(lib, b, ptr, None) == want, (abi_cases.case_id(c), hex(fl))
         # a required pointer left out is rejected before the workspace is looked at
         for k in ("face_index_map", "rgb_map" if plan.rgb else "weight_map"):
             bad = dict(ptr)
@@ -185,4 +261,5 @@ def test_every_case_passes_the_host_argument_checks(lib):
                 a = plan.interpolate_args(ptr, True)
                 a.grad_faces = 0x7000000
                 assert lib.nr_b200_interpolate_backward(ctypes.byref(a), None) == NR_ERR_INVALID_ARG, abi_cases.case_id(c)
-    assert n_offset >= 60 and n_short >= 15 and n_corner >= 20 and n_attr >= 40, (n_offset, n_short, n_corner, n_attr)
+    assert n_offset >= 60 and n_short >= 15 and n_corner >= 20 and n_attr >= 40 and n_interior >= 17, \
+        (n_offset, n_short, n_corner, n_attr, n_interior)

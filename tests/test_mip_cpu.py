@@ -126,3 +126,31 @@ def test_texture_filter_argument_checks():
             nr.rasterize(faces, img, 16, face_uvs=uvs, texture_filter=f)
     import neural_renderer
     assert neural_renderer.Renderer().texture_filter == "bilinear"
+
+
+def test_fp32_level_of_detail_restatement():
+    """oracles.lod32 (the header's fp32 LOD, used where the float64 LOD alone moves a trilinear comparison) returns fp32
+    values, agrees with oracles.lod64 to fp32 accuracy on well-conditioned faces and clamps as the header states"""
+    from oracles import lod32, lod64
+    g = torch.Generator().manual_seed(5)
+    B, F, S, Ht, Wt = 2, 6, 12, 37, 29
+    L = len(mip_levels(Ht, Wt))
+    xy = (torch.rand((B, F, 3, 2), generator=g) * 1.6 - 0.8).double()
+    z = (torch.rand((B, F, 3, 1), generator=g) * 2 + 1).double()
+    faces = torch.cat((xy, z), dim=-1).float().double()
+    fim = torch.randint(0, F, (B, S, S), generator=g).to(torch.int32)
+    w = torch.rand((B, 3, S, S), generator=g) + 0.05
+    wmap = w / w.sum(1, keepdim=True)
+    fi, bidx = fim.long(), torch.arange(B)[:, None, None]
+    zc = faces[..., 2][bidx, fi].float()  # [B,S,S,3]
+    q = wmap.permute(0, 2, 3, 1) / zc
+    dmap = 1.0 / ((q[..., 0] + q[..., 1]) + q[..., 2])
+    spread = 10.0 ** torch.linspace(-3, 2, B * F).reshape(B, F, 1, 1).double()
+    uvs = (0.5 + spread * (torch.rand((B, F, 3, 2), generator=g).double() - 0.5)).float().double()
+    uvk = uvs[bidx, fi]
+    a = lod64(faces, fim, wmap, dmap, uvk, S, Ht, Wt, L)
+    b = lod32(faces, fim, wmap, dmap, uvk, S, Ht, Wt, L)
+    assert torch.equal(b, b.float().double())
+    assert ((b == 0) | (b == L - 1)).any() and ((b > 0) & (b < L - 1)).any()
+    inner = (a > 0.01) & (a < L - 1.01)
+    assert float((a - b).abs()[inner].max()) <= 1e-4 * L
