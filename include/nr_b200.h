@@ -268,6 +268,47 @@ typedef struct nr_b200_backward_args {
     float *grad_face_uvs;
 } nr_b200_backward_args;
 
+/* Phong shading, additive to ABI 4: one struct (nr_b200_phong_args), two entry points (nr_b200_forward_phong /
+ * nr_b200_backward_phong) and a glue pair (nr_b200_corner_shading / _backward).  Ambient + diffuse + specular evaluated at
+ * every pixel from a normal and a position interpolated per pixel; the forward and backward structs are unchanged.
+ *   corner_shading [Bc,F,3,6]: per face corner k (the face's own order; F counts fill_back copies, which the caller gives
+ *   their corners with the normal negated) the shading normal N_k (3 floats), then the shading position P_k (3 floats).
+ *   params [Bp,16] (device): A[3] ambient intensity * colour, D[3] directional intensity * colour, d[3] light direction
+ *   (towards the light, not normalised, as for face_light), K[3] specular intensity * colour, sigma the shininess, e[3] the
+ *   eye position in the frame of P and N.  Bc, Bp in {1, B}; 1 = one set for every item (its gradient is the sum over the
+ *   items).
+ *   Covered raster pixel with winner weights w_k, depth zp and the winner's OWN vertex depths z_k (NR_TEX_Z_BATCH0 has no
+ *   effect on this), fp32, every fused multiply-add explicit:
+ *     l_k = w_k (zp / z_k)   (the l_k of NR_TEX_UV),   n = sum_k l_k N_k,   p = sum_k l_k P_k   (the fma chain of corner_light)
+ *     nh = n / (|n| + 1e-5),   dh = d / (|d| + 1e-5),   vh = (e - p) / (|e - p| + 1e-5)
+ *     c = nh . d,   L_c = A_c + D_c max(c, 0)   (the diffuse term uses d as given, like face_light)
+ *     r = 2 (nh . dh) nh - dh,   q = max(r . vh, 0),   h = [c > 0] [q > 0] q^sigma   (q^sigma = exp2(sigma log2 q))
+ *     rgb_c = L_c s_c + K_c h
+ *   with s the UNLIT sample exactly as the unlit path computes it (ts^3 cube, bilinear image or trilinear pyramid).  The
+ *   background is not lit; anti-aliasing pools on top; silhouettes and depth ignore shading; NR_FWD_STAGE_TEXTURES is
+ *   ignored.  Held to a float64 evaluation of the same expression, not bit-pinned.
+ *   Backward (nr_b200_backward_phong), texture half (NR_BWD_PART_TEXTURES): grad_textures and grad_face_uvs as on the smooth
+ *   path with the pixel's L_c in place of the corner interpolant (d rgb_c / d s_c = L_c);
+ *   grad_corner_shading[f,k] += l_k (d loss / d n, d loss / d p); grad_params receives the exact derivative of the
+ *   expression above (through nh with its 1e-5, dh, vh, q^sigma with ln q for sigma, A, D and K).  The masks [c > 0],
+ *   [q > 0] and both max take subgradient 0 at their kinks.  Each gradient output may be NULL (not wanted) and is
+ *   zero-filled first unless NR_GRAD_ACCUMULATE; without grad_rgb it stays zero.  fp32 atomics, not bit-pinned.
+ *   Faces half unchanged: the edge scan reads the Phong rgb map, the depth gradient is unchanged, and no vertex gradient
+ *   flows through l_k: NR_GRAD_INTERIOR with Phong is NR_ERR_UNSUPPORTED before any launch.
+ *   Host rejections (NR_ERR_INVALID_ARG, before any launch): a NULL phong struct or a struct_size mismatch, a NULL
+ *   corner_shading or params, Bc or Bp not in {1, B}, face_light or corner_light set, no NR_RETURN_RGB, and a backward
+ *   that asks for grad_corner_shading or grad_params without `textures` (both need s). */
+typedef struct nr_b200_phong_args {
+    uint32_t struct_size;          /* sizeof(nr_b200_phong_args) */
+    int32_t shading_batch;         /* Bc: 1 or B */
+    int32_t params_batch;          /* Bp: 1 or B */
+    int32_t _pad0;
+    const float *corner_shading;   /* [Bc,F,3,6] */
+    const float *params;           /* [Bp,16] */
+    float *grad_corner_shading;    /* backward: [Bc,F,3,6] or NULL */
+    float *grad_params;            /* backward: [Bp,16] or NULL */
+} nr_b200_phong_args;
+
 /* Attribute interpolation, additive to ABI 4: two flag bits, one struct and two entry points.  Renders C >= 1 arbitrary
  * channels (normals, positions, UVs, labels, features) through the maps an ordinary forward call wrote (face_index_map,
  * weight_map; a silhouette-only forward suffices), with gradients into the attributes and, through the perspective
@@ -346,6 +387,12 @@ NR_B200_API int nr_b200_backward(const nr_b200_backward_args *args, void *cuda_s
  * not wanted (part of the texture half, NR_BWD_PART_TEXTURES).  nr_b200_backward is this call with corner_light NULL. */
 NR_B200_API int nr_b200_backward_corner_light(const nr_b200_backward_args *args, const float *corner_light,
                                               float *grad_corner_light, void *cuda_stream);
+/* Phong shading (nr_b200_phong_args above).  The forward takes `args` with face_light and corner_light NULL and the
+ * workspace of nr_b200_forward_workspace_bytes; the backward is that of such a forward, `args` as for nr_b200_backward (with
+ * face_light NULL), the same `phong` corner_shading / params, and its grad_corner_shading / grad_params filled by the
+ * texture half. */
+NR_B200_API int nr_b200_forward_phong(const nr_b200_forward_args *args, const nr_b200_phong_args *phong, void *cuda_stream);
+NR_B200_API int nr_b200_backward_phong(const nr_b200_backward_args *args, const nr_b200_phong_args *phong, void *cuda_stream);
 /* Attribute interpolation (nr_b200_interpolate_args above): the image `out`, and its backward into grad_attributes and the
  * interior vertex gradient.  One kernel launch each (plus the zero-fill of the backward). */
 NR_B200_API int nr_b200_interpolate(const nr_b200_interpolate_args *args, void *cuda_stream);
@@ -427,6 +474,18 @@ NR_B200_API int nr_b200_corner_lighting_backward(const float *vertex_normals, co
                                                  const float *grad_corner_light, int32_t batch_size, int32_t num_vertices,
                                                  int32_t num_faces, uint32_t flags, float *grad_vertex_normals,
                                                  void *cuda_stream);
+/* Phong shading glue (feeds nr_b200_phong_args.corner_shading) from vertex normals [B,Nv,3], vertices [B,Nv,3] (the
+ * positions P, in the frame of the eye) and the index set `faces` ([B,Nf,3] or [Nf,3] with NR_INDICES_SHARED):
+ *   corner_shading[b,f,k,:] = (sgn n, v),   n = vertex_normals[b, faces[f,k]],  v = vertices[b, faces[f,k]]
+ *   (both 0 for an index outside [0, Nv)), sgn = -1 for the reversed copies f >= Nf/2 with NR_TEX_FILL_BACK (Nf even), else 1.
+ * The backward scatters d loss / d corner_shading [B,Nf,3,6] into grad_vertex_normals and grad_vertices [B,Nv,3] (either may
+ * be NULL, not both; each zero-filled first unless NR_GRAD_ACCUMULATE; atomics). */
+NR_B200_API int nr_b200_corner_shading(const float *vertex_normals, const float *vertices, const int32_t *faces,
+                                       int32_t batch_size, int32_t num_vertices, int32_t num_faces, uint32_t flags,
+                                       float *corner_shading, void *cuda_stream);
+NR_B200_API int nr_b200_corner_shading_backward(const int32_t *faces, const float *grad_corner_shading, int32_t batch_size,
+                                                int32_t num_vertices, int32_t num_faces, uint32_t flags,
+                                                float *grad_vertex_normals, float *grad_vertices, void *cuda_stream);
 
 /* Texture baking of load_obj (reference load_obj.py:88-137): every texel (a, b, c) of the ts^3 cube of face f is the
  * bilinear sample of `image` [H,W,3] (rows already flipped, load_obj.py:82) at the UV position with barycentric

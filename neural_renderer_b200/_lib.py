@@ -46,6 +46,8 @@ EXPORTED_SYMBOLS = (
     "nr_b200_forward",
     "nr_b200_backward",
     "nr_b200_backward_corner_light",
+    "nr_b200_forward_phong",
+    "nr_b200_backward_phong",
     "nr_b200_interpolate",
     "nr_b200_interpolate_backward",
     "nr_b200_vertices_to_faces",
@@ -59,6 +61,8 @@ EXPORTED_SYMBOLS = (
     "nr_b200_vertex_normals_backward",
     "nr_b200_corner_lighting",
     "nr_b200_corner_lighting_backward",
+    "nr_b200_corner_shading",
+    "nr_b200_corner_shading_backward",
     "nr_b200_bake_textures",
     "nr_b200_mip_texels",
     "nr_b200_mip_build",
@@ -109,6 +113,15 @@ class BackwardArgs(ctypes.Structure):
     ]
 
 
+class PhongArgs(ctypes.Structure):
+    _fields_ = [
+        ("struct_size", ctypes.c_uint32), ("shading_batch", ctypes.c_int32),
+        ("params_batch", ctypes.c_int32), ("_pad0", ctypes.c_int32),
+        ("corner_shading", ctypes.c_void_p), ("params", ctypes.c_void_p),
+        ("grad_corner_shading", ctypes.c_void_p), ("grad_params", ctypes.c_void_p),
+    ]
+
+
 class InterpolateArgs(ctypes.Structure):
     _fields_ = [
         ("struct_size", ctypes.c_uint32), ("flags", ctypes.c_uint32),
@@ -154,6 +167,10 @@ def load():
     lib.nr_b200_backward_corner_light.restype = ctypes.c_int
     lib.nr_b200_backward_corner_light.argtypes = [ctypes.POINTER(BackwardArgs), ctypes.c_void_p, ctypes.c_void_p,
                                                   ctypes.c_void_p]
+    lib.nr_b200_forward_phong.restype = ctypes.c_int
+    lib.nr_b200_forward_phong.argtypes = [ctypes.POINTER(ForwardArgs), ctypes.POINTER(PhongArgs), ctypes.c_void_p]
+    lib.nr_b200_backward_phong.restype = ctypes.c_int
+    lib.nr_b200_backward_phong.argtypes = [ctypes.POINTER(BackwardArgs), ctypes.POINTER(PhongArgs), ctypes.c_void_p]
     for name in ("nr_b200_interpolate", "nr_b200_interpolate_backward"):
         fn = getattr(lib, name)
         fn.restype = ctypes.c_int
@@ -190,6 +207,12 @@ def load():
     lib.nr_b200_corner_lighting_backward.restype = ctypes.c_int
     lib.nr_b200_corner_lighting_backward.argtypes = [ctypes.c_void_p] * 4 + [ctypes.c_int32] * 3 + [ctypes.c_uint32,
                                                                                                   ctypes.c_void_p, ctypes.c_void_p]
+    lib.nr_b200_corner_shading.restype = ctypes.c_int
+    lib.nr_b200_corner_shading.argtypes = [ctypes.c_void_p] * 3 + [ctypes.c_int32] * 3 + [ctypes.c_uint32, ctypes.c_void_p,
+                                                                                        ctypes.c_void_p]
+    lib.nr_b200_corner_shading_backward.restype = ctypes.c_int
+    lib.nr_b200_corner_shading_backward.argtypes = [ctypes.c_void_p] * 2 + [ctypes.c_int32] * 3 + [ctypes.c_uint32] + \
+        [ctypes.c_void_p] * 3
     lib.nr_b200_bake_textures.restype = ctypes.c_int
     lib.nr_b200_bake_textures.argtypes = [ctypes.c_void_p] * 3 + [ctypes.c_int32] * 4 + [ctypes.c_void_p, ctypes.c_void_p]
     lib.nr_b200_mip_texels.restype = ctypes.c_size_t

@@ -46,6 +46,7 @@
 #include "nr_interior.h"
 #include "nr_internal.h"
 #include "nr_math.cuh"
+#include "nr_phong.h"
 
 #ifndef NR_ES_CTAS_PER_1024
 #define NR_ES_CTAS_PER_1024 6   // k_edge_scan CTAs per SM at 128 threads (6 = 80 registers; 8 = 64 spills on sm_90 and was
@@ -147,6 +148,11 @@ struct BwdParams {
     // smooth shading (appended likewise): corner_light [B,F,3,3] (the kCorner variants) and its gradient, or nullptr
     const float* corner_light;
     float* grad_corner_light;
+    // Phong shading (appended likewise, the kLight == 3 variants): corner_shading [Bc,F,3,6] and params [Bp,16]
+    const float* phong_cs;
+    const float* phong_prm;
+    size_t cs_bstride;   // faces per item in phong_cs (0 with Bc = 1)
+    size_t prm_bstride;  // floats per item in phong_prm (0 with Bp = 1)
 };
 
 //@phase helpers: rcp / vector RED / load_grad (inlined)
@@ -971,17 +977,21 @@ __device__ __forceinline__ void light_grad_scatter(float (&gl)[N], int fn, int l
 // that sit next to each other with the same (cube, cell) therefore add their 8 x 3 contributions together with
 // kTgCombine shuffle steps first (runs of up to 2^kTgCombine lanes collapse into one lane's reductions).
 //
+// kLight: 0 = face_light or unlit, 2 = corner_light, 3 = Phong.
 // kCorner (corner_light): the pixel's light L_c = the corner factors interpolated with its perspective weights l_k (own
 // vertex depths) takes face_light's place, and d loss / d corner_light = l_k g_c s_c goes through the same run reduction.
-template <int kTgCombine, bool kCorner>
-__global__ void __launch_bounds__(256, kTgCombine ? (kCorner ? NR_TGC_MIN_CTAS : 4) : NR_TG_MIN_CTAS) k_texture_grad(const __grid_constant__ BwdParams p) {
+// kPhong: L_c = the diffuse part of the Phong expression at the pixel (nr::phong_diffuse) takes face_light's place; the
+// Phong gradients themselves come from k_phong_grad (nr_phong.cu).
+template <int kTgCombine, int kLight>
+__global__ void __launch_bounds__(256, kTgCombine ? (kLight >= 2 ? NR_TGC_MIN_CTAS : 4) : NR_TG_MIN_CTAS) k_texture_grad(const __grid_constant__ BwdParams p) {
+    constexpr bool kCorner = kLight == 2, kPhong = kLight == 3;
     const int S = p.S;
     const size_t plane = (size_t)S * S;
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;  // pixel within the image (image orientation)
     const int b = blockIdx.y;
     const int lane = threadIdx.x & 31;
     const int fn = (i < plane) ? __ldg(p.fim + (size_t)b * plane + i) : -1;
-    const bool want_light = (kCorner ? p.grad_corner_light : p.grad_face_light) != nullptr;  // uniform
+    const bool want_light = !kPhong && (kCorner ? p.grad_corner_light : p.grad_face_light) != nullptr;  // uniform
     if (kTgCombine) {
         if (!want_light && !__any_sync(0xffffffffu, fn >= 0)) return;  // warp-uniform
     } else {
@@ -1019,15 +1029,21 @@ __global__ void __launch_bounds__(256, kTgCombine ? (kCorner ? NR_TGC_MIN_CTAS :
             z2 = __ldg(nr::face_vertex_t<true>(p.src, zb, fn, 2) + 2);
         }
         const nr::TexCoord tc = nr::texture_coords(w, zp, z0, z1, z2, ts, p.tex_cmp, p.tex_val);
-        float lam[3] = {0.0f, 0.0f, 0.0f}, L[3];  // kCorner: perspective weights (own depths) and light of the pixel
-        if constexpr (kCorner) {  // l_k with the item's own depths (NR_TEX_Z_BATCH0 only moves the cube coordinates)
+        float lam[3] = {0.0f, 0.0f, 0.0f}, L[3];  // kCorner / kPhong: perspective weights (own depths) and light of the pixel
+        if constexpr (kCorner || kPhong) {  // l_k with the item's own depths (NR_TEX_Z_BATCH0 only moves the cube coordinates)
             float oz[3] = {z0, z1, z2};
             if (zb != b) {
 #pragma unroll
                 for (int k = 0; k < 3; k++) oz[k] = __ldg(nr::face_vertex(p.src, b, fn, k) + 2);
             }
             nr::perspective_weights(w, zp, oz[0], oz[1], oz[2], lam);
-            nr::corner_light_at(p.corner_light + ((size_t)b * p.F + fn) * 9, lam, L);
+            if constexpr (kCorner) {
+                nr::corner_light_at(p.corner_light + ((size_t)b * p.F + fn) * 9, lam, L);
+            } else {
+                nr::PhongEval E;
+                nr::phong_diffuse(p.phong_cs + ((size_t)b * p.cs_bstride + fn) * 18, lam, p.phong_prm + (size_t)b * p.prm_bstride, E);
+                L[0] = E.L[0]; L[1] = E.L[1]; L[2] = E.L[2];
+            }
         }
         // NR_TEX_FILL_BACK: the reversed copy of face f - F/2 shares that face's cube, axes reversed
         int cube = fn, ncubes = p.F;
@@ -1055,7 +1071,7 @@ __global__ void __launch_bounds__(256, kTgCombine ? (kCorner ? NR_TGC_MIN_CTAS :
                 gl0 = r * g0; gl1 = g * g1; gl2 = bl * g2;
             }
         }
-        if constexpr (kCorner) {  // d rgb / d texel = weight * interpolated light
+        if constexpr (kCorner || kPhong) {  // d rgb / d texel = weight * interpolated light
             g0 *= L[0]; g1 *= L[1]; g2 *= L[2];
         } else if (p.face_light) {  // d rgb / d texel = weight * light
             const float* lp = p.face_light + ((size_t)b * p.F + fn) * 3;
@@ -1165,10 +1181,12 @@ __device__ __forceinline__ void red_add_6(float* t, const float v[6]) {
 // weight) goes to UV corner k as l_k (gu, gv), corners reversed back for a fill_back copy.  Runs of neighbouring lanes
 // that show the same face sum their 6 floats with shuffles and the run's first lane adds them.
 //
+// kLight: 0 = face_light or unlit, 2 = corner_light, 3 = Phong.
 // kCorner (corner_light): as in k_texture_grad, the interpolated light L_c replaces face_light (also in the face_uvs
-// gradient) and the 9-float corner-light gradient goes through the run reduction.
-template <int kTgCombine, bool kMip, bool kUvGrad, bool kCorner>
+// gradient) and the 9-float corner-light gradient goes through the run reduction.  kPhong: likewise with the Phong L_c.
+template <int kTgCombine, bool kMip, bool kUvGrad, int kLight>
 __device__ __forceinline__ void image_grad(const BwdParams& p) {
+    constexpr bool kCorner = kLight == 2, kPhong = kLight == 3;
     constexpr int kPairs = kMip ? 4 : 2;
     const int S = p.S;
     const size_t plane = (size_t)S * S;
@@ -1176,7 +1194,7 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
     const int b = blockIdx.y;
     const int lane = threadIdx.x & 31;
     const int fn = (i < plane) ? __ldg(p.fim + (size_t)b * plane + i) : -1;
-    const bool want_light = (kCorner ? p.grad_corner_light : p.grad_face_light) != nullptr;  // uniform
+    const bool want_light = !kPhong && (kCorner ? p.grad_corner_light : p.grad_face_light) != nullptr;  // uniform
     if (!want_light && !__any_sync(0xffffffffu, fn >= 0)) return;  // warp-uniform
     float gl0 = 0.0f, gl1 = 0.0f, gl2 = 0.0f;  // d loss / d face_light of this pixel
     float glc[kCorner ? 9 : 1];                // kCorner: d loss / d corner_light of this pixel
@@ -1232,10 +1250,15 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
         float uv[6], u, v;
         nr::load_face_uvs(p.uvs + ((uint32_t)b * p.uv_bstride + (uint32_t)uf * 6u), rev, uv);
         nr::pixel_uv(w, zp, z0, z1, z2, uv, u, v);
-        float lam[3] = {0.0f, 0.0f, 0.0f}, L[3];  // kCorner: perspective weights and light of the pixel
+        float lam[3] = {0.0f, 0.0f, 0.0f}, L[3];  // kCorner / kPhong: perspective weights and light of the pixel
         if constexpr (kCorner) {
             nr::perspective_weights(w, zp, z0, z1, z2, lam);
             nr::corner_light_at(p.corner_light + ((size_t)b * p.F + fn) * 9, lam, L);
+        } else if constexpr (kPhong) {
+            nr::perspective_weights(w, zp, z0, z1, z2, lam);
+            nr::PhongEval E;
+            nr::phong_diffuse(p.phong_cs + ((size_t)b * p.cs_bstride + fn) * 18, lam, p.phong_prm + (size_t)b * p.prm_bstride, E);
+            L[0] = E.L[0]; L[1] = E.L[1]; L[2] = E.L[2];
         }
         const uint32_t img_off = (uint32_t)b * p.img_bstride;
         // level(s) and their weights: the bilinear variant is level 0 of an image with weight 1
@@ -1251,7 +1274,7 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
         const nr::UvTaps t0 = nr::uv_taps(u, v, kMip ? p.mip.h[lv[0]] : p.Ht, kMip ? p.mip.w[lv[0]] : p.Wt);
         if constexpr (kUvGrad) {
             float lt[3] = {1.0f, 1.0f, 1.0f};
-            if constexpr (kCorner) {
+            if constexpr (kCorner || kPhong) {
                 lt[0] = L[0]; lt[1] = L[1]; lt[2] = L[2];
             } else if (p.face_light) {
                 const float* lp = p.face_light + ((size_t)b * p.F + fn) * 3;
@@ -1299,7 +1322,7 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
             if constexpr (kCorner) corner_light_grad(c, g0, g1, g2, lam, glc);
             else { gl0 = c[0] * g0; gl1 = c[1] * g1; gl2 = c[2] * g2; }
         }
-        if constexpr (kCorner) {  // d rgb / d texel = weight * interpolated light
+        if constexpr (kCorner || kPhong) {  // d rgb / d texel = weight * interpolated light
             g0 *= L[0]; g1 *= L[1]; g2 *= L[2];
         } else if (p.face_light) {  // d rgb / d texel = weight * light
             const float* lp = p.face_light + ((size_t)b * p.F + fn) * 3;
@@ -1410,13 +1433,13 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
     }
 }
 
-template <int kTgCombine, bool kUvGrad, bool kCorner>
+template <int kTgCombine, bool kUvGrad, int kLight>
 __global__ void __launch_bounds__(256, kUvGrad ? NR_IGU_MIN_CTAS : NR_IG_MIN_CTAS) k_image_grad(const __grid_constant__ BwdParams p) {
-    image_grad<kTgCombine, false, kUvGrad, kCorner>(p);
+    image_grad<kTgCombine, false, kUvGrad, kLight>(p);
 }
-template <int kTgCombine, bool kUvGrad, bool kCorner>
+template <int kTgCombine, bool kUvGrad, int kLight>
 __global__ void __launch_bounds__(256, kUvGrad ? NR_IGMU_MIN_CTAS : NR_IGM_MIN_CTAS) k_image_grad_mip(const __grid_constant__ BwdParams p) {
-    image_grad<kTgCombine, true, kUvGrad, kCorner>(p);
+    image_grad<kTgCombine, true, kUvGrad, kLight>(p);
 }
 
 // ----------------------------------------------------------------------------------------------- k_depth_grad
@@ -1571,9 +1594,9 @@ extern "C" size_t nr_b200_backward_workspace_bytes(int32_t B, int32_t F, int32_t
     return bin_layout(B, F, S, strip_rec_bytes(S, both)).total;
 }
 
-// nr_b200_backward (corner_light NULL) and nr_b200_backward_corner_light (smooth shading)
+// nr_b200_backward (corner_light, phong NULL), nr_b200_backward_corner_light (smooth shading) and nr_b200_backward_phong
 static int backward_impl(const nr_b200_backward_args* args, const float* corner_light, float* grad_corner_light,
-                         void* cuda_stream) {
+                         const nr_b200_phong_args* phong, void* cuda_stream) {
     nr_internal::launch_count() = 0;
     // Two layouts: the full struct, and the ABI-4 struct from before grad_face_uvs (which then reads as NULL).  Only the
     // caller's struct_size bytes are read.
@@ -1614,9 +1637,14 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
     const bool smooth = corner_light != nullptr;
     if (smooth && (!rgb || a->face_light)) return NR_ERR_INVALID_ARG;
     if (grad_corner_light && (!smooth || !a->textures)) return NR_ERR_INVALID_ARG;
+    // Phong: only for RGB and instead of face_light / corner_light; its gradients read the (unlit) textures
+    const bool phong_grads = phong && (phong->grad_corner_shading || phong->grad_params);
+    if (phong && (!rgb || a->face_light || smooth || !nr_internal::phong_args_ok(phong, B))) return NR_ERR_INVALID_ARG;
+    if (phong_grads && !a->textures) return NR_ERR_INVALID_ARG;
     // NR_GRAD_INTERIOR: the sampler's derivative reads the textures; the cubes of NR_TEX_Z_BATCH0 sample item b with the
     // depths of item 0, so their derivative would cross items (B = 1 is the plain sampler)
     const bool interior = (flags & NR_GRAD_INTERIOR) != 0;
+    if (interior && phong) return NR_ERR_UNSUPPORTED;  // no vertex gradient through l_k of the Phong normal and position
     if (interior && (!rgb || !a->textures)) return NR_ERR_INVALID_ARG;
     if (interior && !uv && (flags & NR_TEX_Z_BATCH0) && B > 1) return NR_ERR_INVALID_ARG;
     if ((flags & NR_ANTI_ALIASING) && (S & 1)) return NR_ERR_INVALID_ARG;
@@ -1664,6 +1692,12 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
         if (part_tex && grad_corner_light &&
             cudaMemsetAsync(grad_corner_light, 0, (size_t)B * F * 9 * sizeof(float), stream) != cudaSuccess)
             return NR_ERR_CUDA;
+        if (part_tex && phong && phong->grad_corner_shading &&
+            cudaMemsetAsync(phong->grad_corner_shading, 0, (size_t)phong->shading_batch * F * 18 * sizeof(float), stream) != cudaSuccess)
+            return NR_ERR_CUDA;
+        if (part_tex && phong && phong->grad_params &&
+            cudaMemsetAsync(phong->grad_params, 0, (size_t)phong->params_batch * 16 * sizeof(float), stream) != cudaSuccess)
+            return NR_ERR_CUDA;
         nr_internal::prof_end(stream);
     }
 
@@ -1690,31 +1724,54 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
         p.grad_uvs = a->grad_face_uvs;
     }
     p.corner_light = corner_light; p.grad_corner_light = grad_corner_light;
+    if (phong) {
+        p.phong_cs = phong->corner_shading; p.phong_prm = phong->params;
+        p.cs_bstride = phong->shading_batch == 1 ? 0 : (size_t)F;
+        p.prm_bstride = phong->params_batch == 1 ? 0 : 16;
+    }
+    const int light = phong ? 3 : (smooth ? 2 : 0);
 
     const dim3 pgrid((unsigned)(((size_t)S * S + 255) / 256), B);
     auto launch_texture_grad = [&]() {
         if (mip) {
             nr_internal::LaunchScope ls("k_image_grad", stream);
-            if (smooth && uv_grad) k_image_grad_mip<NR_TG_COMBINE, true, true><<<pgrid, 256, 0, stream>>>(p);
-            else if (smooth) k_image_grad_mip<NR_TG_COMBINE, false, true><<<pgrid, 256, 0, stream>>>(p);
-            else if (uv_grad) k_image_grad_mip<NR_TG_COMBINE, true, false><<<pgrid, 256, 0, stream>>>(p);
-            else k_image_grad_mip<NR_TG_COMBINE, false, false><<<pgrid, 256, 0, stream>>>(p);
+            if (light == 3 && uv_grad) k_image_grad_mip<NR_TG_COMBINE, true, 3><<<pgrid, 256, 0, stream>>>(p);
+            else if (light == 3) k_image_grad_mip<NR_TG_COMBINE, false, 3><<<pgrid, 256, 0, stream>>>(p);
+            else if (smooth && uv_grad) k_image_grad_mip<NR_TG_COMBINE, true, 2><<<pgrid, 256, 0, stream>>>(p);
+            else if (smooth) k_image_grad_mip<NR_TG_COMBINE, false, 2><<<pgrid, 256, 0, stream>>>(p);
+            else if (uv_grad) k_image_grad_mip<NR_TG_COMBINE, true, 0><<<pgrid, 256, 0, stream>>>(p);
+            else k_image_grad_mip<NR_TG_COMBINE, false, 0><<<pgrid, 256, 0, stream>>>(p);
             return;
         }
         if (uv) {
             nr_internal::LaunchScope ls("k_image_grad", stream);
-            if (smooth && uv_grad) k_image_grad<NR_TG_COMBINE, true, true><<<pgrid, 256, 0, stream>>>(p);
-            else if (smooth) k_image_grad<NR_TG_COMBINE, false, true><<<pgrid, 256, 0, stream>>>(p);
-            else if (uv_grad) k_image_grad<NR_TG_COMBINE, true, false><<<pgrid, 256, 0, stream>>>(p);
-            else k_image_grad<NR_TG_COMBINE, false, false><<<pgrid, 256, 0, stream>>>(p);
+            if (light == 3 && uv_grad) k_image_grad<NR_TG_COMBINE, true, 3><<<pgrid, 256, 0, stream>>>(p);
+            else if (light == 3) k_image_grad<NR_TG_COMBINE, false, 3><<<pgrid, 256, 0, stream>>>(p);
+            else if (smooth && uv_grad) k_image_grad<NR_TG_COMBINE, true, 2><<<pgrid, 256, 0, stream>>>(p);
+            else if (smooth) k_image_grad<NR_TG_COMBINE, false, 2><<<pgrid, 256, 0, stream>>>(p);
+            else if (uv_grad) k_image_grad<NR_TG_COMBINE, true, 0><<<pgrid, 256, 0, stream>>>(p);
+            else k_image_grad<NR_TG_COMBINE, false, 0><<<pgrid, 256, 0, stream>>>(p);
             return;
         }
         nr_internal::LaunchScope ls("k_texture_grad", stream);
-        if (smooth) k_texture_grad<NR_TG_COMBINE, true><<<pgrid, 256, 0, stream>>>(p);
-        else k_texture_grad<NR_TG_COMBINE, false><<<pgrid, 256, 0, stream>>>(p);
+        if (light == 3) k_texture_grad<NR_TG_COMBINE, 3><<<pgrid, 256, 0, stream>>>(p);
+        else if (smooth) k_texture_grad<NR_TG_COMBINE, 2><<<pgrid, 256, 0, stream>>>(p);
+        else k_texture_grad<NR_TG_COMBINE, 0><<<pgrid, 256, 0, stream>>>(p);
+    };
+    // Phong: d loss / d corner_shading and d params per pixel (nr_phong.cu), part of the texture half
+    auto launch_phong_grad = [&]() {
+        if (!phong_grads) return;
+        nr_internal::PhongGradLaunch pl{};
+        pl.args = a; pl.src = src; pl.phong = phong;
+        pl.tex_bstride = (flags & NR_TEX_SHARED) ? 0 : (uv ? img_floats : ncubes * (size_t)ts * ts * ts * 3);
+        pl.uv_bstride = p.uv_bstride;
+        pl.tex_cmp = p.tex_cmp; pl.tex_val = p.tex_val;
+        pl.mip = mip ? &mt : nullptr;
+        nr_internal::launch_phong_grad(pl, stream);
     };
     // K6 first, unless its output buffer is zero-filled by the edge scan
     if (part_tex && rgb && p.g_rgb && !fill_in_scan) launch_texture_grad();
+    if (part_tex && rgb && p.g_rgb) launch_phong_grad();
     if (!part_faces) return cudaGetLastError() == cudaSuccess ? NR_OK : NR_ERR_CUDA;
 
     // K5 runs when an rgb or alpha gradient exists (rasterize.py:523); without upstream gradients it contributes 0
@@ -1814,7 +1871,7 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
 }
 
 extern "C" int nr_b200_backward(const nr_b200_backward_args* args, void* cuda_stream) {
-    return backward_impl(args, nullptr, nullptr, cuda_stream);
+    return backward_impl(args, nullptr, nullptr, nullptr, cuda_stream);
 }
 
 extern "C" int nr_b200_backward_corner_light(const nr_b200_backward_args* args, const float* corner_light,
@@ -1823,5 +1880,13 @@ extern "C" int nr_b200_backward_corner_light(const nr_b200_backward_args* args, 
         nr_internal::launch_count() = 0;
         return NR_ERR_INVALID_ARG;
     }
-    return backward_impl(args, corner_light, grad_corner_light, cuda_stream);
+    return backward_impl(args, corner_light, grad_corner_light, nullptr, cuda_stream);
+}
+
+extern "C" int nr_b200_backward_phong(const nr_b200_backward_args* args, const nr_b200_phong_args* phong, void* cuda_stream) {
+    if (!phong) {
+        nr_internal::launch_count() = 0;
+        return NR_ERR_INVALID_ARG;
+    }
+    return backward_impl(args, nullptr, nullptr, phong, cuda_stream);
 }

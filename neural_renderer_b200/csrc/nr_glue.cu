@@ -403,6 +403,58 @@ __global__ void __launch_bounds__(256) k_corner_light_bwd(const float* __restric
     }
 }
 
+// corner_shading[b,f,k,:] = (sgn n, v) of the corner's vertex (zeros for an index outside [0, Nv)); sgn = -1 for the
+// reversed copies f >= Nf/2 with NR_TEX_FILL_BACK
+__global__ void __launch_bounds__(256) k_corner_shading_fwd(const float* __restrict__ normals, const float* __restrict__ vertices,
+                                                            const int32_t* __restrict__ faces, int Nv, int Nf, uint32_t flags,
+                                                            float* __restrict__ out) {
+    const int b = blockIdx.y;
+    const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= Nf) return;
+    const int32_t* fi = faces + ((size_t)((flags & NR_INDICES_SHARED) ? 0 : b) * Nf + f) * 3;
+    const float sgn = ((flags & NR_TEX_FILL_BACK) && f >= (Nf >> 1)) ? -1.0f : 1.0f;
+    float* o = out + ((size_t)b * Nf + f) * 18;
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        const int idx = __ldg(fi + k);
+        float n[3] = {0.0f, 0.0f, 0.0f}, v[3] = {0.0f, 0.0f, 0.0f};
+        if ((unsigned)idx < (unsigned)Nv) {
+            const float* qn = normals + ((size_t)b * Nv + idx) * 3;
+            const float* qv = vertices + ((size_t)b * Nv + idx) * 3;
+#pragma unroll
+            for (int c = 0; c < 3; c++) { n[c] = sgn * __ldg(qn + c); v[c] = __ldg(qv + c); }
+        }
+#pragma unroll
+        for (int c = 0; c < 3; c++) { o[6 * k + c] = n[c]; o[6 * k + 3 + c] = v[c]; }
+    }
+}
+
+__global__ void __launch_bounds__(256) k_corner_shading_bwd(const int32_t* __restrict__ faces, const float* __restrict__ grad,
+                                                            int Nv, int Nf, uint32_t flags, float* __restrict__ grad_normals,
+                                                            float* __restrict__ grad_vertices) {
+    const int b = blockIdx.y;
+    const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= Nf) return;
+    const int32_t* fi = faces + ((size_t)((flags & NR_INDICES_SHARED) ? 0 : b) * Nf + f) * 3;
+    const float sgn = ((flags & NR_TEX_FILL_BACK) && f >= (Nf >> 1)) ? -1.0f : 1.0f;
+    const float* g = grad + ((size_t)b * Nf + f) * 18;
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        const int idx = __ldg(fi + k);
+        if ((unsigned)idx >= (unsigned)Nv) continue;
+        if (grad_normals) {
+            float* o = grad_normals + ((size_t)b * Nv + idx) * 3;
+#pragma unroll
+            for (int c = 0; c < 3; c++) atomicAdd(o + c, sgn * __ldg(g + 6 * k + c));
+        }
+        if (grad_vertices) {
+            float* o = grad_vertices + ((size_t)b * Nv + idx) * 3;
+#pragma unroll
+            for (int c = 0; c < 3; c++) atomicAdd(o + c, __ldg(g + 6 * k + 3 + c));
+        }
+    }
+}
+
 struct VnLayout {
     size_t n;  // corners of the index set (items x 3 Nf)
     int end_bit;
@@ -669,6 +721,41 @@ extern "C" int nr_b200_corner_lighting_backward(const float* normals, const int3
         k_corner_light_bwd<<<dim3((unsigned)((Nf + 255) / 256), B), 256, 0, stream>>>(normals, faces, light_params,
                                                                                      grad_corner_light, Nv, Nf, flags,
                                                                                      grad_normals);
+    }
+    return cudaGetLastError() == cudaSuccess ? NR_OK : NR_ERR_CUDA;
+}
+
+extern "C" int nr_b200_corner_shading(const float* normals, const float* vertices, const int32_t* faces, int32_t B, int32_t Nv,
+                                      int32_t Nf, uint32_t flags, float* corner_shading, void* cuda_stream) {
+    nr_internal::launch_count() = 0;
+    if (!normals || !vertices || !faces || !corner_shading || B <= 0 || Nv <= 0 || Nf <= 0 || B > 65535) return NR_ERR_INVALID_ARG;
+    if ((flags & NR_TEX_FILL_BACK) && (Nf & 1)) return NR_ERR_INVALID_ARG;
+    cudaStream_t stream = (cudaStream_t)cuda_stream;
+    {
+        nr_internal::LaunchScope ls("k_corner_shading_fwd", stream);
+        k_corner_shading_fwd<<<dim3((unsigned)((Nf + 255) / 256), B), 256, 0, stream>>>(normals, vertices, faces, Nv, Nf, flags,
+                                                                                       corner_shading);
+    }
+    return cudaGetLastError() == cudaSuccess ? NR_OK : NR_ERR_CUDA;
+}
+
+extern "C" int nr_b200_corner_shading_backward(const int32_t* faces, const float* grad_corner_shading, int32_t B, int32_t Nv,
+                                               int32_t Nf, uint32_t flags, float* grad_normals, float* grad_vertices,
+                                               void* cuda_stream) {
+    nr_internal::launch_count() = 0;
+    if (!faces || !grad_corner_shading || (!grad_normals && !grad_vertices) || B <= 0 || Nv <= 0 || Nf <= 0 || B > 65535)
+        return NR_ERR_INVALID_ARG;
+    if ((flags & NR_TEX_FILL_BACK) && (Nf & 1)) return NR_ERR_INVALID_ARG;
+    cudaStream_t stream = (cudaStream_t)cuda_stream;
+    if (!(flags & NR_GRAD_ACCUMULATE)) {
+        const size_t bytes = (size_t)B * Nv * 3 * sizeof(float);
+        if (grad_normals && cudaMemsetAsync(grad_normals, 0, bytes, stream) != cudaSuccess) return NR_ERR_CUDA;
+        if (grad_vertices && cudaMemsetAsync(grad_vertices, 0, bytes, stream) != cudaSuccess) return NR_ERR_CUDA;
+    }
+    {
+        nr_internal::LaunchScope ls("k_corner_shading_bwd", stream);
+        k_corner_shading_bwd<<<dim3((unsigned)((Nf + 255) / 256), B), 256, 0, stream>>>(faces, grad_corner_shading, Nv, Nf, flags,
+                                                                                       grad_normals, grad_vertices);
     }
     return cudaGetLastError() == cudaSuccess ? NR_OK : NR_ERR_CUDA;
 }

@@ -48,6 +48,12 @@ inline bool make_face_grad(uint32_t flags, float* grad_faces, float* grad_vertic
     return true;
 }
 
+// the checks every Phong entry point makes on its nr_b200_phong_args (the size first: only then are the fields read)
+inline bool phong_args_ok(const nr_b200_phong_args* ph, int B) {
+    return ph->struct_size == sizeof(nr_b200_phong_args) && ph->corner_shading && ph->params &&
+           (ph->shading_batch == 1 || ph->shading_batch == B) && (ph->params_batch == 1 || ph->params_batch == B);
+}
+
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) is issued once per (kernel instantiation, device, size high-water
 // mark) instead of on every launch: `slot` is a function-local static of the launching template.
 struct SmemOptIn {

@@ -1,0 +1,218 @@
+// nr_phong.cu -- the Phong-shading gradients of nr_b200_backward_phong (include/nr_b200.h, nr_b200_phong_args).
+//
+//   k_phong_grad<kTex, kIdx>   one thread per raster pixel, modelled on k_interior_grad.  The winner's perspective weights
+//                   l_k and the unlit sample s are recomputed with the forward's device helpers (the depth map gives zp;
+//                   per-face cubes read the sampler depths NR_TEX_Z_BATCH0 selects), nr::phong_at evaluates the forward's
+//                   expression and nr::phong_grad its derivative.  The 18 corner floats l_k (d loss / d n, d loss / d p) go
+//                   through k_depth_grad's segmented run reduction (runs of neighbouring lanes that show the same face)
+//                   before one set of atomics per run; the 16 parameter floats are summed over the warp, then over the CTA
+//                   in shared memory, before 16 atomics per CTA.  kTex: 0 = per-face cubes, 1 = bilinear image,
+//                   2 = trilinear pyramid.  Anti-aliasing and fill_back are runtime flags.
+//
+// It belongs to the texture half of the backward: the texture-gradient kernels (K6, k_image_grad) only need the pixel's
+// L_c, and keeping the 34 gradient floats out of them keeps their register budgets (DESIGN.md section 4g).
+#include <cuda_runtime.h>
+#include <stdint.h>
+#include <string.h>
+
+#include "nr_b200.h"
+#include "nr_internal.h"
+#include "nr_math.cuh"
+#include "nr_phong.h"
+
+namespace {
+
+struct PhongParams {
+    nr::FaceSrc src;
+    const int32_t* fim;     // [B,S,S]
+    const float* wmap;      // [B,3,S,S]
+    const float* dmap;      // [B,S,S]
+    const float* g;         // grad_rgb [B,3,H,W] (API layout)
+    const float* textures;  // cubes [.,F',ts,ts,ts,3], image [.,Ht,Wt,3] or packed pyramid [.,P,3]
+    size_t tex_bstride;     // floats per item in textures (0 = shared)
+    const float* uvs;       // [.,F',3,2]
+    uint32_t uv_bstride;    // floats per item in uvs (0 = shared)
+    const float* cs;        // corner_shading [Bc,F,3,6]
+    const float* prm;       // params [Bp,16]
+    float* grad_cs;         // or nullptr
+    float* grad_prm;        // or nullptr
+    size_t cs_bstride;      // faces per item in cs (0 with Bc = 1)
+    size_t prm_bstride;     // floats per item in prm (0 with Bp = 1)
+    int S, F, ts, Ht, Wt;
+    int aa, fill_back, z_batch0;
+    float tex_cmp, tex_val;
+    nr::MipTable mip;  // kTex 2
+};
+
+template <int kTex, bool kIdx>
+__global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ PhongParams p) {
+    __shared__ float s_prm[8][16];
+    const int S = p.S;
+    const size_t plane = (size_t)S * S;
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int b = blockIdx.y;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int fn = (i < plane) ? __ldg(p.fim + (size_t)b * plane + i) : -1;
+    if (!__syncthreads_or(fn >= 0)) return;  // CTA-uniform
+    float cg[18], gprm[16];
+#pragma unroll
+    for (int k = 0; k < 18; k++) cg[k] = 0.0f;
+#pragma unroll
+    for (int k = 0; k < 16; k++) gprm[k] = 0.0f;
+    if (fn >= 0) {
+        const int r = (int)(i / S), c = (int)(i % S);
+        const bool aa = p.aa != 0;
+        const int H = aa ? (S >> 1) : S;
+        const size_t gplane = (size_t)H * H;
+        const size_t goff = aa ? (size_t)(r >> 1) * H + (c >> 1) : i;
+        const float gscale = aa ? 0.25f : 1.0f;  // the pooling backward
+        const float* gb = p.g + (size_t)b * 3 * gplane + goff;
+        const float g[3] = {__ldg(gb) * gscale, __ldg(gb + gplane) * gscale, __ldg(gb + 2 * gplane) * gscale};
+        const float* wm = p.wmap + (size_t)b * 3 * plane + i;
+        const float w[3] = {__ldg(wm), __ldg(wm + plane), __ldg(wm + 2 * plane)};
+        const float zp = __ldg(p.dmap + (size_t)b * plane + i);
+        float v[9];
+        if constexpr (kTex == 2) {
+            nr::load_face(p.src, b, fn, v);
+        } else {
+#pragma unroll
+            for (int k = 0; k < 3; k++) v[3 * k + 2] = __ldg(nr::face_vertex_t<kIdx>(p.src, b, fn, k) + 2);
+        }
+        const float z[3] = {v[2], v[5], v[8]};
+        float lam[3];
+        nr::perspective_weights(w, zp, z[0], z[1], z[2], lam);
+        // fill_back: face f >= F/2 is the reversed copy of face f - F/2 (cube axes / UV corners reversed)
+        int tf = fn;
+        bool rev = false;
+        if (p.fill_back) {
+            const int half = p.F >> 1;
+            if (fn >= half) { tf = fn - half; rev = true; }
+        }
+        float s[3];  // the unlit sample, as the forward computes it
+        if constexpr (kTex == 0) {
+            const int ts = p.ts;
+            float zt[3] = {z[0], z[1], z[2]};  // the sampler's depths: item 0's with NR_TEX_Z_BATCH0
+            if (p.z_batch0 && b != 0) {
+#pragma unroll
+                for (int k = 0; k < 3; k++) zt[k] = __ldg(nr::face_vertex_t<kIdx>(p.src, 0, fn, k) + 2);
+            }
+            const nr::TexCoord tc = nr::texture_coords(w, zp, zt[0], zt[1], zt[2], ts, p.tex_cmp, p.tex_val);
+            const float* tex = p.textures + ((size_t)b * p.tex_bstride + (size_t)tf * (size_t)(ts * ts * ts) * 3);
+            s[0] = s[1] = s[2] = 0.0f;
+#pragma unroll
+            for (int pn = 0; pn < 8; pn++) {
+                const float cw = nr::corner_weight(tc, pn);
+                const float* t = tex + (rev ? nr::corner_index_rev(tc, pn, ts) : nr::corner_index(tc, pn, ts)) * 3;
+                s[0] = __fmaf_rn(cw, __ldg(t), s[0]);
+                s[1] = __fmaf_rn(cw, __ldg(t + 1), s[1]);
+                s[2] = __fmaf_rn(cw, __ldg(t + 2), s[2]);
+            }
+        } else {
+            float uv[6], u, vv;
+            nr::load_face_uvs(p.uvs + ((size_t)b * p.uv_bstride + (size_t)tf * 6u), rev, uv);
+            nr::pixel_uv(w, zp, z[0], z[1], z[2], uv, u, vv);
+            const float* img = p.textures + (size_t)b * p.tex_bstride;
+            if constexpr (kTex == 2) {
+                const float fS = (float)S;
+                float inv[9];
+                nr::face_inverse(nr::to_pixel(v[0], fS), nr::to_pixel(v[1], fS), nr::to_pixel(v[3], fS), nr::to_pixel(v[4], fS),
+                                 nr::to_pixel(v[6], fS), nr::to_pixel(v[7], fS), inv);
+                const float lod = nr::mip_lod(inv, w, zp, z[0], z[1], z[2], uv, p.Ht, p.Wt, p.mip.levels);
+                nr::mip_blend<false>(img, p.mip, nr::mip_levels(lod, p.mip.levels), u, vv, 1.0f, 1.0f, 1.0f, s);
+            } else {
+                nr::uv_blend<false>(img, p.Wt, nr::uv_taps(u, vv, p.Ht, p.Wt), 1.0f, 1.0f, 1.0f, s);
+            }
+        }
+        const float* prm = p.prm + (size_t)b * p.prm_bstride;
+        nr::PhongEval E;
+        nr::phong_at(p.cs + ((size_t)b * p.cs_bstride + fn) * 18, lam, prm, E);
+        float gn[3], gp[3];
+        nr::phong_grad(E, prm, g, s, gn, gp, gprm);
+#pragma unroll
+        for (int k = 0; k < 3; k++)
+#pragma unroll
+            for (int j = 0; j < 3; j++) {
+                cg[6 * k + j] = __fmul_rn(lam[k], gn[j]);
+                cg[6 * k + 3 + j] = __fmul_rn(lam[k], gp[j]);
+            }
+    }
+    if (p.grad_cs) {  // uniform
+        // the segmented run reduction of k_depth_grad over 18 floats, then one set of atomics per run
+        const int fn_prev = __shfl_up_sync(0xffffffffu, fn, 1);
+        const uint32_t heads = __ballot_sync(0xffffffffu, lane == 0 || fn != fn_prev);
+        const uint32_t later = heads & ~((2u << lane) - 1u);
+        const int run_end = (lane == 31 || later == 0) ? 31 : (__ffs(later) - 2);
+#pragma unroll
+        for (int off = 1; off < 32; off <<= 1) {
+            const bool take = lane + off <= run_end;
+#pragma unroll
+            for (int k = 0; k < 18; k++) {
+                const float t = __shfl_down_sync(0xffffffffu, cg[k], off);
+                if (take) cg[k] += t;
+            }
+        }
+        if (fn >= 0 && ((heads >> lane) & 1u)) {
+            float* o = p.grad_cs + ((size_t)b * p.cs_bstride + fn) * 18;
+#pragma unroll
+            for (int k = 0; k < 18; k++) atomicAdd(o + k, cg[k]);
+        }
+    }
+    if (p.grad_prm) {  // uniform: warp sums, then the CTA's sum in shared memory, 16 atomics per CTA
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1)
+#pragma unroll
+            for (int k = 0; k < 16; k++) gprm[k] += __shfl_xor_sync(0xffffffffu, gprm[k], off);
+        if (lane == 0) {
+#pragma unroll
+            for (int k = 0; k < 16; k++) s_prm[warp][k] = gprm[k];
+        }
+        __syncthreads();
+        if (threadIdx.x < 16) {
+            float t = 0.0f;
+            const int nw = (int)(blockDim.x >> 5);
+            for (int w = 0; w < nw; w++) t += s_prm[w][threadIdx.x];
+            atomicAdd(p.grad_prm + (size_t)b * p.prm_bstride + threadIdx.x, t);
+        }
+    }
+}
+
+template <int kTex>
+void launch_t(const PhongParams& p, bool idx, dim3 grid, cudaStream_t s) {
+    if (idx) k_phong_grad<kTex, true><<<grid, 256, 0, s>>>(p);
+    else k_phong_grad<kTex, false><<<grid, 256, 0, s>>>(p);
+}
+
+}  // namespace
+
+namespace nr_internal {
+
+void launch_phong_grad(const PhongGradLaunch& L, cudaStream_t stream) {
+    const nr_b200_backward_args* a = L.args;
+    const nr_b200_phong_args* ph = L.phong;
+    const uint32_t flags = a->flags;
+    PhongParams p;
+    memset(&p, 0, sizeof(p));
+    p.src = L.src;
+    p.fim = a->face_index_map; p.wmap = a->weight_map; p.dmap = a->depth_map; p.g = a->grad_rgb;
+    p.textures = a->textures; p.tex_bstride = L.tex_bstride;
+    p.uvs = a->face_uvs; p.uv_bstride = L.uv_bstride;
+    p.cs = ph->corner_shading; p.prm = ph->params;
+    p.grad_cs = ph->grad_corner_shading; p.grad_prm = ph->grad_params;
+    p.cs_bstride = ph->shading_batch == 1 ? 0 : (size_t)a->num_faces;
+    p.prm_bstride = ph->params_batch == 1 ? 0 : 16;
+    p.S = a->raster_size; p.F = a->num_faces; p.ts = a->texture_size;
+    p.Ht = a->texture_height; p.Wt = a->texture_width;
+    p.aa = (flags & NR_ANTI_ALIASING) ? 1 : 0;
+    p.fill_back = (flags & NR_TEX_FILL_BACK) ? 1 : 0;
+    p.z_batch0 = (flags & NR_TEX_Z_BATCH0) ? 1 : 0;
+    p.tex_cmp = L.tex_cmp; p.tex_val = L.tex_val;
+    if (L.mip) p.mip = *L.mip;
+    const bool idx = (flags & NR_FACES_INDEXED) != 0;
+    const dim3 grid((unsigned)(((size_t)p.S * p.S + 255) / 256), a->batch_size);
+    LaunchScope ls("k_phong_grad", stream);
+    if (flags & NR_TEX_MIPMAP) launch_t<2>(p, idx, grid, stream);
+    else if (flags & NR_TEX_UV) launch_t<1>(p, idx, grid, stream);
+    else launch_t<0>(p, idx, grid, stream);
+}
+
+}  // namespace nr_internal

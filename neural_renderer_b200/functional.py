@@ -625,3 +625,110 @@ def corner_light(vertex_normals, faces, intensity_ambient=0.5, intensity_directi
     flags = (_lib.NR_CAM_SHARED if vertex_normals.shape[0] != 1 else 0) | (_lib.NR_INDICES_SHARED if shared else 0) | \
         (_lib.NR_TEX_FILL_BACK if fill_back else 0)
     return _CornerLighting.apply(vertex_normals, faces_i32, params, flags)
+
+
+def _corner_shading_torch(vertex_normals, vertices, faces, fill_back):
+    faces = faces[None] if faces.dim() == 2 else faces
+    nf = faces.shape[1]
+    n, _ = _gather_vertices(vertex_normals, faces)  # [B,F,3 corners,3], zeros for an out-of-range index
+    p, _ = _gather_vertices(vertices, faces)
+    if fill_back:
+        sign = torch.ones(nf, dtype=n.dtype, device=n.device)
+        sign[nf // 2:] = -1
+        n = n * sign[None, :, None, None]
+    return torch.cat((n, p), dim=3)
+
+
+class _CornerShading(torch.autograd.Function):
+    """corner_shading [B,F,3,6] from vertex normals and vertices (nr_b200_corner_shading*); faces_i32 [1|B,F,3]."""
+
+    @staticmethod
+    def forward(ctx, normals, vertices, faces_i32, flags):
+        import ctypes
+        from . import _lib
+        lib = _lib.load()
+        n = normals.detach().to(torch.float32).contiguous()
+        v = vertices.detach().to(torch.float32).contiguous()
+        bs, nv = n.shape[:2]
+        nf = faces_i32.shape[1]
+        out = torch.empty((bs, nf, 3, 6), dtype=torch.float32, device=n.device)
+        with torch.cuda.device(n.device):
+            stream = ctypes.c_void_p(torch.cuda.current_stream(n.device).cuda_stream)
+            _lib.check(lib.nr_b200_corner_shading(n.data_ptr(), v.data_ptr(), faces_i32.data_ptr(), bs, nv, nf, flags,
+                                                  out.data_ptr(), stream))
+        ctx.save_for_backward(faces_i32)
+        ctx.flags, ctx.bs, ctx.nv = flags, bs, nv
+        return out
+
+    @staticmethod
+    def backward(ctx, grad):
+        import ctypes
+        from . import _lib
+        lib = _lib.load()
+        faces_i32, = ctx.saved_tensors
+        want_n, want_v = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        if not (want_n or want_v):
+            return None, None, None, None
+        g = grad.detach().to(torch.float32).contiguous()
+        grad_n = torch.empty((ctx.bs, ctx.nv, 3), dtype=torch.float32, device=g.device) if want_n else None
+        grad_v = torch.empty((ctx.bs, ctx.nv, 3), dtype=torch.float32, device=g.device) if want_v else None
+        ptr = lambda t: None if t is None else t.data_ptr()
+        with torch.cuda.device(g.device):
+            stream = ctypes.c_void_p(torch.cuda.current_stream(g.device).cuda_stream)
+            _lib.check(lib.nr_b200_corner_shading_backward(faces_i32.data_ptr(), g.data_ptr(), ctx.bs, ctx.nv,
+                                                           faces_i32.shape[1], ctx.flags, ptr(grad_n), ptr(grad_v), stream))
+        return grad_n, grad_v, None, None
+
+
+def corner_shading(vertex_normals, vertices, faces, fill_back=False):
+    """Per-corner shading normal and position [B,F,3,6] for rasterize(..., corner_shading=...) (Phong shading): corner k of
+    face f holds (n, v) of vertex faces[f,k], n from `vertex_normals` [B,Nv,3] and v from `vertices` [B,Nv,3] (the positions
+    in the frame of the eye of F.phong_params).  `faces` [F,3] / [1|B,F,3] is the index set the rasterizer receives; with
+    fill_back=True faces [F/2, F) are the reversed copies and get -n.  An index outside [0, Nv) gives zeros.  One CUDA
+    kernel pair for CUDA float32 tensors, the torch formulation otherwise; both inputs receive gradients."""
+    assert vertex_normals.dim() == 3 and vertex_normals.shape[2] == 3
+    assert tuple(vertices.shape) == tuple(vertex_normals.shape)
+    nf = faces.shape[-2]
+    if fill_back and nf % 2:
+        raise ValueError("fill_back needs an even number of faces (front faces, then their reversed copies)")
+    if not (_fused_camera_ok(vertex_normals) and _fused_camera_ok(vertices) and faces.is_cuda):
+        return _corner_shading_torch(vertex_normals, vertices, faces, fill_back)
+    from . import _lib
+    faces_i32, shared = _index_set(faces, vertex_normals.shape[0])
+    flags = (_lib.NR_INDICES_SHARED if shared else 0) | (_lib.NR_TEX_FILL_BACK if fill_back else 0)
+    return _CornerShading.apply(vertex_normals, vertices, faces_i32, flags)
+
+
+def phong_params(intensity_ambient=0.5, intensity_directional=0.5, intensity_specular=0.2, color_ambient=(1, 1, 1),
+                 color_directional=(1, 1, 1), color_specular=(1, 1, 1), direction=(0, 1, 0), shininess=64.0, eye=(0, 0, 0),
+                 device=None):
+    """Phong parameters [1|B,16] for rasterize(..., shading_params=...): {ambient intensity * colour (3), directional
+    intensity * colour (3), light direction (3, towards the light, not normalised), specular intensity * colour (3),
+    shininess, eye position (3)}.  Built with torch ops, so tensor-valued arguments (intensities and shininess scalar or
+    [B], colours, direction and eye [3] or [B,3]) receive gradients.  `device`: where plain numbers go (default: the device
+    of the first tensor argument, else the CPU)."""
+    args = (intensity_ambient, intensity_directional, intensity_specular, color_ambient, color_directional, color_specular,
+            direction, shininess, eye)
+    if device is None:
+        device = next((a.device for a in args if isinstance(a, torch.Tensor)), torch.device('cpu'))
+    key = None
+    if _is_plain(*args):  # plain numbers: one cached device tensor per value (no host copy per call, CUDA-graph safe)
+        import numpy as np
+        key = ("phong",) + tuple(tuple(np.asarray(a, dtype=np.float64).reshape(-1).tolist()) for a in args) + (str(device),)
+        if key in _CAMERA_CACHE:
+            return _CAMERA_CACHE[key]
+
+    def as_t(x, cols):
+        t = x.to(device=device, dtype=torch.float32) if isinstance(x, torch.Tensor) else \
+            torch.tensor(x, dtype=torch.float32, device=device)
+        return t.reshape(-1, cols) if t.dim() <= 1 else t
+
+    A = as_t(intensity_ambient, 1) * as_t(color_ambient, 3)
+    D = as_t(intensity_directional, 1) * as_t(color_directional, 3)
+    K = as_t(intensity_specular, 1) * as_t(color_specular, 3)
+    parts = [A, D, as_t(direction, 3), K, as_t(shininess, 1), as_t(eye, 3)]
+    n = max(p.shape[0] for p in parts)
+    if any(p.shape[0] not in (1, n) for p in parts):
+        raise ValueError("Phong parameters must hold one entry or one per batch item")
+    out = torch.cat([p.expand(n, -1) for p in parts], dim=1)
+    return out if key is None else _cache_put(key, out)

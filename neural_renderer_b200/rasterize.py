@@ -61,7 +61,7 @@ def _ptr(t):
 
 
 def _check_inputs(faces, textures, return_rgb, face_light=None, textures_fill_back=False, vertices=None, face_uvs=None,
-                  corner_light=None):
+                  corner_light=None, corner_shading=None, shading_params=None):
     # rasterize.py:66-90 (chainer type_check) -> TypeError / ValueError with the same conditions
     if not isinstance(faces, torch.Tensor):
         raise TypeError("faces must be a torch.Tensor")
@@ -103,6 +103,8 @@ def _check_inputs(faces, textures, return_rgb, face_light=None, textures_fill_ba
                 or textures.shape[0] not in (1, batch_size) or textures.shape[1] != num_cubes):
             raise ValueError("textures must have shape [batch size, num faces, ts, ts, ts, 3] with ts >= 2 and match "
                              "faces, got %s" % (tuple(textures.shape),))
+    if corner_shading is not None or shading_params is not None:
+        _check_phong_inputs(corner_shading, shading_params, face_light, corner_light, return_rgb, batch_size, num_faces)
     if return_rgb and face_light is not None:
         if not isinstance(face_light, torch.Tensor) or tuple(face_light.shape) != (batch_size, num_faces, 3):
             raise ValueError("face_light must have shape [batch size, num faces, 3]")
@@ -120,6 +122,27 @@ def _check_inputs(faces, textures, return_rgb, face_light=None, textures_fill_ba
         if not corner_light.is_cuda:
             raise NotImplementedError("neural_renderer_b200 has no CPU implementation (inputs must be CUDA tensors)")
     if not faces.is_cuda or (return_rgb and not textures.is_cuda) or (return_rgb and face_uvs is not None and not face_uvs.is_cuda):
+        raise NotImplementedError("neural_renderer_b200 has no CPU implementation (inputs must be CUDA tensors)")
+
+
+def _check_phong_inputs(corner_shading, shading_params, face_light, corner_light, return_rgb, batch_size, num_faces):
+    # Phong shading: corner_shading [F,3,6] / [1|B,F,3,6] and shading_params [16] / [1|B,16], always together
+    if corner_shading is None or shading_params is None:
+        raise ValueError("corner_shading and shading_params must be given together (Phong shading)")
+    if face_light is not None or corner_light is not None:
+        raise ValueError("Phong shading (corner_shading / shading_params) is exclusive with face_light and corner_light")
+    if not return_rgb:
+        raise ValueError("Phong shading lights the RGB image: it needs return_rgb")
+    for name, t in (("corner_shading", corner_shading), ("shading_params", shading_params)):
+        if not isinstance(t, torch.Tensor) or not t.is_floating_point():
+            raise TypeError("%s must be a floating point torch.Tensor" % name)
+    cs, sp = corner_shading, shading_params
+    if not ((cs.dim() == 3 or (cs.dim() == 4 and cs.shape[0] in (1, batch_size))) and tuple(cs.shape[-3:]) == (num_faces, 3, 6)):
+        raise ValueError("corner_shading must have shape [num faces, 3, 6] or [batch size, num faces, 3, 6] (num faces counts "
+                         "fill_back copies), got %s" % (tuple(cs.shape),))
+    if not ((sp.dim() == 1 or (sp.dim() == 2 and sp.shape[0] in (1, batch_size))) and sp.shape[-1] == 16):
+        raise ValueError("shading_params must have shape [16] or [batch size, 16], got %s" % (tuple(sp.shape),))
+    if not cs.is_cuda or not sp.is_cuda:
         raise NotImplementedError("neural_renderer_b200 has no CPU implementation (inputs must be CUDA tensors)")
 
 
@@ -212,13 +235,17 @@ class _RasterizeFunction(torch.autograd.Function):
     the `Rasterize` object can look at them)."""
 
     @staticmethod
-    def forward(ctx, geom, textures, face_light, cfg, indices, face_uvs=None, corner_light=None):
+    def forward(ctx, geom, textures, face_light, cfg, indices, face_uvs=None, corner_light=None, corner_shading=None,
+                shading_params=None):
         lib = _lib.load()
         dev = geom.device
         geom_c = geom.detach().contiguous()
         tex_c = textures.detach().contiguous() if textures is not None else None
         light_c = face_light.detach().to(torch.float32).contiguous() if face_light is not None else None
         corner_c = corner_light.detach().to(torch.float32).contiguous() if corner_light is not None else None
+        # Phong shading: corner_shading [Bc,F,3,6] and params [Bp,16], Bc / Bp = 1 for one set shared by every item
+        cs_c = corner_shading.detach().to(torch.float32).contiguous() if corner_shading is not None else None
+        sp_c = shading_params.detach().to(torch.float32).contiguous() if shading_params is not None else None
         flags = cfg.flags
         if indices is not None:
             B, Nv = geom_c.shape[:2]
@@ -281,7 +308,11 @@ class _RasterizeFunction(torch.autograd.Function):
             a.face_light = _ptr(light_c)
             a.face_uvs, (a.texture_height, a.texture_width) = _ptr(uv_c), tex_hw
             a.corner_light = _ptr(corner_c)
-            _lib.check(lib.nr_b200_forward(ctypes.byref(a), _stream_ptr(dev)))
+            if cs_c is None:
+                _lib.check(lib.nr_b200_forward(ctypes.byref(a), _stream_ptr(dev)))
+            else:
+                ph = _phong_args(cs_c, sp_c)
+                _lib.check(lib.nr_b200_forward_phong(ctypes.byref(a), ctypes.byref(ph), _stream_ptr(dev)))
         ctx.cfg = cfg
         ctx.flags = flags
         ctx.ts = ts
@@ -292,10 +323,14 @@ class _RasterizeFunction(torch.autograd.Function):
         need_light_grad = light_c is not None and ctx.needs_input_grad[2]
         ctx.need_corner_grad = corner_c is not None and ctx.needs_input_grad[6]
         ctx.need_uv_grad = uv_c is not None and want_rgb and ctx.needs_input_grad[5]
+        ctx.need_cs_grad = cs_c is not None and ctx.needs_input_grad[7]
+        ctx.need_sp_grad = sp_c is not None and ctx.needs_input_grad[8]
         # interior_gradient: the backward differentiates the sampler, so it reads the textures (and face_uvs / corner_light)
         ctx.interior = cfg.interior and want_rgb and ctx.needs_input_grad[0]
-        need_tex = need_light_grad or ctx.need_uv_grad or ctx.need_corner_grad or ctx.interior
-        ctx.save_for_backward(geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c if need_tex else None, indices, uv_c, corner_c)
+        need_tex = need_light_grad or ctx.need_uv_grad or ctx.need_corner_grad or ctx.interior or ctx.need_cs_grad or \
+            ctx.need_sp_grad
+        ctx.save_for_backward(geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c if need_tex else None, indices, uv_c, corner_c,
+                              cs_c, sp_c)
         if cfg.aa:
             rgb_o, alpha_o, depth_o = out_rgb, out_alpha, out_depth
         else:
@@ -308,7 +343,7 @@ class _RasterizeFunction(torch.autograd.Function):
         lib = _lib.load()
         cfg = ctx.cfg
         flags = ctx.flags | (_lib.NR_GRAD_INTERIOR if ctx.interior else 0)
-        geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c, indices, uv_c, corner_c = ctx.saved_tensors
+        geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c, indices, uv_c, corner_c, cs_c, sp_c = ctx.saved_tensors
         dev = geom_c.device
         B, F = geom_c.shape[0], ctx.F
         want_rgb = bool(flags & _lib.NR_RETURN_RGB)
@@ -327,6 +362,9 @@ class _RasterizeFunction(torch.autograd.Function):
             grad_light = torch.empty_like(light_c) if (want_rgb and light_c is not None and ctx.needs_input_grad[2]) else None
             grad_uvs = torch.empty_like(uv_c) if ctx.need_uv_grad else None  # same layout as face_uvs: [1|B,F',3,2]
             grad_corner = torch.empty_like(corner_c) if ctx.need_corner_grad else None
+            grad_cs = torch.empty_like(cs_c) if ctx.need_cs_grad else None
+            grad_sp = torch.empty_like(sp_c) if ctx.need_sp_grad else None
+            ph = _phong_args(cs_c, sp_c, grad_cs, grad_sp) if cs_c is not None else None
             ws_bytes = lib.nr_b200_backward_workspace_bytes(B, F, cfg.S, ctx.ts, flags)
             ws = torch.empty((max(ws_bytes, 16),), dtype=torch.uint8, device=dev)
             a = _lib.BackwardArgs()
@@ -349,6 +387,8 @@ class _RasterizeFunction(torch.autograd.Function):
             hook = _TEXTURE_GRAD_HOOK if (want_rgb and g_rgb is not None) else None
 
             def call():
+                if ph is not None:  # Phong: grad_corner_shading / grad_params are filled by the texture half
+                    return lib.nr_b200_backward_phong(ctypes.byref(a), ctypes.byref(ph), _stream_ptr(dev))
                 if corner_c is None:
                     return lib.nr_b200_backward(ctypes.byref(a), _stream_ptr(dev))
                 # smooth shading: grad_corner_light is filled by the texture half
@@ -367,7 +407,16 @@ class _RasterizeFunction(torch.autograd.Function):
                 _lib.check(call())
                 if pending is not None:
                     pending.wait()
-        return grad_geom, grad_textures, grad_light, None, None, grad_uvs, grad_corner
+        return grad_geom, grad_textures, grad_light, None, None, grad_uvs, grad_corner, grad_cs, grad_sp
+
+
+def _phong_args(cs_c, sp_c, grad_cs=None, grad_sp=None):
+    ph = _lib.PhongArgs()
+    ph.struct_size = ctypes.sizeof(_lib.PhongArgs)
+    ph.shading_batch, ph.params_batch = int(cs_c.shape[0]), int(sp_c.shape[0])
+    ph.corner_shading, ph.params = _ptr(cs_c), _ptr(sp_c)
+    ph.grad_corner_shading, ph.grad_params = _ptr(grad_cs), _ptr(grad_sp)
+    return ph
 
 
 class _MipPyramid(torch.autograd.Function):
@@ -404,7 +453,10 @@ TEXTURE_FILTERS = ('bilinear', 'trilinear')
 
 def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_color, return_rgb, return_alpha,
          return_depth, face_light=None, textures_fill_back=False, vertices=None, reference_exact=None, face_uvs=None,
-         texture_filter='bilinear', corner_light=None, interior_gradient=False):
+         texture_filter='bilinear', corner_light=None, interior_gradient=False, corner_shading=None, shading_params=None):
+    if (corner_shading is not None or shading_params is not None) and interior_gradient:
+        raise ValueError("interior_gradient=True is not supported with Phong shading (corner_shading / shading_params): no "
+                         "vertex gradient flows through the interpolation of the per-pixel normal and position")
     if texture_filter not in TEXTURE_FILTERS:
         raise ValueError("texture_filter must be one of %s, got %r" % (TEXTURE_FILTERS, texture_filter))
     if texture_filter == 'trilinear' and face_uvs is None:
@@ -415,7 +467,9 @@ def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_
         raise ValueError("interior_gradient=True with per-face cubes needs every item's own depths when the batch has more "
                          "than one item: the reference-exact sampler reads the depths of item 0 for every item, so its "
                          "derivative would cross items.  Pass reference_exact=False (or set_reference_exact(False))")
-    _check_inputs(faces, textures, return_rgb, face_light, textures_fill_back, vertices, face_uvs, corner_light)
+    _check_inputs(faces, textures, return_rgb, face_light, textures_fill_back, vertices, face_uvs, corner_light,
+                  corner_shading, shading_params)
+    phong = corner_shading is not None
     indices = None
     if vertices is not None:
         geom = vertices if vertices.dtype == torch.float32 else vertices.float()
@@ -441,6 +495,15 @@ def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_
                 face_uvs = face_uvs[:1]  # an expanded shared UV set (NR_UV_SHARED)
         if textures.shape[0] == batch_size > 1 and textures.stride(0) == 0:
             textures = textures[:1]  # an expanded shared texture set: sample it in place (NR_TEX_SHARED)
+        if phong:
+            corner_shading = corner_shading.float() if corner_shading.dtype != torch.float32 else corner_shading
+            shading_params = shading_params.float() if shading_params.dtype != torch.float32 else shading_params
+            corner_shading = corner_shading[None] if corner_shading.dim() == 3 else corner_shading
+            shading_params = shading_params[None] if shading_params.dim() == 1 else shading_params
+            if corner_shading.shape[0] == batch_size > 1 and corner_shading.stride(0) == 0:
+                corner_shading = corner_shading[:1]  # an expanded shared set (Bc = 1)
+            if shading_params.shape[0] == batch_size > 1 and shading_params.stride(0) == 0:
+                shading_params = shading_params[:1]
     cfg = _make_config(image_size, anti_aliasing, near, far, eps, background_color, return_rgb, return_alpha,
                        return_depth, geom.device, batch_size, reference_exact)
     if return_rgb and textures_fill_back:
@@ -455,7 +518,8 @@ def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_
         cfg.flags |= _lib.NR_TEX_MIPMAP
         textures = _MipPyramid.apply(textures)
     return _RasterizeFunction.apply(geom, textures if return_rgb else None, face_light if return_rgb else None, cfg,
-                                    indices, face_uvs, corner_light)
+                                    indices, face_uvs, corner_light, corner_shading if return_rgb else None,
+                                    shading_params if return_rgb else None)
 
 
 def rasterize_rgbad(
@@ -479,6 +543,8 @@ def rasterize_rgbad(
         texture_filter='bilinear',
         corner_light=None,
         interior_gradient=False,
+        corner_shading=None,
+        shading_params=None,
 ):
     """Generate RGB, alpha channel, and depth images from faces and textures (for RGB).  rasterize.py:900-977.
 
@@ -524,11 +590,20 @@ def rasterize_rgbad(
                               (include/nr_b200.h, NR_GRAD_INTERIOR), with the cell, level of detail and clamps held fixed.
                               What photometric alignment of a textured mesh needs.  Per-face cubes with a batch > 1 need
                               reference_exact=False.
+      corner_shading [F,3,6] / [1|B,F,3,6], shading_params [16] / [1|B,16]   Phong shading, always together: per face
+                              corner (the order of `faces`; F counts fill_back copies, give them the negated normal) a
+                              shading normal and a position, interpolated per pixel with the perspective-correct weights;
+                              shading_params = {ambient[3], directional[3], direction[3], specular[3], shininess, eye[3]}
+                              (F.corner_shading / F.phong_params build both).  rgb = (ambient + directional relu(n . d))
+                              * sample + specular * q^shininess, the highlight of the reflected light towards the eye
+                              (include/nr_b200.h).  Exclusive with face_light / corner_light and with
+                              interior_gradient; both receive gradients (a batch of 1 gets the sum over the items).
     `textures` with batch size 1 (or an expanded stride-0 batch) while the geometry batch is larger = one texture set
     shared by every item (a mesh seen from B viewpoints, mesh.py:29-34); its gradient is the sum over the items."""
     rgb, alpha, depth, _, _ = _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_color,
                                    return_rgb, return_alpha, return_depth, face_light, textures_fill_back, vertices,
-                                   reference_exact, face_uvs, texture_filter, corner_light, interior_gradient)
+                                   reference_exact, face_uvs, texture_filter, corner_light, interior_gradient,
+                                   corner_shading, shading_params)
     return {
         'rgb': rgb if return_rgb else None,
         'alpha': alpha if return_alpha else None,
@@ -554,6 +629,8 @@ def rasterize(
         texture_filter='bilinear',
         corner_light=None,
         interior_gradient=False,
+        corner_shading=None,
+        shading_params=None,
 ):
     """RGB images [B,3,H,W] from faces and textures.  rasterize.py:980-1008 (keyword-only extras: rasterize_rgbad; in
     texture-image mode both the image and face_uvs receive gradients)."""
@@ -561,7 +638,7 @@ def rasterize(
         faces, textures, image_size, anti_aliasing, near, far, eps, background_color, True, False, False,
         face_light=face_light, textures_fill_back=textures_fill_back, vertices=vertices,
         reference_exact=reference_exact, face_uvs=face_uvs, texture_filter=texture_filter, corner_light=corner_light,
-        interior_gradient=interior_gradient)['rgb']
+        interior_gradient=interior_gradient, corner_shading=corner_shading, shading_params=shading_params)['rgb']
 
 
 def rasterize_silhouettes(

@@ -32,6 +32,10 @@ class Renderer(object):
         self.light_color_ambient = [1, 1, 1]  # white
         self.light_color_directional = [1, 1, 1]  # white
         self.light_direction = [0, 1, 0]  # up-to-down
+        # specular highlight of shading='phong' (flat and smooth ignore these)
+        self.light_intensity_specular = 0.2
+        self.light_color_specular = [1, 1, 1]
+        self.light_shininess = 64.0
 
         # rasterization
         self.rasterizer_eps = 1e-3
@@ -46,8 +50,9 @@ class Renderer(object):
         # image (minified images neither alias nor leave texels without gradient); per-face cubes ignore it
         self.texture_filter = 'bilinear'
         # 'flat': the reference's one light factor per face; 'smooth': the light evaluated at every vertex from its
-        # area-weighted normal and interpolated across the face (Gouraud), with vertex gradients through the normals.
-        # Silhouettes and depth ignore it
+        # area-weighted normal and interpolated across the face (Gouraud), with vertex gradients through the normals;
+        # 'phong': normal and position interpolated to every pixel, ambient + diffuse + a specular highlight towards `eye`
+        # (also with perspective=False: the viewer is a point at `eye`).  Silhouettes and depth ignore it
         self.shading = 'flat'
         # True: render() also sends the vertices the derivative of the colour inside each face (texture moving under the
         # face, smooth light) -- photometric alignment; per-face cubes with a batch > 1 need reference_exact=False
@@ -100,13 +105,15 @@ class Renderer(object):
         the image and a `face_uvs` with requires_grad receive gradients (fused: the fill_back copies' UV gradient is
         folded into the original faces in the kernel; op by op: through the cat / flip of the doubled corners)."""
         texture_filter = self.texture_filter if face_uvs is not None else 'bilinear'
-        if self.shading not in ('flat', 'smooth'):
-            raise ValueError("shading must be 'flat' or 'smooth', got %r" % (self.shading,))
+        if self.shading not in ('flat', 'smooth', 'phong'):
+            raise ValueError("shading must be 'flat', 'smooth' or 'phong', got %r" % (self.shading,))
         fused = (self.fused and self._fusable(vertices, faces) and textures.is_cuda and textures.dtype == torch.float32)
         light_args = (self.light_intensity_ambient, self.light_intensity_directional, self.light_color_ambient,
                       self.light_color_directional, self.light_direction)
         if self.shading == 'smooth':
             return self._render_smooth(vertices, faces, textures, face_uvs, texture_filter, fused, light_args)
+        if self.shading == 'phong':
+            return self._render_phong(vertices, faces, textures, face_uvs, texture_filter, fused)
         if fused:
             # lighting.py:29-52, renderer.py:78-80 and vertices_to_faces (renderer.py:103) folded into the rasterizer:
             # neither `textures * light`, nor the doubled texture tensor, nor faces [B,F,3,3] exist; pixel values are
@@ -191,3 +198,38 @@ class Renderer(object):
             faces, textures, self.image_size, self.anti_aliasing, self.near, self.far, self.rasterizer_eps,
             self.background_color, reference_exact=self.reference_exact, face_uvs=face_uvs,
             texture_filter=texture_filter, corner_light=corner, interior_gradient=self.interior_gradient)
+
+    def _render_phong(self, vertices, faces, textures, face_uvs, texture_filter, fused):
+        # vertex normals of the original faces, then per corner of the drawn faces (copies: reversed normal) the normal and
+        # the world-space position; the light, the specular highlight and the eye (self.eye, world space) are per pixel
+        if self.interior_gradient:
+            raise ValueError("shading='phong' does not support interior_gradient=True: no vertex gradient flows through the "
+                             "per-pixel interpolation of the Phong normal and position")
+        params = F.phong_params(self.light_intensity_ambient, self.light_intensity_directional, self.light_intensity_specular,
+                                self.light_color_ambient, self.light_color_directional, self.light_color_specular,
+                                self.light_direction, self.light_shininess, self.eye, device=vertices.device)
+        if fused:
+            indices = self._indices(faces)
+            # one mesh seen from B viewpoints (an expanded, stride-0 vertex batch and a shared index set): one corner set
+            shared = vertices.shape[0] > 1 and vertices.stride(0) == 0 and indices.shape[0] == 1
+            v1, f1 = (vertices[:1], faces[:1]) if shared else (vertices, faces)
+            cs = F.corner_shading(F.vertex_normals(v1, f1), v1, indices, fill_back=self.fill_back)
+            return rasterize(
+                indices, textures, self.image_size, self.anti_aliasing, self.near, self.far, self.rasterizer_eps,
+                self.background_color, textures_fill_back=self.fill_back, vertices=self._transform(vertices),
+                reference_exact=self.reference_exact, face_uvs=face_uvs, texture_filter=texture_filter,
+                corner_shading=cs, shading_params=params)
+        # op by op: torch normals and corners, materialised faces, doubled textures / UV corners for fill_back
+        normals = F._vertex_normals_torch(vertices, faces)
+        if self.fill_back:
+            faces = torch.cat((faces, faces.flip(2)), dim=1)
+            if face_uvs is not None:
+                face_uvs = torch.cat((face_uvs, face_uvs.flip(-2)), dim=-3)
+            else:
+                textures = torch.cat((textures, textures.permute(0, 1, 4, 3, 2, 5)), dim=1)
+        cs = F._corner_shading_torch(normals, vertices, faces, self.fill_back)
+        faces = F.vertices_to_faces(self._transform(vertices), faces)
+        return rasterize(
+            faces, textures, self.image_size, self.anti_aliasing, self.near, self.far, self.rasterizer_eps,
+            self.background_color, reference_exact=self.reference_exact, face_uvs=face_uvs,
+            texture_filter=texture_filter, corner_shading=cs, shading_params=params)
