@@ -309,6 +309,38 @@ typedef struct nr_b200_phong_args {
     float *grad_params;            /* backward: [Bp,16] or NULL */
 } nr_b200_phong_args;
 
+/* Light sets for Phong shading, additive to ABI 4: one struct (nr_b200_lights_args) and two entry points
+ * (nr_b200_forward_lights / nr_b200_backward_lights).  NL extra lights, 0 <= NL <= 8, on top of the light that `params`
+ * carries ("light 0"): NL = 0 is nr_b200_*_phong exactly (the same kernels), and params D = K = 0 leaves only the set.
+ *   lights [Bl,NL,12] (device), Bl in {1, B} (1 = one set for every item, its gradient the sum over the items), per light j:
+ *     0-2 D_j diffuse intensity * colour,  3-5 K_j specular intensity * colour,
+ *     6-8 x_j: the direction towards the light (directional, not normalised) or the light's position (point), in the frame
+ *         of P and e,  9 f_j falloff (point lights only),  10 kind: > 0.5 = point light, else directional,  11 reserved.
+ *   Covered raster pixel: nh, p, vh, L_c and h of the Phong expression above, then for j = 0 .. NL-1 in order
+ *     directional: c_j = nh . x_j,   lh_j = x_j / (|x_j| + 1e-5),   a_j = 1
+ *     point:       u_j = x_j - p,  r_j = |u_j|,  lh_j = u_j / (r_j + 1e-5),  c_j = nh . lh_j,  a_j = 1 / (1 + f_j r_j^2)
+ *     L_c = fma(D_jc, a_j max(c_j, 0), L_c)
+ *     q_j = max((2 (nh . lh_j) nh - lh_j) . vh, 0),   h_j = [c_j > 0] [q_j > 0] q_j^sigma   (sigma of params)
+ *   and rgb_c = fma(K_c, h, L_c s_c) (L_c now every light's diffuse term), then rgb_c = fma(K_jc, a_j h_j, rgb_c) for
+ *   j = 0 .. NL-1 in order.  So a directional record with params D = K = 0 gives nr_b200_forward_phong with that light in
+ *   params bit for bit.  Held to a float64 evaluation, not bit-pinned otherwise.
+ *   Backward (nr_b200_backward_lights), texture half: grad_textures / grad_face_uvs with the pixel's full L_c;
+ *   grad_corner_shading also through lh_j and a_j of the point lights (they depend on p); grad_params as for Phong;
+ *   grad_lights [Bl,NL,12] the exact derivative in slots 0-9, 0 in slots 10-11.  Masks and max take subgradient 0.  Each
+ *   gradient output may be NULL and is zero-filled first unless NR_GRAD_ACCUMULATE.  The faces half is unchanged;
+ *   NR_GRAD_INTERIOR is NR_ERR_UNSUPPORTED, as for Phong.
+ *   Host rejections (NR_ERR_INVALID_ARG, before any launch), besides those of nr_b200_*_phong: a struct_size mismatch,
+ *   NL < 0 or NL > 8, lights NULL with NL > 0, Bl not in {1, B}, and grad_lights without `textures`.  A NULL `lights`
+ *   struct is allowed: the call is then nr_b200_*_phong. */
+typedef struct nr_b200_lights_args {
+    uint32_t struct_size;  /* sizeof(nr_b200_lights_args) */
+    int32_t lights_batch;  /* Bl: 1 or B */
+    int32_t num_lights;    /* NL: 0 .. 8 */
+    int32_t _pad0;
+    const float *lights;   /* [Bl,NL,12] */
+    float *grad_lights;    /* backward: [Bl,NL,12] or NULL */
+} nr_b200_lights_args;
+
 /* Attribute interpolation, additive to ABI 4: two flag bits, one struct and two entry points.  Renders C >= 1 arbitrary
  * channels (normals, positions, UVs, labels, features) through the maps an ordinary forward call wrote (face_index_map,
  * weight_map; a silhouette-only forward suffices), with gradients into the attributes and, through the perspective
@@ -393,6 +425,12 @@ NR_B200_API int nr_b200_backward_corner_light(const nr_b200_backward_args *args,
  * texture half. */
 NR_B200_API int nr_b200_forward_phong(const nr_b200_forward_args *args, const nr_b200_phong_args *phong, void *cuda_stream);
 NR_B200_API int nr_b200_backward_phong(const nr_b200_backward_args *args, const nr_b200_phong_args *phong, void *cuda_stream);
+/* Phong shading with a light set (nr_b200_lights_args above): the Phong calls with `lights` added; lights NULL or NL = 0
+ * runs exactly nr_b200_forward_phong / nr_b200_backward_phong.  grad_lights is filled by the texture half. */
+NR_B200_API int nr_b200_forward_lights(const nr_b200_forward_args *args, const nr_b200_phong_args *phong,
+                                       const nr_b200_lights_args *lights, void *cuda_stream);
+NR_B200_API int nr_b200_backward_lights(const nr_b200_backward_args *args, const nr_b200_phong_args *phong,
+                                        const nr_b200_lights_args *lights, void *cuda_stream);
 /* Attribute interpolation (nr_b200_interpolate_args above): the image `out`, and its backward into grad_attributes and the
  * interior vertex gradient.  One kernel launch each (plus the zero-fill of the backward). */
 NR_B200_API int nr_b200_interpolate(const nr_b200_interpolate_args *args, void *cuda_stream);

@@ -48,6 +48,8 @@ EXPORTED_SYMBOLS = (
     "nr_b200_backward_corner_light",
     "nr_b200_forward_phong",
     "nr_b200_backward_phong",
+    "nr_b200_forward_lights",
+    "nr_b200_backward_lights",
     "nr_b200_interpolate",
     "nr_b200_interpolate_backward",
     "nr_b200_vertices_to_faces",
@@ -122,6 +124,14 @@ class PhongArgs(ctypes.Structure):
     ]
 
 
+class LightsArgs(ctypes.Structure):
+    _fields_ = [
+        ("struct_size", ctypes.c_uint32), ("lights_batch", ctypes.c_int32),
+        ("num_lights", ctypes.c_int32), ("_pad0", ctypes.c_int32),
+        ("lights", ctypes.c_void_p), ("grad_lights", ctypes.c_void_p),
+    ]
+
+
 class InterpolateArgs(ctypes.Structure):
     _fields_ = [
         ("struct_size", ctypes.c_uint32), ("flags", ctypes.c_uint32),
@@ -171,6 +181,12 @@ def load():
     lib.nr_b200_forward_phong.argtypes = [ctypes.POINTER(ForwardArgs), ctypes.POINTER(PhongArgs), ctypes.c_void_p]
     lib.nr_b200_backward_phong.restype = ctypes.c_int
     lib.nr_b200_backward_phong.argtypes = [ctypes.POINTER(BackwardArgs), ctypes.POINTER(PhongArgs), ctypes.c_void_p]
+    lib.nr_b200_forward_lights.restype = ctypes.c_int
+    lib.nr_b200_forward_lights.argtypes = [ctypes.POINTER(ForwardArgs), ctypes.POINTER(PhongArgs), ctypes.POINTER(LightsArgs),
+                                           ctypes.c_void_p]
+    lib.nr_b200_backward_lights.restype = ctypes.c_int
+    lib.nr_b200_backward_lights.argtypes = [ctypes.POINTER(BackwardArgs), ctypes.POINTER(PhongArgs),
+                                            ctypes.POINTER(LightsArgs), ctypes.c_void_p]
     for name in ("nr_b200_interpolate", "nr_b200_interpolate_backward"):
         fn = getattr(lib, name)
         fn.restype = ctypes.c_int

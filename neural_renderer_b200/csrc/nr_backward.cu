@@ -153,6 +153,10 @@ struct BwdParams {
     const float* phong_prm;
     size_t cs_bstride;   // faces per item in phong_cs (0 with Bc = 1)
     size_t prm_bstride;  // floats per item in phong_prm (0 with Bp = 1)
+    // light set (appended likewise, the kLight == 4 variants): lights [Bl,NL,12]
+    const float* lts;
+    size_t lt_bstride;   // floats per item in lts (0 with Bl = 1)
+    int NL;
 };
 
 //@phase helpers: rcp / vector RED / load_grad (inlined)
@@ -977,14 +981,14 @@ __device__ __forceinline__ void light_grad_scatter(float (&gl)[N], int fn, int l
 // that sit next to each other with the same (cube, cell) therefore add their 8 x 3 contributions together with
 // kTgCombine shuffle steps first (runs of up to 2^kTgCombine lanes collapse into one lane's reductions).
 //
-// kLight: 0 = face_light or unlit, 2 = corner_light, 3 = Phong.
+// kLight: 0 = face_light or unlit, 2 = corner_light, 3 = Phong, 4 = Phong with a light set.
 // kCorner (corner_light): the pixel's light L_c = the corner factors interpolated with its perspective weights l_k (own
 // vertex depths) takes face_light's place, and d loss / d corner_light = l_k g_c s_c goes through the same run reduction.
 // kPhong: L_c = the diffuse part of the Phong expression at the pixel (nr::phong_diffuse) takes face_light's place; the
-// Phong gradients themselves come from k_phong_grad (nr_phong.cu).
+// Phong gradients themselves come from k_phong_grad (nr_phong.cu).  Mode 4 adds the set's diffuse terms to L_c.
 template <int kTgCombine, int kLight>
 __global__ void __launch_bounds__(256, kTgCombine ? (kLight >= 2 ? NR_TGC_MIN_CTAS : 4) : NR_TG_MIN_CTAS) k_texture_grad(const __grid_constant__ BwdParams p) {
-    constexpr bool kCorner = kLight == 2, kPhong = kLight == 3;
+    constexpr bool kCorner = kLight == 2, kPhong = kLight >= 3;
     const int S = p.S;
     const size_t plane = (size_t)S * S;
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;  // pixel within the image (image orientation)
@@ -1041,7 +1045,14 @@ __global__ void __launch_bounds__(256, kTgCombine ? (kLight >= 2 ? NR_TGC_MIN_CT
                 nr::corner_light_at(p.corner_light + ((size_t)b * p.F + fn) * 9, lam, L);
             } else {
                 nr::PhongEval E;
-                nr::phong_diffuse(p.phong_cs + ((size_t)b * p.cs_bstride + fn) * 18, lam, p.phong_prm + (size_t)b * p.prm_bstride, E);
+                const float* cs = p.phong_cs + ((size_t)b * p.cs_bstride + fn) * 18;
+                const float* prm = p.phong_prm + (size_t)b * p.prm_bstride;
+                if constexpr (kLight == 4) {
+                    float pos[3];
+                    nr::phong_lights_diffuse(cs, lam, prm, p.lts + (size_t)b * p.lt_bstride, p.NL, E, pos);
+                } else {
+                    nr::phong_diffuse(cs, lam, prm, E);
+                }
                 L[0] = E.L[0]; L[1] = E.L[1]; L[2] = E.L[2];
             }
         }
@@ -1181,12 +1192,12 @@ __device__ __forceinline__ void red_add_6(float* t, const float v[6]) {
 // weight) goes to UV corner k as l_k (gu, gv), corners reversed back for a fill_back copy.  Runs of neighbouring lanes
 // that show the same face sum their 6 floats with shuffles and the run's first lane adds them.
 //
-// kLight: 0 = face_light or unlit, 2 = corner_light, 3 = Phong.
+// kLight: 0 = face_light or unlit, 2 = corner_light, 3 = Phong, 4 = Phong with a light set.
 // kCorner (corner_light): as in k_texture_grad, the interpolated light L_c replaces face_light (also in the face_uvs
 // gradient) and the 9-float corner-light gradient goes through the run reduction.  kPhong: likewise with the Phong L_c.
 template <int kTgCombine, bool kMip, bool kUvGrad, int kLight>
 __device__ __forceinline__ void image_grad(const BwdParams& p) {
-    constexpr bool kCorner = kLight == 2, kPhong = kLight == 3;
+    constexpr bool kCorner = kLight == 2, kPhong = kLight >= 3;
     constexpr int kPairs = kMip ? 4 : 2;
     const int S = p.S;
     const size_t plane = (size_t)S * S;
@@ -1257,7 +1268,14 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
         } else if constexpr (kPhong) {
             nr::perspective_weights(w, zp, z0, z1, z2, lam);
             nr::PhongEval E;
-            nr::phong_diffuse(p.phong_cs + ((size_t)b * p.cs_bstride + fn) * 18, lam, p.phong_prm + (size_t)b * p.prm_bstride, E);
+            const float* cs = p.phong_cs + ((size_t)b * p.cs_bstride + fn) * 18;
+            const float* prm = p.phong_prm + (size_t)b * p.prm_bstride;
+            if constexpr (kLight == 4) {
+                float pos[3];
+                nr::phong_lights_diffuse(cs, lam, prm, p.lts + (size_t)b * p.lt_bstride, p.NL, E, pos);
+            } else {
+                nr::phong_diffuse(cs, lam, prm, E);
+            }
             L[0] = E.L[0]; L[1] = E.L[1]; L[2] = E.L[2];
         }
         const uint32_t img_off = (uint32_t)b * p.img_bstride;
@@ -1594,9 +1612,10 @@ extern "C" size_t nr_b200_backward_workspace_bytes(int32_t B, int32_t F, int32_t
     return bin_layout(B, F, S, strip_rec_bytes(S, both)).total;
 }
 
-// nr_b200_backward (corner_light, phong NULL), nr_b200_backward_corner_light (smooth shading) and nr_b200_backward_phong
+// nr_b200_backward (corner_light, phong, lights NULL), nr_b200_backward_corner_light (smooth shading), nr_b200_backward_phong
+// (lights NULL) and nr_b200_backward_lights
 static int backward_impl(const nr_b200_backward_args* args, const float* corner_light, float* grad_corner_light,
-                         const nr_b200_phong_args* phong, void* cuda_stream) {
+                         const nr_b200_phong_args* phong, const nr_b200_lights_args* lights, void* cuda_stream) {
     nr_internal::launch_count() = 0;
     // Two layouts: the full struct, and the ABI-4 struct from before grad_face_uvs (which then reads as NULL).  Only the
     // caller's struct_size bytes are read.
@@ -1638,8 +1657,11 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
     if (smooth && (!rgb || a->face_light)) return NR_ERR_INVALID_ARG;
     if (grad_corner_light && (!smooth || !a->textures)) return NR_ERR_INVALID_ARG;
     // Phong: only for RGB and instead of face_light / corner_light; its gradients read the (unlit) textures
-    const bool phong_grads = phong && (phong->grad_corner_shading || phong->grad_params);
     if (phong && (!rgb || a->face_light || smooth || !nr_internal::phong_args_ok(phong, B))) return NR_ERR_INVALID_ARG;
+    // light set: grad_lights needs s as well
+    if (lights && (!nr_internal::lights_args_ok(lights, B) || (lights->grad_lights && !a->textures))) return NR_ERR_INVALID_ARG;
+    if (lights && lights->num_lights == 0) lights = nullptr;  // the Phong call exactly
+    const bool phong_grads = phong && (phong->grad_corner_shading || phong->grad_params || (lights && lights->grad_lights));
     if (phong_grads && !a->textures) return NR_ERR_INVALID_ARG;
     // NR_GRAD_INTERIOR: the sampler's derivative reads the textures; the cubes of NR_TEX_Z_BATCH0 sample item b with the
     // depths of item 0, so their derivative would cross items (B = 1 is the plain sampler)
@@ -1698,6 +1720,9 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
         if (part_tex && phong && phong->grad_params &&
             cudaMemsetAsync(phong->grad_params, 0, (size_t)phong->params_batch * 16 * sizeof(float), stream) != cudaSuccess)
             return NR_ERR_CUDA;
+        if (part_tex && lights && lights->grad_lights &&
+            cudaMemsetAsync(lights->grad_lights, 0, (size_t)lights->lights_batch * lights->num_lights * 12 * sizeof(float), stream) != cudaSuccess)
+            return NR_ERR_CUDA;
         nr_internal::prof_end(stream);
     }
 
@@ -1729,13 +1754,19 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
         p.cs_bstride = phong->shading_batch == 1 ? 0 : (size_t)F;
         p.prm_bstride = phong->params_batch == 1 ? 0 : 16;
     }
-    const int light = phong ? 3 : (smooth ? 2 : 0);
+    if (lights) {
+        p.lts = lights->lights; p.NL = lights->num_lights;
+        p.lt_bstride = lights->lights_batch == 1 ? 0 : (size_t)lights->num_lights * 12;
+    }
+    const int light = lights ? 4 : (phong ? 3 : (smooth ? 2 : 0));
 
     const dim3 pgrid((unsigned)(((size_t)S * S + 255) / 256), B);
     auto launch_texture_grad = [&]() {
         if (mip) {
             nr_internal::LaunchScope ls("k_image_grad", stream);
-            if (light == 3 && uv_grad) k_image_grad_mip<NR_TG_COMBINE, true, 3><<<pgrid, 256, 0, stream>>>(p);
+            if (light == 4 && uv_grad) k_image_grad_mip<NR_TG_COMBINE, true, 4><<<pgrid, 256, 0, stream>>>(p);
+            else if (light == 4) k_image_grad_mip<NR_TG_COMBINE, false, 4><<<pgrid, 256, 0, stream>>>(p);
+            else if (light == 3 && uv_grad) k_image_grad_mip<NR_TG_COMBINE, true, 3><<<pgrid, 256, 0, stream>>>(p);
             else if (light == 3) k_image_grad_mip<NR_TG_COMBINE, false, 3><<<pgrid, 256, 0, stream>>>(p);
             else if (smooth && uv_grad) k_image_grad_mip<NR_TG_COMBINE, true, 2><<<pgrid, 256, 0, stream>>>(p);
             else if (smooth) k_image_grad_mip<NR_TG_COMBINE, false, 2><<<pgrid, 256, 0, stream>>>(p);
@@ -1745,7 +1776,9 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
         }
         if (uv) {
             nr_internal::LaunchScope ls("k_image_grad", stream);
-            if (light == 3 && uv_grad) k_image_grad<NR_TG_COMBINE, true, 3><<<pgrid, 256, 0, stream>>>(p);
+            if (light == 4 && uv_grad) k_image_grad<NR_TG_COMBINE, true, 4><<<pgrid, 256, 0, stream>>>(p);
+            else if (light == 4) k_image_grad<NR_TG_COMBINE, false, 4><<<pgrid, 256, 0, stream>>>(p);
+            else if (light == 3 && uv_grad) k_image_grad<NR_TG_COMBINE, true, 3><<<pgrid, 256, 0, stream>>>(p);
             else if (light == 3) k_image_grad<NR_TG_COMBINE, false, 3><<<pgrid, 256, 0, stream>>>(p);
             else if (smooth && uv_grad) k_image_grad<NR_TG_COMBINE, true, 2><<<pgrid, 256, 0, stream>>>(p);
             else if (smooth) k_image_grad<NR_TG_COMBINE, false, 2><<<pgrid, 256, 0, stream>>>(p);
@@ -1754,7 +1787,8 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
             return;
         }
         nr_internal::LaunchScope ls("k_texture_grad", stream);
-        if (light == 3) k_texture_grad<NR_TG_COMBINE, 3><<<pgrid, 256, 0, stream>>>(p);
+        if (light == 4) k_texture_grad<NR_TG_COMBINE, 4><<<pgrid, 256, 0, stream>>>(p);
+        else if (light == 3) k_texture_grad<NR_TG_COMBINE, 3><<<pgrid, 256, 0, stream>>>(p);
         else if (smooth) k_texture_grad<NR_TG_COMBINE, 2><<<pgrid, 256, 0, stream>>>(p);
         else k_texture_grad<NR_TG_COMBINE, 0><<<pgrid, 256, 0, stream>>>(p);
     };
@@ -1762,7 +1796,7 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
     auto launch_phong_grad = [&]() {
         if (!phong_grads) return;
         nr_internal::PhongGradLaunch pl{};
-        pl.args = a; pl.src = src; pl.phong = phong;
+        pl.args = a; pl.src = src; pl.phong = phong; pl.lights = lights;
         pl.tex_bstride = (flags & NR_TEX_SHARED) ? 0 : (uv ? img_floats : ncubes * (size_t)ts * ts * ts * 3);
         pl.uv_bstride = p.uv_bstride;
         pl.tex_cmp = p.tex_cmp; pl.tex_val = p.tex_val;
@@ -1871,7 +1905,7 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
 }
 
 extern "C" int nr_b200_backward(const nr_b200_backward_args* args, void* cuda_stream) {
-    return backward_impl(args, nullptr, nullptr, nullptr, cuda_stream);
+    return backward_impl(args, nullptr, nullptr, nullptr, nullptr, cuda_stream);
 }
 
 extern "C" int nr_b200_backward_corner_light(const nr_b200_backward_args* args, const float* corner_light,
@@ -1880,7 +1914,7 @@ extern "C" int nr_b200_backward_corner_light(const nr_b200_backward_args* args, 
         nr_internal::launch_count() = 0;
         return NR_ERR_INVALID_ARG;
     }
-    return backward_impl(args, corner_light, grad_corner_light, nullptr, cuda_stream);
+    return backward_impl(args, corner_light, grad_corner_light, nullptr, nullptr, cuda_stream);
 }
 
 extern "C" int nr_b200_backward_phong(const nr_b200_backward_args* args, const nr_b200_phong_args* phong, void* cuda_stream) {
@@ -1888,5 +1922,14 @@ extern "C" int nr_b200_backward_phong(const nr_b200_backward_args* args, const n
         nr_internal::launch_count() = 0;
         return NR_ERR_INVALID_ARG;
     }
-    return backward_impl(args, nullptr, nullptr, phong, cuda_stream);
+    return backward_impl(args, nullptr, nullptr, phong, nullptr, cuda_stream);
+}
+
+extern "C" int nr_b200_backward_lights(const nr_b200_backward_args* args, const nr_b200_phong_args* phong,
+                                       const nr_b200_lights_args* lights, void* cuda_stream) {
+    if (!phong) {
+        nr_internal::launch_count() = 0;
+        return NR_ERR_INVALID_ARG;
+    }
+    return backward_impl(args, nullptr, nullptr, phong, lights, cuda_stream);
 }

@@ -75,6 +75,9 @@ constexpr int kOwnTable = 256;         // rows / fragments per pass whose owner 
 #ifndef NR_RESOLVE_PHONG_MIN_CTAS
 #define NR_RESOLVE_PHONG_MIN_CTAS 4      // Phong-shaded (kLight == 3) variants, every sampler (DESIGN.md section 4g)
 #endif
+#ifndef NR_RESOLVE_LIGHTS_MIN_CTAS
+#define NR_RESOLVE_LIGHTS_MIN_CTAS 4     // Phong with a light set (kLight == 4), every sampler (DESIGN.md section 4h)
+#endif
 constexpr int kResolveTileW = 32, kResolveTileH = 8;  // API pixels per k_resolve CTA (256 threads, 8 x 4 per warp)
 constexpr uint32_t kStageBytes = 32 * 1024;  // shared memory of a k_resolve CTA for staged texture cubes
 
@@ -118,6 +121,10 @@ struct FwdParams {
     const float* phong_prm;
     size_t cs_bstride;   // faces per item in phong_cs (0 with Bc = 1)
     size_t prm_bstride;  // floats per item in phong_prm (0 with Bp = 1)
+    // light set (appended likewise, the kLight == 4 variants): lights [Bl,NL,12]
+    const float* lts;
+    size_t lt_bstride;   // floats per item in lts (0 with Bl = 1)
+    int NL;
 };
 
 // rasterize.py:291-292  xp = (2 * xi + 1 - is) / is evaluated in double and rounded to float.  Both operands are
@@ -462,7 +469,8 @@ __device__ __forceinline__ int face_cube(const FwdParams& p, int fn, bool& rev) 
 // one pixel, every texel straight from global memory (anti-aliased quads, texture sizes the bulk copy cannot stage);
 // kUV: bilinear sample of the texture image at the pixel's perspective-correct UV instead of the ts^3 cube; kMip:
 // trilinear sample of its mip pyramid at the pixel's level of detail.  kLight: 0 = unlit, 1 = face_light multiplies every
-// texel, 2 = corner_light interpolated to the pixel multiplies the unlit sample, 3 = Phong shading of the unlit sample
+// texel, 2 = corner_light interpolated to the pixel multiplies the unlit sample, 3 = Phong shading of the unlit sample, 4 = the
+// same with a light set
 template <int kLight, bool kUV = false, bool kMip = false>
 __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigned long long key, int xi, int yi, float bgr,
                                               float bgg, float bgb) {
@@ -529,6 +537,17 @@ __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigne
             nr::phong_rgb(E, prm, s, rgb);
             o.r = rgb[0]; o.g = rgb[1]; o.b = rgb[2];
         }
+        if constexpr (kLight == 4) {  // Phong with a light set
+            float l[3], rgb[3], pos[3];
+            nr::perspective_weights(w, zp, cc.y, cc.z, cc.w, l);
+            const float* prm = p.phong_prm + (size_t)b * p.prm_bstride;
+            const float* lts = p.lts + (size_t)b * p.lt_bstride;
+            nr::PhongEval E;
+            nr::phong_lights_at(p.phong_cs + ((size_t)b * p.cs_bstride + fn) * 18, l, prm, lts, p.NL, E, pos);
+            const float s[3] = {o.r, o.g, o.b};
+            nr::phong_lights_rgb(E, pos, prm, lts, p.NL, s, rgb);
+            o.r = rgb[0]; o.g = rgb[1]; o.b = rgb[2];
+        }
     }
     return o;
 }
@@ -551,7 +570,7 @@ __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigne
 // kTex == 2 (NR_TEX_UV): the direct variants with the texture-image sampler (shade_pixel<kLit, true>), same tile map.
 // kTex == 3 (NR_TEX_UV | NR_TEX_MIPMAP): the same with the trilinear pyramid sampler (shade_pixel<kLit, true, true>).
 template <bool kAA, int kTex, int kLight>
-__global__ void __launch_bounds__(256, kLight == 3 ? NR_RESOLVE_PHONG_MIN_CTAS : kTex == 3 ? NR_RESOLVE_MIP_MIN_CTAS : (kLight == 2 ? (kAA ? NR_RESOLVE_SMOOTH_AA_MIN_CTAS : NR_RESOLVE_SMOOTH_MIN_CTAS) : (kAA ? 5 : NR_RESOLVE_MIN_CTAS))) k_resolve(const __grid_constant__ FwdParams p, int nslots) {
+__global__ void __launch_bounds__(256, kLight == 4 ? NR_RESOLVE_LIGHTS_MIN_CTAS : kLight == 3 ? NR_RESOLVE_PHONG_MIN_CTAS : kTex == 3 ? NR_RESOLVE_MIP_MIN_CTAS : (kLight == 2 ? (kAA ? NR_RESOLVE_SMOOTH_AA_MIN_CTAS : NR_RESOLVE_SMOOTH_MIN_CTAS) : (kAA ? 5 : NR_RESOLVE_MIN_CTAS))) k_resolve(const __grid_constant__ FwdParams p, int nslots) {
     constexpr bool kStage = kTex == 1;  // kTex: 0 = every texel straight from global memory, 1 = cubes staged with cp.async.bulk
     constexpr bool kUV = kTex >= 2;     //       2 = texture image through per-corner UVs, 3 = its mip pyramid
     constexpr bool kMip = kTex == 3;
@@ -724,8 +743,9 @@ extern "C" size_t nr_b200_forward_workspace_bytes(int32_t B, int32_t F, int32_t 
     return fwd_layout(B, F, S).total;
 }
 
-// nr_b200_forward (phong NULL) and nr_b200_forward_phong
-static int forward_impl(const nr_b200_forward_args* args, const nr_b200_phong_args* phong, void* cuda_stream) {
+// nr_b200_forward (phong, lights NULL), nr_b200_forward_phong (lights NULL) and nr_b200_forward_lights
+static int forward_impl(const nr_b200_forward_args* args, const nr_b200_phong_args* phong, const nr_b200_lights_args* lights,
+                        void* cuda_stream) {
     nr_internal::launch_count() = 0;
     // Two layouts: the full struct, and the ABI-4 struct from before corner_light (which then reads as NULL).  Only the
     // caller's struct_size bytes are read.
@@ -757,6 +777,8 @@ static int forward_impl(const nr_b200_forward_args* args, const nr_b200_phong_ar
     // Phong: only for RGB, and instead of face_light / corner_light
     if (phong && (!(flags & NR_RETURN_RGB) || a->face_light || smooth || !nr_internal::phong_args_ok(phong, B)))
         return NR_ERR_INVALID_ARG;
+    if (lights && !nr_internal::lights_args_ok(lights, B)) return NR_ERR_INVALID_ARG;
+    if (lights && lights->num_lights == 0) lights = nullptr;  // the Phong call exactly
     if ((flags & NR_ANTI_ALIASING) && (S & 1)) return NR_ERR_INVALID_ARG;
     if (S > 32767 || B > 65535) return NR_ERR_UNSUPPORTED;  // 32-bit pixel offsets; batch = grid.z of the resolve pass
     // NR_TEX_UV: image (NR_TEX_MIPMAP: pyramid) and UV offsets are 32-bit in the kernels
@@ -783,6 +805,10 @@ static int forward_impl(const nr_b200_forward_args* args, const nr_b200_phong_ar
         p.phong_cs = phong->corner_shading; p.phong_prm = phong->params;
         p.cs_bstride = phong->shading_batch == 1 ? 0 : (size_t)F;
         p.prm_bstride = phong->params_batch == 1 ? 0 : 16;
+    }
+    if (lights) {
+        p.lts = lights->lights; p.NL = lights->num_lights;
+        p.lt_bstride = lights->lights_batch == 1 ? 0 : (size_t)lights->num_lights * 12;
     }
     p.big_cnt = (int*)(wsb + L.off_cnt);
     p.work_next = p.big_cnt + B;
@@ -851,7 +877,7 @@ static int forward_impl(const nr_b200_forward_args* args, const nr_b200_phong_ar
         // Staging whole cubes with cp.async.bulk needs 16-byte aligned, 16-byte sized cubes; up to kStageBytes of
         // shared memory per CTA hold the cubes of the row's runs (the rest of the runs read global memory)
         const bool aa = (flags & NR_ANTI_ALIASING) != 0;
-        const int light = phong ? 3 : (smooth ? 2 : (p.face_light != nullptr ? 1 : 0));
+        const int light = lights ? 4 : phong ? 3 : (smooth ? 2 : (p.face_light != nullptr ? 1 : 0));
         const uint32_t cube_bytes = (flags & NR_RETURN_RGB) ? (uint32_t)(ts * ts * ts) * 12u : 0u;
         const bool stage = !uv && !smooth && !phong && (flags & NR_FWD_STAGE_TEXTURES) && !aa && (flags & NR_RETURN_RGB) && (cube_bytes % 16u) == 0 &&
                            cube_bytes <= kStageBytes / 8 && ((uintptr_t)a->textures & 15) == 0;
@@ -869,7 +895,8 @@ static int forward_impl(const nr_b200_forward_args* args, const nr_b200_phong_ar
     } while (0)
 #define NR_RESOLVE_LIT(AA, TEX)                                                                    \
     do {                                                                                            \
-        if (light == 3) NR_RESOLVE(AA, TEX, 3);                                                     \
+        if (light == 4) NR_RESOLVE(AA, TEX, 4);                                                     \
+        else if (light == 3) NR_RESOLVE(AA, TEX, 3);                                                \
         else if (light == 2) NR_RESOLVE(AA, TEX, 2);                                                \
         else if (light == 1) NR_RESOLVE(AA, TEX, 1);                                                \
         else NR_RESOLVE(AA, TEX, 0);                                                                \
@@ -892,12 +919,23 @@ static int forward_impl(const nr_b200_forward_args* args, const nr_b200_phong_ar
     return cudaGetLastError() == cudaSuccess ? NR_OK : NR_ERR_CUDA;
 }
 
-extern "C" int nr_b200_forward(const nr_b200_forward_args* args, void* cuda_stream) { return forward_impl(args, nullptr, cuda_stream); }
+extern "C" int nr_b200_forward(const nr_b200_forward_args* args, void* cuda_stream) {
+    return forward_impl(args, nullptr, nullptr, cuda_stream);
+}
 
 extern "C" int nr_b200_forward_phong(const nr_b200_forward_args* args, const nr_b200_phong_args* phong, void* cuda_stream) {
     if (!phong) {
         nr_internal::launch_count() = 0;
         return NR_ERR_INVALID_ARG;
     }
-    return forward_impl(args, phong, cuda_stream);
+    return forward_impl(args, phong, nullptr, cuda_stream);
+}
+
+extern "C" int nr_b200_forward_lights(const nr_b200_forward_args* args, const nr_b200_phong_args* phong,
+                                      const nr_b200_lights_args* lights, void* cuda_stream) {
+    if (!phong) {
+        nr_internal::launch_count() = 0;
+        return NR_ERR_INVALID_ARG;
+    }
+    return forward_impl(args, phong, lights, cuda_stream);
 }

@@ -54,6 +54,13 @@ inline bool phong_args_ok(const nr_b200_phong_args* ph, int B) {
            (ph->shading_batch == 1 || ph->shading_batch == B) && (ph->params_batch == 1 || ph->params_batch == B);
 }
 
+// the same for a light set (nr_b200_lights_args); NL = 0 needs no lights pointer
+constexpr int kMaxLights = 8;
+inline bool lights_args_ok(const nr_b200_lights_args* ls, int B) {
+    return ls->struct_size == sizeof(nr_b200_lights_args) && ls->num_lights >= 0 && ls->num_lights <= kMaxLights &&
+           (ls->lights || ls->num_lights == 0) && (ls->lights_batch == 1 || ls->lights_batch == B);
+}
+
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) is issued once per (kernel instantiation, device, size high-water
 // mark) instead of on every launch: `slot` is a function-local static of the launching template.
 struct SmemOptIn {

@@ -1,6 +1,7 @@
-// nr_phong.cu -- the Phong-shading gradients of nr_b200_backward_phong (include/nr_b200.h, nr_b200_phong_args).
+// nr_phong.cu -- the Phong-shading gradients of nr_b200_backward_phong and nr_b200_backward_lights (include/nr_b200.h,
+// nr_b200_phong_args, nr_b200_lights_args).
 //
-//   k_phong_grad<kTex, kIdx>   one thread per raster pixel, modelled on k_interior_grad.  The winner's perspective weights
+//   k_phong_grad<kTex, kIdx, kLights>   one thread per raster pixel, modelled on k_interior_grad.  The winner's perspective weights
 //                   l_k and the unlit sample s are recomputed with the forward's device helpers (the depth map gives zp;
 //                   per-face cubes read the sampler depths NR_TEX_Z_BATCH0 selects), nr::phong_at evaluates the forward's
 //                   expression and nr::phong_grad its derivative.  The 18 corner floats l_k (d loss / d n, d loss / d p) go
@@ -8,6 +9,10 @@
 //                   before one set of atomics per run; the 16 parameter floats are summed over the warp, then over the CTA
 //                   in shared memory, before 16 atomics per CTA.  kTex: 0 = per-face cubes, 1 = bilinear image,
 //                   2 = trilinear pyramid.  Anti-aliasing and fill_back are runtime flags.
+//                   kLights (a light set, NL > 0): after light 0 the pixel keeps its d loss / d nh, d vh and d p
+//                   accumulators across the loop over the lights (nr::phong_light_grad); each light's 10 record floats
+//                   are summed over the warp into shared memory, and after the loop over the CTA before 10 atomics per
+//                   light per CTA, so no NL x 10 register array exists.
 //
 // It belongs to the texture half of the backward: the texture-gradient kernels (K6, k_image_grad) only need the pixel's
 // L_c, and keeping the 34 gradient floats out of them keeps their register budgets (DESIGN.md section 4g).
@@ -42,9 +47,14 @@ struct PhongParams {
     int aa, fill_back, z_batch0;
     float tex_cmp, tex_val;
     nr::MipTable mip;  // kTex 2
+    // kLights: lights [Bl,NL,12] and their gradient (or nullptr)
+    const float* lts;
+    float* grad_lts;
+    size_t lt_bstride;      // floats per item in lts (0 with Bl = 1)
+    int NL;
 };
 
-template <int kTex, bool kIdx>
+template <int kTex, bool kIdx, bool kLights>
 __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ PhongParams p) {
     __shared__ float s_prm[8][16];
     const int S = p.S;
@@ -59,6 +69,9 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
     for (int k = 0; k < 18; k++) cg[k] = 0.0f;
 #pragma unroll
     for (int k = 0; k < 16; k++) gprm[k] = 0.0f;
+    // kLights: what the loop over the lights needs of the covered pixel below
+    nr::PhongEval xE;
+    float xg[3], xs[3], xlam[3], xpos[3], xgn[3], xgp[3];
     if (fn >= 0) {
         const int r = (int)(i / S), c = (int)(i % S);
         const bool aa = p.aa != 0;
@@ -128,13 +141,63 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
         nr::phong_at(p.cs + ((size_t)b * p.cs_bstride + fn) * 18, lam, prm, E);
         float gn[3], gp[3];
         nr::phong_grad(E, prm, g, s, gn, gp, gprm);
+        if constexpr (kLights) {  // the set's gradients read neither E.L nor the set's diffuse terms
+            nr::phong_position(p.cs + ((size_t)b * p.cs_bstride + fn) * 18, lam, xpos);
+            xE = E;
 #pragma unroll
-        for (int k = 0; k < 3; k++)
-#pragma unroll
-            for (int j = 0; j < 3; j++) {
-                cg[6 * k + j] = __fmul_rn(lam[k], gn[j]);
-                cg[6 * k + 3 + j] = __fmul_rn(lam[k], gp[j]);
+            for (int k = 0; k < 3; k++) {
+                xg[k] = g[k]; xs[k] = s[k]; xlam[k] = lam[k]; xgn[k] = gn[k]; xgp[k] = gp[k];
             }
+        } else {
+#pragma unroll
+            for (int k = 0; k < 3; k++)
+#pragma unroll
+                for (int j = 0; j < 3; j++) {
+                    cg[6 * k + j] = __fmul_rn(lam[k], gn[j]);
+                    cg[6 * k + 3 + j] = __fmul_rn(lam[k], gp[j]);
+                }
+        }
+    }
+    if constexpr (kLights) {
+        __shared__ float s_lt[8][nr_internal::kMaxLights * 10];  // per warp: each light's 10 record floats
+        const float* lts = p.lts + (size_t)b * p.lt_bstride;
+        const float sigma = __ldg(p.prm + (size_t)b * p.prm_bstride + 12);
+        float gnh[3] = {0.0f, 0.0f, 0.0f}, gvh[3] = {0.0f, 0.0f, 0.0f}, gsig = 0.0f;
+        for (int j = 0; j < p.NL; j++) {  // uniform
+            float gl[10];
+#pragma unroll
+            for (int k = 0; k < 10; k++) gl[k] = 0.0f;
+            if (fn >= 0) nr::phong_light_grad(lts + 12 * j, xE, xpos, sigma, xg, xs, gnh, gvh, xgp, gsig, gl);
+            if (p.grad_lts) {  // uniform
+#pragma unroll
+                for (int off = 16; off > 0; off >>= 1)
+#pragma unroll
+                    for (int k = 0; k < 10; k++) gl[k] += __shfl_xor_sync(0xffffffffu, gl[k], off);
+                if (lane == 0) {
+#pragma unroll
+                    for (int k = 0; k < 10; k++) s_lt[warp][10 * j + k] = gl[k];
+                }
+            }
+        }
+        if (fn >= 0) {
+            nr::phong_lights_grad_end(xE, gnh, gvh, gsig, xgn, xgp, gprm);
+#pragma unroll
+            for (int k = 0; k < 3; k++)
+#pragma unroll
+                for (int j = 0; j < 3; j++) {
+                    cg[6 * k + j] = __fmul_rn(xlam[k], xgn[j]);
+                    cg[6 * k + 3 + j] = __fmul_rn(xlam[k], xgp[j]);
+                }
+        }
+        if (p.grad_lts) {  // uniform: the CTA's sum of each light's 10 floats, then 10 atomics per light
+            __syncthreads();
+            const int nw = (int)(blockDim.x >> 5);
+            for (int t = threadIdx.x; t < 10 * p.NL; t += blockDim.x) {
+                float v = 0.0f;
+                for (int w = 0; w < nw; w++) v += s_lt[w][t];
+                atomicAdd(p.grad_lts + (size_t)b * p.lt_bstride + (size_t)(t / 10) * 12 + t % 10, v);
+            }
+        }
     }
     if (p.grad_cs) {  // uniform
         // the segmented run reduction of k_depth_grad over 18 floats, then one set of atomics per run
@@ -178,8 +241,10 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
 
 template <int kTex>
 void launch_t(const PhongParams& p, bool idx, dim3 grid, cudaStream_t s) {
-    if (idx) k_phong_grad<kTex, true><<<grid, 256, 0, s>>>(p);
-    else k_phong_grad<kTex, false><<<grid, 256, 0, s>>>(p);
+    if (p.NL > 0 && idx) k_phong_grad<kTex, true, true><<<grid, 256, 0, s>>>(p);
+    else if (p.NL > 0) k_phong_grad<kTex, false, true><<<grid, 256, 0, s>>>(p);
+    else if (idx) k_phong_grad<kTex, true, false><<<grid, 256, 0, s>>>(p);
+    else k_phong_grad<kTex, false, false><<<grid, 256, 0, s>>>(p);
 }
 
 }  // namespace
@@ -207,6 +272,10 @@ void launch_phong_grad(const PhongGradLaunch& L, cudaStream_t stream) {
     p.z_batch0 = (flags & NR_TEX_Z_BATCH0) ? 1 : 0;
     p.tex_cmp = L.tex_cmp; p.tex_val = L.tex_val;
     if (L.mip) p.mip = *L.mip;
+    if (L.lights) {
+        p.lts = L.lights->lights; p.grad_lts = L.lights->grad_lights; p.NL = L.lights->num_lights;
+        p.lt_bstride = L.lights->lights_batch == 1 ? 0 : (size_t)p.NL * 12;
+    }
     const bool idx = (flags & NR_FACES_INDEXED) != 0;
     const dim3 grid((unsigned)(((size_t)p.S * p.S + 255) / 256), a->batch_size);
     LaunchScope ls("k_phong_grad", stream);

@@ -732,3 +732,66 @@ def phong_params(intensity_ambient=0.5, intensity_directional=0.5, intensity_spe
         raise ValueError("Phong parameters must hold one entry or one per batch item")
     out = torch.cat([p.expand(n, -1) for p in parts], dim=1)
     return out if key is None else _cache_put(key, out)
+
+
+def _light_record(kind, x, intensity, color, intensity_specular, color_specular, falloff, device):
+    args = (x, intensity, color, intensity_specular, color_specular, falloff)
+    if device is None:
+        device = next((a.device for a in args if isinstance(a, torch.Tensor)), torch.device('cpu'))
+    key = None
+    if _is_plain(*args):  # plain numbers: one cached device tensor per value (no host copy per call, CUDA-graph safe)
+        import numpy as np
+        key = ("light", kind) + tuple(tuple(np.asarray(a, dtype=np.float64).reshape(-1).tolist()) for a in args) + \
+            (str(device),)
+        if key in _CAMERA_CACHE:
+            return _CAMERA_CACHE[key]
+
+    def as_t(v, cols):
+        t = v.to(device=device, dtype=torch.float32) if isinstance(v, torch.Tensor) else \
+            torch.tensor(v, dtype=torch.float32, device=device)
+        return t.reshape(-1, cols) if t.dim() <= 1 else t
+
+    D = as_t(intensity, 1) * as_t(color, 3)
+    K = as_t(intensity_specular, 1) * as_t(color_specular, 3)
+    f = as_t(falloff, 1)
+    parts = [D, K, as_t(x, 3), f]
+    n = max(p.shape[0] for p in parts)
+    if any(p.shape[0] not in (1, n) for p in parts):
+        raise ValueError("light parameters must hold one entry or one per batch item")
+    tail = torch.tensor([[kind, 0.0]], dtype=torch.float32, device=device)
+    out = torch.cat([p.expand(n, -1) for p in parts] + [tail.expand(n, -1)], dim=1)
+    return out if key is None else _cache_put(key, out)
+
+
+def directional_light(direction, intensity=0.5, color=(1, 1, 1), intensity_specular=0.2, color_specular=(1, 1, 1),
+                      device=None):
+    """One directional light record [1|B,12] for F.light_set / rasterize(..., lights=...): {diffuse intensity * colour
+    (3), specular intensity * colour (3), direction towards the light (3, not normalised), 0, 0 (directional), 0}.
+    Built with torch ops, so tensor-valued arguments (intensities scalar or [B], colours and direction [3] or [B,3])
+    receive gradients.  `device`: where plain numbers go (default: the device of the first tensor argument, else the
+    CPU)."""
+    return _light_record(0.0, direction, intensity, color, intensity_specular, color_specular, 0.0, device)
+
+
+def point_light(position, intensity=0.5, color=(1, 1, 1), intensity_specular=0.2, color_specular=(1, 1, 1), falloff=0.0,
+                device=None):
+    """One point light record [1|B,12]: as F.directional_light with the light's position (in the frame of the shading
+    positions and the eye) in slots 6-8, the falloff f in slot 9 (attenuation 1 / (1 + f r^2) at distance r; 0 = none,
+    as PyTorch3D's PointLights) and kind 1.  The position and the falloff may be tensors that receive gradients."""
+    return _light_record(1.0, position, intensity, color, intensity_specular, color_specular, falloff, device)
+
+
+def light_set(*records):
+    """Stack light records ([12], [1|B,12] from F.directional_light / F.point_light) into the [1|B,NL,12] set of
+    rasterize(..., lights=...), NL <= 8, in order; records of one item serve every item.  Differentiable."""
+    if not records:
+        raise ValueError("light_set needs at least one light record")
+    if len(records) > 8:
+        raise ValueError("a light set holds at most 8 lights, got %d" % len(records))
+    recs = [r.reshape(1, 12) if r.dim() == 1 else r for r in records]
+    if any(r.dim() != 2 or r.shape[1] != 12 for r in recs):
+        raise ValueError("light records must have shape [12] or [batch size, 12]")
+    n = max(r.shape[0] for r in recs)
+    if any(r.shape[0] not in (1, n) for r in recs):
+        raise ValueError("light records must hold one entry or one per batch item")
+    return torch.stack([r.expand(n, -1) for r in recs], dim=1)

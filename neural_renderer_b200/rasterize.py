@@ -61,7 +61,7 @@ def _ptr(t):
 
 
 def _check_inputs(faces, textures, return_rgb, face_light=None, textures_fill_back=False, vertices=None, face_uvs=None,
-                  corner_light=None, corner_shading=None, shading_params=None):
+                  corner_light=None, corner_shading=None, shading_params=None, lights=None):
     # rasterize.py:66-90 (chainer type_check) -> TypeError / ValueError with the same conditions
     if not isinstance(faces, torch.Tensor):
         raise TypeError("faces must be a torch.Tensor")
@@ -103,6 +103,8 @@ def _check_inputs(faces, textures, return_rgb, face_light=None, textures_fill_ba
                 or textures.shape[0] not in (1, batch_size) or textures.shape[1] != num_cubes):
             raise ValueError("textures must have shape [batch size, num faces, ts, ts, ts, 3] with ts >= 2 and match "
                              "faces, got %s" % (tuple(textures.shape),))
+    if lights is not None:
+        _check_lights(lights, corner_shading, batch_size)
     if corner_shading is not None or shading_params is not None:
         _check_phong_inputs(corner_shading, shading_params, face_light, corner_light, return_rgb, batch_size, num_faces)
     if return_rgb and face_light is not None:
@@ -143,6 +145,20 @@ def _check_phong_inputs(corner_shading, shading_params, face_light, corner_light
     if not ((sp.dim() == 1 or (sp.dim() == 2 and sp.shape[0] in (1, batch_size))) and sp.shape[-1] == 16):
         raise ValueError("shading_params must have shape [16] or [batch size, 16], got %s" % (tuple(sp.shape),))
     if not cs.is_cuda or not sp.is_cuda:
+        raise NotImplementedError("neural_renderer_b200 has no CPU implementation (inputs must be CUDA tensors)")
+
+
+def _check_lights(lights, corner_shading, batch_size):
+    # light set [NL,12] / [1|B,NL,12], NL <= 8, on top of Phong shading's light
+    if corner_shading is None:
+        raise ValueError("lights needs Phong shading (corner_shading / shading_params)")
+    if not isinstance(lights, torch.Tensor) or not lights.is_floating_point():
+        raise TypeError("lights must be a floating point torch.Tensor")
+    if not ((lights.dim() == 2 or (lights.dim() == 3 and lights.shape[0] in (1, batch_size))) and lights.shape[-1] == 12
+            and lights.shape[-2] <= 8):
+        raise ValueError("lights must have shape [num lights, 12] or [batch size, num lights, 12] with at most 8 lights, "
+                         "got %s" % (tuple(lights.shape),))
+    if not lights.is_cuda:
         raise NotImplementedError("neural_renderer_b200 has no CPU implementation (inputs must be CUDA tensors)")
 
 
@@ -236,7 +252,7 @@ class _RasterizeFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, geom, textures, face_light, cfg, indices, face_uvs=None, corner_light=None, corner_shading=None,
-                shading_params=None):
+                shading_params=None, lights=None):
         lib = _lib.load()
         dev = geom.device
         geom_c = geom.detach().contiguous()
@@ -246,6 +262,7 @@ class _RasterizeFunction(torch.autograd.Function):
         # Phong shading: corner_shading [Bc,F,3,6] and params [Bp,16], Bc / Bp = 1 for one set shared by every item
         cs_c = corner_shading.detach().to(torch.float32).contiguous() if corner_shading is not None else None
         sp_c = shading_params.detach().to(torch.float32).contiguous() if shading_params is not None else None
+        lt_c = lights.detach().to(torch.float32).contiguous() if lights is not None else None  # [Bl,NL,12], NL >= 1
         flags = cfg.flags
         if indices is not None:
             B, Nv = geom_c.shape[:2]
@@ -310,6 +327,9 @@ class _RasterizeFunction(torch.autograd.Function):
             a.corner_light = _ptr(corner_c)
             if cs_c is None:
                 _lib.check(lib.nr_b200_forward(ctypes.byref(a), _stream_ptr(dev)))
+            elif lt_c is not None:
+                ph, la = _phong_args(cs_c, sp_c), _lights_args(lt_c)
+                _lib.check(lib.nr_b200_forward_lights(ctypes.byref(a), ctypes.byref(ph), ctypes.byref(la), _stream_ptr(dev)))
             else:
                 ph = _phong_args(cs_c, sp_c)
                 _lib.check(lib.nr_b200_forward_phong(ctypes.byref(a), ctypes.byref(ph), _stream_ptr(dev)))
@@ -325,12 +345,13 @@ class _RasterizeFunction(torch.autograd.Function):
         ctx.need_uv_grad = uv_c is not None and want_rgb and ctx.needs_input_grad[5]
         ctx.need_cs_grad = cs_c is not None and ctx.needs_input_grad[7]
         ctx.need_sp_grad = sp_c is not None and ctx.needs_input_grad[8]
+        ctx.need_lt_grad = lt_c is not None and ctx.needs_input_grad[9]
         # interior_gradient: the backward differentiates the sampler, so it reads the textures (and face_uvs / corner_light)
         ctx.interior = cfg.interior and want_rgb and ctx.needs_input_grad[0]
         need_tex = need_light_grad or ctx.need_uv_grad or ctx.need_corner_grad or ctx.interior or ctx.need_cs_grad or \
-            ctx.need_sp_grad
+            ctx.need_sp_grad or ctx.need_lt_grad
         ctx.save_for_backward(geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c if need_tex else None, indices, uv_c, corner_c,
-                              cs_c, sp_c)
+                              cs_c, sp_c, lt_c)
         if cfg.aa:
             rgb_o, alpha_o, depth_o = out_rgb, out_alpha, out_depth
         else:
@@ -343,7 +364,7 @@ class _RasterizeFunction(torch.autograd.Function):
         lib = _lib.load()
         cfg = ctx.cfg
         flags = ctx.flags | (_lib.NR_GRAD_INTERIOR if ctx.interior else 0)
-        geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c, indices, uv_c, corner_c, cs_c, sp_c = ctx.saved_tensors
+        geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c, indices, uv_c, corner_c, cs_c, sp_c, lt_c = ctx.saved_tensors
         dev = geom_c.device
         B, F = geom_c.shape[0], ctx.F
         want_rgb = bool(flags & _lib.NR_RETURN_RGB)
@@ -365,6 +386,8 @@ class _RasterizeFunction(torch.autograd.Function):
             grad_cs = torch.empty_like(cs_c) if ctx.need_cs_grad else None
             grad_sp = torch.empty_like(sp_c) if ctx.need_sp_grad else None
             ph = _phong_args(cs_c, sp_c, grad_cs, grad_sp) if cs_c is not None else None
+            grad_lt = torch.empty_like(lt_c) if ctx.need_lt_grad else None
+            la = _lights_args(lt_c, grad_lt) if lt_c is not None else None
             ws_bytes = lib.nr_b200_backward_workspace_bytes(B, F, cfg.S, ctx.ts, flags)
             ws = torch.empty((max(ws_bytes, 16),), dtype=torch.uint8, device=dev)
             a = _lib.BackwardArgs()
@@ -387,6 +410,8 @@ class _RasterizeFunction(torch.autograd.Function):
             hook = _TEXTURE_GRAD_HOOK if (want_rgb and g_rgb is not None) else None
 
             def call():
+                if la is not None:  # light set: grad_lights too is filled by the texture half
+                    return lib.nr_b200_backward_lights(ctypes.byref(a), ctypes.byref(ph), ctypes.byref(la), _stream_ptr(dev))
                 if ph is not None:  # Phong: grad_corner_shading / grad_params are filled by the texture half
                     return lib.nr_b200_backward_phong(ctypes.byref(a), ctypes.byref(ph), _stream_ptr(dev))
                 if corner_c is None:
@@ -407,7 +432,7 @@ class _RasterizeFunction(torch.autograd.Function):
                 _lib.check(call())
                 if pending is not None:
                     pending.wait()
-        return grad_geom, grad_textures, grad_light, None, None, grad_uvs, grad_corner, grad_cs, grad_sp
+        return grad_geom, grad_textures, grad_light, None, None, grad_uvs, grad_corner, grad_cs, grad_sp, grad_lt
 
 
 def _phong_args(cs_c, sp_c, grad_cs=None, grad_sp=None):
@@ -417,6 +442,14 @@ def _phong_args(cs_c, sp_c, grad_cs=None, grad_sp=None):
     ph.corner_shading, ph.params = _ptr(cs_c), _ptr(sp_c)
     ph.grad_corner_shading, ph.grad_params = _ptr(grad_cs), _ptr(grad_sp)
     return ph
+
+
+def _lights_args(lt_c, grad_lt=None):
+    la = _lib.LightsArgs()
+    la.struct_size = ctypes.sizeof(_lib.LightsArgs)
+    la.lights_batch, la.num_lights = int(lt_c.shape[0]), int(lt_c.shape[1])
+    la.lights, la.grad_lights = _ptr(lt_c), _ptr(grad_lt)
+    return la
 
 
 class _MipPyramid(torch.autograd.Function):
@@ -453,7 +486,8 @@ TEXTURE_FILTERS = ('bilinear', 'trilinear')
 
 def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_color, return_rgb, return_alpha,
          return_depth, face_light=None, textures_fill_back=False, vertices=None, reference_exact=None, face_uvs=None,
-         texture_filter='bilinear', corner_light=None, interior_gradient=False, corner_shading=None, shading_params=None):
+         texture_filter='bilinear', corner_light=None, interior_gradient=False, corner_shading=None, shading_params=None,
+         lights=None):
     if (corner_shading is not None or shading_params is not None) and interior_gradient:
         raise ValueError("interior_gradient=True is not supported with Phong shading (corner_shading / shading_params): no "
                          "vertex gradient flows through the interpolation of the per-pixel normal and position")
@@ -468,7 +502,7 @@ def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_
                          "than one item: the reference-exact sampler reads the depths of item 0 for every item, so its "
                          "derivative would cross items.  Pass reference_exact=False (or set_reference_exact(False))")
     _check_inputs(faces, textures, return_rgb, face_light, textures_fill_back, vertices, face_uvs, corner_light,
-                  corner_shading, shading_params)
+                  corner_shading, shading_params, lights)
     phong = corner_shading is not None
     indices = None
     if vertices is not None:
@@ -504,6 +538,13 @@ def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_
                 corner_shading = corner_shading[:1]  # an expanded shared set (Bc = 1)
             if shading_params.shape[0] == batch_size > 1 and shading_params.stride(0) == 0:
                 shading_params = shading_params[:1]
+            if lights is not None:
+                lights = lights.float() if lights.dtype != torch.float32 else lights
+                lights = lights[None] if lights.dim() == 2 else lights
+                if lights.shape[0] == batch_size > 1 and lights.stride(0) == 0:
+                    lights = lights[:1]  # an expanded shared set (Bl = 1)
+                if lights.shape[1] == 0:
+                    lights = None  # no extra light: Phong exactly
     cfg = _make_config(image_size, anti_aliasing, near, far, eps, background_color, return_rgb, return_alpha,
                        return_depth, geom.device, batch_size, reference_exact)
     if return_rgb and textures_fill_back:
@@ -519,7 +560,7 @@ def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_
         textures = _MipPyramid.apply(textures)
     return _RasterizeFunction.apply(geom, textures if return_rgb else None, face_light if return_rgb else None, cfg,
                                     indices, face_uvs, corner_light, corner_shading if return_rgb else None,
-                                    shading_params if return_rgb else None)
+                                    shading_params if return_rgb else None, lights if return_rgb else None)
 
 
 def rasterize_rgbad(
@@ -545,6 +586,7 @@ def rasterize_rgbad(
         interior_gradient=False,
         corner_shading=None,
         shading_params=None,
+        lights=None,
 ):
     """Generate RGB, alpha channel, and depth images from faces and textures (for RGB).  rasterize.py:900-977.
 
@@ -598,12 +640,18 @@ def rasterize_rgbad(
                               * sample + specular * q^shininess, the highlight of the reflected light towards the eye
                               (include/nr_b200.h).  Exclusive with face_light / corner_light and with
                               interior_gradient; both receive gradients (a batch of 1 gets the sum over the items).
+      lights [NL,12] / [1|B,NL,12]   Phong shading with up to 8 more lights after shading_params' own, directional or
+                              point (F.directional_light / F.point_light / F.light_set build them): each adds its diffuse
+                              term a relu(n . l) to the light of the sample and its highlight a q^shininess, with a point
+                              light's direction and attenuation a = 1 / (1 + falloff r^2) evaluated at every pixel
+                              (include/nr_b200.h, nr_b200_lights_args).  Only with corner_shading / shading_params;
+                              receives gradients (a batch of 1 gets the sum over the items).
     `textures` with batch size 1 (or an expanded stride-0 batch) while the geometry batch is larger = one texture set
     shared by every item (a mesh seen from B viewpoints, mesh.py:29-34); its gradient is the sum over the items."""
     rgb, alpha, depth, _, _ = _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_color,
                                    return_rgb, return_alpha, return_depth, face_light, textures_fill_back, vertices,
                                    reference_exact, face_uvs, texture_filter, corner_light, interior_gradient,
-                                   corner_shading, shading_params)
+                                   corner_shading, shading_params, lights)
     return {
         'rgb': rgb if return_rgb else None,
         'alpha': alpha if return_alpha else None,
@@ -631,6 +679,7 @@ def rasterize(
         interior_gradient=False,
         corner_shading=None,
         shading_params=None,
+        lights=None,
 ):
     """RGB images [B,3,H,W] from faces and textures.  rasterize.py:980-1008 (keyword-only extras: rasterize_rgbad; in
     texture-image mode both the image and face_uvs receive gradients)."""
@@ -638,7 +687,8 @@ def rasterize(
         faces, textures, image_size, anti_aliasing, near, far, eps, background_color, True, False, False,
         face_light=face_light, textures_fill_back=textures_fill_back, vertices=vertices,
         reference_exact=reference_exact, face_uvs=face_uvs, texture_filter=texture_filter, corner_light=corner_light,
-        interior_gradient=interior_gradient, corner_shading=corner_shading, shading_params=shading_params)['rgb']
+        interior_gradient=interior_gradient, corner_shading=corner_shading, shading_params=shading_params,
+        lights=lights)['rgb']
 
 
 def rasterize_silhouettes(

@@ -36,6 +36,9 @@ class Renderer(object):
         self.light_intensity_specular = 0.2
         self.light_color_specular = [1, 1, 1]
         self.light_shininess = 64.0
+        # extra lights of shading='phong' on top of the light above: a list of F.directional_light / F.point_light
+        # records, or one stacked [NL,12] / [1|B,NL,12] tensor (F.light_set), at most 8.  Empty = that light alone
+        self.lights = []
 
         # rasterization
         self.rasterizer_eps = 1e-3
@@ -107,6 +110,9 @@ class Renderer(object):
         texture_filter = self.texture_filter if face_uvs is not None else 'bilinear'
         if self.shading not in ('flat', 'smooth', 'phong'):
             raise ValueError("shading must be 'flat', 'smooth' or 'phong', got %r" % (self.shading,))
+        n_lights = self.lights.shape[-2] if isinstance(self.lights, torch.Tensor) else len(self.lights)
+        if self.shading != 'phong' and n_lights:
+            raise ValueError("lights (a light set) needs shading='phong', got shading=%r" % (self.shading,))
         fused = (self.fused and self._fusable(vertices, faces) and textures.is_cuda and textures.dtype == torch.float32)
         light_args = (self.light_intensity_ambient, self.light_intensity_directional, self.light_color_ambient,
                       self.light_color_directional, self.light_direction)
@@ -199,6 +205,11 @@ class Renderer(object):
             self.background_color, reference_exact=self.reference_exact, face_uvs=face_uvs,
             texture_filter=texture_filter, corner_light=corner, interior_gradient=self.interior_gradient)
 
+    def _light_set(self):
+        if isinstance(self.lights, torch.Tensor):
+            return self.lights if self.lights.shape[-2] > 0 else None
+        return F.light_set(*self.lights) if len(self.lights) else None
+
     def _render_phong(self, vertices, faces, textures, face_uvs, texture_filter, fused):
         # vertex normals of the original faces, then per corner of the drawn faces (copies: reversed normal) the normal and
         # the world-space position; the light, the specular highlight and the eye (self.eye, world space) are per pixel
@@ -208,6 +219,9 @@ class Renderer(object):
         params = F.phong_params(self.light_intensity_ambient, self.light_intensity_directional, self.light_intensity_specular,
                                 self.light_color_ambient, self.light_color_directional, self.light_color_specular,
                                 self.light_direction, self.light_shininess, self.eye, device=vertices.device)
+        lights = self._light_set()
+        if lights is not None:
+            lights = lights.to(vertices.device)
         if fused:
             indices = self._indices(faces)
             # one mesh seen from B viewpoints (an expanded, stride-0 vertex batch and a shared index set): one corner set
@@ -218,7 +232,7 @@ class Renderer(object):
                 indices, textures, self.image_size, self.anti_aliasing, self.near, self.far, self.rasterizer_eps,
                 self.background_color, textures_fill_back=self.fill_back, vertices=self._transform(vertices),
                 reference_exact=self.reference_exact, face_uvs=face_uvs, texture_filter=texture_filter,
-                corner_shading=cs, shading_params=params)
+                corner_shading=cs, shading_params=params, lights=lights)
         # op by op: torch normals and corners, materialised faces, doubled textures / UV corners for fill_back
         normals = F._vertex_normals_torch(vertices, faces)
         if self.fill_back:
@@ -232,4 +246,4 @@ class Renderer(object):
         return rasterize(
             faces, textures, self.image_size, self.anti_aliasing, self.near, self.far, self.rasterizer_eps,
             self.background_color, reference_exact=self.reference_exact, face_uvs=face_uvs,
-            texture_filter=texture_filter, corner_shading=cs, shading_params=params)
+            texture_filter=texture_filter, corner_shading=cs, shading_params=params, lights=lights)
