@@ -341,6 +341,38 @@ typedef struct nr_b200_lights_args {
     float *grad_lights;    /* backward: [Bl,NL,12] or NULL */
 } nr_b200_lights_args;
 
+/* Environment lighting for Phong shading, additive to ABI 4: one struct (nr_b200_sh_args) and two entry points
+ * (nr_b200_forward_sh / nr_b200_backward_sh).  Second-order real spherical harmonics (9 coefficients per channel) hold the
+ * diffuse irradiance of a distant environment (Ramamoorthi & Hanrahan 2001).
+ *   sh [Bs,9,3] (device), coefficient k = 0..8 major, channel minor; Bs in {1, B} (1 = one environment for every item, its
+ *   gradient the sum over the items).  The coefficients are irradiance-ready: already convolved with the clamped cosine
+ *   and divided by pi, so S = (1/C0, 0, ..., 0) gives E = 1 and a white albedo under a uniform environment of radiance r
+ *   renders r.  Frame: that of corner_shading's normals (the frame of e and of the light positions).
+ *   Covered raster pixel: nh = (x, y, z) = n / (|n| + 1e-5) of the Phong expression, as is (not renormalised, so |nh| is
+ *   slightly below 1), fp32 with every fused multiply-add explicit:
+ *     Y0 = C0,  Y1 = C1 y,  Y2 = C1 z,  Y3 = C1 x,  Y4 = C2 (x y),  Y5 = C2 (y z),  Y6 = C3 fma(3 z, z, -1),
+ *     Y7 = C2 (x z),  Y8 = C4 fma(x, x, -(y y))
+ *     C0 = 0.28209479 = 1/(2 sqrt(pi)),  C1 = 0.48860251 = sqrt(3/(4 pi)),  C2 = 1.09254843 = sqrt(15/(4 pi)),
+ *     C3 = 0.31539157 = sqrt(5/(16 pi)),  C4 = 0.54627422 = sqrt(15/(16 pi))
+ *     E_c = S[0][c] Y0, then E_c = fma(S[k][c], Y_k, E_c) for k = 1 .. 8 in order
+ *   E_c is not clamped: an environment whose coefficients make it negative somewhere gives negative irradiance there, and
+ *   that is passed through.  Order of terms: L_c of the light-set expression above (params' ambient + diffuse, then the
+ *   set's diffuse terms in order), then L_c = L_c + E_c, then rgb_c = fma(K_c, h, L_c s_c) and the set's highlights as
+ *   for nr_b200_forward_lights.  So S = 0 gives nr_b200_forward_lights (NL = 0: nr_b200_forward_phong) bit for bit.
+ *   Backward (nr_b200_backward_sh), texture half: grad_textures / grad_face_uvs with the pixel's full L_c;
+ *   grad_corner_shading also through d E / d nh (E does not depend on p); grad_params and grad_lights as without SH;
+ *   grad_sh[k][c] += Y_k(nh) g_c s_c.  Each gradient output may be NULL and is zero-filled first unless
+ *   NR_GRAD_ACCUMULATE.  The faces half is unchanged; NR_GRAD_INTERIOR is NR_ERR_UNSUPPORTED, as for Phong.
+ *   Host rejections (NR_ERR_INVALID_ARG, before any launch), besides those of nr_b200_*_lights: a struct_size mismatch,
+ *   Bs not in {1, B}, sh NULL, and grad_sh without `textures`.  A NULL `sh` struct is allowed: the call is then
+ *   nr_b200_*_lights with the same `lights`. */
+typedef struct nr_b200_sh_args {
+    uint32_t struct_size;  /* sizeof(nr_b200_sh_args) = 24 */
+    int32_t sh_batch;      /* Bs: 1 or B */
+    const float *sh;       /* [Bs,9,3] */
+    float *grad_sh;        /* backward: [Bs,9,3] or NULL */
+} nr_b200_sh_args;
+
 /* Attribute interpolation, additive to ABI 4: two flag bits, one struct and two entry points.  Renders C >= 1 arbitrary
  * channels (normals, positions, UVs, labels, features) through the maps an ordinary forward call wrote (face_index_map,
  * weight_map; a silhouette-only forward suffices), with gradients into the attributes and, through the perspective
@@ -431,6 +463,13 @@ NR_B200_API int nr_b200_forward_lights(const nr_b200_forward_args *args, const n
                                        const nr_b200_lights_args *lights, void *cuda_stream);
 NR_B200_API int nr_b200_backward_lights(const nr_b200_backward_args *args, const nr_b200_phong_args *phong,
                                         const nr_b200_lights_args *lights, void *cuda_stream);
+/* Phong shading with a light set and an SH environment (nr_b200_sh_args above): the light-set calls with `sh` added;
+ * lights may be NULL (no set), and sh NULL runs exactly nr_b200_forward_lights / nr_b200_backward_lights.  grad_sh is
+ * filled by the texture half. */
+NR_B200_API int nr_b200_forward_sh(const nr_b200_forward_args *args, const nr_b200_phong_args *phong,
+                                   const nr_b200_lights_args *lights, const nr_b200_sh_args *sh, void *cuda_stream);
+NR_B200_API int nr_b200_backward_sh(const nr_b200_backward_args *args, const nr_b200_phong_args *phong,
+                                    const nr_b200_lights_args *lights, const nr_b200_sh_args *sh, void *cuda_stream);
 /* Attribute interpolation (nr_b200_interpolate_args above): the image `out`, and its backward into grad_attributes and the
  * interior vertex gradient.  One kernel launch each (plus the zero-fill of the backward). */
 NR_B200_API int nr_b200_interpolate(const nr_b200_interpolate_args *args, void *cuda_stream);

@@ -50,6 +50,8 @@ EXPORTED_SYMBOLS = (
     "nr_b200_backward_phong",
     "nr_b200_forward_lights",
     "nr_b200_backward_lights",
+    "nr_b200_forward_sh",
+    "nr_b200_backward_sh",
     "nr_b200_interpolate",
     "nr_b200_interpolate_backward",
     "nr_b200_vertices_to_faces",
@@ -132,6 +134,13 @@ class LightsArgs(ctypes.Structure):
     ]
 
 
+class ShArgs(ctypes.Structure):
+    _fields_ = [
+        ("struct_size", ctypes.c_uint32), ("sh_batch", ctypes.c_int32),
+        ("sh", ctypes.c_void_p), ("grad_sh", ctypes.c_void_p),
+    ]
+
+
 class InterpolateArgs(ctypes.Structure):
     _fields_ = [
         ("struct_size", ctypes.c_uint32), ("flags", ctypes.c_uint32),
@@ -187,6 +196,12 @@ def load():
     lib.nr_b200_backward_lights.restype = ctypes.c_int
     lib.nr_b200_backward_lights.argtypes = [ctypes.POINTER(BackwardArgs), ctypes.POINTER(PhongArgs),
                                             ctypes.POINTER(LightsArgs), ctypes.c_void_p]
+    lib.nr_b200_forward_sh.restype = ctypes.c_int
+    lib.nr_b200_forward_sh.argtypes = [ctypes.POINTER(ForwardArgs), ctypes.POINTER(PhongArgs), ctypes.POINTER(LightsArgs),
+                                       ctypes.POINTER(ShArgs), ctypes.c_void_p]
+    lib.nr_b200_backward_sh.restype = ctypes.c_int
+    lib.nr_b200_backward_sh.argtypes = [ctypes.POINTER(BackwardArgs), ctypes.POINTER(PhongArgs), ctypes.POINTER(LightsArgs),
+                                        ctypes.POINTER(ShArgs), ctypes.c_void_p]
     for name in ("nr_b200_interpolate", "nr_b200_interpolate_backward"):
         fn = getattr(lib, name)
         fn.restype = ctypes.c_int

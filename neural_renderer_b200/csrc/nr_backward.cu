@@ -157,6 +157,9 @@ struct BwdParams {
     const float* lts;
     size_t lt_bstride;   // floats per item in lts (0 with Bl = 1)
     int NL;
+    // SH environment (appended likewise, the kLight == 5 variants, with the set above or NL = 0): sh [Bs,9,3]
+    const float* sh;
+    size_t sh_bstride;   // floats per item in sh (0 with Bs = 1)
 };
 
 //@phase helpers: rcp / vector RED / load_grad (inlined)
@@ -981,11 +984,12 @@ __device__ __forceinline__ void light_grad_scatter(float (&gl)[N], int fn, int l
 // that sit next to each other with the same (cube, cell) therefore add their 8 x 3 contributions together with
 // kTgCombine shuffle steps first (runs of up to 2^kTgCombine lanes collapse into one lane's reductions).
 //
-// kLight: 0 = face_light or unlit, 2 = corner_light, 3 = Phong, 4 = Phong with a light set.
+// kLight: 0 = face_light or unlit, 2 = corner_light, 3 = Phong, 4 = Phong with a light set, 5 = Phong with an SH environment.
 // kCorner (corner_light): the pixel's light L_c = the corner factors interpolated with its perspective weights l_k (own
 // vertex depths) takes face_light's place, and d loss / d corner_light = l_k g_c s_c goes through the same run reduction.
 // kPhong: L_c = the diffuse part of the Phong expression at the pixel (nr::phong_diffuse) takes face_light's place; the
-// Phong gradients themselves come from k_phong_grad (nr_phong.cu).  Mode 4 adds the set's diffuse terms to L_c.
+// Phong gradients themselves come from k_phong_grad (nr_phong.cu).  Mode 4 adds the set's diffuse terms to L_c, mode 5
+// those of a set (NL may be 0) and the SH irradiance E_c.
 template <int kTgCombine, int kLight>
 __global__ void __launch_bounds__(256, kTgCombine ? (kLight >= 2 ? NR_TGC_MIN_CTAS : 4) : NR_TG_MIN_CTAS) k_texture_grad(const __grid_constant__ BwdParams p) {
     constexpr bool kCorner = kLight == 2, kPhong = kLight >= 3;
@@ -1047,7 +1051,10 @@ __global__ void __launch_bounds__(256, kTgCombine ? (kLight >= 2 ? NR_TGC_MIN_CT
                 nr::PhongEval E;
                 const float* cs = p.phong_cs + ((size_t)b * p.cs_bstride + fn) * 18;
                 const float* prm = p.phong_prm + (size_t)b * p.prm_bstride;
-                if constexpr (kLight == 4) {
+                if constexpr (kLight == 5) {
+                    float pos[3];
+                    nr::phong_sh_diffuse(cs, lam, prm, p.lts + (size_t)b * p.lt_bstride, p.NL, p.sh + (size_t)b * p.sh_bstride, E, pos);
+                } else if constexpr (kLight == 4) {
                     float pos[3];
                     nr::phong_lights_diffuse(cs, lam, prm, p.lts + (size_t)b * p.lt_bstride, p.NL, E, pos);
                 } else {
@@ -1192,7 +1199,7 @@ __device__ __forceinline__ void red_add_6(float* t, const float v[6]) {
 // weight) goes to UV corner k as l_k (gu, gv), corners reversed back for a fill_back copy.  Runs of neighbouring lanes
 // that show the same face sum their 6 floats with shuffles and the run's first lane adds them.
 //
-// kLight: 0 = face_light or unlit, 2 = corner_light, 3 = Phong, 4 = Phong with a light set.
+// kLight: 0 = face_light or unlit, 2 = corner_light, 3 = Phong, 4 = Phong with a light set, 5 = Phong with an SH environment.
 // kCorner (corner_light): as in k_texture_grad, the interpolated light L_c replaces face_light (also in the face_uvs
 // gradient) and the 9-float corner-light gradient goes through the run reduction.  kPhong: likewise with the Phong L_c.
 template <int kTgCombine, bool kMip, bool kUvGrad, int kLight>
@@ -1270,7 +1277,10 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
             nr::PhongEval E;
             const float* cs = p.phong_cs + ((size_t)b * p.cs_bstride + fn) * 18;
             const float* prm = p.phong_prm + (size_t)b * p.prm_bstride;
-            if constexpr (kLight == 4) {
+            if constexpr (kLight == 5) {
+                float pos[3];
+                nr::phong_sh_diffuse(cs, lam, prm, p.lts + (size_t)b * p.lt_bstride, p.NL, p.sh + (size_t)b * p.sh_bstride, E, pos);
+            } else if constexpr (kLight == 4) {
                 float pos[3];
                 nr::phong_lights_diffuse(cs, lam, prm, p.lts + (size_t)b * p.lt_bstride, p.NL, E, pos);
             } else {
@@ -1612,10 +1622,11 @@ extern "C" size_t nr_b200_backward_workspace_bytes(int32_t B, int32_t F, int32_t
     return bin_layout(B, F, S, strip_rec_bytes(S, both)).total;
 }
 
-// nr_b200_backward (corner_light, phong, lights NULL), nr_b200_backward_corner_light (smooth shading), nr_b200_backward_phong
-// (lights NULL) and nr_b200_backward_lights
+// nr_b200_backward (corner_light, phong, lights, sh NULL), nr_b200_backward_corner_light (smooth shading),
+// nr_b200_backward_phong (lights, sh NULL), nr_b200_backward_lights (sh NULL) and nr_b200_backward_sh
 static int backward_impl(const nr_b200_backward_args* args, const float* corner_light, float* grad_corner_light,
-                         const nr_b200_phong_args* phong, const nr_b200_lights_args* lights, void* cuda_stream) {
+                         const nr_b200_phong_args* phong, const nr_b200_lights_args* lights, const nr_b200_sh_args* sh,
+                         void* cuda_stream) {
     nr_internal::launch_count() = 0;
     // Two layouts: the full struct, and the ABI-4 struct from before grad_face_uvs (which then reads as NULL).  Only the
     // caller's struct_size bytes are read.
@@ -1660,8 +1671,11 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
     if (phong && (!rgb || a->face_light || smooth || !nr_internal::phong_args_ok(phong, B))) return NR_ERR_INVALID_ARG;
     // light set: grad_lights needs s as well
     if (lights && (!nr_internal::lights_args_ok(lights, B) || (lights->grad_lights && !a->textures))) return NR_ERR_INVALID_ARG;
+    // SH environment: grad_sh needs s as well
+    if (sh && (!nr_internal::sh_args_ok(sh, B) || (sh->grad_sh && !a->textures))) return NR_ERR_INVALID_ARG;
     if (lights && lights->num_lights == 0) lights = nullptr;  // the Phong call exactly
-    const bool phong_grads = phong && (phong->grad_corner_shading || phong->grad_params || (lights && lights->grad_lights));
+    const bool phong_grads = phong && (phong->grad_corner_shading || phong->grad_params || (lights && lights->grad_lights) ||
+                                       (sh && sh->grad_sh));
     if (phong_grads && !a->textures) return NR_ERR_INVALID_ARG;
     // NR_GRAD_INTERIOR: the sampler's derivative reads the textures; the cubes of NR_TEX_Z_BATCH0 sample item b with the
     // depths of item 0, so their derivative would cross items (B = 1 is the plain sampler)
@@ -1723,6 +1737,9 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
         if (part_tex && lights && lights->grad_lights &&
             cudaMemsetAsync(lights->grad_lights, 0, (size_t)lights->lights_batch * lights->num_lights * 12 * sizeof(float), stream) != cudaSuccess)
             return NR_ERR_CUDA;
+        if (part_tex && sh && sh->grad_sh &&
+            cudaMemsetAsync(sh->grad_sh, 0, (size_t)sh->sh_batch * 27 * sizeof(float), stream) != cudaSuccess)
+            return NR_ERR_CUDA;
         nr_internal::prof_end(stream);
     }
 
@@ -1758,13 +1775,19 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
         p.lts = lights->lights; p.NL = lights->num_lights;
         p.lt_bstride = lights->lights_batch == 1 ? 0 : (size_t)lights->num_lights * 12;
     }
-    const int light = lights ? 4 : (phong ? 3 : (smooth ? 2 : 0));
+    if (sh) {
+        p.sh = sh->sh;
+        p.sh_bstride = sh->sh_batch == 1 ? 0 : 27;
+    }
+    const int light = sh ? 5 : (lights ? 4 : (phong ? 3 : (smooth ? 2 : 0)));
 
     const dim3 pgrid((unsigned)(((size_t)S * S + 255) / 256), B);
     auto launch_texture_grad = [&]() {
         if (mip) {
             nr_internal::LaunchScope ls("k_image_grad", stream);
-            if (light == 4 && uv_grad) k_image_grad_mip<NR_TG_COMBINE, true, 4><<<pgrid, 256, 0, stream>>>(p);
+            if (light == 5 && uv_grad) k_image_grad_mip<NR_TG_COMBINE, true, 5><<<pgrid, 256, 0, stream>>>(p);
+            else if (light == 5) k_image_grad_mip<NR_TG_COMBINE, false, 5><<<pgrid, 256, 0, stream>>>(p);
+            else if (light == 4 && uv_grad) k_image_grad_mip<NR_TG_COMBINE, true, 4><<<pgrid, 256, 0, stream>>>(p);
             else if (light == 4) k_image_grad_mip<NR_TG_COMBINE, false, 4><<<pgrid, 256, 0, stream>>>(p);
             else if (light == 3 && uv_grad) k_image_grad_mip<NR_TG_COMBINE, true, 3><<<pgrid, 256, 0, stream>>>(p);
             else if (light == 3) k_image_grad_mip<NR_TG_COMBINE, false, 3><<<pgrid, 256, 0, stream>>>(p);
@@ -1776,7 +1799,9 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
         }
         if (uv) {
             nr_internal::LaunchScope ls("k_image_grad", stream);
-            if (light == 4 && uv_grad) k_image_grad<NR_TG_COMBINE, true, 4><<<pgrid, 256, 0, stream>>>(p);
+            if (light == 5 && uv_grad) k_image_grad<NR_TG_COMBINE, true, 5><<<pgrid, 256, 0, stream>>>(p);
+            else if (light == 5) k_image_grad<NR_TG_COMBINE, false, 5><<<pgrid, 256, 0, stream>>>(p);
+            else if (light == 4 && uv_grad) k_image_grad<NR_TG_COMBINE, true, 4><<<pgrid, 256, 0, stream>>>(p);
             else if (light == 4) k_image_grad<NR_TG_COMBINE, false, 4><<<pgrid, 256, 0, stream>>>(p);
             else if (light == 3 && uv_grad) k_image_grad<NR_TG_COMBINE, true, 3><<<pgrid, 256, 0, stream>>>(p);
             else if (light == 3) k_image_grad<NR_TG_COMBINE, false, 3><<<pgrid, 256, 0, stream>>>(p);
@@ -1787,7 +1812,8 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
             return;
         }
         nr_internal::LaunchScope ls("k_texture_grad", stream);
-        if (light == 4) k_texture_grad<NR_TG_COMBINE, 4><<<pgrid, 256, 0, stream>>>(p);
+        if (light == 5) k_texture_grad<NR_TG_COMBINE, 5><<<pgrid, 256, 0, stream>>>(p);
+        else if (light == 4) k_texture_grad<NR_TG_COMBINE, 4><<<pgrid, 256, 0, stream>>>(p);
         else if (light == 3) k_texture_grad<NR_TG_COMBINE, 3><<<pgrid, 256, 0, stream>>>(p);
         else if (smooth) k_texture_grad<NR_TG_COMBINE, 2><<<pgrid, 256, 0, stream>>>(p);
         else k_texture_grad<NR_TG_COMBINE, 0><<<pgrid, 256, 0, stream>>>(p);
@@ -1796,7 +1822,7 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
     auto launch_phong_grad = [&]() {
         if (!phong_grads) return;
         nr_internal::PhongGradLaunch pl{};
-        pl.args = a; pl.src = src; pl.phong = phong; pl.lights = lights;
+        pl.args = a; pl.src = src; pl.phong = phong; pl.lights = lights; pl.sh = sh;
         pl.tex_bstride = (flags & NR_TEX_SHARED) ? 0 : (uv ? img_floats : ncubes * (size_t)ts * ts * ts * 3);
         pl.uv_bstride = p.uv_bstride;
         pl.tex_cmp = p.tex_cmp; pl.tex_val = p.tex_val;
@@ -1905,7 +1931,7 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
 }
 
 extern "C" int nr_b200_backward(const nr_b200_backward_args* args, void* cuda_stream) {
-    return backward_impl(args, nullptr, nullptr, nullptr, nullptr, cuda_stream);
+    return backward_impl(args, nullptr, nullptr, nullptr, nullptr, nullptr, cuda_stream);
 }
 
 extern "C" int nr_b200_backward_corner_light(const nr_b200_backward_args* args, const float* corner_light,
@@ -1914,7 +1940,7 @@ extern "C" int nr_b200_backward_corner_light(const nr_b200_backward_args* args, 
         nr_internal::launch_count() = 0;
         return NR_ERR_INVALID_ARG;
     }
-    return backward_impl(args, corner_light, grad_corner_light, nullptr, nullptr, cuda_stream);
+    return backward_impl(args, corner_light, grad_corner_light, nullptr, nullptr, nullptr, cuda_stream);
 }
 
 extern "C" int nr_b200_backward_phong(const nr_b200_backward_args* args, const nr_b200_phong_args* phong, void* cuda_stream) {
@@ -1922,7 +1948,7 @@ extern "C" int nr_b200_backward_phong(const nr_b200_backward_args* args, const n
         nr_internal::launch_count() = 0;
         return NR_ERR_INVALID_ARG;
     }
-    return backward_impl(args, nullptr, nullptr, phong, nullptr, cuda_stream);
+    return backward_impl(args, nullptr, nullptr, phong, nullptr, nullptr, cuda_stream);
 }
 
 extern "C" int nr_b200_backward_lights(const nr_b200_backward_args* args, const nr_b200_phong_args* phong,
@@ -1931,5 +1957,14 @@ extern "C" int nr_b200_backward_lights(const nr_b200_backward_args* args, const 
         nr_internal::launch_count() = 0;
         return NR_ERR_INVALID_ARG;
     }
-    return backward_impl(args, nullptr, nullptr, phong, lights, cuda_stream);
+    return backward_impl(args, nullptr, nullptr, phong, lights, nullptr, cuda_stream);
+}
+
+extern "C" int nr_b200_backward_sh(const nr_b200_backward_args* args, const nr_b200_phong_args* phong,
+                                   const nr_b200_lights_args* lights, const nr_b200_sh_args* sh, void* cuda_stream) {
+    if (!phong) {
+        nr_internal::launch_count() = 0;
+        return NR_ERR_INVALID_ARG;
+    }
+    return backward_impl(args, nullptr, nullptr, phong, lights, sh, cuda_stream);
 }

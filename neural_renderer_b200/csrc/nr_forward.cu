@@ -78,6 +78,9 @@ constexpr int kOwnTable = 256;         // rows / fragments per pass whose owner 
 #ifndef NR_RESOLVE_LIGHTS_MIN_CTAS
 #define NR_RESOLVE_LIGHTS_MIN_CTAS 4     // Phong with a light set (kLight == 4), every sampler (DESIGN.md section 4h)
 #endif
+#ifndef NR_RESOLVE_SH_MIN_CTAS
+#define NR_RESOLVE_SH_MIN_CTAS 4         // Phong with an SH environment (kLight == 5), every sampler (DESIGN.md section 4i)
+#endif
 constexpr int kResolveTileW = 32, kResolveTileH = 8;  // API pixels per k_resolve CTA (256 threads, 8 x 4 per warp)
 constexpr uint32_t kStageBytes = 32 * 1024;  // shared memory of a k_resolve CTA for staged texture cubes
 
@@ -125,6 +128,9 @@ struct FwdParams {
     const float* lts;
     size_t lt_bstride;   // floats per item in lts (0 with Bl = 1)
     int NL;
+    // SH environment (appended likewise, the kLight == 5 variants, with the set above or NL = 0): sh [Bs,9,3]
+    const float* sh;
+    size_t sh_bstride;   // floats per item in sh (0 with Bs = 1)
 };
 
 // rasterize.py:291-292  xp = (2 * xi + 1 - is) / is evaluated in double and rounded to float.  Both operands are
@@ -470,7 +476,7 @@ __device__ __forceinline__ int face_cube(const FwdParams& p, int fn, bool& rev) 
 // kUV: bilinear sample of the texture image at the pixel's perspective-correct UV instead of the ts^3 cube; kMip:
 // trilinear sample of its mip pyramid at the pixel's level of detail.  kLight: 0 = unlit, 1 = face_light multiplies every
 // texel, 2 = corner_light interpolated to the pixel multiplies the unlit sample, 3 = Phong shading of the unlit sample, 4 = the
-// same with a light set
+// same with a light set, 5 = the same with an SH environment (and a light set or none)
 template <int kLight, bool kUV = false, bool kMip = false>
 __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigned long long key, int xi, int yi, float bgr,
                                               float bgg, float bgb) {
@@ -548,6 +554,18 @@ __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigne
             nr::phong_lights_rgb(E, pos, prm, lts, p.NL, s, rgb);
             o.r = rgb[0]; o.g = rgb[1]; o.b = rgb[2];
         }
+        if constexpr (kLight == 5) {  // Phong with an SH environment: E_c joins L_c after the set's diffuse terms
+            float l[3], rgb[3], pos[3];
+            nr::perspective_weights(w, zp, cc.y, cc.z, cc.w, l);
+            const float* prm = p.phong_prm + (size_t)b * p.prm_bstride;
+            const float* lts = p.lts + (size_t)b * p.lt_bstride;
+            nr::PhongEval E;
+            nr::phong_sh_at(p.phong_cs + ((size_t)b * p.cs_bstride + fn) * 18, l, prm, lts, p.NL, p.sh + (size_t)b * p.sh_bstride,
+                            E, pos);
+            const float s[3] = {o.r, o.g, o.b};
+            nr::phong_lights_rgb(E, pos, prm, lts, p.NL, s, rgb);
+            o.r = rgb[0]; o.g = rgb[1]; o.b = rgb[2];
+        }
     }
     return o;
 }
@@ -570,7 +588,7 @@ __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigne
 // kTex == 2 (NR_TEX_UV): the direct variants with the texture-image sampler (shade_pixel<kLit, true>), same tile map.
 // kTex == 3 (NR_TEX_UV | NR_TEX_MIPMAP): the same with the trilinear pyramid sampler (shade_pixel<kLit, true, true>).
 template <bool kAA, int kTex, int kLight>
-__global__ void __launch_bounds__(256, kLight == 4 ? NR_RESOLVE_LIGHTS_MIN_CTAS : kLight == 3 ? NR_RESOLVE_PHONG_MIN_CTAS : kTex == 3 ? NR_RESOLVE_MIP_MIN_CTAS : (kLight == 2 ? (kAA ? NR_RESOLVE_SMOOTH_AA_MIN_CTAS : NR_RESOLVE_SMOOTH_MIN_CTAS) : (kAA ? 5 : NR_RESOLVE_MIN_CTAS))) k_resolve(const __grid_constant__ FwdParams p, int nslots) {
+__global__ void __launch_bounds__(256, kLight == 5 ? NR_RESOLVE_SH_MIN_CTAS : kLight == 4 ? NR_RESOLVE_LIGHTS_MIN_CTAS : kLight == 3 ? NR_RESOLVE_PHONG_MIN_CTAS : kTex == 3 ? NR_RESOLVE_MIP_MIN_CTAS : (kLight == 2 ? (kAA ? NR_RESOLVE_SMOOTH_AA_MIN_CTAS : NR_RESOLVE_SMOOTH_MIN_CTAS) : (kAA ? 5 : NR_RESOLVE_MIN_CTAS))) k_resolve(const __grid_constant__ FwdParams p, int nslots) {
     constexpr bool kStage = kTex == 1;  // kTex: 0 = every texel straight from global memory, 1 = cubes staged with cp.async.bulk
     constexpr bool kUV = kTex >= 2;     //       2 = texture image through per-corner UVs, 3 = its mip pyramid
     constexpr bool kMip = kTex == 3;
@@ -743,9 +761,10 @@ extern "C" size_t nr_b200_forward_workspace_bytes(int32_t B, int32_t F, int32_t 
     return fwd_layout(B, F, S).total;
 }
 
-// nr_b200_forward (phong, lights NULL), nr_b200_forward_phong (lights NULL) and nr_b200_forward_lights
+// nr_b200_forward (phong, lights, sh NULL), nr_b200_forward_phong (lights, sh NULL), nr_b200_forward_lights (sh NULL) and
+// nr_b200_forward_sh
 static int forward_impl(const nr_b200_forward_args* args, const nr_b200_phong_args* phong, const nr_b200_lights_args* lights,
-                        void* cuda_stream) {
+                        const nr_b200_sh_args* sh, void* cuda_stream) {
     nr_internal::launch_count() = 0;
     // Two layouts: the full struct, and the ABI-4 struct from before corner_light (which then reads as NULL).  Only the
     // caller's struct_size bytes are read.
@@ -778,6 +797,7 @@ static int forward_impl(const nr_b200_forward_args* args, const nr_b200_phong_ar
     if (phong && (!(flags & NR_RETURN_RGB) || a->face_light || smooth || !nr_internal::phong_args_ok(phong, B)))
         return NR_ERR_INVALID_ARG;
     if (lights && !nr_internal::lights_args_ok(lights, B)) return NR_ERR_INVALID_ARG;
+    if (sh && !nr_internal::sh_args_ok(sh, B)) return NR_ERR_INVALID_ARG;
     if (lights && lights->num_lights == 0) lights = nullptr;  // the Phong call exactly
     if ((flags & NR_ANTI_ALIASING) && (S & 1)) return NR_ERR_INVALID_ARG;
     if (S > 32767 || B > 65535) return NR_ERR_UNSUPPORTED;  // 32-bit pixel offsets; batch = grid.z of the resolve pass
@@ -809,6 +829,10 @@ static int forward_impl(const nr_b200_forward_args* args, const nr_b200_phong_ar
     if (lights) {
         p.lts = lights->lights; p.NL = lights->num_lights;
         p.lt_bstride = lights->lights_batch == 1 ? 0 : (size_t)lights->num_lights * 12;
+    }
+    if (sh) {
+        p.sh = sh->sh;
+        p.sh_bstride = sh->sh_batch == 1 ? 0 : 27;
     }
     p.big_cnt = (int*)(wsb + L.off_cnt);
     p.work_next = p.big_cnt + B;
@@ -877,7 +901,7 @@ static int forward_impl(const nr_b200_forward_args* args, const nr_b200_phong_ar
         // Staging whole cubes with cp.async.bulk needs 16-byte aligned, 16-byte sized cubes; up to kStageBytes of
         // shared memory per CTA hold the cubes of the row's runs (the rest of the runs read global memory)
         const bool aa = (flags & NR_ANTI_ALIASING) != 0;
-        const int light = lights ? 4 : phong ? 3 : (smooth ? 2 : (p.face_light != nullptr ? 1 : 0));
+        const int light = sh ? 5 : lights ? 4 : phong ? 3 : (smooth ? 2 : (p.face_light != nullptr ? 1 : 0));
         const uint32_t cube_bytes = (flags & NR_RETURN_RGB) ? (uint32_t)(ts * ts * ts) * 12u : 0u;
         const bool stage = !uv && !smooth && !phong && (flags & NR_FWD_STAGE_TEXTURES) && !aa && (flags & NR_RETURN_RGB) && (cube_bytes % 16u) == 0 &&
                            cube_bytes <= kStageBytes / 8 && ((uintptr_t)a->textures & 15) == 0;
@@ -895,7 +919,8 @@ static int forward_impl(const nr_b200_forward_args* args, const nr_b200_phong_ar
     } while (0)
 #define NR_RESOLVE_LIT(AA, TEX)                                                                    \
     do {                                                                                            \
-        if (light == 4) NR_RESOLVE(AA, TEX, 4);                                                     \
+        if (light == 5) NR_RESOLVE(AA, TEX, 5);                                                     \
+        else if (light == 4) NR_RESOLVE(AA, TEX, 4);                                                \
         else if (light == 3) NR_RESOLVE(AA, TEX, 3);                                                \
         else if (light == 2) NR_RESOLVE(AA, TEX, 2);                                                \
         else if (light == 1) NR_RESOLVE(AA, TEX, 1);                                                \
@@ -920,7 +945,7 @@ static int forward_impl(const nr_b200_forward_args* args, const nr_b200_phong_ar
 }
 
 extern "C" int nr_b200_forward(const nr_b200_forward_args* args, void* cuda_stream) {
-    return forward_impl(args, nullptr, nullptr, cuda_stream);
+    return forward_impl(args, nullptr, nullptr, nullptr, cuda_stream);
 }
 
 extern "C" int nr_b200_forward_phong(const nr_b200_forward_args* args, const nr_b200_phong_args* phong, void* cuda_stream) {
@@ -928,7 +953,7 @@ extern "C" int nr_b200_forward_phong(const nr_b200_forward_args* args, const nr_
         nr_internal::launch_count() = 0;
         return NR_ERR_INVALID_ARG;
     }
-    return forward_impl(args, phong, nullptr, cuda_stream);
+    return forward_impl(args, phong, nullptr, nullptr, cuda_stream);
 }
 
 extern "C" int nr_b200_forward_lights(const nr_b200_forward_args* args, const nr_b200_phong_args* phong,
@@ -937,5 +962,14 @@ extern "C" int nr_b200_forward_lights(const nr_b200_forward_args* args, const nr
         nr_internal::launch_count() = 0;
         return NR_ERR_INVALID_ARG;
     }
-    return forward_impl(args, phong, lights, cuda_stream);
+    return forward_impl(args, phong, lights, nullptr, cuda_stream);
+}
+
+extern "C" int nr_b200_forward_sh(const nr_b200_forward_args* args, const nr_b200_phong_args* phong,
+                                  const nr_b200_lights_args* lights, const nr_b200_sh_args* sh, void* cuda_stream) {
+    if (!phong) {
+        nr_internal::launch_count() = 0;
+        return NR_ERR_INVALID_ARG;
+    }
+    return forward_impl(args, phong, lights, sh, cuda_stream);
 }

@@ -61,6 +61,11 @@ inline bool lights_args_ok(const nr_b200_lights_args* ls, int B) {
            (ls->lights || ls->num_lights == 0) && (ls->lights_batch == 1 || ls->lights_batch == B);
 }
 
+// the same for an SH environment (nr_b200_sh_args)
+inline bool sh_args_ok(const nr_b200_sh_args* sh, int B) {
+    return sh->struct_size == sizeof(nr_b200_sh_args) && sh->sh && (sh->sh_batch == 1 || sh->sh_batch == B);
+}
+
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) is issued once per (kernel instantiation, device, size high-water
 // mark) instead of on every launch: `slot` is a function-local static of the launching template.
 struct SmemOptIn {

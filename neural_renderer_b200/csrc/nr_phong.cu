@@ -1,7 +1,7 @@
-// nr_phong.cu -- the Phong-shading gradients of nr_b200_backward_phong and nr_b200_backward_lights (include/nr_b200.h,
-// nr_b200_phong_args, nr_b200_lights_args).
+// nr_phong.cu -- the Phong-shading gradients of nr_b200_backward_phong, nr_b200_backward_lights and nr_b200_backward_sh
+// (include/nr_b200.h, nr_b200_phong_args, nr_b200_lights_args, nr_b200_sh_args).
 //
-//   k_phong_grad<kTex, kIdx, kLights>   one thread per raster pixel, modelled on k_interior_grad.  The winner's perspective weights
+//   k_phong_grad<kTex, kIdx, kLights, kSH>   one thread per raster pixel, modelled on k_interior_grad.  The winner's perspective weights
 //                   l_k and the unlit sample s are recomputed with the forward's device helpers (the depth map gives zp;
 //                   per-face cubes read the sampler depths NR_TEX_Z_BATCH0 selects), nr::phong_at evaluates the forward's
 //                   expression and nr::phong_grad its derivative.  The 18 corner floats l_k (d loss / d n, d loss / d p) go
@@ -13,6 +13,11 @@
 //                   accumulators across the loop over the lights (nr::phong_light_grad); each light's 10 record floats
 //                   are summed over the warp into shared memory, and after the loop over the CTA before 10 atomics per
 //                   light per CTA, so no NL x 10 register array exists.
+//                   kSH (an SH environment): with kLights, after the loop over the lights d E / d nh joins the
+//                   d loss / d nh accumulator before the normalisation chain; without, d E / d nh goes through that chain
+//                   on its own and is added to light 0's normal gradient.  The 27 floats Y_k g_c s_c are summed over the
+//                   warp one at a time into shared memory, then over the CTA before 27 atomics per CTA
+//                   (sh_grad_reduce), so no 27-float register array exists.
 //
 // It belongs to the texture half of the backward: the texture-gradient kernels (K6, k_image_grad) only need the pixel's
 // L_c, and keeping the 34 gradient floats out of them keeps their register budgets (DESIGN.md section 4g).
@@ -52,9 +57,33 @@ struct PhongParams {
     float* grad_lts;
     size_t lt_bstride;      // floats per item in lts (0 with Bl = 1)
     int NL;
+    // kSH: sh [Bs,9,3] and its gradient (or nullptr)
+    const float* sh;
+    float* grad_sh;
+    size_t sh_bstride;      // floats per item in sh (0 with Bs = 1)
 };
 
-template <int kTex, bool kIdx, bool kLights>
+// kSH: the 27 floats Y_k w_c of grad_sh summed over the warp one at a time into shared memory, then over the CTA before 27
+// atomics into `o` (item b's [9,3] slot, or slot 0 with Bs = 1).  Every thread of the CTA calls it (0 off the mesh).
+__device__ __forceinline__ void sh_grad_reduce(const float Y[9], const float ws[3], float* o, int lane, int warp) {
+    __shared__ float s_sh[8][27];
+#pragma unroll
+    for (int t = 0; t < 27; t++) {
+        float v = __fmul_rn(Y[t / 3], ws[t % 3]);
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+        if (lane == 0) s_sh[warp][t] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x < 27) {
+        float v = 0.0f;
+        const int nw = (int)(blockDim.x >> 5);
+        for (int w = 0; w < nw; w++) v += s_sh[w][threadIdx.x];
+        atomicAdd(o + threadIdx.x, v);
+    }
+}
+
+template <int kTex, bool kIdx, bool kLights, bool kSH>
 __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ PhongParams p) {
     __shared__ float s_prm[8][16];
     const int S = p.S;
@@ -72,6 +101,14 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
     // kLights: what the loop over the lights needs of the covered pixel below
     nr::PhongEval xE;
     float xg[3], xs[3], xlam[3], xpos[3], xgn[3], xgp[3];
+    // kSH without kLights: Y_k(nh) and g_c s_c of the covered pixel, 0 elsewhere
+    float shY[9], shw[3];
+    if constexpr (kSH && !kLights) {
+#pragma unroll
+        for (int k = 0; k < 9; k++) shY[k] = 0.0f;
+#pragma unroll
+        for (int k = 0; k < 3; k++) shw[k] = 0.0f;
+    }
     if (fn >= 0) {
         const int r = (int)(i / S), c = (int)(i % S);
         const bool aa = p.aa != 0;
@@ -149,6 +186,16 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
                 xg[k] = g[k]; xs[k] = s[k]; xlam[k] = lam[k]; xgn[k] = gn[k]; xgp[k] = gp[k];
             }
         } else {
+            if constexpr (kSH) {  // no light set: d E / d nh through the normalisation chain on its own (it is linear)
+                float gnh[3] = {0.0f, 0.0f, 0.0f}, t[3];
+#pragma unroll
+                for (int k = 0; k < 3; k++) shw[k] = __fmul_rn(g[k], s[k]);
+                nr::sh_basis(E.nh, shY);
+                nr::sh_grad_nh(p.sh + (size_t)b * p.sh_bstride, E.nh, shw, gnh);
+                nr::normalize_eps_grad(E.n, E.n_len, gnh, t);
+#pragma unroll
+                for (int k = 0; k < 3; k++) gn[k] = __fadd_rn(gn[k], t[k]);
+            }
 #pragma unroll
             for (int k = 0; k < 3; k++)
 #pragma unroll
@@ -179,6 +226,21 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
                 }
             }
         }
+        if constexpr (kSH) {  // before the normalisation chain: d E / d nh joins gnh
+            float Y[9], ws[3];             // Y_k(nh) and g_c s_c (d rgb_c / d L_c = s_c); 0 off the mesh
+            if (fn >= 0) {
+#pragma unroll
+                for (int k = 0; k < 3; k++) ws[k] = __fmul_rn(xg[k], xs[k]);
+                nr::sh_basis(xE.nh, Y);
+                nr::sh_grad_nh(p.sh + (size_t)b * p.sh_bstride, xE.nh, ws, gnh);
+            } else {
+#pragma unroll
+                for (int k = 0; k < 9; k++) Y[k] = 0.0f;
+#pragma unroll
+                for (int k = 0; k < 3; k++) ws[k] = 0.0f;
+            }
+            if (p.grad_sh) sh_grad_reduce(Y, ws, p.grad_sh + (size_t)b * p.sh_bstride, lane, warp);  // uniform
+        }
         if (fn >= 0) {
             nr::phong_lights_grad_end(xE, gnh, gvh, gsig, xgn, xgp, gprm);
 #pragma unroll
@@ -198,6 +260,9 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
                 atomicAdd(p.grad_lts + (size_t)b * p.lt_bstride + (size_t)(t / 10) * 12 + t % 10, v);
             }
         }
+    }
+    if constexpr (kSH && !kLights) {
+        if (p.grad_sh) sh_grad_reduce(shY, shw, p.grad_sh + (size_t)b * p.sh_bstride, lane, warp);  // uniform
     }
     if (p.grad_cs) {  // uniform
         // the segmented run reduction of k_depth_grad over 18 floats, then one set of atomics per run
@@ -241,10 +306,14 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
 
 template <int kTex>
 void launch_t(const PhongParams& p, bool idx, dim3 grid, cudaStream_t s) {
-    if (p.NL > 0 && idx) k_phong_grad<kTex, true, true><<<grid, 256, 0, s>>>(p);
-    else if (p.NL > 0) k_phong_grad<kTex, false, true><<<grid, 256, 0, s>>>(p);
-    else if (idx) k_phong_grad<kTex, true, false><<<grid, 256, 0, s>>>(p);
-    else k_phong_grad<kTex, false, false><<<grid, 256, 0, s>>>(p);
+    if (p.sh && p.NL > 0 && idx) k_phong_grad<kTex, true, true, true><<<grid, 256, 0, s>>>(p);
+    else if (p.sh && p.NL > 0) k_phong_grad<kTex, false, true, true><<<grid, 256, 0, s>>>(p);
+    else if (p.sh && idx) k_phong_grad<kTex, true, false, true><<<grid, 256, 0, s>>>(p);
+    else if (p.sh) k_phong_grad<kTex, false, false, true><<<grid, 256, 0, s>>>(p);
+    else if (p.NL > 0 && idx) k_phong_grad<kTex, true, true, false><<<grid, 256, 0, s>>>(p);
+    else if (p.NL > 0) k_phong_grad<kTex, false, true, false><<<grid, 256, 0, s>>>(p);
+    else if (idx) k_phong_grad<kTex, true, false, false><<<grid, 256, 0, s>>>(p);
+    else k_phong_grad<kTex, false, false, false><<<grid, 256, 0, s>>>(p);
 }
 
 }  // namespace
@@ -275,6 +344,10 @@ void launch_phong_grad(const PhongGradLaunch& L, cudaStream_t stream) {
     if (L.lights) {
         p.lts = L.lights->lights; p.grad_lts = L.lights->grad_lights; p.NL = L.lights->num_lights;
         p.lt_bstride = L.lights->lights_batch == 1 ? 0 : (size_t)p.NL * 12;
+    }
+    if (L.sh) {
+        p.sh = L.sh->sh; p.grad_sh = L.sh->grad_sh;
+        p.sh_bstride = L.sh->sh_batch == 1 ? 0 : 27;
     }
     const bool idx = (flags & NR_FACES_INDEXED) != 0;
     const dim3 grid((unsigned)(((size_t)p.S * p.S + 255) / 256), a->batch_size);

@@ -14,6 +14,7 @@ struct PhongGradLaunch {
     const nr_b200_backward_args* args;  // the checked call (flags, maps, grad_rgb, textures, face_uvs)
     const nr_b200_phong_args* phong;    // the checked Phong inputs and gradient outputs
     const nr_b200_lights_args* lights;  // the checked light set (NL > 0), or nullptr
+    const nr_b200_sh_args* sh;          // the checked SH environment, or nullptr
     nr::FaceSrc src;
     size_t tex_bstride;       // floats per item in `textures` (0 = shared)
     uint32_t uv_bstride;      // floats per item in face_uvs (0 = shared)

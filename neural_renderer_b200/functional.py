@@ -795,3 +795,45 @@ def light_set(*records):
     if any(r.shape[0] not in (1, n) for r in recs):
         raise ValueError("light records must hold one entry or one per batch item")
     return torch.stack([r.expand(n, -1) for r in recs], dim=1)
+
+
+# second-order real SH constants of include/nr_b200.h (nr_b200_sh_args): C0 = 1/(2 sqrt(pi)), C1 = sqrt(3/(4 pi)),
+# C2 = sqrt(15/(4 pi)), C3 = sqrt(5/(16 pi)), C4 = sqrt(15/(16 pi))
+SH_C = (0.5 / math.sqrt(math.pi), math.sqrt(3.0 / (4.0 * math.pi)), math.sqrt(15.0 / (4.0 * math.pi)),
+        math.sqrt(5.0 / (16.0 * math.pi)), math.sqrt(15.0 / (16.0 * math.pi)))
+
+
+def _sh_basis_torch(d):
+    """The 9 real SH basis functions of include/nr_b200.h at directions d [...,3] -> [...,9] (d used as given)."""
+    x, y, z = d.unbind(-1)
+    c0, c1, c2, c3, c4 = SH_C
+    return torch.stack([torch.full_like(x, c0), c1 * y, c1 * z, c1 * x, c2 * x * y, c2 * y * z, c3 * (3 * z * z - 1),
+                        c2 * x * z, c4 * (x * x - y * y)], dim=-1)
+
+
+def sh_from_environment_map(envmap):
+    """Irradiance-ready second-order SH coefficients [1|B,9,3] (rasterize(..., environment_sh=...),
+    Renderer.environment_sh) from a lat-long HDR environment map [He,We,3] / [1|B,He,We,3] of radiance.
+
+    Convention: row 0 is the top.  Texel (i, j) is the direction omega = (sin t sin p, cos t, sin t cos p) with
+    t_i = pi (i + 1/2) / He measured from +y and p_j = 2 pi (j + 1/2) / We, in the frame of the shading normals, and
+    covers the solid angle dOmega_i = sin t_i (pi / He) (2 pi / We) (the midpoint rule).  Then
+        S[k][c] = a_l sum_{i,j} env[i,j,c] Y_k(omega_ij) dOmega_i,   a_0 = 1, a_1 = 2/3, a_2 = 1/4
+    (a_l = A_l / pi, the clamped-cosine convolution of Ramamoorthi & Hanrahan 2001, divided by pi), so a uniform map of
+    radiance r gives S = (r / C0, 0, ...) and renders a white albedo as r.  Pure torch in the map's dtype and device,
+    differentiable with respect to the map; rotate the map (or the geometry) to rotate the environment."""
+    if not isinstance(envmap, torch.Tensor) or not envmap.is_floating_point():
+        raise TypeError("envmap must be a floating point torch.Tensor")
+    env = envmap[None] if envmap.dim() == 3 else envmap
+    if env.dim() != 4 or env.shape[-1] != 3 or env.shape[1] < 1 or env.shape[2] < 1:
+        raise ValueError("envmap must have shape [He, We, 3] or [batch size, He, We, 3], got %s" % (tuple(envmap.shape),))
+    He, We = int(env.shape[1]), int(env.shape[2])
+    kw = dict(dtype=env.dtype, device=env.device)
+    t = math.pi * (torch.arange(He, **kw) + 0.5) / He
+    p = 2.0 * math.pi * (torch.arange(We, **kw) + 0.5) / We
+    st = torch.sin(t)[:, None]
+    omega = torch.stack([st * torch.sin(p)[None, :], torch.cos(t)[:, None].expand(He, We), st * torch.cos(p)[None, :]], -1)
+    dw = torch.sin(t) * (math.pi / He) * (2.0 * math.pi / We)  # [He]
+    Y = _sh_basis_torch(omega) * dw[:, None, None]  # [He,We,9]
+    a = torch.tensor([1.0] + [2.0 / 3.0] * 3 + [0.25] * 5, **kw)
+    return torch.einsum('bhwc,hwk->bkc', env, Y) * a[None, :, None]

@@ -61,7 +61,7 @@ def _ptr(t):
 
 
 def _check_inputs(faces, textures, return_rgb, face_light=None, textures_fill_back=False, vertices=None, face_uvs=None,
-                  corner_light=None, corner_shading=None, shading_params=None, lights=None):
+                  corner_light=None, corner_shading=None, shading_params=None, lights=None, environment_sh=None):
     # rasterize.py:66-90 (chainer type_check) -> TypeError / ValueError with the same conditions
     if not isinstance(faces, torch.Tensor):
         raise TypeError("faces must be a torch.Tensor")
@@ -105,6 +105,8 @@ def _check_inputs(faces, textures, return_rgb, face_light=None, textures_fill_ba
                              "faces, got %s" % (tuple(textures.shape),))
     if lights is not None:
         _check_lights(lights, corner_shading, batch_size)
+    if environment_sh is not None:
+        _check_environment_sh(environment_sh, corner_shading, return_rgb, batch_size)
     if corner_shading is not None or shading_params is not None:
         _check_phong_inputs(corner_shading, shading_params, face_light, corner_light, return_rgb, batch_size, num_faces)
     if return_rgb and face_light is not None:
@@ -159,6 +161,20 @@ def _check_lights(lights, corner_shading, batch_size):
         raise ValueError("lights must have shape [num lights, 12] or [batch size, num lights, 12] with at most 8 lights, "
                          "got %s" % (tuple(lights.shape),))
     if not lights.is_cuda:
+        raise NotImplementedError("neural_renderer_b200 has no CPU implementation (inputs must be CUDA tensors)")
+
+
+def _check_environment_sh(sh, corner_shading, return_rgb, batch_size):
+    # irradiance-ready SH coefficients [9,3] / [1|B,9,3] on top of Phong shading's lights
+    if corner_shading is None:
+        raise ValueError("environment_sh needs Phong shading (corner_shading / shading_params)")
+    if not return_rgb:
+        raise ValueError("environment_sh lights the RGB image: it needs return_rgb")
+    if not isinstance(sh, torch.Tensor) or not sh.is_floating_point():
+        raise TypeError("environment_sh must be a floating point torch.Tensor")
+    if not ((sh.dim() == 2 or (sh.dim() == 3 and sh.shape[0] in (1, batch_size))) and tuple(sh.shape[-2:]) == (9, 3)):
+        raise ValueError("environment_sh must have shape [9, 3] or [batch size, 9, 3], got %s" % (tuple(sh.shape),))
+    if not sh.is_cuda:
         raise NotImplementedError("neural_renderer_b200 has no CPU implementation (inputs must be CUDA tensors)")
 
 
@@ -252,7 +268,7 @@ class _RasterizeFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, geom, textures, face_light, cfg, indices, face_uvs=None, corner_light=None, corner_shading=None,
-                shading_params=None, lights=None):
+                shading_params=None, lights=None, environment_sh=None):
         lib = _lib.load()
         dev = geom.device
         geom_c = geom.detach().contiguous()
@@ -263,6 +279,7 @@ class _RasterizeFunction(torch.autograd.Function):
         cs_c = corner_shading.detach().to(torch.float32).contiguous() if corner_shading is not None else None
         sp_c = shading_params.detach().to(torch.float32).contiguous() if shading_params is not None else None
         lt_c = lights.detach().to(torch.float32).contiguous() if lights is not None else None  # [Bl,NL,12], NL >= 1
+        sh_c = environment_sh.detach().to(torch.float32).contiguous() if environment_sh is not None else None  # [Bs,9,3]
         flags = cfg.flags
         if indices is not None:
             B, Nv = geom_c.shape[:2]
@@ -327,6 +344,11 @@ class _RasterizeFunction(torch.autograd.Function):
             a.corner_light = _ptr(corner_c)
             if cs_c is None:
                 _lib.check(lib.nr_b200_forward(ctypes.byref(a), _stream_ptr(dev)))
+            elif sh_c is not None:
+                ph, sa = _phong_args(cs_c, sp_c), _sh_args(sh_c)
+                la = _lights_args(lt_c) if lt_c is not None else None
+                _lib.check(lib.nr_b200_forward_sh(ctypes.byref(a), ctypes.byref(ph), ctypes.byref(la) if la is not None else None,
+                                                  ctypes.byref(sa), _stream_ptr(dev)))
             elif lt_c is not None:
                 ph, la = _phong_args(cs_c, sp_c), _lights_args(lt_c)
                 _lib.check(lib.nr_b200_forward_lights(ctypes.byref(a), ctypes.byref(ph), ctypes.byref(la), _stream_ptr(dev)))
@@ -346,12 +368,13 @@ class _RasterizeFunction(torch.autograd.Function):
         ctx.need_cs_grad = cs_c is not None and ctx.needs_input_grad[7]
         ctx.need_sp_grad = sp_c is not None and ctx.needs_input_grad[8]
         ctx.need_lt_grad = lt_c is not None and ctx.needs_input_grad[9]
+        ctx.need_sh_grad = sh_c is not None and ctx.needs_input_grad[10]
         # interior_gradient: the backward differentiates the sampler, so it reads the textures (and face_uvs / corner_light)
         ctx.interior = cfg.interior and want_rgb and ctx.needs_input_grad[0]
         need_tex = need_light_grad or ctx.need_uv_grad or ctx.need_corner_grad or ctx.interior or ctx.need_cs_grad or \
-            ctx.need_sp_grad or ctx.need_lt_grad
+            ctx.need_sp_grad or ctx.need_lt_grad or ctx.need_sh_grad
         ctx.save_for_backward(geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c if need_tex else None, indices, uv_c, corner_c,
-                              cs_c, sp_c, lt_c)
+                              cs_c, sp_c, lt_c, sh_c)
         if cfg.aa:
             rgb_o, alpha_o, depth_o = out_rgb, out_alpha, out_depth
         else:
@@ -364,7 +387,7 @@ class _RasterizeFunction(torch.autograd.Function):
         lib = _lib.load()
         cfg = ctx.cfg
         flags = ctx.flags | (_lib.NR_GRAD_INTERIOR if ctx.interior else 0)
-        geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c, indices, uv_c, corner_c, cs_c, sp_c, lt_c = ctx.saved_tensors
+        geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c, indices, uv_c, corner_c, cs_c, sp_c, lt_c, sh_c = ctx.saved_tensors
         dev = geom_c.device
         B, F = geom_c.shape[0], ctx.F
         want_rgb = bool(flags & _lib.NR_RETURN_RGB)
@@ -388,6 +411,8 @@ class _RasterizeFunction(torch.autograd.Function):
             ph = _phong_args(cs_c, sp_c, grad_cs, grad_sp) if cs_c is not None else None
             grad_lt = torch.empty_like(lt_c) if ctx.need_lt_grad else None
             la = _lights_args(lt_c, grad_lt) if lt_c is not None else None
+            grad_sh = torch.empty_like(sh_c) if ctx.need_sh_grad else None
+            sa = _sh_args(sh_c, grad_sh) if sh_c is not None else None
             ws_bytes = lib.nr_b200_backward_workspace_bytes(B, F, cfg.S, ctx.ts, flags)
             ws = torch.empty((max(ws_bytes, 16),), dtype=torch.uint8, device=dev)
             a = _lib.BackwardArgs()
@@ -410,6 +435,9 @@ class _RasterizeFunction(torch.autograd.Function):
             hook = _TEXTURE_GRAD_HOOK if (want_rgb and g_rgb is not None) else None
 
             def call():
+                if sa is not None:  # SH environment (with or without a light set): grad_sh is filled by the texture half
+                    return lib.nr_b200_backward_sh(ctypes.byref(a), ctypes.byref(ph), ctypes.byref(la) if la is not None else None,
+                                                   ctypes.byref(sa), _stream_ptr(dev))
                 if la is not None:  # light set: grad_lights too is filled by the texture half
                     return lib.nr_b200_backward_lights(ctypes.byref(a), ctypes.byref(ph), ctypes.byref(la), _stream_ptr(dev))
                 if ph is not None:  # Phong: grad_corner_shading / grad_params are filled by the texture half
@@ -432,7 +460,7 @@ class _RasterizeFunction(torch.autograd.Function):
                 _lib.check(call())
                 if pending is not None:
                     pending.wait()
-        return grad_geom, grad_textures, grad_light, None, None, grad_uvs, grad_corner, grad_cs, grad_sp, grad_lt
+        return grad_geom, grad_textures, grad_light, None, None, grad_uvs, grad_corner, grad_cs, grad_sp, grad_lt, grad_sh
 
 
 def _phong_args(cs_c, sp_c, grad_cs=None, grad_sp=None):
@@ -450,6 +478,14 @@ def _lights_args(lt_c, grad_lt=None):
     la.lights_batch, la.num_lights = int(lt_c.shape[0]), int(lt_c.shape[1])
     la.lights, la.grad_lights = _ptr(lt_c), _ptr(grad_lt)
     return la
+
+
+def _sh_args(sh_c, grad_sh=None):
+    sa = _lib.ShArgs()
+    sa.struct_size = ctypes.sizeof(_lib.ShArgs)
+    sa.sh_batch = int(sh_c.shape[0])
+    sa.sh, sa.grad_sh = _ptr(sh_c), _ptr(grad_sh)
+    return sa
 
 
 class _MipPyramid(torch.autograd.Function):
@@ -487,7 +523,7 @@ TEXTURE_FILTERS = ('bilinear', 'trilinear')
 def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_color, return_rgb, return_alpha,
          return_depth, face_light=None, textures_fill_back=False, vertices=None, reference_exact=None, face_uvs=None,
          texture_filter='bilinear', corner_light=None, interior_gradient=False, corner_shading=None, shading_params=None,
-         lights=None):
+         lights=None, environment_sh=None):
     if (corner_shading is not None or shading_params is not None) and interior_gradient:
         raise ValueError("interior_gradient=True is not supported with Phong shading (corner_shading / shading_params): no "
                          "vertex gradient flows through the interpolation of the per-pixel normal and position")
@@ -502,7 +538,7 @@ def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_
                          "than one item: the reference-exact sampler reads the depths of item 0 for every item, so its "
                          "derivative would cross items.  Pass reference_exact=False (or set_reference_exact(False))")
     _check_inputs(faces, textures, return_rgb, face_light, textures_fill_back, vertices, face_uvs, corner_light,
-                  corner_shading, shading_params, lights)
+                  corner_shading, shading_params, lights, environment_sh)
     phong = corner_shading is not None
     indices = None
     if vertices is not None:
@@ -545,6 +581,12 @@ def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_
                     lights = lights[:1]  # an expanded shared set (Bl = 1)
                 if lights.shape[1] == 0:
                     lights = None  # no extra light: Phong exactly
+            if environment_sh is not None:
+                sh = environment_sh.float() if environment_sh.dtype != torch.float32 else environment_sh
+                sh = sh[None] if sh.dim() == 2 else sh
+                if sh.shape[0] == batch_size > 1 and sh.stride(0) == 0:
+                    sh = sh[:1]  # an expanded shared environment (Bs = 1)
+                environment_sh = sh
     cfg = _make_config(image_size, anti_aliasing, near, far, eps, background_color, return_rgb, return_alpha,
                        return_depth, geom.device, batch_size, reference_exact)
     if return_rgb and textures_fill_back:
@@ -560,7 +602,8 @@ def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_
         textures = _MipPyramid.apply(textures)
     return _RasterizeFunction.apply(geom, textures if return_rgb else None, face_light if return_rgb else None, cfg,
                                     indices, face_uvs, corner_light, corner_shading if return_rgb else None,
-                                    shading_params if return_rgb else None, lights if return_rgb else None)
+                                    shading_params if return_rgb else None, lights if return_rgb else None,
+                                    environment_sh if return_rgb else None)
 
 
 def rasterize_rgbad(
@@ -587,6 +630,7 @@ def rasterize_rgbad(
         corner_shading=None,
         shading_params=None,
         lights=None,
+        environment_sh=None,
 ):
     """Generate RGB, alpha channel, and depth images from faces and textures (for RGB).  rasterize.py:900-977.
 
@@ -646,12 +690,19 @@ def rasterize_rgbad(
                               light's direction and attenuation a = 1 / (1 + falloff r^2) evaluated at every pixel
                               (include/nr_b200.h, nr_b200_lights_args).  Only with corner_shading / shading_params;
                               receives gradients (a batch of 1 gets the sum over the items).
+      environment_sh [9,3] / [1|B,9,3]   Phong shading lit by an environment as well: second-order spherical-harmonic
+                              coefficients (k major, channel minor; F.sh_from_environment_map makes them from a lat-long
+                              map), irradiance-ready (S = (1/C0, 0, ...) gives irradiance 1).  The irradiance
+                              E_c = sum_k S[k][c] Y_k(n) at the pixel's normal is added to the light of the sample after
+                              every diffuse term, unclamped (include/nr_b200.h, nr_b200_sh_args).  Only with
+                              corner_shading / shading_params; composes with `lights`; receives gradients (a batch of 1
+                              gets the sum over the items).
     `textures` with batch size 1 (or an expanded stride-0 batch) while the geometry batch is larger = one texture set
     shared by every item (a mesh seen from B viewpoints, mesh.py:29-34); its gradient is the sum over the items."""
     rgb, alpha, depth, _, _ = _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_color,
                                    return_rgb, return_alpha, return_depth, face_light, textures_fill_back, vertices,
                                    reference_exact, face_uvs, texture_filter, corner_light, interior_gradient,
-                                   corner_shading, shading_params, lights)
+                                   corner_shading, shading_params, lights, environment_sh)
     return {
         'rgb': rgb if return_rgb else None,
         'alpha': alpha if return_alpha else None,
@@ -680,6 +731,7 @@ def rasterize(
         corner_shading=None,
         shading_params=None,
         lights=None,
+        environment_sh=None,
 ):
     """RGB images [B,3,H,W] from faces and textures.  rasterize.py:980-1008 (keyword-only extras: rasterize_rgbad; in
     texture-image mode both the image and face_uvs receive gradients)."""
@@ -688,7 +740,7 @@ def rasterize(
         face_light=face_light, textures_fill_back=textures_fill_back, vertices=vertices,
         reference_exact=reference_exact, face_uvs=face_uvs, texture_filter=texture_filter, corner_light=corner_light,
         interior_gradient=interior_gradient, corner_shading=corner_shading, shading_params=shading_params,
-        lights=lights)['rgb']
+        lights=lights, environment_sh=environment_sh)['rgb']
 
 
 def rasterize_silhouettes(

@@ -39,6 +39,9 @@ class Renderer(object):
         # extra lights of shading='phong' on top of the light above: a list of F.directional_light / F.point_light
         # records, or one stacked [NL,12] / [1|B,NL,12] tensor (F.light_set), at most 8.  Empty = that light alone
         self.lights = []
+        # environment light of shading='phong': irradiance-ready SH coefficients [9,3] / [1|B,9,3]
+        # (F.sh_from_environment_map), added to every pixel's diffuse light.  None = no environment
+        self.environment_sh = None
 
         # rasterization
         self.rasterizer_eps = 1e-3
@@ -113,6 +116,8 @@ class Renderer(object):
         n_lights = self.lights.shape[-2] if isinstance(self.lights, torch.Tensor) else len(self.lights)
         if self.shading != 'phong' and n_lights:
             raise ValueError("lights (a light set) needs shading='phong', got shading=%r" % (self.shading,))
+        if self.shading != 'phong' and self.environment_sh is not None:
+            raise ValueError("environment_sh (an SH environment) needs shading='phong', got shading=%r" % (self.shading,))
         fused = (self.fused and self._fusable(vertices, faces) and textures.is_cuda and textures.dtype == torch.float32)
         light_args = (self.light_intensity_ambient, self.light_intensity_directional, self.light_color_ambient,
                       self.light_color_directional, self.light_direction)
@@ -222,6 +227,9 @@ class Renderer(object):
         lights = self._light_set()
         if lights is not None:
             lights = lights.to(vertices.device)
+        sh = self.environment_sh
+        if sh is not None:
+            sh = sh.to(vertices.device)
         if fused:
             indices = self._indices(faces)
             # one mesh seen from B viewpoints (an expanded, stride-0 vertex batch and a shared index set): one corner set
@@ -232,7 +240,7 @@ class Renderer(object):
                 indices, textures, self.image_size, self.anti_aliasing, self.near, self.far, self.rasterizer_eps,
                 self.background_color, textures_fill_back=self.fill_back, vertices=self._transform(vertices),
                 reference_exact=self.reference_exact, face_uvs=face_uvs, texture_filter=texture_filter,
-                corner_shading=cs, shading_params=params, lights=lights)
+                corner_shading=cs, shading_params=params, lights=lights, environment_sh=sh)
         # op by op: torch normals and corners, materialised faces, doubled textures / UV corners for fill_back
         normals = F._vertex_normals_torch(vertices, faces)
         if self.fill_back:
@@ -246,4 +254,4 @@ class Renderer(object):
         return rasterize(
             faces, textures, self.image_size, self.anti_aliasing, self.near, self.far, self.rasterizer_eps,
             self.background_color, reference_exact=self.reference_exact, face_uvs=face_uvs,
-            texture_filter=texture_filter, corner_shading=cs, shading_params=params, lights=lights)
+            texture_filter=texture_filter, corner_shading=cs, shading_params=params, lights=lights, environment_sh=sh)
