@@ -28,6 +28,8 @@
 //   k_image_grad      K6 for a texture image sampled through per-corner UVs (NR_TEX_UV): four bilinear taps per pixel,
 //                     two 6-float horizontal pairs scattered the same way.  k_image_grad_mip: the trilinear variant
 //                     (NR_TEX_MIPMAP), up to four pairs on two levels of the packed pyramid.
+//   The texture-gradient kernels are instantiated per light mode (nr_shading.cuh) except kLightFace, which their
+//   kLightNone variant serves with a run-time face_light pointer.
 //   k_depth_grad      K7 (rasterize.py:805-847): analytic d zp / d(x, y, z) of the winning face, summed per run of
 //                     neighbouring lanes that show the same face before the atomics.
 //
@@ -121,8 +123,8 @@ struct BwdParams {
     const int* strip_list;  // face indices, grouped by (item, axis, strip)
     float* grad_textures;
     const float* textures;
-    const float* face_light;
     float* grad_face_light;
+    float* grad_corner_light;  // d loss / d corner_light (the kLightCorner variants), or nullptr
     int B, F, S, ts, nchunks;
     int W;          // lines per strip (power of two)
     int w_log2, nstrips;
@@ -145,21 +147,8 @@ struct BwdParams {
     nr::MipTable mip;
     // d loss / d face_uvs (appended likewise): the layout of `uvs` (uv_bstride floats per item), or nullptr
     float* grad_uvs;
-    // smooth shading (appended likewise): corner_light [B,F,3,3] (the kCorner variants) and its gradient, or nullptr
-    const float* corner_light;
-    float* grad_corner_light;
-    // Phong shading (appended likewise, the kLight == 3 variants): corner_shading [Bc,F,3,6] and params [Bp,16]
-    const float* phong_cs;
-    const float* phong_prm;
-    size_t cs_bstride;   // faces per item in phong_cs (0 with Bc = 1)
-    size_t prm_bstride;  // floats per item in phong_prm (0 with Bp = 1)
-    // light set (appended likewise, the kLight == 4 variants): lights [Bl,NL,12]
-    const float* lts;
-    size_t lt_bstride;   // floats per item in lts (0 with Bl = 1)
-    int NL;
-    // SH environment (appended likewise, the kLight == 5 variants, with the set above or NL = 0): sh [Bs,9,3]
-    const float* sh;
-    size_t sh_bstride;   // floats per item in sh (0 with Bs = 1)
+    // what lights the pixel (appended likewise): face_light, corner_light or the Phong inputs of the call's light mode
+    nr::Shading shading;
 };
 
 //@phase helpers: rcp / vector RED / load_grad (inlined)
@@ -984,15 +973,14 @@ __device__ __forceinline__ void light_grad_scatter(float (&gl)[N], int fn, int l
 // that sit next to each other with the same (cube, cell) therefore add their 8 x 3 contributions together with
 // kTgCombine shuffle steps first (runs of up to 2^kTgCombine lanes collapse into one lane's reductions).
 //
-// kLight: 0 = face_light or unlit, 2 = corner_light, 3 = Phong, 4 = Phong with a light set, 5 = Phong with an SH environment.
-// kCorner (corner_light): the pixel's light L_c = the corner factors interpolated with its perspective weights l_k (own
-// vertex depths) takes face_light's place, and d loss / d corner_light = l_k g_c s_c goes through the same run reduction.
-// kPhong: L_c = the diffuse part of the Phong expression at the pixel (nr::phong_diffuse) takes face_light's place; the
-// Phong gradients themselves come from k_phong_grad (nr_phong.cu).  Mode 4 adds the set's diffuse terms to L_c, mode 5
-// those of a set (NL may be 0) and the SH irradiance E_c.
+// kLight (nr_shading.cuh): kLightNone serves unlit and face_light calls.  kCorner (kLightCorner): the pixel's light
+// L_c = the corner factors interpolated with its perspective weights l_k (own vertex depths) takes face_light's place, and
+// d loss / d corner_light = l_k g_c s_c goes through the same run reduction.  kPhong (the Phong modes): L_c = the diffuse
+// part of the Phong expression at the pixel (nr::pixel_light) takes face_light's place; the Phong gradients themselves
+// come from k_phong_grad (nr_phong.cu).
 template <int kTgCombine, int kLight>
-__global__ void __launch_bounds__(256, kTgCombine ? (kLight >= 2 ? NR_TGC_MIN_CTAS : 4) : NR_TG_MIN_CTAS) k_texture_grad(const __grid_constant__ BwdParams p) {
-    constexpr bool kCorner = kLight == 2, kPhong = kLight >= 3;
+__global__ void __launch_bounds__(256, kTgCombine ? (kLight >= nr::kLightCorner ? NR_TGC_MIN_CTAS : 4) : NR_TG_MIN_CTAS) k_texture_grad(const __grid_constant__ BwdParams p) {
+    constexpr bool kCorner = kLight == nr::kLightCorner, kPhong = kLight >= nr::kLightPhong;
     const int S = p.S;
     const size_t plane = (size_t)S * S;
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;  // pixel within the image (image orientation)
@@ -1045,23 +1033,7 @@ __global__ void __launch_bounds__(256, kTgCombine ? (kLight >= 2 ? NR_TGC_MIN_CT
                 for (int k = 0; k < 3; k++) oz[k] = __ldg(nr::face_vertex(p.src, b, fn, k) + 2);
             }
             nr::perspective_weights(w, zp, oz[0], oz[1], oz[2], lam);
-            if constexpr (kCorner) {
-                nr::corner_light_at(p.corner_light + ((size_t)b * p.F + fn) * 9, lam, L);
-            } else {
-                nr::PhongEval E;
-                const float* cs = p.phong_cs + ((size_t)b * p.cs_bstride + fn) * 18;
-                const float* prm = p.phong_prm + (size_t)b * p.prm_bstride;
-                if constexpr (kLight == 5) {
-                    float pos[3];
-                    nr::phong_sh_diffuse(cs, lam, prm, p.lts + (size_t)b * p.lt_bstride, p.NL, p.sh + (size_t)b * p.sh_bstride, E, pos);
-                } else if constexpr (kLight == 4) {
-                    float pos[3];
-                    nr::phong_lights_diffuse(cs, lam, prm, p.lts + (size_t)b * p.lt_bstride, p.NL, E, pos);
-                } else {
-                    nr::phong_diffuse(cs, lam, prm, E);
-                }
-                L[0] = E.L[0]; L[1] = E.L[1]; L[2] = E.L[2];
-            }
+            nr::pixel_light<kLight>(p.shading, b, p.F, fn, lam, L);
         }
         // NR_TEX_FILL_BACK: the reversed copy of face f - F/2 shares that face's cube, axes reversed
         int cube = fn, ncubes = p.F;
@@ -1091,8 +1063,8 @@ __global__ void __launch_bounds__(256, kTgCombine ? (kLight >= 2 ? NR_TGC_MIN_CT
         }
         if constexpr (kCorner || kPhong) {  // d rgb / d texel = weight * interpolated light
             g0 *= L[0]; g1 *= L[1]; g2 *= L[2];
-        } else if (p.face_light) {  // d rgb / d texel = weight * light
-            const float* lp = p.face_light + ((size_t)b * p.F + fn) * 3;
+        } else if (p.shading.face_light) {  // d rgb / d texel = weight * light
+            const float* lp = p.shading.face_light + p.shading.fl_off(b, p.F, fn);
             g0 *= __ldg(lp); g1 *= __ldg(lp + 1); g2 *= __ldg(lp + 2);
         }
         float* gt = p.grad_textures + cube_off;
@@ -1199,12 +1171,11 @@ __device__ __forceinline__ void red_add_6(float* t, const float v[6]) {
 // weight) goes to UV corner k as l_k (gu, gv), corners reversed back for a fill_back copy.  Runs of neighbouring lanes
 // that show the same face sum their 6 floats with shuffles and the run's first lane adds them.
 //
-// kLight: 0 = face_light or unlit, 2 = corner_light, 3 = Phong, 4 = Phong with a light set, 5 = Phong with an SH environment.
-// kCorner (corner_light): as in k_texture_grad, the interpolated light L_c replaces face_light (also in the face_uvs
+// kLight: as in k_texture_grad.  kCorner (kLightCorner): as in k_texture_grad, the interpolated light L_c replaces face_light (also in the face_uvs
 // gradient) and the 9-float corner-light gradient goes through the run reduction.  kPhong: likewise with the Phong L_c.
 template <int kTgCombine, bool kMip, bool kUvGrad, int kLight>
 __device__ __forceinline__ void image_grad(const BwdParams& p) {
-    constexpr bool kCorner = kLight == 2, kPhong = kLight >= 3;
+    constexpr bool kCorner = kLight == nr::kLightCorner, kPhong = kLight >= nr::kLightPhong;
     constexpr int kPairs = kMip ? 4 : 2;
     const int S = p.S;
     const size_t plane = (size_t)S * S;
@@ -1269,24 +1240,9 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
         nr::load_face_uvs(p.uvs + ((uint32_t)b * p.uv_bstride + (uint32_t)uf * 6u), rev, uv);
         nr::pixel_uv(w, zp, z0, z1, z2, uv, u, v);
         float lam[3] = {0.0f, 0.0f, 0.0f}, L[3];  // kCorner / kPhong: perspective weights and light of the pixel
-        if constexpr (kCorner) {
+        if constexpr (kCorner || kPhong) {
             nr::perspective_weights(w, zp, z0, z1, z2, lam);
-            nr::corner_light_at(p.corner_light + ((size_t)b * p.F + fn) * 9, lam, L);
-        } else if constexpr (kPhong) {
-            nr::perspective_weights(w, zp, z0, z1, z2, lam);
-            nr::PhongEval E;
-            const float* cs = p.phong_cs + ((size_t)b * p.cs_bstride + fn) * 18;
-            const float* prm = p.phong_prm + (size_t)b * p.prm_bstride;
-            if constexpr (kLight == 5) {
-                float pos[3];
-                nr::phong_sh_diffuse(cs, lam, prm, p.lts + (size_t)b * p.lt_bstride, p.NL, p.sh + (size_t)b * p.sh_bstride, E, pos);
-            } else if constexpr (kLight == 4) {
-                float pos[3];
-                nr::phong_lights_diffuse(cs, lam, prm, p.lts + (size_t)b * p.lt_bstride, p.NL, E, pos);
-            } else {
-                nr::phong_diffuse(cs, lam, prm, E);
-            }
-            L[0] = E.L[0]; L[1] = E.L[1]; L[2] = E.L[2];
+            nr::pixel_light<kLight>(p.shading, b, p.F, fn, lam, L);
         }
         const uint32_t img_off = (uint32_t)b * p.img_bstride;
         // level(s) and their weights: the bilinear variant is level 0 of an image with weight 1
@@ -1304,8 +1260,8 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
             float lt[3] = {1.0f, 1.0f, 1.0f};
             if constexpr (kCorner || kPhong) {
                 lt[0] = L[0]; lt[1] = L[1]; lt[2] = L[2];
-            } else if (p.face_light) {
-                const float* lp = p.face_light + ((size_t)b * p.F + fn) * 3;
+            } else if (p.shading.face_light) {
+                const float* lp = p.shading.face_light + p.shading.fl_off(b, p.F, fn);
                 lt[0] = __ldg(lp); lt[1] = __ldg(lp + 1); lt[2] = __ldg(lp + 2);
             }
             const float h[3] = {g0 * lt[0], g1 * lt[1], g2 * lt[2]};  // d loss / d unlit tap value, per unit weight
@@ -1352,8 +1308,8 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
         }
         if constexpr (kCorner || kPhong) {  // d rgb / d texel = weight * interpolated light
             g0 *= L[0]; g1 *= L[1]; g2 *= L[2];
-        } else if (p.face_light) {  // d rgb / d texel = weight * light
-            const float* lp = p.face_light + ((size_t)b * p.F + fn) * 3;
+        } else if (p.shading.face_light) {  // d rgb / d texel = weight * light
+            const float* lp = p.shading.face_light + p.shading.fl_off(b, p.F, fn);
             g0 *= __ldg(lp); g1 *= __ldg(lp + 1); g2 *= __ldg(lp + 2);
         }
         float* gi = p.grad_textures + img_off;
@@ -1663,20 +1619,19 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
     if (rgb && part_tex && !a->grad_textures) return NR_ERR_INVALID_ARG;
     if (rgb && (flags & NR_TEX_FILL_BACK) && (F & 1)) return NR_ERR_INVALID_ARG;
     if (rgb && a->grad_face_light && !a->textures) return NR_ERR_INVALID_ARG;
-    // smooth shading: corner_light only for RGB and instead of face_light; its gradient reads the (unlit) textures
-    const bool smooth = corner_light != nullptr;
-    if (smooth && (!rgb || a->face_light)) return NR_ERR_INVALID_ARG;
-    if (grad_corner_light && (!smooth || !a->textures)) return NR_ERR_INVALID_ARG;
-    // Phong: only for RGB and instead of face_light / corner_light; its gradients read the (unlit) textures
-    if (phong && (!rgb || a->face_light || smooth || !nr_internal::phong_args_ok(phong, B))) return NR_ERR_INVALID_ARG;
-    // light set: grad_lights needs s as well
-    if (lights && (!nr_internal::lights_args_ok(lights, B) || (lights->grad_lights && !a->textures))) return NR_ERR_INVALID_ARG;
-    // SH environment: grad_sh needs s as well
-    if (sh && (!nr_internal::sh_args_ok(sh, B) || (sh->grad_sh && !a->textures))) return NR_ERR_INVALID_ARG;
-    if (lights && lights->num_lights == 0) lights = nullptr;  // the Phong call exactly
-    const bool phong_grads = phong && (phong->grad_corner_shading || phong->grad_params || (lights && lights->grad_lights) ||
-                                       (sh && sh->grad_sh));
-    if (phong_grads && !a->textures) return NR_ERR_INVALID_ARG;
+    nr::Shading shading;
+    const int light = nr_internal::make_shading(rgb, a->face_light, corner_light, phong, lights, sh, B, F, &shading);
+    if (light < 0) return NR_ERR_INVALID_ARG;
+    // the shading gradients: grad_corner_light needs corner_light, and every one reads the (unlit) textures (also a
+    // grad_lights of a set of NL = 0 lights, which then receives nothing)
+    if (grad_corner_light && !corner_light) return NR_ERR_INVALID_ARG;
+    float* grad_cs = phong ? phong->grad_corner_shading : nullptr;
+    float* grad_prm = phong ? phong->grad_params : nullptr;
+    float* grad_lts = shading.NL > 0 ? lights->grad_lights : nullptr;
+    float* grad_sh = sh ? sh->grad_sh : nullptr;
+    if (!a->textures && (grad_corner_light || grad_cs || grad_prm || (lights && lights->grad_lights) || grad_sh))
+        return NR_ERR_INVALID_ARG;
+    const bool phong_grads = grad_cs || grad_prm || grad_lts || grad_sh;
     // NR_GRAD_INTERIOR: the sampler's derivative reads the textures; the cubes of NR_TEX_Z_BATCH0 sample item b with the
     // depths of item 0, so their derivative would cross items (B = 1 is the plain sampler)
     const bool interior = (flags & NR_GRAD_INTERIOR) != 0;
@@ -1728,17 +1683,15 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
         if (part_tex && grad_corner_light &&
             cudaMemsetAsync(grad_corner_light, 0, (size_t)B * F * 9 * sizeof(float), stream) != cudaSuccess)
             return NR_ERR_CUDA;
-        if (part_tex && phong && phong->grad_corner_shading &&
-            cudaMemsetAsync(phong->grad_corner_shading, 0, (size_t)phong->shading_batch * F * 18 * sizeof(float), stream) != cudaSuccess)
+        if (part_tex && grad_cs &&
+            cudaMemsetAsync(grad_cs, 0, (size_t)phong->shading_batch * F * 18 * sizeof(float), stream) != cudaSuccess)
             return NR_ERR_CUDA;
-        if (part_tex && phong && phong->grad_params &&
-            cudaMemsetAsync(phong->grad_params, 0, (size_t)phong->params_batch * 16 * sizeof(float), stream) != cudaSuccess)
+        if (part_tex && grad_prm && cudaMemsetAsync(grad_prm, 0, (size_t)phong->params_batch * 16 * sizeof(float), stream) != cudaSuccess)
             return NR_ERR_CUDA;
-        if (part_tex && lights && lights->grad_lights &&
-            cudaMemsetAsync(lights->grad_lights, 0, (size_t)lights->lights_batch * lights->num_lights * 12 * sizeof(float), stream) != cudaSuccess)
+        if (part_tex && grad_lts &&
+            cudaMemsetAsync(grad_lts, 0, (size_t)lights->lights_batch * lights->num_lights * 12 * sizeof(float), stream) != cudaSuccess)
             return NR_ERR_CUDA;
-        if (part_tex && sh && sh->grad_sh &&
-            cudaMemsetAsync(sh->grad_sh, 0, (size_t)sh->sh_batch * 27 * sizeof(float), stream) != cudaSuccess)
+        if (part_tex && grad_sh && cudaMemsetAsync(grad_sh, 0, (size_t)sh->sh_batch * 27 * sizeof(float), stream) != cudaSuccess)
             return NR_ERR_CUDA;
         nr_internal::prof_end(stream);
     }
@@ -1749,7 +1702,7 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
     p.fim = a->face_index_map; p.wmap = a->weight_map; p.dmap = a->depth_map; p.rgb = a->rgb_map;
     p.g_rgb = rgb ? a->grad_rgb : nullptr; p.g_alpha = alpha ? a->grad_alpha : nullptr; p.g_depth = depth ? a->grad_depth : nullptr;
     p.grad_textures = a->grad_textures;
-    p.textures = a->textures; p.face_light = rgb ? a->face_light : nullptr; p.grad_face_light = rgb ? a->grad_face_light : nullptr;
+    p.textures = a->textures; p.grad_face_light = rgb ? a->grad_face_light : nullptr;
     p.B = B; p.F = F; p.S = S; p.ts = ts;
     p.flags = flags;
     p.eps = (float)a->eps;
@@ -1765,64 +1718,30 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
         if (mip) p.mip = mt;
         p.grad_uvs = a->grad_face_uvs;
     }
-    p.corner_light = corner_light; p.grad_corner_light = grad_corner_light;
-    if (phong) {
-        p.phong_cs = phong->corner_shading; p.phong_prm = phong->params;
-        p.cs_bstride = phong->shading_batch == 1 ? 0 : (size_t)F;
-        p.prm_bstride = phong->params_batch == 1 ? 0 : 16;
-    }
-    if (lights) {
-        p.lts = lights->lights; p.NL = lights->num_lights;
-        p.lt_bstride = lights->lights_batch == 1 ? 0 : (size_t)lights->num_lights * 12;
-    }
-    if (sh) {
-        p.sh = sh->sh;
-        p.sh_bstride = sh->sh_batch == 1 ? 0 : 27;
-    }
-    const int light = sh ? 5 : (lights ? 4 : (phong ? 3 : (smooth ? 2 : 0)));
-
+    p.grad_corner_light = grad_corner_light;
+    p.shading = shading;
     const dim3 pgrid((unsigned)(((size_t)S * S + 255) / 256), B);
     auto launch_texture_grad = [&]() {
-        if (mip) {
-            nr_internal::LaunchScope ls("k_image_grad", stream);
-            if (light == 5 && uv_grad) k_image_grad_mip<NR_TG_COMBINE, true, 5><<<pgrid, 256, 0, stream>>>(p);
-            else if (light == 5) k_image_grad_mip<NR_TG_COMBINE, false, 5><<<pgrid, 256, 0, stream>>>(p);
-            else if (light == 4 && uv_grad) k_image_grad_mip<NR_TG_COMBINE, true, 4><<<pgrid, 256, 0, stream>>>(p);
-            else if (light == 4) k_image_grad_mip<NR_TG_COMBINE, false, 4><<<pgrid, 256, 0, stream>>>(p);
-            else if (light == 3 && uv_grad) k_image_grad_mip<NR_TG_COMBINE, true, 3><<<pgrid, 256, 0, stream>>>(p);
-            else if (light == 3) k_image_grad_mip<NR_TG_COMBINE, false, 3><<<pgrid, 256, 0, stream>>>(p);
-            else if (smooth && uv_grad) k_image_grad_mip<NR_TG_COMBINE, true, 2><<<pgrid, 256, 0, stream>>>(p);
-            else if (smooth) k_image_grad_mip<NR_TG_COMBINE, false, 2><<<pgrid, 256, 0, stream>>>(p);
-            else if (uv_grad) k_image_grad_mip<NR_TG_COMBINE, true, 0><<<pgrid, 256, 0, stream>>>(p);
-            else k_image_grad_mip<NR_TG_COMBINE, false, 0><<<pgrid, 256, 0, stream>>>(p);
-            return;
-        }
-        if (uv) {
-            nr_internal::LaunchScope ls("k_image_grad", stream);
-            if (light == 5 && uv_grad) k_image_grad<NR_TG_COMBINE, true, 5><<<pgrid, 256, 0, stream>>>(p);
-            else if (light == 5) k_image_grad<NR_TG_COMBINE, false, 5><<<pgrid, 256, 0, stream>>>(p);
-            else if (light == 4 && uv_grad) k_image_grad<NR_TG_COMBINE, true, 4><<<pgrid, 256, 0, stream>>>(p);
-            else if (light == 4) k_image_grad<NR_TG_COMBINE, false, 4><<<pgrid, 256, 0, stream>>>(p);
-            else if (light == 3 && uv_grad) k_image_grad<NR_TG_COMBINE, true, 3><<<pgrid, 256, 0, stream>>>(p);
-            else if (light == 3) k_image_grad<NR_TG_COMBINE, false, 3><<<pgrid, 256, 0, stream>>>(p);
-            else if (smooth && uv_grad) k_image_grad<NR_TG_COMBINE, true, 2><<<pgrid, 256, 0, stream>>>(p);
-            else if (smooth) k_image_grad<NR_TG_COMBINE, false, 2><<<pgrid, 256, 0, stream>>>(p);
-            else if (uv_grad) k_image_grad<NR_TG_COMBINE, true, 0><<<pgrid, 256, 0, stream>>>(p);
-            else k_image_grad<NR_TG_COMBINE, false, 0><<<pgrid, 256, 0, stream>>>(p);
-            return;
-        }
-        nr_internal::LaunchScope ls("k_texture_grad", stream);
-        if (light == 5) k_texture_grad<NR_TG_COMBINE, 5><<<pgrid, 256, 0, stream>>>(p);
-        else if (light == 4) k_texture_grad<NR_TG_COMBINE, 4><<<pgrid, 256, 0, stream>>>(p);
-        else if (light == 3) k_texture_grad<NR_TG_COMBINE, 3><<<pgrid, 256, 0, stream>>>(p);
-        else if (smooth) k_texture_grad<NR_TG_COMBINE, 2><<<pgrid, 256, 0, stream>>>(p);
-        else k_texture_grad<NR_TG_COMBINE, 0><<<pgrid, 256, 0, stream>>>(p);
+        nr_internal::LaunchScope ls(uv ? "k_image_grad" : "k_texture_grad", stream);
+        // face_light is the kLightNone variant's run-time branch
+        const int tg_light = light == nr::kLightFace ? nr::kLightNone : light;
+        nr::dispatch_light<nr::kLightNone, nr::kLightCorner, nr::kLightPhong, nr::kLightPhongSet, nr::kLightPhongSH>(tg_light, [&](auto kL) {
+            if (!uv) {
+                k_texture_grad<NR_TG_COMBINE, kL><<<pgrid, 256, 0, stream>>>(p);
+                return;
+            }
+            nr::dispatch_bool(uv_grad, [&](auto kUvGrad) {
+                if (mip) k_image_grad_mip<NR_TG_COMBINE, kUvGrad, kL><<<pgrid, 256, 0, stream>>>(p);
+                else k_image_grad<NR_TG_COMBINE, kUvGrad, kL><<<pgrid, 256, 0, stream>>>(p);
+            });
+        });
     };
-    // Phong: d loss / d corner_shading and d params per pixel (nr_phong.cu), part of the texture half
+    // Phong: d loss / d corner_shading, params, lights and sh per pixel (nr_phong.cu), part of the texture half
     auto launch_phong_grad = [&]() {
         if (!phong_grads) return;
         nr_internal::PhongGradLaunch pl{};
-        pl.args = a; pl.src = src; pl.phong = phong; pl.lights = lights; pl.sh = sh;
+        pl.args = a; pl.src = src; pl.shading = shading; pl.light = light;
+        pl.grad_cs = grad_cs; pl.grad_prm = grad_prm; pl.grad_lts = grad_lts; pl.grad_sh = grad_sh;
         pl.tex_bstride = (flags & NR_TEX_SHARED) ? 0 : (uv ? img_floats : ncubes * (size_t)ts * ts * ts * 3);
         pl.uv_bstride = p.uv_bstride;
         pl.tex_cmp = p.tex_cmp; pl.tex_val = p.tex_val;
@@ -1920,7 +1839,7 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
     }
     if (interior && p.g_rgb) {  // the interior term of the rgb image (nr_interior.cu), into the same face / vertex gradient
         nr_internal::InteriorLaunch il{};
-        il.args = a; il.src = src; il.dst = dst; il.corner_light = corner_light;
+        il.args = a; il.src = src; il.dst = dst; il.shading = shading; il.light = light;
         il.tex_bstride = (flags & NR_TEX_SHARED) ? 0 : (uv ? img_floats : ncubes * (size_t)ts * ts * ts * 3);
         il.uv_bstride = p.uv_bstride;
         il.tex_cmp = p.tex_cmp; il.tex_val = p.tex_val;

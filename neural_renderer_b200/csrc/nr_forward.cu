@@ -26,7 +26,8 @@
 //   k_resolve        one thread per pixel (per 2x2 quad when anti-aliasing): decode the winner, read its record,
 //                    re-evaluate the weights with the same expression tree, sample the ts^3 texture (K4), composite the
 //                    background and stream all maps out as planar, row-flipped (image orientation) coalesced rows; with
-//                    anti-aliasing the thread also emits the pooled API pixel.
+//                    anti-aliasing the thread also emits the pooled API pixel.  One variant per sampler, anti-aliasing and
+//                    light mode (nr_shading.cuh: unlit, face_light, corner_light, Phong, Phong + light set, Phong + SH).
 //
 // Nothing depends on the screen being tiled: work is linear in the number of faces (a 1 M-face mesh costs 1 M lane
 // set-ups, not 1 M box tests per tile) and in the number of covered pixels.
@@ -67,19 +68,19 @@ constexpr int kOwnTable = 256;         // rows / fragments per pass whose owner 
                                    // they spill (-Xptxas -v)
 #endif
 #ifndef NR_RESOLVE_SMOOTH_MIN_CTAS
-#define NR_RESOLVE_SMOOTH_MIN_CTAS 6     // smooth-shaded (kLight == 2) cube / bilinear variants: 40 registers, no spills
+#define NR_RESOLVE_SMOOTH_MIN_CTAS 6     // smooth-shaded (kLightCorner) cube / bilinear variants: 40 registers, no spills
 #endif
 #ifndef NR_RESOLVE_SMOOTH_AA_MIN_CTAS
 #define NR_RESOLVE_SMOOTH_AA_MIN_CTAS 4  // the same with anti-aliasing: the cube variant spills at 5 CTAs (48 registers)
 #endif
 #ifndef NR_RESOLVE_PHONG_MIN_CTAS
-#define NR_RESOLVE_PHONG_MIN_CTAS 4      // Phong-shaded (kLight == 3) variants, every sampler (DESIGN.md section 4g)
+#define NR_RESOLVE_PHONG_MIN_CTAS 4      // Phong-shaded (kLightPhong) variants, every sampler (DESIGN.md section 4g)
 #endif
 #ifndef NR_RESOLVE_LIGHTS_MIN_CTAS
-#define NR_RESOLVE_LIGHTS_MIN_CTAS 4     // Phong with a light set (kLight == 4), every sampler (DESIGN.md section 4h)
+#define NR_RESOLVE_LIGHTS_MIN_CTAS 4     // Phong with a light set (kLightPhongSet), every sampler (DESIGN.md section 4h)
 #endif
 #ifndef NR_RESOLVE_SH_MIN_CTAS
-#define NR_RESOLVE_SH_MIN_CTAS 4         // Phong with an SH environment (kLight == 5), every sampler (DESIGN.md section 4i)
+#define NR_RESOLVE_SH_MIN_CTAS 4         // Phong with an SH environment (kLightPhongSH), every sampler (DESIGN.md section 4i)
 #endif
 constexpr int kResolveTileW = 32, kResolveTileH = 8;  // API pixels per k_resolve CTA (256 threads, 8 x 4 per warp)
 constexpr uint32_t kStageBytes = 32 * 1024;  // shared memory of a k_resolve CTA for staged texture cubes
@@ -89,7 +90,6 @@ struct FwdParams {
     size_t tex_bstride;  // cubes per batch item in `textures` (0 with NR_TEX_SHARED)
     const float* textures;
     const float* bg_batch;
-    const float* face_light;
     unsigned long long* zbuf;  // [B,S,S] raster orientation (row = yi): ordered zp << 32 | face index, ~0 = empty
     float4* tab;               // [B,F,3] float4: {inv0..3}, {inv4..7}, {inv8, z0, z1, z2} of every drawn face
     int* big_cnt;              // [B] number of big faces - 1 (memset to 0xFF = -1)
@@ -117,20 +117,8 @@ struct FwdParams {
     int Ht, Wt;
     // NR_TEX_MIPMAP (appended likewise): `textures` is the packed pyramid, img_bstride its floats per item
     nr::MipTable mip;
-    // smooth shading (appended likewise): corner_light [B,F,3,3], or nullptr
-    const float* corner_light;
-    // Phong shading (appended likewise): corner_shading [Bc,F,3,6] and params [Bp,16]; strides 0 for a shared set
-    const float* phong_cs;
-    const float* phong_prm;
-    size_t cs_bstride;   // faces per item in phong_cs (0 with Bc = 1)
-    size_t prm_bstride;  // floats per item in phong_prm (0 with Bp = 1)
-    // light set (appended likewise, the kLight == 4 variants): lights [Bl,NL,12]
-    const float* lts;
-    size_t lt_bstride;   // floats per item in lts (0 with Bl = 1)
-    int NL;
-    // SH environment (appended likewise, the kLight == 5 variants, with the set above or NL = 0): sh [Bs,9,3]
-    const float* sh;
-    size_t sh_bstride;   // floats per item in sh (0 with Bs = 1)
+    // what lights the pixel (appended likewise): face_light, corner_light or the Phong inputs of the call's light mode
+    nr::Shading shading;
 };
 
 // rasterize.py:291-292  xp = (2 * xi + 1 - is) / is evaluated in double and rounded to float.  Both operands are
@@ -433,7 +421,7 @@ __device__ __forceinline__ void blend_corners(const FwdParams& p, const nr::TexC
     const int ts = p.ts;
     float l0 = 1.0f, l1 = 1.0f, l2 = 1.0f;
     if (kLit) {
-        const float* lp = p.face_light + ((size_t)b * p.F + fn) * 3;
+        const float* lp = p.shading.face_light + p.shading.fl_off(b, p.F, fn);
         l0 = __ldg(lp); l1 = __ldg(lp + 1); l2 = __ldg(lp + 2);
     }
     r = g = bl = 0.0f;
@@ -474,9 +462,8 @@ __device__ __forceinline__ int face_cube(const FwdParams& p, int fn, bool& rev) 
 
 // one pixel, every texel straight from global memory (anti-aliased quads, texture sizes the bulk copy cannot stage);
 // kUV: bilinear sample of the texture image at the pixel's perspective-correct UV instead of the ts^3 cube; kMip:
-// trilinear sample of its mip pyramid at the pixel's level of detail.  kLight: 0 = unlit, 1 = face_light multiplies every
-// texel, 2 = corner_light interpolated to the pixel multiplies the unlit sample, 3 = Phong shading of the unlit sample, 4 = the
-// same with a light set, 5 = the same with an SH environment (and a light set or none)
+// trilinear sample of its mip pyramid at the pixel's level of detail.  kLight (nr_shading.cuh): kLightFace multiplies every
+// texel by face_light, the later modes shade the unlit sample (nr::shade)
 template <int kLight, bool kUV = false, bool kMip = false>
 __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigned long long key, int xi, int yi, float bgr,
                                               float bgg, float bgb) {
@@ -503,18 +490,18 @@ __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigne
             nr::load_face_uvs(p.uvs + ((uint32_t)b * p.uv_bstride + (uint32_t)uf * 6u), rev, uv);
             nr::pixel_uv(w, zp, cc.y, cc.z, cc.w, uv, u, v);
             float l0 = 1.0f, l1 = 1.0f, l2 = 1.0f;
-            if (kLight == 1) {
-                const float* lp = p.face_light + ((size_t)b * p.F + fn) * 3;
+            if (kLight == nr::kLightFace) {
+                const float* lp = p.shading.face_light + p.shading.fl_off(b, p.F, fn);
                 l0 = __ldg(lp); l1 = __ldg(lp + 1); l2 = __ldg(lp + 2);
             }
             float c[3];
             if constexpr (kMip) {
                 const float lod = nr::mip_lod(inv, w, zp, cc.y, cc.z, cc.w, uv, p.Ht, p.Wt, p.mip.levels);
-                nr::mip_blend<kLight == 1>(p.textures + (uint32_t)b * p.img_bstride, p.mip, nr::mip_levels(lod, p.mip.levels), u,
-                                           v, l0, l1, l2, c);
+                nr::mip_blend<kLight == nr::kLightFace>(p.textures + (uint32_t)b * p.img_bstride, p.mip,
+                                                        nr::mip_levels(lod, p.mip.levels), u, v, l0, l1, l2, c);
             } else {
                 const nr::UvTaps t = nr::uv_taps(u, v, p.Ht, p.Wt);
-                nr::uv_blend<kLight == 1>(p.textures + (uint32_t)b * p.img_bstride, p.Wt, t, l0, l1, l2, c);
+                nr::uv_blend<kLight == nr::kLightFace>(p.textures + (uint32_t)b * p.img_bstride, p.Wt, t, l0, l1, l2, c);
             }
             o.r = c[0]; o.g = c[1]; o.b = c[2];
         } else {
@@ -525,49 +512,26 @@ __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigne
             bool rev;
             const int cube = face_cube(p, fn, rev);
             const float* tex = p.textures + ((size_t)b * p.tex_bstride + cube) * (size_t)(ts * ts * ts) * 3;
-            blend_corners<kLight == 1>(p, tc, tex, rev, b, fn, o.r, o.g, o.b);
+            blend_corners<kLight == nr::kLightFace>(p, tc, tex, rev, b, fn, o.r, o.g, o.b);
         }
-        if constexpr (kLight == 2) {  // smooth shading: the light interpolated with the pixel's l_k times the unlit sample
-            float l[3], L[3];
+        if constexpr (kLight >= nr::kLightCorner) {  // the light of the pixel's l_k (own depths) on the unlit sample
+            float l[3], c[3] = {o.r, o.g, o.b};
             nr::perspective_weights(w, zp, cc.y, cc.z, cc.w, l);
-            nr::corner_light_at(p.corner_light + ((size_t)b * p.F + fn) * 9, l, L);
-            o.r = __fmul_rn(L[0], o.r); o.g = __fmul_rn(L[1], o.g); o.b = __fmul_rn(L[2], o.b);
-        }
-        if constexpr (kLight == 3) {  // Phong: normal and position interpolated with the pixel's l_k (own depths)
-            float l[3], rgb[3];
-            nr::perspective_weights(w, zp, cc.y, cc.z, cc.w, l);
-            const float* prm = p.phong_prm + (size_t)b * p.prm_bstride;
-            nr::PhongEval E;
-            nr::phong_at(p.phong_cs + ((size_t)b * p.cs_bstride + fn) * 18, l, prm, E);
-            const float s[3] = {o.r, o.g, o.b};
-            nr::phong_rgb(E, prm, s, rgb);
-            o.r = rgb[0]; o.g = rgb[1]; o.b = rgb[2];
-        }
-        if constexpr (kLight == 4) {  // Phong with a light set
-            float l[3], rgb[3], pos[3];
-            nr::perspective_weights(w, zp, cc.y, cc.z, cc.w, l);
-            const float* prm = p.phong_prm + (size_t)b * p.prm_bstride;
-            const float* lts = p.lts + (size_t)b * p.lt_bstride;
-            nr::PhongEval E;
-            nr::phong_lights_at(p.phong_cs + ((size_t)b * p.cs_bstride + fn) * 18, l, prm, lts, p.NL, E, pos);
-            const float s[3] = {o.r, o.g, o.b};
-            nr::phong_lights_rgb(E, pos, prm, lts, p.NL, s, rgb);
-            o.r = rgb[0]; o.g = rgb[1]; o.b = rgb[2];
-        }
-        if constexpr (kLight == 5) {  // Phong with an SH environment: E_c joins L_c after the set's diffuse terms
-            float l[3], rgb[3], pos[3];
-            nr::perspective_weights(w, zp, cc.y, cc.z, cc.w, l);
-            const float* prm = p.phong_prm + (size_t)b * p.prm_bstride;
-            const float* lts = p.lts + (size_t)b * p.lt_bstride;
-            nr::PhongEval E;
-            nr::phong_sh_at(p.phong_cs + ((size_t)b * p.cs_bstride + fn) * 18, l, prm, lts, p.NL, p.sh + (size_t)b * p.sh_bstride,
-                            E, pos);
-            const float s[3] = {o.r, o.g, o.b};
-            nr::phong_lights_rgb(E, pos, prm, lts, p.NL, s, rgb);
-            o.r = rgb[0]; o.g = rgb[1]; o.b = rgb[2];
+            nr::shade<kLight>(p.shading, b, p.F, fn, l, c);
+            o.r = c[0]; o.g = c[1]; o.b = c[2];
         }
     }
     return o;
+}
+
+// CTAs per SM each k_resolve variant is compiled for (the NR_RESOLVE_*_MIN_CTAS above)
+constexpr int resolve_min_ctas(bool aa, int tex, int light) {
+    if (light == nr::kLightPhongSH) return NR_RESOLVE_SH_MIN_CTAS;
+    if (light == nr::kLightPhongSet) return NR_RESOLVE_LIGHTS_MIN_CTAS;
+    if (light == nr::kLightPhong) return NR_RESOLVE_PHONG_MIN_CTAS;
+    if (tex == 3) return NR_RESOLVE_MIP_MIN_CTAS;
+    if (light == nr::kLightCorner) return aa ? NR_RESOLVE_SMOOTH_AA_MIN_CTAS : NR_RESOLVE_SMOOTH_MIN_CTAS;
+    return aa ? 5 : NR_RESOLVE_MIN_CTAS;
 }
 
 //@phase resolve + stores
@@ -585,10 +549,10 @@ __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigne
 // for the shared-memory writes of the copy plus the bank conflicts of the 24 scattered reads.  The direct gather is
 // therefore the default.
 //
-// kTex == 2 (NR_TEX_UV): the direct variants with the texture-image sampler (shade_pixel<kLit, true>), same tile map.
-// kTex == 3 (NR_TEX_UV | NR_TEX_MIPMAP): the same with the trilinear pyramid sampler (shade_pixel<kLit, true, true>).
+// kTex == 2 (NR_TEX_UV): the direct variants with the texture-image sampler (shade_pixel<kLight, true>), same tile map.
+// kTex == 3 (NR_TEX_UV | NR_TEX_MIPMAP): the same with the trilinear pyramid sampler (shade_pixel<kLight, true, true>).
 template <bool kAA, int kTex, int kLight>
-__global__ void __launch_bounds__(256, kLight == 5 ? NR_RESOLVE_SH_MIN_CTAS : kLight == 4 ? NR_RESOLVE_LIGHTS_MIN_CTAS : kLight == 3 ? NR_RESOLVE_PHONG_MIN_CTAS : kTex == 3 ? NR_RESOLVE_MIP_MIN_CTAS : (kLight == 2 ? (kAA ? NR_RESOLVE_SMOOTH_AA_MIN_CTAS : NR_RESOLVE_SMOOTH_MIN_CTAS) : (kAA ? 5 : NR_RESOLVE_MIN_CTAS))) k_resolve(const __grid_constant__ FwdParams p, int nslots) {
+__global__ void __launch_bounds__(256, resolve_min_ctas(kAA, kTex, kLight)) k_resolve(const __grid_constant__ FwdParams p, int nslots) {
     constexpr bool kStage = kTex == 1;  // kTex: 0 = every texel straight from global memory, 1 = cubes staged with cp.async.bulk
     constexpr bool kUV = kTex >= 2;     //       2 = texture image through per-corner UVs, 3 = its mip pyramid
     constexpr bool kMip = kTex == 3;
@@ -677,9 +641,9 @@ __global__ void __launch_bounds__(256, kLight == 5 ? NR_RESOLVE_SH_MIN_CTAS : kL
         float r, g, bl;
         if (staged) {
             mbar_wait(&s_bar, 0);
-            blend_corners<kLight == 1>(p, tc, stex, rev, b, fn, r, g, bl);
+            blend_corners<kLight == nr::kLightFace>(p, tc, stex, rev, b, fn, r, g, bl);
         } else {
-            blend_corners<kLight == 1>(p, tc, gtex, rev, b, fn, r, g, bl);
+            blend_corners<kLight == nr::kLightFace>(p, tc, gtex, rev, b, fn, r, g, bl);
         }
         rgb[o] = r; rgb[o + plane] = g; rgb[o + 2 * plane] = bl;
     } else if (!kAA) {
@@ -753,6 +717,15 @@ FwdLayout fwd_layout(int B, int F, int S) {
     return L;
 }
 
+// one k_resolve launch (the shared-memory opt-in is a static of each instantiation)
+template <bool kAA, int kTex, int kLight>
+int launch_resolve(const FwdParams& p, dim3 grid, int bx, size_t smem, int nslots, cudaStream_t stream) {
+    static nr_internal::SmemOptIn optin;
+    if (optin.ensure(k_resolve<kAA, kTex, kLight>, smem) != cudaSuccess) return NR_ERR_CUDA;
+    k_resolve<kAA, kTex, kLight><<<grid, bx, smem, stream>>>(p, nslots);
+    return NR_OK;
+}
+
 }  // namespace
 
 extern "C" size_t nr_b200_forward_workspace_bytes(int32_t B, int32_t F, int32_t S, int32_t ts, uint32_t flags) {
@@ -791,14 +764,10 @@ static int forward_impl(const nr_b200_forward_args* args, const nr_b200_phong_ar
     if (uv && (!(flags & NR_RETURN_RGB) || !a->face_uvs || a->texture_height < 1 || a->texture_width < 1)) return NR_ERR_INVALID_ARG;
     const bool mip = (flags & NR_TEX_MIPMAP) != 0;
     if (mip && !uv) return NR_ERR_INVALID_ARG;
-    const bool smooth = a->corner_light != nullptr;  // per-corner light: only for RGB, and instead of face_light
-    if (smooth && (!(flags & NR_RETURN_RGB) || a->face_light)) return NR_ERR_INVALID_ARG;
-    // Phong: only for RGB, and instead of face_light / corner_light
-    if (phong && (!(flags & NR_RETURN_RGB) || a->face_light || smooth || !nr_internal::phong_args_ok(phong, B)))
-        return NR_ERR_INVALID_ARG;
-    if (lights && !nr_internal::lights_args_ok(lights, B)) return NR_ERR_INVALID_ARG;
-    if (sh && !nr_internal::sh_args_ok(sh, B)) return NR_ERR_INVALID_ARG;
-    if (lights && lights->num_lights == 0) lights = nullptr;  // the Phong call exactly
+    nr::Shading shading;
+    const int light = nr_internal::make_shading((flags & NR_RETURN_RGB) != 0, a->face_light, a->corner_light, phong, lights, sh,
+                                                B, F, &shading);
+    if (light < 0) return NR_ERR_INVALID_ARG;
     if ((flags & NR_ANTI_ALIASING) && (S & 1)) return NR_ERR_INVALID_ARG;
     if (S > 32767 || B > 65535) return NR_ERR_UNSUPPORTED;  // 32-bit pixel offsets; batch = grid.z of the resolve pass
     // NR_TEX_UV: image (NR_TEX_MIPMAP: pyramid) and UV offsets are 32-bit in the kernels
@@ -819,21 +788,7 @@ static int forward_impl(const nr_b200_forward_args* args, const nr_b200_phong_ar
     p.src = src;
     p.tex_bstride = (flags & NR_TEX_SHARED) ? 0 : ((flags & NR_TEX_FILL_BACK) ? (size_t)F / 2 : (size_t)F);
     p.textures = a->textures; p.bg_batch = a->background_batch;
-    p.face_light = (flags & NR_RETURN_RGB) ? a->face_light : nullptr;
-    p.corner_light = a->corner_light;
-    if (phong) {
-        p.phong_cs = phong->corner_shading; p.phong_prm = phong->params;
-        p.cs_bstride = phong->shading_batch == 1 ? 0 : (size_t)F;
-        p.prm_bstride = phong->params_batch == 1 ? 0 : 16;
-    }
-    if (lights) {
-        p.lts = lights->lights; p.NL = lights->num_lights;
-        p.lt_bstride = lights->lights_batch == 1 ? 0 : (size_t)lights->num_lights * 12;
-    }
-    if (sh) {
-        p.sh = sh->sh;
-        p.sh_bstride = sh->sh_batch == 1 ? 0 : 27;
-    }
+    p.shading = shading;
     p.big_cnt = (int*)(wsb + L.off_cnt);
     p.work_next = p.big_cnt + B;
     p.any_big = p.big_cnt + B + 1;
@@ -901,45 +856,33 @@ static int forward_impl(const nr_b200_forward_args* args, const nr_b200_phong_ar
         // Staging whole cubes with cp.async.bulk needs 16-byte aligned, 16-byte sized cubes; up to kStageBytes of
         // shared memory per CTA hold the cubes of the row's runs (the rest of the runs read global memory)
         const bool aa = (flags & NR_ANTI_ALIASING) != 0;
-        const int light = sh ? 5 : lights ? 4 : phong ? 3 : (smooth ? 2 : (p.face_light != nullptr ? 1 : 0));
         const uint32_t cube_bytes = (flags & NR_RETURN_RGB) ? (uint32_t)(ts * ts * ts) * 12u : 0u;
-        const bool stage = !uv && !smooth && !phong && (flags & NR_FWD_STAGE_TEXTURES) && !aa && (flags & NR_RETURN_RGB) && (cube_bytes % 16u) == 0 &&
-                           cube_bytes <= kStageBytes / 8 && ((uintptr_t)a->textures & 15) == 0;
+        const bool stage = !uv && light <= nr::kLightFace && (flags & NR_FWD_STAGE_TEXTURES) && !aa && (flags & NR_RETURN_RGB) &&
+                           (cube_bytes % 16u) == 0 && cube_bytes <= kStageBytes / 8 && ((uintptr_t)a->textures & 15) == 0;
         int nslots = 0;
         size_t smem = 0;
         if (stage) {
             nslots = (int)std::min<uint32_t>(kStageBytes / cube_bytes, (uint32_t)bx);
             smem = (size_t)nslots * cube_bytes;
-        }
-#define NR_RESOLVE(AA, TEX, LIT)                                                                    \
-    do {                                                                                            \
-        static nr_internal::SmemOptIn optin;                                                        \
-        if (optin.ensure(k_resolve<AA, TEX, LIT>, smem) != cudaSuccess) return NR_ERR_CUDA;         \
-        k_resolve<AA, TEX, LIT><<<grid, bx, smem, stream>>>(p, nslots);                             \
-    } while (0)
-#define NR_RESOLVE_LIT(AA, TEX)                                                                    \
-    do {                                                                                            \
-        if (light == 5) NR_RESOLVE(AA, TEX, 5);                                                     \
-        else if (light == 4) NR_RESOLVE(AA, TEX, 4);                                                \
-        else if (light == 3) NR_RESOLVE(AA, TEX, 3);                                                \
-        else if (light == 2) NR_RESOLVE(AA, TEX, 2);                                                \
-        else if (light == 1) NR_RESOLVE(AA, TEX, 1);                                                \
-        else NR_RESOLVE(AA, TEX, 0);                                                                \
-    } while (0)
-        if (!stage && !aa) {  // direct variant: 32 x 8 pixel tiles
+        } else if (!aa) {  // direct variant: 32 x 8 pixel tiles
             bx = 256;
             grid = dim3((width + kResolveTileW - 1) / kResolveTileW, (width + kResolveTileH - 1) / kResolveTileH, B);
         }
-        if (mip && aa) NR_RESOLVE_LIT(true, 3);
-        else if (mip) NR_RESOLVE_LIT(false, 3);
-        else if (uv && aa) NR_RESOLVE_LIT(true, 2);
-        else if (uv) NR_RESOLVE_LIT(false, 2);
-        else if (aa) NR_RESOLVE_LIT(true, 0);
-        else if (stage && light == 1) NR_RESOLVE(false, 1, 1);
-        else if (stage) NR_RESOLVE(false, 1, 0);
-        else NR_RESOLVE_LIT(false, 0);
-#undef NR_RESOLVE_LIT
-#undef NR_RESOLVE
+        int rc;
+        if (stage) {
+            rc = nr::dispatch_light<nr::kLightNone, nr::kLightFace>(
+                light, [&](auto kL) { return launch_resolve<false, 1, kL>(p, grid, bx, smem, nslots, stream); });
+        } else {
+            rc = nr::dispatch_bool(aa, [&](auto kAA) {
+                return nr::dispatch_light<nr::kLightNone, nr::kLightFace, nr::kLightCorner, nr::kLightPhong, nr::kLightPhongSet,
+                                          nr::kLightPhongSH>(light, [&](auto kL) {
+                    return mip  ? launch_resolve<kAA, 3, kL>(p, grid, bx, smem, nslots, stream)
+                           : uv ? launch_resolve<kAA, 2, kL>(p, grid, bx, smem, nslots, stream)
+                                : launch_resolve<kAA, 0, kL>(p, grid, bx, smem, nslots, stream);
+                });
+            });
+        }
+        if (rc != NR_OK) return rc;
     }
     return cudaGetLastError() == cudaSuccess ? NR_OK : NR_ERR_CUDA;
 }

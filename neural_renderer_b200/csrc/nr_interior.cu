@@ -10,7 +10,8 @@
 //                   the sampler's derivative comes from the nr_math.cuh helpers with the cell, the level of detail and the
 //                   clamps held fixed, and the 9 floats per pixel go through k_depth_grad's segmented run reduction before
 //                   one set of atomics per run.  kTex: 0 = per-face cubes, 1 = bilinear image, 2 = trilinear pyramid;
-//                   kLight: 0 = unlit, 1 = face_light, 2 = corner_light.  Anti-aliasing and fill_back are runtime flags.
+//                   kLight: kLightNone, kLightFace or kLightCorner (nr_shading.cuh).  Anti-aliasing and fill_back are
+//                   runtime flags.
 //
 // It belongs to the faces half of nr_b200_backward and runs after K5 / K7 into the same (already zero-filled) output.
 #include <cuda_runtime.h>
@@ -34,12 +35,11 @@ struct InteriorParams {
     size_t tex_bstride;     // floats per item in textures (0 = shared)
     const float* uvs;       // [.,F',3,2]
     uint32_t uv_bstride;    // floats per item in uvs (0 = shared)
-    const float* face_light;    // [B,F,3] (kLight 1)
-    const float* corner_light;  // [B,F,3,3] (kLight 2)
     int S, F, ts, Ht, Wt;
     int aa, fill_back;
     float tex_cmp, tex_val;
     nr::MipTable mip;  // kTex 2
+    nr::Shading shading;  // face_light (kLightFace) or corner_light (kLightCorner)
 };
 
 template <int kTex, int kLight, bool kIdx>
@@ -82,15 +82,12 @@ __global__ void __launch_bounds__(256) k_interior_grad(const __grid_constant__ I
         float lx[3], ly[3];
         nr::perspective_weight_grads(inv, z, zp, lam, lx, ly);
         // the light factor L_c of d rgb_c / d s_c
-        float L[3] = {1.0f, 1.0f, 1.0f}, C[9];
-        if constexpr (kLight == 1) {
-            const float* lp = p.face_light + ((size_t)b * p.F + fn) * 3;
-            L[0] = __ldg(lp); L[1] = __ldg(lp + 1); L[2] = __ldg(lp + 2);
-        } else if constexpr (kLight == 2) {
-            const float* cp = p.corner_light + ((size_t)b * p.F + fn) * 9;
+        float L[3], C[9];
+        nr::pixel_light<kLight>(p.shading, b, p.F, fn, lam, L);
+        if constexpr (kLight == nr::kLightCorner) {
+            const float* cp = p.shading.corner_light + p.shading.cl_off(b, p.F, fn);
 #pragma unroll
             for (int k = 0; k < 9; k++) C[k] = __ldg(cp + k);
-            nr::corner_light_at(cp, lam, L);
         }
         const float h[3] = {g[0] * L[0], g[1] * L[1], g[2] * L[2]};  // d loss / d unlit sample
         // fill_back: face f >= F/2 is the reversed copy of face f - F/2 (cube axes / UV corners reversed)
@@ -159,7 +156,7 @@ __global__ void __launch_bounds__(256) k_interior_grad(const __grid_constant__ I
 #pragma unroll
             for (int m = 0; m < 3; m++) P[m] = __fmaf_rn(gv, __fsub_rn(vv, uv[2 * m + 1]), __fmul_rn(gu, __fsub_rn(u, uv[2 * m])));
         }
-        if constexpr (kLight == 2) {
+        if constexpr (kLight == nr::kLightCorner) {
             // smooth shading: d rgb_c / d l_k also holds C_kc s_c; with gs_c = g_c s_c the corner differences give
             // sum_c gs_c (C_kc - C_0c) and sum_c gs_c (L_c - C_mc)
             const float gs[3] = {g[0] * s[0], g[1] * s[1], g[2] * s[2]};
@@ -204,19 +201,6 @@ __global__ void __launch_bounds__(256) k_interior_grad(const __grid_constant__ I
     }
 }
 
-template <int kTex, int kLight>
-void launch_l(const InteriorParams& p, bool idx, dim3 grid, cudaStream_t s) {
-    if (idx) k_interior_grad<kTex, kLight, true><<<grid, 256, 0, s>>>(p);
-    else k_interior_grad<kTex, kLight, false><<<grid, 256, 0, s>>>(p);
-}
-
-template <int kTex>
-void launch_t(const InteriorParams& p, int light, bool idx, dim3 grid, cudaStream_t s) {
-    if (light == 2) launch_l<kTex, 2>(p, idx, grid, s);
-    else if (light == 1) launch_l<kTex, 1>(p, idx, grid, s);
-    else launch_l<kTex, 0>(p, idx, grid, s);
-}
-
 }  // namespace
 
 namespace nr_internal {
@@ -230,20 +214,24 @@ void launch_interior_grad(const InteriorLaunch& L, cudaStream_t stream) {
     p.fim = a->face_index_map; p.wmap = a->weight_map; p.g = a->grad_rgb;
     p.textures = a->textures; p.tex_bstride = L.tex_bstride;
     p.uvs = a->face_uvs; p.uv_bstride = L.uv_bstride;
-    p.face_light = a->face_light; p.corner_light = L.corner_light;
+    p.shading = L.shading;
     p.S = a->raster_size; p.F = a->num_faces; p.ts = a->texture_size;
     p.Ht = a->texture_height; p.Wt = a->texture_width;
     p.aa = (flags & NR_ANTI_ALIASING) ? 1 : 0;
     p.fill_back = (flags & NR_TEX_FILL_BACK) ? 1 : 0;
     p.tex_cmp = L.tex_cmp; p.tex_val = L.tex_val;
     if (L.mip) p.mip = *L.mip;
-    const int light = L.corner_light ? 2 : (a->face_light ? 1 : 0);
     const bool idx = (flags & NR_FACES_INDEXED) != 0;
+    const int tex = (flags & NR_TEX_MIPMAP) ? 2 : (flags & NR_TEX_UV) ? 1 : 0;
     const dim3 grid((unsigned)(((size_t)p.S * p.S + 255) / 256), a->batch_size);
     LaunchScope ls("k_interior_grad", stream);
-    if (flags & NR_TEX_MIPMAP) launch_t<2>(p, light, idx, grid, stream);
-    else if (flags & NR_TEX_UV) launch_t<1>(p, light, idx, grid, stream);
-    else launch_t<0>(p, light, idx, grid, stream);
+    nr::dispatch_light<nr::kLightNone, nr::kLightFace, nr::kLightCorner>(L.light, [&](auto kL) {
+        nr::dispatch_bool(idx, [&](auto kIdx) {
+            if (tex == 2) k_interior_grad<2, kL, kIdx><<<grid, 256, 0, stream>>>(p);
+            else if (tex == 1) k_interior_grad<1, kL, kIdx><<<grid, 256, 0, stream>>>(p);
+            else k_interior_grad<0, kL, kIdx><<<grid, 256, 0, stream>>>(p);
+        });
+    });
 }
 
 }  // namespace nr_internal

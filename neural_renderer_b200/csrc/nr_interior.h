@@ -7,14 +7,16 @@
 #include "nr_b200.h"
 #include "nr_geom.cuh"
 #include "nr_math.cuh"
+#include "nr_shading.cuh"
 
 namespace nr_internal {
 
 struct InteriorLaunch {
-    const nr_b200_backward_args* args;  // the checked call (flags, maps, grad_rgb, textures, face_uvs, face_light)
+    const nr_b200_backward_args* args;  // the checked call (flags, maps, grad_rgb, textures, face_uvs)
     nr::FaceSrc src;
     nr::FaceGrad dst;
-    const float* corner_light;  // smooth shading, or nullptr
+    nr::Shading shading;        // the call's face_light or corner_light (nr_internal::make_shading)
+    int light;                  // its light mode: kLightNone, kLightFace or kLightCorner
     size_t tex_bstride;         // floats per item in `textures` (0 = shared)
     uint32_t uv_bstride;        // floats per item in face_uvs (0 = shared)
     float tex_cmp, tex_val;     // the cube clamp thresholds of the forward

@@ -6,6 +6,7 @@
 
 #include "nr_b200.h"
 #include "nr_geom.cuh"
+#include "nr_shading.cuh"
 
 namespace nr_internal {
 // kernels launched by the last forward/backward call on this thread (nr_b200_last_launch_count)
@@ -64,6 +65,40 @@ inline bool lights_args_ok(const nr_b200_lights_args* ls, int B) {
 // the same for an SH environment (nr_b200_sh_args)
 inline bool sh_args_ok(const nr_b200_sh_args* sh, int B) {
     return sh->struct_size == sizeof(nr_b200_sh_args) && sh->sh && (sh->sh_batch == 1 || sh->sh_batch == B);
+}
+
+// The light mode (nr_shading.cuh) and nr::Shading of a call from its ABI arguments, or -1 for a refused combination
+// (NR_ERR_INVALID_ARG): corner_light only for RGB and instead of face_light; Phong only for RGB and instead of both; the
+// Phong, light-set and SH structs pass their checks.  face_light is ignored without RGB, and a set of NL = 0 lights is
+// the Phong call exactly.
+inline int make_shading(bool rgb, const float* face_light, const float* corner_light, const nr_b200_phong_args* phong,
+                        const nr_b200_lights_args* lights, const nr_b200_sh_args* sh, int B, int F, nr::Shading* s) {
+    *s = nr::Shading{};
+    if (corner_light && (!rgb || face_light)) return -1;
+    if (phong && (!rgb || face_light || corner_light || !phong_args_ok(phong, B))) return -1;
+    if (lights && !lights_args_ok(lights, B)) return -1;
+    if (sh && !sh_args_ok(sh, B)) return -1;
+    if (lights && lights->num_lights == 0) lights = nullptr;
+    s->face_light = rgb ? face_light : nullptr;
+    s->corner_light = corner_light;
+    if (phong) {
+        s->cs = phong->corner_shading; s->prm = phong->params;
+        s->cs_bstride = phong->shading_batch == 1 ? 0 : (size_t)F;
+        s->prm_bstride = phong->params_batch == 1 ? 0 : 16;
+    }
+    if (lights) {
+        s->lts = lights->lights; s->NL = lights->num_lights;
+        s->lt_bstride = lights->lights_batch == 1 ? 0 : (size_t)lights->num_lights * 12;
+    }
+    if (sh) {
+        s->sh = sh->sh;
+        s->sh_bstride = sh->sh_batch == 1 ? 0 : 27;
+    }
+    if (sh) return nr::kLightPhongSH;
+    if (lights) return nr::kLightPhongSet;
+    if (phong) return nr::kLightPhong;
+    if (corner_light) return nr::kLightCorner;
+    return s->face_light ? nr::kLightFace : nr::kLightNone;
 }
 
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) is issued once per (kernel instantiation, device, size high-water

@@ -8,7 +8,9 @@
 //                   through k_depth_grad's segmented run reduction (runs of neighbouring lanes that show the same face)
 //                   before one set of atomics per run; the 16 parameter floats are summed over the warp, then over the CTA
 //                   in shared memory, before 16 atomics per CTA.  kTex: 0 = per-face cubes, 1 = bilinear image,
-//                   2 = trilinear pyramid.  Anti-aliasing and fill_back are runtime flags.
+//                   2 = trilinear pyramid.  Anti-aliasing and fill_back are runtime flags.  kLights / kSH split the
+//                   call's light mode (nr_shading.cuh) by register layout: kLightPhong = neither, kLightPhongSet =
+//                   kLights, kLightPhongSH = kSH with kLights when NL > 0.
 //                   kLights (a light set, NL > 0): after light 0 the pixel keeps its d loss / d nh, d vh and d p
 //                   accumulators across the loop over the lights (nr::phong_light_grad); each light's 10 record floats
 //                   are summed over the warp into shared memory, and after the loop over the CTA before 10 atomics per
@@ -42,25 +44,15 @@ struct PhongParams {
     size_t tex_bstride;     // floats per item in textures (0 = shared)
     const float* uvs;       // [.,F',3,2]
     uint32_t uv_bstride;    // floats per item in uvs (0 = shared)
-    const float* cs;        // corner_shading [Bc,F,3,6]
-    const float* prm;       // params [Bp,16]
-    float* grad_cs;         // or nullptr
-    float* grad_prm;        // or nullptr
-    size_t cs_bstride;      // faces per item in cs (0 with Bc = 1)
-    size_t prm_bstride;     // floats per item in prm (0 with Bp = 1)
+    float* grad_cs;         // the layouts of corner_shading, params, lights (kLights) and sh (kSH), or nullptr
+    float* grad_prm;
+    float* grad_lts;
+    float* grad_sh;
     int S, F, ts, Ht, Wt;
     int aa, fill_back, z_batch0;
     float tex_cmp, tex_val;
     nr::MipTable mip;  // kTex 2
-    // kLights: lights [Bl,NL,12] and their gradient (or nullptr)
-    const float* lts;
-    float* grad_lts;
-    size_t lt_bstride;      // floats per item in lts (0 with Bl = 1)
-    int NL;
-    // kSH: sh [Bs,9,3] and its gradient (or nullptr)
-    const float* sh;
-    float* grad_sh;
-    size_t sh_bstride;      // floats per item in sh (0 with Bs = 1)
+    nr::Shading shading;  // corner_shading, params, lights and sh
 };
 
 // kSH: the 27 floats Y_k w_c of grad_sh summed over the warp one at a time into shared memory, then over the CTA before 27
@@ -173,13 +165,13 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
                 nr::uv_blend<false>(img, p.Wt, nr::uv_taps(u, vv, p.Ht, p.Wt), 1.0f, 1.0f, 1.0f, s);
             }
         }
-        const float* prm = p.prm + (size_t)b * p.prm_bstride;
+        const float* prm = p.shading.prm + p.shading.prm_off(b);
         nr::PhongEval E;
-        nr::phong_at(p.cs + ((size_t)b * p.cs_bstride + fn) * 18, lam, prm, E);
+        nr::phong_at(p.shading.cs + p.shading.cs_off(b, fn), lam, prm, E);
         float gn[3], gp[3];
         nr::phong_grad(E, prm, g, s, gn, gp, gprm);
         if constexpr (kLights) {  // the set's gradients read neither E.L nor the set's diffuse terms
-            nr::phong_position(p.cs + ((size_t)b * p.cs_bstride + fn) * 18, lam, xpos);
+            nr::phong_position(p.shading.cs + p.shading.cs_off(b, fn), lam, xpos);
             xE = E;
 #pragma unroll
             for (int k = 0; k < 3; k++) {
@@ -191,7 +183,7 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
 #pragma unroll
                 for (int k = 0; k < 3; k++) shw[k] = __fmul_rn(g[k], s[k]);
                 nr::sh_basis(E.nh, shY);
-                nr::sh_grad_nh(p.sh + (size_t)b * p.sh_bstride, E.nh, shw, gnh);
+                nr::sh_grad_nh(p.shading.sh + p.shading.sh_off(b), E.nh, shw, gnh);
                 nr::normalize_eps_grad(E.n, E.n_len, gnh, t);
 #pragma unroll
                 for (int k = 0; k < 3; k++) gn[k] = __fadd_rn(gn[k], t[k]);
@@ -207,10 +199,10 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
     }
     if constexpr (kLights) {
         __shared__ float s_lt[8][nr_internal::kMaxLights * 10];  // per warp: each light's 10 record floats
-        const float* lts = p.lts + (size_t)b * p.lt_bstride;
-        const float sigma = __ldg(p.prm + (size_t)b * p.prm_bstride + 12);
+        const float* lts = p.shading.lts + p.shading.lts_off(b);
+        const float sigma = __ldg(p.shading.prm + p.shading.prm_off(b) + 12);
         float gnh[3] = {0.0f, 0.0f, 0.0f}, gvh[3] = {0.0f, 0.0f, 0.0f}, gsig = 0.0f;
-        for (int j = 0; j < p.NL; j++) {  // uniform
+        for (int j = 0; j < p.shading.NL; j++) {  // uniform
             float gl[10];
 #pragma unroll
             for (int k = 0; k < 10; k++) gl[k] = 0.0f;
@@ -232,14 +224,14 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
 #pragma unroll
                 for (int k = 0; k < 3; k++) ws[k] = __fmul_rn(xg[k], xs[k]);
                 nr::sh_basis(xE.nh, Y);
-                nr::sh_grad_nh(p.sh + (size_t)b * p.sh_bstride, xE.nh, ws, gnh);
+                nr::sh_grad_nh(p.shading.sh + p.shading.sh_off(b), xE.nh, ws, gnh);
             } else {
 #pragma unroll
                 for (int k = 0; k < 9; k++) Y[k] = 0.0f;
 #pragma unroll
                 for (int k = 0; k < 3; k++) ws[k] = 0.0f;
             }
-            if (p.grad_sh) sh_grad_reduce(Y, ws, p.grad_sh + (size_t)b * p.sh_bstride, lane, warp);  // uniform
+            if (p.grad_sh) sh_grad_reduce(Y, ws, p.grad_sh + p.shading.sh_off(b), lane, warp);  // uniform
         }
         if (fn >= 0) {
             nr::phong_lights_grad_end(xE, gnh, gvh, gsig, xgn, xgp, gprm);
@@ -254,15 +246,15 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
         if (p.grad_lts) {  // uniform: the CTA's sum of each light's 10 floats, then 10 atomics per light
             __syncthreads();
             const int nw = (int)(blockDim.x >> 5);
-            for (int t = threadIdx.x; t < 10 * p.NL; t += blockDim.x) {
+            for (int t = threadIdx.x; t < 10 * p.shading.NL; t += blockDim.x) {
                 float v = 0.0f;
                 for (int w = 0; w < nw; w++) v += s_lt[w][t];
-                atomicAdd(p.grad_lts + (size_t)b * p.lt_bstride + (size_t)(t / 10) * 12 + t % 10, v);
+                atomicAdd(p.grad_lts + p.shading.lts_off(b) + (size_t)(t / 10) * 12 + t % 10, v);
             }
         }
     }
     if constexpr (kSH && !kLights) {
-        if (p.grad_sh) sh_grad_reduce(shY, shw, p.grad_sh + (size_t)b * p.sh_bstride, lane, warp);  // uniform
+        if (p.grad_sh) sh_grad_reduce(shY, shw, p.grad_sh + p.shading.sh_off(b), lane, warp);  // uniform
     }
     if (p.grad_cs) {  // uniform
         // the segmented run reduction of k_depth_grad over 18 floats, then one set of atomics per run
@@ -280,7 +272,7 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
             }
         }
         if (fn >= 0 && ((heads >> lane) & 1u)) {
-            float* o = p.grad_cs + ((size_t)b * p.cs_bstride + fn) * 18;
+            float* o = p.grad_cs + p.shading.cs_off(b, fn);
 #pragma unroll
             for (int k = 0; k < 18; k++) atomicAdd(o + k, cg[k]);
         }
@@ -299,21 +291,9 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
             float t = 0.0f;
             const int nw = (int)(blockDim.x >> 5);
             for (int w = 0; w < nw; w++) t += s_prm[w][threadIdx.x];
-            atomicAdd(p.grad_prm + (size_t)b * p.prm_bstride + threadIdx.x, t);
+            atomicAdd(p.grad_prm + p.shading.prm_off(b) + threadIdx.x, t);
         }
     }
-}
-
-template <int kTex>
-void launch_t(const PhongParams& p, bool idx, dim3 grid, cudaStream_t s) {
-    if (p.sh && p.NL > 0 && idx) k_phong_grad<kTex, true, true, true><<<grid, 256, 0, s>>>(p);
-    else if (p.sh && p.NL > 0) k_phong_grad<kTex, false, true, true><<<grid, 256, 0, s>>>(p);
-    else if (p.sh && idx) k_phong_grad<kTex, true, false, true><<<grid, 256, 0, s>>>(p);
-    else if (p.sh) k_phong_grad<kTex, false, false, true><<<grid, 256, 0, s>>>(p);
-    else if (p.NL > 0 && idx) k_phong_grad<kTex, true, true, false><<<grid, 256, 0, s>>>(p);
-    else if (p.NL > 0) k_phong_grad<kTex, false, true, false><<<grid, 256, 0, s>>>(p);
-    else if (idx) k_phong_grad<kTex, true, false, false><<<grid, 256, 0, s>>>(p);
-    else k_phong_grad<kTex, false, false, false><<<grid, 256, 0, s>>>(p);
 }
 
 }  // namespace
@@ -322,7 +302,6 @@ namespace nr_internal {
 
 void launch_phong_grad(const PhongGradLaunch& L, cudaStream_t stream) {
     const nr_b200_backward_args* a = L.args;
-    const nr_b200_phong_args* ph = L.phong;
     const uint32_t flags = a->flags;
     PhongParams p;
     memset(&p, 0, sizeof(p));
@@ -330,10 +309,7 @@ void launch_phong_grad(const PhongGradLaunch& L, cudaStream_t stream) {
     p.fim = a->face_index_map; p.wmap = a->weight_map; p.dmap = a->depth_map; p.g = a->grad_rgb;
     p.textures = a->textures; p.tex_bstride = L.tex_bstride;
     p.uvs = a->face_uvs; p.uv_bstride = L.uv_bstride;
-    p.cs = ph->corner_shading; p.prm = ph->params;
-    p.grad_cs = ph->grad_corner_shading; p.grad_prm = ph->grad_params;
-    p.cs_bstride = ph->shading_batch == 1 ? 0 : (size_t)a->num_faces;
-    p.prm_bstride = ph->params_batch == 1 ? 0 : 16;
+    p.grad_cs = L.grad_cs; p.grad_prm = L.grad_prm; p.grad_lts = L.grad_lts; p.grad_sh = L.grad_sh;
     p.S = a->raster_size; p.F = a->num_faces; p.ts = a->texture_size;
     p.Ht = a->texture_height; p.Wt = a->texture_width;
     p.aa = (flags & NR_ANTI_ALIASING) ? 1 : 0;
@@ -341,20 +317,22 @@ void launch_phong_grad(const PhongGradLaunch& L, cudaStream_t stream) {
     p.z_batch0 = (flags & NR_TEX_Z_BATCH0) ? 1 : 0;
     p.tex_cmp = L.tex_cmp; p.tex_val = L.tex_val;
     if (L.mip) p.mip = *L.mip;
-    if (L.lights) {
-        p.lts = L.lights->lights; p.grad_lts = L.lights->grad_lights; p.NL = L.lights->num_lights;
-        p.lt_bstride = L.lights->lights_batch == 1 ? 0 : (size_t)p.NL * 12;
-    }
-    if (L.sh) {
-        p.sh = L.sh->sh; p.grad_sh = L.sh->grad_sh;
-        p.sh_bstride = L.sh->sh_batch == 1 ? 0 : 27;
-    }
+    p.shading = L.shading;
     const bool idx = (flags & NR_FACES_INDEXED) != 0;
+    const int tex = (flags & NR_TEX_MIPMAP) ? 2 : (flags & NR_TEX_UV) ? 1 : 0;
     const dim3 grid((unsigned)(((size_t)p.S * p.S + 255) / 256), a->batch_size);
     LaunchScope ls("k_phong_grad", stream);
-    if (flags & NR_TEX_MIPMAP) launch_t<2>(p, idx, grid, stream);
-    else if (flags & NR_TEX_UV) launch_t<1>(p, idx, grid, stream);
-    else launch_t<0>(p, idx, grid, stream);
+    // the kernel's split of the mode: a light set of NL > 0 lights (kLightPhongSet, or kLightPhongSH with one), an SH
+    // environment
+    nr::dispatch_bool(p.shading.NL > 0, [&](auto kLights) {
+        nr::dispatch_bool(L.light == nr::kLightPhongSH, [&](auto kSH) {
+            nr::dispatch_bool(idx, [&](auto kIdx) {
+                if (tex == 2) k_phong_grad<2, kIdx, kLights, kSH><<<grid, 256, 0, stream>>>(p);
+                else if (tex == 1) k_phong_grad<1, kIdx, kLights, kSH><<<grid, 256, 0, stream>>>(p);
+                else k_phong_grad<0, kIdx, kLights, kSH><<<grid, 256, 0, stream>>>(p);
+            });
+        });
+    });
 }
 
 }  // namespace nr_internal

@@ -1,4 +1,4 @@
-// nr_phong.h -- host interface of the Phong-gradient kernel (nr_phong.cu) for nr_b200_backward_phong (not part of the ABI).
+// nr_phong.h -- host interface of the Phong-gradient kernel (nr_phong.cu) for the Phong light modes of the backward (not part of the ABI).
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>
@@ -7,14 +7,18 @@
 #include "nr_b200.h"
 #include "nr_geom.cuh"
 #include "nr_math.cuh"
+#include "nr_shading.cuh"
 
 namespace nr_internal {
 
 struct PhongGradLaunch {
     const nr_b200_backward_args* args;  // the checked call (flags, maps, grad_rgb, textures, face_uvs)
-    const nr_b200_phong_args* phong;    // the checked Phong inputs and gradient outputs
-    const nr_b200_lights_args* lights;  // the checked light set (NL > 0), or nullptr
-    const nr_b200_sh_args* sh;          // the checked SH environment, or nullptr
+    nr::Shading shading;                // the call's Phong inputs (nr_internal::make_shading)
+    int light;                          // its light mode: kLightPhong, kLightPhongSet or kLightPhongSH
+    float* grad_cs;                     // d loss / d corner_shading, params, lights (NL > 0) and sh, or nullptr
+    float* grad_prm;
+    float* grad_lts;
+    float* grad_sh;
     nr::FaceSrc src;
     size_t tex_bstride;       // floats per item in `textures` (0 = shared)
     uint32_t uv_bstride;      // floats per item in face_uvs (0 = shared)

@@ -1,0 +1,120 @@
+// nr_shading.cuh -- what lights a pixel: the light mode of a call and the shading inputs it reads, the counterpart of
+// nr_geom.cuh's "where a face comes from".
+//
+// The host picks the mode and fills one nr::Shading from the ABI arguments (nr_internal::make_shading, nr_internal.h);
+// every kernel that shades or differentiates a pixel is instantiated per mode and reads its inputs from that record.
+#pragma once
+#include <cuda_runtime.h>
+#include <stddef.h>
+
+#include <type_traits>
+
+#include "nr_math.cuh"
+
+namespace nr {
+
+// The light modes, in the order of their template parameter kLight.
+constexpr int kLightNone = 0;      // unlit
+constexpr int kLightFace = 1;      // face_light [B,F,3] multiplies every texel inside the samplers.  The backward
+                                   // kernels have no mode-1 instantiation: their kLightNone variant serves unlit and
+                                   // face_light calls alike and tests the face_light pointer at run time.
+constexpr int kLightCorner = 2;    // corner_light [B,F,3,3] interpolated to the pixel multiplies the unlit sample
+constexpr int kLightPhong = 3;     // Phong shading of the unlit sample (corner_shading, params)
+constexpr int kLightPhongSet = 4;  // the same with a light set of NL > 0 lights
+constexpr int kLightPhongSH = 5;   // the same with an SH environment, and a light set of NL >= 0 lights
+
+// The shading inputs of one call; strides are 0 for a set shared by every batch item.
+struct Shading {
+    const float* face_light;    // [B,F,3] (kLightFace), or nullptr
+    const float* corner_light;  // [B,F,3,3] (kLightCorner), or nullptr
+    const float* cs;            // corner_shading [Bc,F,3,6] (the Phong modes)
+    const float* prm;           // params [Bp,16]
+    size_t cs_bstride;          // faces per item in cs (0 with Bc = 1)
+    size_t prm_bstride;         // floats per item in prm (0 with Bp = 1)
+    const float* lts;           // lights [Bl,NL,12] (kLightPhongSet, kLightPhongSH), or nullptr with NL = 0
+    size_t lt_bstride;          // floats per item in lts (0 with Bl = 1)
+    int NL;
+    const float* sh;            // [Bs,9,3] (kLightPhongSH)
+    size_t sh_bstride;          // floats per item in sh (0 with Bs = 1)
+
+    // float offsets of item b's records (and of face fn's; F = faces per item of the [B,F,...] light tensors), shared
+    // with the gradients of the same layout
+    __host__ __device__ __forceinline__ size_t fl_off(int b, int F, int fn) const { return ((size_t)b * F + fn) * 3; }
+    __host__ __device__ __forceinline__ size_t cl_off(int b, int F, int fn) const { return ((size_t)b * F + fn) * 9; }
+    __host__ __device__ __forceinline__ size_t cs_off(int b, int fn) const { return ((size_t)b * cs_bstride + fn) * 18; }
+    __host__ __device__ __forceinline__ size_t prm_off(int b) const { return (size_t)b * prm_bstride; }
+    __host__ __device__ __forceinline__ size_t lts_off(int b) const { return (size_t)b * lt_bstride; }
+    __host__ __device__ __forceinline__ size_t sh_off(int b) const { return (size_t)b * sh_bstride; }
+};
+
+// L_c = d rgb_c / d s_c of face fn's pixel with perspective weights l (own vertex depths): 1, face_light, the
+// interpolated corner light, or the diffuse part of the Phong expression (with the set's diffuse terms, then E_c)
+template <int kLight>
+__device__ __forceinline__ void pixel_light(const Shading& s, int b, int F, int fn, const float l[3], float L[3]) {
+    if constexpr (kLight == kLightNone) {
+        L[0] = L[1] = L[2] = 1.0f;
+    } else if constexpr (kLight == kLightFace) {
+        const float* lp = s.face_light + s.fl_off(b, F, fn);
+        L[0] = __ldg(lp); L[1] = __ldg(lp + 1); L[2] = __ldg(lp + 2);
+    } else if constexpr (kLight == kLightCorner) {
+        corner_light_at(s.corner_light + s.cl_off(b, F, fn), l, L);
+    } else {
+        const float* cs = s.cs + s.cs_off(b, fn);
+        PhongEval E;
+        phong_diffuse(cs, l, s.prm + s.prm_off(b), E);
+        if constexpr (kLight >= kLightPhongSet) {
+            float pos[3];
+            phong_position(cs, l, pos);
+            lights_diffuse_loop(s.lts + s.lts_off(b), s.NL, pos, E);
+        }
+        if constexpr (kLight == kLightPhongSH) sh_add_irradiance(s.sh + s.sh_off(b), E);
+        L[0] = E.L[0]; L[1] = E.L[1]; L[2] = E.L[2];
+    }
+}
+
+// rgb of face fn's pixel from its unlit sample c (in place) and perspective weights l, for the modes that shade the
+// sample after sampling (kLightCorner and the Phong modes; face_light is applied per texel by the samplers)
+template <int kLight>
+__device__ __forceinline__ void shade(const Shading& s, int b, int F, int fn, const float l[3], float c[3]) {
+    static_assert(kLight >= kLightCorner, "unlit and face_light samples are final");
+    if constexpr (kLight == kLightCorner) {
+        float L[3];
+        corner_light_at(s.corner_light + s.cl_off(b, F, fn), l, L);
+        c[0] = __fmul_rn(L[0], c[0]); c[1] = __fmul_rn(L[1], c[1]); c[2] = __fmul_rn(L[2], c[2]);
+    } else {
+        const float* prm = s.prm + s.prm_off(b);
+        const float* lts = s.lts + s.lts_off(b);  // the set modes
+        const float* cs = s.cs + s.cs_off(b, fn);
+        PhongEval E;
+        phong_at(cs, l, prm, E);
+        float rgb[3];
+        if constexpr (kLight == kLightPhong) {
+            phong_rgb(E, prm, c, rgb);
+        } else {
+            float pos[3];
+            phong_position(cs, l, pos);
+            lights_diffuse_loop(lts, s.NL, pos, E);
+            if constexpr (kLight == kLightPhongSH) sh_add_irradiance(s.sh + s.sh_off(b), E);
+            phong_lights_rgb(E, pos, prm, lts, s.NL, c, rgb);
+        }
+        c[0] = rgb[0]; c[1] = rgb[1]; c[2] = rgb[2];
+    }
+}
+
+// Host-side dispatch of a run-time choice to a compile-time one.  dispatch_light<kModes...>(mode, fn) calls
+// fn(std::integral_constant<int, M>{}) for the M of kModes equal to mode (the modes the launched kernel is instantiated
+// for; the caller never passes another, the last listed one would take it) and returns what fn returns.
+template <int kMode, int... kRest, class Fn>
+inline auto dispatch_light(int mode, Fn&& fn) {
+    if constexpr (sizeof...(kRest) > 0) {
+        if (mode != kMode) return dispatch_light<kRest...>(mode, fn);
+    }
+    return fn(std::integral_constant<int, kMode>{});
+}
+// fn(std::true_type{}) or fn(std::false_type{})
+template <class Fn>
+inline auto dispatch_bool(bool v, Fn&& fn) {
+    return v ? fn(std::true_type{}) : fn(std::false_type{});
+}
+
+}  // namespace nr

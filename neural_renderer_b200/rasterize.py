@@ -344,17 +344,11 @@ class _RasterizeFunction(torch.autograd.Function):
             a.corner_light = _ptr(corner_c)
             if cs_c is None:
                 _lib.check(lib.nr_b200_forward(ctypes.byref(a), _stream_ptr(dev)))
-            elif sh_c is not None:
-                ph, sa = _phong_args(cs_c, sp_c), _sh_args(sh_c)
-                la = _lights_args(lt_c) if lt_c is not None else None
-                _lib.check(lib.nr_b200_forward_sh(ctypes.byref(a), ctypes.byref(ph), ctypes.byref(la) if la is not None else None,
-                                                  ctypes.byref(sa), _stream_ptr(dev)))
-            elif lt_c is not None:
-                ph, la = _phong_args(cs_c, sp_c), _lights_args(lt_c)
-                _lib.check(lib.nr_b200_forward_lights(ctypes.byref(a), ctypes.byref(ph), ctypes.byref(la), _stream_ptr(dev)))
-            else:
+            else:  # every Phong render, with NULL lights / sh where absent
                 ph = _phong_args(cs_c, sp_c)
-                _lib.check(lib.nr_b200_forward_phong(ctypes.byref(a), ctypes.byref(ph), _stream_ptr(dev)))
+                la = _lights_args(lt_c) if lt_c is not None else None
+                sa = _sh_args(sh_c) if sh_c is not None else None
+                _lib.check(lib.nr_b200_forward_sh(ctypes.byref(a), ctypes.byref(ph), _byref(la), _byref(sa), _stream_ptr(dev)))
         ctx.cfg = cfg
         ctx.flags = flags
         ctx.ts = ts
@@ -435,13 +429,8 @@ class _RasterizeFunction(torch.autograd.Function):
             hook = _TEXTURE_GRAD_HOOK if (want_rgb and g_rgb is not None) else None
 
             def call():
-                if sa is not None:  # SH environment (with or without a light set): grad_sh is filled by the texture half
-                    return lib.nr_b200_backward_sh(ctypes.byref(a), ctypes.byref(ph), ctypes.byref(la) if la is not None else None,
-                                                   ctypes.byref(sa), _stream_ptr(dev))
-                if la is not None:  # light set: grad_lights too is filled by the texture half
-                    return lib.nr_b200_backward_lights(ctypes.byref(a), ctypes.byref(ph), ctypes.byref(la), _stream_ptr(dev))
-                if ph is not None:  # Phong: grad_corner_shading / grad_params are filled by the texture half
-                    return lib.nr_b200_backward_phong(ctypes.byref(a), ctypes.byref(ph), _stream_ptr(dev))
+                if ph is not None:  # Phong: grad_corner_shading, grad_params, grad_lights, grad_sh are filled by the texture half
+                    return lib.nr_b200_backward_sh(ctypes.byref(a), ctypes.byref(ph), _byref(la), _byref(sa), _stream_ptr(dev))
                 if corner_c is None:
                     return lib.nr_b200_backward(ctypes.byref(a), _stream_ptr(dev))
                 # smooth shading: grad_corner_light is filled by the texture half
@@ -461,6 +450,21 @@ class _RasterizeFunction(torch.autograd.Function):
                 if pending is not None:
                     pending.wait()
         return grad_geom, grad_textures, grad_light, None, None, grad_uvs, grad_corner, grad_cs, grad_sp, grad_lt, grad_sh
+
+
+def _byref(s):
+    return ctypes.byref(s) if s is not None else None
+
+
+def _batched(t, batch_size, dims=None):
+    """t as float32 with the batch axis added when it has `dims` dimensions; an expanded (stride-0) batch of batch_size
+    collapses to one shared item, which the kernels read in place."""
+    t = t if t.dtype == torch.float32 else t.float()
+    if t.dim() == dims:
+        t = t[None]
+    if t.shape[0] == batch_size > 1 and t.stride(0) == 0:
+        t = t[:1]
+    return t
 
 
 def _phong_args(cs_c, sp_c, grad_cs=None, grad_sp=None):
@@ -553,40 +557,20 @@ def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_
     if not return_rgb:
         face_uvs = None
     if return_rgb:
-        if textures.dtype != torch.float32:
-            textures = textures.float()
+        # a texture image [Ht,Wt,3] (with face_uvs) is one image for every item; shared sets are read in place
+        # (NR_TEX_SHARED, NR_UV_SHARED, Bc / Bp / Bl / Bs = 1)
+        textures = _batched(textures, batch_size, 3 if face_uvs is not None else None)
         if face_uvs is not None:
-            if textures.dim() == 3:
-                textures = textures[None]  # one image for every item
-            face_uvs = face_uvs.float() if face_uvs.dtype != torch.float32 else face_uvs
-            if face_uvs.dim() == 3:
-                face_uvs = face_uvs[None]
-            if face_uvs.shape[0] == batch_size > 1 and face_uvs.stride(0) == 0:
-                face_uvs = face_uvs[:1]  # an expanded shared UV set (NR_UV_SHARED)
-        if textures.shape[0] == batch_size > 1 and textures.stride(0) == 0:
-            textures = textures[:1]  # an expanded shared texture set: sample it in place (NR_TEX_SHARED)
+            face_uvs = _batched(face_uvs, batch_size, 3)
         if phong:
-            corner_shading = corner_shading.float() if corner_shading.dtype != torch.float32 else corner_shading
-            shading_params = shading_params.float() if shading_params.dtype != torch.float32 else shading_params
-            corner_shading = corner_shading[None] if corner_shading.dim() == 3 else corner_shading
-            shading_params = shading_params[None] if shading_params.dim() == 1 else shading_params
-            if corner_shading.shape[0] == batch_size > 1 and corner_shading.stride(0) == 0:
-                corner_shading = corner_shading[:1]  # an expanded shared set (Bc = 1)
-            if shading_params.shape[0] == batch_size > 1 and shading_params.stride(0) == 0:
-                shading_params = shading_params[:1]
+            corner_shading = _batched(corner_shading, batch_size, 3)
+            shading_params = _batched(shading_params, batch_size, 1)
             if lights is not None:
-                lights = lights.float() if lights.dtype != torch.float32 else lights
-                lights = lights[None] if lights.dim() == 2 else lights
-                if lights.shape[0] == batch_size > 1 and lights.stride(0) == 0:
-                    lights = lights[:1]  # an expanded shared set (Bl = 1)
+                lights = _batched(lights, batch_size, 2)
                 if lights.shape[1] == 0:
                     lights = None  # no extra light: Phong exactly
             if environment_sh is not None:
-                sh = environment_sh.float() if environment_sh.dtype != torch.float32 else environment_sh
-                sh = sh[None] if sh.dim() == 2 else sh
-                if sh.shape[0] == batch_size > 1 and sh.stride(0) == 0:
-                    sh = sh[:1]  # an expanded shared environment (Bs = 1)
-                environment_sh = sh
+                environment_sh = _batched(environment_sh, batch_size, 2)
     cfg = _make_config(image_size, anti_aliasing, near, far, eps, background_color, return_rgb, return_alpha,
                        return_depth, geom.device, batch_size, reference_exact)
     if return_rgb and textures_fill_back:
@@ -913,11 +897,7 @@ def rasterize_attributes(
     else:
         geom = faces if faces.dtype == torch.float32 else faces.float()
     batch_size = geom.shape[0]
-    attrs = attrs if attrs.dtype == torch.float32 else attrs.float()
-    if attrs.dim() == (2 if per_vertex else 3):
-        attrs = attrs[None]
-    if attrs.shape[0] == batch_size > 1 and attrs.stride(0) == 0:
-        attrs = attrs[:1]  # an expanded shared set (NR_ATTR_SHARED)
+    attrs = _batched(attrs, batch_size, 2 if per_vertex else 3)  # an expanded shared set: NR_ATTR_SHARED
     _, alpha, _, fim, wmap = _run(indices if indices is not None else geom, None, image_size, anti_aliasing, near, far,
                                   eps, None, False, True, False, vertices=geom if indices is not None else None)
     flags = (_lib.NR_ANTI_ALIASING if anti_aliasing else 0) | (_lib.NR_ATTR_PER_VERTEX if per_vertex else 0)
