@@ -17,7 +17,14 @@ per corner) needs RGB, the short struct layouts (ending before corner_light / gr
 per-vertex attributes need indexed geometry, and the interior gradient refuses per-face cubes sampled with the depths of
 item 0 (NR_TEX_Z_BATCH0) at B > 1; fill_back doubles the faces (F even) and anti-aliasing doubles the raster (even) by
 construction of the geometry, so no case is skipped.  The attribute channel count C is not a dimension: it rotates over
-ATTR_CHANNELS with the case id (abi_harness.Plan)."""
+ATTR_CHANNELS with the case id (abi_harness.Plan).
+
+The Phong light modes (light "phong", "phong_set", "phong_sh": nr_b200_*_phong / _lights / _sh) joined as a fourth
+stage.  Their dimensions -- the batch of each shading input (Bc, Bp, Bl, Bs: one set shared by every item, or one per
+item), the light count NL, the entry point and the shininess -- mean something only under a Phong level and are None
+elsewhere, so the cases of the earlier stages keep every level they had.  Attribute interpolation reads only the maps,
+which shading leaves as they are, so it is None under a Phong level.  Phong needs RGB and refuses the interior
+gradient; NL = 0 (SH without a light set) exists only with the SH environment, and a set of NL = 0 lights has no batch."""
 import itertools
 
 DIMS = [
@@ -29,7 +36,7 @@ DIMS = [
     ("ts", [2, 3, 4, 5, 6]),
     ("image", ["item", "shared"]),
     ("uvs", ["item", "shared"]),
-    ("light", ["none", "face", "corner"]),
+    ("light", ["none", "face", "corner", "phong", "phong_set", "phong_sh"]),
     ("bg", ["uniform", "per_batch"]),
     ("outputs", ["r", "a", "d", "ra", "rd", "ad", "rad"]),
     ("z_batch0", [False, True]),
@@ -42,13 +49,42 @@ DIMS = [
     ("layout", ["full", "short"]),
     ("attr", ["off", "corner", "corner_shared", "vertex", "vertex_shared"]),
     ("interior", ["off", "on"]),
+    # the Phong modes (abi_harness.Plan): NL, the entry point, Bc, Bp, Bl, Bs ("shared" = 1, "item" = B) and sigma (16:
+    # the shininess the feature tests hold the gradients at; at 64, q^sigma multiplies the fp32 error of q by sigma and
+    # grad_params / grad_lights per element reach 8.8e-4 / 5.2e-4 against gates of 5e-4 / 2e-4)
+    ("nl", [0, 1, 3, 8]),
+    ("entry", ["own", "via_sh", "via_lights_nl0"]),
+    ("shading_batch", ["shared", "item"]),
+    ("params_batch", ["shared", "item"]),
+    ("lights_batch", ["shared", "item"]),
+    ("sh_batch", ["shared", "item"]),
+    ("sigma", [1.0, 16.0]),
 ]
 NAMES = [n for n, _ in DIMS]
 LEVELS = dict(DIMS)
 
 
-def active(dim, kind):
-    """whether `dim` means anything for texture kind `kind`"""
+PHONG = ("phong", "phong_set", "phong_sh")
+PHONG_DIMS = ["nl", "entry", "shading_batch", "params_batch", "lights_batch", "sh_batch", "sigma"]
+OLD_LIGHTS = ["none", "face", "corner"]
+
+
+def active(dim, c):
+    """whether `dim` means anything for the case (or partial case) `c`: its texture kind, and for the Phong dimensions
+    its light and light count"""
+    kind, light = c["kind"], c.get("light")
+    if dim in ("shading_batch", "params_batch", "sigma"):
+        return light in PHONG
+    if dim == "entry":  # nr_b200_*_sh is the SH mode's own entry point
+        return light in ("phong", "phong_set")
+    if dim == "nl":
+        return light in ("phong_set", "phong_sh")
+    if dim == "lights_batch":
+        return light in ("phong_set", "phong_sh") and c.get("nl") != 0
+    if dim == "sh_batch":
+        return light == "phong_sh"
+    if dim == "attr":  # the interpolation reads only the maps, which shading does not change
+        return light not in PHONG
     if dim == "ts":
         return kind in ("cube", "cube_shared")
     if dim in ("image", "uvs", "uv_grad"):
@@ -74,7 +110,29 @@ def compatible(a):
     if (a.get("interior") == "on" and kind in ("cube", "cube_shared") and a.get("z_batch0") is True
             and a.get("batch") == "B3"):
         return False  # the cubes would be sampled with item 0's depths: the derivative would cross items (refused)
+    light = a.get("light")
+    if light in PHONG and a.get("interior") == "on":
+        return False  # no vertex gradient through the Phong normal and position (NR_ERR_UNSUPPORTED)
+    if a.get("nl") == 0 and (light == "phong_set" or a.get("lights_batch") is not None):
+        return False  # NL = 0 is SH without a set: the set modes have lights, and no set has no batch
+    if a.get("entry") == "via_lights_nl0" and light not in (None, "phong"):
+        return False  # an empty light set is the plain Phong call
     return True
+
+
+def _context(a):
+    """the first completion of partial assignment `a` by a texture kind (and, for a Phong dimension, a light and NL)
+    under which each of its dimensions means something and the rules hold, or None"""
+    kinds = [a["kind"]] if "kind" in a else LEVELS["kind"]
+    lights, nls = [None], [None]
+    if any(d in PHONG_DIMS for d in a):
+        lights = [a["light"]] if "light" in a else list(PHONG)
+        nls = [a["nl"]] if "nl" in a else [None] + LEVELS["nl"]
+    for k, lt, nl in itertools.product(kinds, lights, nls):
+        c = {**a, "kind": k, **({"light": lt} if lt is not None else {}), **({"nl": nl} if nl is not None else {})}
+        if all(active(d, c) for d in a if d != "kind") and compatible(c):
+            return c
+    return None
 
 
 def required_pairs(levels=LEVELS):
@@ -84,10 +142,7 @@ def required_pairs(levels=LEVELS):
         for l1 in levels[d1]:
             for l2 in levels[d2]:
                 a = {d1: l1, d2: l2}
-                if not compatible(a):
-                    continue
-                kinds = [a["kind"]] if "kind" in a else LEVELS["kind"]
-                if any(active(d1, k) and active(d2, k) and compatible({**a, "kind": k}) for k in kinds):
+                if compatible(a) and _context(a) is not None:
                     out.add(((d1, l1), (d2, l2)))
     return out
 
@@ -103,7 +158,7 @@ def _fill(case, covered, order, choices=LEVELS):
     for name in NAMES:
         if name in case:
             continue
-        if not active(name, case["kind"]):
+        if not active(name, case):
             case[name] = None
             continue
         levels = choices[name]
@@ -172,9 +227,13 @@ MUST_NEW += [{"kind": "cube", "stage": True, "_aa": False, "pointers": "fresh", 
          {"kind": "cube_shared", "stage": True, "_aa": False, "pointers": "fresh", "ts": 4, "light": "none"},
          {"kind": "cube", "stage": True, "_aa": False, "pointers": "fresh", "ts": 6, "light": "none", "fill_back": False,
           "batch": "B3", "raster": "even"}]
-# the matrix as it stood before the interior vertex gradient joined it: every level but that flag, held off
-FROZEN = {**LEVELS, "interior": ["off"]}
-FROZEN_PAIRS = {n: LEVELS[n] for n in NAMES if n != "interior"}
+# the matrix as it stood before the interior vertex gradient joined it: every level but that flag, held off (and
+# without the Phong modes)
+FROZEN = {**LEVELS, "light": OLD_LIGHTS, "interior": ["off"]}
+FROZEN_PAIRS = {n: FROZEN[n] for n in NAMES if n != "interior" and n not in PHONG_DIMS}
+# the matrix as it stood before the Phong modes joined it
+INTERIOR = {**LEVELS, "light": OLD_LIGHTS}
+INTERIOR_PAIRS = {n: INTERIOR[n] for n in NAMES if n not in PHONG_DIMS}
 
 # the interior vertex gradient (NR_GRAD_INTERIOR) with an rgb upstream gradient, for every texture kind: every light, a
 # fresh and an accumulating backward, one call and two halves, with and without fill_back and anti-aliasing, spread over
@@ -205,6 +264,47 @@ MUST_INTERIOR = [{"kind": kind, "light": light, "fill_back": fb, "_aa": aa, "bac
                   "interior": "on", "upstream": ("all", "only_rgb")[i % 2], **extra}
                  for i, (kind, light, fb, aa, bwd, geom, batch, extra) in enumerate(_I)]
 
+# The Phong modes, every shading gradient given (optional pointers) with an rgb upstream gradient, for every texture
+# kind: a fresh and an accumulating backward, one call and two halves in both orders, with and without fill_back and
+# anti-aliasing.  The geometry and NL of the rows reach every instantiation k_phong_grad<kTex, kIdx, kLights, kSH>
+# (nr_phong.cu) -- per-face and indexed geometry under Phong alone, a light set, SH without a set (NL = 0) and SH with
+# one -- and the full set of 8 lights (s_lt[8][80]) at least once per texture kind.
+PHONG_ROWS = [(False, False, "one", "faces"), (True, True, "acc_halves", "idx_item"), (True, False, "faces_tex", "idx_shared"),
+              (False, True, "acc_one", "faces")]
+PHONG_NL = {"phong_set": [8, 3, 1, 3], "phong_sh": [0, 0, 8, 1]}
+MUST_PHONG = [{"kind": kind, "light": mode, "fill_back": fb, "_aa": aa, "backward": bwd, "geometry": geom,
+               "optional": "given", "upstream": ("all", "only_rgb")[i % 2],
+               **({"nl": PHONG_NL[mode][i]} if mode in PHONG_NL else {})}
+              for mode in PHONG for kind in ("cube", "cube_shared", "uv", "mip")
+              for i, (fb, aa, bwd, geom) in enumerate(PHONG_ROWS)]
+# cube Phong with NR_TEX_Z_BATCH0 at three items on per-item index sets: the sampler (forward and k_phong_grad) reads item
+# 0's depths, the perspective weights l_k of the normal and position the item's own
+MUST_PHONG += [{"kind": kind, "light": mode, "z_batch0": True, "batch": "B3", "geometry": "idx_item", "optional": "given",
+                "upstream": "all", **nl}
+               for kind, mode, nl in (("cube", "phong", {}), ("cube", "phong_set", {"nl": 3}),
+                                      ("cube_shared", "phong_sh", {"nl": 0}), ("cube_shared", "phong_sh", {"nl": 3}))]
+# the short forward / backward layouts under every mode: the NaN field past the forward's struct_size is corner_light,
+# which the host would refuse next to a Phong struct if it read it
+MUST_PHONG += [{"kind": kind, "light": mode, "layout": "short", "optional": "given", "upstream": "all"}
+               for kind, mode in (("cube", "phong"), ("uv", "phong_set"), ("mip", "phong_sh"))]
+# every shading gradient given without an rgb upstream gradient: fresh ones come back 0, accumulated ones keep their
+# prefill bit for bit (slots 10-11 of grad_lights included)
+MUST_PHONG += [{"kind": kind, "light": mode, "upstream": "no_rgb", "outputs": "rad", "optional": "given", "backward": bwd,
+                **nl}
+               for kind, mode, nl in (("cube", "phong", {}), ("uv", "phong_set", {"nl": 3}), ("mip", "phong_sh", {"nl": 8}))
+               for bwd in ("one", "acc_one")]
+# Bc = Bp = Bl = Bs = 1 at three items, and all of them = B
+MUST_PHONG += [{"kind": kind, "light": "phong_sh", "nl": 3, "batch": "B3", "optional": "given", "upstream": "all",
+                **{d: lv for d in ("shading_batch", "params_batch", "lights_batch", "sh_batch")}}
+               for kind, lv in (("cube", "shared"), ("uv", "item"), ("mip", "shared"), ("cube_shared", "item"))]
+# shared textures / UVs at three items under every mode
+MUST_PHONG += [{"kind": "uv", "light": "phong", "batch": "B3", "image": "shared", "uvs": "item", "optional": "given",
+                "upstream": "all"},
+               {"kind": "mip", "light": "phong_set", "nl": 1, "batch": "B3", "image": "item", "uvs": "shared",
+                "optional": "given", "upstream": "all"},
+               {"kind": "cube_shared", "light": "phong_sh", "nl": 3, "batch": "B3", "optional": "given",
+                "upstream": "only_rgb"}]
+
 
 def _complete(out, covered, choices, pairs):
     """append rows until every pair of `pairs` (required_pairs of some levels) is covered"""
@@ -212,9 +312,7 @@ def _complete(out, covered, choices, pairs):
     n = len(out)
     while missing:
         (d1, l1), (d2, l2) = missing[0]
-        seed = {d1: l1, d2: l2}
-        if "kind" not in seed:  # a kind under which both levels mean something
-            seed["kind"] = next(k for k in LEVELS["kind"] if active(d1, k) and active(d2, k) and compatible({**seed, "kind": k}))
+        seed = _context({d1: l1, d2: l2})  # with a kind (and light) under which both levels mean something
         c = _fill(seed, covered, n, choices)
         covered |= pairs_of(c)
         out.append(c)
@@ -242,8 +340,14 @@ def cases():
         covered |= pairs_of(c)
         out.append(c)
     _complete(out, covered, FROZEN, required_pairs(FROZEN_PAIRS))
-    # then the interior rows and the pairs of every level
+    # then the interior rows and the pairs of every level but the Phong modes
     for seed in MUST_INTERIOR:
+        c = _fill(dict(seed), covered, len(out), INTERIOR)
+        covered |= pairs_of(c)
+        out.append(c)
+    _complete(out, covered, INTERIOR, required_pairs(INTERIOR_PAIRS))
+    # then the Phong rows and the pairs of every level
+    for seed in MUST_PHONG:
         c = _fill(dict(seed), covered, len(out))
         covered |= pairs_of(c)
         out.append(c)
@@ -256,9 +360,20 @@ def cases():
 def case_id(c):
     parts = [c["kind"] + ("%d" % c["ts"] if c["ts"] else ""), "fb" if c["fill_back"] else "", c["raster"], c["backward"],
              c["geometry"], ("img-" + c["image"] + ",uv-" + c["uvs"]) if c["image"] else "",
-             "uvgrad" if c["uv_grad"] == "given" else "", {"none": "", "face": "lit", "corner": "smooth"}[c["light"]],
+             "uvgrad" if c["uv_grad"] == "given" else "", _light_id(c),
              "stage" if c["stage"] else "", "bgB" if c["bg"] == "per_batch" else "", c["outputs"],
              "z0" if c["z_batch0"] else "", c["batch"], "up-" + c["upstream"], c["pointers"],
              "nulls" if c["optional"] == "null" else "", "short" if c["layout"] == "short" else "",
-             "" if c["attr"] == "off" else "attr-" + c["attr"], "interior" if c["interior"] == "on" else ""]
+             "" if c["attr"] in (None, "off") else "attr-" + c["attr"], "interior" if c["interior"] == "on" else ""]
     return "%03d-" % c["id"] + "-".join(p for p in parts if p)
+
+
+def _light_id(c):
+    light = c["light"]
+    if light not in PHONG:
+        return {"none": "", "face": "lit", "corner": "smooth"}[light]
+    parts = [{"phong": "phong", "phong_set": "set%d", "phong_sh": "sh%d"}[light].replace("%d", str(c["nl"]))]
+    parts += [c["entry"].replace("own", "") if c["entry"] else "", "s%g" % c["sigma"]]
+    parts += [n + c[d][0] for n, d in (("Bc", "shading_batch"), ("Bp", "params_batch"), ("Bl", "lights_batch"),
+                                       ("Bs", "sh_batch")) if c[d]]
+    return "-".join(p for p in parts if p)

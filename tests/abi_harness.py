@@ -1,12 +1,13 @@
-"""Direct C-ABI harness for nr_b200_forward, nr_b200_backward / nr_b200_backward_corner_light and nr_b200_interpolate /
-nr_b200_interpolate_backward (test infrastructure).
+"""Direct C-ABI harness for nr_b200_forward, nr_b200_backward / nr_b200_backward_corner_light, the Phong entry points
+nr_b200_{forward,backward}_{phong,lights,sh} and nr_b200_interpolate / nr_b200_interpolate_backward (test infrastructure).
 
 It fills _lib.ForwardArgs / BackwardArgs / InterpolateArgs itself -- no Python wrapper in between -- from a case of
 abi_cases.py, so that each case controls the exact flag word, the struct size (the full layouts, or the short ones that
 end before corner_light / grad_face_uvs), which optional pointers are NULL, where every user buffer sits (fresh, or 4
 bytes into a slightly larger allocation; grad_textures, grad_face_uvs and grad_corner_light also 8 bytes in: 2-float but
 not 4-float aligned) and what every output buffer holds before the call: NaN in each float output and a sentinel in
-face_index_map, so an element the kernels fail to write shows, or seeded values for NR_GRAD_ACCUMULATE.  Guard words
+face_index_map, so an element the kernels fail to write shows, or seeded values for NR_GRAD_ACCUMULATE.  The Phong
+inputs (corner_shading, params, lights, sh) and their gradients are user buffers like every other.  Guard words
 around every buffer show a store just outside it.  With a short layout the field just past struct_size points at a real,
 NaN-filled, guarded buffer: the forward would light the image with NaN if it read it, and the backward must leave it
 as it was, bit for bit.
@@ -71,11 +72,21 @@ class Plan:
         self.short = c["layout"] == "short"
         self.bg_batch = c["bg"] == "per_batch"
         self.given = c["optional"] == "given"
-        self.attr = c["attr"] != "off"
-        self.attr_pv = c["attr"].startswith("vertex")
-        self.attr_shared = c["attr"].endswith("_shared")
+        self.attr = c["attr"] not in (None, "off")  # None under the Phong modes
+        self.attr_pv = self.attr and c["attr"].startswith("vertex")
+        self.attr_shared = self.attr and c["attr"].endswith("_shared")
         self.C = ATTR_CHANNELS[c["id"] % len(ATTR_CHANNELS)] if self.attr else 0
         self.interior = c["interior"] == "on"  # NR_GRAD_INTERIOR: a backward-only bit (backward_calls)
+        # the Phong modes: the entry point, the batch of each shading input (1 or B) and the light count
+        self.phong = c["light"] in ("phong", "phong_set", "phong_sh")
+        self.sh = c["light"] == "phong_sh"
+        self.entry = "sh" if self.sh else c["entry"]
+        per = lambda d: self.B if c[d] == "item" else 1
+        self.Bc, self.Bp = (per("shading_batch"), per("params_batch")) if self.phong else (0, 0)
+        self.NL = c["nl"] if c["light"] in ("phong_set", "phong_sh") else 0
+        self.Bl = per("lights_batch") if self.NL else 0
+        self.Bs = per("sh_batch") if self.sh else 0
+        self.sigma = c["sigma"]
         f = 0
         f |= L.NR_RETURN_RGB if self.rgb else 0
         f |= L.NR_RETURN_ALPHA if self.alpha else 0
@@ -131,6 +142,13 @@ class Plan:
                 bufs["corner_light"] = ((B, F, 3, 3), f32)
             if self.uv:
                 bufs["face_uvs"] = (uv_shape, f32)
+            if self.phong:
+                bufs["corner_shading"] = ((self.Bc, F, 3, 6), f32)
+                bufs["params"] = ((self.Bp, 16), f32)
+                if self.NL:
+                    bufs["lights"] = ((self.Bl, self.NL, 12), f32)
+                if self.sh:
+                    bufs["sh"] = ((self.Bs, 9, 3), f32)
         if self.short:  # what the fields past the short layouts point at: never to be read
             bufs["past_end_fwd"] = ((B, F, 3, 3), f32)
             bufs["past_end_bwd"] = ((uv_shape if self.uv else (B, F, 3, 2)), f32)
@@ -168,6 +186,10 @@ class Plan:
                 bufs["grad_corner_light"] = ((B, F, 3, 3), f32)
             if self.uv_grad:
                 bufs["grad_face_uvs"] = (uv_shape, f32)
+            if self.phong and self.given:
+                for k in ("corner_shading", "params", "lights", "sh"):
+                    if k in bufs:
+                        bufs["grad_" + k] = (bufs[k][0], f32)
         if self.attr:  # attribute interpolation on the forward's maps, with gradient buffers of its own
             C, Ba = self.C, (1 if self.attr_shared else B)
             bufs["attributes"] = (((Ba, Nv, C) if self.attr_pv else (Ba, F, 3, C)), f32)
@@ -179,7 +201,7 @@ class Plan:
                                                                                       else (B, F, 3, 3)), f32)
         self.bufs = bufs
         # textures may be NULL in the backward unless a gradient that reads them is wanted (the interior gradient reads
-        # the sampler's derivative from them)
+        # the sampler's derivative from them, the Phong gradients the unlit sample)
         self.bwd_textures = self.rgb and (self.given or self.uv_grad or "grad_face_light" in bufs or self.interior)
         p = c["pointers"]
         self.offsets = {k: (0 if p == "fresh" else 4) for k in bufs}
@@ -190,8 +212,9 @@ class Plan:
         self.fwd_outputs = [k for k in ("face_index_map", "weight_map", "depth_map", "rgb_map", "alpha_map", "out_rgb",
                                         "out_alpha", "out_depth") if k in bufs]
         self.grad_outputs = [k for k in ("grad_faces", "grad_vertices", "grad_textures", "grad_face_light",
-                                         "grad_corner_light", "grad_face_uvs", "attr_grad_attributes",
-                                         "attr_grad_faces", "attr_grad_vertices") if k in bufs]
+                                         "grad_corner_light", "grad_face_uvs", "grad_corner_shading", "grad_params",
+                                         "grad_lights", "grad_sh", "attr_grad_attributes", "attr_grad_faces",
+                                         "attr_grad_vertices") if k in bufs]
 
     # ---- the argument structs, from name -> address (int) of each buffer the case passes
     def forward_args(self, ptr, workspace, workspace_bytes):
@@ -232,12 +255,51 @@ class Plan:
         a.workspace, a.workspace_bytes = workspace, workspace_bytes
         return a
 
+    def shading_args(self, ptr, backward):
+        """(PhongArgs, LightsArgs or None, ShArgs or None) of a Phong case: None is a NULL struct.  Entry "via_sh" passes
+        NULL where a mode has no struct, "via_lights_nl0" an empty light set (NL = 0, lights NULL); the gradient pointers
+        only in the backward"""
+        L = _lib()
+        g = (lambda k: ptr.get("grad_" + k)) if backward else (lambda k: None)
+        ph = L.PhongArgs()
+        ph.struct_size = ctypes.sizeof(L.PhongArgs)
+        ph.shading_batch, ph.params_batch = self.Bc, self.Bp
+        ph.corner_shading, ph.params = ptr.get("corner_shading"), ptr.get("params")
+        ph.grad_corner_shading, ph.grad_params = g("corner_shading"), g("params")
+        la = sa = None
+        if self.NL or self.entry == "via_lights_nl0":
+            la = L.LightsArgs()
+            la.struct_size = ctypes.sizeof(L.LightsArgs)
+            la.lights_batch, la.num_lights = max(self.Bl, 1), self.NL
+            la.lights, la.grad_lights = ptr.get("lights"), g("lights")
+        if self.sh:
+            sa = L.ShArgs()
+            sa.struct_size = ctypes.sizeof(L.ShArgs)
+            sa.sh_batch, sa.sh, sa.grad_sh = self.Bs, ptr.get("sh"), g("sh")
+        return ph, la, sa
+
+    def _call(self, lib, a, ptr, stream, backward):
+        """the case's entry point: nr_b200_{forward,backward}_{phong,lights,sh} for the Phong modes (or _sh with NULL
+        structs, or _lights with an empty set), else nr_b200_forward / nr_b200_backward[_corner_light]"""
+        part = "backward" if backward else "forward"
+        if not self.phong:
+            if backward and self.corner:
+                return lib.nr_b200_backward_corner_light(ctypes.byref(a), ptr.get("corner_light"),
+                                                         ptr.get("grad_corner_light"), stream)
+            return getattr(lib, "nr_b200_" + part)(ctypes.byref(a), stream)
+        ph, la, sa = self.shading_args(ptr, backward)
+        ref = lambda s: None if s is None else ctypes.byref(s)
+        if self.entry == "via_sh" or self.sh:
+            return getattr(lib, "nr_b200_%s_sh" % part)(ctypes.byref(a), ctypes.byref(ph), ref(la), ref(sa), stream)
+        if la is not None:  # a light set, or the empty one of "via_lights_nl0"
+            return getattr(lib, "nr_b200_%s_lights" % part)(ctypes.byref(a), ctypes.byref(ph), ctypes.byref(la), stream)
+        return getattr(lib, "nr_b200_%s_phong" % part)(ctypes.byref(a), ctypes.byref(ph), stream)
+
+    def call_forward(self, lib, a, ptr, stream):
+        return self._call(lib, a, ptr, stream, False)
+
     def call_backward(self, lib, a, ptr, stream):
-        """nr_b200_backward_corner_light for a smooth-shaded case, else nr_b200_backward"""
-        if self.corner:
-            return lib.nr_b200_backward_corner_light(ctypes.byref(a), ptr.get("corner_light"),
-                                                     ptr.get("grad_corner_light"), stream)
-        return lib.nr_b200_backward(ctypes.byref(a), stream)
+        return self._call(lib, a, ptr, stream, True)
 
     def interpolate_args(self, ptr, backward):
         """InterpolateArgs of the case's attribute interpolation (forward, or backward with its gradient buffers)"""
@@ -338,12 +400,56 @@ def make_inputs(plan, seed):
     for k in ("past_end_fwd", "past_end_bwd"):
         if k in plan.bufs:
             d[k] = np.full(plan.bufs[k][0], np.nan, np.float32)
+    if plan.phong:
+        phong_inputs(plan, d, np.random.default_rng(3000 + seed))
     return d
 
 
+# the light records of the Phong cases (nr_b200_lights_args: D, K, x, falloff, kind), the first NL of them: directional
+# and point lights on the viewer's side, two of them far enough off the axis that part of the sphere lies in their shadow
+# (c_j < 0), the point lights with and without falloff.  Item b's positions / directions are shifted by 0.05 b.
+LIGHTS = [[0.5, 0.4, 0.3, 0.3, 0.35, 0.4, 0.2, -0.3, -1.0, 0.0, 0.0, 0.0],
+          [0.3, 0.45, 0.35, 0.5, 0.3, 0.2, 0.6, 0.4, -1.5, 0.4, 1.0, 0.0],
+          [0.25, 0.2, 0.4, 0.2, 0.25, 0.3, -0.9, 0.35, -0.6, 0.0, 0.0, 0.0],
+          [0.4, 0.3, 0.2, 0.35, 0.3, 0.25, -0.5, -0.6, -1.0, 0.0, 1.0, 0.0],
+          [0.2, 0.3, 0.25, 0.3, 0.2, 0.35, 0.1, 0.8, -1.0, 0.0, 0.0, 0.0],
+          [0.35, 0.25, 0.3, 0.25, 0.4, 0.3, 1.2, -0.15, 0.5, 0.15, 1.0, 0.0],
+          [0.15, 0.2, 0.3, 0.4, 0.35, 0.3, -0.3, 0.1, -1.0, 0.0, 0.0, 0.0],
+          [0.3, 0.2, 0.15, 0.2, 0.3, 0.25, 0.2, 0.5, -0.8, 0.8, 1.0, 0.0]]
+
+
+def phong_inputs(plan, d, rng):
+    """the Phong inputs of a case: corner_shading [Bc,F,3,6] -- the sphere's normals at the materialised corners
+    (perturbed, turned towards the viewer at -z; the fill_back copies get the negated normal, as the header asks of
+    callers) and the corners themselves as positions --, params [Bp,16], the first NL of LIGHTS [Bl,NL,12] and an SH
+    environment [Bs,9,3] (bright and coloured, direction-dependent)"""
+    from oracles_sh import C0
+    B, F, Ff = plan.B, plan.F, plan.F_front
+    pos = d["faces_mat"][:plan.Bc].astype(np.float64)
+    centre = np.array([0.0, 0.0, 2.75])
+    n = pos - centre
+    n = n / (np.linalg.norm(n, axis=-1, keepdims=True) + 1e-6) + 0.15 * rng.standard_normal(pos.shape)
+    n[..., 2] = -(np.abs(n[..., 2]) + 0.5)
+    if plan.fill_back:
+        n[:, Ff:] = -n[:, Ff:]
+    d["corner_shading"] = np.ascontiguousarray(np.concatenate((n, pos), axis=-1), np.float32)
+    rows = [[0.3, 0.25, 0.2, 0.6, 0.7 - 0.05 * b, 0.8, 0.3, 0.4 + 0.1 * b, -1.0, 0.6, 0.5, 0.4, plan.sigma,
+             0.2, -0.1 - 0.05 * b, -0.5] for b in range(plan.Bp)]
+    d["params"] = np.array(rows, np.float32)
+    if plan.NL:
+        lt = np.array([LIGHTS[:plan.NL]] * plan.Bl, np.float64)
+        lt[..., 6:9] += 0.05 * np.arange(plan.Bl)[:, None, None]
+        d["lights"] = lt.astype(np.float32)
+    if plan.sh:
+        base = 0.25 * rng.standard_normal((9, 3))
+        base[0] = np.array([0.8, 0.7, 0.6]) / C0
+        d["sh"] = np.stack([base + 0.05 * b for b in range(plan.Bs)]).astype(np.float32)
+
+
 def stage_runs(plan):
-    """whether the forward stages texture cubes (the predicate of nr_b200_forward), and the slots per row segment"""
-    if not (plan.rgb and plan.case["stage"] and not plan.uv and not plan.corner and not plan.aa):
+    """whether the forward stages texture cubes (the predicate of nr_b200_forward; Phong ignores the flag), and the
+    slots per row segment"""
+    if not (plan.rgb and plan.case["stage"] and not plan.uv and not plan.corner and not plan.phong and not plan.aa):
         return False, 0
     cube_bytes = plan.ts ** 3 * 12
     ok = cube_bytes % 16 == 0 and cube_bytes <= K_STAGE_BYTES // 8 and plan.offsets["textures"] % 16 == 0
@@ -399,7 +505,7 @@ def workspace(nbytes, dev):
 
 
 def forward(plan, buf, dev):
-    """poison the forward outputs, call nr_b200_forward on the current stream, return the return code"""
+    """poison the forward outputs, call the case's forward entry point on the current stream, return the return code"""
     import torch
     L = _lib()
     lib = L.load()
@@ -407,8 +513,9 @@ def forward(plan, buf, dev):
         poison(buf[k])
     nbytes = lib.nr_b200_forward_workspace_bytes(plan.B, plan.F, plan.S, plan.ts, plan.fwd_flags)
     ws = workspace(nbytes, dev)
-    a = plan.forward_args({k: t.data_ptr() for k, t in buf.items()}, ws.data_ptr(), ws.numel())
-    rc = lib.nr_b200_forward(ctypes.byref(a), ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+    ptr = {k: t.data_ptr() for k, t in buf.items()}
+    a = plan.forward_args(ptr, ws.data_ptr(), ws.numel())
+    rc = plan.call_forward(lib, a, ptr, ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
     torch.cuda.synchronize(dev)
     return rc
 

@@ -1,8 +1,9 @@
 """CPU: the covering array of the C-ABI matrix (tests/abi_cases.py) -- every compatible pair of levels appears, the full
 product of texture kind x fill_back x anti-aliasing x backward mode is there, the conjunctions the pairs do not force are
 reached (the side fill's tail, the light and corner-light gradients, the own-depth reload of the corner-light cube
-gradient, every phase of the face_uvs reduction, texture staging and its overflow, the interior vertex gradient), the
-cases from before the interior gradient joined are unchanged, and every case passes the library's host argument checks
+gradient, every phase of the face_uvs reduction, texture staging and its overflow, the interior vertex gradient, the
+Phong rows), the cases from before the interior gradient and before the Phong modes joined are unchanged, and every case
+passes the library's host argument checks
 (forward and backward called with a NULL workspace, so the call stops at the workspace check before touching a device;
 the interpolation, which has no workspace, only with arguments it rejects before any launch)."""
 import ctypes
@@ -14,7 +15,7 @@ import pytest
 
 import abi_cases
 
-NR_ERR_INVALID_ARG, NR_ERR_WORKSPACE = -1, -2  # include/nr_b200.h
+NR_ERR_INVALID_ARG, NR_ERR_WORKSPACE, NR_ERR_UNSUPPORTED = -1, -2, -4  # include/nr_b200.h
 
 
 @pytest.fixture(scope="module")
@@ -30,11 +31,23 @@ def test_generator_is_deterministic():
 
 def test_cases_before_the_interior_gradient_are_frozen():
     """the 177 cases the matrix held before the interior gradient joined it keep their ids, levels and seeded inputs:
-    without the `interior` key (always "off" there) they hash to the list as it was"""
-    old = [{k: v for k, v in c.items() if k != "interior"} for c in abi_cases.cases()[:177]]
+    without the `interior` key (always "off" there) and the Phong dimensions (None there) they hash to the list as it
+    was"""
+    old = [{k: v for k, v in c.items() if k != "interior" and k not in abi_cases.PHONG_DIMS} for c in abi_cases.cases()[:177]]
     assert all(c["interior"] in (None, "off") for c in abi_cases.cases()[:177])
     assert hashlib.sha256(repr(old).encode()).hexdigest() == \
         "cde6f0825f0973a0dfd6be5efe813401024db41c1de100869a3a5c23bd7ed758"
+
+
+def test_cases_before_the_phong_modes_are_frozen():
+    """the 194 cases the matrix held before the Phong modes joined it keep their ids, levels and seeded inputs: without
+    the Phong dimensions (None there) they hash to the list as it was"""
+    cases = abi_cases.cases()[:194]
+    assert all(c["light"] not in abi_cases.PHONG for c in cases)
+    assert all(c[k] is None for c in cases for k in abi_cases.PHONG_DIMS)
+    old = [{k: v for k, v in c.items() if k not in abi_cases.PHONG_DIMS} for c in cases]
+    assert hashlib.sha256(repr(old).encode()).hexdigest() == \
+        "a9d5ed5efe4abf6c0a8db1a19b93cdcc1de0f2be5b19492bd510d0d0178775ea"
 
 
 def test_every_pair_of_levels_appears():
@@ -45,7 +58,9 @@ def test_every_pair_of_levels_appears():
     # every level of every dimension is reachable, and the rules exclude nothing else
     for name, levels in abi_cases.DIMS:
         assert {c[name] for c in cases if c[name] is not None} == set(levels), name
-    assert len(cases) <= 200
+    # 194 cases before the Phong modes, 67 Phong rows seeded for conjunctions the pairs do not force and about 10 more
+    # for the pairs; the cap keeps the matrix's run time in check (about 20 s on an H100)
+    assert len(cases) <= 280
 
 
 def test_full_product_of_the_fused_paths():
@@ -115,7 +130,7 @@ def test_interior_gradient_is_held_to_the_oracle():
             s |= {("light", c["light"]), ("acc", p.accumulate), ("halves", len(p.backward_calls()) == 2),
                   ("fill_back", p.fill_back), ("aa", p.aa)}
     want = {(k, v) for k in ("acc", "halves", "fill_back", "aa") for v in (False, True)}
-    want |= {("light", v) for v in abi_cases.LEVELS["light"]}
+    want |= {("light", v) for v in abi_cases.OLD_LIGHTS}  # the Phong modes refuse the interior gradient
     for kind in ("cube", "cube_shared", "uv", "mip"):
         assert seen.get(kind, set()) >= want, (kind, want - seen.get(kind, set()))
     want_every = {("geometry", v) for v in abi_cases.LEVELS["geometry"]} | {("batch", v) for v in abi_cases.LEVELS["batch"]}
@@ -209,20 +224,20 @@ def test_cases_hold_the_rules():
     for c in abi_cases.cases():
         assert abi_cases.compatible(c), c
         for name, _ in abi_cases.DIMS:
-            assert (c[name] is not None) == abi_cases.active(name, c["kind"]), (name, c)
+            assert (c[name] is not None) == abi_cases.active(name, c), (name, c)
 
 
 def test_every_case_passes_the_host_argument_checks(lib):
     import abi_harness
     from neural_renderer_b200 import _lib as lib_flags
-    n_offset = n_short = n_corner = n_attr = n_interior = 0
+    n_offset = n_short = n_corner = n_attr = n_interior = n_phong = 0
     for c in abi_cases.cases():
         plan = abi_harness.Plan(c)
         ptr = plan.fake_pointers()
         n_offset += any(v % 16 for v in ptr.values())
         n_short += plan.short
         a = plan.forward_args(ptr, None, 0)
-        assert lib.nr_b200_forward(ctypes.byref(a), None) == NR_ERR_WORKSPACE, abi_cases.case_id(c)
+        assert plan.call_forward(lib, a, ptr, None) == NR_ERR_WORKSPACE, abi_cases.case_id(c)
         for flags in plan.backward_calls():
             b = plan.backward_args(ptr, flags, None, 0)
             assert plan.call_backward(lib, b, ptr, None) == NR_ERR_WORKSPACE, (abi_cases.case_id(c), hex(flags))
@@ -248,7 +263,16 @@ def test_every_case_passes_the_host_argument_checks(lib):
             bad = dict(ptr)
             bad.pop(k)
             a = plan.forward_args(bad, None, 0)
-            assert lib.nr_b200_forward(ctypes.byref(a), None) == NR_ERR_INVALID_ARG, (k, abi_cases.case_id(c))
+            assert plan.call_forward(lib, a, bad, None) == NR_ERR_INVALID_ARG, (k, abi_cases.case_id(c))
+        if plan.phong:  # the Phong inputs are required, and the interior gradient is refused with them
+            n_phong += 1
+            for k in ("corner_shading", "params") + (("lights",) if plan.NL else ()) + (("sh",) if plan.sh else ()):
+                bad = dict(ptr)
+                bad.pop(k)
+                a = plan.forward_args(bad, None, 0)
+                assert plan.call_forward(lib, a, bad, None) == NR_ERR_INVALID_ARG, (k, abi_cases.case_id(c))
+            b = plan.backward_args(ptr, plan.backward_calls()[0] | lib_flags.NR_GRAD_INTERIOR, None, 0)
+            assert plan.call_backward(lib, b, ptr, None) == NR_ERR_UNSUPPORTED, abi_cases.case_id(c)
         # the interpolation has no workspace gate: a valid call would launch, so only calls it rejects before any launch
         if plan.attr:
             n_attr += 1
@@ -261,5 +285,79 @@ def test_every_case_passes_the_host_argument_checks(lib):
                 a = plan.interpolate_args(ptr, True)
                 a.grad_faces = 0x7000000
                 assert lib.nr_b200_interpolate_backward(ctypes.byref(a), None) == NR_ERR_INVALID_ARG, abi_cases.case_id(c)
-    assert n_offset >= 60 and n_short >= 15 and n_corner >= 20 and n_attr >= 40 and n_interior >= 17, \
-        (n_offset, n_short, n_corner, n_attr, n_interior)
+    assert n_offset >= 60 and n_short >= 15 and n_corner >= 20 and n_attr >= 40 and n_interior >= 17 and n_phong >= 70, \
+        (n_offset, n_short, n_corner, n_attr, n_interior, n_phong)
+
+
+def _phong_grads_run(p):
+    """whether the case's backward runs k_phong_grad: Phong, every shading gradient given, an rgb upstream gradient (the
+    texture half runs in every backward mode)"""
+    return p.phong and p.given and p.g_rgb
+
+
+def _variant(p):
+    """the k_phong_grad instantiation of a Phong case: (kTex, kIdx, light variant)"""
+    tex = {"cube": 0, "cube_shared": 0, "uv": 1, "mip": 2}[p.kind]
+    var = {"phong": "none", "phong_set": "set"}.get(p.case["light"]) or ("sh_set" if p.NL else "sh_alone")
+    return tex, p.indexed, var
+
+
+def test_phong_gradients_are_held_to_the_oracle():
+    """every Phong mode x every texture kind with every shading gradient and an rgb upstream gradient: fresh and
+    accumulating, one call and two halves in both orders, with and without fill_back and anti-aliasing; every
+    k_phong_grad<kTex, kIdx, kLights, kSH> instantiation (SH without a set and with one apart); NL = 8 for every kind;
+    every entry point of every mode"""
+    import abi_harness
+    seen, variants, full_set, entries = {}, set(), set(), set()
+    for c in abi_cases.cases():
+        p = abi_harness.Plan(c)
+        if not p.phong:
+            continue
+        entries.add((c["light"], p.entry))
+        if not _phong_grads_run(p):
+            continue
+        s = seen.setdefault((c["light"], p.kind), set())
+        s |= {("acc", p.accumulate), ("halves", len(p.backward_calls()) == 2), ("fill_back", p.fill_back), ("aa", p.aa),
+              ("order", c["backward"])}
+        variants.add(_variant(p))
+        if p.NL == 8:
+            full_set.add(p.kind)
+    want = {(k, v) for k in ("acc", "halves", "fill_back", "aa") for v in (False, True)}
+    want |= {("order", "faces_tex"), ("order", "acc_halves")}  # two halves, faces first and textures first
+    for key in itertools.product(abi_cases.PHONG, ("cube", "cube_shared", "uv", "mip")):
+        assert seen.get(key, set()) >= want, (key, want - seen.get(key, set()))
+    want_v = set(itertools.product((0, 1, 2), (False, True), ("none", "set", "sh_alone", "sh_set")))
+    assert variants == want_v, want_v - variants
+    assert full_set == {"cube", "cube_shared", "uv", "mip"}, full_set
+    assert entries == {("phong", "own"), ("phong", "via_sh"), ("phong", "via_lights_nl0"), ("phong_set", "own"),
+                       ("phong_set", "via_sh"), ("phong_sh", "sh")}, entries
+
+
+def test_phong_rows_next_to_other_flags_are_reached():
+    """cube Phong with NR_TEX_Z_BATCH0 at three items on per-item index sets (every mode); the short layouts under every
+    mode; every shading gradient without an rgb upstream gradient, fresh and accumulating, under every mode (a light
+    set's grad_lights included); Bc = Bp = Bl = Bs = 1 and all = B at three items; shared textures / UVs at three items"""
+    import abi_harness
+    seen = set()
+    for c in abi_cases.cases():
+        p = abi_harness.Plan(c)
+        if not p.phong:
+            continue
+        mode = c["light"]
+        cube = p.kind in ("cube", "cube_shared")
+        if cube and c["z_batch0"] and p.B == 3 and c["geometry"] == "idx_item" and _phong_grads_run(p):
+            seen.add(("z0", mode))
+        if p.short and p.given and p.g_rgb:
+            seen.add(("short", mode))
+        if p.given and not p.g_rgb and (p.g_alpha or p.g_depth) and (mode == "phong" or "grad_lights" in p.bufs):
+            seen.add(("no_rgb", mode, p.accumulate))
+        if p.B == 3 and p.sh and p.NL and _phong_grads_run(p):
+            batches = {p.Bc, p.Bp, p.Bl, p.Bs}
+            if len(batches) == 1:
+                seen.add(("batches", batches.pop()))
+        if p.B == 3 and _phong_grads_run(p) and ((p.flags & abi_harness._lib().NR_TEX_SHARED) or p.uv_shared):
+            seen.add(("shared_tex", mode))
+    want = {("z0", m) for m in abi_cases.PHONG} | {("short", m) for m in abi_cases.PHONG}
+    want |= {("no_rgb", m, acc) for m in abi_cases.PHONG for acc in (False, True)}
+    want |= {("batches", 1), ("batches", 3)} | {("shared_tex", m) for m in abi_cases.PHONG}
+    assert seen >= want, want - seen

@@ -1,5 +1,5 @@
-"""GPU: every pair of the C-ABI flag levels of the rasterizer (forward, backward, smooth-shading backward) and of the
-attribute interpolation on its maps, called directly (tests/abi_harness.py), held to an unfused oracle.
+"""GPU: every pair of the C-ABI flag levels of the rasterizer (forward, backward, smooth-shading backward, the three
+Phong modes through each of their entry points) and of the attribute interpolation on its maps, called directly (tests/abi_harness.py), held to an unfused oracle.
 
 The cases come from the covering array of tests/abi_cases.py.  The oracle never runs the product's fused paths:
   cubes       the inputs are materialised as a float64 torch function of (vertices | faces, textures, light) -- faces by
@@ -22,15 +22,26 @@ The cases come from the covering array of tests/abi_cases.py.  The oracle never 
               attributes gathered in float64 (out-of-range indices read zeros), at the product's weights; the attribute
               and interior vertex gradients by autograd back through the gathers.  A face with an out-of-range corner
               (a zero vertex: z = 0 puts zp below near) must never win a pixel, and that is checked.
+  phong       the three Phong modes (nr_b200_{forward,backward}_{phong,lights,sh}, or _sh with NULL structs, or _lights
+              with an empty set): the light L and the specular colour of oracles_sh.sh_terms64 (every mode) in float64 on
+              the materialised faces and the product's maps, times the unlit sample as for corner light -- the CPU
+              oracle's unlit cube render, or the float64 samplers -- plus the specular colour.  grad_corner_shading,
+              grad_params, grad_lights and grad_sh by float64 autograd of that image; the cube texture gradient from K6
+              fed g L, the image / pyramid and UV gradients through the samplers with L (and the specular colour) held.
+              No Phong kernel is called.  A covered pixel within 1e-5 of a highlight's switch c_j = 0 (K_j != 0) fails
+              the case as a fault of its inputs (near_kinks), and the inputs are chosen so that there is none.  Shading
+              gradients that are 0 in the oracle must come back exactly 0 from a fresh call.
   interior    NR_GRAD_INTERIOR: float64 autograd of oracles_interior.rgb_held64 (the lit sample with the cell, level of
               detail and clamp gates held fixed) in the materialised faces, on the product's maps and the case's own
               cubes / image / unpacked pyramid, UVs and light, times the raster upstream gradient; added to the CPU
               oracle's K5 / K7 face gradient before the chain to the vertices.  Its sample must match the reference
               rgb_map at the covered pixels at the image gate, so it differentiates the image that was rendered.
 Gates: face_index_map, weight_map and depth_map bit-exact; images bit-exact in non-anti-aliased, unlit or flat-lit cube
-mode, 1e-5 relative elsewhere; every gradient tensor 1e-4 per tensor (helpers.rel_err) and per element (helpers.elem_err),
+mode, 1e-5 relative elsewhere (2e-5 for Phong at sigma 16); every gradient tensor 1e-4 per tensor (helpers.rel_err) and per element (helpers.elem_err),
 with the exceptions of the feature tests (test_gpu_smooth.py, test_gpu_uv_grad.py, test_gpu_attr.py, test_gpu_interior.py,
-with their causes there): the trilinear sampler's image and per-element gradients, the attribute image (1e-6), the
+with their causes there; and test_gpu_phong.py, test_gpu_lights.py, test_gpu_sh.py for the Phong rows: per element
+grad_corner_shading 2e-3, grad_params 5e-4, grad_lights 2e-4, grad_sh 1e-4): the trilinear sampler's image and
+per-element gradients, the attribute image (1e-6), the
 attribute gradient per tensor (1e-5), and the interior vertex gradients per element (2.5e-3) -- the interpolation's, and
 grad_faces / grad_vertices of a case with NR_GRAD_INTERIOR and an rgb upstream gradient.
 Measured maxima over this matrix (194 cases, 17 with NR_GRAD_INTERIOR) on an H100 80GB HBM3 at 400 W, per gate:
@@ -48,6 +59,17 @@ Measured maxima over this matrix (194 cases, 17 with NR_GRAD_INTERIOR) on an H10
   NR_GRAD_INTERIOR grad_faces t / elem     9.0e-7 / 5.2e-5 (case 187)           gates 1e-4 / 2.5e-3
   its sample vs the reference rgb_map      6.0e-6; trilinear 8.6e-6 (185, 189)  gates 1e-5, 6e-5
   every other gradient per element         9.5e-5 (case 136; with NR_GRAD_ACCUMULATE 7.5e-5)
+Measured maxima of the 77 Phong rows (cases 194-270) on an H100 80GB HBM3 at 700 W, per gate:
+  image / anti-aliased image, sigma 1      4.1e-7 / 2.0e-7 (cases 218, 213)      gate 1e-5
+  image / anti-aliased image, sigma 16     3.9e-6 / 1.6e-6 (cases 199, 201)      gate 2e-5
+  image, trilinear                         6.2e-6 (case 241)                     gate 6e-5
+  grad_corner_shading per tensor / elem    3.7e-6 / 8.3e-4 (cases 255, 259)      gates 1e-4 / 2e-3
+  grad_params per tensor / element         2.0e-6 / 4.8e-4 (cases 206, 259)      gates 1e-4 / 5e-4
+  grad_lights per tensor / element         2.3e-6 / 1.7e-4 (cases 245, 255)      gates 1e-4 / 2e-4
+  grad_sh per tensor / element             6.2e-7 / 8.1e-5 (cases 239, 238)      gates 1e-4 / 1e-4
+  grad_textures per element                6.1e-5; trilinear 3.0e-4 (219, 241)   gates 1e-4, 5e-4
+  grad_face_uvs per element                4.7e-5; trilinear 1.1e-4 (204, 240)   gates 1e-4, 1.5e-3
+  grad_faces per element                   2.1e-4 (case 214, TOL_GRAD_ELEM_214); 8.5e-5 elsewhere (case 229)
 Every output is poisoned before a call (NaN, face-index sentinel), so an element the kernels do not write fails, and
 guard words around every buffer must survive the calls, so a store just outside one fails; with NR_GRAD_ACCUMULATE the
 gradients are prefilled with seeded values and must come back as prefill + fresh gradient, the prefill untouched bit for
@@ -85,6 +107,22 @@ TOL_ATTR_IMAGE = 1e-6        # interpolated attribute image
 TOL_ATTR = 1e-5              # attribute gradient per tensor (per element TOL_GRAD)
 TOL_INTERIOR = 1e-4          # interior vertex gradient of the interpolation per tensor
 TOL_INTERIOR_ELEM = 2.5e-3   # and per element
+# the gates of the Phong, light-set and SH tests (test_gpu_phong.py, test_gpu_lights.py, test_gpu_sh.py, with their causes
+# there): the image at sigma > 1 (q^sigma multiplies the fp32 relative error of q by sigma), and the shading gradients per
+# element
+TOL_IMAGE_SIGMA = 2e-5
+TOL_CS_ELEM = 2e-3           # grad_corner_shading
+TOL_PARAMS_ELEM = 5e-4       # grad_params
+TOL_LIGHTS_ELEM = 2e-4       # grad_lights
+TOL_SH_ELEM = 1e-4           # grad_sh
+KINK = 1e-5                  # |c_j| below this at a covered pixel: the highlight's switch [c_j > 0] is within fp32 reach
+# Case 214 (cube_shared ts 6, light set NL = 8, rgb + depth) has a face gradient whose largest element is 3437: element
+# [0, 43, 2, 0] (face 43 of item 0, corner 2, x) comes back 3.005895 against 3.005173 in float64 -- 7.2e-4 absolute,
+# 2.1e-7 of the tensor's maximum, elem_err 2.1e-4.  It is the edge scan K5's fp32 sums on the lit rgb map: the same call
+# without the rgb upstream gradient gives 2.2e-6, three runs give the same bits (run-to-run spread 5e-6), and the
+# per-tensor error is 2.8e-7.  That one face gradient is held at TOL_GRAD_ELEM_214; every other row keeps TOL_GRAD.
+TOL_GRAD_ELEM_214 = 2.5e-4
+PHONG_INPUTS = ("corner_shading", "params", "lights", "sh")
 CASES = abi_cases.cases()
 
 
@@ -134,6 +172,8 @@ def oracle(plan, d, got):
     """(forward reference {name: tensor in the product's layout}, fresh gradients {buffer name: float64 numpy})"""
     import nr_oracle
     from oracles import lod32, oracle_rgb, oracle_trilinear_levels, unpack_pyramid
+    from oracles import _bg
+    from oracles_sh import sh_terms64
     from oracles_smooth import smooth_light64, smooth_rgb
     from oracles_uv_grad import oracle_rgb_uv_grad, oracle_trilinear_levels_uv_grad
     B, S = plan.B, plan.S
@@ -152,7 +192,7 @@ def oracle(plan, d, got):
     if plan.alpha:
         ref["alpha_map"] = torch.from_numpy(fn.alpha_map).flip(1)
     if plan.aa:
-        for k in ("alpha", "depth") + (("rgb",) if cube and not plan.corner else ()):
+        for k in ("alpha", "depth") + (("rgb",) if cube and not (plan.corner or plan.phong) else ()):
             if res[k] is not None:
                 ref["out_" + k] = torch.from_numpy(res[k])
     grads = {}
@@ -162,24 +202,41 @@ def oracle(plan, d, got):
     fm = torch.from_numpy(d["faces_mat"]).to(DEV)
     bgd = torch.from_numpy(np.asarray(bg)).to(DEV)
     g_rgb = torch.from_numpy(d["grad_rgb"]).to(DEV).double() if "grad_rgb" in d else None
-    c64 = L64 = None
+    c64 = L64 = spc64 = None
     if plan.corner:  # smooth shading: float64 light from each item's own depths, times the unlit sample
         c64 = torch.from_numpy(d["corner_light"]).to(DEV).double().requires_grad_(True)
         L64 = smooth_light64(fm, fim, wmap, dmap, c64)
+    # Phong (every mode): float64 light L and specular colour on the product's maps; the image is L s + spc
+    ph64 = {k: torch.from_numpy(d[k]).to(DEV).double().requires_grad_(True) for k in PHONG_INPUTS if k in d}
+    if plan.phong:
+        L64, spc64 = sh_terms64(fm, fim, wmap, dmap, ph64["corner_shading"], ph64["params"], ph64.get("lights"),
+                                ph64.get("sh"))
+    shading_ins = [c64] if plan.corner else [ph64[k] for k in PHONG_INPUTS if "grad_" + k in plan.bufs]
+    shading_outs = ["grad_corner_light"] if plan.corner else ["grad_" + k for k in PHONG_INPUTS if "grad_" + k in plan.bufs]
+
+    def lit(unlit, aa, L, spc):
+        """the unlit raster sample [B,3,S,S] lit by the per-pixel light (and the Phong specular colour), the background
+        where uncovered, pooled with anti-aliasing"""
+        if spc is None:
+            return smooth_rgb(unlit, L, fim, bgd, aa)
+        rgb = torch.where((fim >= 0)[..., None], L * unlit.double().permute(0, 2, 3, 1) + spc, _bg(bgd, DEV))
+        rgb = rgb.permute(0, 3, 1, 2)
+        return torch.nn.functional.avg_pool2d(rgb, 2, 2) if aa else rgb
 
     def grad_of(out, ins):
-        if g_rgb is None:
+        if g_rgb is None or not ins:
             return [torch.zeros_like(x) for x in ins]
         return torch.autograd.grad((out * g_rgb).sum(), ins)
     gt_corner = None
-    if cube and plan.corner:
+    if cube and (plan.corner or plan.phong):
         # the CPU oracle's unlit raster sample (bit-exact, NR_TEX_Z_BATCH0 honoured) lit by the float64 light
         unlit = torch.from_numpy(fn.rgb_map).permute(0, 3, 1, 2).flip(2).to(DEV)
-        ref["rgb_map"] = smooth_rgb(unlit, L64, fim, bgd, False).detach()
-        out = smooth_rgb(unlit, L64, fim, bgd, plan.aa)
+        ref["rgb_map"] = lit(unlit, False, L64, spc64).detach()
+        out = lit(unlit, plan.aa, L64, spc64)
         if plan.aa:
             ref["out_rgb"] = out.detach()
-        grads["grad_corner_light"] = grad_of(out, [c64])[0].detach().cpu().numpy()
+        for k, gk in zip(shading_outs, grad_of(out, shading_ins)):
+            grads[k] = gk.detach().cpu().numpy()
         # K6 of the oracle fed the raster upstream gradient times the light, in float64
         if g_rgb is not None:
             G = (_upsample(g_rgb, plan.aa) * L64.detach().permute(0, 3, 1, 2)).flip(2).permute(0, 2, 3, 1)
@@ -209,31 +266,32 @@ def oracle(plan, d, got):
                 return oracle_rgb_uv_grad(fm, fim, wmap, dmap, uv, tex64, light, bg_, plan.fill_back, aa)
             return oracle_rgb(fm, fim, wmap, dmap, uv, tex64, light, bg_, plan.fill_back, aa)
 
-        def image(aa, uv=uvs, uv_grad=False, L=None, lod_fn=None):
-            if plan.corner:  # the unlit sample times the interpolated light
-                return smooth_rgb(sample(False, zero_bg, None, uv, uv_grad, lod_fn), L, fim, bgd, aa)
+        def image(aa, uv=uvs, uv_grad=False, L=None, spc=None, lod_fn=None):
+            if plan.corner or plan.phong:  # the unlit sample times the interpolated light (plus the highlights)
+                return lit(sample(False, zero_bg, None, uv, uv_grad, lod_fn), aa, L, spc)
             return sample(aa, bgd, light64, uv, uv_grad, lod_fn)
-        ref["rgb_map"] = image(False, L=L64).detach()
-        out = image(plan.aa, L=L64)
+        # the light as a constant: the UV gradients come through the sampler alone
+        Ld, spcd = (L64.detach() if L64 is not None else None), (spc64.detach() if spc64 is not None else None)
+        ref["rgb_map"] = image(False, L=L64, spc=spc64).detach()
+        out = image(plan.aa, L=L64, spc=spc64)
         if plan.aa:
             ref["out_rgb"] = out.detach()
-        ins = [tex64] + ([light64] if plan.lit else []) + ([c64] if plan.corner else [])
-        gi = grad_of(out, ins)
+        light_ins = [light64] if plan.lit else []
+        gi = grad_of(out, [tex64] + light_ins + shading_ins)
         grads["grad_textures"] = gi[0].detach().cpu().numpy()
         if "grad_face_light" in plan.bufs:
             grads["grad_face_light"] = gi[1].detach().cpu().numpy()
-        if "grad_corner_light" in plan.bufs:
-            grads["grad_corner_light"] = gi[-1].detach().cpu().numpy()
+        for k, gk in zip(shading_outs, gi[1 + len(light_ins):]):
+            grads[k] = gk.detach().cpu().numpy()
         if plan.uv_grad:  # through the straight-through UV oracles; autograd folds fill_back and sums shared UVs
             uv64 = torch.from_numpy(d["face_uvs"]).to(DEV).double().requires_grad_(True)
-            img = image(plan.aa, uv64[None] if uv64.dim() == 3 else uv64, True, L64.detach() if plan.corner else None)
+            img = image(plan.aa, uv64[None] if uv64.dim() == 3 else uv64, True, Ld, spcd)
             grads["grad_face_uvs"] = grad_of(img, [uv64])[0].detach().cpu().numpy()
         if plan.mip:  # the same gradients at the product's fp32 level of detail (oracles.lod32; see TOL_GRAD_ELEM_MIP)
             alt = grads["lod32"] = {}
-            alt["grad_textures"] = grad_of(image(plan.aa, L=L64, lod_fn=lod32), [tex64])[0].detach().cpu().numpy()
+            alt["grad_textures"] = grad_of(image(plan.aa, L=Ld, spc=spcd, lod_fn=lod32), [tex64])[0].detach().cpu().numpy()
             if plan.uv_grad:
-                img = image(plan.aa, uv64[None] if uv64.dim() == 3 else uv64, True, L64.detach() if plan.corner else None,
-                            lod32)
+                img = image(plan.aa, uv64[None] if uv64.dim() == 3 else uv64, True, Ld, spcd, lod32)
                 alt["grad_face_uvs"] = grad_of(img, [uv64])[0].detach().cpu().numpy()
         # K5 reads the rgb map: feed the oracle's edge scan the product's own (held to the float64 sampler above)
         fn.rgb_map = np.ascontiguousarray(got["rgb_map"].permute(0, 2, 3, 1).flip(1).cpu().numpy())
@@ -334,7 +392,40 @@ GRAD_GATES = {"grad_corner_light": (TOL_GRAD, TOL_GRAD, TOL_CORNER_ELEM_MIP),
               "attr_grad_attributes": (TOL_ATTR, TOL_GRAD, TOL_GRAD),
               "attr_grad_faces": (TOL_INTERIOR, TOL_INTERIOR_ELEM, TOL_INTERIOR_ELEM),
               "attr_grad_vertices": (TOL_INTERIOR, TOL_INTERIOR_ELEM, TOL_INTERIOR_ELEM),
-              "grad_textures": (TOL_GRAD, TOL_GRAD, TOL_GRAD_ELEM_MIP)}
+              "grad_textures": (TOL_GRAD, TOL_GRAD, TOL_GRAD_ELEM_MIP),
+              "grad_corner_shading": (TOL_GRAD, TOL_CS_ELEM, TOL_CS_ELEM),
+              "grad_params": (TOL_GRAD, TOL_PARAMS_ELEM, TOL_PARAMS_ELEM),
+              "grad_lights": (TOL_GRAD, TOL_LIGHTS_ELEM, TOL_LIGHTS_ELEM),
+              "grad_sh": (TOL_GRAD, TOL_SH_ELEM, TOL_SH_ELEM)}
+
+
+def near_kinks(plan, d, got):
+    """covered pixels within fp32 reach of a highlight's switch: |c_j| < KINK in float64 on the product's maps, for light
+    0 of params (c = nh . d) and every light of the set (c_j = nh . x_j, or nh . lh_j for a point light), where K_j is
+    not 0.  [c_j > 0] makes the highlight jump there, so such a pixel could fail for no kernel reason."""
+    from oracles_phong import _norm
+    fim, wmap, dmap = (got[k] for k in ("face_index_map", "weight_map", "depth_map"))
+    B, S = plan.B, plan.S
+    dv = lambda k: torch.from_numpy(d[k]).to(DEV).double()
+    fi = fim.clamp(min=0).long()
+    bidx = torch.arange(B, device=DEV)[:, None, None].expand(B, S, S)
+    cov = fim >= 0
+    z = torch.where(cov[..., None], dv("faces_mat")[..., 2][bidx, fi], torch.ones((), dtype=torch.float64, device=DEV))
+    lam = wmap.double().permute(0, 2, 3, 1) * (dmap.double()[..., None] / z)
+    cs = dv("corner_shading")
+    C = cs[bidx if cs.shape[0] > 1 else torch.zeros_like(bidx), fi]
+    nh = _norm((lam[..., None] * C[..., :3]).sum(dim=3))
+    p = (lam[..., None] * C[..., 3:]).sum(dim=3)
+    prm = dv("params").expand(B, 16)[:, None, None, :]
+    terms = [((nh * prm[..., 6:9]).sum(-1), prm[..., 9:12])]
+    if "lights" in d:
+        lt = dv("lights").expand(B, -1, -1)
+        for j in range(lt.shape[1]):
+            rec = lt[:, j][:, None, None, :]
+            point = rec[..., 10] > 0.5
+            lh = _norm(rec[..., 6:9] - p)
+            terms.append((torch.where(point, (nh * lh).sum(-1), (nh * rec[..., 6:9]).sum(-1)), rec[..., 3:6]))
+    return sum(int(((c.abs() < KINK) & cov & (K != 0).any(-1)).sum()) for c, K in terms)
 
 
 def run_case(c, metrics=None):
@@ -374,15 +465,24 @@ def run_case(c, metrics=None):
         got["attr_out"] = buf["attr_out"]
     for k in got:
         x, r = got[k].cpu(), ref[k].cpu()
-        if k in ("face_index_map", "weight_map", "depth_map", "alpha_map") or (k == "rgb_map" and cube and not plan.corner):
+        if k in ("face_index_map", "weight_map", "depth_map", "alpha_map") or (k == "rgb_map" and cube and not plan.corner
+                                                                                and not plan.phong):
             if not torch.equal(x, r.to(x.dtype)):
                 fails.append("%s: %d elements differ" % (k, int((x != r.to(x.dtype)).sum())))
         else:
             e = rel_err(x.numpy(), r.numpy()) if torch.isfinite(x).all() else float("nan")
-            kind = "attr" if k == "attr_out" else ("mip" if plan.mip else ("smooth" if plan.corner else "image"))
+            kind = "attr" if k == "attr_out" else ("mip" if plan.mip else ("smooth" if plan.corner else
+                                                                           "phong" if plan.phong else "image"))
+            if kind == "phong" and plan.sigma > 1:
+                kind = "phong_sigma"
             note(k, kind, e)
-            if not e <= {"attr": TOL_ATTR_IMAGE, "mip": TOL_IMAGE_MIP}.get(kind, TOL_IMAGE):
+            if not e <= {"attr": TOL_ATTR_IMAGE, "mip": TOL_IMAGE_MIP, "phong_sigma": TOL_IMAGE_SIGMA}.get(kind, TOL_IMAGE):
                 fails.append("%s: rel_err %.3g" % (k, e))
+    if plan.phong:  # the inputs must keep every covered pixel off the highlights' switches (not masked out)
+        n = near_kinks(plan, d, got)
+        if n:
+            fails.append("the case's inputs put %d covered pixels within %g of a highlight's switch c_j = 0 (K_j != 0): "
+                         "choose other inputs" % (n, KINK))
     if plan.interior:  # the interior oracle differentiates the image the reference rendered (at the covered pixels)
         covm = (got["face_index_map"] >= 0)[:, None].expand(-1, 3, -1, -1)
         e = rel_err(ref["held_rgb"][covm].cpu().numpy(), ref["rgb_map"].to(DEV).double()[covm].cpu().numpy())
@@ -427,6 +527,10 @@ def run_case(c, metrics=None):
         if not np.isfinite(x).all():
             fails.append("%s: %d elements not written / not finite" % (k, int((~np.isfinite(x)).sum())))
             continue
+        if k.startswith("grad_") and k[5:] in PHONG_INPUTS and not plan.accumulate and (x[r == 0] != 0).any():
+            # zero-filled, and no atomic reaches what no pixel differentiates (faces without pixels, slots 10-11 of a
+            # light, every element without an rgb upstream gradient)
+            fails.append("%s: %d elements whose gradient is 0 are not 0" % (k, int((x[r == 0] != 0).sum())))
         if plan.accumulate:
             p = prefill[k]
             zero = r == 0
@@ -441,6 +545,8 @@ def run_case(c, metrics=None):
         if interior:
             tol_t, tol_e, tol_e_mip = TOL_INTERIOR, TOL_INTERIOR_ELEM, TOL_INTERIOR_ELEM
         tol_elem = tol_e_mip if plan.mip else tol_e
+        if (c["id"], k) == (214, "grad_faces"):
+            tol_elem = TOL_GRAD_ELEM_214
         note(k, "tensor_interior" if interior else "tensor", e1)
         note(k, ("elem_interior" if interior else "elem_mip" if plan.mip and tol_e_mip != tol_e
                  else ("elem_acc" if plan.accumulate else "elem")), e2)
