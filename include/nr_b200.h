@@ -373,6 +373,51 @@ typedef struct nr_b200_sh_args {
     float *grad_sh;        /* backward: [Bs,9,3] or NULL */
 } nr_b200_sh_args;
 
+/* Tangent-space normal maps for Phong shading, additive to ABI 4: one struct (nr_b200_normal_map_args) and two entry
+ * points (nr_b200_forward_normal_map / nr_b200_backward_normal_map).  The map perturbs the interpolated normal n of the
+ * Phong expression before anything reads it, so params' light, the light set and the SH environment all see the detail.
+ *   normal_map [Bm,Hm,Wm,3] (device), HWC, row 0 = top, holding DECODED tangent-space vectors m = (m_x, m_y, m_z) (not
+ *   [0,1] colours; +y along +v, the OpenGL convention).  corner_tangents [Bt,F,3,4]: per drawn face and corner
+ *   (T_k, w_k), the tangent and its handedness; F counts the fill_back copies, as corner_shading does (a copy gets
+ *   (-T, -w), as its normal is -N).  Bm, Bt in {1, B} (1 = one set for every item, its gradient the sum over the items).
+ *   Covered raster pixel, l_k = the perspective weights of the Phong expression, fp32 with every fma explicit:
+ *     n = sum_k l_k N_k (as nr_b200_phong_args),  t = fma(l_2, T_2, fma(l_1, T_1, l_0 T_0)) per component
+ *     sigma = ((w_0 + w_1) + w_2 < 0) ? -1 : 1   (a majority vote: exact for w in {+-1}, negated for fill_back copies)
+ *     b_i = sigma (n_j t_k - n_k t_j)   ((i,j,k) cyclic; each product rounded, then subtracted; n and t as interpolated,
+ *                                        not renormalised: the pixel-shader convention of MikkTSpace)
+ *     m = the map sampled at the pixel's uv (NR_TEX_UV's uv, fill_back corners reversed) with NR_TEX_UV's bilinear
+ *         addressing clamped at the map's own Hm x Wm, level 0 always (also when the albedo is trilinear), per channel
+ *         as two horizontal lerps and one vertical one, lerp(a, b, f) = fma(f, b - a, a):
+ *           top = lerp(t00, t10, wx1), bot = lerp(t01, t11, wx1), m = lerp(top, bot, wy1)
+ *         (so a constant map returns its value exactly)
+ *     n' = fma(m_z, n, fma(m_y, b, m_x t)) per component
+ *   and the rest of the Phong / light-set / SH expression is unchanged with n' in place of n (nh = n' / (|n'| + 1e-5), c,
+ *   L, r, q, h, every light of the set, E_c).  A map (0,0,1) everywhere gives n' = n, so the render equals
+ *   nr_b200_forward_sh bit for bit.
+ *   Backward, texture half: with g' = d loss / d n' (every light's and the environment's normal gradient through the
+ *   normalisation), gm = (g'.t, g'.b, g'.n), gb = m_y g', gt = m_x g' + sigma (gb x n), gn = m_z g' + sigma (t x gb):
+ *   grad_corner_shading[f,k][0:3] += l_k gn (the position part as without a map), grad_corner_tangents[f,k] +=
+ *   (l_k gt, 0) (no gradient into w), grad_normal_map's four taps += tap weight * gm, and grad_face_uvs also receives the
+ *   map's l_k (gu, gv) by NR_TEX_UV's formula with the map's taps, gm in place of g_c and the map's (Wm-1), (Hm-1) and
+ *   clamp gates.  grad_textures / grad_face_uvs use the pixel's L_c with the mapped normal.  Each gradient output may
+ *   be NULL and is zero-filled first unless NR_GRAD_ACCUMULATE.  The faces half is unchanged.
+ *   Host rejections, before any launch: NR_ERR_INVALID_ARG for a struct_size mismatch, Bm or Bt not in {1, B}, a NULL
+ *   normal_map or corner_tangents, Hm or Wm < 1, no NR_TEX_UV (the map is addressed by the UVs), grad_normal_map or
+ *   grad_corner_tangents without `textures`, and those of nr_b200_*_sh; NR_ERR_UNSUPPORTED for a map beyond 32-bit
+ *   offsets and for NR_GRAD_INTERIOR (as for every Phong mode).  A NULL struct is allowed: the call is then
+ *   nr_b200_*_sh with the same lights and sh. */
+typedef struct nr_b200_normal_map_args {
+    uint32_t struct_size;            /* sizeof(nr_b200_normal_map_args) = 56 */
+    int32_t map_batch;               /* Bm: 1 or B */
+    int32_t tangent_batch;           /* Bt: 1 or B */
+    int32_t map_height, map_width;   /* Hm, Wm >= 1 */
+    int32_t _pad0;
+    const float *normal_map;         /* [Bm,Hm,Wm,3] */
+    const float *corner_tangents;    /* [Bt,F,3,4] */
+    float *grad_normal_map;          /* backward: [Bm,Hm,Wm,3] or NULL */
+    float *grad_corner_tangents;     /* backward: [Bt,F,3,4] or NULL (the w slots receive 0) */
+} nr_b200_normal_map_args;
+
 /* Attribute interpolation, additive to ABI 4: two flag bits, one struct and two entry points.  Renders C >= 1 arbitrary
  * channels (normals, positions, UVs, labels, features) through the maps an ordinary forward call wrote (face_index_map,
  * weight_map; a silhouette-only forward suffices), with gradients into the attributes and, through the perspective
@@ -470,6 +515,15 @@ NR_B200_API int nr_b200_forward_sh(const nr_b200_forward_args *args, const nr_b2
                                    const nr_b200_lights_args *lights, const nr_b200_sh_args *sh, void *cuda_stream);
 NR_B200_API int nr_b200_backward_sh(const nr_b200_backward_args *args, const nr_b200_phong_args *phong,
                                     const nr_b200_lights_args *lights, const nr_b200_sh_args *sh, void *cuda_stream);
+/* Phong shading through a tangent-space normal map (nr_b200_normal_map_args above): the SH calls with `nm` added; lights
+ * and sh may be NULL, and nm NULL runs exactly nr_b200_forward_sh / nr_b200_backward_sh.  grad_normal_map and
+ * grad_corner_tangents are filled by the texture half. */
+NR_B200_API int nr_b200_forward_normal_map(const nr_b200_forward_args *args, const nr_b200_phong_args *phong,
+                                           const nr_b200_lights_args *lights, const nr_b200_sh_args *sh,
+                                           const nr_b200_normal_map_args *nm, void *cuda_stream);
+NR_B200_API int nr_b200_backward_normal_map(const nr_b200_backward_args *args, const nr_b200_phong_args *phong,
+                                            const nr_b200_lights_args *lights, const nr_b200_sh_args *sh,
+                                            const nr_b200_normal_map_args *nm, void *cuda_stream);
 /* Attribute interpolation (nr_b200_interpolate_args above): the image `out`, and its backward into grad_attributes and the
  * interior vertex gradient.  One kernel launch each (plus the zero-fill of the backward). */
 NR_B200_API int nr_b200_interpolate(const nr_b200_interpolate_args *args, void *cuda_stream);

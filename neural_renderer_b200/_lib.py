@@ -52,6 +52,8 @@ EXPORTED_SYMBOLS = (
     "nr_b200_backward_lights",
     "nr_b200_forward_sh",
     "nr_b200_backward_sh",
+    "nr_b200_forward_normal_map",
+    "nr_b200_backward_normal_map",
     "nr_b200_interpolate",
     "nr_b200_interpolate_backward",
     "nr_b200_vertices_to_faces",
@@ -141,6 +143,15 @@ class ShArgs(ctypes.Structure):
     ]
 
 
+class NormalMapArgs(ctypes.Structure):
+    _fields_ = [
+        ("struct_size", ctypes.c_uint32), ("map_batch", ctypes.c_int32), ("tangent_batch", ctypes.c_int32),
+        ("map_height", ctypes.c_int32), ("map_width", ctypes.c_int32), ("_pad0", ctypes.c_int32),
+        ("normal_map", ctypes.c_void_p), ("corner_tangents", ctypes.c_void_p),
+        ("grad_normal_map", ctypes.c_void_p), ("grad_corner_tangents", ctypes.c_void_p),
+    ]
+
+
 class InterpolateArgs(ctypes.Structure):
     _fields_ = [
         ("struct_size", ctypes.c_uint32), ("flags", ctypes.c_uint32),
@@ -202,6 +213,14 @@ def load():
     lib.nr_b200_backward_sh.restype = ctypes.c_int
     lib.nr_b200_backward_sh.argtypes = [ctypes.POINTER(BackwardArgs), ctypes.POINTER(PhongArgs), ctypes.POINTER(LightsArgs),
                                         ctypes.POINTER(ShArgs), ctypes.c_void_p]
+    lib.nr_b200_forward_normal_map.restype = ctypes.c_int
+    lib.nr_b200_forward_normal_map.argtypes = [ctypes.POINTER(ForwardArgs), ctypes.POINTER(PhongArgs),
+                                               ctypes.POINTER(LightsArgs), ctypes.POINTER(ShArgs),
+                                               ctypes.POINTER(NormalMapArgs), ctypes.c_void_p]
+    lib.nr_b200_backward_normal_map.restype = ctypes.c_int
+    lib.nr_b200_backward_normal_map.argtypes = [ctypes.POINTER(BackwardArgs), ctypes.POINTER(PhongArgs),
+                                                ctypes.POINTER(LightsArgs), ctypes.POINTER(ShArgs),
+                                                ctypes.POINTER(NormalMapArgs), ctypes.c_void_p]
     for name in ("nr_b200_interpolate", "nr_b200_interpolate_backward"):
         fn = getattr(lib, name)
         fn.restype = ctypes.c_int

@@ -159,13 +159,8 @@ __device__ __forceinline__ float rcp_approx(float x) {
     return r;
 }
 
-// vector float reductions (no return value): one L2 request for 2 / 4 consecutive, naturally aligned floats
-__device__ __forceinline__ void red_add_v2(float* addr, float a, float b) {
-    asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
-}
-__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
-    asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
+using nr::red_add_v2;  // vector float reductions (nr_math.cuh)
+using nr::red_add_v4;
 
 // upstream gradient of raster pixel (row, col) of plane `pl` -- folds the 2x2 average-pooling backward
 __device__ __forceinline__ float load_grad(const float* g, bool aa, int S, size_t img_plane_index, int row, int col) {
@@ -1151,14 +1146,7 @@ __global__ void __launch_bounds__(256, kTgCombine ? (kLight >= nr::kLightCorner 
 // helpers (nr_math.cuh), and w_xy * light * grad_rgb goes to the taps: per tap row one horizontal pair = 6 consecutive
 // floats, scattered with vector reductions by alignment as in K6.  A shared image receives from every item, so lanes
 // next to each other that hit the same (image, cell) first merge their contributions (kTgCombine shuffle steps).
-__device__ __forceinline__ void red_add_6(float* t, const float v[6]) {
-    switch ((reinterpret_cast<uintptr_t>(t) >> 2) & 3) {
-        case 0: red_add_v4(t, v[0], v[1], v[2], v[3]); red_add_v2(t + 4, v[4], v[5]); break;
-        case 2: red_add_v2(t, v[0], v[1]); red_add_v4(t + 2, v[2], v[3], v[4], v[5]); break;
-        case 3: atomicAdd(t, v[0]); red_add_v4(t + 1, v[1], v[2], v[3], v[4]); atomicAdd(t + 5, v[5]); break;
-        default: atomicAdd(t, v[0]); red_add_v2(t + 1, v[1], v[2]); red_add_v2(t + 3, v[3], v[4]); atomicAdd(t + 5, v[5]); break;
-    }
-}
+using nr::red_add_6;
 
 // kMip (NR_TEX_MIPMAP): trilinear variant.  The pixel's level of detail is recomputed with the forward's nr::mip_lod from
 // the K1 inverse of the same pixel-space vertices (face_inverse(to_pixel(...)), as k_depth_grad) and the saved weight /
@@ -1242,7 +1230,8 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
         float lam[3] = {0.0f, 0.0f, 0.0f}, L[3];  // kCorner / kPhong: perspective weights and light of the pixel
         if constexpr (kCorner || kPhong) {
             nr::perspective_weights(w, zp, z0, z1, z2, lam);
-            nr::pixel_light<kLight>(p.shading, b, p.F, fn, lam, L);
+            if constexpr (kLight == nr::kLightPhongNM) nr::pixel_light_nm(p.shading, b, fn, lam, u, v, L);  // the map at uv
+            else nr::pixel_light<kLight>(p.shading, b, p.F, fn, lam, L);
         }
         const uint32_t img_off = (uint32_t)b * p.img_bstride;
         // level(s) and their weights: the bilinear variant is level 0 of an image with weight 1
@@ -1578,11 +1567,12 @@ extern "C" size_t nr_b200_backward_workspace_bytes(int32_t B, int32_t F, int32_t
     return bin_layout(B, F, S, strip_rec_bytes(S, both)).total;
 }
 
-// nr_b200_backward (corner_light, phong, lights, sh NULL), nr_b200_backward_corner_light (smooth shading),
-// nr_b200_backward_phong (lights, sh NULL), nr_b200_backward_lights (sh NULL) and nr_b200_backward_sh
+// nr_b200_backward (corner_light, phong, lights, sh, nm NULL), nr_b200_backward_corner_light (smooth shading),
+// nr_b200_backward_phong (lights, sh, nm NULL), nr_b200_backward_lights (sh, nm NULL), nr_b200_backward_sh (nm NULL) and
+// nr_b200_backward_normal_map
 static int backward_impl(const nr_b200_backward_args* args, const float* corner_light, float* grad_corner_light,
                          const nr_b200_phong_args* phong, const nr_b200_lights_args* lights, const nr_b200_sh_args* sh,
-                         void* cuda_stream) {
+                         const nr_b200_normal_map_args* nm, void* cuda_stream) {
     nr_internal::launch_count() = 0;
     // Two layouts: the full struct, and the ABI-4 struct from before grad_face_uvs (which then reads as NULL).  Only the
     // caller's struct_size bytes are read.
@@ -1620,8 +1610,9 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
     if (rgb && (flags & NR_TEX_FILL_BACK) && (F & 1)) return NR_ERR_INVALID_ARG;
     if (rgb && a->grad_face_light && !a->textures) return NR_ERR_INVALID_ARG;
     nr::Shading shading;
-    const int light = nr_internal::make_shading(rgb, a->face_light, corner_light, phong, lights, sh, B, F, &shading);
+    const int light = nr_internal::make_shading(rgb, a->face_light, corner_light, phong, lights, sh, nm, B, F, &shading);
     if (light < 0) return NR_ERR_INVALID_ARG;
+    if (nm && !uv) return NR_ERR_INVALID_ARG;  // the map is addressed by the pixel's uv
     // the shading gradients: grad_corner_light needs corner_light, and every one reads the (unlit) textures (also a
     // grad_lights of a set of NL = 0 lights, which then receives nothing)
     if (grad_corner_light && !corner_light) return NR_ERR_INVALID_ARG;
@@ -1629,9 +1620,12 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
     float* grad_prm = phong ? phong->grad_params : nullptr;
     float* grad_lts = shading.NL > 0 ? lights->grad_lights : nullptr;
     float* grad_sh = sh ? sh->grad_sh : nullptr;
-    if (!a->textures && (grad_corner_light || grad_cs || grad_prm || (lights && lights->grad_lights) || grad_sh))
+    float* grad_nm = nm ? nm->grad_normal_map : nullptr;
+    float* grad_tg = nm ? nm->grad_corner_tangents : nullptr;
+    if (!a->textures && (grad_corner_light || grad_cs || grad_prm || (lights && lights->grad_lights) || grad_sh || grad_nm || grad_tg))
         return NR_ERR_INVALID_ARG;
-    const bool phong_grads = grad_cs || grad_prm || grad_lts || grad_sh;
+    // a normal map also sends its own term into grad_face_uvs from the Phong-gradient kernel
+    const bool phong_grads = grad_cs || grad_prm || grad_lts || grad_sh || grad_nm || grad_tg || (nm && uv_grad);
     // NR_GRAD_INTERIOR: the sampler's derivative reads the textures; the cubes of NR_TEX_Z_BATCH0 sample item b with the
     // depths of item 0, so their derivative would cross items (B = 1 is the plain sampler)
     const bool interior = (flags & NR_GRAD_INTERIOR) != 0;
@@ -1652,6 +1646,7 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
     const size_t uv_items = (flags & NR_UV_SHARED) ? 1 : (size_t)B;
     if (uv && (tex_items * img_floats > 0x7FFFFFFFull || uv_floats * uv_items > 0x7FFFFFFFull))
         return NR_ERR_UNSUPPORTED;  // 32-bit image / UV offsets in the kernels
+    if (nm && nr_internal::nm_floats(nm) * (size_t)nm->map_batch > 0x7FFFFFFFull) return NR_ERR_UNSUPPORTED;  // 32-bit map offsets
     const size_t need = nr_b200_backward_workspace_bytes(B, F, S, ts, flags);
     if (!a->workspace || a->workspace_bytes < need || ((uintptr_t)a->workspace & 15)) return NR_ERR_WORKSPACE;
     cudaStream_t stream = (cudaStream_t)cuda_stream;
@@ -1693,6 +1688,12 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
             return NR_ERR_CUDA;
         if (part_tex && grad_sh && cudaMemsetAsync(grad_sh, 0, (size_t)sh->sh_batch * 27 * sizeof(float), stream) != cudaSuccess)
             return NR_ERR_CUDA;
+        if (part_tex && grad_nm &&
+            cudaMemsetAsync(grad_nm, 0, (size_t)nm->map_batch * nr_internal::nm_floats(nm) * sizeof(float), stream) != cudaSuccess)
+            return NR_ERR_CUDA;
+        if (part_tex && grad_tg &&
+            cudaMemsetAsync(grad_tg, 0, (size_t)nm->tangent_batch * F * 12 * sizeof(float), stream) != cudaSuccess)
+            return NR_ERR_CUDA;
         nr_internal::prof_end(stream);
     }
 
@@ -1725,10 +1726,13 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
         nr_internal::LaunchScope ls(uv ? "k_image_grad" : "k_texture_grad", stream);
         // face_light is the kLightNone variant's run-time branch
         const int tg_light = light == nr::kLightFace ? nr::kLightNone : light;
-        nr::dispatch_light<nr::kLightNone, nr::kLightCorner, nr::kLightPhong, nr::kLightPhongSet, nr::kLightPhongSH>(tg_light, [&](auto kL) {
-            if (!uv) {
-                k_texture_grad<NR_TG_COMBINE, kL><<<pgrid, 256, 0, stream>>>(p);
-                return;
+        nr::dispatch_light<nr::kLightNone, nr::kLightCorner, nr::kLightPhong, nr::kLightPhongSet, nr::kLightPhongSH,
+                           nr::kLightPhongNM>(tg_light, [&](auto kL) {
+            if constexpr (kL != nr::kLightPhongNM) {  // a normal map needs NR_TEX_UV
+                if (!uv) {
+                    k_texture_grad<NR_TG_COMBINE, kL><<<pgrid, 256, 0, stream>>>(p);
+                    return;
+                }
             }
             nr::dispatch_bool(uv_grad, [&](auto kUvGrad) {
                 if (mip) k_image_grad_mip<NR_TG_COMBINE, kUvGrad, kL><<<pgrid, 256, 0, stream>>>(p);
@@ -1742,6 +1746,7 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
         nr_internal::PhongGradLaunch pl{};
         pl.args = a; pl.src = src; pl.shading = shading; pl.light = light;
         pl.grad_cs = grad_cs; pl.grad_prm = grad_prm; pl.grad_lts = grad_lts; pl.grad_sh = grad_sh;
+        pl.grad_nm = grad_nm; pl.grad_tg = grad_tg; pl.grad_uvs = nm ? a->grad_face_uvs : nullptr;
         pl.tex_bstride = (flags & NR_TEX_SHARED) ? 0 : (uv ? img_floats : ncubes * (size_t)ts * ts * ts * 3);
         pl.uv_bstride = p.uv_bstride;
         pl.tex_cmp = p.tex_cmp; pl.tex_val = p.tex_val;
@@ -1850,7 +1855,7 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
 }
 
 extern "C" int nr_b200_backward(const nr_b200_backward_args* args, void* cuda_stream) {
-    return backward_impl(args, nullptr, nullptr, nullptr, nullptr, nullptr, cuda_stream);
+    return backward_impl(args, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, cuda_stream);
 }
 
 extern "C" int nr_b200_backward_corner_light(const nr_b200_backward_args* args, const float* corner_light,
@@ -1859,7 +1864,7 @@ extern "C" int nr_b200_backward_corner_light(const nr_b200_backward_args* args, 
         nr_internal::launch_count() = 0;
         return NR_ERR_INVALID_ARG;
     }
-    return backward_impl(args, corner_light, grad_corner_light, nullptr, nullptr, nullptr, cuda_stream);
+    return backward_impl(args, corner_light, grad_corner_light, nullptr, nullptr, nullptr, nullptr, cuda_stream);
 }
 
 extern "C" int nr_b200_backward_phong(const nr_b200_backward_args* args, const nr_b200_phong_args* phong, void* cuda_stream) {
@@ -1867,7 +1872,7 @@ extern "C" int nr_b200_backward_phong(const nr_b200_backward_args* args, const n
         nr_internal::launch_count() = 0;
         return NR_ERR_INVALID_ARG;
     }
-    return backward_impl(args, nullptr, nullptr, phong, nullptr, nullptr, cuda_stream);
+    return backward_impl(args, nullptr, nullptr, phong, nullptr, nullptr, nullptr, cuda_stream);
 }
 
 extern "C" int nr_b200_backward_lights(const nr_b200_backward_args* args, const nr_b200_phong_args* phong,
@@ -1876,7 +1881,7 @@ extern "C" int nr_b200_backward_lights(const nr_b200_backward_args* args, const 
         nr_internal::launch_count() = 0;
         return NR_ERR_INVALID_ARG;
     }
-    return backward_impl(args, nullptr, nullptr, phong, lights, nullptr, cuda_stream);
+    return backward_impl(args, nullptr, nullptr, phong, lights, nullptr, nullptr, cuda_stream);
 }
 
 extern "C" int nr_b200_backward_sh(const nr_b200_backward_args* args, const nr_b200_phong_args* phong,
@@ -1885,5 +1890,15 @@ extern "C" int nr_b200_backward_sh(const nr_b200_backward_args* args, const nr_b
         nr_internal::launch_count() = 0;
         return NR_ERR_INVALID_ARG;
     }
-    return backward_impl(args, nullptr, nullptr, phong, lights, sh, cuda_stream);
+    return backward_impl(args, nullptr, nullptr, phong, lights, sh, nullptr, cuda_stream);
+}
+
+extern "C" int nr_b200_backward_normal_map(const nr_b200_backward_args* args, const nr_b200_phong_args* phong,
+                                           const nr_b200_lights_args* lights, const nr_b200_sh_args* sh,
+                                           const nr_b200_normal_map_args* nm, void* cuda_stream) {
+    if (!phong) {
+        nr_internal::launch_count() = 0;
+        return NR_ERR_INVALID_ARG;
+    }
+    return backward_impl(args, nullptr, nullptr, phong, lights, sh, nm, cuda_stream);
 }

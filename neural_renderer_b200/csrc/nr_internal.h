@@ -67,17 +67,28 @@ inline bool sh_args_ok(const nr_b200_sh_args* sh, int B) {
     return sh->struct_size == sizeof(nr_b200_sh_args) && sh->sh && (sh->sh_batch == 1 || sh->sh_batch == B);
 }
 
+// the same for a normal map (nr_b200_normal_map_args)
+inline bool nm_args_ok(const nr_b200_normal_map_args* nm, int B) {
+    return nm->struct_size == sizeof(nr_b200_normal_map_args) && nm->normal_map && nm->corner_tangents &&
+           (nm->map_batch == 1 || nm->map_batch == B) && (nm->tangent_batch == 1 || nm->tangent_batch == B) &&
+           nm->map_height >= 1 && nm->map_width >= 1;
+}
+// floats of one item's normal map (the kernels' offsets into it are 32-bit: the caller refuses more than 2^31 - 1 in all)
+inline size_t nm_floats(const nr_b200_normal_map_args* nm) { return (size_t)nm->map_height * (size_t)nm->map_width * 3; }
+
 // The light mode (nr_shading.cuh) and nr::Shading of a call from its ABI arguments, or -1 for a refused combination
 // (NR_ERR_INVALID_ARG): corner_light only for RGB and instead of face_light; Phong only for RGB and instead of both; the
-// Phong, light-set and SH structs pass their checks.  face_light is ignored without RGB, and a set of NL = 0 lights is
-// the Phong call exactly.
+// Phong, light-set, SH and normal-map structs pass their checks.  face_light is ignored without RGB, and a set of NL = 0
+// lights is the Phong call exactly.
 inline int make_shading(bool rgb, const float* face_light, const float* corner_light, const nr_b200_phong_args* phong,
-                        const nr_b200_lights_args* lights, const nr_b200_sh_args* sh, int B, int F, nr::Shading* s) {
+                        const nr_b200_lights_args* lights, const nr_b200_sh_args* sh, const nr_b200_normal_map_args* nm,
+                        int B, int F, nr::Shading* s) {
     *s = nr::Shading{};
     if (corner_light && (!rgb || face_light)) return -1;
     if (phong && (!rgb || face_light || corner_light || !phong_args_ok(phong, B))) return -1;
     if (lights && !lights_args_ok(lights, B)) return -1;
     if (sh && !sh_args_ok(sh, B)) return -1;
+    if (nm && (!phong || !nm_args_ok(nm, B))) return -1;
     if (lights && lights->num_lights == 0) lights = nullptr;
     s->face_light = rgb ? face_light : nullptr;
     s->corner_light = corner_light;
@@ -93,6 +104,13 @@ inline int make_shading(bool rgb, const float* face_light, const float* corner_l
     if (sh) {
         s->sh = sh->sh;
         s->sh_bstride = sh->sh_batch == 1 ? 0 : 27;
+    }
+    if (nm) {
+        s->nm = nm->normal_map; s->tg = nm->corner_tangents;
+        s->nm_bstride = nm->map_batch == 1 ? 0u : (uint32_t)nm_floats(nm);
+        s->tg_bstride = nm->tangent_batch == 1 ? 0 : (size_t)F;
+        s->Hm = nm->map_height; s->Wm = nm->map_width;
+        return nr::kLightPhongNM;
     }
     if (sh) return nr::kLightPhongSH;
     if (lights) return nr::kLightPhongSet;

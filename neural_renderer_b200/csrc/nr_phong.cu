@@ -1,7 +1,8 @@
-// nr_phong.cu -- the Phong-shading gradients of nr_b200_backward_phong, nr_b200_backward_lights and nr_b200_backward_sh
-// (include/nr_b200.h, nr_b200_phong_args, nr_b200_lights_args, nr_b200_sh_args).
+// nr_phong.cu -- the Phong-shading gradients of nr_b200_backward_phong, nr_b200_backward_lights, nr_b200_backward_sh and
+// nr_b200_backward_normal_map (include/nr_b200.h, nr_b200_phong_args, nr_b200_lights_args, nr_b200_sh_args,
+// nr_b200_normal_map_args).
 //
-//   k_phong_grad<kTex, kIdx, kLights, kSH>   one thread per raster pixel, modelled on k_interior_grad.  The winner's perspective weights
+//   k_phong_grad<kTex, kIdx, kLights, kSH, kNM>   one thread per raster pixel, modelled on k_interior_grad.  The winner's perspective weights
 //                   l_k and the unlit sample s are recomputed with the forward's device helpers (the depth map gives zp;
 //                   per-face cubes read the sampler depths NR_TEX_Z_BATCH0 selects), nr::phong_at evaluates the forward's
 //                   expression and nr::phong_grad its derivative.  The 18 corner floats l_k (d loss / d n, d loss / d p) go
@@ -20,6 +21,11 @@
 //                   on its own and is added to light 0's normal gradient.  The 27 floats Y_k g_c s_c are summed over the
 //                   warp one at a time into shared memory, then over the CTA before 27 atomics per CTA
 //                   (sh_grad_reduce), so no 27-float register array exists.
+//                   kNM (kLightPhongNM, a tangent-space normal map; kTex 1 / 2): the expression is evaluated with the
+//                   mapped normal n' (nr::nm_pixel_normal), so the chains above end in g' = d loss / d n'.  Then
+//                   nm_grad_tail samples the map and builds the frame again and sends gm to the map's four taps (two
+//                   6-float rows by vector reductions, as k_image_grad); the 9 tangent floats l_k gt and the 6 UV floats l_k (gu, gv) widen the run reduction to 33.
+//                   The launcher picks kLights = NL > 0 and kSH = (sh given) as for the other modes.
 //
 // It belongs to the texture half of the backward: the texture-gradient kernels (K6, k_image_grad) only need the pixel's
 // L_c, and keeping the 34 gradient floats out of them keeps their register budgets (DESIGN.md section 4g).
@@ -52,8 +58,60 @@ struct PhongParams {
     int aa, fill_back, z_batch0;
     float tex_cmp, tex_val;
     nr::MipTable mip;  // kTex 2
-    nr::Shading shading;  // corner_shading, params, lights and sh
+    nr::Shading shading;  // corner_shading, params, lights, sh and the normal map
+    float* grad_nm;       // kNM: the layouts of normal_map, corner_tangents and face_uvs, or nullptr
+    float* grad_tg;
+    float* grad_uvs;
 };
+
+// kNM, once g' = d loss / d n' of the pixel is known: the map's sample (with its uv derivative) and the frame again, the
+// same loads and arithmetic as nm_pixel_normal; gn = g' on entry, d loss / d n (of the interpolated normal) on return.
+// d loss / d m goes to the map's four taps (tap weight x gm) by vector reductions; cgx[0..8] = l_k gt (corner-major) and
+// cgx[9..14] = l_k (gu, gv) for the stored face's UV corners (a fill_back copy's corner k is corner 2 - k).
+__device__ __forceinline__ void nm_grad_tail(const PhongParams& p, int b, int fn, const float lam[3], float u, float v, bool rev,
+                                             float gn[3], float* cgx) {
+    const nr::Shading& s = p.shading;
+    const nr::UvTaps t = nr::uv_taps(u, v, s.Hm, s.Wm);
+    float m[3], du[3], dv[3], np[3];
+    nr::nm_sample<true>(s.nm + s.nm_off(b), s.Hm, s.Wm, t, m, du, dv);
+    nr::NmFrame F;
+    nr::nm_normal(s.cs + s.cs_off(b, fn), s.tg + s.tg_off(b, fn), lam, m, F, np);
+    float gm[3], gt[3], gi[3];
+    nr::nm_normal_grad(F, m, gn, gm, gt, gi);
+#pragma unroll
+    for (int k = 0; k < 3; k++) gn[k] = gi[k];
+    if (p.grad_nm) {  // uniform: per tap row the horizontal pair (x0, x1) = 6 consecutive floats, by vector reductions
+        const uint32_t row3 = (uint32_t)s.Wm * 3u, c0 = (uint32_t)t.x0 * 3u;
+        float* q0 = p.grad_nm + s.nm_off(b) + (uint32_t)t.r0 * row3 + c0;
+        float* q1 = p.grad_nm + s.nm_off(b) + (uint32_t)t.r1 * row3 + c0;
+        float v0[6], v1[6];
+#pragma unroll
+        for (int k = 0; k < 3; k++) {
+            v0[k] = __fmul_rn(t.w00, gm[k]); v0[3 + k] = __fmul_rn(t.w10, gm[k]);
+            v1[k] = __fmul_rn(t.w01, gm[k]); v1[3 + k] = __fmul_rn(t.w11, gm[k]);
+        }
+        if (t.x1 != t.x0) {
+            nr::red_add_6(q0, v0);
+            nr::red_add_6(q1, v1);
+        } else {  // a clamped column (x1 = x0, weight 0 on x1): both taps are one texel
+#pragma unroll
+            for (int k = 0; k < 3; k++) {
+                atomicAdd(q0 + k, __fadd_rn(v0[k], v0[3 + k]));
+                atomicAdd(q1 + k, __fadd_rn(v1[k], v1[3 + k]));
+            }
+        }
+    }
+#pragma unroll
+    for (int k = 0; k < 3; k++)
+#pragma unroll
+        for (int j = 0; j < 3; j++) cgx[3 * k + j] = __fmul_rn(lam[k], gt[j]);
+    const float gu = __fmaf_rn(gm[2], du[2], __fmaf_rn(gm[1], du[1], __fmul_rn(gm[0], du[0])));
+    const float gv = __fmaf_rn(gm[2], dv[2], __fmaf_rn(gm[1], dv[1], __fmul_rn(gm[0], dv[0])));
+    const float s0 = rev ? lam[2] : lam[0], s2 = rev ? lam[0] : lam[2];
+    cgx[9] = __fmul_rn(s0, gu); cgx[10] = __fmul_rn(s0, gv);
+    cgx[11] = __fmul_rn(lam[1], gu); cgx[12] = __fmul_rn(lam[1], gv);
+    cgx[13] = __fmul_rn(s2, gu); cgx[14] = __fmul_rn(s2, gv);
+}
 
 // kSH: the 27 floats Y_k w_c of grad_sh summed over the warp one at a time into shared memory, then over the CTA before 27
 // atomics into `o` (item b's [9,3] slot, or slot 0 with Bs = 1).  Every thread of the CTA calls it (0 off the mesh).
@@ -75,8 +133,10 @@ __device__ __forceinline__ void sh_grad_reduce(const float Y[9], const float ws[
     }
 }
 
-template <int kTex, bool kIdx, bool kLights, bool kSH>
+template <int kTex, bool kIdx, bool kLights, bool kSH, bool kNM>
 __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ PhongParams p) {
+    static_assert(!kNM || kTex != 0, "a normal map needs NR_TEX_UV");
+    constexpr int kCg = kNM ? 33 : 18;  // the corner floats of the run reduction
     __shared__ float s_prm[8][16];
     const int S = p.S;
     const size_t plane = (size_t)S * S;
@@ -85,9 +145,9 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int fn = (i < plane) ? __ldg(p.fim + (size_t)b * plane + i) : -1;
     if (!__syncthreads_or(fn >= 0)) return;  // CTA-uniform
-    float cg[18], gprm[16];
+    float cg[kCg], gprm[16];
 #pragma unroll
-    for (int k = 0; k < 18; k++) cg[k] = 0.0f;
+    for (int k = 0; k < kCg; k++) cg[k] = 0.0f;
 #pragma unroll
     for (int k = 0; k < 16; k++) gprm[k] = 0.0f;
     // kLights: what the loop over the lights needs of the covered pixel below
@@ -101,6 +161,9 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
 #pragma unroll
         for (int k = 0; k < 3; k++) shw[k] = 0.0f;
     }
+    float nmu = 0.0f, nmv = 0.0f;  // kNM: the pixel's uv, its UV face and whether it is a fill_back copy
+    int nmtf = 0;
+    bool nmrev = false;
     if (fn >= 0) {
         const int r = (int)(i / S), c = (int)(i % S);
         const bool aa = p.aa != 0;
@@ -167,7 +230,18 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
         }
         const float* prm = p.shading.prm + p.shading.prm_off(b);
         nr::PhongEval E;
-        nr::phong_at(p.shading.cs + p.shading.cs_off(b, fn), lam, prm, E);
+        if constexpr (kNM) {  // the mapped normal in E.n, then the rest of phong_at
+            float uv[6], m[3];
+            nr::load_face_uvs(p.uvs + ((size_t)b * p.uv_bstride + (size_t)tf * 6u), rev, uv);
+            nr::pixel_uv(w, zp, z[0], z[1], z[2], uv, nmu, nmv);
+            nmtf = tf; nmrev = rev;
+            nr::NmFrame Fm;
+            nr::nm_pixel_normal(p.shading, b, fn, lam, nmu, nmv, m, Fm, E);
+            nr::phong_diffuse_n(prm, E);
+            nr::phong_specular(p.shading.cs + p.shading.cs_off(b, fn), lam, prm, E);
+        } else {
+            nr::phong_at(p.shading.cs + p.shading.cs_off(b, fn), lam, prm, E);
+        }
         float gn[3], gp[3];
         nr::phong_grad(E, prm, g, s, gn, gp, gprm);
         if constexpr (kLights) {  // the set's gradients read neither E.L nor the set's diffuse terms
@@ -188,6 +262,7 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
 #pragma unroll
                 for (int k = 0; k < 3; k++) gn[k] = __fadd_rn(gn[k], t[k]);
             }
+            if constexpr (kNM) nm_grad_tail(p, b, fn, lam, nmu, nmv, nmrev, gn, cg + 18);
 #pragma unroll
             for (int k = 0; k < 3; k++)
 #pragma unroll
@@ -235,6 +310,7 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
         }
         if (fn >= 0) {
             nr::phong_lights_grad_end(xE, gnh, gvh, gsig, xgn, xgp, gprm);
+            if constexpr (kNM) nm_grad_tail(p, b, fn, xlam, nmu, nmv, nmrev, xgn, cg + 18);
 #pragma unroll
             for (int k = 0; k < 3; k++)
 #pragma unroll
@@ -256,8 +332,8 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
     if constexpr (kSH && !kLights) {
         if (p.grad_sh) sh_grad_reduce(shY, shw, p.grad_sh + p.shading.sh_off(b), lane, warp);  // uniform
     }
-    if (p.grad_cs) {  // uniform
-        // the segmented run reduction of k_depth_grad over 18 floats, then one set of atomics per run
+    if (kNM ? (p.grad_cs || p.grad_tg || p.grad_uvs) : p.grad_cs != nullptr) {  // uniform
+        // the segmented run reduction of k_depth_grad over 18 (kNM: 33) floats, then one set of atomics per run
         const int fn_prev = __shfl_up_sync(0xffffffffu, fn, 1);
         const uint32_t heads = __ballot_sync(0xffffffffu, lane == 0 || fn != fn_prev);
         const uint32_t later = heads & ~((2u << lane) - 1u);
@@ -266,15 +342,31 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
         for (int off = 1; off < 32; off <<= 1) {
             const bool take = lane + off <= run_end;
 #pragma unroll
-            for (int k = 0; k < 18; k++) {
+            for (int k = 0; k < kCg; k++) {
                 const float t = __shfl_down_sync(0xffffffffu, cg[k], off);
                 if (take) cg[k] += t;
             }
         }
         if (fn >= 0 && ((heads >> lane) & 1u)) {
-            float* o = p.grad_cs + p.shading.cs_off(b, fn);
+            if (!kNM || p.grad_cs) {
+                float* o = p.grad_cs + p.shading.cs_off(b, fn);
 #pragma unroll
-            for (int k = 0; k < 18; k++) atomicAdd(o + k, cg[k]);
+                for (int k = 0; k < 18; k++) atomicAdd(o + k, cg[k]);
+            }
+            if constexpr (kNM) {
+                if (p.grad_tg) {
+                    float* o = p.grad_tg + p.shading.tg_off(b, fn);
+#pragma unroll
+                    for (int k = 0; k < 3; k++)
+#pragma unroll
+                        for (int j = 0; j < 3; j++) atomicAdd(o + 4 * k + j, cg[18 + 3 * k + j]);
+                }
+                if (p.grad_uvs) {
+                    float* o = p.grad_uvs + ((size_t)b * p.uv_bstride + (size_t)nmtf * 6u);
+#pragma unroll
+                    for (int k = 0; k < 6; k++) atomicAdd(o + k, cg[27 + k]);
+                }
+            }
         }
     }
     if (p.grad_prm) {  // uniform: warp sums, then the CTA's sum in shared memory, 16 atomics per CTA
@@ -318,18 +410,22 @@ void launch_phong_grad(const PhongGradLaunch& L, cudaStream_t stream) {
     p.tex_cmp = L.tex_cmp; p.tex_val = L.tex_val;
     if (L.mip) p.mip = *L.mip;
     p.shading = L.shading;
+    p.grad_nm = L.grad_nm; p.grad_tg = L.grad_tg; p.grad_uvs = L.grad_uvs;
     const bool idx = (flags & NR_FACES_INDEXED) != 0;
     const int tex = (flags & NR_TEX_MIPMAP) ? 2 : (flags & NR_TEX_UV) ? 1 : 0;
     const dim3 grid((unsigned)(((size_t)p.S * p.S + 255) / 256), a->batch_size);
     LaunchScope ls("k_phong_grad", stream);
-    // the kernel's split of the mode: a light set of NL > 0 lights (kLightPhongSet, or kLightPhongSH with one), an SH
-    // environment
+    // the kernel's split of the mode: a light set of NL > 0 lights (kLightPhongSet, or kLightPhongSH / kLightPhongNM with
+    // one), an SH environment (kLightPhongSH, or kLightPhongNM with one), a normal map (kLightPhongNM, NR_TEX_UV only)
     nr::dispatch_bool(p.shading.NL > 0, [&](auto kLights) {
-        nr::dispatch_bool(L.light == nr::kLightPhongSH, [&](auto kSH) {
+        nr::dispatch_bool(p.shading.sh != nullptr, [&](auto kSH) {
             nr::dispatch_bool(idx, [&](auto kIdx) {
-                if (tex == 2) k_phong_grad<2, kIdx, kLights, kSH><<<grid, 256, 0, stream>>>(p);
-                else if (tex == 1) k_phong_grad<1, kIdx, kLights, kSH><<<grid, 256, 0, stream>>>(p);
-                else k_phong_grad<0, kIdx, kLights, kSH><<<grid, 256, 0, stream>>>(p);
+                if (L.light == nr::kLightPhongNM) {
+                    if (tex == 2) k_phong_grad<2, kIdx, kLights, kSH, true><<<grid, 256, 0, stream>>>(p);
+                    else k_phong_grad<1, kIdx, kLights, kSH, true><<<grid, 256, 0, stream>>>(p);
+                } else if (tex == 2) k_phong_grad<2, kIdx, kLights, kSH, false><<<grid, 256, 0, stream>>>(p);
+                else if (tex == 1) k_phong_grad<1, kIdx, kLights, kSH, false><<<grid, 256, 0, stream>>>(p);
+                else k_phong_grad<0, kIdx, kLights, kSH, false><<<grid, 256, 0, stream>>>(p);
             });
         });
     });

@@ -22,6 +22,8 @@ constexpr int kLightCorner = 2;    // corner_light [B,F,3,3] interpolated to the
 constexpr int kLightPhong = 3;     // Phong shading of the unlit sample (corner_shading, params)
 constexpr int kLightPhongSet = 4;  // the same with a light set of NL > 0 lights
 constexpr int kLightPhongSH = 5;   // the same with an SH environment, and a light set of NL >= 0 lights
+constexpr int kLightPhongNM = 6;   // Phong through a tangent-space normal map (NR_TEX_UV only), with a light set of NL >= 0
+                                   // lights and an optional SH environment (both uniform per launch, decided at run time)
 
 // The shading inputs of one call; strides are 0 for a set shared by every batch item.
 struct Shading {
@@ -36,6 +38,11 @@ struct Shading {
     int NL;
     const float* sh;            // [Bs,9,3] (kLightPhongSH)
     size_t sh_bstride;          // floats per item in sh (0 with Bs = 1)
+    const float* nm;            // normal map [Bm,Hm,Wm,3] (kLightPhongNM)
+    const float* tg;            // corner tangents [Bt,F,3,4] (kLightPhongNM)
+    uint32_t nm_bstride;        // floats per item in nm (0 with Bm = 1; 32-bit, checked on the host)
+    size_t tg_bstride;          // faces per item in tg (0 with Bt = 1)
+    int Hm, Wm;
 
     // float offsets of item b's records (and of face fn's; F = faces per item of the [B,F,...] light tensors), shared
     // with the gradients of the same layout
@@ -45,7 +52,54 @@ struct Shading {
     __host__ __device__ __forceinline__ size_t prm_off(int b) const { return (size_t)b * prm_bstride; }
     __host__ __device__ __forceinline__ size_t lts_off(int b) const { return (size_t)b * lt_bstride; }
     __host__ __device__ __forceinline__ size_t sh_off(int b) const { return (size_t)b * sh_bstride; }
+    __host__ __device__ __forceinline__ uint32_t nm_off(int b) const { return (uint32_t)b * nm_bstride; }
+    __host__ __device__ __forceinline__ size_t tg_off(int b, int fn) const { return ((size_t)b * tg_bstride + fn) * 12; }
 };
+
+// kLightPhongNM: the map's sample at the pixel's (u, v) and the frame of face fn's pixel, the mapped normal in E.n
+// (nr::nm_normal); m and the frame are returned for the backward
+__device__ __forceinline__ void nm_pixel_normal(const Shading& s, int b, int fn, const float l[3], float u, float v, float m[3],
+                                                NmFrame& F, PhongEval& E) {
+    float du[3], dv[3];
+    nm_sample<false>(s.nm + s.nm_off(b), s.Hm, s.Wm, uv_taps(u, v, s.Hm, s.Wm), m, du, dv);
+    nm_normal(s.cs + s.cs_off(b, fn), s.tg + s.tg_off(b, fn), l, m, F, E.n);
+}
+// pixel_light of kLightPhongNM, which also needs the pixel's (u, v): the diffuse part of the Phong expression with the
+// mapped normal, the set's diffuse terms (NL >= 0), then E_c when an environment is given
+__device__ __forceinline__ void pixel_light_nm(const Shading& s, int b, int fn, const float l[3], float u, float v, float L[3]) {
+    const float* cs = s.cs + s.cs_off(b, fn);
+    PhongEval E;
+    NmFrame F;
+    float m[3];
+    nm_pixel_normal(s, b, fn, l, u, v, m, F, E);
+    phong_diffuse_n(s.prm + s.prm_off(b), E);
+    if (s.NL > 0) {  // uniform
+        float pos[3];
+        phong_position(cs, l, pos);
+        lights_diffuse_loop(s.lts + s.lts_off(b), s.NL, pos, E);
+    }
+    if (s.sh) sh_add_irradiance(s.sh + s.sh_off(b), E);  // uniform
+    L[0] = E.L[0]; L[1] = E.L[1]; L[2] = E.L[2];
+}
+// shade of kLightPhongNM: the rgb of the light-set / SH expression with the mapped normal (NL = 0 and no environment:
+// phong_lights_rgb is phong_rgb, so a flat map renders as the modes 3-5 do, bit for bit)
+__device__ __forceinline__ void shade_nm(const Shading& s, int b, int fn, const float l[3], float u, float v, float c[3]) {
+    const float* prm = s.prm + s.prm_off(b);
+    const float* lts = s.lts + s.lts_off(b);
+    const float* cs = s.cs + s.cs_off(b, fn);
+    PhongEval E;
+    NmFrame F;
+    float m[3];
+    nm_pixel_normal(s, b, fn, l, u, v, m, F, E);
+    phong_diffuse_n(prm, E);
+    phong_specular(cs, l, prm, E);
+    float pos[3], rgb[3];
+    phong_position(cs, l, pos);
+    lights_diffuse_loop(lts, s.NL, pos, E);
+    if (s.sh) sh_add_irradiance(s.sh + s.sh_off(b), E);  // uniform
+    phong_lights_rgb(E, pos, prm, lts, s.NL, c, rgb);
+    c[0] = rgb[0]; c[1] = rgb[1]; c[2] = rgb[2];
+}
 
 // L_c = d rgb_c / d s_c of face fn's pixel with perspective weights l (own vertex depths): 1, face_light, the
 // interpolated corner light, or the diffuse part of the Phong expression (with the set's diffuse terms, then E_c)

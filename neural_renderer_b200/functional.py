@@ -837,3 +837,71 @@ def sh_from_environment_map(envmap):
     Y = _sh_basis_torch(omega) * dw[:, None, None]  # [He,We,9]
     a = torch.tensor([1.0] + [2.0 / 3.0] * 3 + [0.25] * 5, **kw)
     return torch.einsum('bhwc,hwk->bkc', env, Y) * a[None, :, None]
+
+
+def vertex_tangents(vertices, faces, face_uvs, vertex_normals):
+    """Per-vertex tangents [B,Nv,4] = (T, w) for a tangent-space normal map (F.corner_tangents, then
+    rasterize(..., normal_map=, corner_tangents=), Renderer.normal_map).  vertices / vertex_normals [B,Nv,3], faces [F,3] /
+    [1|B,F,3] (the original faces, not the fill_back-doubled set), face_uvs [F,3,2] / [1|B,F,3,2] (OBJ convention, v up).
+
+    Per face, with e1 = v1 - v0, e2 = v2 - v0 and (du_k, dv_k) = uv_k - uv_0: s = sign(du1 dv2 - du2 dv1) (a face with
+    s = 0 is skipped), T_f = s (e1 dv2 - e2 dv1) and B_f = s (e2 du1 - e1 du2).  The sums over a vertex's corners are
+    orthogonalised against n_v and normalised, T_v = t / (|t| + 1e-5) with t = T - (n_v . T) n_v, and w_v = -1 where
+    (n_v x T_v) . sum B_f < 0, else 1 (the map's +y then runs along +v).  An unreferenced vertex gets (0, 0, 0, 1).
+    Tangents are summed by vertex, so a UV seam shares one tangent across it.  Pure torch, differentiable with
+    respect to the vertices, the UVs and the normals (not through w)."""
+    bs, nv = vertices.shape[:2]
+    faces = faces[None] if faces.dim() == 2 else faces
+    uvs = face_uvs[None] if face_uvs.dim() == 3 else face_uvs
+    v, ok = _gather_vertices(vertices, faces)  # [B,F,3,3]
+    uvs = uvs.to(v.dtype).expand(bs, -1, -1, -1)
+    e1, e2 = v[:, :, 1] - v[:, :, 0], v[:, :, 2] - v[:, :, 0]
+    d1, d2 = uvs[:, :, 1] - uvs[:, :, 0], uvs[:, :, 2] - uvs[:, :, 0]
+    du1, dv1, du2, dv2 = d1[..., :1], d1[..., 1:], d2[..., :1], d2[..., 1:]
+    s = torch.sign(du1 * dv2 - du2 * dv1) * ok.all(dim=2)[..., None].to(v.dtype)
+    tf = s * (e1 * dv2 - e2 * dv1)
+    bf = s * (e2 * du1 - e1 * du2)
+    idx = faces.long().expand(bs, -1, -1)
+    corner_ok = ((idx >= 0) & (idx < nv))[..., None].to(v.dtype)
+    target = (idx.clamp(0, nv - 1) + (torch.arange(bs, device=vertices.device) * nv)[:, None, None]).reshape(-1)
+    zeros = torch.zeros((bs * nv, 3), dtype=v.dtype, device=v.device)
+    t = zeros.index_add(0, target, (tf[:, :, None, :] * corner_ok).reshape(-1, 3)).reshape(bs, nv, 3)
+    b = zeros.index_add(0, target, (bf[:, :, None, :] * corner_ok).reshape(-1, 3)).reshape(bs, nv, 3)
+    n = vertex_normals.to(v.dtype).expand(bs, nv, 3)
+    t = t - (n * t).sum(dim=2, keepdim=True) * n
+    t = t / (torch.linalg.vector_norm(t, dim=2, keepdim=True) + 1e-5)
+    w = torch.where((torch.linalg.cross(n, t, dim=2) * b).sum(dim=2, keepdim=True) < 0, -1.0, 1.0).to(v.dtype)
+    return torch.cat((t, w), dim=2)
+
+
+def corner_tangents(vertex_tangents, faces, fill_back=False):
+    """Per-corner tangents [B,F,3,4] for rasterize(..., corner_tangents=...): corner k of face f holds (T, w) of vertex
+    faces[f,k] from `vertex_tangents` [B,Nv,4] (F.vertex_tangents).  `faces` [F,3] / [1|B,F,3] is the index set the
+    rasterizer receives, as for F.corner_shading; with fill_back=True faces [F/2, F) are the reversed copies and get
+    (-T, -w), so that their mapped normal is exactly the negated one of the original face.  An index outside [0, Nv)
+    gives zeros.  Pure torch, differentiable with respect to the tangents."""
+    assert vertex_tangents.dim() == 3 and vertex_tangents.shape[2] == 4
+    faces = faces[None] if faces.dim() == 2 else faces
+    nf = faces.shape[1]
+    if fill_back and nf % 2:
+        raise ValueError("fill_back needs an even number of faces (front faces, then their reversed copies)")
+    bs, nv = vertex_tangents.shape[:2]
+    idx = faces.long().expand(bs, -1, -1)
+    ok = ((idx >= 0) & (idx < nv))[..., None].to(vertex_tangents.dtype)
+    flat = idx.clamp(0, nv - 1) + (torch.arange(bs, device=vertex_tangents.device) * nv)[:, None, None]
+    out = vertex_tangents.reshape(bs * nv, 4)[flat] * ok
+    if fill_back:
+        sign = torch.ones(nf, dtype=out.dtype, device=out.device)
+        sign[nf // 2:] = -1
+        out = out * sign[None, :, None, None]
+    return out
+
+
+def decode_normal_map(image, green_down=False):
+    """A normal-map image of [0,1] colours [...,3] -> the decoded tangent-space vectors 2 image - 1 that
+    rasterize(..., normal_map=...) and Renderer.normal_map take.  green_down=True negates y, for maps authored with +y
+    along -v (the DirectX convention).  Differentiable; not renormalised (the shading normalises the mapped normal)."""
+    m = 2.0 * image - 1.0
+    if green_down:
+        m = m * torch.tensor([1.0, -1.0, 1.0], dtype=m.dtype, device=m.device)
+    return m

@@ -61,7 +61,8 @@ def _ptr(t):
 
 
 def _check_inputs(faces, textures, return_rgb, face_light=None, textures_fill_back=False, vertices=None, face_uvs=None,
-                  corner_light=None, corner_shading=None, shading_params=None, lights=None, environment_sh=None):
+                  corner_light=None, corner_shading=None, shading_params=None, lights=None, environment_sh=None,
+                  normal_map=None, corner_tangents=None):
     # rasterize.py:66-90 (chainer type_check) -> TypeError / ValueError with the same conditions
     if not isinstance(faces, torch.Tensor):
         raise TypeError("faces must be a torch.Tensor")
@@ -107,6 +108,8 @@ def _check_inputs(faces, textures, return_rgb, face_light=None, textures_fill_ba
         _check_lights(lights, corner_shading, batch_size)
     if environment_sh is not None:
         _check_environment_sh(environment_sh, corner_shading, return_rgb, batch_size)
+    if normal_map is not None or corner_tangents is not None:
+        _check_normal_map(normal_map, corner_tangents, corner_shading, face_uvs, return_rgb, batch_size, num_faces)
     if corner_shading is not None or shading_params is not None:
         _check_phong_inputs(corner_shading, shading_params, face_light, corner_light, return_rgb, batch_size, num_faces)
     if return_rgb and face_light is not None:
@@ -175,6 +178,32 @@ def _check_environment_sh(sh, corner_shading, return_rgb, batch_size):
     if not ((sh.dim() == 2 or (sh.dim() == 3 and sh.shape[0] in (1, batch_size))) and tuple(sh.shape[-2:]) == (9, 3)):
         raise ValueError("environment_sh must have shape [9, 3] or [batch size, 9, 3], got %s" % (tuple(sh.shape),))
     if not sh.is_cuda:
+        raise NotImplementedError("neural_renderer_b200 has no CPU implementation (inputs must be CUDA tensors)")
+
+
+def _check_normal_map(normal_map, corner_tangents, corner_shading, face_uvs, return_rgb, batch_size, num_faces):
+    # decoded tangent-space normal map [Hm,Wm,3] / [1|B,Hm,Wm,3] and corner tangents [F,3,4] / [1|B,F,3,4], always together,
+    # on top of Phong shading of a texture image
+    if normal_map is None or corner_tangents is None:
+        raise ValueError("normal_map and corner_tangents go together: give both")
+    if corner_shading is None:
+        raise ValueError("normal_map needs Phong shading (corner_shading / shading_params)")
+    if not return_rgb:
+        raise ValueError("normal_map shades the RGB image: it needs return_rgb")
+    if face_uvs is None:
+        raise ValueError("normal_map is addressed by the UVs: it needs a texture image with face_uvs")
+    for name, t in (("normal_map", normal_map), ("corner_tangents", corner_tangents)):
+        if not isinstance(t, torch.Tensor) or not t.is_floating_point():
+            raise TypeError("%s must be a floating point torch.Tensor" % name)
+    if not ((normal_map.dim() == 3 or (normal_map.dim() == 4 and normal_map.shape[0] in (1, batch_size)))
+            and normal_map.shape[-1] == 3 and normal_map.shape[-2] >= 1 and normal_map.shape[-3] >= 1):
+        raise ValueError("normal_map must have shape [height, width, 3] or [batch size, height, width, 3], got %s"
+                         % (tuple(normal_map.shape),))
+    if not ((corner_tangents.dim() == 3 or (corner_tangents.dim() == 4 and corner_tangents.shape[0] in (1, batch_size)))
+            and tuple(corner_tangents.shape[-3:]) == (num_faces, 3, 4)):
+        raise ValueError("corner_tangents must have shape [num faces, 3, 4] or [batch size, num faces, 3, 4] with num faces "
+                         "= %d (the drawn faces, fill_back copies included), got %s" % (num_faces, tuple(corner_tangents.shape)))
+    if not normal_map.is_cuda or not corner_tangents.is_cuda:
         raise NotImplementedError("neural_renderer_b200 has no CPU implementation (inputs must be CUDA tensors)")
 
 
@@ -268,7 +297,7 @@ class _RasterizeFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, geom, textures, face_light, cfg, indices, face_uvs=None, corner_light=None, corner_shading=None,
-                shading_params=None, lights=None, environment_sh=None):
+                shading_params=None, lights=None, environment_sh=None, normal_map=None, corner_tangents=None):
         lib = _lib.load()
         dev = geom.device
         geom_c = geom.detach().contiguous()
@@ -280,6 +309,8 @@ class _RasterizeFunction(torch.autograd.Function):
         sp_c = shading_params.detach().to(torch.float32).contiguous() if shading_params is not None else None
         lt_c = lights.detach().to(torch.float32).contiguous() if lights is not None else None  # [Bl,NL,12], NL >= 1
         sh_c = environment_sh.detach().to(torch.float32).contiguous() if environment_sh is not None else None  # [Bs,9,3]
+        nm_c = normal_map.detach().to(torch.float32).contiguous() if normal_map is not None else None  # [Bm,Hm,Wm,3]
+        tg_c = corner_tangents.detach().to(torch.float32).contiguous() if corner_tangents is not None else None  # [Bt,F,3,4]
         flags = cfg.flags
         if indices is not None:
             B, Nv = geom_c.shape[:2]
@@ -348,7 +379,12 @@ class _RasterizeFunction(torch.autograd.Function):
                 ph = _phong_args(cs_c, sp_c)
                 la = _lights_args(lt_c) if lt_c is not None else None
                 sa = _sh_args(sh_c) if sh_c is not None else None
-                _lib.check(lib.nr_b200_forward_sh(ctypes.byref(a), ctypes.byref(ph), _byref(la), _byref(sa), _stream_ptr(dev)))
+                if nm_c is None:
+                    _lib.check(lib.nr_b200_forward_sh(ctypes.byref(a), ctypes.byref(ph), _byref(la), _byref(sa), _stream_ptr(dev)))
+                else:
+                    na = _normal_map_args(nm_c, tg_c)
+                    _lib.check(lib.nr_b200_forward_normal_map(ctypes.byref(a), ctypes.byref(ph), _byref(la), _byref(sa),
+                                                              ctypes.byref(na), _stream_ptr(dev)))
         ctx.cfg = cfg
         ctx.flags = flags
         ctx.ts = ts
@@ -363,12 +399,14 @@ class _RasterizeFunction(torch.autograd.Function):
         ctx.need_sp_grad = sp_c is not None and ctx.needs_input_grad[8]
         ctx.need_lt_grad = lt_c is not None and ctx.needs_input_grad[9]
         ctx.need_sh_grad = sh_c is not None and ctx.needs_input_grad[10]
+        ctx.need_nm_grad = nm_c is not None and ctx.needs_input_grad[11]
+        ctx.need_tg_grad = tg_c is not None and ctx.needs_input_grad[12]
         # interior_gradient: the backward differentiates the sampler, so it reads the textures (and face_uvs / corner_light)
         ctx.interior = cfg.interior and want_rgb and ctx.needs_input_grad[0]
         need_tex = need_light_grad or ctx.need_uv_grad or ctx.need_corner_grad or ctx.interior or ctx.need_cs_grad or \
-            ctx.need_sp_grad or ctx.need_lt_grad or ctx.need_sh_grad
+            ctx.need_sp_grad or ctx.need_lt_grad or ctx.need_sh_grad or ctx.need_nm_grad or ctx.need_tg_grad
         ctx.save_for_backward(geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c if need_tex else None, indices, uv_c, corner_c,
-                              cs_c, sp_c, lt_c, sh_c)
+                              cs_c, sp_c, lt_c, sh_c, nm_c, tg_c)
         if cfg.aa:
             rgb_o, alpha_o, depth_o = out_rgb, out_alpha, out_depth
         else:
@@ -381,7 +419,8 @@ class _RasterizeFunction(torch.autograd.Function):
         lib = _lib.load()
         cfg = ctx.cfg
         flags = ctx.flags | (_lib.NR_GRAD_INTERIOR if ctx.interior else 0)
-        geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c, indices, uv_c, corner_c, cs_c, sp_c, lt_c, sh_c = ctx.saved_tensors
+        geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c, indices, uv_c, corner_c, cs_c, sp_c, lt_c, sh_c, nm_c, tg_c = \
+            ctx.saved_tensors
         dev = geom_c.device
         B, F = geom_c.shape[0], ctx.F
         want_rgb = bool(flags & _lib.NR_RETURN_RGB)
@@ -407,6 +446,9 @@ class _RasterizeFunction(torch.autograd.Function):
             la = _lights_args(lt_c, grad_lt) if lt_c is not None else None
             grad_sh = torch.empty_like(sh_c) if ctx.need_sh_grad else None
             sa = _sh_args(sh_c, grad_sh) if sh_c is not None else None
+            grad_nm = torch.empty_like(nm_c) if ctx.need_nm_grad else None
+            grad_tg = torch.empty_like(tg_c) if ctx.need_tg_grad else None
+            na = _normal_map_args(nm_c, tg_c, grad_nm, grad_tg) if nm_c is not None else None
             ws_bytes = lib.nr_b200_backward_workspace_bytes(B, F, cfg.S, ctx.ts, flags)
             ws = torch.empty((max(ws_bytes, 16),), dtype=torch.uint8, device=dev)
             a = _lib.BackwardArgs()
@@ -429,6 +471,9 @@ class _RasterizeFunction(torch.autograd.Function):
             hook = _TEXTURE_GRAD_HOOK if (want_rgb and g_rgb is not None) else None
 
             def call():
+                if na is not None:  # normal map: grad_normal_map, grad_corner_tangents are filled by the texture half too
+                    return lib.nr_b200_backward_normal_map(ctypes.byref(a), ctypes.byref(ph), _byref(la), _byref(sa),
+                                                           ctypes.byref(na), _stream_ptr(dev))
                 if ph is not None:  # Phong: grad_corner_shading, grad_params, grad_lights, grad_sh are filled by the texture half
                     return lib.nr_b200_backward_sh(ctypes.byref(a), ctypes.byref(ph), _byref(la), _byref(sa), _stream_ptr(dev))
                 if corner_c is None:
@@ -449,7 +494,8 @@ class _RasterizeFunction(torch.autograd.Function):
                 _lib.check(call())
                 if pending is not None:
                     pending.wait()
-        return grad_geom, grad_textures, grad_light, None, None, grad_uvs, grad_corner, grad_cs, grad_sp, grad_lt, grad_sh
+        return (grad_geom, grad_textures, grad_light, None, None, grad_uvs, grad_corner, grad_cs, grad_sp, grad_lt, grad_sh,
+                grad_nm, grad_tg)
 
 
 def _byref(s):
@@ -492,6 +538,16 @@ def _sh_args(sh_c, grad_sh=None):
     return sa
 
 
+def _normal_map_args(nm_c, tg_c, grad_nm=None, grad_tg=None):
+    na = _lib.NormalMapArgs()
+    na.struct_size = ctypes.sizeof(_lib.NormalMapArgs)
+    na.map_batch, na.tangent_batch = int(nm_c.shape[0]), int(tg_c.shape[0])
+    na.map_height, na.map_width = int(nm_c.shape[1]), int(nm_c.shape[2])
+    na.normal_map, na.corner_tangents = _ptr(nm_c), _ptr(tg_c)
+    na.grad_normal_map, na.grad_corner_tangents = _ptr(grad_nm), _ptr(grad_tg)
+    return na
+
+
 class _MipPyramid(torch.autograd.Function):
     """image [Bt,Ht,Wt,3] -> packed mip pyramid [Bt,P,3] (nr_b200_mip_build); the backward collapses the pyramid gradient
     into the image gradient (nr_b200_mip_collapse, the exact transpose of the build)."""
@@ -527,7 +583,7 @@ TEXTURE_FILTERS = ('bilinear', 'trilinear')
 def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_color, return_rgb, return_alpha,
          return_depth, face_light=None, textures_fill_back=False, vertices=None, reference_exact=None, face_uvs=None,
          texture_filter='bilinear', corner_light=None, interior_gradient=False, corner_shading=None, shading_params=None,
-         lights=None, environment_sh=None):
+         lights=None, environment_sh=None, normal_map=None, corner_tangents=None):
     if (corner_shading is not None or shading_params is not None) and interior_gradient:
         raise ValueError("interior_gradient=True is not supported with Phong shading (corner_shading / shading_params): no "
                          "vertex gradient flows through the interpolation of the per-pixel normal and position")
@@ -542,7 +598,7 @@ def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_
                          "than one item: the reference-exact sampler reads the depths of item 0 for every item, so its "
                          "derivative would cross items.  Pass reference_exact=False (or set_reference_exact(False))")
     _check_inputs(faces, textures, return_rgb, face_light, textures_fill_back, vertices, face_uvs, corner_light,
-                  corner_shading, shading_params, lights, environment_sh)
+                  corner_shading, shading_params, lights, environment_sh, normal_map, corner_tangents)
     phong = corner_shading is not None
     indices = None
     if vertices is not None:
@@ -571,6 +627,9 @@ def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_
                     lights = None  # no extra light: Phong exactly
             if environment_sh is not None:
                 environment_sh = _batched(environment_sh, batch_size, 2)
+            if normal_map is not None:
+                normal_map = _batched(normal_map, batch_size, 3)
+                corner_tangents = _batched(corner_tangents, batch_size, 3)
     cfg = _make_config(image_size, anti_aliasing, near, far, eps, background_color, return_rgb, return_alpha,
                        return_depth, geom.device, batch_size, reference_exact)
     if return_rgb and textures_fill_back:
@@ -587,7 +646,8 @@ def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_
     return _RasterizeFunction.apply(geom, textures if return_rgb else None, face_light if return_rgb else None, cfg,
                                     indices, face_uvs, corner_light, corner_shading if return_rgb else None,
                                     shading_params if return_rgb else None, lights if return_rgb else None,
-                                    environment_sh if return_rgb else None)
+                                    environment_sh if return_rgb else None, normal_map if return_rgb else None,
+                                    corner_tangents if return_rgb else None)
 
 
 def rasterize_rgbad(
@@ -615,6 +675,8 @@ def rasterize_rgbad(
         shading_params=None,
         lights=None,
         environment_sh=None,
+        normal_map=None,
+        corner_tangents=None,
 ):
     """Generate RGB, alpha channel, and depth images from faces and textures (for RGB).  rasterize.py:900-977.
 
@@ -681,12 +743,20 @@ def rasterize_rgbad(
                               every diffuse term, unclamped (include/nr_b200.h, nr_b200_sh_args).  Only with
                               corner_shading / shading_params; composes with `lights`; receives gradients (a batch of 1
                               gets the sum over the items).
+      normal_map [Hm,Wm,3] / [1|B,Hm,Wm,3], corner_tangents [F,3,4] / [1|B,F,3,4]   Phong shading through a tangent-space
+                              normal map, always given together: the map holds decoded vectors (F.decode_normal_map; row 0
+                              = top, +y along +v) sampled bilinearly at the pixel's uv, and corner_tangents the (T, w)
+                              of every drawn face's corners (F.corner_tangents; F counts the fill_back copies, as
+                              corner_shading).  The shading normal becomes m_x t + m_y b + m_z n with b = sign(w) n x t
+                              (include/nr_b200.h, nr_b200_normal_map_args), for every light and the environment.  Needs
+                              corner_shading and a texture image with face_uvs; both receive gradients (a batch of 1
+                              gets the sum over the items), and face_uvs receives the map's term too.
     `textures` with batch size 1 (or an expanded stride-0 batch) while the geometry batch is larger = one texture set
     shared by every item (a mesh seen from B viewpoints, mesh.py:29-34); its gradient is the sum over the items."""
     rgb, alpha, depth, _, _ = _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_color,
                                    return_rgb, return_alpha, return_depth, face_light, textures_fill_back, vertices,
                                    reference_exact, face_uvs, texture_filter, corner_light, interior_gradient,
-                                   corner_shading, shading_params, lights, environment_sh)
+                                   corner_shading, shading_params, lights, environment_sh, normal_map, corner_tangents)
     return {
         'rgb': rgb if return_rgb else None,
         'alpha': alpha if return_alpha else None,
@@ -716,6 +786,8 @@ def rasterize(
         shading_params=None,
         lights=None,
         environment_sh=None,
+        normal_map=None,
+        corner_tangents=None,
 ):
     """RGB images [B,3,H,W] from faces and textures.  rasterize.py:980-1008 (keyword-only extras: rasterize_rgbad; in
     texture-image mode both the image and face_uvs receive gradients)."""
@@ -724,7 +796,7 @@ def rasterize(
         face_light=face_light, textures_fill_back=textures_fill_back, vertices=vertices,
         reference_exact=reference_exact, face_uvs=face_uvs, texture_filter=texture_filter, corner_light=corner_light,
         interior_gradient=interior_gradient, corner_shading=corner_shading, shading_params=shading_params,
-        lights=lights, environment_sh=environment_sh)['rgb']
+        lights=lights, environment_sh=environment_sh, normal_map=normal_map, corner_tangents=corner_tangents)['rgb']
 
 
 def rasterize_silhouettes(

@@ -42,6 +42,10 @@ class Renderer(object):
         # environment light of shading='phong': irradiance-ready SH coefficients [9,3] / [1|B,9,3]
         # (F.sh_from_environment_map), added to every pixel's diffuse light.  None = no environment
         self.environment_sh = None
+        # tangent-space normal map of shading='phong' with a texture image and face_uvs: decoded vectors [Hm,Wm,3] /
+        # [1|B,Hm,Wm,3] (F.decode_normal_map), sampled at the same UVs; the tangents come from F.vertex_tangents of the
+        # mesh.  It may require grad.  None = the interpolated normals alone
+        self.normal_map = None
 
         # rasterization
         self.rasterizer_eps = 1e-3
@@ -118,6 +122,11 @@ class Renderer(object):
             raise ValueError("lights (a light set) needs shading='phong', got shading=%r" % (self.shading,))
         if self.shading != 'phong' and self.environment_sh is not None:
             raise ValueError("environment_sh (an SH environment) needs shading='phong', got shading=%r" % (self.shading,))
+        if self.normal_map is not None:
+            if self.shading != 'phong':
+                raise ValueError("normal_map needs shading='phong', got shading=%r" % (self.shading,))
+            if face_uvs is None:
+                raise ValueError("normal_map is addressed by the UVs: it needs a texture image and face_uvs")
         fused = (self.fused and self._fusable(vertices, faces) and textures.is_cuda and textures.dtype == torch.float32)
         light_args = (self.light_intensity_ambient, self.light_intensity_directional, self.light_color_ambient,
                       self.light_color_directional, self.light_direction)
@@ -230,19 +239,35 @@ class Renderer(object):
         sh = self.environment_sh
         if sh is not None:
             sh = sh.to(vertices.device)
+        nm = self.normal_map
+        if nm is not None:
+            nm = nm.to(vertices.device)
         if fused:
             indices = self._indices(faces)
             # one mesh seen from B viewpoints (an expanded, stride-0 vertex batch and a shared index set): one corner set
             shared = vertices.shape[0] > 1 and vertices.stride(0) == 0 and indices.shape[0] == 1
             v1, f1 = (vertices[:1], faces[:1]) if shared else (vertices, faces)
-            cs = F.corner_shading(F.vertex_normals(v1, f1), v1, indices, fill_back=self.fill_back)
+            vn = F.vertex_normals(v1, f1)
+            cs = F.corner_shading(vn, v1, indices, fill_back=self.fill_back)
+            ct = None
+            if nm is not None:
+                # the shared mesh gets one tangent set too when its UVs are shared ([F,3,2], a batch of 1 or an
+                # expanded one); UVs that differ per item give every item the frame of its own UVs
+                uv_shared = face_uvs.dim() == 3 or face_uvs.shape[0] == 1 or face_uvs.stride(0) == 0
+                if shared and uv_shared:
+                    vt = F.vertex_tangents(v1, f1, face_uvs[:1] if face_uvs.dim() == 4 else face_uvs, vn)
+                else:
+                    vt = F.vertex_tangents(vertices, faces, face_uvs, vn.expand(vertices.shape[0], -1, -1))
+                ct = F.corner_tangents(vt, indices, fill_back=self.fill_back)
             return rasterize(
                 indices, textures, self.image_size, self.anti_aliasing, self.near, self.far, self.rasterizer_eps,
                 self.background_color, textures_fill_back=self.fill_back, vertices=self._transform(vertices),
                 reference_exact=self.reference_exact, face_uvs=face_uvs, texture_filter=texture_filter,
-                corner_shading=cs, shading_params=params, lights=lights, environment_sh=sh)
+                corner_shading=cs, shading_params=params, lights=lights, environment_sh=sh, normal_map=nm,
+                corner_tangents=ct)
         # op by op: torch normals and corners, materialised faces, doubled textures / UV corners for fill_back
         normals = F._vertex_normals_torch(vertices, faces)
+        vt = F.vertex_tangents(vertices, faces, face_uvs, normals) if nm is not None else None
         if self.fill_back:
             faces = torch.cat((faces, faces.flip(2)), dim=1)
             if face_uvs is not None:
@@ -250,8 +275,10 @@ class Renderer(object):
             else:
                 textures = torch.cat((textures, textures.permute(0, 1, 4, 3, 2, 5)), dim=1)
         cs = F._corner_shading_torch(normals, vertices, faces, self.fill_back)
+        ct = F.corner_tangents(vt, faces, fill_back=self.fill_back) if vt is not None else None
         faces = F.vertices_to_faces(self._transform(vertices), faces)
         return rasterize(
             faces, textures, self.image_size, self.anti_aliasing, self.near, self.far, self.rasterizer_eps,
             self.background_color, reference_exact=self.reference_exact, face_uvs=face_uvs,
-            texture_filter=texture_filter, corner_shading=cs, shading_params=params, lights=lights, environment_sh=sh)
+            texture_filter=texture_filter, corner_shading=cs, shading_params=params, lights=lights, environment_sh=sh,
+            normal_map=nm, corner_tangents=ct)
