@@ -418,6 +418,40 @@ typedef struct nr_b200_normal_map_args {
     float *grad_corner_tangents;     /* backward: [Bt,F,3,4] or NULL (the w slots receive 0) */
 } nr_b200_normal_map_args;
 
+/* Specular maps for Phong shading, additive to ABI 4: one struct (nr_b200_specular_map_args) and two entry points
+ * (nr_b200_forward_specular_map / nr_b200_backward_specular_map).  The map makes the specular colour and the shininess
+ * vary over the surface; everything diffuse is unchanged.
+ *   specular_map [Bq,Hq,Wq,4] (device, 16-byte aligned), HWC, row 0 = top, each texel (ks_r, ks_g, ks_b, sigma'),
+ *   Bq in {1, B} (1 = one map for every item, its gradient the sum over the items).
+ *   Covered raster pixel: (ks, sigma') = the map sampled at the pixel's uv exactly as nr_b200_normal_map_args samples its
+ *   map (NR_TEX_UV's uv, fill_back corners reversed, taps clamped at the map's own Hq x Wq, level 0 always, per channel
+ *   top = lerp(t00, t10, wx1), bot = lerp(t01, t11, wx1), q = lerp(top, bot, wy1), lerp(a, b, f) = fma(f, b - a, a), so
+ *   a constant map returns its value exactly).  With K'_c = ks_c * K_c and K'_jc = ks_c * K_jc (each product rounded),
+ *   the Phong / light-set / SH / normal-map expression is unchanged with K', K'_j and sigma' in place of K, K_j and
+ *   params' sigma:  h = [c > 0][q > 0] q^sigma',  rgb_c = fma(K'_c, h, L_c s_c), then fma(K'_jc, a_j h_j, rgb_c) per
+ *   light in order.  sigma' replaces params' shininess for params' light and for every light of the set, and is not
+ *   clamped.  A constant map (1, 1, 1, sigma of params) renders bit for bit as the same call without the map, and L_c
+ *   never reads the map.
+ *   Backward, texture half: g' = the upstream gradient of each highlight as without the map; the normal, position,
+ *   tangent, light and eye chains are evaluated with K' and sigma'.  grad_params[9+c] += g_c h ks_c, and grad_params[12]
+ *   receives 0 from a pixel shaded through the map (sigma is not read there); grad_lights[j][3+c] += g_c a_j h_j ks_c.
+ *   grad_specular_map's four taps += tap weight * gq with gq_c = g_c (K_c h + sum_j K_jc a_j h_j) for c < 3 and
+ *   gq_3 = sum_c g_c (K'_c h ln q + sum_j K'_jc a_j h_j ln q_j); grad_face_uvs also receives the map's l_k (gu, gv) by
+ *   NR_TEX_UV's formula with the map's taps, gq in place of g_c and the map's (Wq-1), (Hq-1) and clamp gates (with a
+ *   normal map too, the two UV terms add).  Masks and max take subgradient 0.  Each gradient output may be NULL and
+ *   is zero-filled first unless NR_GRAD_ACCUMULATE.  The faces half is unchanged.
+ *   Host rejections, before any launch: NR_ERR_INVALID_ARG for a struct_size mismatch, Bq not in {1, B}, a NULL or
+ *   not 16-byte aligned specular_map, Hq or Wq < 1, no NR_TEX_UV (the map is addressed by the UVs), grad_specular_map
+ *   without `textures`, and those of nr_b200_*_normal_map; NR_ERR_UNSUPPORTED for a map beyond 32-bit offsets and for
+ *   NR_GRAD_INTERIOR (as for every Phong mode).  A NULL struct is allowed: the call is then nr_b200_*_normal_map. */
+typedef struct nr_b200_specular_map_args {
+    uint32_t struct_size;            /* sizeof(nr_b200_specular_map_args) = 32 */
+    int32_t map_batch;               /* Bq: 1 or B */
+    int32_t map_height, map_width;   /* Hq, Wq >= 1 */
+    const float *specular_map;       /* [Bq,Hq,Wq,4], 16-byte aligned */
+    float *grad_specular_map;        /* backward: [Bq,Hq,Wq,4] or NULL (any 4-byte alignment) */
+} nr_b200_specular_map_args;
+
 /* Attribute interpolation, additive to ABI 4: two flag bits, one struct and two entry points.  Renders C >= 1 arbitrary
  * channels (normals, positions, UVs, labels, features) through the maps an ordinary forward call wrote (face_index_map,
  * weight_map; a silhouette-only forward suffices), with gradients into the attributes and, through the perspective
@@ -524,6 +558,17 @@ NR_B200_API int nr_b200_forward_normal_map(const nr_b200_forward_args *args, con
 NR_B200_API int nr_b200_backward_normal_map(const nr_b200_backward_args *args, const nr_b200_phong_args *phong,
                                             const nr_b200_lights_args *lights, const nr_b200_sh_args *sh,
                                             const nr_b200_normal_map_args *nm, void *cuda_stream);
+/* Phong shading through a specular map (nr_b200_specular_map_args above): the normal-map calls with `sm` added; lights,
+ * sh and nm may be NULL, and sm NULL runs exactly nr_b200_forward_normal_map / nr_b200_backward_normal_map.
+ * grad_specular_map is filled by the texture half. */
+NR_B200_API int nr_b200_forward_specular_map(const nr_b200_forward_args *args, const nr_b200_phong_args *phong,
+                                             const nr_b200_lights_args *lights, const nr_b200_sh_args *sh,
+                                             const nr_b200_normal_map_args *nm, const nr_b200_specular_map_args *sm,
+                                             void *cuda_stream);
+NR_B200_API int nr_b200_backward_specular_map(const nr_b200_backward_args *args, const nr_b200_phong_args *phong,
+                                              const nr_b200_lights_args *lights, const nr_b200_sh_args *sh,
+                                              const nr_b200_normal_map_args *nm, const nr_b200_specular_map_args *sm,
+                                              void *cuda_stream);
 /* Attribute interpolation (nr_b200_interpolate_args above): the image `out`, and its backward into grad_attributes and the
  * interior vertex gradient.  One kernel launch each (plus the zero-fill of the backward). */
 NR_B200_API int nr_b200_interpolate(const nr_b200_interpolate_args *args, void *cuda_stream);

@@ -54,6 +54,8 @@ EXPORTED_SYMBOLS = (
     "nr_b200_backward_sh",
     "nr_b200_forward_normal_map",
     "nr_b200_backward_normal_map",
+    "nr_b200_forward_specular_map",
+    "nr_b200_backward_specular_map",
     "nr_b200_interpolate",
     "nr_b200_interpolate_backward",
     "nr_b200_vertices_to_faces",
@@ -152,6 +154,14 @@ class NormalMapArgs(ctypes.Structure):
     ]
 
 
+class SpecularMapArgs(ctypes.Structure):
+    _fields_ = [
+        ("struct_size", ctypes.c_uint32), ("map_batch", ctypes.c_int32),
+        ("map_height", ctypes.c_int32), ("map_width", ctypes.c_int32),
+        ("specular_map", ctypes.c_void_p), ("grad_specular_map", ctypes.c_void_p),
+    ]
+
+
 class InterpolateArgs(ctypes.Structure):
     _fields_ = [
         ("struct_size", ctypes.c_uint32), ("flags", ctypes.c_uint32),
@@ -221,6 +231,16 @@ def load():
     lib.nr_b200_backward_normal_map.argtypes = [ctypes.POINTER(BackwardArgs), ctypes.POINTER(PhongArgs),
                                                 ctypes.POINTER(LightsArgs), ctypes.POINTER(ShArgs),
                                                 ctypes.POINTER(NormalMapArgs), ctypes.c_void_p]
+    lib.nr_b200_forward_specular_map.restype = ctypes.c_int
+    lib.nr_b200_forward_specular_map.argtypes = [ctypes.POINTER(ForwardArgs), ctypes.POINTER(PhongArgs),
+                                                 ctypes.POINTER(LightsArgs), ctypes.POINTER(ShArgs),
+                                                 ctypes.POINTER(NormalMapArgs), ctypes.POINTER(SpecularMapArgs),
+                                                 ctypes.c_void_p]
+    lib.nr_b200_backward_specular_map.restype = ctypes.c_int
+    lib.nr_b200_backward_specular_map.argtypes = [ctypes.POINTER(BackwardArgs), ctypes.POINTER(PhongArgs),
+                                                  ctypes.POINTER(LightsArgs), ctypes.POINTER(ShArgs),
+                                                  ctypes.POINTER(NormalMapArgs), ctypes.POINTER(SpecularMapArgs),
+                                                  ctypes.c_void_p]
     for name in ("nr_b200_interpolate", "nr_b200_interpolate_backward"):
         fn = getattr(lib, name)
         fn.restype = ctypes.c_int

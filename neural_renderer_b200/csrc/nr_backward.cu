@@ -1567,12 +1567,12 @@ extern "C" size_t nr_b200_backward_workspace_bytes(int32_t B, int32_t F, int32_t
     return bin_layout(B, F, S, strip_rec_bytes(S, both)).total;
 }
 
-// nr_b200_backward (corner_light, phong, lights, sh, nm NULL), nr_b200_backward_corner_light (smooth shading),
-// nr_b200_backward_phong (lights, sh, nm NULL), nr_b200_backward_lights (sh, nm NULL), nr_b200_backward_sh (nm NULL) and
-// nr_b200_backward_normal_map
+// nr_b200_backward (corner_light, phong, lights, sh, nm, sm NULL), nr_b200_backward_corner_light (smooth shading),
+// nr_b200_backward_phong (lights, sh, nm, sm NULL), nr_b200_backward_lights (sh, nm, sm NULL), nr_b200_backward_sh (nm, sm
+// NULL), nr_b200_backward_normal_map (sm NULL) and nr_b200_backward_specular_map
 static int backward_impl(const nr_b200_backward_args* args, const float* corner_light, float* grad_corner_light,
                          const nr_b200_phong_args* phong, const nr_b200_lights_args* lights, const nr_b200_sh_args* sh,
-                         const nr_b200_normal_map_args* nm, void* cuda_stream) {
+                         const nr_b200_normal_map_args* nm, const nr_b200_specular_map_args* sm, void* cuda_stream) {
     nr_internal::launch_count() = 0;
     // Two layouts: the full struct, and the ABI-4 struct from before grad_face_uvs (which then reads as NULL).  Only the
     // caller's struct_size bytes are read.
@@ -1610,9 +1610,9 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
     if (rgb && (flags & NR_TEX_FILL_BACK) && (F & 1)) return NR_ERR_INVALID_ARG;
     if (rgb && a->grad_face_light && !a->textures) return NR_ERR_INVALID_ARG;
     nr::Shading shading;
-    const int light = nr_internal::make_shading(rgb, a->face_light, corner_light, phong, lights, sh, nm, B, F, &shading);
+    const int light = nr_internal::make_shading(rgb, a->face_light, corner_light, phong, lights, sh, nm, sm, B, F, &shading);
     if (light < 0) return NR_ERR_INVALID_ARG;
-    if (nm && !uv) return NR_ERR_INVALID_ARG;  // the map is addressed by the pixel's uv
+    if ((nm || sm) && !uv) return NR_ERR_INVALID_ARG;  // the maps are addressed by the pixel's uv
     // the shading gradients: grad_corner_light needs corner_light, and every one reads the (unlit) textures (also a
     // grad_lights of a set of NL = 0 lights, which then receives nothing)
     if (grad_corner_light && !corner_light) return NR_ERR_INVALID_ARG;
@@ -1622,10 +1622,12 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
     float* grad_sh = sh ? sh->grad_sh : nullptr;
     float* grad_nm = nm ? nm->grad_normal_map : nullptr;
     float* grad_tg = nm ? nm->grad_corner_tangents : nullptr;
-    if (!a->textures && (grad_corner_light || grad_cs || grad_prm || (lights && lights->grad_lights) || grad_sh || grad_nm || grad_tg))
+    float* grad_sm = sm ? sm->grad_specular_map : nullptr;
+    if (!a->textures &&
+        (grad_corner_light || grad_cs || grad_prm || (lights && lights->grad_lights) || grad_sh || grad_nm || grad_tg || grad_sm))
         return NR_ERR_INVALID_ARG;
-    // a normal map also sends its own term into grad_face_uvs from the Phong-gradient kernel
-    const bool phong_grads = grad_cs || grad_prm || grad_lts || grad_sh || grad_nm || grad_tg || (nm && uv_grad);
+    // a normal or specular map also sends its own term into grad_face_uvs from the Phong-gradient kernel
+    const bool phong_grads = grad_cs || grad_prm || grad_lts || grad_sh || grad_nm || grad_tg || grad_sm || ((nm || sm) && uv_grad);
     // NR_GRAD_INTERIOR: the sampler's derivative reads the textures; the cubes of NR_TEX_Z_BATCH0 sample item b with the
     // depths of item 0, so their derivative would cross items (B = 1 is the plain sampler)
     const bool interior = (flags & NR_GRAD_INTERIOR) != 0;
@@ -1647,6 +1649,7 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
     if (uv && (tex_items * img_floats > 0x7FFFFFFFull || uv_floats * uv_items > 0x7FFFFFFFull))
         return NR_ERR_UNSUPPORTED;  // 32-bit image / UV offsets in the kernels
     if (nm && nr_internal::nm_floats(nm) * (size_t)nm->map_batch > 0x7FFFFFFFull) return NR_ERR_UNSUPPORTED;  // 32-bit map offsets
+    if (sm && nr_internal::sm_floats(sm) * (size_t)sm->map_batch > 0x7FFFFFFFull) return NR_ERR_UNSUPPORTED;
     const size_t need = nr_b200_backward_workspace_bytes(B, F, S, ts, flags);
     if (!a->workspace || a->workspace_bytes < need || ((uintptr_t)a->workspace & 15)) return NR_ERR_WORKSPACE;
     cudaStream_t stream = (cudaStream_t)cuda_stream;
@@ -1694,6 +1697,9 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
         if (part_tex && grad_tg &&
             cudaMemsetAsync(grad_tg, 0, (size_t)nm->tangent_batch * F * 12 * sizeof(float), stream) != cudaSuccess)
             return NR_ERR_CUDA;
+        if (part_tex && grad_sm &&
+            cudaMemsetAsync(grad_sm, 0, (size_t)sm->map_batch * nr_internal::sm_floats(sm) * sizeof(float), stream) != cudaSuccess)
+            return NR_ERR_CUDA;
         nr_internal::prof_end(stream);
     }
 
@@ -1724,8 +1730,11 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
     const dim3 pgrid((unsigned)(((size_t)S * S + 255) / 256), B);
     auto launch_texture_grad = [&]() {
         nr_internal::LaunchScope ls(uv ? "k_image_grad" : "k_texture_grad", stream);
-        // face_light is the kLightNone variant's run-time branch
-        const int tg_light = light == nr::kLightFace ? nr::kLightNone : light;
+        // face_light is the kLightNone variant's run-time branch; L_c of a specular-map render is that of the same call
+        // without the map
+        const int tg_light = light == nr::kLightFace ? nr::kLightNone
+                           : light != nr::kLightPhongSM ? light
+                           : nm ? nr::kLightPhongNM : sh ? nr::kLightPhongSH : shading.NL > 0 ? nr::kLightPhongSet : nr::kLightPhong;
         nr::dispatch_light<nr::kLightNone, nr::kLightCorner, nr::kLightPhong, nr::kLightPhongSet, nr::kLightPhongSH,
                            nr::kLightPhongNM>(tg_light, [&](auto kL) {
             if constexpr (kL != nr::kLightPhongNM) {  // a normal map needs NR_TEX_UV
@@ -1746,7 +1755,8 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
         nr_internal::PhongGradLaunch pl{};
         pl.args = a; pl.src = src; pl.shading = shading; pl.light = light;
         pl.grad_cs = grad_cs; pl.grad_prm = grad_prm; pl.grad_lts = grad_lts; pl.grad_sh = grad_sh;
-        pl.grad_nm = grad_nm; pl.grad_tg = grad_tg; pl.grad_uvs = nm ? a->grad_face_uvs : nullptr;
+        pl.grad_nm = grad_nm; pl.grad_tg = grad_tg; pl.grad_uvs = (nm || sm) ? a->grad_face_uvs : nullptr;
+        pl.grad_sm = grad_sm;
         pl.tex_bstride = (flags & NR_TEX_SHARED) ? 0 : (uv ? img_floats : ncubes * (size_t)ts * ts * ts * 3);
         pl.uv_bstride = p.uv_bstride;
         pl.tex_cmp = p.tex_cmp; pl.tex_val = p.tex_val;
@@ -1855,7 +1865,7 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
 }
 
 extern "C" int nr_b200_backward(const nr_b200_backward_args* args, void* cuda_stream) {
-    return backward_impl(args, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, cuda_stream);
+    return backward_impl(args, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, cuda_stream);
 }
 
 extern "C" int nr_b200_backward_corner_light(const nr_b200_backward_args* args, const float* corner_light,
@@ -1864,7 +1874,7 @@ extern "C" int nr_b200_backward_corner_light(const nr_b200_backward_args* args, 
         nr_internal::launch_count() = 0;
         return NR_ERR_INVALID_ARG;
     }
-    return backward_impl(args, corner_light, grad_corner_light, nullptr, nullptr, nullptr, nullptr, cuda_stream);
+    return backward_impl(args, corner_light, grad_corner_light, nullptr, nullptr, nullptr, nullptr, nullptr, cuda_stream);
 }
 
 extern "C" int nr_b200_backward_phong(const nr_b200_backward_args* args, const nr_b200_phong_args* phong, void* cuda_stream) {
@@ -1872,7 +1882,7 @@ extern "C" int nr_b200_backward_phong(const nr_b200_backward_args* args, const n
         nr_internal::launch_count() = 0;
         return NR_ERR_INVALID_ARG;
     }
-    return backward_impl(args, nullptr, nullptr, phong, nullptr, nullptr, nullptr, cuda_stream);
+    return backward_impl(args, nullptr, nullptr, phong, nullptr, nullptr, nullptr, nullptr, cuda_stream);
 }
 
 extern "C" int nr_b200_backward_lights(const nr_b200_backward_args* args, const nr_b200_phong_args* phong,
@@ -1881,7 +1891,7 @@ extern "C" int nr_b200_backward_lights(const nr_b200_backward_args* args, const 
         nr_internal::launch_count() = 0;
         return NR_ERR_INVALID_ARG;
     }
-    return backward_impl(args, nullptr, nullptr, phong, lights, nullptr, nullptr, cuda_stream);
+    return backward_impl(args, nullptr, nullptr, phong, lights, nullptr, nullptr, nullptr, cuda_stream);
 }
 
 extern "C" int nr_b200_backward_sh(const nr_b200_backward_args* args, const nr_b200_phong_args* phong,
@@ -1890,7 +1900,7 @@ extern "C" int nr_b200_backward_sh(const nr_b200_backward_args* args, const nr_b
         nr_internal::launch_count() = 0;
         return NR_ERR_INVALID_ARG;
     }
-    return backward_impl(args, nullptr, nullptr, phong, lights, sh, nullptr, cuda_stream);
+    return backward_impl(args, nullptr, nullptr, phong, lights, sh, nullptr, nullptr, cuda_stream);
 }
 
 extern "C" int nr_b200_backward_normal_map(const nr_b200_backward_args* args, const nr_b200_phong_args* phong,
@@ -1900,5 +1910,16 @@ extern "C" int nr_b200_backward_normal_map(const nr_b200_backward_args* args, co
         nr_internal::launch_count() = 0;
         return NR_ERR_INVALID_ARG;
     }
-    return backward_impl(args, nullptr, nullptr, phong, lights, sh, nm, cuda_stream);
+    return backward_impl(args, nullptr, nullptr, phong, lights, sh, nm, nullptr, cuda_stream);
+}
+
+extern "C" int nr_b200_backward_specular_map(const nr_b200_backward_args* args, const nr_b200_phong_args* phong,
+                                             const nr_b200_lights_args* lights, const nr_b200_sh_args* sh,
+                                             const nr_b200_normal_map_args* nm, const nr_b200_specular_map_args* sm,
+                                             void* cuda_stream) {
+    if (!phong) {
+        nr_internal::launch_count() = 0;
+        return NR_ERR_INVALID_ARG;
+    }
+    return backward_impl(args, nullptr, nullptr, phong, lights, sh, nm, sm, cuda_stream);
 }

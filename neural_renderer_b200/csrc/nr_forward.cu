@@ -85,6 +85,9 @@ constexpr int kOwnTable = 256;         // rows / fragments per pass whose owner 
 #ifndef NR_RESOLVE_NM_MIN_CTAS
 #define NR_RESOLVE_NM_MIN_CTAS 4         // Phong through a normal map (kLightPhongNM), both image samplers (DESIGN.md section 4k)
 #endif
+#ifndef NR_RESOLVE_SM_MIN_CTAS
+#define NR_RESOLVE_SM_MIN_CTAS 4         // Phong through a specular map (kLightPhongSM), both image samplers (DESIGN.md section 4l)
+#endif
 constexpr int kResolveTileW = 32, kResolveTileH = 8;  // API pixels per k_resolve CTA (256 threads, 8 x 4 per warp)
 constexpr uint32_t kStageBytes = 32 * 1024;  // shared memory of a k_resolve CTA for staged texture cubes
 
@@ -506,10 +509,10 @@ __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigne
                 const nr::UvTaps t = nr::uv_taps(u, v, p.Ht, p.Wt);
                 nr::uv_blend<kLight == nr::kLightFace>(p.textures + (uint32_t)b * p.img_bstride, p.Wt, t, l0, l1, l2, c);
             }
-            if constexpr (kLight == nr::kLightPhongNM) {  // the map is sampled at the same uv
+            if constexpr (kLight >= nr::kLightPhongNM) {  // the maps are sampled at the same uv
                 float l[3];
                 nr::perspective_weights(w, zp, cc.y, cc.z, cc.w, l);
-                nr::shade_nm(p.shading, b, fn, l, u, v, c);
+                nr::shade_mapped<kLight == nr::kLightPhongSM>(p.shading, b, fn, l, u, v, c);
             }
             o.r = c[0]; o.g = c[1]; o.b = c[2];
         } else {
@@ -522,7 +525,7 @@ __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigne
             const float* tex = p.textures + ((size_t)b * p.tex_bstride + cube) * (size_t)(ts * ts * ts) * 3;
             blend_corners<kLight == nr::kLightFace>(p, tc, tex, rev, b, fn, o.r, o.g, o.b);
         }
-        if constexpr (kLight >= nr::kLightCorner && kLight != nr::kLightPhongNM) {  // the light of the pixel's l_k (own depths) on the unlit sample
+        if constexpr (kLight >= nr::kLightCorner && kLight < nr::kLightPhongNM) {  // the light of the pixel's l_k (own depths) on the unlit sample
             float l[3], c[3] = {o.r, o.g, o.b};
             nr::perspective_weights(w, zp, cc.y, cc.z, cc.w, l);
             nr::shade<kLight>(p.shading, b, p.F, fn, l, c);
@@ -534,6 +537,7 @@ __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigne
 
 // CTAs per SM each k_resolve variant is compiled for (the NR_RESOLVE_*_MIN_CTAS above)
 constexpr int resolve_min_ctas(bool aa, int tex, int light) {
+    if (light == nr::kLightPhongSM) return NR_RESOLVE_SM_MIN_CTAS;
     if (light == nr::kLightPhongNM) return NR_RESOLVE_NM_MIN_CTAS;
     if (light == nr::kLightPhongSH) return NR_RESOLVE_SH_MIN_CTAS;
     if (light == nr::kLightPhongSet) return NR_RESOLVE_LIGHTS_MIN_CTAS;
@@ -743,10 +747,12 @@ extern "C" size_t nr_b200_forward_workspace_bytes(int32_t B, int32_t F, int32_t 
     return fwd_layout(B, F, S).total;
 }
 
-// nr_b200_forward (phong, lights, sh, nm NULL), nr_b200_forward_phong (lights, sh, nm NULL), nr_b200_forward_lights (sh, nm
-// NULL), nr_b200_forward_sh (nm NULL) and nr_b200_forward_normal_map
+// nr_b200_forward (phong, lights, sh, nm, sm NULL), nr_b200_forward_phong (lights, sh, nm, sm NULL), nr_b200_forward_lights
+// (sh, nm, sm NULL), nr_b200_forward_sh (nm, sm NULL), nr_b200_forward_normal_map (sm NULL) and
+// nr_b200_forward_specular_map
 static int forward_impl(const nr_b200_forward_args* args, const nr_b200_phong_args* phong, const nr_b200_lights_args* lights,
-                        const nr_b200_sh_args* sh, const nr_b200_normal_map_args* nm, void* cuda_stream) {
+                        const nr_b200_sh_args* sh, const nr_b200_normal_map_args* nm, const nr_b200_specular_map_args* sm,
+                        void* cuda_stream) {
     nr_internal::launch_count() = 0;
     // Two layouts: the full struct, and the ABI-4 struct from before corner_light (which then reads as NULL).  Only the
     // caller's struct_size bytes are read.
@@ -775,9 +781,9 @@ static int forward_impl(const nr_b200_forward_args* args, const nr_b200_phong_ar
     if (mip && !uv) return NR_ERR_INVALID_ARG;
     nr::Shading shading;
     const int light = nr_internal::make_shading((flags & NR_RETURN_RGB) != 0, a->face_light, a->corner_light, phong, lights, sh,
-                                                nm, B, F, &shading);
+                                                nm, sm, B, F, &shading);
     if (light < 0) return NR_ERR_INVALID_ARG;
-    if (nm && !uv) return NR_ERR_INVALID_ARG;  // the map is addressed by the pixel's uv
+    if ((nm || sm) && !uv) return NR_ERR_INVALID_ARG;  // the maps are addressed by the pixel's uv
     if ((flags & NR_ANTI_ALIASING) && (S & 1)) return NR_ERR_INVALID_ARG;
     if (S > 32767 || B > 65535) return NR_ERR_UNSUPPORTED;  // 32-bit pixel offsets; batch = grid.z of the resolve pass
     // NR_TEX_UV: image (NR_TEX_MIPMAP: pyramid) and UV offsets are 32-bit in the kernels
@@ -789,6 +795,7 @@ static int forward_impl(const nr_b200_forward_args* args, const nr_b200_phong_ar
                uv_floats * ((flags & NR_UV_SHARED) ? 1 : B) > 0x7FFFFFFFull))
         return NR_ERR_UNSUPPORTED;
     if (nm && nr_internal::nm_floats(nm) * (size_t)nm->map_batch > 0x7FFFFFFFull) return NR_ERR_UNSUPPORTED;  // 32-bit map offsets
+    if (sm && nr_internal::sm_floats(sm) * (size_t)sm->map_batch > 0x7FFFFFFFull) return NR_ERR_UNSUPPORTED;
     const size_t need = nr_b200_forward_workspace_bytes(B, F, S, ts, flags);
     if (!a->workspace || a->workspace_bytes < need || ((uintptr_t)a->workspace & 15)) return NR_ERR_WORKSPACE;
     cudaStream_t stream = (cudaStream_t)cuda_stream;
@@ -886,8 +893,8 @@ static int forward_impl(const nr_b200_forward_args* args, const nr_b200_phong_ar
         } else {
             rc = nr::dispatch_bool(aa, [&](auto kAA) {
                 return nr::dispatch_light<nr::kLightNone, nr::kLightFace, nr::kLightCorner, nr::kLightPhong, nr::kLightPhongSet,
-                                          nr::kLightPhongSH, nr::kLightPhongNM>(light, [&](auto kL) {
-                    if constexpr (kL == nr::kLightPhongNM) {  // NR_TEX_UV only
+                                          nr::kLightPhongSH, nr::kLightPhongNM, nr::kLightPhongSM>(light, [&](auto kL) {
+                    if constexpr (kL >= nr::kLightPhongNM) {  // NR_TEX_UV only
                         return mip ? launch_resolve<kAA, 3, kL>(p, grid, bx, smem, nslots, stream)
                                    : launch_resolve<kAA, 2, kL>(p, grid, bx, smem, nslots, stream);
                     } else {
@@ -904,7 +911,7 @@ static int forward_impl(const nr_b200_forward_args* args, const nr_b200_phong_ar
 }
 
 extern "C" int nr_b200_forward(const nr_b200_forward_args* args, void* cuda_stream) {
-    return forward_impl(args, nullptr, nullptr, nullptr, nullptr, cuda_stream);
+    return forward_impl(args, nullptr, nullptr, nullptr, nullptr, nullptr, cuda_stream);
 }
 
 extern "C" int nr_b200_forward_phong(const nr_b200_forward_args* args, const nr_b200_phong_args* phong, void* cuda_stream) {
@@ -912,7 +919,7 @@ extern "C" int nr_b200_forward_phong(const nr_b200_forward_args* args, const nr_
         nr_internal::launch_count() = 0;
         return NR_ERR_INVALID_ARG;
     }
-    return forward_impl(args, phong, nullptr, nullptr, nullptr, cuda_stream);
+    return forward_impl(args, phong, nullptr, nullptr, nullptr, nullptr, cuda_stream);
 }
 
 extern "C" int nr_b200_forward_lights(const nr_b200_forward_args* args, const nr_b200_phong_args* phong,
@@ -921,7 +928,7 @@ extern "C" int nr_b200_forward_lights(const nr_b200_forward_args* args, const nr
         nr_internal::launch_count() = 0;
         return NR_ERR_INVALID_ARG;
     }
-    return forward_impl(args, phong, lights, nullptr, nullptr, cuda_stream);
+    return forward_impl(args, phong, lights, nullptr, nullptr, nullptr, cuda_stream);
 }
 
 extern "C" int nr_b200_forward_sh(const nr_b200_forward_args* args, const nr_b200_phong_args* phong,
@@ -930,7 +937,7 @@ extern "C" int nr_b200_forward_sh(const nr_b200_forward_args* args, const nr_b20
         nr_internal::launch_count() = 0;
         return NR_ERR_INVALID_ARG;
     }
-    return forward_impl(args, phong, lights, sh, nullptr, cuda_stream);
+    return forward_impl(args, phong, lights, sh, nullptr, nullptr, cuda_stream);
 }
 
 extern "C" int nr_b200_forward_normal_map(const nr_b200_forward_args* args, const nr_b200_phong_args* phong,
@@ -940,5 +947,16 @@ extern "C" int nr_b200_forward_normal_map(const nr_b200_forward_args* args, cons
         nr_internal::launch_count() = 0;
         return NR_ERR_INVALID_ARG;
     }
-    return forward_impl(args, phong, lights, sh, nm, cuda_stream);
+    return forward_impl(args, phong, lights, sh, nm, nullptr, cuda_stream);
+}
+
+extern "C" int nr_b200_forward_specular_map(const nr_b200_forward_args* args, const nr_b200_phong_args* phong,
+                                            const nr_b200_lights_args* lights, const nr_b200_sh_args* sh,
+                                            const nr_b200_normal_map_args* nm, const nr_b200_specular_map_args* sm,
+                                            void* cuda_stream) {
+    if (!phong) {
+        nr_internal::launch_count() = 0;
+        return NR_ERR_INVALID_ARG;
+    }
+    return forward_impl(args, phong, lights, sh, nm, sm, cuda_stream);
 }

@@ -76,19 +76,29 @@ inline bool nm_args_ok(const nr_b200_normal_map_args* nm, int B) {
 // floats of one item's normal map (the kernels' offsets into it are 32-bit: the caller refuses more than 2^31 - 1 in all)
 inline size_t nm_floats(const nr_b200_normal_map_args* nm) { return (size_t)nm->map_height * (size_t)nm->map_width * 3; }
 
+// the same for a specular map (nr_b200_specular_map_args); its texels are read as aligned 16-byte vectors
+inline bool sm_args_ok(const nr_b200_specular_map_args* sm, int B) {
+    return sm->struct_size == sizeof(nr_b200_specular_map_args) && sm->specular_map &&
+           ((uintptr_t)sm->specular_map & 15) == 0 && (sm->map_batch == 1 || sm->map_batch == B) && sm->map_height >= 1 &&
+           sm->map_width >= 1;
+}
+// floats of one item's specular map (32-bit offsets in the kernels, as nm_floats)
+inline size_t sm_floats(const nr_b200_specular_map_args* sm) { return (size_t)sm->map_height * (size_t)sm->map_width * 4; }
+
 // The light mode (nr_shading.cuh) and nr::Shading of a call from its ABI arguments, or -1 for a refused combination
 // (NR_ERR_INVALID_ARG): corner_light only for RGB and instead of face_light; Phong only for RGB and instead of both; the
-// Phong, light-set, SH and normal-map structs pass their checks.  face_light is ignored without RGB, and a set of NL = 0
-// lights is the Phong call exactly.
+// Phong, light-set, SH, normal-map and specular-map structs pass their checks.  face_light is ignored without RGB, and a
+// set of NL = 0 lights is the Phong call exactly.
 inline int make_shading(bool rgb, const float* face_light, const float* corner_light, const nr_b200_phong_args* phong,
                         const nr_b200_lights_args* lights, const nr_b200_sh_args* sh, const nr_b200_normal_map_args* nm,
-                        int B, int F, nr::Shading* s) {
+                        const nr_b200_specular_map_args* sm, int B, int F, nr::Shading* s) {
     *s = nr::Shading{};
     if (corner_light && (!rgb || face_light)) return -1;
     if (phong && (!rgb || face_light || corner_light || !phong_args_ok(phong, B))) return -1;
     if (lights && !lights_args_ok(lights, B)) return -1;
     if (sh && !sh_args_ok(sh, B)) return -1;
     if (nm && (!phong || !nm_args_ok(nm, B))) return -1;
+    if (sm && (!phong || !sm_args_ok(sm, B))) return -1;
     if (lights && lights->num_lights == 0) lights = nullptr;
     s->face_light = rgb ? face_light : nullptr;
     s->corner_light = corner_light;
@@ -110,8 +120,14 @@ inline int make_shading(bool rgb, const float* face_light, const float* corner_l
         s->nm_bstride = nm->map_batch == 1 ? 0u : (uint32_t)nm_floats(nm);
         s->tg_bstride = nm->tangent_batch == 1 ? 0 : (size_t)F;
         s->Hm = nm->map_height; s->Wm = nm->map_width;
-        return nr::kLightPhongNM;
     }
+    if (sm) {
+        s->sm = sm->specular_map;
+        s->sm_bstride = sm->map_batch == 1 ? 0u : (uint32_t)sm_floats(sm);
+        s->Hq = sm->map_height; s->Wq = sm->map_width;
+        return nr::kLightPhongSM;
+    }
+    if (nm) return nr::kLightPhongNM;
     if (sh) return nr::kLightPhongSH;
     if (lights) return nr::kLightPhongSet;
     if (phong) return nr::kLightPhong;

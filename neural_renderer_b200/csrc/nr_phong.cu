@@ -1,8 +1,8 @@
-// nr_phong.cu -- the Phong-shading gradients of nr_b200_backward_phong, nr_b200_backward_lights, nr_b200_backward_sh and
-// nr_b200_backward_normal_map (include/nr_b200.h, nr_b200_phong_args, nr_b200_lights_args, nr_b200_sh_args,
-// nr_b200_normal_map_args).
+// nr_phong.cu -- the Phong-shading gradients of nr_b200_backward_phong, nr_b200_backward_lights, nr_b200_backward_sh,
+// nr_b200_backward_normal_map and nr_b200_backward_specular_map (include/nr_b200.h, nr_b200_phong_args,
+// nr_b200_lights_args, nr_b200_sh_args, nr_b200_normal_map_args, nr_b200_specular_map_args).
 //
-//   k_phong_grad<kTex, kIdx, kLights, kSH, kNM>   one thread per raster pixel, modelled on k_interior_grad.  The winner's perspective weights
+//   k_phong_grad<kTex, kIdx, kLights, kSH, kNM, kSM>   one thread per raster pixel, modelled on k_interior_grad.  The winner's perspective weights
 //                   l_k and the unlit sample s are recomputed with the forward's device helpers (the depth map gives zp;
 //                   per-face cubes read the sampler depths NR_TEX_Z_BATCH0 selects), nr::phong_at evaluates the forward's
 //                   expression and nr::phong_grad its derivative.  The 18 corner floats l_k (d loss / d n, d loss / d p) go
@@ -26,6 +26,13 @@
 //                   nm_grad_tail samples the map and builds the frame again and sends gm to the map's four taps (two
 //                   6-float rows by vector reductions, as k_image_grad); the 9 tangent floats l_k gt and the 6 UV floats l_k (gu, gv) widen the run reduction to 33.
 //                   The launcher picks kLights = NL > 0 and kSH = (sh given) as for the other modes.
+//                   kSM (kLightPhongSM, a specular map; kTex 1 / 2; kNM = a normal map given too): the map's sample
+//                   (ks, sigma') at the pixel's uv enters the expression and its derivative as K' = ks K, K'_j = ks K_j and
+//                   sigma' (the sq argument of the nr_math.cuh helpers).  Per pixel gq_c = K_c g_c h + sum_j K_jc g_c a_j h_j
+//                   is split off the K and K_j gradients (which keep ks_c times theirs) and gq_3 = d loss / d sigma' off
+//                   params' slot 12, which receives 0; sm_grad_tail samples the map again and sends gq to its four taps (one
+//                   16-byte vector reduction each) and l_k (gu, gv) to the UV floats of the run reduction (24, or shared with
+//                   the normal map's six in 33).
 //
 // It belongs to the texture half of the backward: the texture-gradient kernels (K6, k_image_grad) only need the pixel's
 // L_c, and keeping the 34 gradient floats out of them keeps their register budgets (DESIGN.md section 4g).
@@ -62,6 +69,7 @@ struct PhongParams {
     float* grad_nm;       // kNM: the layouts of normal_map, corner_tangents and face_uvs, or nullptr
     float* grad_tg;
     float* grad_uvs;
+    float* grad_sm;       // kSM: the layout of specular_map, or nullptr
 };
 
 // kNM, once g' = d loss / d n' of the pixel is known: the map's sample (with its uv derivative) and the frame again, the
@@ -113,6 +121,43 @@ __device__ __forceinline__ void nm_grad_tail(const PhongParams& p, int b, int fn
     cgx[13] = __fmul_rn(s2, gu); cgx[14] = __fmul_rn(s2, gv);
 }
 
+// kSM, once gq = d loss / d (ks, sigma') of the pixel is known: the map's uv derivative at the same taps, tap weight x gq to
+// the four taps of grad_sm (a clamped column, x1 = x0, merges its two taps first), and l_k (gu, gv) added into cuv[0..5]
+// for the stored face's UV corners (a fill_back copy's corner k is corner 2 - k)
+__device__ __forceinline__ void sm_grad_tail(const PhongParams& p, int b, const float lam[3], float u, float v, bool rev,
+                                             const float gq[4], float* cuv) {
+    const nr::Shading& s = p.shading;
+    const nr::UvTaps t = nr::uv_taps(u, v, s.Hq, s.Wq);
+    float q[4], du[4], dv[4];
+    nr::sm_sample<true>(s.sm + s.sm_off(b), s.Hq, s.Wq, t, q, du, dv);
+    if (p.grad_sm) {  // uniform
+        float* g0 = p.grad_sm + s.sm_off(b) + ((uint32_t)t.r0 * (uint32_t)s.Wq + (uint32_t)t.x0) * 4u;
+        float* g1 = p.grad_sm + s.sm_off(b) + ((uint32_t)t.r1 * (uint32_t)s.Wq + (uint32_t)t.x0) * 4u;
+        float v00[4], v10[4], v01[4], v11[4];
+#pragma unroll
+        for (int k = 0; k < 4; k++) {
+            v00[k] = __fmul_rn(t.w00, gq[k]); v10[k] = __fmul_rn(t.w10, gq[k]);
+            v01[k] = __fmul_rn(t.w01, gq[k]); v11[k] = __fmul_rn(t.w11, gq[k]);
+        }
+        if (t.x1 != t.x0) {
+            nr::red_add_4(g0, v00); nr::red_add_4(g0 + 4, v10);
+            nr::red_add_4(g1, v01); nr::red_add_4(g1 + 4, v11);
+        } else {
+#pragma unroll
+            for (int k = 0; k < 4; k++) { v00[k] = __fadd_rn(v00[k], v10[k]); v01[k] = __fadd_rn(v01[k], v11[k]); }
+            nr::red_add_4(g0, v00);
+            nr::red_add_4(g1, v01);
+        }
+    }
+    float gu = __fmul_rn(gq[0], du[0]), gv = __fmul_rn(gq[0], dv[0]);
+#pragma unroll
+    for (int k = 1; k < 4; k++) { gu = __fmaf_rn(gq[k], du[k], gu); gv = __fmaf_rn(gq[k], dv[k], gv); }
+    const float s0 = rev ? lam[2] : lam[0], s2 = rev ? lam[0] : lam[2];
+    cuv[0] = __fmaf_rn(s0, gu, cuv[0]); cuv[1] = __fmaf_rn(s0, gv, cuv[1]);
+    cuv[2] = __fmaf_rn(lam[1], gu, cuv[2]); cuv[3] = __fmaf_rn(lam[1], gv, cuv[3]);
+    cuv[4] = __fmaf_rn(s2, gu, cuv[4]); cuv[5] = __fmaf_rn(s2, gv, cuv[5]);
+}
+
 // kSH: the 27 floats Y_k w_c of grad_sh summed over the warp one at a time into shared memory, then over the CTA before 27
 // atomics into `o` (item b's [9,3] slot, or slot 0 with Bs = 1).  Every thread of the CTA calls it (0 off the mesh).
 __device__ __forceinline__ void sh_grad_reduce(const float Y[9], const float ws[3], float* o, int lane, int warp) {
@@ -133,10 +178,11 @@ __device__ __forceinline__ void sh_grad_reduce(const float Y[9], const float ws[
     }
 }
 
-template <int kTex, bool kIdx, bool kLights, bool kSH, bool kNM>
+template <int kTex, bool kIdx, bool kLights, bool kSH, bool kNM, bool kSM>
 __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ PhongParams p) {
-    static_assert(!kNM || kTex != 0, "a normal map needs NR_TEX_UV");
-    constexpr int kCg = kNM ? 33 : 18;  // the corner floats of the run reduction
+    static_assert(!(kNM || kSM) || kTex != 0, "the maps need NR_TEX_UV");
+    constexpr int kCg = kNM ? 33 : kSM ? 24 : 18;  // the corner floats of the run reduction
+    constexpr int kUv = kNM ? 27 : 18;              // kNM / kSM: where its 6 UV floats start
     __shared__ float s_prm[8][16];
     const int S = p.S;
     const size_t plane = (size_t)S * S;
@@ -161,9 +207,12 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
 #pragma unroll
         for (int k = 0; k < 3; k++) shw[k] = 0.0f;
     }
-    float nmu = 0.0f, nmv = 0.0f;  // kNM: the pixel's uv, its UV face and whether it is a fill_back copy
+    float nmu = 0.0f, nmv = 0.0f;  // kNM / kSM: the pixel's uv, its UV face and whether it is a fill_back copy
     int nmtf = 0;
     bool nmrev = false;
+    // kSM: the map's sample (ks, sigma') and d loss / d (ks, sigma') of the covered pixel
+    float smq[4] = {0.0f, 0.0f, 0.0f, 0.0f}, gq[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+    const float* sq = kSM ? smq : nullptr;
     if (fn >= 0) {
         const int r = (int)(i / S), c = (int)(i % S);
         const bool aa = p.aa != 0;
@@ -230,20 +279,33 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
         }
         const float* prm = p.shading.prm + p.shading.prm_off(b);
         nr::PhongEval E;
-        if constexpr (kNM) {  // the mapped normal in E.n, then the rest of phong_at
-            float uv[6], m[3];
+        if constexpr (kNM || kSM) {  // the mapped normal (or n) in E.n and the specular sample, then the rest of phong_at
+            float uv[6];
             nr::load_face_uvs(p.uvs + ((size_t)b * p.uv_bstride + (size_t)tf * 6u), rev, uv);
             nr::pixel_uv(w, zp, z[0], z[1], z[2], uv, nmu, nmv);
             nmtf = tf; nmrev = rev;
-            nr::NmFrame Fm;
-            nr::nm_pixel_normal(p.shading, b, fn, lam, nmu, nmv, m, Fm, E);
+            if constexpr (kNM) {
+                float m[3];
+                nr::NmFrame Fm;
+                nr::nm_pixel_normal(p.shading, b, fn, lam, nmu, nmv, m, Fm, E);
+            } else {
+                nr::phong_normal(p.shading.cs + p.shading.cs_off(b, fn), lam, E.n);
+            }
+            if constexpr (kSM) nr::sm_pixel_sample(p.shading, b, nmu, nmv, smq);
             nr::phong_diffuse_n(prm, E);
-            nr::phong_specular(p.shading.cs + p.shading.cs_off(b, fn), lam, prm, E);
+            nr::phong_specular(p.shading.cs + p.shading.cs_off(b, fn), lam, prm, E, sq);
         } else {
             nr::phong_at(p.shading.cs + p.shading.cs_off(b, fn), lam, prm, E);
         }
         float gn[3], gp[3];
-        nr::phong_grad(E, prm, g, s, gn, gp, gprm);
+        nr::phong_grad(E, prm, g, s, gn, gp, gprm, sq);
+        if constexpr (kSM) {  // g_c h: K_c's share to the map, ks_c's to K_c
+#pragma unroll
+            for (int k = 0; k < 3; k++) {
+                gq[k] = __fmul_rn(__ldg(prm + 9 + k), gprm[9 + k]);
+                gprm[9 + k] = __fmul_rn(smq[k], gprm[9 + k]);
+            }
+        }
         if constexpr (kLights) {  // the set's gradients read neither E.L nor the set's diffuse terms
             nr::phong_position(p.shading.cs + p.shading.cs_off(b, fn), lam, xpos);
             xE = E;
@@ -263,6 +325,11 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
                 for (int k = 0; k < 3; k++) gn[k] = __fadd_rn(gn[k], t[k]);
             }
             if constexpr (kNM) nm_grad_tail(p, b, fn, lam, nmu, nmv, nmrev, gn, cg + 18);
+            if constexpr (kSM) {  // d loss / d sigma' goes to the map, not to params' sigma
+                gq[3] = gprm[12];
+                gprm[12] = 0.0f;
+                sm_grad_tail(p, b, lam, nmu, nmv, nmrev, gq, cg + kUv);
+            }
 #pragma unroll
             for (int k = 0; k < 3; k++)
 #pragma unroll
@@ -275,13 +342,22 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
     if constexpr (kLights) {
         __shared__ float s_lt[8][nr_internal::kMaxLights * 10];  // per warp: each light's 10 record floats
         const float* lts = p.shading.lts + p.shading.lts_off(b);
-        const float sigma = __ldg(p.shading.prm + p.shading.prm_off(b) + 12);
+        const float sigma = kSM ? smq[3] : __ldg(p.shading.prm + p.shading.prm_off(b) + 12);
         float gnh[3] = {0.0f, 0.0f, 0.0f}, gvh[3] = {0.0f, 0.0f, 0.0f}, gsig = 0.0f;
         for (int j = 0; j < p.shading.NL; j++) {  // uniform
             float gl[10];
 #pragma unroll
             for (int k = 0; k < 10; k++) gl[k] = 0.0f;
-            if (fn >= 0) nr::phong_light_grad(lts + 12 * j, xE, xpos, sigma, xg, xs, gnh, gvh, xgp, gsig, gl);
+            if (fn >= 0) {
+                nr::phong_light_grad(lts + 12 * j, xE, xpos, sigma, xg, xs, gnh, gvh, xgp, gsig, gl, sq);
+                if constexpr (kSM) {  // g_c a_j h_j: K_jc's share to the map, ks_c's to K_jc
+#pragma unroll
+                    for (int k = 0; k < 3; k++) {
+                        gq[k] = __fmaf_rn(__ldg(lts + 12 * j + 3 + k), gl[3 + k], gq[k]);
+                        gl[3 + k] = __fmul_rn(smq[k], gl[3 + k]);
+                    }
+                }
+            }
             if (p.grad_lts) {  // uniform
 #pragma unroll
                 for (int off = 16; off > 0; off >>= 1)
@@ -311,6 +387,11 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
         if (fn >= 0) {
             nr::phong_lights_grad_end(xE, gnh, gvh, gsig, xgn, xgp, gprm);
             if constexpr (kNM) nm_grad_tail(p, b, fn, xlam, nmu, nmv, nmrev, xgn, cg + 18);
+            if constexpr (kSM) {
+                gq[3] = gprm[12];
+                gprm[12] = 0.0f;
+                sm_grad_tail(p, b, xlam, nmu, nmv, nmrev, gq, cg + kUv);
+            }
 #pragma unroll
             for (int k = 0; k < 3; k++)
 #pragma unroll
@@ -332,8 +413,8 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
     if constexpr (kSH && !kLights) {
         if (p.grad_sh) sh_grad_reduce(shY, shw, p.grad_sh + p.shading.sh_off(b), lane, warp);  // uniform
     }
-    if (kNM ? (p.grad_cs || p.grad_tg || p.grad_uvs) : p.grad_cs != nullptr) {  // uniform
-        // the segmented run reduction of k_depth_grad over 18 (kNM: 33) floats, then one set of atomics per run
+    if ((kNM || kSM) ? (p.grad_cs || p.grad_tg || p.grad_uvs) : p.grad_cs != nullptr) {  // uniform
+        // the segmented run reduction of k_depth_grad over 18 (kNM: 33, kSM: 24) floats, then one set of atomics per run
         const int fn_prev = __shfl_up_sync(0xffffffffu, fn, 1);
         const uint32_t heads = __ballot_sync(0xffffffffu, lane == 0 || fn != fn_prev);
         const uint32_t later = heads & ~((2u << lane) - 1u);
@@ -348,7 +429,7 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
             }
         }
         if (fn >= 0 && ((heads >> lane) & 1u)) {
-            if (!kNM || p.grad_cs) {
+            if (!(kNM || kSM) || p.grad_cs) {
                 float* o = p.grad_cs + p.shading.cs_off(b, fn);
 #pragma unroll
                 for (int k = 0; k < 18; k++) atomicAdd(o + k, cg[k]);
@@ -361,10 +442,12 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
 #pragma unroll
                         for (int j = 0; j < 3; j++) atomicAdd(o + 4 * k + j, cg[18 + 3 * k + j]);
                 }
+            }
+            if constexpr (kNM || kSM) {
                 if (p.grad_uvs) {
                     float* o = p.grad_uvs + ((size_t)b * p.uv_bstride + (size_t)nmtf * 6u);
 #pragma unroll
-                    for (int k = 0; k < 6; k++) atomicAdd(o + k, cg[27 + k]);
+                    for (int k = 0; k < 6; k++) atomicAdd(o + k, cg[kUv + k]);
                 }
             }
         }
@@ -410,22 +493,28 @@ void launch_phong_grad(const PhongGradLaunch& L, cudaStream_t stream) {
     p.tex_cmp = L.tex_cmp; p.tex_val = L.tex_val;
     if (L.mip) p.mip = *L.mip;
     p.shading = L.shading;
-    p.grad_nm = L.grad_nm; p.grad_tg = L.grad_tg; p.grad_uvs = L.grad_uvs;
+    p.grad_nm = L.grad_nm; p.grad_tg = L.grad_tg; p.grad_uvs = L.grad_uvs; p.grad_sm = L.grad_sm;
     const bool idx = (flags & NR_FACES_INDEXED) != 0;
     const int tex = (flags & NR_TEX_MIPMAP) ? 2 : (flags & NR_TEX_UV) ? 1 : 0;
     const dim3 grid((unsigned)(((size_t)p.S * p.S + 255) / 256), a->batch_size);
     LaunchScope ls("k_phong_grad", stream);
     // the kernel's split of the mode: a light set of NL > 0 lights (kLightPhongSet, or kLightPhongSH / kLightPhongNM with
-    // one), an SH environment (kLightPhongSH, or kLightPhongNM with one), a normal map (kLightPhongNM, NR_TEX_UV only)
+    // one), an SH environment (kLightPhongSH, or kLightPhongNM / kLightPhongSM with one), a normal map (kLightPhongNM, or
+    // kLightPhongSM with one; NR_TEX_UV only), a specular map (kLightPhongSM)
     nr::dispatch_bool(p.shading.NL > 0, [&](auto kLights) {
         nr::dispatch_bool(p.shading.sh != nullptr, [&](auto kSH) {
             nr::dispatch_bool(idx, [&](auto kIdx) {
-                if (L.light == nr::kLightPhongNM) {
-                    if (tex == 2) k_phong_grad<2, kIdx, kLights, kSH, true><<<grid, 256, 0, stream>>>(p);
-                    else k_phong_grad<1, kIdx, kLights, kSH, true><<<grid, 256, 0, stream>>>(p);
-                } else if (tex == 2) k_phong_grad<2, kIdx, kLights, kSH, false><<<grid, 256, 0, stream>>>(p);
-                else if (tex == 1) k_phong_grad<1, kIdx, kLights, kSH, false><<<grid, 256, 0, stream>>>(p);
-                else k_phong_grad<0, kIdx, kLights, kSH, false><<<grid, 256, 0, stream>>>(p);
+                if (L.light == nr::kLightPhongSM) {
+                    nr::dispatch_bool(p.shading.nm != nullptr, [&](auto kNM) {
+                        if (tex == 2) k_phong_grad<2, kIdx, kLights, kSH, kNM, true><<<grid, 256, 0, stream>>>(p);
+                        else k_phong_grad<1, kIdx, kLights, kSH, kNM, true><<<grid, 256, 0, stream>>>(p);
+                    });
+                } else if (L.light == nr::kLightPhongNM) {
+                    if (tex == 2) k_phong_grad<2, kIdx, kLights, kSH, true, false><<<grid, 256, 0, stream>>>(p);
+                    else k_phong_grad<1, kIdx, kLights, kSH, true, false><<<grid, 256, 0, stream>>>(p);
+                } else if (tex == 2) k_phong_grad<2, kIdx, kLights, kSH, false, false><<<grid, 256, 0, stream>>>(p);
+                else if (tex == 1) k_phong_grad<1, kIdx, kLights, kSH, false, false><<<grid, 256, 0, stream>>>(p);
+                else k_phong_grad<0, kIdx, kLights, kSH, false, false><<<grid, 256, 0, stream>>>(p);
             });
         });
     });

@@ -24,6 +24,8 @@ constexpr int kLightPhongSet = 4;  // the same with a light set of NL > 0 lights
 constexpr int kLightPhongSH = 5;   // the same with an SH environment, and a light set of NL >= 0 lights
 constexpr int kLightPhongNM = 6;   // Phong through a tangent-space normal map (NR_TEX_UV only), with a light set of NL >= 0
                                    // lights and an optional SH environment (both uniform per launch, decided at run time)
+constexpr int kLightPhongSM = 7;   // Phong through a specular map (NR_TEX_UV only), with a light set of NL >= 0 lights, an
+                                   // optional SH environment and an optional normal map (all uniform, decided at run time)
 
 // The shading inputs of one call; strides are 0 for a set shared by every batch item.
 struct Shading {
@@ -43,6 +45,9 @@ struct Shading {
     uint32_t nm_bstride;        // floats per item in nm (0 with Bm = 1; 32-bit, checked on the host)
     size_t tg_bstride;          // faces per item in tg (0 with Bt = 1)
     int Hm, Wm;
+    const float* sm;            // specular map [Bq,Hq,Wq,4] (kLightPhongSM)
+    uint32_t sm_bstride;        // floats per item in sm (0 with Bq = 1; 32-bit, checked on the host)
+    int Hq, Wq;
 
     // float offsets of item b's records (and of face fn's; F = faces per item of the [B,F,...] light tensors), shared
     // with the gradients of the same layout
@@ -54,6 +59,7 @@ struct Shading {
     __host__ __device__ __forceinline__ size_t sh_off(int b) const { return (size_t)b * sh_bstride; }
     __host__ __device__ __forceinline__ uint32_t nm_off(int b) const { return (uint32_t)b * nm_bstride; }
     __host__ __device__ __forceinline__ size_t tg_off(int b, int fn) const { return ((size_t)b * tg_bstride + fn) * 12; }
+    __host__ __device__ __forceinline__ uint32_t sm_off(int b) const { return (uint32_t)b * sm_bstride; }
 };
 
 // kLightPhongNM: the map's sample at the pixel's (u, v) and the frame of face fn's pixel, the mapped normal in E.n
@@ -81,23 +87,38 @@ __device__ __forceinline__ void pixel_light_nm(const Shading& s, int b, int fn, 
     if (s.sh) sh_add_irradiance(s.sh + s.sh_off(b), E);  // uniform
     L[0] = E.L[0]; L[1] = E.L[1]; L[2] = E.L[2];
 }
-// shade of kLightPhongNM: the rgb of the light-set / SH expression with the mapped normal (NL = 0 and no environment:
-// phong_lights_rgb is phong_rgb, so a flat map renders as the modes 3-5 do, bit for bit)
-__device__ __forceinline__ void shade_nm(const Shading& s, int b, int fn, const float l[3], float u, float v, float c[3]) {
+// kLightPhongSM: the specular map's sample sq = (ks, sigma') at the pixel's (u, v)
+__device__ __forceinline__ void sm_pixel_sample(const Shading& s, int b, float u, float v, float sq[4]) {
+    float du[4], dv[4];
+    sm_sample<false>(s.sm + s.sm_off(b), s.Hq, s.Wq, uv_taps(u, v, s.Hq, s.Wq), sq, du, dv);
+}
+// shade of kLightPhongNM (kSM false) and kLightPhongSM (kSM): the rgb of the light-set / SH expression with the mapped
+// normal (kSM: the interpolated one when no normal map is given) and kSM's K' and sigma' (NL = 0 and no environment:
+// phong_lights_rgb is phong_rgb, so a flat normal map and a constant (1, 1, 1, sigma) specular map render as the modes
+// 3-5 do, bit for bit)
+template <bool kSM>
+__device__ __forceinline__ void shade_mapped(const Shading& s, int b, int fn, const float l[3], float u, float v, float c[3]) {
     const float* prm = s.prm + s.prm_off(b);
     const float* lts = s.lts + s.lts_off(b);
     const float* cs = s.cs + s.cs_off(b, fn);
     PhongEval E;
-    NmFrame F;
-    float m[3];
-    nm_pixel_normal(s, b, fn, l, u, v, m, F, E);
+    if (!kSM || s.nm) {  // uniform
+        NmFrame F;
+        float m[3];
+        nm_pixel_normal(s, b, fn, l, u, v, m, F, E);
+    } else {
+        phong_normal(cs, l, E.n);
+    }
+    float sq[4];
+    if constexpr (kSM) sm_pixel_sample(s, b, u, v, sq);
+    const float* q = kSM ? sq : nullptr;
     phong_diffuse_n(prm, E);
-    phong_specular(cs, l, prm, E);
+    phong_specular(cs, l, prm, E, q);
     float pos[3], rgb[3];
     phong_position(cs, l, pos);
     lights_diffuse_loop(lts, s.NL, pos, E);
     if (s.sh) sh_add_irradiance(s.sh + s.sh_off(b), E);  // uniform
-    phong_lights_rgb(E, pos, prm, lts, s.NL, c, rgb);
+    phong_lights_rgb(E, pos, prm, lts, s.NL, c, rgb, q);
     c[0] = rgb[0]; c[1] = rgb[1]; c[2] = rgb[2];
 }
 

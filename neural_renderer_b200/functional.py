@@ -905,3 +905,18 @@ def decode_normal_map(image, green_down=False):
     if green_down:
         m = m * torch.tensor([1.0, -1.0, 1.0], dtype=m.dtype, device=m.device)
     return m
+
+
+def specular_map(color, shininess):
+    """A specular colour [...,H,W,3] and a shininess [...,H,W] (or a scalar / any tensor that broadcasts to [...,H,W])
+    -> the [...,H,W,4] map (ks_r, ks_g, ks_b, shininess) that rasterize(..., specular_map=...) and Renderer.specular_map
+    take.  Differentiable in both; the shininess is not clamped, so a fit may want to pass exp(log_shininess)."""
+    if not isinstance(color, torch.Tensor) or color.dim() < 3 or color.shape[-1] != 3:
+        raise ValueError("color must have shape [..., height, width, 3], got %s"
+                         % (tuple(color.shape) if isinstance(color, torch.Tensor) else type(color).__name__,))
+    sig = torch.as_tensor(shininess, dtype=color.dtype, device=color.device)
+    try:
+        sig = sig.expand(color.shape[:-1])
+    except RuntimeError:
+        raise ValueError("shininess must broadcast to %s, got %s" % (tuple(color.shape[:-1]), tuple(sig.shape))) from None
+    return torch.cat((color, sig[..., None]), dim=-1)

@@ -62,7 +62,7 @@ def _ptr(t):
 
 def _check_inputs(faces, textures, return_rgb, face_light=None, textures_fill_back=False, vertices=None, face_uvs=None,
                   corner_light=None, corner_shading=None, shading_params=None, lights=None, environment_sh=None,
-                  normal_map=None, corner_tangents=None):
+                  normal_map=None, corner_tangents=None, specular_map=None):
     # rasterize.py:66-90 (chainer type_check) -> TypeError / ValueError with the same conditions
     if not isinstance(faces, torch.Tensor):
         raise TypeError("faces must be a torch.Tensor")
@@ -110,6 +110,8 @@ def _check_inputs(faces, textures, return_rgb, face_light=None, textures_fill_ba
         _check_environment_sh(environment_sh, corner_shading, return_rgb, batch_size)
     if normal_map is not None or corner_tangents is not None:
         _check_normal_map(normal_map, corner_tangents, corner_shading, face_uvs, return_rgb, batch_size, num_faces)
+    if specular_map is not None:
+        _check_specular_map(specular_map, corner_shading, face_uvs, return_rgb, batch_size)
     if corner_shading is not None or shading_params is not None:
         _check_phong_inputs(corner_shading, shading_params, face_light, corner_light, return_rgb, batch_size, num_faces)
     if return_rgb and face_light is not None:
@@ -207,6 +209,25 @@ def _check_normal_map(normal_map, corner_tangents, corner_shading, face_uvs, ret
         raise NotImplementedError("neural_renderer_b200 has no CPU implementation (inputs must be CUDA tensors)")
 
 
+def _check_specular_map(specular_map, corner_shading, face_uvs, return_rgb, batch_size):
+    # specular map [Hq,Wq,4] / [1|B,Hq,Wq,4] of (ks_r, ks_g, ks_b, shininess) on top of Phong shading of a texture image
+    if corner_shading is None:
+        raise ValueError("specular_map needs Phong shading (corner_shading / shading_params)")
+    if not return_rgb:
+        raise ValueError("specular_map shades the RGB image: it needs return_rgb")
+    if face_uvs is None:
+        raise ValueError("specular_map is addressed by the UVs: it needs a texture image with face_uvs")
+    if not isinstance(specular_map, torch.Tensor) or not specular_map.is_floating_point():
+        raise TypeError("specular_map must be a floating point torch.Tensor")
+    sm = specular_map
+    if not ((sm.dim() == 3 or (sm.dim() == 4 and sm.shape[0] in (1, batch_size)))
+            and sm.shape[-1] == 4 and sm.shape[-2] >= 1 and sm.shape[-3] >= 1):
+        raise ValueError("specular_map must have shape [height, width, 4] or [batch size, height, width, 4], got %s"
+                         % (tuple(sm.shape),))
+    if not sm.is_cuda:
+        raise NotImplementedError("neural_renderer_b200 has no CPU implementation (inputs must be CUDA tensors)")
+
+
 def _check_uv_inputs(image, face_uvs, batch_size, num_uv_faces):
     # texture image [Ht,Wt,3] / [1|B,Ht,Wt,3] and per-corner UVs [F,3,2] / [1|B,F,3,2] (F/2 faces with textures_fill_back)
     if not isinstance(face_uvs, torch.Tensor) or not face_uvs.is_floating_point():
@@ -297,7 +318,8 @@ class _RasterizeFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, geom, textures, face_light, cfg, indices, face_uvs=None, corner_light=None, corner_shading=None,
-                shading_params=None, lights=None, environment_sh=None, normal_map=None, corner_tangents=None):
+                shading_params=None, lights=None, environment_sh=None, normal_map=None, corner_tangents=None,
+                specular_map=None):
         lib = _lib.load()
         dev = geom.device
         geom_c = geom.detach().contiguous()
@@ -311,6 +333,9 @@ class _RasterizeFunction(torch.autograd.Function):
         sh_c = environment_sh.detach().to(torch.float32).contiguous() if environment_sh is not None else None  # [Bs,9,3]
         nm_c = normal_map.detach().to(torch.float32).contiguous() if normal_map is not None else None  # [Bm,Hm,Wm,3]
         tg_c = corner_tangents.detach().to(torch.float32).contiguous() if corner_tangents is not None else None  # [Bt,F,3,4]
+        sm_c = specular_map.detach().to(torch.float32).contiguous() if specular_map is not None else None  # [Bq,Hq,Wq,4]
+        if sm_c is not None and sm_c.data_ptr() % 16:
+            sm_c = sm_c.clone()  # the kernels read a texel as one aligned 16-byte vector
         flags = cfg.flags
         if indices is not None:
             B, Nv = geom_c.shape[:2]
@@ -379,7 +404,12 @@ class _RasterizeFunction(torch.autograd.Function):
                 ph = _phong_args(cs_c, sp_c)
                 la = _lights_args(lt_c) if lt_c is not None else None
                 sa = _sh_args(sh_c) if sh_c is not None else None
-                if nm_c is None:
+                if sm_c is not None:
+                    na = _normal_map_args(nm_c, tg_c) if nm_c is not None else None
+                    _lib.check(lib.nr_b200_forward_specular_map(ctypes.byref(a), ctypes.byref(ph), _byref(la), _byref(sa),
+                                                                _byref(na), ctypes.byref(_specular_map_args(sm_c)),
+                                                                _stream_ptr(dev)))
+                elif nm_c is None:
                     _lib.check(lib.nr_b200_forward_sh(ctypes.byref(a), ctypes.byref(ph), _byref(la), _byref(sa), _stream_ptr(dev)))
                 else:
                     na = _normal_map_args(nm_c, tg_c)
@@ -401,12 +431,13 @@ class _RasterizeFunction(torch.autograd.Function):
         ctx.need_sh_grad = sh_c is not None and ctx.needs_input_grad[10]
         ctx.need_nm_grad = nm_c is not None and ctx.needs_input_grad[11]
         ctx.need_tg_grad = tg_c is not None and ctx.needs_input_grad[12]
+        ctx.need_sm_grad = sm_c is not None and ctx.needs_input_grad[13]
         # interior_gradient: the backward differentiates the sampler, so it reads the textures (and face_uvs / corner_light)
         ctx.interior = cfg.interior and want_rgb and ctx.needs_input_grad[0]
         need_tex = need_light_grad or ctx.need_uv_grad or ctx.need_corner_grad or ctx.interior or ctx.need_cs_grad or \
-            ctx.need_sp_grad or ctx.need_lt_grad or ctx.need_sh_grad or ctx.need_nm_grad or ctx.need_tg_grad
+            ctx.need_sp_grad or ctx.need_lt_grad or ctx.need_sh_grad or ctx.need_nm_grad or ctx.need_tg_grad or ctx.need_sm_grad
         ctx.save_for_backward(geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c if need_tex else None, indices, uv_c, corner_c,
-                              cs_c, sp_c, lt_c, sh_c, nm_c, tg_c)
+                              cs_c, sp_c, lt_c, sh_c, nm_c, tg_c, sm_c)
         if cfg.aa:
             rgb_o, alpha_o, depth_o = out_rgb, out_alpha, out_depth
         else:
@@ -419,7 +450,7 @@ class _RasterizeFunction(torch.autograd.Function):
         lib = _lib.load()
         cfg = ctx.cfg
         flags = ctx.flags | (_lib.NR_GRAD_INTERIOR if ctx.interior else 0)
-        geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c, indices, uv_c, corner_c, cs_c, sp_c, lt_c, sh_c, nm_c, tg_c = \
+        geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c, indices, uv_c, corner_c, cs_c, sp_c, lt_c, sh_c, nm_c, tg_c, sm_c = \
             ctx.saved_tensors
         dev = geom_c.device
         B, F = geom_c.shape[0], ctx.F
@@ -449,6 +480,8 @@ class _RasterizeFunction(torch.autograd.Function):
             grad_nm = torch.empty_like(nm_c) if ctx.need_nm_grad else None
             grad_tg = torch.empty_like(tg_c) if ctx.need_tg_grad else None
             na = _normal_map_args(nm_c, tg_c, grad_nm, grad_tg) if nm_c is not None else None
+            grad_sm = torch.empty_like(sm_c) if ctx.need_sm_grad else None
+            qa = _specular_map_args(sm_c, grad_sm) if sm_c is not None else None
             ws_bytes = lib.nr_b200_backward_workspace_bytes(B, F, cfg.S, ctx.ts, flags)
             ws = torch.empty((max(ws_bytes, 16),), dtype=torch.uint8, device=dev)
             a = _lib.BackwardArgs()
@@ -471,6 +504,9 @@ class _RasterizeFunction(torch.autograd.Function):
             hook = _TEXTURE_GRAD_HOOK if (want_rgb and g_rgb is not None) else None
 
             def call():
+                if qa is not None:  # specular map: grad_specular_map is filled by the texture half too
+                    return lib.nr_b200_backward_specular_map(ctypes.byref(a), ctypes.byref(ph), _byref(la), _byref(sa),
+                                                             _byref(na), ctypes.byref(qa), _stream_ptr(dev))
                 if na is not None:  # normal map: grad_normal_map, grad_corner_tangents are filled by the texture half too
                     return lib.nr_b200_backward_normal_map(ctypes.byref(a), ctypes.byref(ph), _byref(la), _byref(sa),
                                                            ctypes.byref(na), _stream_ptr(dev))
@@ -495,7 +531,7 @@ class _RasterizeFunction(torch.autograd.Function):
                 if pending is not None:
                     pending.wait()
         return (grad_geom, grad_textures, grad_light, None, None, grad_uvs, grad_corner, grad_cs, grad_sp, grad_lt, grad_sh,
-                grad_nm, grad_tg)
+                grad_nm, grad_tg, grad_sm)
 
 
 def _byref(s):
@@ -548,6 +584,14 @@ def _normal_map_args(nm_c, tg_c, grad_nm=None, grad_tg=None):
     return na
 
 
+def _specular_map_args(sm_c, grad_sm=None):
+    qa = _lib.SpecularMapArgs()
+    qa.struct_size = ctypes.sizeof(_lib.SpecularMapArgs)
+    qa.map_batch, qa.map_height, qa.map_width = int(sm_c.shape[0]), int(sm_c.shape[1]), int(sm_c.shape[2])
+    qa.specular_map, qa.grad_specular_map = _ptr(sm_c), _ptr(grad_sm)
+    return qa
+
+
 class _MipPyramid(torch.autograd.Function):
     """image [Bt,Ht,Wt,3] -> packed mip pyramid [Bt,P,3] (nr_b200_mip_build); the backward collapses the pyramid gradient
     into the image gradient (nr_b200_mip_collapse, the exact transpose of the build)."""
@@ -583,7 +627,7 @@ TEXTURE_FILTERS = ('bilinear', 'trilinear')
 def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_color, return_rgb, return_alpha,
          return_depth, face_light=None, textures_fill_back=False, vertices=None, reference_exact=None, face_uvs=None,
          texture_filter='bilinear', corner_light=None, interior_gradient=False, corner_shading=None, shading_params=None,
-         lights=None, environment_sh=None, normal_map=None, corner_tangents=None):
+         lights=None, environment_sh=None, normal_map=None, corner_tangents=None, specular_map=None):
     if (corner_shading is not None or shading_params is not None) and interior_gradient:
         raise ValueError("interior_gradient=True is not supported with Phong shading (corner_shading / shading_params): no "
                          "vertex gradient flows through the interpolation of the per-pixel normal and position")
@@ -598,7 +642,7 @@ def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_
                          "than one item: the reference-exact sampler reads the depths of item 0 for every item, so its "
                          "derivative would cross items.  Pass reference_exact=False (or set_reference_exact(False))")
     _check_inputs(faces, textures, return_rgb, face_light, textures_fill_back, vertices, face_uvs, corner_light,
-                  corner_shading, shading_params, lights, environment_sh, normal_map, corner_tangents)
+                  corner_shading, shading_params, lights, environment_sh, normal_map, corner_tangents, specular_map)
     phong = corner_shading is not None
     indices = None
     if vertices is not None:
@@ -630,6 +674,8 @@ def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_
             if normal_map is not None:
                 normal_map = _batched(normal_map, batch_size, 3)
                 corner_tangents = _batched(corner_tangents, batch_size, 3)
+            if specular_map is not None:
+                specular_map = _batched(specular_map, batch_size, 3)
     cfg = _make_config(image_size, anti_aliasing, near, far, eps, background_color, return_rgb, return_alpha,
                        return_depth, geom.device, batch_size, reference_exact)
     if return_rgb and textures_fill_back:
@@ -647,7 +693,7 @@ def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_
                                     indices, face_uvs, corner_light, corner_shading if return_rgb else None,
                                     shading_params if return_rgb else None, lights if return_rgb else None,
                                     environment_sh if return_rgb else None, normal_map if return_rgb else None,
-                                    corner_tangents if return_rgb else None)
+                                    corner_tangents if return_rgb else None, specular_map if return_rgb else None)
 
 
 def rasterize_rgbad(
@@ -677,6 +723,7 @@ def rasterize_rgbad(
         environment_sh=None,
         normal_map=None,
         corner_tangents=None,
+        specular_map=None,
 ):
     """Generate RGB, alpha channel, and depth images from faces and textures (for RGB).  rasterize.py:900-977.
 
@@ -751,12 +798,22 @@ def rasterize_rgbad(
                               (include/nr_b200.h, nr_b200_normal_map_args), for every light and the environment.  Needs
                               corner_shading and a texture image with face_uvs; both receive gradients (a batch of 1
                               gets the sum over the items), and face_uvs receives the map's term too.
+      specular_map [Hq,Wq,4] / [1|B,Hq,Wq,4]   Phong shading through a specular map: per texel (ks_r, ks_g, ks_b,
+                              shininess) (F.specular_map packs them; row 0 = top), sampled bilinearly at the pixel's uv.
+                              Every highlight's colour is multiplied by ks and the map's shininess replaces
+                              shading_params' for shading_params' light and every light of `lights`; the diffuse terms
+                              do not change (include/nr_b200.h, nr_b200_specular_map_args).  A map (1, 1, 1, shininess)
+                              renders as no map.  Needs corner_shading and a texture image with face_uvs; composes with
+                              lights, environment_sh and normal_map.  It receives gradients (a batch of 1 gets the sum
+                              over the items; shading_params' shininess then gets none), and face_uvs receives the
+                              map's term too.
     `textures` with batch size 1 (or an expanded stride-0 batch) while the geometry batch is larger = one texture set
     shared by every item (a mesh seen from B viewpoints, mesh.py:29-34); its gradient is the sum over the items."""
     rgb, alpha, depth, _, _ = _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_color,
                                    return_rgb, return_alpha, return_depth, face_light, textures_fill_back, vertices,
                                    reference_exact, face_uvs, texture_filter, corner_light, interior_gradient,
-                                   corner_shading, shading_params, lights, environment_sh, normal_map, corner_tangents)
+                                   corner_shading, shading_params, lights, environment_sh, normal_map, corner_tangents,
+                                   specular_map)
     return {
         'rgb': rgb if return_rgb else None,
         'alpha': alpha if return_alpha else None,
@@ -788,6 +845,7 @@ def rasterize(
         environment_sh=None,
         normal_map=None,
         corner_tangents=None,
+        specular_map=None,
 ):
     """RGB images [B,3,H,W] from faces and textures.  rasterize.py:980-1008 (keyword-only extras: rasterize_rgbad; in
     texture-image mode both the image and face_uvs receive gradients)."""
@@ -796,7 +854,8 @@ def rasterize(
         face_light=face_light, textures_fill_back=textures_fill_back, vertices=vertices,
         reference_exact=reference_exact, face_uvs=face_uvs, texture_filter=texture_filter, corner_light=corner_light,
         interior_gradient=interior_gradient, corner_shading=corner_shading, shading_params=shading_params,
-        lights=lights, environment_sh=environment_sh, normal_map=normal_map, corner_tangents=corner_tangents)['rgb']
+        lights=lights, environment_sh=environment_sh, normal_map=normal_map, corner_tangents=corner_tangents,
+        specular_map=specular_map)['rgb']
 
 
 def rasterize_silhouettes(

@@ -46,6 +46,10 @@ class Renderer(object):
         # [1|B,Hm,Wm,3] (F.decode_normal_map), sampled at the same UVs; the tangents come from F.vertex_tangents of the
         # mesh.  It may require grad.  None = the interpolated normals alone
         self.normal_map = None
+        # specular map of shading='phong' with a texture image and face_uvs: per texel (ks_r, ks_g, ks_b, shininess)
+        # [Hq,Wq,4] / [1|B,Hq,Wq,4] (F.specular_map), sampled at the same UVs; ks multiplies every highlight and the
+        # shininess replaces light_shininess.  It may require grad.  None = light_color_specular and light_shininess alone
+        self.specular_map = None
 
         # rasterization
         self.rasterizer_eps = 1e-3
@@ -127,6 +131,11 @@ class Renderer(object):
                 raise ValueError("normal_map needs shading='phong', got shading=%r" % (self.shading,))
             if face_uvs is None:
                 raise ValueError("normal_map is addressed by the UVs: it needs a texture image and face_uvs")
+        if self.specular_map is not None:
+            if self.shading != 'phong':
+                raise ValueError("specular_map needs shading='phong', got shading=%r" % (self.shading,))
+            if face_uvs is None:
+                raise ValueError("specular_map is addressed by the UVs: it needs a texture image and face_uvs")
         fused = (self.fused and self._fusable(vertices, faces) and textures.is_cuda and textures.dtype == torch.float32)
         light_args = (self.light_intensity_ambient, self.light_intensity_directional, self.light_color_ambient,
                       self.light_color_directional, self.light_direction)
@@ -242,6 +251,9 @@ class Renderer(object):
         nm = self.normal_map
         if nm is not None:
             nm = nm.to(vertices.device)
+        sm = self.specular_map
+        if sm is not None:
+            sm = sm.to(vertices.device)
         if fused:
             indices = self._indices(faces)
             # one mesh seen from B viewpoints (an expanded, stride-0 vertex batch and a shared index set): one corner set
@@ -264,7 +276,7 @@ class Renderer(object):
                 self.background_color, textures_fill_back=self.fill_back, vertices=self._transform(vertices),
                 reference_exact=self.reference_exact, face_uvs=face_uvs, texture_filter=texture_filter,
                 corner_shading=cs, shading_params=params, lights=lights, environment_sh=sh, normal_map=nm,
-                corner_tangents=ct)
+                corner_tangents=ct, specular_map=sm)
         # op by op: torch normals and corners, materialised faces, doubled textures / UV corners for fill_back
         normals = F._vertex_normals_torch(vertices, faces)
         vt = F.vertex_tangents(vertices, faces, face_uvs, normals) if nm is not None else None
@@ -281,4 +293,4 @@ class Renderer(object):
             faces, textures, self.image_size, self.anti_aliasing, self.near, self.far, self.rasterizer_eps,
             self.background_color, reference_exact=self.reference_exact, face_uvs=face_uvs,
             texture_filter=texture_filter, corner_shading=cs, shading_params=params, lights=lights, environment_sh=sh,
-            normal_map=nm, corner_tangents=ct)
+            normal_map=nm, corner_tangents=ct, specular_map=sm)
