@@ -5,7 +5,7 @@ nr_b200_interpolate_backward (test infrastructure).
 `cases()` returns the case list of tests/test_gpu_abi_matrix.py: the full product of texture kind x fill_back x
 anti-aliasing x backward mode, with every other dimension filled in greedily so that every compatible pair of levels of
 any two dimensions appears in at least one case; rows are added until no pair is missing.  No randomness: the same list
-on every machine.  The cases are generated in three frozen stages, each one exactly as it was when the next joined, so
+on every machine.  The cases are generated in frozen stages, each one exactly as it was when the next joined, so
 the ids, inputs and oracle of every earlier case stay the same: the matrix as it stood before smooth shading, the
 face_uvs gradient, texture staging, the short layouts and interpolation joined it (BASE); then the rows and pairs of
 those levels, with the interior vertex gradient off (FROZEN); then the interior rows and the pairs of every level.
@@ -24,7 +24,17 @@ stage.  Their dimensions -- the batch of each shading input (Bc, Bp, Bl, Bs: one
 item), the light count NL, the entry point and the shininess -- mean something only under a Phong level and are None
 elsewhere, so the cases of the earlier stages keep every level they had.  Attribute interpolation reads only the maps,
 which shading leaves as they are, so it is None under a Phong level.  Phong needs RGB and refuses the interior
-gradient; NL = 0 (SH without a light set) exists only with the SH environment, and a set of NL = 0 lights has no batch."""
+gradient; NL = 0 (SH without a light set) exists only with the SH environment, and a set of NL = 0 lights has no batch.
+
+The normal map and the specular map (nr_b200_*_normal_map / nr_b200_*_specular_map) joined as a fifth stage, after the
+271 cases of the first four, which are generated exactly as they were with `maps` held "off" and `map_entry` "direct".
+`maps` (off, nm, sm, nm_sm) and `map_entry` mean something under a Phong level on a texture image (the maps are addressed
+by the image's UVs): "direct" is the narrowest entry point that takes the structs given (without a map, the call the
+`entry` dimension chooses), "via_nm" nr_b200_*_normal_map with a NULL map struct, "via_sm" nr_b200_*_specular_map with
+NULL for each absent map.  The batches Bm, Bt (with a normal map) and Bq (with a specular map) and `map_grads` -- which
+of grad_normal_map / grad_corner_tangents / grad_specular_map are wanted: all, the texels only, the tangents only, none
+-- are None elsewhere.  `map_grads` is independent of `optional`, which keeps governing the Phong shading gradients, and
+of `uv_grad`: with both of the others off, grad_face_uvs receives the maps' UV term from a kernel that runs for it alone."""
 import itertools
 
 DIMS = [
@@ -59,6 +69,14 @@ DIMS = [
     ("lights_batch", ["shared", "item"]),
     ("sh_batch", ["shared", "item"]),
     ("sigma", [1.0, 16.0]),
+    # the normal map and the specular map (abi_harness.Plan): which maps the call carries, the entry point they travel
+    # through, Bm, Bt, Bq ("shared" = 1, "item" = B) and which of the maps' gradient outputs are wanted
+    ("maps", ["off", "nm", "sm", "nm_sm"]),
+    ("map_entry", ["direct", "via_nm", "via_sm"]),
+    ("nm_batch", ["shared", "item"]),
+    ("tg_batch", ["shared", "item"]),
+    ("sm_batch", ["shared", "item"]),
+    ("map_grads", ["all", "texels", "tangents", "null"]),
 ]
 NAMES = [n for n, _ in DIMS]
 LEVELS = dict(DIMS)
@@ -67,12 +85,17 @@ LEVELS = dict(DIMS)
 PHONG = ("phong", "phong_set", "phong_sh")
 PHONG_DIMS = ["nl", "entry", "shading_batch", "params_batch", "lights_batch", "sh_batch", "sigma"]
 OLD_LIGHTS = ["none", "face", "corner"]
+MAP_DIMS = ["maps", "map_entry", "nm_batch", "tg_batch", "sm_batch", "map_grads"]
 
 
 def active(dim, c):
     """whether `dim` means anything for the case (or partial case) `c`: its texture kind, and for the Phong dimensions
     its light and light count"""
     kind, light = c["kind"], c.get("light")
+    if dim in MAP_DIMS:  # the maps are addressed by the UVs of a texture image
+        maps = c.get("maps")
+        return light in PHONG and kind in ("uv", "mip") and (
+            dim in ("maps", "map_entry") or maps in {"sm_batch": ("sm", "nm_sm"), "map_grads": ("nm", "sm", "nm_sm")}.get(dim, ("nm", "nm_sm")))
     if dim in ("shading_batch", "params_batch", "sigma"):
         return light in PHONG
     if dim == "entry":  # nr_b200_*_sh is the SH mode's own entry point
@@ -117,6 +140,13 @@ def compatible(a):
         return False  # NL = 0 is SH without a set: the set modes have lights, and no set has no batch
     if a.get("entry") == "via_lights_nl0" and light not in (None, "phong"):
         return False  # an empty light set is the plain Phong call
+    maps, via = a.get("maps"), a.get("map_entry")
+    if via == "via_nm" and maps not in (None, "off"):
+        return False  # nr_b200_*_normal_map is the direct call of a normal map, and takes no specular map
+    if via == "via_sm" and maps in ("sm", "nm_sm"):
+        return False  # nr_b200_*_specular_map is the direct call of a specular map
+    if a.get("map_grads") == "tangents" and maps == "sm":
+        return False  # grad_corner_tangents belongs to the normal map's struct
     return True
 
 
@@ -124,12 +154,16 @@ def _context(a):
     """the first completion of partial assignment `a` by a texture kind (and, for a Phong dimension, a light and NL)
     under which each of its dimensions means something and the rules hold, or None"""
     kinds = [a["kind"]] if "kind" in a else LEVELS["kind"]
-    lights, nls = [None], [None]
-    if any(d in PHONG_DIMS for d in a):
+    lights, nls, mapses = [None], [None], [None]
+    if any(d in PHONG_DIMS or d in MAP_DIMS for d in a):
         lights = [a["light"]] if "light" in a else list(PHONG)
+    if any(d in PHONG_DIMS for d in a):
         nls = [a["nl"]] if "nl" in a else [None] + LEVELS["nl"]
-    for k, lt, nl in itertools.product(kinds, lights, nls):
-        c = {**a, "kind": k, **({"light": lt} if lt is not None else {}), **({"nl": nl} if nl is not None else {})}
+    if any(d in MAP_DIMS[2:] for d in a):
+        mapses = [a["maps"]] if "maps" in a else LEVELS["maps"]
+    for k, lt, nl, mp in itertools.product(kinds, lights, nls, mapses):
+        c = {**a, "kind": k, **({"light": lt} if lt is not None else {}), **({"nl": nl} if nl is not None else {}),
+             **({"maps": mp} if mp is not None else {})}
         if all(active(d, c) for d in a if d != "kind") and compatible(c):
             return c
     return None
@@ -230,10 +264,10 @@ MUST_NEW += [{"kind": "cube", "stage": True, "_aa": False, "pointers": "fresh", 
 # the matrix as it stood before the interior vertex gradient joined it: every level but that flag, held off (and
 # without the Phong modes)
 FROZEN = {**LEVELS, "light": OLD_LIGHTS, "interior": ["off"]}
-FROZEN_PAIRS = {n: FROZEN[n] for n in NAMES if n != "interior" and n not in PHONG_DIMS}
+FROZEN_PAIRS = {n: FROZEN[n] for n in NAMES if n != "interior" and n not in PHONG_DIMS + MAP_DIMS}
 # the matrix as it stood before the Phong modes joined it
 INTERIOR = {**LEVELS, "light": OLD_LIGHTS}
-INTERIOR_PAIRS = {n: INTERIOR[n] for n in NAMES if n not in PHONG_DIMS}
+INTERIOR_PAIRS = {n: INTERIOR[n] for n in NAMES if n not in PHONG_DIMS + MAP_DIMS}
 
 # the interior vertex gradient (NR_GRAD_INTERIOR) with an rgb upstream gradient, for every texture kind: every light, a
 # fresh and an accumulating backward, one call and two halves, with and without fill_back and anti-aliasing, spread over
@@ -304,6 +338,81 @@ MUST_PHONG += [{"kind": "uv", "light": "phong", "batch": "B3", "image": "shared"
                 "optional": "given", "upstream": "all"},
                {"kind": "cube_shared", "light": "phong_sh", "nl": 3, "batch": "B3", "optional": "given",
                 "upstream": "only_rgb"}]
+# the matrix as it stood before the normal map and the specular map joined it: no map, through the entry point the
+# `entry` dimension chooses
+NO_MAPS = {**LEVELS, "maps": ["off"], "map_entry": ["direct"]}
+NO_MAPS_PAIRS = {n: LEVELS[n] for n in NAMES if n not in MAP_DIMS}
+
+# The maps (light modes 6 and 7: nr_b200_*_normal_map / nr_b200_*_specular_map), every gradient given with an rgb upstream
+# gradient.  Each of the 48 instantiations k_phong_grad<kTex, kIdx, kLights, kSH, kNM, kSM> (nr_phong.cu) with kNM || kSM
+# once: nm, sm and both x bilinear and trilinear albedo x per-face and indexed geometry x Phong alone, a light set, SH
+# without a set and SH with one -- for sm alone these are also the four targets of the texture gradient's re-mapping of
+# mode 7 (nr_backward.cu, tg_light), for both samplers.  The eight rows of a (maps, sampler) take the eight entries of
+# MAP_ROWS, from a start that moves on, so each has a fresh and an accumulating backward, one call and two halves in both
+# orders, with and without fill_back and anti-aliasing.  The rows' pointer levels walk fresh / 4 / 8 bytes in, and the
+# map sizes follow the case id (abi_harness.Plan), so that grad_normal_map sits 0, 4 and 8 bytes and grad_specular_map
+# 0, 4, 8 and 12 bytes past a 16-byte boundary, each with a one-texel-wide and a wider map (tests/test_abi_cases_cpu.py).
+MAP_ROWS = [(False, False, "one"), (True, True, "acc_halves"), (True, False, "faces_tex"), (False, True, "acc_one"),
+            (False, True, "tex_faces"), (True, False, "acc_one"), (False, False, "acc_halves"), (True, True, "one")]
+MAP_VARIANTS = [("phong", {}), ("phong_set", {"nl": 3}), ("phong_sh", {"nl": 0}), ("phong_sh", {"nl": 1})]
+_ALL = {"optional": "given", "map_grads": "all", "upstream": "all"}
+MUST_MAPS = []
+for _s, (_maps, _kind) in enumerate(itertools.product(("nm", "sm", "nm_sm"), ("uv", "mip"))):
+    for _i, (_geom, (_mode, _nl)) in enumerate(itertools.product((False, True), MAP_VARIANTS)):
+        _fb, _aa, _bwd = MAP_ROWS[(_i + 3 * _s) % 8]
+        _j = len(MUST_MAPS)
+        MUST_MAPS.append({"kind": _kind, "light": _mode, **_nl, "maps": _maps, "map_entry": "direct", "fill_back": _fb,
+                          "_aa": _aa, "backward": _bwd, "uv_grad": "given",
+                          "geometry": ("idx_item", "idx_shared")[_j % 2] if _geom else "faces",
+                          "pointers": ("fresh", "off4", "off8")[_j % 3], **_ALL,
+                          "upstream": ("all", "only_rgb")[_i % 2]})
+# the full set of 8 lights (s_lt[8][80], the highest register use) with both maps, once per sampler
+MUST_MAPS += [{"kind": kind, "light": mode, "nl": 8, "maps": "nm_sm", "uv_grad": "given", **_ALL}
+              for kind, mode in (("uv", "phong_set"), ("mip", "phong_sh"))]
+# the maps' UV term alone: grad_face_uvs wanted and every shading and map gradient NULL (k_phong_grad then runs for that
+# term only), for both samplers; then the reverse, the maps' texels wanted and neither grad_face_uvs nor a shading gradient;
+# and grad_corner_tangents alone (a branch of its own in the run reduction)
+MUST_MAPS += [{"kind": kind, "light": mode, **nl, "maps": maps, "optional": "null", "map_grads": "null", "uv_grad": "given",
+               "upstream": "all"}
+              for kind in ("uv", "mip") for maps, mode, nl in (("nm", "phong", {}), ("sm", "phong_set", {"nl": 3}),
+                                                               ("nm_sm", "phong_sh", {"nl": 1}))]
+MUST_MAPS += [{"kind": kind, "light": "phong_set", "nl": 1, "maps": maps, "optional": "null", "map_grads": "texels",
+               "uv_grad": "null", "upstream": "all"}
+              for kind, maps in (("uv", "nm"), ("mip", "sm"), ("uv", "nm_sm"))]
+MUST_MAPS += [{"kind": "mip", "light": "phong", "maps": "nm", "optional": "null", "map_grads": "tangents", "uv_grad": "given",
+               "upstream": "all"}]
+# shared UVs at three items with fill_back (the maps' UV term summed over the items, the copies' corners reversed: `rev`
+# in nm_grad_tail / sm_grad_tail), with a shared and with a per-item image
+MUST_MAPS += [{"kind": kind, "light": "phong_set", "nl": 3, "maps": maps, "batch": "B3", "uvs": "shared", "image": image,
+               "fill_back": True, "uv_grad": "given", **_ALL}
+              for kind, maps, image in (("uv", "nm", "shared"), ("mip", "sm", "item"))]
+# Bm = Bt = Bq = 1 next to Bc = Bp = Bl = Bs = B at three items, the reverse, all of them 1 and all of them B
+MUST_MAPS += [{"kind": kind, "light": "phong_sh", "nl": 3, "maps": "nm_sm", "batch": "B3", "uv_grad": "given", **_ALL,
+               **{d: m for d in ("nm_batch", "tg_batch", "sm_batch")},
+               **{d: o for d in ("shading_batch", "params_batch", "lights_batch", "sh_batch")}}
+              for kind, m, o in (("uv", "shared", "item"), ("mip", "item", "shared"), ("mip", "shared", "shared"),
+                                 ("uv", "item", "item"))]
+# the short layouts: the NaN buffer behind the field past the short backward struct is where the maps' UV term would land
+MUST_MAPS += [{"kind": kind, "light": mode, **nl, "maps": maps, "layout": "short", **_ALL}
+              for kind, maps, mode, nl in (("uv", "nm", "phong", {}), ("mip", "sm", "phong_set", {"nl": 3}),
+                                           ("uv", "nm_sm", "phong_sh", {"nl": 1}))]
+# every gradient given without an rgb upstream gradient: fresh ones come back 0, accumulated ones keep their prefill
+MUST_MAPS += [{"kind": kind, "light": "phong_set", "nl": 3, "maps": "nm_sm", "upstream": "no_rgb", "outputs": "rad",
+               "optional": "given", "map_grads": "all", "uv_grad": "given", "backward": bwd}
+              for kind, bwd in (("uv", "one"), ("mip", "acc_one"))]
+# NR_TEX_Z_BATCH0 at three items on per-item index sets: images ignore the flag, and the maps must too
+MUST_MAPS += [{"kind": "uv", "light": "phong_set", "nl": 1, "maps": "nm_sm", "z_batch0": True, "batch": "B3",
+               "geometry": "idx_item", "uv_grad": "given", **_ALL}]
+# no map through the map entry points (a NULL nm; a NULL nm and a NULL sm) under every earlier mode, and a normal map
+# through nr_b200_*_specular_map with a NULL sm
+MUST_MAPS += [{"kind": kind, "light": mode, **nl, "maps": "off", "map_entry": via, "optional": "given", "upstream": "all",
+               "uv_grad": "given"}
+              for via, kind in (("via_nm", "uv"), ("via_sm", "mip"))
+              for mode, nl in (("phong", {}), ("phong_set", {"nl": 3}), ("phong_sh", {"nl": 3}))]
+MUST_MAPS += [{"kind": "uv", "light": "phong_sh", "nl": 0, "maps": "nm", "map_entry": "via_sm", "uv_grad": "given", **_ALL}]
+# out-of-range indices (faces that never win a pixel) with both maps
+MUST_MAPS += [{"kind": "mip", "light": "phong_set", "nl": 3, "maps": "nm_sm", "geometry": "idx_shared_oor", "uv_grad": "given",
+               **_ALL}]
 
 
 def _complete(out, covered, choices, pairs):
@@ -346,8 +455,14 @@ def cases():
         covered |= pairs_of(c)
         out.append(c)
     _complete(out, covered, INTERIOR, required_pairs(INTERIOR_PAIRS))
-    # then the Phong rows and the pairs of every level
+    # then the Phong rows and the pairs of every level but the maps
     for seed in MUST_PHONG:
+        c = _fill(dict(seed), covered, len(out), NO_MAPS)
+        covered |= pairs_of(c)
+        out.append(c)
+    _complete(out, covered, NO_MAPS, required_pairs(NO_MAPS_PAIRS))
+    # then the map rows and the pairs of every level
+    for seed in MUST_MAPS:
         c = _fill(dict(seed), covered, len(out))
         covered |= pairs_of(c)
         out.append(c)
@@ -376,4 +491,8 @@ def _light_id(c):
     parts += [c["entry"].replace("own", "") if c["entry"] else "", "s%g" % c["sigma"]]
     parts += [n + c[d][0] for n, d in (("Bc", "shading_batch"), ("Bp", "params_batch"), ("Bl", "lights_batch"),
                                        ("Bs", "sh_batch")) if c[d]]
+    if c["maps"] not in (None, "off") or c["map_entry"] not in (None, "direct"):  # earlier ids keep their names
+        parts += [c["maps"], c["map_entry"].replace("direct", "")]  # "off" here is a NULL map struct
+        parts += [n + c[d][0] for n, d in (("Bm", "nm_batch"), ("Bt", "tg_batch"), ("Bq", "sm_batch")) if c[d]]
+        parts += ["mg-" + c["map_grads"]] if c["map_grads"] else []
     return "-".join(p for p in parts if p)

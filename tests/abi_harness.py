@@ -1,5 +1,6 @@
 """Direct C-ABI harness for nr_b200_forward, nr_b200_backward / nr_b200_backward_corner_light, the Phong entry points
-nr_b200_{forward,backward}_{phong,lights,sh} and nr_b200_interpolate / nr_b200_interpolate_backward (test infrastructure).
+nr_b200_{forward,backward}_{phong,lights,sh,normal_map,specular_map} and nr_b200_interpolate /
+nr_b200_interpolate_backward (test infrastructure).
 
 It fills _lib.ForwardArgs / BackwardArgs / InterpolateArgs itself -- no Python wrapper in between -- from a case of
 abi_cases.py, so that each case controls the exact flag word, the struct size (the full layouts, or the short ones that
@@ -7,7 +8,9 @@ end before corner_light / grad_face_uvs), which optional pointers are NULL, wher
 bytes into a slightly larger allocation; grad_textures, grad_face_uvs and grad_corner_light also 8 bytes in: 2-float but
 not 4-float aligned) and what every output buffer holds before the call: NaN in each float output and a sentinel in
 face_index_map, so an element the kernels fail to write shows, or seeded values for NR_GRAD_ACCUMULATE.  The Phong
-inputs (corner_shading, params, lights, sh) and their gradients are user buffers like every other.  Guard words
+inputs (corner_shading, params, lights, sh), the maps (normal_map, corner_tangents, specular_map) and their gradients
+are user buffers like every other; grad_normal_map and grad_corner_tangents also sit 8 bytes in, grad_specular_map 8 or
+12 (its 4-float reduction splits by phase), and specular_map itself always on a 16-byte boundary, as the ABI demands.  Guard words
 around every buffer show a store just outside it.  With a short layout the field just past struct_size points at a real,
 NaN-filled, guarded buffer: the forward would light the image with NaN if it read it, and the backward must leave it
 as it was, bit for bit.
@@ -29,6 +32,9 @@ F_FRONT = {False: 201, True: 101}  # front faces; fill_back appends the reversed
 UV_SIZES = [(17, 41), (32, 32), (9, 30), (1, 9), (24, 13)]
 MIP_SIZES = [(37, 29), (64, 48), (17, 41), (1, 9)]
 ATTR_CHANNELS = [1, 3, 4, 16]
+# normal-map and specular-map sizes (H, W): one texel, one row, one column (the clamped x1 == x0 of every pixel), odd, even
+MAP_SIZES = [(1, 1), (1, 23), (19, 1), (37, 53), (16, 16), (9, 11)]
+MAP_GRADS = ("grad_normal_map", "grad_corner_tangents", "grad_specular_map")
 K_STAGE_BYTES = 32 * 1024  # shared memory of a staged k_resolve CTA (csrc/nr_forward.cu kStageBytes)
 
 
@@ -87,6 +93,14 @@ class Plan:
         self.Bl = per("lights_batch") if self.NL else 0
         self.Bs = per("sh_batch") if self.sh else 0
         self.sigma = c["sigma"]
+        # the maps: which of them the call carries, the entry point, the batch of each (1 or B), and their sizes, which
+        # rotate with the case id independently of each other (and of the albedo's)
+        self.nm, self.sm = c["maps"] in ("nm", "nm_sm"), c["maps"] in ("sm", "nm_sm")
+        self.map_entry = c["map_entry"] or "direct"
+        self.Bm, self.Bt = (per("nm_batch"), per("tg_batch")) if self.nm else (0, 0)
+        self.Bq = per("sm_batch") if self.sm else 0
+        self.Hm, self.Wm = MAP_SIZES[c["id"] % 6] if self.nm else (0, 0)
+        self.Hq, self.Wq = MAP_SIZES[c["id"] // 2 % 6] if self.sm else (0, 0)
         f = 0
         f |= L.NR_RETURN_RGB if self.rgb else 0
         f |= L.NR_RETURN_ALPHA if self.alpha else 0
@@ -149,6 +163,11 @@ class Plan:
                     bufs["lights"] = ((self.Bl, self.NL, 12), f32)
                 if self.sh:
                     bufs["sh"] = ((self.Bs, 9, 3), f32)
+            if self.nm:
+                bufs["normal_map"] = ((self.Bm, self.Hm, self.Wm, 3), f32)
+                bufs["corner_tangents"] = ((self.Bt, F, 3, 4), f32)
+            if self.sm:
+                bufs["specular_map"] = ((self.Bq, self.Hq, self.Wq, 4), f32)
         if self.short:  # what the fields past the short layouts point at: never to be read
             bufs["past_end_fwd"] = ((B, F, 3, 3), f32)
             bufs["past_end_bwd"] = ((uv_shape if self.uv else (B, F, 3, 2)), f32)
@@ -190,6 +209,11 @@ class Plan:
                 for k in ("corner_shading", "params", "lights", "sh"):
                     if k in bufs:
                         bufs["grad_" + k] = (bufs[k][0], f32)
+            wanted = {"all": ("normal_map", "corner_tangents", "specular_map"), "texels": ("normal_map", "specular_map"),
+                      "tangents": ("corner_tangents",)}.get(c["map_grads"], ())
+            for k in wanted:
+                if k in bufs:
+                    bufs["grad_" + k] = (bufs[k][0], f32)
         if self.attr:  # attribute interpolation on the forward's maps, with gradient buffers of its own
             C, Ba = self.C, (1 if self.attr_shared else B)
             bufs["attributes"] = (((Ba, Nv, C) if self.attr_pv else (Ba, F, 3, C)), f32)
@@ -202,19 +226,25 @@ class Plan:
         self.bufs = bufs
         # textures may be NULL in the backward unless a gradient that reads them is wanted (the interior gradient reads
         # the sampler's derivative from them, the Phong gradients the unlit sample)
-        self.bwd_textures = self.rgb and (self.given or self.uv_grad or "grad_face_light" in bufs or self.interior)
+        self.bwd_textures = self.rgb and (self.given or self.uv_grad or "grad_face_light" in bufs or self.interior
+                                          or any(k in bufs for k in MAP_GRADS))
         p = c["pointers"]
         self.offsets = {k: (0 if p == "fresh" else 4) for k in bufs}
         if p == "off8":
-            for k in ("grad_textures", "grad_face_uvs", "grad_corner_light"):
+            for k in ("grad_textures", "grad_face_uvs", "grad_corner_light", "grad_normal_map", "grad_corner_tangents",
+                      "grad_specular_map"):
                 if k in bufs:
                     self.offsets[k] = 8
+            if "grad_specular_map" in bufs and c["id"] % 2:  # red_add_4 splits by phase: 12 bytes in on odd ids
+                self.offsets["grad_specular_map"] = 12
+        if self.sm:
+            self.offsets["specular_map"] = 0  # read as 16-byte vectors: the ABI demands the alignment
         self.fwd_outputs = [k for k in ("face_index_map", "weight_map", "depth_map", "rgb_map", "alpha_map", "out_rgb",
                                         "out_alpha", "out_depth") if k in bufs]
         self.grad_outputs = [k for k in ("grad_faces", "grad_vertices", "grad_textures", "grad_face_light",
                                          "grad_corner_light", "grad_face_uvs", "grad_corner_shading", "grad_params",
                                          "grad_lights", "grad_sh", "attr_grad_attributes", "attr_grad_faces",
-                                         "attr_grad_vertices") if k in bufs]
+                                         "attr_grad_vertices") + MAP_GRADS if k in bufs]
 
     # ---- the argument structs, from name -> address (int) of each buffer the case passes
     def forward_args(self, ptr, workspace, workspace_bytes):
@@ -278,9 +308,38 @@ class Plan:
             sa.sh_batch, sa.sh, sa.grad_sh = self.Bs, ptr.get("sh"), g("sh")
         return ph, la, sa
 
+    def normal_map_args(self, ptr, backward):
+        """NormalMapArgs of a case with a normal map, else None (a NULL struct); the gradient pointers only in the
+        backward"""
+        if not self.nm:
+            return None
+        L = _lib()
+        na = L.NormalMapArgs()
+        na.struct_size = ctypes.sizeof(L.NormalMapArgs)
+        na.map_batch, na.tangent_batch, na.map_height, na.map_width = self.Bm, self.Bt, self.Hm, self.Wm
+        na.normal_map, na.corner_tangents = ptr.get("normal_map"), ptr.get("corner_tangents")
+        if backward:
+            na.grad_normal_map, na.grad_corner_tangents = ptr.get("grad_normal_map"), ptr.get("grad_corner_tangents")
+        return na
+
+    def specular_map_args(self, ptr, backward):
+        """SpecularMapArgs of a case with a specular map, else None (a NULL struct)"""
+        if not self.sm:
+            return None
+        L = _lib()
+        qa = L.SpecularMapArgs()
+        qa.struct_size = ctypes.sizeof(L.SpecularMapArgs)
+        qa.map_batch, qa.map_height, qa.map_width = self.Bq, self.Hq, self.Wq
+        qa.specular_map = ptr.get("specular_map")
+        if backward:
+            qa.grad_specular_map = ptr.get("grad_specular_map")
+        return qa
+
     def _call(self, lib, a, ptr, stream, backward):
         """the case's entry point: nr_b200_{forward,backward}_{phong,lights,sh} for the Phong modes (or _sh with NULL
-        structs, or _lights with an empty set), else nr_b200_forward / nr_b200_backward[_corner_light]"""
+        structs, or _lights with an empty set), or with a map (or map_entry "via_nm" / "via_sm" without one: NULL map
+        structs) nr_b200_*_normal_map / nr_b200_*_specular_map, the narrowest that takes the structs given unless
+        map_entry says otherwise; else nr_b200_forward / nr_b200_backward[_corner_light]"""
         part = "backward" if backward else "forward"
         if not self.phong:
             if backward and self.corner:
@@ -289,6 +348,13 @@ class Plan:
             return getattr(lib, "nr_b200_" + part)(ctypes.byref(a), stream)
         ph, la, sa = self.shading_args(ptr, backward)
         ref = lambda s: None if s is None else ctypes.byref(s)
+        if self.nm or self.sm or self.map_entry != "direct":
+            na, qa = self.normal_map_args(ptr, backward), self.specular_map_args(ptr, backward)
+            if self.sm or self.map_entry == "via_sm":
+                return getattr(lib, "nr_b200_%s_specular_map" % part)(ctypes.byref(a), ctypes.byref(ph), ref(la), ref(sa),
+                                                                      ref(na), ref(qa), stream)
+            return getattr(lib, "nr_b200_%s_normal_map" % part)(ctypes.byref(a), ctypes.byref(ph), ref(la), ref(sa),
+                                                                ref(na), stream)
         if self.entry == "via_sh" or self.sh:
             return getattr(lib, "nr_b200_%s_sh" % part)(ctypes.byref(a), ctypes.byref(ph), ref(la), ref(sa), stream)
         if la is not None:  # a light set, or the empty one of "via_lights_nl0"
@@ -402,6 +468,8 @@ def make_inputs(plan, seed):
             d[k] = np.full(plan.bufs[k][0], np.nan, np.float32)
     if plan.phong:
         phong_inputs(plan, d, np.random.default_rng(3000 + seed))
+    if plan.nm or plan.sm:
+        map_inputs(plan, d, np.random.default_rng(7000 + seed))
     return d
 
 
@@ -444,6 +512,44 @@ def phong_inputs(plan, d, rng):
         base = 0.25 * rng.standard_normal((9, 3))
         base[0] = np.array([0.8, 0.7, 0.6]) / C0
         d["sh"] = np.stack([base + 0.05 * b for b in range(plan.Bs)]).astype(np.float32)
+
+
+def map_inputs(plan, d, rng):
+    """the map inputs of a case (from a generator of their own, so the other inputs keep their bits): normal_map
+    [Bm,Hm,Wm,3] -- decoded unit vectors tilted up to 30 degrees from +z, every item its own --, corner_tangents
+    [Bt,F,3,4] -- across the corner normals, two faces in five with handedness -1 and one in seven with mixed signs over
+    its corners (the majority vote decides), the fill_back copies (-T, -w) at their reversed corners --, and specular_map
+    [Bq,Hq,Wq,4] -- ks in [0.2, 1], shininess in [4, 24]; with fill_back every other copy then takes its normal back to
+    the viewer's side.  With a specular map params' shininess is NaN: the header pins
+    that a pixel shaded through the map never reads it, and a read would show in the image and in every gradient."""
+    Ff = plan.F_front
+    if plan.nm:
+        shape = (plan.Bm, plan.Hm, plan.Wm)
+        tilt, turn = np.radians(30.0) * np.sqrt(rng.random(shape)), 2 * np.pi * rng.random(shape)
+        m = np.stack((np.sin(tilt) * np.cos(turn), np.sin(tilt) * np.sin(turn), np.cos(tilt)), axis=-1)
+        d["normal_map"] = np.ascontiguousarray(m, np.float32)
+        n = d["corner_shading"][..., :3].astype(np.float64)
+        n = n[[min(b, n.shape[0] - 1) for b in range(plan.Bt)], :Ff]
+        t = np.cross(n, np.array([0.3, 1.0, 0.2]) + 0.2 * rng.standard_normal(n.shape))
+        t = t / np.linalg.norm(t, axis=-1, keepdims=True) + 0.1 * rng.standard_normal(n.shape)
+        w = np.where(rng.random((plan.Bt, Ff, 1)) < 0.4, -1.0, 1.0) * np.ones((1, 1, 3))
+        mixed = rng.random((plan.Bt, Ff)) < 1 / 7
+        corner = rng.integers(0, 3, (plan.Bt, Ff))
+        w[mixed, corner[mixed]] *= -1.0
+        tg = np.concatenate((t, w[..., None]), axis=-1)
+        if plan.fill_back:
+            tg = np.concatenate((tg, -tg[:, :, ::-1]), axis=1)
+        d["corner_tangents"] = np.ascontiguousarray(tg, np.float32)
+    if plan.sm:
+        shape = (plan.Bq, plan.Hq, plan.Wq)
+        q = np.concatenate((0.2 + 0.8 * rng.random(shape + (3,)), 4.0 + 20.0 * rng.random(shape + (1,))), axis=-1)
+        d["specular_map"] = np.ascontiguousarray(q, np.float32)
+        d["params"][:, 12] = np.nan
+        if plan.fill_back:
+            # a copy's negated normal faces away from the viewer and the lights, so no copy would carry a highlight and
+            # the specular map's gradient and UV term would be 0 on every copy's pixel (`rev` in sm_grad_tail unseen):
+            # every other copy keeps its front face's side, as a two-sided material would
+            d["corner_shading"][:, Ff::2, :, :3] *= -1.0
 
 
 def stage_runs(plan):

