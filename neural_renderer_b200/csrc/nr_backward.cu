@@ -1028,7 +1028,7 @@ __global__ void __launch_bounds__(256, kTgCombine ? (kLight >= nr::kLightCorner 
                 for (int k = 0; k < 3; k++) oz[k] = __ldg(nr::face_vertex(p.src, b, fn, k) + 2);
             }
             nr::perspective_weights(w, zp, oz[0], oz[1], oz[2], lam);
-            nr::pixel_light<kLight>(p.shading, b, p.F, fn, lam, L);
+            nr::pixel_light<kLight>(p.shading, b, p.F, fn, lam, 0.0f, 0.0f, L);  // no uv: the cube modes have no map
         }
         // NR_TEX_FILL_BACK: the reversed copy of face f - F/2 shares that face's cube, axes reversed
         int cube = fn, ncubes = p.F;
@@ -1230,8 +1230,7 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
         float lam[3] = {0.0f, 0.0f, 0.0f}, L[3];  // kCorner / kPhong: perspective weights and light of the pixel
         if constexpr (kCorner || kPhong) {
             nr::perspective_weights(w, zp, z0, z1, z2, lam);
-            if constexpr (kLight == nr::kLightPhongNM) nr::pixel_light_nm(p.shading, b, fn, lam, u, v, L);  // the map at uv
-            else nr::pixel_light<kLight>(p.shading, b, p.F, fn, lam, L);
+            nr::pixel_light<kLight>(p.shading, b, p.F, fn, lam, u, v, L);
         }
         const uint32_t img_off = (uint32_t)b * p.img_bstride;
         // level(s) and their weights: the bilinear variant is level 0 of an image with weight 1
@@ -1567,12 +1566,10 @@ extern "C" size_t nr_b200_backward_workspace_bytes(int32_t B, int32_t F, int32_t
     return bin_layout(B, F, S, strip_rec_bytes(S, both)).total;
 }
 
-// nr_b200_backward (corner_light, phong, lights, sh, nm, sm NULL), nr_b200_backward_corner_light (smooth shading),
-// nr_b200_backward_phong (lights, sh, nm, sm NULL), nr_b200_backward_lights (sh, nm, sm NULL), nr_b200_backward_sh (nm, sm
-// NULL), nr_b200_backward_normal_map (sm NULL) and nr_b200_backward_specular_map
+// nr_b200_backward (no corner_light, no Phong inputs), nr_b200_backward_corner_light (smooth shading) and the five Phong
+// entry points
 static int backward_impl(const nr_b200_backward_args* args, const float* corner_light, float* grad_corner_light,
-                         const nr_b200_phong_args* phong, const nr_b200_lights_args* lights, const nr_b200_sh_args* sh,
-                         const nr_b200_normal_map_args* nm, const nr_b200_specular_map_args* sm, void* cuda_stream) {
+                         const nr_internal::PhongCall& pc, void* cuda_stream) {
     nr_internal::launch_count() = 0;
     // Two layouts: the full struct, and the ABI-4 struct from before grad_face_uvs (which then reads as NULL).  Only the
     // caller's struct_size bytes are read.
@@ -1610,24 +1607,32 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
     if (rgb && (flags & NR_TEX_FILL_BACK) && (F & 1)) return NR_ERR_INVALID_ARG;
     if (rgb && a->grad_face_light && !a->textures) return NR_ERR_INVALID_ARG;
     nr::Shading shading;
-    const int light = nr_internal::make_shading(rgb, a->face_light, corner_light, phong, lights, sh, nm, sm, B, F, &shading);
+    const int light = nr_internal::make_shading(rgb, a->face_light, corner_light, pc, B, F, &shading);
     if (light < 0) return NR_ERR_INVALID_ARG;
+    const nr_b200_phong_args* phong = pc.phong;
+    const nr_b200_normal_map_args* nm = pc.nm;
+    const nr_b200_specular_map_args* sm = pc.sm;
     if ((nm || sm) && !uv) return NR_ERR_INVALID_ARG;  // the maps are addressed by the pixel's uv
-    // the shading gradients: grad_corner_light needs corner_light, and every one reads the (unlit) textures (also a
-    // grad_lights of a set of NL = 0 lights, which then receives nothing)
+    // The Phong gradient outputs in ABI order, with their float counts.  A set of NL = 0 lights has a grad_lights of 0
+    // floats: it needs the textures like every other, and is never written.
+    const struct { float* ptr; size_t floats; } phong_out[] = {
+        {phong ? phong->grad_corner_shading : nullptr, phong ? (size_t)phong->shading_batch * F * 18 : 0},
+        {phong ? phong->grad_params : nullptr, phong ? (size_t)phong->params_batch * 16 : 0},
+        {pc.lights ? pc.lights->grad_lights : nullptr, pc.lights ? (size_t)pc.lights->lights_batch * shading.NL * 12 : 0},
+        {pc.sh ? pc.sh->grad_sh : nullptr, pc.sh ? (size_t)pc.sh->sh_batch * 27 : 0},
+        {nm ? nm->grad_normal_map : nullptr, nm ? (size_t)nm->map_batch * nr_internal::nm_floats(nm) : 0},
+        {nm ? nm->grad_corner_tangents : nullptr, nm ? (size_t)nm->tangent_batch * F * 12 : 0},
+        {sm ? sm->grad_specular_map : nullptr, sm ? (size_t)sm->map_batch * nr_internal::sm_floats(sm) : 0},
+    };
+    // the shading gradients: grad_corner_light needs corner_light, and every one reads the (unlit) textures
     if (grad_corner_light && !corner_light) return NR_ERR_INVALID_ARG;
-    float* grad_cs = phong ? phong->grad_corner_shading : nullptr;
-    float* grad_prm = phong ? phong->grad_params : nullptr;
-    float* grad_lts = shading.NL > 0 ? lights->grad_lights : nullptr;
-    float* grad_sh = sh ? sh->grad_sh : nullptr;
-    float* grad_nm = nm ? nm->grad_normal_map : nullptr;
-    float* grad_tg = nm ? nm->grad_corner_tangents : nullptr;
-    float* grad_sm = sm ? sm->grad_specular_map : nullptr;
-    if (!a->textures &&
-        (grad_corner_light || grad_cs || grad_prm || (lights && lights->grad_lights) || grad_sh || grad_nm || grad_tg || grad_sm))
-        return NR_ERR_INVALID_ARG;
     // a normal or specular map also sends its own term into grad_face_uvs from the Phong-gradient kernel
-    const bool phong_grads = grad_cs || grad_prm || grad_lts || grad_sh || grad_nm || grad_tg || grad_sm || ((nm || sm) && uv_grad);
+    bool any_phong_out = false, phong_grads = (nm || sm) && uv_grad;
+    for (const auto& o : phong_out) {
+        any_phong_out |= o.ptr != nullptr;
+        phong_grads |= o.ptr && o.floats;
+    }
+    if (!a->textures && (grad_corner_light || any_phong_out)) return NR_ERR_INVALID_ARG;
     // NR_GRAD_INTERIOR: the sampler's derivative reads the textures; the cubes of NR_TEX_Z_BATCH0 sample item b with the
     // depths of item 0, so their derivative would cross items (B = 1 is the plain sampler)
     const bool interior = (flags & NR_GRAD_INTERIOR) != 0;
@@ -1681,25 +1686,9 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
         if (part_tex && grad_corner_light &&
             cudaMemsetAsync(grad_corner_light, 0, (size_t)B * F * 9 * sizeof(float), stream) != cudaSuccess)
             return NR_ERR_CUDA;
-        if (part_tex && grad_cs &&
-            cudaMemsetAsync(grad_cs, 0, (size_t)phong->shading_batch * F * 18 * sizeof(float), stream) != cudaSuccess)
-            return NR_ERR_CUDA;
-        if (part_tex && grad_prm && cudaMemsetAsync(grad_prm, 0, (size_t)phong->params_batch * 16 * sizeof(float), stream) != cudaSuccess)
-            return NR_ERR_CUDA;
-        if (part_tex && grad_lts &&
-            cudaMemsetAsync(grad_lts, 0, (size_t)lights->lights_batch * lights->num_lights * 12 * sizeof(float), stream) != cudaSuccess)
-            return NR_ERR_CUDA;
-        if (part_tex && grad_sh && cudaMemsetAsync(grad_sh, 0, (size_t)sh->sh_batch * 27 * sizeof(float), stream) != cudaSuccess)
-            return NR_ERR_CUDA;
-        if (part_tex && grad_nm &&
-            cudaMemsetAsync(grad_nm, 0, (size_t)nm->map_batch * nr_internal::nm_floats(nm) * sizeof(float), stream) != cudaSuccess)
-            return NR_ERR_CUDA;
-        if (part_tex && grad_tg &&
-            cudaMemsetAsync(grad_tg, 0, (size_t)nm->tangent_batch * F * 12 * sizeof(float), stream) != cudaSuccess)
-            return NR_ERR_CUDA;
-        if (part_tex && grad_sm &&
-            cudaMemsetAsync(grad_sm, 0, (size_t)sm->map_batch * nr_internal::sm_floats(sm) * sizeof(float), stream) != cudaSuccess)
-            return NR_ERR_CUDA;
+        for (const auto& o : phong_out)
+            if (part_tex && o.ptr && o.floats && cudaMemsetAsync(o.ptr, 0, o.floats * sizeof(float), stream) != cudaSuccess)
+                return NR_ERR_CUDA;
         nr_internal::prof_end(stream);
     }
 
@@ -1734,7 +1723,7 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
         // without the map
         const int tg_light = light == nr::kLightFace ? nr::kLightNone
                            : light != nr::kLightPhongSM ? light
-                           : nm ? nr::kLightPhongNM : sh ? nr::kLightPhongSH : shading.NL > 0 ? nr::kLightPhongSet : nr::kLightPhong;
+                           : nm ? nr::kLightPhongNM : pc.sh ? nr::kLightPhongSH : shading.NL > 0 ? nr::kLightPhongSet : nr::kLightPhong;
         nr::dispatch_light<nr::kLightNone, nr::kLightCorner, nr::kLightPhong, nr::kLightPhongSet, nr::kLightPhongSH,
                            nr::kLightPhongNM>(tg_light, [&](auto kL) {
             if constexpr (kL != nr::kLightPhongNM) {  // a normal map needs NR_TEX_UV
@@ -1749,14 +1738,14 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
             });
         });
     };
-    // Phong: d loss / d corner_shading, params, lights and sh per pixel (nr_phong.cu), part of the texture half
+    // Phong: d loss / d corner_shading, params, lights, sh and the maps per pixel (nr_phong.cu), part of the texture half
     auto launch_phong_grad = [&]() {
         if (!phong_grads) return;
+        auto written = [&](int k) { return phong_out[k].floats ? phong_out[k].ptr : nullptr; };
         nr_internal::PhongGradLaunch pl{};
-        pl.args = a; pl.src = src; pl.shading = shading; pl.light = light;
-        pl.grad_cs = grad_cs; pl.grad_prm = grad_prm; pl.grad_lts = grad_lts; pl.grad_sh = grad_sh;
-        pl.grad_nm = grad_nm; pl.grad_tg = grad_tg; pl.grad_uvs = (nm || sm) ? a->grad_face_uvs : nullptr;
-        pl.grad_sm = grad_sm;
+        pl.args = a; pl.src = src; pl.shading = shading;
+        pl.grad = {written(0), written(1), written(2), written(3), written(4), written(5), written(6),
+                   (nm || sm) ? a->grad_face_uvs : nullptr};
         pl.tex_bstride = (flags & NR_TEX_SHARED) ? 0 : (uv ? img_floats : ncubes * (size_t)ts * ts * ts * 3);
         pl.uv_bstride = p.uv_bstride;
         pl.tex_cmp = p.tex_cmp; pl.tex_val = p.tex_val;
@@ -1865,7 +1854,7 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
 }
 
 extern "C" int nr_b200_backward(const nr_b200_backward_args* args, void* cuda_stream) {
-    return backward_impl(args, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, cuda_stream);
+    return backward_impl(args, nullptr, nullptr, {}, cuda_stream);
 }
 
 extern "C" int nr_b200_backward_corner_light(const nr_b200_backward_args* args, const float* corner_light,
@@ -1874,52 +1863,33 @@ extern "C" int nr_b200_backward_corner_light(const nr_b200_backward_args* args, 
         nr_internal::launch_count() = 0;
         return NR_ERR_INVALID_ARG;
     }
-    return backward_impl(args, corner_light, grad_corner_light, nullptr, nullptr, nullptr, nullptr, nullptr, cuda_stream);
+    return backward_impl(args, corner_light, grad_corner_light, {}, cuda_stream);
 }
 
 extern "C" int nr_b200_backward_phong(const nr_b200_backward_args* args, const nr_b200_phong_args* phong, void* cuda_stream) {
-    if (!phong) {
-        nr_internal::launch_count() = 0;
-        return NR_ERR_INVALID_ARG;
-    }
-    return backward_impl(args, nullptr, nullptr, phong, nullptr, nullptr, nullptr, nullptr, cuda_stream);
+    return phong ? backward_impl(args, nullptr, nullptr, {phong}, cuda_stream) : nr_internal::refuse_null_phong();
 }
 
 extern "C" int nr_b200_backward_lights(const nr_b200_backward_args* args, const nr_b200_phong_args* phong,
                                        const nr_b200_lights_args* lights, void* cuda_stream) {
-    if (!phong) {
-        nr_internal::launch_count() = 0;
-        return NR_ERR_INVALID_ARG;
-    }
-    return backward_impl(args, nullptr, nullptr, phong, lights, nullptr, nullptr, nullptr, cuda_stream);
+    return phong ? backward_impl(args, nullptr, nullptr, {phong, lights}, cuda_stream) : nr_internal::refuse_null_phong();
 }
 
 extern "C" int nr_b200_backward_sh(const nr_b200_backward_args* args, const nr_b200_phong_args* phong,
                                    const nr_b200_lights_args* lights, const nr_b200_sh_args* sh, void* cuda_stream) {
-    if (!phong) {
-        nr_internal::launch_count() = 0;
-        return NR_ERR_INVALID_ARG;
-    }
-    return backward_impl(args, nullptr, nullptr, phong, lights, sh, nullptr, nullptr, cuda_stream);
+    return phong ? backward_impl(args, nullptr, nullptr, {phong, lights, sh}, cuda_stream) : nr_internal::refuse_null_phong();
 }
 
 extern "C" int nr_b200_backward_normal_map(const nr_b200_backward_args* args, const nr_b200_phong_args* phong,
                                            const nr_b200_lights_args* lights, const nr_b200_sh_args* sh,
                                            const nr_b200_normal_map_args* nm, void* cuda_stream) {
-    if (!phong) {
-        nr_internal::launch_count() = 0;
-        return NR_ERR_INVALID_ARG;
-    }
-    return backward_impl(args, nullptr, nullptr, phong, lights, sh, nm, nullptr, cuda_stream);
+    return phong ? backward_impl(args, nullptr, nullptr, {phong, lights, sh, nm}, cuda_stream) : nr_internal::refuse_null_phong();
 }
 
 extern "C" int nr_b200_backward_specular_map(const nr_b200_backward_args* args, const nr_b200_phong_args* phong,
                                              const nr_b200_lights_args* lights, const nr_b200_sh_args* sh,
                                              const nr_b200_normal_map_args* nm, const nr_b200_specular_map_args* sm,
                                              void* cuda_stream) {
-    if (!phong) {
-        nr_internal::launch_count() = 0;
-        return NR_ERR_INVALID_ARG;
-    }
-    return backward_impl(args, nullptr, nullptr, phong, lights, sh, nm, sm, cuda_stream);
+    return phong ? backward_impl(args, nullptr, nullptr, {phong, lights, sh, nm, sm}, cuda_stream)
+                 : nr_internal::refuse_null_phong();
 }

@@ -488,11 +488,12 @@ __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigne
     o.fim = fn; o.w0 = w[0]; o.w1 = w[1]; o.w2 = w[2]; o.depth = zp; o.alpha = 1.0f;
     o.r = o.g = o.b = 0.0f;
     if (p.flags & NR_RETURN_RGB) {
+        float u = 0.0f, v = 0.0f;  // kUV: the pixel's uv, where the maps of modes 6-7 are sampled too
         if constexpr (kUV) {
             // the winner's own vertex depths (no batch-0 quirk); fill_back copies read face fn - F/2's corners reversed
             bool rev;
             const int uf = face_cube(p, fn, rev);
-            float uv[6], u, v;
+            float uv[6];
             nr::load_face_uvs(p.uvs + ((uint32_t)b * p.uv_bstride + (uint32_t)uf * 6u), rev, uv);
             nr::pixel_uv(w, zp, cc.y, cc.z, cc.w, uv, u, v);
             float l0 = 1.0f, l1 = 1.0f, l2 = 1.0f;
@@ -509,11 +510,6 @@ __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigne
                 const nr::UvTaps t = nr::uv_taps(u, v, p.Ht, p.Wt);
                 nr::uv_blend<kLight == nr::kLightFace>(p.textures + (uint32_t)b * p.img_bstride, p.Wt, t, l0, l1, l2, c);
             }
-            if constexpr (kLight >= nr::kLightPhongNM) {  // the maps are sampled at the same uv
-                float l[3];
-                nr::perspective_weights(w, zp, cc.y, cc.z, cc.w, l);
-                nr::shade_mapped<kLight == nr::kLightPhongSM>(p.shading, b, fn, l, u, v, c);
-            }
             o.r = c[0]; o.g = c[1]; o.b = c[2];
         } else {
             float z0, z1, z2;
@@ -525,10 +521,10 @@ __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigne
             const float* tex = p.textures + ((size_t)b * p.tex_bstride + cube) * (size_t)(ts * ts * ts) * 3;
             blend_corners<kLight == nr::kLightFace>(p, tc, tex, rev, b, fn, o.r, o.g, o.b);
         }
-        if constexpr (kLight >= nr::kLightCorner && kLight < nr::kLightPhongNM) {  // the light of the pixel's l_k (own depths) on the unlit sample
+        if constexpr (kLight >= nr::kLightCorner) {  // the light of the pixel's l_k (own depths) on the unlit sample
             float l[3], c[3] = {o.r, o.g, o.b};
             nr::perspective_weights(w, zp, cc.y, cc.z, cc.w, l);
-            nr::shade<kLight>(p.shading, b, p.F, fn, l, c);
+            nr::shade<kLight>(p.shading, b, p.F, fn, l, u, v, c);
             o.r = c[0]; o.g = c[1]; o.b = c[2];
         }
     }
@@ -747,12 +743,8 @@ extern "C" size_t nr_b200_forward_workspace_bytes(int32_t B, int32_t F, int32_t 
     return fwd_layout(B, F, S).total;
 }
 
-// nr_b200_forward (phong, lights, sh, nm, sm NULL), nr_b200_forward_phong (lights, sh, nm, sm NULL), nr_b200_forward_lights
-// (sh, nm, sm NULL), nr_b200_forward_sh (nm, sm NULL), nr_b200_forward_normal_map (sm NULL) and
-// nr_b200_forward_specular_map
-static int forward_impl(const nr_b200_forward_args* args, const nr_b200_phong_args* phong, const nr_b200_lights_args* lights,
-                        const nr_b200_sh_args* sh, const nr_b200_normal_map_args* nm, const nr_b200_specular_map_args* sm,
-                        void* cuda_stream) {
+// nr_b200_forward (no Phong inputs) and the five Phong entry points
+static int forward_impl(const nr_b200_forward_args* args, const nr_internal::PhongCall& pc, void* cuda_stream) {
     nr_internal::launch_count() = 0;
     // Two layouts: the full struct, and the ABI-4 struct from before corner_light (which then reads as NULL).  Only the
     // caller's struct_size bytes are read.
@@ -780,9 +772,10 @@ static int forward_impl(const nr_b200_forward_args* args, const nr_b200_phong_ar
     const bool mip = (flags & NR_TEX_MIPMAP) != 0;
     if (mip && !uv) return NR_ERR_INVALID_ARG;
     nr::Shading shading;
-    const int light = nr_internal::make_shading((flags & NR_RETURN_RGB) != 0, a->face_light, a->corner_light, phong, lights, sh,
-                                                nm, sm, B, F, &shading);
+    const int light = nr_internal::make_shading((flags & NR_RETURN_RGB) != 0, a->face_light, a->corner_light, pc, B, F, &shading);
     if (light < 0) return NR_ERR_INVALID_ARG;
+    const nr_b200_normal_map_args* nm = pc.nm;
+    const nr_b200_specular_map_args* sm = pc.sm;
     if ((nm || sm) && !uv) return NR_ERR_INVALID_ARG;  // the maps are addressed by the pixel's uv
     if ((flags & NR_ANTI_ALIASING) && (S & 1)) return NR_ERR_INVALID_ARG;
     if (S > 32767 || B > 65535) return NR_ERR_UNSUPPORTED;  // 32-bit pixel offsets; batch = grid.z of the resolve pass
@@ -911,52 +904,32 @@ static int forward_impl(const nr_b200_forward_args* args, const nr_b200_phong_ar
 }
 
 extern "C" int nr_b200_forward(const nr_b200_forward_args* args, void* cuda_stream) {
-    return forward_impl(args, nullptr, nullptr, nullptr, nullptr, nullptr, cuda_stream);
+    return forward_impl(args, {}, cuda_stream);
 }
 
 extern "C" int nr_b200_forward_phong(const nr_b200_forward_args* args, const nr_b200_phong_args* phong, void* cuda_stream) {
-    if (!phong) {
-        nr_internal::launch_count() = 0;
-        return NR_ERR_INVALID_ARG;
-    }
-    return forward_impl(args, phong, nullptr, nullptr, nullptr, nullptr, cuda_stream);
+    return phong ? forward_impl(args, {phong}, cuda_stream) : nr_internal::refuse_null_phong();
 }
 
 extern "C" int nr_b200_forward_lights(const nr_b200_forward_args* args, const nr_b200_phong_args* phong,
                                       const nr_b200_lights_args* lights, void* cuda_stream) {
-    if (!phong) {
-        nr_internal::launch_count() = 0;
-        return NR_ERR_INVALID_ARG;
-    }
-    return forward_impl(args, phong, lights, nullptr, nullptr, nullptr, cuda_stream);
+    return phong ? forward_impl(args, {phong, lights}, cuda_stream) : nr_internal::refuse_null_phong();
 }
 
 extern "C" int nr_b200_forward_sh(const nr_b200_forward_args* args, const nr_b200_phong_args* phong,
                                   const nr_b200_lights_args* lights, const nr_b200_sh_args* sh, void* cuda_stream) {
-    if (!phong) {
-        nr_internal::launch_count() = 0;
-        return NR_ERR_INVALID_ARG;
-    }
-    return forward_impl(args, phong, lights, sh, nullptr, nullptr, cuda_stream);
+    return phong ? forward_impl(args, {phong, lights, sh}, cuda_stream) : nr_internal::refuse_null_phong();
 }
 
 extern "C" int nr_b200_forward_normal_map(const nr_b200_forward_args* args, const nr_b200_phong_args* phong,
                                           const nr_b200_lights_args* lights, const nr_b200_sh_args* sh,
                                           const nr_b200_normal_map_args* nm, void* cuda_stream) {
-    if (!phong) {
-        nr_internal::launch_count() = 0;
-        return NR_ERR_INVALID_ARG;
-    }
-    return forward_impl(args, phong, lights, sh, nm, nullptr, cuda_stream);
+    return phong ? forward_impl(args, {phong, lights, sh, nm}, cuda_stream) : nr_internal::refuse_null_phong();
 }
 
 extern "C" int nr_b200_forward_specular_map(const nr_b200_forward_args* args, const nr_b200_phong_args* phong,
                                             const nr_b200_lights_args* lights, const nr_b200_sh_args* sh,
                                             const nr_b200_normal_map_args* nm, const nr_b200_specular_map_args* sm,
                                             void* cuda_stream) {
-    if (!phong) {
-        nr_internal::launch_count() = 0;
-        return NR_ERR_INVALID_ARG;
-    }
-    return forward_impl(args, phong, lights, sh, nm, sm, cuda_stream);
+    return phong ? forward_impl(args, {phong, lights, sh, nm, sm}, cuda_stream) : nr_internal::refuse_null_phong();
 }

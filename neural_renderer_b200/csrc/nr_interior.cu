@@ -83,7 +83,7 @@ __global__ void __launch_bounds__(256) k_interior_grad(const __grid_constant__ I
         nr::perspective_weight_grads(inv, z, zp, lam, lx, ly);
         // the light factor L_c of d rgb_c / d s_c
         float L[3], C[9];
-        nr::pixel_light<kLight>(p.shading, b, p.F, fn, lam, L);
+        nr::pixel_light<kLight>(p.shading, b, p.F, fn, lam, 0.0f, 0.0f, L);  // no Phong mode, so no map reads the uv
         if constexpr (kLight == nr::kLightCorner) {
             const float* cp = p.shading.corner_light + p.shading.cl_off(b, p.F, fn);
 #pragma unroll

@@ -85,13 +85,29 @@ inline bool sm_args_ok(const nr_b200_specular_map_args* sm, int B) {
 // floats of one item's specular map (32-bit offsets in the kernels, as nm_floats)
 inline size_t sm_floats(const nr_b200_specular_map_args* sm) { return (size_t)sm->map_height * (size_t)sm->map_width * 4; }
 
+// The Phong inputs of a call as the ABI passes them, each NULL when absent (all NULL: no Phong shading).  Every Phong
+// entry point is nr_b200_*_specular_map with its missing trailing structs NULL.
+struct PhongCall {
+    const nr_b200_phong_args* phong;
+    const nr_b200_lights_args* lights;
+    const nr_b200_sh_args* sh;
+    const nr_b200_normal_map_args* nm;
+    const nr_b200_specular_map_args* sm;
+};
+
+// What a Phong entry point returns for a NULL phong struct: nothing else is read and nothing is launched
+inline int refuse_null_phong() {
+    launch_count() = 0;
+    return NR_ERR_INVALID_ARG;
+}
+
 // The light mode (nr_shading.cuh) and nr::Shading of a call from its ABI arguments, or -1 for a refused combination
 // (NR_ERR_INVALID_ARG): corner_light only for RGB and instead of face_light; Phong only for RGB and instead of both; the
 // Phong, light-set, SH, normal-map and specular-map structs pass their checks.  face_light is ignored without RGB, and a
 // set of NL = 0 lights is the Phong call exactly.
-inline int make_shading(bool rgb, const float* face_light, const float* corner_light, const nr_b200_phong_args* phong,
-                        const nr_b200_lights_args* lights, const nr_b200_sh_args* sh, const nr_b200_normal_map_args* nm,
-                        const nr_b200_specular_map_args* sm, int B, int F, nr::Shading* s) {
+inline int make_shading(bool rgb, const float* face_light, const float* corner_light, const PhongCall& c, int B, int F,
+                        nr::Shading* s) {
+    auto [phong, lights, sh, nm, sm] = c;
     *s = nr::Shading{};
     if (corner_light && (!rgb || face_light)) return -1;
     if (phong && (!rgb || face_light || corner_light || !phong_args_ok(phong, B))) return -1;

@@ -25,14 +25,15 @@
 //                   mapped normal n' (nr::nm_pixel_normal), so the chains above end in g' = d loss / d n'.  Then
 //                   nm_grad_tail samples the map and builds the frame again and sends gm to the map's four taps (two
 //                   6-float rows by vector reductions, as k_image_grad); the 9 tangent floats l_k gt and the 6 UV floats l_k (gu, gv) widen the run reduction to 33.
-//                   The launcher picks kLights = NL > 0 and kSH = (sh given) as for the other modes.
+//                   The launcher takes kLights (NL > 0), kSH, kNM and kSM from which inputs the record holds.
 //                   kSM (kLightPhongSM, a specular map; kTex 1 / 2; kNM = a normal map given too): the map's sample
 //                   (ks, sigma') at the pixel's uv enters the expression and its derivative as K' = ks K, K'_j = ks K_j and
 //                   sigma' (the sq argument of the nr_math.cuh helpers).  Per pixel gq_c = K_c g_c h + sum_j K_jc g_c a_j h_j
 //                   is split off the K and K_j gradients (which keep ks_c times theirs) and gq_3 = d loss / d sigma' off
 //                   params' slot 12, which receives 0; sm_grad_tail samples the map again and sends gq to its four taps (one
 //                   16-byte vector reduction each) and l_k (gu, gv) to the UV floats of the run reduction (24, or shared with
-//                   the normal map's six in 33).
+//                   the normal map's six in 33).  Both map tails and the corner floats are written by pixel_grad_tail,
+//                   after light 0 alone or after the loop over the lights.
 //
 // It belongs to the texture half of the backward: the texture-gradient kernels (K6, k_image_grad) only need the pixel's
 // L_c, and keeping the 34 gradient floats out of them keeps their register budgets (DESIGN.md section 4g).
@@ -65,7 +66,7 @@ struct PhongParams {
     int aa, fill_back, z_batch0;
     float tex_cmp, tex_val;
     nr::MipTable mip;  // kTex 2
-    nr::Shading shading;  // corner_shading, params, lights, sh and the normal map
+    nr::Shading shading;  // corner_shading, params, lights, sh and the maps
     float* grad_nm;       // kNM: the layouts of normal_map, corner_tangents and face_uvs, or nullptr
     float* grad_tg;
     float* grad_uvs;
@@ -158,6 +159,31 @@ __device__ __forceinline__ void sm_grad_tail(const PhongParams& p, int b, const 
     cuv[4] = __fmaf_rn(s2, gu, cuv[4]); cuv[5] = __fmaf_rn(s2, gv, cuv[5]);
 }
 
+// where the maps' 6 UV floats start in the run reduction: after the 18 corner floats and kNM's 9 tangent floats
+template <bool kNM>
+constexpr int kUvAt = kNM ? 27 : 18;
+
+// The per-pixel end of k_phong_grad once gn = d loss / d n (kNM: d loss / d n') and gp = d loss / d p are known: the map
+// tails (kSM: d loss / d sigma' goes to the map as gq[3], not to params' slot 12), then the 18 corner floats of cg
+template <bool kNM, bool kSM>
+__device__ __forceinline__ void pixel_grad_tail(const PhongParams& p, int b, int fn, const float lam[3], float u, float v,
+                                                bool rev, float gn[3], const float gp[3], float gq[4], float gprm[16],
+                                                float* cg) {
+    if constexpr (kNM) nm_grad_tail(p, b, fn, lam, u, v, rev, gn, cg + 18);
+    if constexpr (kSM) {
+        gq[3] = gprm[12];
+        gprm[12] = 0.0f;
+        sm_grad_tail(p, b, lam, u, v, rev, gq, cg + kUvAt<kNM>);
+    }
+#pragma unroll
+    for (int k = 0; k < 3; k++)
+#pragma unroll
+        for (int j = 0; j < 3; j++) {
+            cg[6 * k + j] = __fmul_rn(lam[k], gn[j]);
+            cg[6 * k + 3 + j] = __fmul_rn(lam[k], gp[j]);
+        }
+}
+
 // kSH: the 27 floats Y_k w_c of grad_sh summed over the warp one at a time into shared memory, then over the CTA before 27
 // atomics into `o` (item b's [9,3] slot, or slot 0 with Bs = 1).  Every thread of the CTA calls it (0 off the mesh).
 __device__ __forceinline__ void sh_grad_reduce(const float Y[9], const float ws[3], float* o, int lane, int warp) {
@@ -182,7 +208,6 @@ template <int kTex, bool kIdx, bool kLights, bool kSH, bool kNM, bool kSM>
 __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ PhongParams p) {
     static_assert(!(kNM || kSM) || kTex != 0, "the maps need NR_TEX_UV");
     constexpr int kCg = kNM ? 33 : kSM ? 24 : 18;  // the corner floats of the run reduction
-    constexpr int kUv = kNM ? 27 : 18;              // kNM / kSM: where its 6 UV floats start
     __shared__ float s_prm[8][16];
     const int S = p.S;
     const size_t plane = (size_t)S * S;
@@ -324,19 +349,7 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
 #pragma unroll
                 for (int k = 0; k < 3; k++) gn[k] = __fadd_rn(gn[k], t[k]);
             }
-            if constexpr (kNM) nm_grad_tail(p, b, fn, lam, nmu, nmv, nmrev, gn, cg + 18);
-            if constexpr (kSM) {  // d loss / d sigma' goes to the map, not to params' sigma
-                gq[3] = gprm[12];
-                gprm[12] = 0.0f;
-                sm_grad_tail(p, b, lam, nmu, nmv, nmrev, gq, cg + kUv);
-            }
-#pragma unroll
-            for (int k = 0; k < 3; k++)
-#pragma unroll
-                for (int j = 0; j < 3; j++) {
-                    cg[6 * k + j] = __fmul_rn(lam[k], gn[j]);
-                    cg[6 * k + 3 + j] = __fmul_rn(lam[k], gp[j]);
-                }
+            pixel_grad_tail<kNM, kSM>(p, b, fn, lam, nmu, nmv, nmrev, gn, gp, gq, gprm, cg);
         }
     }
     if constexpr (kLights) {
@@ -386,19 +399,7 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
         }
         if (fn >= 0) {
             nr::phong_lights_grad_end(xE, gnh, gvh, gsig, xgn, xgp, gprm);
-            if constexpr (kNM) nm_grad_tail(p, b, fn, xlam, nmu, nmv, nmrev, xgn, cg + 18);
-            if constexpr (kSM) {
-                gq[3] = gprm[12];
-                gprm[12] = 0.0f;
-                sm_grad_tail(p, b, xlam, nmu, nmv, nmrev, gq, cg + kUv);
-            }
-#pragma unroll
-            for (int k = 0; k < 3; k++)
-#pragma unroll
-                for (int j = 0; j < 3; j++) {
-                    cg[6 * k + j] = __fmul_rn(xlam[k], xgn[j]);
-                    cg[6 * k + 3 + j] = __fmul_rn(xlam[k], xgp[j]);
-                }
+            pixel_grad_tail<kNM, kSM>(p, b, fn, xlam, nmu, nmv, nmrev, xgn, xgp, gq, gprm, cg);
         }
         if (p.grad_lts) {  // uniform: the CTA's sum of each light's 10 floats, then 10 atomics per light
             __syncthreads();
@@ -447,7 +448,7 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
                 if (p.grad_uvs) {
                     float* o = p.grad_uvs + ((size_t)b * p.uv_bstride + (size_t)nmtf * 6u);
 #pragma unroll
-                    for (int k = 0; k < 6; k++) atomicAdd(o + k, cg[kUv + k]);
+                    for (int k = 0; k < 6; k++) atomicAdd(o + k, cg[kUvAt<kNM> + k]);
                 }
             }
         }
@@ -484,7 +485,7 @@ void launch_phong_grad(const PhongGradLaunch& L, cudaStream_t stream) {
     p.fim = a->face_index_map; p.wmap = a->weight_map; p.dmap = a->depth_map; p.g = a->grad_rgb;
     p.textures = a->textures; p.tex_bstride = L.tex_bstride;
     p.uvs = a->face_uvs; p.uv_bstride = L.uv_bstride;
-    p.grad_cs = L.grad_cs; p.grad_prm = L.grad_prm; p.grad_lts = L.grad_lts; p.grad_sh = L.grad_sh;
+    p.grad_cs = L.grad.cs; p.grad_prm = L.grad.prm; p.grad_lts = L.grad.lts; p.grad_sh = L.grad.sh;
     p.S = a->raster_size; p.F = a->num_faces; p.ts = a->texture_size;
     p.Ht = a->texture_height; p.Wt = a->texture_width;
     p.aa = (flags & NR_ANTI_ALIASING) ? 1 : 0;
@@ -493,28 +494,24 @@ void launch_phong_grad(const PhongGradLaunch& L, cudaStream_t stream) {
     p.tex_cmp = L.tex_cmp; p.tex_val = L.tex_val;
     if (L.mip) p.mip = *L.mip;
     p.shading = L.shading;
-    p.grad_nm = L.grad_nm; p.grad_tg = L.grad_tg; p.grad_uvs = L.grad_uvs; p.grad_sm = L.grad_sm;
+    p.grad_nm = L.grad.nm; p.grad_tg = L.grad.tg; p.grad_uvs = L.grad.uvs; p.grad_sm = L.grad.sm;
     const bool idx = (flags & NR_FACES_INDEXED) != 0;
     const int tex = (flags & NR_TEX_MIPMAP) ? 2 : (flags & NR_TEX_UV) ? 1 : 0;
     const dim3 grid((unsigned)(((size_t)p.S * p.S + 255) / 256), a->batch_size);
     LaunchScope ls("k_phong_grad", stream);
-    // the kernel's split of the mode: a light set of NL > 0 lights (kLightPhongSet, or kLightPhongSH / kLightPhongNM with
-    // one), an SH environment (kLightPhongSH, or kLightPhongNM / kLightPhongSM with one), a normal map (kLightPhongNM, or
-    // kLightPhongSM with one; NR_TEX_UV only), a specular map (kLightPhongSM)
+    // the kernel's split of the light mode (3-7): a light set of NL > 0 lights, an SH environment, a normal map and a
+    // specular map, each read from the record
     nr::dispatch_bool(p.shading.NL > 0, [&](auto kLights) {
         nr::dispatch_bool(p.shading.sh != nullptr, [&](auto kSH) {
             nr::dispatch_bool(idx, [&](auto kIdx) {
-                if (L.light == nr::kLightPhongSM) {
-                    nr::dispatch_bool(p.shading.nm != nullptr, [&](auto kNM) {
-                        if (tex == 2) k_phong_grad<2, kIdx, kLights, kSH, kNM, true><<<grid, 256, 0, stream>>>(p);
-                        else k_phong_grad<1, kIdx, kLights, kSH, kNM, true><<<grid, 256, 0, stream>>>(p);
+                nr::dispatch_bool(p.shading.nm != nullptr, [&](auto kNM) {
+                    nr::dispatch_bool(p.shading.sm != nullptr, [&](auto kSM) {
+                        if (tex == 2) k_phong_grad<2, kIdx, kLights, kSH, kNM, kSM><<<grid, 256, 0, stream>>>(p);
+                        else if (tex == 1) k_phong_grad<1, kIdx, kLights, kSH, kNM, kSM><<<grid, 256, 0, stream>>>(p);
+                        else if constexpr (!kNM && !kSM)  // the maps need NR_TEX_UV (checked on the host)
+                            k_phong_grad<0, kIdx, kLights, kSH, false, false><<<grid, 256, 0, stream>>>(p);
                     });
-                } else if (L.light == nr::kLightPhongNM) {
-                    if (tex == 2) k_phong_grad<2, kIdx, kLights, kSH, true, false><<<grid, 256, 0, stream>>>(p);
-                    else k_phong_grad<1, kIdx, kLights, kSH, true, false><<<grid, 256, 0, stream>>>(p);
-                } else if (tex == 2) k_phong_grad<2, kIdx, kLights, kSH, false, false><<<grid, 256, 0, stream>>>(p);
-                else if (tex == 1) k_phong_grad<1, kIdx, kLights, kSH, false, false><<<grid, 256, 0, stream>>>(p);
-                else k_phong_grad<0, kIdx, kLights, kSH, false, false><<<grid, 256, 0, stream>>>(p);
+                });
             });
         });
     });

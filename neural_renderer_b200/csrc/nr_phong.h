@@ -11,18 +11,17 @@
 
 namespace nr_internal {
 
+// what k_phong_grad writes, each in the layout of its input, or nullptr
+struct PhongGrads {
+    float *cs, *prm, *lts, *sh;  // d loss / d corner_shading, params, lights (NL > 0) and sh
+    float *nm, *tg, *sm;         // d loss / d normal_map, corner_tangents and specular_map
+    float* uvs;                  // with a map: the maps' term of d loss / d face_uvs
+};
+
 struct PhongGradLaunch {
     const nr_b200_backward_args* args;  // the checked call (flags, maps, grad_rgb, textures, face_uvs)
     nr::Shading shading;                // the call's Phong inputs (nr_internal::make_shading)
-    int light;                          // its light mode: kLightPhong, kLightPhongSet, kLightPhongSH, kLightPhongNM or kLightPhongSM
-    float* grad_cs;                     // d loss / d corner_shading, params, lights (NL > 0) and sh, or nullptr
-    float* grad_prm;
-    float* grad_lts;
-    float* grad_sh;
-    float* grad_nm;                     // kLightPhongNM: d loss / d normal_map, corner_tangents, and the map's term of
-    float* grad_tg;                     // d loss / d face_uvs, or nullptr
-    float* grad_uvs;
-    float* grad_sm;                     // kLightPhongSM: d loss / d specular_map, or nullptr
+    PhongGrads grad;
     nr::FaceSrc src;
     size_t tex_bstride;       // floats per item in `textures` (0 = shared)
     uint32_t uv_bstride;      // floats per item in face_uvs (0 = shared)

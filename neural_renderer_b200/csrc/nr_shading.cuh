@@ -70,62 +70,38 @@ __device__ __forceinline__ void nm_pixel_normal(const Shading& s, int b, int fn,
     nm_sample<false>(s.nm + s.nm_off(b), s.Hm, s.Wm, uv_taps(u, v, s.Hm, s.Wm), m, du, dv);
     nm_normal(s.cs + s.cs_off(b, fn), s.tg + s.tg_off(b, fn), l, m, F, E.n);
 }
-// pixel_light of kLightPhongNM, which also needs the pixel's (u, v): the diffuse part of the Phong expression with the
-// mapped normal, the set's diffuse terms (NL >= 0), then E_c when an environment is given
-__device__ __forceinline__ void pixel_light_nm(const Shading& s, int b, int fn, const float l[3], float u, float v, float L[3]) {
-    const float* cs = s.cs + s.cs_off(b, fn);
-    PhongEval E;
-    NmFrame F;
-    float m[3];
-    nm_pixel_normal(s, b, fn, l, u, v, m, F, E);
-    phong_diffuse_n(s.prm + s.prm_off(b), E);
-    if (s.NL > 0) {  // uniform
-        float pos[3];
-        phong_position(cs, l, pos);
-        lights_diffuse_loop(s.lts + s.lts_off(b), s.NL, pos, E);
-    }
-    if (s.sh) sh_add_irradiance(s.sh + s.sh_off(b), E);  // uniform
-    L[0] = E.L[0]; L[1] = E.L[1]; L[2] = E.L[2];
-}
 // kLightPhongSM: the specular map's sample sq = (ks, sigma') at the pixel's (u, v)
 __device__ __forceinline__ void sm_pixel_sample(const Shading& s, int b, float u, float v, float sq[4]) {
     float du[4], dv[4];
     sm_sample<false>(s.sm + s.sm_off(b), s.Hq, s.Wq, uv_taps(u, v, s.Hq, s.Wq), sq, du, dv);
 }
-// shade of kLightPhongNM (kSM false) and kLightPhongSM (kSM): the rgb of the light-set / SH expression with the mapped
-// normal (kSM: the interpolated one when no normal map is given) and kSM's K' and sigma' (NL = 0 and no environment:
-// phong_lights_rgb is phong_rgb, so a flat normal map and a constant (1, 1, 1, sigma) specular map render as the modes
-// 3-5 do, bit for bit)
-template <bool kSM>
-__device__ __forceinline__ void shade_mapped(const Shading& s, int b, int fn, const float l[3], float u, float v, float c[3]) {
-    const float* prm = s.prm + s.prm_off(b);
-    const float* lts = s.lts + s.lts_off(b);
-    const float* cs = s.cs + s.cs_off(b, fn);
-    PhongEval E;
-    if (!kSM || s.nm) {  // uniform
+
+// What the Phong modes read besides corner_shading and params: modes 3-5 fix it at compile time, the maps' modes 6-7
+// test the light set (NL >= 0), the SH environment and (mode 7) the normal map at run time, uniform per launch.
+template <int kLight>
+__device__ __forceinline__ bool reads_sh(const Shading& s) {
+    return kLight == kLightPhongSH || (kLight >= kLightPhongNM && s.sh);
+}
+// E.n of a Phong mode's pixel (cs = face fn's corner_shading): the mapped normal n' at the pixel's (u, v), or the
+// interpolated n
+template <int kLight>
+__device__ __forceinline__ void pixel_normal(const Shading& s, int b, int fn, const float* cs, const float l[3], float u, float v,
+                                             PhongEval& E) {
+    if (kLight == kLightPhongNM || (kLight == kLightPhongSM && s.nm)) {  // uniform
         NmFrame F;
         float m[3];
         nm_pixel_normal(s, b, fn, l, u, v, m, F, E);
     } else {
         phong_normal(cs, l, E.n);
     }
-    float sq[4];
-    if constexpr (kSM) sm_pixel_sample(s, b, u, v, sq);
-    const float* q = kSM ? sq : nullptr;
-    phong_diffuse_n(prm, E);
-    phong_specular(cs, l, prm, E, q);
-    float pos[3], rgb[3];
-    phong_position(cs, l, pos);
-    lights_diffuse_loop(lts, s.NL, pos, E);
-    if (s.sh) sh_add_irradiance(s.sh + s.sh_off(b), E);  // uniform
-    phong_lights_rgb(E, pos, prm, lts, s.NL, c, rgb, q);
-    c[0] = rgb[0]; c[1] = rgb[1]; c[2] = rgb[2];
 }
 
-// L_c = d rgb_c / d s_c of face fn's pixel with perspective weights l (own vertex depths): 1, face_light, the
-// interpolated corner light, or the diffuse part of the Phong expression (with the set's diffuse terms, then E_c)
+// L_c = d rgb_c / d s_c of face fn's pixel with perspective weights l (own vertex depths) and uv (u, v) (read by the
+// normal map only): 1, face_light, the interpolated corner light, or the diffuse part of the Phong expression (with the
+// set's diffuse terms, then E_c).  The specular map never enters L_c.
 template <int kLight>
-__device__ __forceinline__ void pixel_light(const Shading& s, int b, int F, int fn, const float l[3], float L[3]) {
+__device__ __forceinline__ void pixel_light(const Shading& s, int b, int F, int fn, const float l[3], float u, float v,
+                                            float L[3]) {
     if constexpr (kLight == kLightNone) {
         L[0] = L[1] = L[2] = 1.0f;
     } else if constexpr (kLight == kLightFace) {
@@ -136,21 +112,30 @@ __device__ __forceinline__ void pixel_light(const Shading& s, int b, int F, int 
     } else {
         const float* cs = s.cs + s.cs_off(b, fn);
         PhongEval E;
-        phong_diffuse(cs, l, s.prm + s.prm_off(b), E);
-        if constexpr (kLight >= kLightPhongSet) {
-            float pos[3];
-            phong_position(cs, l, pos);
-            lights_diffuse_loop(s.lts + s.lts_off(b), s.NL, pos, E);
+        if constexpr (kLight >= kLightPhongNM) {  // modes 3-5 form params' address before the normal, which their SASS keeps
+            pixel_normal<kLight>(s, b, fn, cs, l, u, v, E);
+            phong_diffuse_n(s.prm + s.prm_off(b), E);
+        } else {
+            phong_diffuse(cs, l, s.prm + s.prm_off(b), E);
         }
-        if constexpr (kLight == kLightPhongSH) sh_add_irradiance(s.sh + s.sh_off(b), E);
+        if constexpr (kLight >= kLightPhongSet) {
+            if (kLight < kLightPhongNM || s.NL > 0) {  // uniform
+                float pos[3];
+                phong_position(cs, l, pos);
+                lights_diffuse_loop(s.lts + s.lts_off(b), s.NL, pos, E);
+            }
+        }
+        if (reads_sh<kLight>(s)) sh_add_irradiance(s.sh + s.sh_off(b), E);  // uniform
         L[0] = E.L[0]; L[1] = E.L[1]; L[2] = E.L[2];
     }
 }
 
-// rgb of face fn's pixel from its unlit sample c (in place) and perspective weights l, for the modes that shade the
-// sample after sampling (kLightCorner and the Phong modes; face_light is applied per texel by the samplers)
+// rgb of face fn's pixel from its unlit sample c (in place), perspective weights l and uv (u, v) (read by the maps
+// only), for the modes that shade the sample after sampling (kLightCorner and the Phong modes; face_light is applied
+// per texel by the samplers).  With NL = 0 and no environment phong_lights_rgb is phong_rgb, so a flat normal map and a
+// constant (1, 1, 1, sigma) specular map render as modes 3-5 do, bit for bit.
 template <int kLight>
-__device__ __forceinline__ void shade(const Shading& s, int b, int F, int fn, const float l[3], float c[3]) {
+__device__ __forceinline__ void shade(const Shading& s, int b, int F, int fn, const float l[3], float u, float v, float c[3]) {
     static_assert(kLight >= kLightCorner, "unlit and face_light samples are final");
     if constexpr (kLight == kLightCorner) {
         float L[3];
@@ -160,8 +145,13 @@ __device__ __forceinline__ void shade(const Shading& s, int b, int F, int fn, co
         const float* prm = s.prm + s.prm_off(b);
         const float* lts = s.lts + s.lts_off(b);  // the set modes
         const float* cs = s.cs + s.cs_off(b, fn);
+        float sq[4];  // kLightPhongSM: K' and sigma' come from the specular map
+        const float* q = kLight == kLightPhongSM ? sq : nullptr;
         PhongEval E;
-        phong_at(cs, l, prm, E);
+        pixel_normal<kLight>(s, b, fn, cs, l, u, v, E);
+        if constexpr (kLight == kLightPhongSM) sm_pixel_sample(s, b, u, v, sq);
+        phong_diffuse_n(prm, E);
+        phong_specular(cs, l, prm, E, q);
         float rgb[3];
         if constexpr (kLight == kLightPhong) {
             phong_rgb(E, prm, c, rgb);
@@ -169,8 +159,8 @@ __device__ __forceinline__ void shade(const Shading& s, int b, int F, int fn, co
             float pos[3];
             phong_position(cs, l, pos);
             lights_diffuse_loop(lts, s.NL, pos, E);
-            if constexpr (kLight == kLightPhongSH) sh_add_irradiance(s.sh + s.sh_off(b), E);
-            phong_lights_rgb(E, pos, prm, lts, s.NL, c, rgb);
+            if (reads_sh<kLight>(s)) sh_add_irradiance(s.sh + s.sh_off(b), E);  // uniform
+            phong_lights_rgb(E, pos, prm, lts, s.NL, c, rgb, q);
         }
         c[0] = rgb[0]; c[1] = rgb[1]; c[2] = rgb[2];
     }

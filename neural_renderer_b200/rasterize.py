@@ -317,25 +317,17 @@ class _RasterizeFunction(torch.autograd.Function):
     the `Rasterize` object can look at them)."""
 
     @staticmethod
-    def forward(ctx, geom, textures, face_light, cfg, indices, face_uvs=None, corner_light=None, corner_shading=None,
-                shading_params=None, lights=None, environment_sh=None, normal_map=None, corner_tangents=None,
-                specular_map=None):
+    def forward(ctx, geom, textures, face_light, cfg, indices, face_uvs, corner_light, *phong):
         lib = _lib.load()
         dev = geom.device
         geom_c = geom.detach().contiguous()
         tex_c = textures.detach().contiguous() if textures is not None else None
         light_c = face_light.detach().to(torch.float32).contiguous() if face_light is not None else None
         corner_c = corner_light.detach().to(torch.float32).contiguous() if corner_light is not None else None
-        # Phong shading: corner_shading [Bc,F,3,6] and params [Bp,16], Bc / Bp = 1 for one set shared by every item
-        cs_c = corner_shading.detach().to(torch.float32).contiguous() if corner_shading is not None else None
-        sp_c = shading_params.detach().to(torch.float32).contiguous() if shading_params is not None else None
-        lt_c = lights.detach().to(torch.float32).contiguous() if lights is not None else None  # [Bl,NL,12], NL >= 1
-        sh_c = environment_sh.detach().to(torch.float32).contiguous() if environment_sh is not None else None  # [Bs,9,3]
-        nm_c = normal_map.detach().to(torch.float32).contiguous() if normal_map is not None else None  # [Bm,Hm,Wm,3]
-        tg_c = corner_tangents.detach().to(torch.float32).contiguous() if corner_tangents is not None else None  # [Bt,F,3,4]
-        sm_c = specular_map.detach().to(torch.float32).contiguous() if specular_map is not None else None  # [Bq,Hq,Wq,4]
-        if sm_c is not None and sm_c.data_ptr() % 16:
-            sm_c = sm_c.clone()  # the kernels read a texel as one aligned 16-byte vector
+        # Phong shading: the inputs of _PHONG_DIMS with their batch axes (1 for a set shared by every item), or None
+        phong_c = [t.detach().to(torch.float32).contiguous() if t is not None else None for t in phong]
+        if phong_c[6] is not None and phong_c[6].data_ptr() % 16:
+            phong_c[6] = phong_c[6].clone()  # specular_map: the kernels read a texel as one aligned 16-byte vector
         flags = cfg.flags
         if indices is not None:
             B, Nv = geom_c.shape[:2]
@@ -398,23 +390,10 @@ class _RasterizeFunction(torch.autograd.Function):
             a.face_light = _ptr(light_c)
             a.face_uvs, (a.texture_height, a.texture_width) = _ptr(uv_c), tex_hw
             a.corner_light = _ptr(corner_c)
-            if cs_c is None:
+            if phong_c[0] is None:
                 _lib.check(lib.nr_b200_forward(ctypes.byref(a), _stream_ptr(dev)))
-            else:  # every Phong render, with NULL lights / sh where absent
-                ph = _phong_args(cs_c, sp_c)
-                la = _lights_args(lt_c) if lt_c is not None else None
-                sa = _sh_args(sh_c) if sh_c is not None else None
-                if sm_c is not None:
-                    na = _normal_map_args(nm_c, tg_c) if nm_c is not None else None
-                    _lib.check(lib.nr_b200_forward_specular_map(ctypes.byref(a), ctypes.byref(ph), _byref(la), _byref(sa),
-                                                                _byref(na), ctypes.byref(_specular_map_args(sm_c)),
-                                                                _stream_ptr(dev)))
-                elif nm_c is None:
-                    _lib.check(lib.nr_b200_forward_sh(ctypes.byref(a), ctypes.byref(ph), _byref(la), _byref(sa), _stream_ptr(dev)))
-                else:
-                    na = _normal_map_args(nm_c, tg_c)
-                    _lib.check(lib.nr_b200_forward_normal_map(ctypes.byref(a), ctypes.byref(ph), _byref(la), _byref(sa),
-                                                              ctypes.byref(na), _stream_ptr(dev)))
+            else:  # every Phong render, with NULL structs where an input is absent
+                _lib.check(lib.nr_b200_forward_specular_map(ctypes.byref(a), *_phong_structs(phong_c), _stream_ptr(dev)))
         ctx.cfg = cfg
         ctx.flags = flags
         ctx.ts = ts
@@ -425,19 +404,12 @@ class _RasterizeFunction(torch.autograd.Function):
         need_light_grad = light_c is not None and ctx.needs_input_grad[2]
         ctx.need_corner_grad = corner_c is not None and ctx.needs_input_grad[6]
         ctx.need_uv_grad = uv_c is not None and want_rgb and ctx.needs_input_grad[5]
-        ctx.need_cs_grad = cs_c is not None and ctx.needs_input_grad[7]
-        ctx.need_sp_grad = sp_c is not None and ctx.needs_input_grad[8]
-        ctx.need_lt_grad = lt_c is not None and ctx.needs_input_grad[9]
-        ctx.need_sh_grad = sh_c is not None and ctx.needs_input_grad[10]
-        ctx.need_nm_grad = nm_c is not None and ctx.needs_input_grad[11]
-        ctx.need_tg_grad = tg_c is not None and ctx.needs_input_grad[12]
-        ctx.need_sm_grad = sm_c is not None and ctx.needs_input_grad[13]
+        ctx.need_phong_grad = [t is not None and need for t, need in zip(phong_c, ctx.needs_input_grad[7:])]
         # interior_gradient: the backward differentiates the sampler, so it reads the textures (and face_uvs / corner_light)
         ctx.interior = cfg.interior and want_rgb and ctx.needs_input_grad[0]
-        need_tex = need_light_grad or ctx.need_uv_grad or ctx.need_corner_grad or ctx.interior or ctx.need_cs_grad or \
-            ctx.need_sp_grad or ctx.need_lt_grad or ctx.need_sh_grad or ctx.need_nm_grad or ctx.need_tg_grad or ctx.need_sm_grad
+        need_tex = need_light_grad or ctx.need_uv_grad or ctx.need_corner_grad or ctx.interior or any(ctx.need_phong_grad)
         ctx.save_for_backward(geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c if need_tex else None, indices, uv_c, corner_c,
-                              cs_c, sp_c, lt_c, sh_c, nm_c, tg_c, sm_c)
+                              *phong_c)
         if cfg.aa:
             rgb_o, alpha_o, depth_o = out_rgb, out_alpha, out_depth
         else:
@@ -450,8 +422,7 @@ class _RasterizeFunction(torch.autograd.Function):
         lib = _lib.load()
         cfg = ctx.cfg
         flags = ctx.flags | (_lib.NR_GRAD_INTERIOR if ctx.interior else 0)
-        geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c, indices, uv_c, corner_c, cs_c, sp_c, lt_c, sh_c, nm_c, tg_c, sm_c = \
-            ctx.saved_tensors
+        geom_c, fim, wmap, dmap, rgb_map, light_c, tex_c, indices, uv_c, corner_c, *phong_c = ctx.saved_tensors
         dev = geom_c.device
         B, F = geom_c.shape[0], ctx.F
         want_rgb = bool(flags & _lib.NR_RETURN_RGB)
@@ -470,18 +441,8 @@ class _RasterizeFunction(torch.autograd.Function):
             grad_light = torch.empty_like(light_c) if (want_rgb and light_c is not None and ctx.needs_input_grad[2]) else None
             grad_uvs = torch.empty_like(uv_c) if ctx.need_uv_grad else None  # same layout as face_uvs: [1|B,F',3,2]
             grad_corner = torch.empty_like(corner_c) if ctx.need_corner_grad else None
-            grad_cs = torch.empty_like(cs_c) if ctx.need_cs_grad else None
-            grad_sp = torch.empty_like(sp_c) if ctx.need_sp_grad else None
-            ph = _phong_args(cs_c, sp_c, grad_cs, grad_sp) if cs_c is not None else None
-            grad_lt = torch.empty_like(lt_c) if ctx.need_lt_grad else None
-            la = _lights_args(lt_c, grad_lt) if lt_c is not None else None
-            grad_sh = torch.empty_like(sh_c) if ctx.need_sh_grad else None
-            sa = _sh_args(sh_c, grad_sh) if sh_c is not None else None
-            grad_nm = torch.empty_like(nm_c) if ctx.need_nm_grad else None
-            grad_tg = torch.empty_like(tg_c) if ctx.need_tg_grad else None
-            na = _normal_map_args(nm_c, tg_c, grad_nm, grad_tg) if nm_c is not None else None
-            grad_sm = torch.empty_like(sm_c) if ctx.need_sm_grad else None
-            qa = _specular_map_args(sm_c, grad_sm) if sm_c is not None else None
+            grad_phong = [torch.empty_like(t) if need else None for t, need in zip(phong_c, ctx.need_phong_grad)]
+            phong_structs = _phong_structs(phong_c, grad_phong) if phong_c[0] is not None else None
             ws_bytes = lib.nr_b200_backward_workspace_bytes(B, F, cfg.S, ctx.ts, flags)
             ws = torch.empty((max(ws_bytes, 16),), dtype=torch.uint8, device=dev)
             a = _lib.BackwardArgs()
@@ -504,14 +465,8 @@ class _RasterizeFunction(torch.autograd.Function):
             hook = _TEXTURE_GRAD_HOOK if (want_rgb and g_rgb is not None) else None
 
             def call():
-                if qa is not None:  # specular map: grad_specular_map is filled by the texture half too
-                    return lib.nr_b200_backward_specular_map(ctypes.byref(a), ctypes.byref(ph), _byref(la), _byref(sa),
-                                                             _byref(na), ctypes.byref(qa), _stream_ptr(dev))
-                if na is not None:  # normal map: grad_normal_map, grad_corner_tangents are filled by the texture half too
-                    return lib.nr_b200_backward_normal_map(ctypes.byref(a), ctypes.byref(ph), _byref(la), _byref(sa),
-                                                           ctypes.byref(na), _stream_ptr(dev))
-                if ph is not None:  # Phong: grad_corner_shading, grad_params, grad_lights, grad_sh are filled by the texture half
-                    return lib.nr_b200_backward_sh(ctypes.byref(a), ctypes.byref(ph), _byref(la), _byref(sa), _stream_ptr(dev))
+                if phong_structs is not None:  # Phong: every Phong input's gradient is filled by the texture half
+                    return lib.nr_b200_backward_specular_map(ctypes.byref(a), *phong_structs, _stream_ptr(dev))
                 if corner_c is None:
                     return lib.nr_b200_backward(ctypes.byref(a), _stream_ptr(dev))
                 # smooth shading: grad_corner_light is filled by the texture half
@@ -530,12 +485,24 @@ class _RasterizeFunction(torch.autograd.Function):
                 _lib.check(call())
                 if pending is not None:
                     pending.wait()
-        return (grad_geom, grad_textures, grad_light, None, None, grad_uvs, grad_corner, grad_cs, grad_sp, grad_lt, grad_sh,
-                grad_nm, grad_tg, grad_sm)
+        return (grad_geom, grad_textures, grad_light, None, None, grad_uvs, grad_corner, *grad_phong)
 
 
-def _byref(s):
-    return ctypes.byref(s) if s is not None else None
+# The Phong inputs in the order of the C ABI (nr_b200_forward_specular_map), with the dimensions each has without a batch
+# axis: corner_shading, shading_params, lights, environment_sh, normal_map, corner_tangents, specular_map
+_PHONG_DIMS = (3, 1, 2, 2, 3, 3, 3)
+
+
+def _phong_structs(t, g=(None,) * 7):
+    """The five struct arguments of nr_b200_*_specular_map for the Phong inputs t (and their gradient buffers g), NULL
+    where an input is absent: each NULL trailing struct makes the call exactly the narrower entry point's."""
+    cs, sp, lt, sh, nm, tg, sm = t
+    g_cs, g_sp, g_lt, g_sh, g_nm, g_tg, g_sm = g
+    return (ctypes.byref(_phong_args(cs, sp, g_cs, g_sp)),
+            ctypes.byref(_lights_args(lt, g_lt)) if lt is not None else None,
+            ctypes.byref(_sh_args(sh, g_sh)) if sh is not None else None,
+            ctypes.byref(_normal_map_args(nm, tg, g_nm, g_tg)) if nm is not None else None,
+            ctypes.byref(_specular_map_args(sm, g_sm)) if sm is not None else None)
 
 
 def _batched(t, batch_size, dims=None):
@@ -643,7 +610,7 @@ def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_
                          "derivative would cross items.  Pass reference_exact=False (or set_reference_exact(False))")
     _check_inputs(faces, textures, return_rgb, face_light, textures_fill_back, vertices, face_uvs, corner_light,
                   corner_shading, shading_params, lights, environment_sh, normal_map, corner_tangents, specular_map)
-    phong = corner_shading is not None
+    phong = [corner_shading, shading_params, lights, environment_sh, normal_map, corner_tangents, specular_map]
     indices = None
     if vertices is not None:
         geom = vertices if vertices.dtype == torch.float32 else vertices.float()
@@ -656,26 +623,16 @@ def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_
     batch_size = geom.shape[0]
     if not return_rgb:
         face_uvs = None
+        phong = [None] * len(_PHONG_DIMS)
     if return_rgb:
         # a texture image [Ht,Wt,3] (with face_uvs) is one image for every item; shared sets are read in place
-        # (NR_TEX_SHARED, NR_UV_SHARED, Bc / Bp / Bl / Bs = 1)
+        # (NR_TEX_SHARED, NR_UV_SHARED, and a batch of 1 for each Phong input)
         textures = _batched(textures, batch_size, 3 if face_uvs is not None else None)
         if face_uvs is not None:
             face_uvs = _batched(face_uvs, batch_size, 3)
-        if phong:
-            corner_shading = _batched(corner_shading, batch_size, 3)
-            shading_params = _batched(shading_params, batch_size, 1)
-            if lights is not None:
-                lights = _batched(lights, batch_size, 2)
-                if lights.shape[1] == 0:
-                    lights = None  # no extra light: Phong exactly
-            if environment_sh is not None:
-                environment_sh = _batched(environment_sh, batch_size, 2)
-            if normal_map is not None:
-                normal_map = _batched(normal_map, batch_size, 3)
-                corner_tangents = _batched(corner_tangents, batch_size, 3)
-            if specular_map is not None:
-                specular_map = _batched(specular_map, batch_size, 3)
+        phong = [_batched(t, batch_size, dims) if t is not None else None for t, dims in zip(phong, _PHONG_DIMS)]
+        if phong[2] is not None and phong[2].shape[1] == 0:
+            phong[2] = None  # lights: no extra light is Phong exactly
     cfg = _make_config(image_size, anti_aliasing, near, far, eps, background_color, return_rgb, return_alpha,
                        return_depth, geom.device, batch_size, reference_exact)
     if return_rgb and textures_fill_back:
@@ -690,10 +647,7 @@ def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_
         cfg.flags |= _lib.NR_TEX_MIPMAP
         textures = _MipPyramid.apply(textures)
     return _RasterizeFunction.apply(geom, textures if return_rgb else None, face_light if return_rgb else None, cfg,
-                                    indices, face_uvs, corner_light, corner_shading if return_rgb else None,
-                                    shading_params if return_rgb else None, lights if return_rgb else None,
-                                    environment_sh if return_rgb else None, normal_map if return_rgb else None,
-                                    corner_tangents if return_rgb else None, specular_map if return_rgb else None)
+                                    indices, face_uvs, corner_light, *phong)
 
 
 def rasterize_rgbad(
