@@ -108,7 +108,6 @@ constexpr int kStripBytesDefault = 16 * 1024; // shared memory budget for the st
 struct BwdParams {
     nr::FaceSrc src;
     nr::FaceGrad dst;
-    size_t tex_bstride;  // cubes per batch item in textures / grad_textures (0 with NR_TEX_SHARED)
     const int32_t* fim;
     const float* wmap;
     const float* dmap;
@@ -121,8 +120,7 @@ struct BwdParams {
     const int* strip_cnt;   // [B*2*(nstrips+1)]  faces per (item, axis, strip); slot nstrips = faces wider than kWideStrips
     const int* strip_off;   // exclusive prefix of strip_cnt
     const int* strip_list;  // face indices, grouped by (item, axis, strip)
-    float* grad_textures;
-    const float* textures;
+    float* grad_textures;   // the layout of tex.tex
     float* grad_face_light;
     float* grad_corner_light;  // d loss / d corner_light (the kLightCorner variants), or nullptr
     int B, F, S, ts, nchunks;
@@ -138,16 +136,10 @@ struct BwdParams {
     int debug_skip; // ablation knob of experiment builds (NR_B200_ES_SKIP): 1 = no in-scan, 2 = no out-scan, 4 = no task processing
 #endif
     uint32_t flags;
-    float eps, two_over_S, tex_cmp, tex_val;
-    // NR_TEX_UV (appended, so the cube variants keep their parameter offsets): textures / grad_textures = image [Bt,Ht,Wt,3]
-    const float* uvs;
-    uint32_t uv_bstride, img_bstride;  // floats per item (0 = shared)
-    int Ht, Wt;
-    // NR_TEX_MIPMAP (appended likewise): textures / grad_textures = the packed pyramid [Bt,P,3]
-    nr::MipTable mip;
-    // d loss / d face_uvs (appended likewise): the layout of `uvs` (uv_bstride floats per item), or nullptr
-    float* grad_uvs;
-    // what lights the pixel (appended likewise): face_light, corner_light or the Phong inputs of the call's light mode
+    float eps, two_over_S;
+    nr::Texture tex;  // what the pixel samples
+    float* grad_uvs;  // d loss / d face_uvs (the layout of tex.uvs), or nullptr
+    // what lights the pixel: face_light, corner_light or the Phong inputs of the call's light mode
     nr::Shading shading;
 };
 
@@ -1019,7 +1011,7 @@ __global__ void __launch_bounds__(256, kTgCombine ? (kLight >= nr::kLightCorner 
             z1 = __ldg(nr::face_vertex_t<true>(p.src, zb, fn, 1) + 2);
             z2 = __ldg(nr::face_vertex_t<true>(p.src, zb, fn, 2) + 2);
         }
-        const nr::TexCoord tc = nr::texture_coords(w, zp, z0, z1, z2, ts, p.tex_cmp, p.tex_val);
+        const nr::TexCoord tc = nr::texture_coords(w, zp, z0, z1, z2, ts, p.tex.tex_cmp, p.tex.tex_val);
         float lam[3] = {0.0f, 0.0f, 0.0f}, L[3];  // kCorner / kPhong: perspective weights (own depths) and light of the pixel
         if constexpr (kCorner || kPhong) {  // l_k with the item's own depths (NR_TEX_Z_BATCH0 only moves the cube coordinates)
             float oz[3] = {z0, z1, z2};
@@ -1030,25 +1022,18 @@ __global__ void __launch_bounds__(256, kTgCombine ? (kLight >= nr::kLightCorner 
             nr::perspective_weights(w, zp, oz[0], oz[1], oz[2], lam);
             nr::pixel_light<kLight>(p.shading, b, p.F, fn, lam, 0.0f, 0.0f, L);  // no uv: the cube modes have no map
         }
-        // NR_TEX_FILL_BACK: the reversed copy of face f - F/2 shares that face's cube, axes reversed
+        // NR_TEX_FILL_BACK as nr::stored_face, written out: through the helper nvcc allocates this kernel's registers
+        // differently (+8 instructions)
         int cube = fn, ncubes = p.F;
         bool rev = false;
         if (p.flags & NR_TEX_FILL_BACK) {
             ncubes = p.F >> 1;
             if (fn >= ncubes) { cube = fn - ncubes; rev = true; }
         }
-        const size_t cube_off = ((size_t)b * p.tex_bstride + cube) * (size_t)(ts * ts * ts) * 3;
+        const size_t cube_off = p.tex.cube_off(b, cube, ts);
         if (want_light) {  // unlit sample (same blend as the forward pass) times the upstream gradient
-            const float* tex = p.textures + cube_off;
-            float r = 0.0f, g = 0.0f, bl = 0.0f;
-#pragma unroll
-            for (int pn = 0; pn < 8; pn++) {
-                const float cw = nr::corner_weight(tc, pn);
-                const float* t = tex + (rev ? nr::corner_index_rev(tc, pn, ts) : nr::corner_index(tc, pn, ts)) * 3;
-                r = __fmaf_rn(cw, __ldg(t + 0), r);
-                g = __fmaf_rn(cw, __ldg(t + 1), g);
-                bl = __fmaf_rn(cw, __ldg(t + 2), bl);
-            }
+            float r, g, bl;
+            nr::cube_blend<false, true>(p.tex.tex + cube_off, tc, ts, rev, nullptr, r, g, bl);
             if constexpr (kCorner) {
                 const float s3[3] = {r, g, bl};
                 corner_light_grad(s3, g0, g1, g2, lam, glc);
@@ -1218,32 +1203,19 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
             z1 = __ldg(nr::face_vertex_t<true>(p.src, b, fn, 1) + 2);
             z2 = __ldg(nr::face_vertex_t<true>(p.src, b, fn, 2) + 2);
         }
-        int uf = fn;
-        bool rev = false;
-        if (p.flags & NR_TEX_FILL_BACK) {
-            const int half = p.F >> 1;
-            if (fn >= half) { uf = fn - half; rev = true; }
-        }
+        bool rev;
+        const int uf = nr::stored_face(p.flags & NR_TEX_FILL_BACK, p.F, fn, rev);
         float uv[6], u, v;
-        nr::load_face_uvs(p.uvs + ((uint32_t)b * p.uv_bstride + (uint32_t)uf * 6u), rev, uv);
+        nr::face_uvs(p.tex, b, uf, rev, uv);
         nr::pixel_uv(w, zp, z0, z1, z2, uv, u, v);
         float lam[3] = {0.0f, 0.0f, 0.0f}, L[3];  // kCorner / kPhong: perspective weights and light of the pixel
         if constexpr (kCorner || kPhong) {
             nr::perspective_weights(w, zp, z0, z1, z2, lam);
             nr::pixel_light<kLight>(p.shading, b, p.F, fn, lam, u, v, L);
         }
-        const uint32_t img_off = (uint32_t)b * p.img_bstride;
-        // level(s) and their weights: the bilinear variant is level 0 of an image with weight 1
-        int lv[2] = {0, 0};
-        float lw[2] = {1.0f, 0.0f};
-        int nlev = 1;
-        if constexpr (kMip) {
-            const nr::MipLevels m = nr::mip_levels(nr::mip_lod(inv, w, zp, z0, z1, z2, uv, p.Ht, p.Wt, p.mip.levels), p.mip.levels);
-            lv[0] = m.l0; lv[1] = m.l1;
-            lw[0] = __fsub_rn(1.0f, m.f); lw[1] = m.f;
-            nlev = m.f != 0.0f ? 2 : 1;
-        }
-        const nr::UvTaps t0 = nr::uv_taps(u, v, kMip ? p.mip.h[lv[0]] : p.Ht, kMip ? p.mip.w[lv[0]] : p.Wt);
+        const uint32_t img_off = p.tex.img_off(b);
+        const nr::LevelPair lp = nr::level_pair<kMip>(p.tex, inv, w, zp, z0, z1, z2, uv);
+        const nr::UvTaps t0 = nr::uv_taps(u, v, p.tex.level_h<kMip>(lp.l[0]), p.tex.level_w<kMip>(lp.l[0]));
         if constexpr (kUvGrad) {
             float lt[3] = {1.0f, 1.0f, 1.0f};
             if constexpr (kCorner || kPhong) {
@@ -1253,21 +1225,8 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
                 lt[0] = __ldg(lp); lt[1] = __ldg(lp + 1); lt[2] = __ldg(lp + 2);
             }
             const float h[3] = {g0 * lt[0], g1 * lt[1], g2 * lt[2]};  // d loss / d unlit tap value, per unit weight
-            float c[3], gu = 0.0f, gv = 0.0f;
-#pragma unroll
-            for (int q = 0; q < 2; q++) {
-                if (q >= nlev) break;
-                const int Hl = kMip ? p.mip.h[lv[q]] : p.Ht, Wl = kMip ? p.mip.w[lv[q]] : p.Wt;
-                const nr::UvTaps t = q == 0 ? t0 : nr::uv_taps(u, v, Hl, Wl);
-                float bl[3], du[3], dv[3];
-                nr::uv_blend_grad(p.textures + img_off + (kMip ? p.mip.off[lv[q]] : 0u), Hl, Wl, t, bl, du, dv);
-#pragma unroll
-                for (int k = 0; k < 3; k++) c[k] = q == 0 ? bl[k] : __fmaf_rn(lw[1], bl[k], __fmul_rn(lw[0], c[k]));  // mip_blend
-                const float eu = __fmaf_rn(h[2], du[2], __fmaf_rn(h[1], du[1], __fmul_rn(h[0], du[0])));
-                const float ev = __fmaf_rn(h[2], dv[2], __fmaf_rn(h[1], dv[1], __fmul_rn(h[0], dv[0])));
-                gu = __fmaf_rn(lw[q], eu, gu);
-                gv = __fmaf_rn(lw[q], ev, gv);
-            }
+            float c[3], gu, gv;
+            nr::image_sample_grad<kMip>(p.tex, p.tex.tex + img_off, lp, t0, u, v, h, c, gu, gv);
             if constexpr (kCorner) {
                 if (want_light) corner_light_grad(c, g0, g1, g2, lam, glc);
             } else {
@@ -1280,16 +1239,16 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
             uvg[0] = __fmul_rn(s0, gu); uvg[1] = __fmul_rn(s0, gv);
             uvg[2] = __fmul_rn(l1, gu); uvg[3] = __fmul_rn(l1, gv);
             uvg[4] = __fmul_rn(s2, gu); uvg[5] = __fmul_rn(s2, gv);
-            uv_at = (uint32_t)b * p.uv_bstride + (uint32_t)uf * 6u;
+            uv_at = p.tex.uv_off(b, uf);
         }
         if (!kUvGrad && want_light) {  // unlit sample (same blend as the forward pass) times the upstream gradient
             float c[3];
             if constexpr (kMip) {
                 nr::MipLevels m;
-                m.l0 = lv[0]; m.l1 = lv[1]; m.f = lw[1];
-                nr::mip_blend<false>(p.textures + img_off, p.mip, m, u, v, 1.0f, 1.0f, 1.0f, c);
+                m.l0 = lp.l[0]; m.l1 = lp.l[1]; m.f = lp.a[1];
+                nr::mip_blend<false>(p.tex.tex + img_off, p.tex.mip, m, u, v, 1.0f, 1.0f, 1.0f, c);
             } else {
-                nr::uv_blend<false>(p.textures + img_off, p.Wt, t0, 1.0f, 1.0f, 1.0f, c);
+                nr::uv_blend<false>(p.tex.tex + img_off, p.tex.Wt, t0, 1.0f, 1.0f, 1.0f, c);
             }
             if constexpr (kCorner) corner_light_grad(c, g0, g1, g2, lam, glc);
             else { gl0 = c[0] * g0; gl1 = c[1] * g1; gl2 = c[2] * g2; }
@@ -1303,9 +1262,9 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
         float* gi = p.grad_textures + img_off;
 #pragma unroll
         for (int q = 0; q < kPairs / 2; q++) {
-            if (q >= nlev) break;
-            const int Hl = kMip ? p.mip.h[lv[q]] : p.Ht, Wl = kMip ? p.mip.w[lv[q]] : p.Wt;
-            const uint32_t loff = kMip ? p.mip.off[lv[q]] : 0u;
+            if (q >= lp.n) break;
+            const int Hl = p.tex.level_h<kMip>(lp.l[q]), Wl = p.tex.level_w<kMip>(lp.l[q]);
+            const uint32_t loff = p.tex.level_off<kMip>(lp.l[q]);
             const nr::UvTaps t = q == 0 ? t0 : nr::uv_taps(u, v, Hl, Wl);
             const uint32_t row3 = (uint32_t)Wl * 3u;
             tp[2 * q] = gi + loff + (uint32_t)t.r0 * row3 + (uint32_t)t.x0 * 3u;
@@ -1313,8 +1272,8 @@ __device__ __forceinline__ void image_grad(const BwdParams& p) {
             adjacent[q] = t.x1 != t.x0;
             const long long k = (long long)((img_off + loff) / 3u) + t.cell;
             if (q == 0) key = k; else key1 = k;
-            const float h0 = kMip ? __fmul_rn(lw[q], g0) : g0, h1 = kMip ? __fmul_rn(lw[q], g1) : g1,
-                        h2 = kMip ? __fmul_rn(lw[q], g2) : g2;
+            const float h0 = kMip ? __fmul_rn(lp.a[q], g0) : g0, h1 = kMip ? __fmul_rn(lp.a[q], g1) : g1,
+                        h2 = kMip ? __fmul_rn(lp.a[q], g2) : g2;
             float* v0 = val[2 * q];
             float* v1 = val[2 * q + 1];
             v0[0] = t.w00 * h0; v0[1] = t.w00 * h1; v0[2] = t.w00 * h2;
@@ -1478,12 +1437,6 @@ __global__ void __launch_bounds__(256) k_depth_grad(const __grid_constant__ BwdP
     }
 }
 
-inline float float_le(double d) {
-    float f = (float)d;
-    if ((double)f > d) f = nextafterf(f, -INFINITY);
-    return f;
-}
-
 template <int kMode, int kT, bool kIdx, bool kCol>
 int launch_edge_scan_c(const BwdParams& p, int nstrips, size_t smem, cudaStream_t stream) {
     static nr_internal::SmemOptIn optin;
@@ -1594,17 +1547,17 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
     if (part_faces && !nr_internal::make_face_grad(flags, a->grad_faces, a->grad_vertices, a->face_indices, F, a->num_vertices, &dst))
         return NR_ERR_INVALID_ARG;
     const bool rgb = (flags & NR_RETURN_RGB) != 0, alpha = (flags & NR_RETURN_ALPHA) != 0, depth = (flags & NR_RETURN_DEPTH) != 0;
-    const bool uv = (flags & NR_TEX_UV) != 0;
-    if (uv && (!rgb || !a->face_uvs || a->texture_height < 1 || a->texture_width < 1)) return NR_ERR_INVALID_ARG;
-    const bool mip = (flags & NR_TEX_MIPMAP) != 0;
-    if (mip && !uv) return NR_ERR_INVALID_ARG;
+    const bool uv = (flags & NR_TEX_UV) != 0, mip = (flags & NR_TEX_MIPMAP) != 0;
+    nr::Texture tex;
+    size_t tex_floats, uv_floats;  // of grad_textures and grad_face_uvs
+    const int tex_rc = nr_internal::make_texture(a, &tex, &tex_floats, &uv_floats);
+    if (tex_rc == NR_ERR_INVALID_ARG) return tex_rc;
     // d loss / d face_uvs: only for the texture-image sampler, and it reads the image (pyramid).  It has the layout of
-    // face_uvs, so the 32-bit UV offset check below covers it.
+    // face_uvs, so make_texture's 32-bit UV offset check covers it.
     const bool uv_grad = a->grad_face_uvs != nullptr;
     if (uv_grad && (!uv || !rgb || !a->textures)) return NR_ERR_INVALID_ARG;
-    if (rgb && (!a->rgb_map || (!uv && ts < 2))) return NR_ERR_INVALID_ARG;
+    if (rgb && !a->rgb_map) return NR_ERR_INVALID_ARG;
     if (rgb && part_tex && !a->grad_textures) return NR_ERR_INVALID_ARG;
-    if (rgb && (flags & NR_TEX_FILL_BACK) && (F & 1)) return NR_ERR_INVALID_ARG;
     if (rgb && a->grad_face_light && !a->textures) return NR_ERR_INVALID_ARG;
     nr::Shading shading;
     const int light = nr_internal::make_shading(rgb, a->face_light, corner_light, pc, B, F, &shading);
@@ -1642,24 +1595,13 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
     if ((flags & NR_ANTI_ALIASING) && (S & 1)) return NR_ERR_INVALID_ARG;
     if (S > 32767 || B > 65535) return NR_ERR_UNSUPPORTED;
     if ((size_t)B * F * 2 * kWideStrips >= (size_t)0x7FFFFFFF) return NR_ERR_UNSUPPORTED;  // 32-bit list offsets
-    const size_t ncubes = (flags & NR_TEX_FILL_BACK) ? (size_t)F / 2 : (size_t)F;
-    const size_t tex_items = (flags & NR_TEX_SHARED) ? 1 : (size_t)B;
-    // NR_TEX_UV: the image gradient [Bt,Ht,Wt,3], NR_TEX_MIPMAP: the pyramid gradient [Bt,P,3] (the zero-fill below and the
-    // edge scan's side fill are sized from it)
-    nr::MipTable mt{};
-    const size_t img_floats = mip ? nr::mip_table(a->texture_height, a->texture_width, &mt) * 3
-                                  : (uv ? (size_t)a->texture_height * (size_t)a->texture_width * 3 : 0);
-    const size_t uv_floats = ncubes * 6;
-    const size_t uv_items = (flags & NR_UV_SHARED) ? 1 : (size_t)B;
-    if (uv && (tex_items * img_floats > 0x7FFFFFFFull || uv_floats * uv_items > 0x7FFFFFFFull))
-        return NR_ERR_UNSUPPORTED;  // 32-bit image / UV offsets in the kernels
+    if (tex_rc != NR_OK) return tex_rc;  // 32-bit image / UV offsets
     if (nm && nr_internal::nm_floats(nm) * (size_t)nm->map_batch > 0x7FFFFFFFull) return NR_ERR_UNSUPPORTED;  // 32-bit map offsets
     if (sm && nr_internal::sm_floats(sm) * (size_t)sm->map_batch > 0x7FFFFFFFull) return NR_ERR_UNSUPPORTED;
     const size_t need = nr_b200_backward_workspace_bytes(B, F, S, ts, flags);
     if (!a->workspace || a->workspace_bytes < need || ((uintptr_t)a->workspace & 15)) return NR_ERR_WORKSPACE;
     cudaStream_t stream = (cudaStream_t)cuda_stream;
 
-    const size_t tex_floats = uv ? tex_items * img_floats : tex_items * ncubes * ts * ts * ts * 3;
     // When one call runs both halves, grad_textures is zero-filled by the CTAs of the edge scan (a side job of an
     // issue-bound kernel instead of a memset of its own) and K6 runs after the edge scan.  Separate halves (the caller wants
     // the texture gradient first, for a collective) and unaligned buffers keep the memset.
@@ -1681,7 +1623,7 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
             return NR_ERR_CUDA;
         if (part_tex && rgb && a->grad_face_light && cudaMemsetAsync(a->grad_face_light, 0, (size_t)B * F * 3 * sizeof(float), stream) != cudaSuccess)
             return NR_ERR_CUDA;
-        if (part_tex && uv_grad && cudaMemsetAsync(a->grad_face_uvs, 0, uv_items * uv_floats * sizeof(float), stream) != cudaSuccess)
+        if (part_tex && uv_grad && cudaMemsetAsync(a->grad_face_uvs, 0, uv_floats * sizeof(float), stream) != cudaSuccess)
             return NR_ERR_CUDA;
         if (part_tex && grad_corner_light &&
             cudaMemsetAsync(grad_corner_light, 0, (size_t)B * F * 9 * sizeof(float), stream) != cudaSuccess)
@@ -1694,26 +1636,16 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
 
     BwdParams p{};
     p.src = src; p.dst = dst;
-    p.tex_bstride = (flags & NR_TEX_SHARED) ? 0 : ncubes;
+    p.tex = tex;
     p.fim = a->face_index_map; p.wmap = a->weight_map; p.dmap = a->depth_map; p.rgb = a->rgb_map;
     p.g_rgb = rgb ? a->grad_rgb : nullptr; p.g_alpha = alpha ? a->grad_alpha : nullptr; p.g_depth = depth ? a->grad_depth : nullptr;
     p.grad_textures = a->grad_textures;
-    p.textures = a->textures; p.grad_face_light = rgb ? a->grad_face_light : nullptr;
+    p.grad_face_light = rgb ? a->grad_face_light : nullptr;
     p.B = B; p.F = F; p.S = S; p.ts = ts;
     p.flags = flags;
     p.eps = (float)a->eps;
     p.two_over_S = 2.0f / (float)S;
-    const double tmax = (double)(ts - 1) - a->eps;
-    p.tex_cmp = float_le(tmax);
-    p.tex_val = (float)tmax;
-    if (uv) {
-        p.uvs = a->face_uvs;
-        p.uv_bstride = (flags & NR_UV_SHARED) ? 0u : (uint32_t)uv_floats;
-        p.img_bstride = (flags & NR_TEX_SHARED) ? 0u : (uint32_t)img_floats;
-        p.Ht = a->texture_height; p.Wt = a->texture_width;
-        if (mip) p.mip = mt;
-        p.grad_uvs = a->grad_face_uvs;
-    }
+    if (uv) p.grad_uvs = a->grad_face_uvs;
     p.grad_corner_light = grad_corner_light;
     p.shading = shading;
     const dim3 pgrid((unsigned)(((size_t)S * S + 255) / 256), B);
@@ -1743,13 +1675,9 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
         if (!phong_grads) return;
         auto written = [&](int k) { return phong_out[k].floats ? phong_out[k].ptr : nullptr; };
         nr_internal::PhongGradLaunch pl{};
-        pl.args = a; pl.src = src; pl.shading = shading;
+        pl.args = a; pl.src = src; pl.shading = shading; pl.tex = tex;
         pl.grad = {written(0), written(1), written(2), written(3), written(4), written(5), written(6),
                    (nm || sm) ? a->grad_face_uvs : nullptr};
-        pl.tex_bstride = (flags & NR_TEX_SHARED) ? 0 : (uv ? img_floats : ncubes * (size_t)ts * ts * ts * 3);
-        pl.uv_bstride = p.uv_bstride;
-        pl.tex_cmp = p.tex_cmp; pl.tex_val = p.tex_val;
-        pl.mip = mip ? &mt : nullptr;
         nr_internal::launch_phong_grad(pl, stream);
     };
     // K6 first, unless its output buffer is zero-filled by the edge scan
@@ -1843,11 +1771,7 @@ static int backward_impl(const nr_b200_backward_args* args, const float* corner_
     }
     if (interior && p.g_rgb) {  // the interior term of the rgb image (nr_interior.cu), into the same face / vertex gradient
         nr_internal::InteriorLaunch il{};
-        il.args = a; il.src = src; il.dst = dst; il.shading = shading; il.light = light;
-        il.tex_bstride = (flags & NR_TEX_SHARED) ? 0 : (uv ? img_floats : ncubes * (size_t)ts * ts * ts * 3);
-        il.uv_bstride = p.uv_bstride;
-        il.tex_cmp = p.tex_cmp; il.tex_val = p.tex_val;
-        il.mip = mip ? &mt : nullptr;
+        il.args = a; il.src = src; il.dst = dst; il.shading = shading; il.tex = tex; il.light = light;
         nr_internal::launch_interior_grad(il, stream);
     }
     return cudaGetLastError() == cudaSuccess ? NR_OK : NR_ERR_CUDA;

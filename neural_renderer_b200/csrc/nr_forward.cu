@@ -93,8 +93,6 @@ constexpr uint32_t kStageBytes = 32 * 1024;  // shared memory of a k_resolve CTA
 
 struct FwdParams {
     nr::FaceSrc src;
-    size_t tex_bstride;  // cubes per batch item in `textures` (0 with NR_TEX_SHARED)
-    const float* textures;
     const float* bg_batch;
     unsigned long long* zbuf;  // [B,S,S] raster orientation (row = yi): ordered zp << 32 | face index, ~0 = empty
     float4* tab;               // [B,F,3] float4: {inv0..3}, {inv4..7}, {inv8, z0, z1, z2} of every drawn face
@@ -114,16 +112,10 @@ struct FwdParams {
     int B, F, S, ts, ngroups;
     int big_area;  // faces whose (clipped) pixel box is larger go through k_raster_big
     uint32_t flags;
-    float near_lo, far_cmp, far_val, tex_cmp, tex_val;
+    float near_lo, far_cmp, far_val;
     float bg[3];
-    // NR_TEX_UV (appended, so the cube variants keep their parameter offsets): `textures` is the image [Bt,Ht,Wt,3]
-    const float* uvs;      // face_uvs [B,F,3,2] / [F,3,2] (F/2 faces with NR_TEX_FILL_BACK)
-    uint32_t uv_bstride;   // floats per item in face_uvs (0 with NR_UV_SHARED)
-    uint32_t img_bstride;  // floats per item in the image (0 with NR_TEX_SHARED)
-    int Ht, Wt;
-    // NR_TEX_MIPMAP (appended likewise): `textures` is the packed pyramid, img_bstride its floats per item
-    nr::MipTable mip;
-    // what lights the pixel (appended likewise): face_light, corner_light or the Phong inputs of the call's light mode
+    nr::Texture tex;  // what the pixel samples
+    // what lights the pixel: face_light, corner_light or the Phong inputs of the call's light mode
     nr::Shading shading;
 };
 
@@ -421,30 +413,6 @@ struct PixelGeom {
     float zp, w[3];
 };
 
-template <bool kLit>
-__device__ __forceinline__ void blend_corners(const FwdParams& p, const nr::TexCoord& tc, const float* tex, bool rev, int b, int fn,
-                                              float& r, float& g, float& bl) {
-    const int ts = p.ts;
-    float l0 = 1.0f, l1 = 1.0f, l2 = 1.0f;
-    if (kLit) {
-        const float* lp = p.shading.face_light + p.shading.fl_off(b, p.F, fn);
-        l0 = __ldg(lp); l1 = __ldg(lp + 1); l2 = __ldg(lp + 2);
-    }
-    r = g = bl = 0.0f;
-#pragma unroll
-    for (int pn = 0; pn < 8; pn++) {
-        const float cw = nr::corner_weight(tc, pn);
-        const float* t = tex + (rev ? nr::corner_index_rev(tc, pn, ts) : nr::corner_index(tc, pn, ts)) * 3;
-        float t0 = t[0], t1 = t[1], t2 = t[2];
-        if (kLit) {  // lighting.py:52 texel * light, rounded like the materialised product
-            t0 = __fmul_rn(t0, l0); t1 = __fmul_rn(t1, l1); t2 = __fmul_rn(t2, l2);
-        }
-        r = __fmaf_rn(cw, t0, r);
-        g = __fmaf_rn(cw, t1, g);
-        bl = __fmaf_rn(cw, t2, bl);
-    }
-}
-
 // rasterize.py:389 -- the sampler's vertex depths come from batch item 0 (NR_TEX_Z_BATCH0: the table k_raster_faces
 // left), else from the winner's record
 __device__ __forceinline__ void sampler_depths(const FwdParams& p, int fn, const float4& cc, float& z0, float& z1, float& z2) {
@@ -455,15 +423,10 @@ __device__ __forceinline__ void sampler_depths(const FwdParams& p, int fn, const
     }
 }
 
-// cube of face fn (NR_TEX_FILL_BACK: the reversed copy of face f - F/2 samples that face's cube with reversed axes; with
-// NR_TEX_UV the same index picks the face's UV corners, reversed)
-__device__ __forceinline__ int face_cube(const FwdParams& p, int fn, bool& rev) {
-    rev = false;
-    if (p.flags & NR_TEX_FILL_BACK) {
-        const int ncubes = p.F >> 1;
-        if (fn >= ncubes) { rev = true; return fn - ncubes; }
-    }
-    return fn;
+// face fn's face_light (kLightFace; nullptr in the other modes, whose samples are unlit)
+template <int kLight>
+__device__ __forceinline__ const float* face_light_of(const FwdParams& p, int b, int fn) {
+    return kLight == nr::kLightFace ? p.shading.face_light + p.shading.fl_off(b, p.F, fn) : nullptr;
 }
 
 // one pixel, every texel straight from global memory (anti-aliased quads, texture sizes the bulk copy cannot stage);
@@ -492,9 +455,9 @@ __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigne
         if constexpr (kUV) {
             // the winner's own vertex depths (no batch-0 quirk); fill_back copies read face fn - F/2's corners reversed
             bool rev;
-            const int uf = face_cube(p, fn, rev);
+            const int uf = nr::stored_face(p.flags & NR_TEX_FILL_BACK, p.F, fn, rev);
             float uv[6];
-            nr::load_face_uvs(p.uvs + ((uint32_t)b * p.uv_bstride + (uint32_t)uf * 6u), rev, uv);
+            nr::face_uvs(p.tex, b, uf, rev, uv);
             nr::pixel_uv(w, zp, cc.y, cc.z, cc.w, uv, u, v);
             float l0 = 1.0f, l1 = 1.0f, l2 = 1.0f;
             if (kLight == nr::kLightFace) {
@@ -503,23 +466,23 @@ __device__ __forceinline__ Shaded shade_pixel(const FwdParams& p, int b, unsigne
             }
             float c[3];
             if constexpr (kMip) {
-                const float lod = nr::mip_lod(inv, w, zp, cc.y, cc.z, cc.w, uv, p.Ht, p.Wt, p.mip.levels);
-                nr::mip_blend<kLight == nr::kLightFace>(p.textures + (uint32_t)b * p.img_bstride, p.mip,
-                                                        nr::mip_levels(lod, p.mip.levels), u, v, l0, l1, l2, c);
+                const float lod = nr::mip_lod(inv, w, zp, cc.y, cc.z, cc.w, uv, p.tex.Ht, p.tex.Wt, p.tex.mip.levels);
+                nr::mip_blend<kLight == nr::kLightFace>(p.tex.tex + p.tex.img_off(b), p.tex.mip,
+                                                        nr::mip_levels(lod, p.tex.mip.levels), u, v, l0, l1, l2, c);
             } else {
-                const nr::UvTaps t = nr::uv_taps(u, v, p.Ht, p.Wt);
-                nr::uv_blend<kLight == nr::kLightFace>(p.textures + (uint32_t)b * p.img_bstride, p.Wt, t, l0, l1, l2, c);
+                const nr::UvTaps t = nr::uv_taps(u, v, p.tex.Ht, p.tex.Wt);
+                nr::uv_blend<kLight == nr::kLightFace>(p.tex.tex + p.tex.img_off(b), p.tex.Wt, t, l0, l1, l2, c);
             }
             o.r = c[0]; o.g = c[1]; o.b = c[2];
         } else {
             float z0, z1, z2;
             sampler_depths(p, fn, cc, z0, z1, z2);
             const int ts = p.ts;
-            const nr::TexCoord tc = nr::texture_coords(w, zp, z0, z1, z2, ts, p.tex_cmp, p.tex_val);
+            const nr::TexCoord tc = nr::texture_coords(w, zp, z0, z1, z2, ts, p.tex.tex_cmp, p.tex.tex_val);
             bool rev;
-            const int cube = face_cube(p, fn, rev);
-            const float* tex = p.textures + ((size_t)b * p.tex_bstride + cube) * (size_t)(ts * ts * ts) * 3;
-            blend_corners<kLight == nr::kLightFace>(p, tc, tex, rev, b, fn, o.r, o.g, o.b);
+            const int cube = nr::stored_face(p.flags & NR_TEX_FILL_BACK, p.F, fn, rev);
+            const float* tex = p.tex.tex + p.tex.cube_off(b, cube, ts);
+            nr::cube_blend<kLight == nr::kLightFace, false>(tex, tc, ts, rev, face_light_of<kLight>(p, b, fn), o.r, o.g, o.b);
         }
         if constexpr (kLight >= nr::kLightCorner) {  // the light of the pixel's l_k (own depths) on the unlit sample
             float l[3], c[3] = {o.r, o.g, o.b};
@@ -602,7 +565,7 @@ __global__ void __launch_bounds__(256, resolve_min_ctas(kAA, kTex, kLight)) k_re
         const bool covered = key != ~0ull;
         const int fn = (int)(uint32_t)(key & 0xFFFFFFFFull);
         bool rev = false;
-        const int cube = covered ? face_cube(p, fn, rev) : -1;
+        const int cube = covered ? nr::stored_face(p.flags & NR_TEX_FILL_BACK, p.F, fn, rev) : -1;
         const int left = __shfl_up_sync(0xffffffffu, cube, 1);
         const bool head = covered && (lane == 0 || cube != left);
         const uint32_t heads = __ballot_sync(0xffffffffu, head);
@@ -620,7 +583,7 @@ __global__ void __launch_bounds__(256, resolve_min_ctas(kAA, kTex, kLight)) k_re
         const int slot = base + __popc(heads & ((2u << lane) - 1u)) - 1;  // run of this pixel (2u << 31 wraps: all heads)
         const bool staged = covered && slot < nslots;
         if (tid == 0) mbar_arrive_expect_tx(&s_bar, (uint32_t)min(total, nslots) * cube_bytes);
-        const float* gtex = p.textures + ((size_t)b * p.tex_bstride + (covered ? cube : 0)) * (size_t)(ts * ts * ts) * 3;
+        const float* gtex = p.tex.tex + p.tex.cube_off(b, covered ? cube : 0, ts);
         float* stex = reinterpret_cast<float*>(stage_raw) + (size_t)(staged ? slot : 0) * (cube_bytes >> 2);
         if (head && staged) bulk_copy_g2s(stex, gtex, cube_bytes, &s_bar);
         if (col >= S) return;
@@ -642,7 +605,7 @@ __global__ void __launch_bounds__(256, resolve_min_ctas(kAA, kTex, kLight)) k_re
         nr::barycentric_weights(inv, (float)col, (float)yi, w);
         float z0, z1, z2;
         sampler_depths(p, fn, cc, z0, z1, z2);
-        const nr::TexCoord tc = nr::texture_coords(w, zp, z0, z1, z2, ts, p.tex_cmp, p.tex_val);
+        const nr::TexCoord tc = nr::texture_coords(w, zp, z0, z1, z2, ts, p.tex.tex_cmp, p.tex.tex_val);
         fim[o] = fn;
         dmap[o] = zp;
         wmap[o] = w[0]; wmap[o + plane] = w[1]; wmap[o + 2 * plane] = w[2];
@@ -650,9 +613,9 @@ __global__ void __launch_bounds__(256, resolve_min_ctas(kAA, kTex, kLight)) k_re
         float r, g, bl;
         if (staged) {
             mbar_wait(&s_bar, 0);
-            blend_corners<kLight == nr::kLightFace>(p, tc, stex, rev, b, fn, r, g, bl);
+            nr::cube_blend<kLight == nr::kLightFace, false>(stex, tc, ts, rev, face_light_of<kLight>(p, b, fn), r, g, bl);
         } else {
-            blend_corners<kLight == nr::kLightFace>(p, tc, gtex, rev, b, fn, r, g, bl);
+            nr::cube_blend<kLight == nr::kLightFace, false>(gtex, tc, ts, rev, face_light_of<kLight>(p, b, fn), r, g, bl);
         }
         rgb[o] = r; rgb[o + plane] = g; rgb[o + 2 * plane] = bl;
     } else if (!kAA) {
@@ -700,11 +663,6 @@ __global__ void __launch_bounds__(256, resolve_min_ctas(kAA, kTex, kLight)) k_re
     }
 }
 
-inline float float_le(double d) {  // largest float <= d
-    float f = (float)d;
-    if ((double)f > d) f = nextafterf(f, -INFINITY);
-    return f;
-}
 inline float float_ge(double d) {  // smallest float >= d
     float f = (float)d;
     if ((double)f < d) f = nextafterf(f, INFINITY);
@@ -762,15 +720,13 @@ static int forward_impl(const nr_b200_forward_args* args, const nr_internal::Pho
     if (!a->face_index_map || !a->weight_map || !a->depth_map) return NR_ERR_INVALID_ARG;
     nr::FaceSrc src{};
     if (!nr_internal::make_face_src(flags, a->faces, a->vertices, a->face_indices, F, a->num_vertices, &src)) return NR_ERR_INVALID_ARG;
-    const bool uv = (flags & NR_TEX_UV) != 0;
-    if (flags & NR_RETURN_RGB) {
-        if (!a->textures || !a->rgb_map || (!uv && ts < 2)) return NR_ERR_INVALID_ARG;
-        if ((flags & NR_TEX_FILL_BACK) && (F & 1)) return NR_ERR_INVALID_ARG;
-        if ((flags & NR_BG_PER_BATCH) && !a->background_batch) return NR_ERR_INVALID_ARG;
-    }
-    if (uv && (!(flags & NR_RETURN_RGB) || !a->face_uvs || a->texture_height < 1 || a->texture_width < 1)) return NR_ERR_INVALID_ARG;
-    const bool mip = (flags & NR_TEX_MIPMAP) != 0;
-    if (mip && !uv) return NR_ERR_INVALID_ARG;
+    const bool uv = (flags & NR_TEX_UV) != 0, mip = (flags & NR_TEX_MIPMAP) != 0;
+    if ((flags & NR_RETURN_RGB) && (!a->textures || !a->rgb_map || ((flags & NR_BG_PER_BATCH) && !a->background_batch)))
+        return NR_ERR_INVALID_ARG;
+    nr::Texture tex;
+    size_t tex_floats, uv_floats;
+    const int tex_rc = nr_internal::make_texture(a, &tex, &tex_floats, &uv_floats);
+    if (tex_rc == NR_ERR_INVALID_ARG) return tex_rc;
     nr::Shading shading;
     const int light = nr_internal::make_shading((flags & NR_RETURN_RGB) != 0, a->face_light, a->corner_light, pc, B, F, &shading);
     if (light < 0) return NR_ERR_INVALID_ARG;
@@ -779,14 +735,7 @@ static int forward_impl(const nr_b200_forward_args* args, const nr_internal::Pho
     if ((nm || sm) && !uv) return NR_ERR_INVALID_ARG;  // the maps are addressed by the pixel's uv
     if ((flags & NR_ANTI_ALIASING) && (S & 1)) return NR_ERR_INVALID_ARG;
     if (S > 32767 || B > 65535) return NR_ERR_UNSUPPORTED;  // 32-bit pixel offsets; batch = grid.z of the resolve pass
-    // NR_TEX_UV: image (NR_TEX_MIPMAP: pyramid) and UV offsets are 32-bit in the kernels
-    nr::MipTable mt{};
-    const size_t img_floats = mip ? nr::mip_table(a->texture_height, a->texture_width, &mt) * 3
-                                  : (uv ? (size_t)a->texture_height * (size_t)a->texture_width * 3 : 0);
-    const size_t uv_floats = (size_t)((flags & NR_TEX_FILL_BACK) ? F / 2 : F) * 6;
-    if (uv && (img_floats * ((flags & NR_TEX_SHARED) ? 1 : B) > 0x7FFFFFFFull ||
-               uv_floats * ((flags & NR_UV_SHARED) ? 1 : B) > 0x7FFFFFFFull))
-        return NR_ERR_UNSUPPORTED;
+    if (tex_rc != NR_OK) return tex_rc;  // 32-bit image / UV offsets
     if (nm && nr_internal::nm_floats(nm) * (size_t)nm->map_batch > 0x7FFFFFFFull) return NR_ERR_UNSUPPORTED;  // 32-bit map offsets
     if (sm && nr_internal::sm_floats(sm) * (size_t)sm->map_batch > 0x7FFFFFFFull) return NR_ERR_UNSUPPORTED;
     const size_t need = nr_b200_forward_workspace_bytes(B, F, S, ts, flags);
@@ -797,8 +746,8 @@ static int forward_impl(const nr_b200_forward_args* args, const nr_internal::Pho
 
     FwdParams p{};
     p.src = src;
-    p.tex_bstride = (flags & NR_TEX_SHARED) ? 0 : ((flags & NR_TEX_FILL_BACK) ? (size_t)F / 2 : (size_t)F);
-    p.textures = a->textures; p.bg_batch = a->background_batch;
+    p.tex = tex;
+    p.bg_batch = a->background_batch;
     p.shading = shading;
     p.big_cnt = (int*)(wsb + L.off_cnt);
     p.work_next = p.big_cnt + B;
@@ -807,13 +756,6 @@ static int forward_impl(const nr_b200_forward_args* args, const nr_internal::Pho
     p.tab = (float4*)(wsb + L.off_tab);
     p.big_list = (int*)(wsb + L.off_list);
     p.z0tab = ((flags & NR_RETURN_RGB) && (flags & NR_TEX_Z_BATCH0) && !uv) ? (float4*)(wsb + L.off_z0) : nullptr;
-    if (uv) {
-        p.uvs = a->face_uvs;
-        p.uv_bstride = (flags & NR_UV_SHARED) ? 0u : (uint32_t)uv_floats;
-        p.img_bstride = (flags & NR_TEX_SHARED) ? 0u : (uint32_t)img_floats;
-        p.Ht = a->texture_height; p.Wt = a->texture_width;
-        if (mip) p.mip = mt;
-    }
     p.fim = a->face_index_map; p.wmap = a->weight_map; p.dmap = a->depth_map; p.rgb = a->rgb_map; p.alpha = a->alpha_map;
     p.out_rgb = a->out_rgb; p.out_alpha = a->out_alpha; p.out_depth = a->out_depth;
     p.B = B; p.F = F; p.S = S; p.ts = ts; p.ngroups = (F + 31) / 32;
@@ -821,12 +763,9 @@ static int forward_impl(const nr_b200_forward_args* args, const nr_internal::Pho
     // the background only colours the RGB image: without NR_RETURN_RGB, background_batch is neither checked above nor
     // read (it may be NULL), so the resolve pass must not see NR_BG_PER_BATCH either
     p.flags = (flags & NR_RETURN_RGB) ? flags : (flags & ~NR_BG_PER_BATCH);
-    p.near_lo = float_le(a->near_);
+    p.near_lo = nr_internal::float_le(a->near_);
     p.far_cmp = fminf(float_ge(a->far_), (float)a->far_);
     p.far_val = (float)a->far_;
-    const double tmax = (double)(ts - 1) - a->eps;
-    p.tex_cmp = float_le(tmax);
-    p.tex_val = (float)tmax;
     p.bg[0] = a->background[0]; p.bg[1] = a->background[1]; p.bg[2] = a->background[2];
 
     {   // z-buffer = "empty" (~0), big-face counters = -1: one fill

@@ -31,14 +31,9 @@ struct InteriorParams {
     const int32_t* fim;     // [B,S,S]
     const float* wmap;      // [B,3,S,S]
     const float* g;         // grad_rgb [B,3,H,W] (API layout)
-    const float* textures;  // cubes [.,F',ts,ts,ts,3], image [.,Ht,Wt,3] or packed pyramid [.,P,3]
-    size_t tex_bstride;     // floats per item in textures (0 = shared)
-    const float* uvs;       // [.,F',3,2]
-    uint32_t uv_bstride;    // floats per item in uvs (0 = shared)
-    int S, F, ts, Ht, Wt;
+    int S, F, ts;
     int aa, fill_back;
-    float tex_cmp, tex_val;
-    nr::MipTable mip;  // kTex 2
+    nr::Texture tex;
     nr::Shading shading;  // face_light (kLightFace) or corner_light (kLightCorner)
 };
 
@@ -90,28 +85,22 @@ __global__ void __launch_bounds__(256) k_interior_grad(const __grid_constant__ I
             for (int k = 0; k < 9; k++) C[k] = __ldg(cp + k);
         }
         const float h[3] = {g[0] * L[0], g[1] * L[1], g[2] * L[2]};  // d loss / d unlit sample
-        // fill_back: face f >= F/2 is the reversed copy of face f - F/2 (cube axes / UV corners reversed)
-        int tf = fn;
-        bool rev = false;
-        if (p.fill_back) {
-            const int half = p.F >> 1;
-            if (fn >= half) { tf = fn - half; rev = true; }
-        }
+        bool rev;
+        const int tf = nr::stored_face(p.fill_back, p.F, fn, rev);
         float s[3];              // the unlit sample
         float D1, D2, P[3];      // the sampler's part of D_k = G_k - G_0 and P_m = sum_k l_k G_k - G_m
         if constexpr (kTex == 0) {
             const int ts = p.ts;
-            const nr::TexCoord tc = nr::texture_coords(w, zp, z[0], z[1], z[2], ts, p.tex_cmp, p.tex_val);
+            const nr::TexCoord tc = nr::texture_coords(w, zp, z[0], z[1], z[2], ts, p.tex.tex_cmp, p.tex.tex_val);
             float dt[3][3];
-            nr::cube_blend_axis_grad(p.textures + ((size_t)b * p.tex_bstride + (size_t)tf * (size_t)(ts * ts * ts) * 3), tc, ts,
-                                     rev, s, dt);
+            nr::cube_blend_axis_grad(p.tex.tex + p.tex.cube_off(b, tf, ts), tc, ts, rev, s, dt);
             const float fts1 = (float)(ts - 1);
             float G[3];
 #pragma unroll
             for (int k = 0; k < 3; k++) {
                 // the clamp gate of texture_coords on the unclamped coordinate (NaN -> 0)
                 const float t = __fmul_rn(__fmul_rn(w[k], fts1), __fdiv_rn(zp, z[k]));
-                const bool in = t >= 0.0f && t <= p.tex_cmp;
+                const bool in = t >= 0.0f && t <= p.tex.tex_cmp;
                 const float e = __fmaf_rn(h[2], dt[k][2], __fmaf_rn(h[1], dt[k][1], __fmul_rn(h[0], dt[k][0])));
                 G[k] = in ? __fmul_rn(fts1, e) : 0.0f;
             }
@@ -120,35 +109,15 @@ __global__ void __launch_bounds__(256) k_interior_grad(const __grid_constant__ I
 #pragma unroll
             for (int m = 0; m < 3; m++) P[m] = __fsub_rn(lg, G[m]);
         } else {
+            constexpr bool kMip = kTex == 2;
             float uv[6], u, vv;
-            nr::load_face_uvs(p.uvs + ((size_t)b * p.uv_bstride + (size_t)tf * 6u), rev, uv);
+            nr::face_uvs(p.tex, b, tf, rev, uv);
             nr::pixel_uv(w, zp, z[0], z[1], z[2], uv, u, vv);
-            const float* img = p.textures + (size_t)b * p.tex_bstride;
-            int lv[2] = {0, 0};
-            float lw[2] = {1.0f, 0.0f};
-            int nlev = 1;
-            if constexpr (kTex == 2) {
-                const nr::MipLevels m = nr::mip_levels(nr::mip_lod(inv, w, zp, z[0], z[1], z[2], uv, p.Ht, p.Wt, p.mip.levels),
-                                                       p.mip.levels);
-                lv[0] = m.l0; lv[1] = m.l1;
-                lw[0] = __fsub_rn(1.0f, m.f); lw[1] = m.f;
-                nlev = m.f != 0.0f ? 2 : 1;
-            }
             // gu = sum_l a_l sum_c h_c Du_c^l (gv alike): d loss / d u with the light folded in (image_grad's kUvGrad sum)
-            float gu = 0.0f, gv = 0.0f;
-#pragma unroll
-            for (int q = 0; q < 2; q++) {
-                if (q >= nlev) break;
-                const int Hl = kTex == 2 ? p.mip.h[lv[q]] : p.Ht, Wl = kTex == 2 ? p.mip.w[lv[q]] : p.Wt;
-                float bl[3], du[3], dv[3];
-                nr::uv_blend_grad(img + (kTex == 2 ? p.mip.off[lv[q]] : 0u), Hl, Wl, nr::uv_taps(u, vv, Hl, Wl), bl, du, dv);
-#pragma unroll
-                for (int k = 0; k < 3; k++) s[k] = q == 0 ? bl[k] : __fmaf_rn(lw[1], bl[k], __fmul_rn(lw[0], s[k]));
-                const float eu = __fmaf_rn(h[2], du[2], __fmaf_rn(h[1], du[1], __fmul_rn(h[0], du[0])));
-                const float ev = __fmaf_rn(h[2], dv[2], __fmaf_rn(h[1], dv[1], __fmul_rn(h[0], dv[0])));
-                gu = __fmaf_rn(lw[q], eu, gu);
-                gv = __fmaf_rn(lw[q], ev, gv);
-            }
+            const nr::LevelPair lp = nr::level_pair<kMip>(p.tex, inv, w, zp, z[0], z[1], z[2], uv);
+            const nr::UvTaps t0 = nr::uv_taps(u, vv, p.tex.level_h<kMip>(lp.l[0]), p.tex.level_w<kMip>(lp.l[0]));
+            float gu, gv;
+            nr::image_sample_grad<kMip>(p.tex, p.tex.tex + p.tex.img_off(b), lp, t0, u, vv, h, s, gu, gv);
             // G_k = gu u_k + gv v_k: differences of the UV corners (no fp32 cancellation for corners close together far
             // from 0), and sum_k l_k uv_k = the pixel's uv
             D1 = __fmaf_rn(gv, __fsub_rn(uv[3], uv[1]), __fmul_rn(gu, __fsub_rn(uv[2], uv[0])));
@@ -212,15 +181,11 @@ void launch_interior_grad(const InteriorLaunch& L, cudaStream_t stream) {
     memset(&p, 0, sizeof(p));
     p.src = L.src; p.dst = L.dst;
     p.fim = a->face_index_map; p.wmap = a->weight_map; p.g = a->grad_rgb;
-    p.textures = a->textures; p.tex_bstride = L.tex_bstride;
-    p.uvs = a->face_uvs; p.uv_bstride = L.uv_bstride;
+    p.tex = L.tex;
     p.shading = L.shading;
     p.S = a->raster_size; p.F = a->num_faces; p.ts = a->texture_size;
-    p.Ht = a->texture_height; p.Wt = a->texture_width;
     p.aa = (flags & NR_ANTI_ALIASING) ? 1 : 0;
     p.fill_back = (flags & NR_TEX_FILL_BACK) ? 1 : 0;
-    p.tex_cmp = L.tex_cmp; p.tex_val = L.tex_val;
-    if (L.mip) p.mip = *L.mip;
     const bool idx = (flags & NR_FACES_INDEXED) != 0;
     const int tex = (flags & NR_TEX_MIPMAP) ? 2 : (flags & NR_TEX_UV) ? 1 : 0;
     const dim3 grid((unsigned)(((size_t)p.S * p.S + 255) / 256), a->batch_size);

@@ -8,6 +8,7 @@
 #include "nr_geom.cuh"
 #include "nr_math.cuh"
 #include "nr_shading.cuh"
+#include "nr_texture.cuh"
 
 namespace nr_internal {
 
@@ -17,10 +18,7 @@ struct InteriorLaunch {
     nr::FaceGrad dst;
     nr::Shading shading;        // the call's face_light or corner_light (nr_internal::make_shading)
     int light;                  // its light mode: kLightNone, kLightFace or kLightCorner
-    size_t tex_bstride;         // floats per item in `textures` (0 = shared)
-    uint32_t uv_bstride;        // floats per item in face_uvs (0 = shared)
-    float tex_cmp, tex_val;     // the cube clamp thresholds of the forward
-    const nr::MipTable* mip;    // NR_TEX_MIPMAP: the pyramid's level table, else nullptr
+    nr::Texture tex;            // what the pixel samples (nr_internal::make_texture)
 };
 
 // one launch of k_interior_grad, adding d loss / d vertices through l_k into src / dst's gradient (faces half); launch

@@ -2,11 +2,14 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <math.h>
+
 #include <atomic>
 
 #include "nr_b200.h"
 #include "nr_geom.cuh"
 #include "nr_shading.cuh"
+#include "nr_texture.cuh"
 
 namespace nr_internal {
 // kernels launched by the last forward/backward call on this thread (nr_b200_last_launch_count)
@@ -149,6 +152,52 @@ inline int make_shading(bool rgb, const float* face_light, const float* corner_l
     if (phong) return nr::kLightPhong;
     if (corner_light) return nr::kLightCorner;
     return s->face_light ? nr::kLightFace : nr::kLightNone;
+}
+
+inline float float_le(double d) {  // largest float <= d
+    float f = (float)d;
+    if ((double)f > d) f = nextafterf(f, -INFINITY);
+    return f;
+}
+
+// The nr::Texture of a call from its ABI arguments (nr_b200_forward_args or nr_b200_backward_args), and the floats of
+// its whole texel and face_uvs buffers (the sizes of their gradients).  Returns NR_ERR_INVALID_ARG for a refused
+// combination: NR_TEX_UV without RGB, face_uvs or an image of at least 1 x 1; NR_TEX_MIPMAP without NR_TEX_UV; RGB cubes
+// with ts < 2; RGB with NR_TEX_FILL_BACK and an odd F.  Returns NR_ERR_UNSUPPORTED when the image or UV offsets do not
+// fit the kernels' 32 bits.  The caller returns NR_ERR_INVALID_ARG at once and NR_ERR_UNSUPPORTED after its own
+// NR_ERR_INVALID_ARG rules.
+template <class Args>
+inline int make_texture(const Args* a, nr::Texture* t, size_t* tex_floats, size_t* uv_floats) {
+    const uint32_t flags = a->flags;
+    const bool rgb = (flags & NR_RETURN_RGB) != 0, uv = (flags & NR_TEX_UV) != 0, mip = (flags & NR_TEX_MIPMAP) != 0;
+    const int B = a->batch_size, F = a->num_faces, ts = a->texture_size;
+    *t = nr::Texture{};
+    if (uv && (!rgb || !a->face_uvs || a->texture_height < 1 || a->texture_width < 1)) return NR_ERR_INVALID_ARG;
+    if (mip && !uv) return NR_ERR_INVALID_ARG;
+    if (rgb && !uv && ts < 2) return NR_ERR_INVALID_ARG;
+    if (rgb && (flags & NR_TEX_FILL_BACK) && (F & 1)) return NR_ERR_INVALID_ARG;
+    const size_t faces = (flags & NR_TEX_FILL_BACK) ? (size_t)F / 2 : (size_t)F;  // stored faces per item
+    const size_t tex_items = (flags & NR_TEX_SHARED) ? 1 : (size_t)B, uv_items = (flags & NR_UV_SHARED) ? 1 : (size_t)B;
+    t->tex = a->textures;
+    t->cube_bstride = (flags & NR_TEX_SHARED) ? 0 : faces;
+    const double tmax = (double)(ts - 1) - a->eps;
+    t->tex_cmp = float_le(tmax);
+    t->tex_val = (float)tmax;
+    *uv_floats = 0;
+    if (!uv) {
+        *tex_floats = tex_items * faces * ts * ts * ts * 3;
+        return NR_OK;
+    }
+    const size_t img_floats = mip ? nr::mip_table(a->texture_height, a->texture_width, &t->mip) * 3
+                                  : (size_t)a->texture_height * (size_t)a->texture_width * 3;
+    *tex_floats = tex_items * img_floats;
+    *uv_floats = uv_items * faces * 6;
+    if (*tex_floats > 0x7FFFFFFFull || *uv_floats > 0x7FFFFFFFull) return NR_ERR_UNSUPPORTED;
+    t->uvs = a->face_uvs;
+    t->uv_bstride = (flags & NR_UV_SHARED) ? 0u : (uint32_t)(faces * 6);
+    t->img_bstride = (flags & NR_TEX_SHARED) ? 0u : (uint32_t)img_floats;
+    t->Ht = a->texture_height; t->Wt = a->texture_width;
+    return NR_OK;
 }
 
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) is issued once per (kernel instantiation, device, size high-water

@@ -54,18 +54,13 @@ struct PhongParams {
     const float* wmap;      // [B,3,S,S]
     const float* dmap;      // [B,S,S]
     const float* g;         // grad_rgb [B,3,H,W] (API layout)
-    const float* textures;  // cubes [.,F',ts,ts,ts,3], image [.,Ht,Wt,3] or packed pyramid [.,P,3]
-    size_t tex_bstride;     // floats per item in textures (0 = shared)
-    const float* uvs;       // [.,F',3,2]
-    uint32_t uv_bstride;    // floats per item in uvs (0 = shared)
     float* grad_cs;         // the layouts of corner_shading, params, lights (kLights) and sh (kSH), or nullptr
     float* grad_prm;
     float* grad_lts;
     float* grad_sh;
-    int S, F, ts, Ht, Wt;
+    int S, F, ts;
     int aa, fill_back, z_batch0;
-    float tex_cmp, tex_val;
-    nr::MipTable mip;  // kTex 2
+    nr::Texture tex;
     nr::Shading shading;  // corner_shading, params, lights, sh and the maps
     float* grad_nm;       // kNM: the layouts of normal_map, corner_tangents and face_uvs, or nullptr
     float* grad_tg;
@@ -260,14 +255,10 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
         const float z[3] = {v[2], v[5], v[8]};
         float lam[3];
         nr::perspective_weights(w, zp, z[0], z[1], z[2], lam);
-        // fill_back: face f >= F/2 is the reversed copy of face f - F/2 (cube axes / UV corners reversed)
-        int tf = fn;
-        bool rev = false;
-        if (p.fill_back) {
-            const int half = p.F >> 1;
-            if (fn >= half) { tf = fn - half; rev = true; }
-        }
+        bool rev;
+        const int tf = nr::stored_face(p.fill_back, p.F, fn, rev);
         float s[3];  // the unlit sample, as the forward computes it
+        float uv[6];  // kTex 1 / 2: the face's UV corners
         if constexpr (kTex == 0) {
             const int ts = p.ts;
             float zt[3] = {z[0], z[1], z[2]};  // the sampler's depths: item 0's with NR_TEX_Z_BATCH0
@@ -275,38 +266,27 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
 #pragma unroll
                 for (int k = 0; k < 3; k++) zt[k] = __ldg(nr::face_vertex_t<kIdx>(p.src, 0, fn, k) + 2);
             }
-            const nr::TexCoord tc = nr::texture_coords(w, zp, zt[0], zt[1], zt[2], ts, p.tex_cmp, p.tex_val);
-            const float* tex = p.textures + ((size_t)b * p.tex_bstride + (size_t)tf * (size_t)(ts * ts * ts) * 3);
-            s[0] = s[1] = s[2] = 0.0f;
-#pragma unroll
-            for (int pn = 0; pn < 8; pn++) {
-                const float cw = nr::corner_weight(tc, pn);
-                const float* t = tex + (rev ? nr::corner_index_rev(tc, pn, ts) : nr::corner_index(tc, pn, ts)) * 3;
-                s[0] = __fmaf_rn(cw, __ldg(t), s[0]);
-                s[1] = __fmaf_rn(cw, __ldg(t + 1), s[1]);
-                s[2] = __fmaf_rn(cw, __ldg(t + 2), s[2]);
-            }
+            const nr::TexCoord tc = nr::texture_coords(w, zp, zt[0], zt[1], zt[2], ts, p.tex.tex_cmp, p.tex.tex_val);
+            nr::cube_blend<false, true>(p.tex.tex + p.tex.cube_off(b, tf, ts), tc, ts, rev, nullptr, s[0], s[1], s[2]);
         } else {
-            float uv[6], u, vv;
-            nr::load_face_uvs(p.uvs + ((size_t)b * p.uv_bstride + (size_t)tf * 6u), rev, uv);
+            float u, vv;
+            nr::face_uvs(p.tex, b, tf, rev, uv);
             nr::pixel_uv(w, zp, z[0], z[1], z[2], uv, u, vv);
-            const float* img = p.textures + (size_t)b * p.tex_bstride;
+            const float* img = p.tex.tex + p.tex.img_off(b);
             if constexpr (kTex == 2) {
                 const float fS = (float)S;
                 float inv[9];
                 nr::face_inverse(nr::to_pixel(v[0], fS), nr::to_pixel(v[1], fS), nr::to_pixel(v[3], fS), nr::to_pixel(v[4], fS),
                                  nr::to_pixel(v[6], fS), nr::to_pixel(v[7], fS), inv);
-                const float lod = nr::mip_lod(inv, w, zp, z[0], z[1], z[2], uv, p.Ht, p.Wt, p.mip.levels);
-                nr::mip_blend<false>(img, p.mip, nr::mip_levels(lod, p.mip.levels), u, vv, 1.0f, 1.0f, 1.0f, s);
+                const float lod = nr::mip_lod(inv, w, zp, z[0], z[1], z[2], uv, p.tex.Ht, p.tex.Wt, p.tex.mip.levels);
+                nr::mip_blend<false>(img, p.tex.mip, nr::mip_levels(lod, p.tex.mip.levels), u, vv, 1.0f, 1.0f, 1.0f, s);
             } else {
-                nr::uv_blend<false>(img, p.Wt, nr::uv_taps(u, vv, p.Ht, p.Wt), 1.0f, 1.0f, 1.0f, s);
+                nr::uv_blend<false>(img, p.tex.Wt, nr::uv_taps(u, vv, p.tex.Ht, p.tex.Wt), 1.0f, 1.0f, 1.0f, s);
             }
         }
         const float* prm = p.shading.prm + p.shading.prm_off(b);
         nr::PhongEval E;
         if constexpr (kNM || kSM) {  // the mapped normal (or n) in E.n and the specular sample, then the rest of phong_at
-            float uv[6];
-            nr::load_face_uvs(p.uvs + ((size_t)b * p.uv_bstride + (size_t)tf * 6u), rev, uv);
             nr::pixel_uv(w, zp, z[0], z[1], z[2], uv, nmu, nmv);
             nmtf = tf; nmrev = rev;
             if constexpr (kNM) {
@@ -446,7 +426,7 @@ __global__ void __launch_bounds__(256) k_phong_grad(const __grid_constant__ Phon
             }
             if constexpr (kNM || kSM) {
                 if (p.grad_uvs) {
-                    float* o = p.grad_uvs + ((size_t)b * p.uv_bstride + (size_t)nmtf * 6u);
+                    float* o = p.grad_uvs + p.tex.uv_off(b, nmtf);
 #pragma unroll
                     for (int k = 0; k < 6; k++) atomicAdd(o + k, cg[kUvAt<kNM> + k]);
                 }
@@ -483,16 +463,12 @@ void launch_phong_grad(const PhongGradLaunch& L, cudaStream_t stream) {
     memset(&p, 0, sizeof(p));
     p.src = L.src;
     p.fim = a->face_index_map; p.wmap = a->weight_map; p.dmap = a->depth_map; p.g = a->grad_rgb;
-    p.textures = a->textures; p.tex_bstride = L.tex_bstride;
-    p.uvs = a->face_uvs; p.uv_bstride = L.uv_bstride;
     p.grad_cs = L.grad.cs; p.grad_prm = L.grad.prm; p.grad_lts = L.grad.lts; p.grad_sh = L.grad.sh;
     p.S = a->raster_size; p.F = a->num_faces; p.ts = a->texture_size;
-    p.Ht = a->texture_height; p.Wt = a->texture_width;
     p.aa = (flags & NR_ANTI_ALIASING) ? 1 : 0;
     p.fill_back = (flags & NR_TEX_FILL_BACK) ? 1 : 0;
     p.z_batch0 = (flags & NR_TEX_Z_BATCH0) ? 1 : 0;
-    p.tex_cmp = L.tex_cmp; p.tex_val = L.tex_val;
-    if (L.mip) p.mip = *L.mip;
+    p.tex = L.tex;
     p.shading = L.shading;
     p.grad_nm = L.grad.nm; p.grad_tg = L.grad.tg; p.grad_uvs = L.grad.uvs; p.grad_sm = L.grad.sm;
     const bool idx = (flags & NR_FACES_INDEXED) != 0;

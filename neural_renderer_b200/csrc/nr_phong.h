@@ -8,6 +8,7 @@
 #include "nr_geom.cuh"
 #include "nr_math.cuh"
 #include "nr_shading.cuh"
+#include "nr_texture.cuh"
 
 namespace nr_internal {
 
@@ -23,10 +24,7 @@ struct PhongGradLaunch {
     nr::Shading shading;                // the call's Phong inputs (nr_internal::make_shading)
     PhongGrads grad;
     nr::FaceSrc src;
-    size_t tex_bstride;       // floats per item in `textures` (0 = shared)
-    uint32_t uv_bstride;      // floats per item in face_uvs (0 = shared)
-    float tex_cmp, tex_val;   // the cube clamp thresholds of the forward
-    const nr::MipTable* mip;  // NR_TEX_MIPMAP: the pyramid's level table, else nullptr
+    nr::Texture tex;                    // what the pixel samples (nr_internal::make_texture)
 };
 
 // one launch of k_phong_grad, adding into grad_corner_shading / grad_params (texture half); launch errors surface through
