@@ -513,6 +513,60 @@ typedef struct nr_b200_interpolate_args {
     float *grad_vertices;          /* backward: [B,Nv,3] or NULL; only with NR_FACES_INDEXED */
 } nr_b200_interpolate_args;
 
+/* Soft silhouettes (within ABI 4, additive): per-pixel coverage aggregated over every face within reach (SoftRas, Liu et
+ * al. 2019), with gradients into the vertices from every face a pixel reaches -- not only from the edges a hard pixel
+ * flips on.  Geometry as nr_b200_forward: faces [B,F,3,3], or vertices [B,Nv,3] + int32 face_indices [F,3] / [B,F,3]
+ * with NR_FACES_INDEXED (an index outside [0, Nv) reads the zero vertex); NDC x, y and camera z.
+ *   API pixel (r, c) of the S x S image (row 0 at the top, as the hard alpha): p = (x, y), x = (2c + 1 - S) / S,
+ *   y = (2 (S-1-r) + 1 - S) / S (div.rn; the hard rasterizer's pixel centres).  Face j:
+ *     takes part when every vertex depth satisfies near <= z <= far (fp32) and its x, y are finite; otherwise it is
+ *     skipped entirely.  (A per-face test: the hard rasterizer tests the interpolated depth per pixel.)
+ *     d_j^2 = min over its three edges (v_k, v_k+1) of the squared distance from p to the closed segment, NDC units
+ *     (t = clamp(((p - a) . e) / |e|^2, 0, 1), |e| = 0 gives t = 0);  inside_j = p strictly inside by the edge-function
+ *     signs, either winding (all three > 0 or all three < 0; a zero-area face has no inside);
+ *     x_j = +d_j^2 / sigma inside, -d_j^2 / sigma outside (fp32, d^2 * (1 / sigma));  D_j = sigmoid(x_j).
+ *     Cut-off: an outside face contributes only when d_j^2 <= sigma ln((1 - eps) / eps), i.e. D_j >= eps = NR_SOFT_EPS.
+ *   alpha = 1 - prod_j (1 - D_j) = -expm1(Lambda), Lambda = -sum_j softplus(x_j), softplus(x) = max(x,0) + log1p(exp(-|x|)).
+ *   The sum is taken in 64-bit fixed point (each term rounded to 2^-40, terms and sum saturated at 64, where alpha is
+ *   1.0f): integer adds do not depend on the order the faces arrive in, so alpha is bit-for-bit deterministic.
+ *   Winding does not matter, so pass each face once: a duplicated face (a fill_back copy) counts twice, 1 - (1 - D)^2.
+ *   Backward: d alpha / d x_j = (1 - alpha) D_j (exact, no division, from the saved alpha); d x_j / d(x, y) of the two
+ *   endpoints a, b of the nearest edge: +-(1/sigma) (-2 (1 - t)(p - q), -2 t (p - q)), q = a + t e the nearest point
+ *   (the subgradient of the active edge and segment branch; the cut-off is held fixed).  Every gradient into z is 0.
+ *   grad_faces [B,F,3,3] (materialised) or grad_vertices [B,Nv,3] (NR_FACES_INDEXED; shared indices reduce over the
+ *   items' own vertices, out-of-range indices are skipped), zero-filled first unless NR_GRAD_ACCUMULATE; grad_alpha NULL
+ *   = zeros.  fp32 atomics, not bit-pinned.
+ *   sigma > 0 and finite; 1e-5 gives a reach of sqrt(sigma ln((1-eps)/eps)) S / 2, about 1.2 pixels at S = 256.
+ *   Scratch: nr_b200_soft_workspace_bytes (both passes; the backward bins the faces again, nothing is kept between calls).
+ *   Host rejections (NR_ERR_INVALID_ARG, before any launch): struct_size != sizeof(nr_b200_soft_args), B, F or S < 1, a
+ *   non-finite or non-positive sigma, near > far (or NaN), missing geometry for the chosen form, a NULL alpha, in the
+ *   backward a NULL gradient output for the form or grad_faces with / grad_vertices without NR_FACES_INDEXED, and
+ *   B > 65535, S > 32767 or B F 16 > 2^31 - 1 (the grid, 16-bit tile boxes and 32-bit list offsets).  Then
+ *   NR_ERR_WORKSPACE for a missing, short or unaligned workspace. */
+#define NR_SOFT_EPS 1e-4
+
+typedef struct nr_b200_soft_args {
+    uint32_t struct_size; /* sizeof(nr_b200_soft_args) */
+    uint32_t flags;       /* NR_FACES_INDEXED / NR_INDICES_SHARED, NR_GRAD_ACCUMULATE (backward) */
+    int32_t batch_size;   /* B */
+    int32_t num_faces;    /* F */
+    int32_t image_size;   /* S */
+    int32_t num_vertices; /* Nv (NR_FACES_INDEXED) */
+    float sigma;          /* > 0 */
+    float near_;          /* faces with a vertex depth outside [near, far] take no part */
+    float far_;
+    int32_t _pad0;
+    const float *faces;          /* [B,F,3,3], or NULL with NR_FACES_INDEXED */
+    const float *vertices;       /* [B,Nv,3], NR_FACES_INDEXED only */
+    const int32_t *face_indices; /* [B,F,3], or [F,3] with NR_INDICES_SHARED */
+    float *alpha;                /* [B,S,S]: written by the forward, read by the backward */
+    const float *grad_alpha;     /* backward: [B,S,S] or NULL (zeros) */
+    float *grad_faces;           /* backward: [B,F,3,3]; not with NR_FACES_INDEXED */
+    float *grad_vertices;        /* backward: [B,Nv,3]; only with NR_FACES_INDEXED */
+    void *workspace;             /* nr_b200_soft_workspace_bytes() bytes, 16-byte aligned */
+    size_t workspace_bytes;
+} nr_b200_soft_args;
+
 /* ABI version of the loaded library (== NR_B200_ABI_VERSION it was built with). */
 NR_B200_API int nr_b200_abi_version(void);
 NR_B200_API const char *nr_b200_error_string(int code);
@@ -573,6 +627,12 @@ NR_B200_API int nr_b200_backward_specular_map(const nr_b200_backward_args *args,
  * interior vertex gradient.  One kernel launch each (plus the zero-fill of the backward). */
 NR_B200_API int nr_b200_interpolate(const nr_b200_interpolate_args *args, void *cuda_stream);
 NR_B200_API int nr_b200_interpolate_backward(const nr_b200_interpolate_args *args, void *cuda_stream);
+/* Soft silhouettes (nr_b200_soft_args above): alpha [B,S,S], and its backward into grad_faces / grad_vertices.  The
+ * workspace size is pure host arithmetic (0 for sizes or a sigma the calls refuse); `flags` is accepted for the future. */
+NR_B200_API size_t nr_b200_soft_workspace_bytes(int32_t batch_size, int32_t num_faces, int32_t image_size, float sigma,
+                                                uint32_t flags);
+NR_B200_API int nr_b200_soft_silhouettes(const nr_b200_soft_args *args, void *cuda_stream);
+NR_B200_API int nr_b200_soft_silhouettes_backward(const nr_b200_soft_args *args, void *cuda_stream);
 
 /* vertices_to_faces (reference vertices_to_faces.py:4-21), the step either side of the rasterizer:
  *   forward   out_faces[b,f,k,:] = vertices[b, faces[b,f,k], :]           ([B,Nv,3] x [B,Nf,3] int32 -> [B,Nf,3,3])

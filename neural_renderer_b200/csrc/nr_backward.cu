@@ -1471,6 +1471,11 @@ int launch_edge_scan(const BwdParams& p, int nstrips, size_t smem, cudaStream_t 
 
 }  // namespace
 
+void nr_internal::strip_scan(const int* cnt, int* off, int seg_len, long long seg_stride, int nseg, cudaStream_t stream) {
+    nr_internal::LaunchScope ls("k_strip_scan", stream);
+    k_strip_scan<<<nseg, 256, 0, stream>>>(cnt, off, seg_len, seg_stride);
+}
+
 namespace {
 struct BinLayout {
     int W, w_log2, nstrips;

@@ -24,6 +24,10 @@ struct LaunchScope {
     ~LaunchScope() { prof_end(s); launch_count()++; }
 };
 
+// Exclusive prefix sums of nseg segments of seg_len counters, segment i offset by i * seg_stride (k_strip_scan of
+// nr_backward.cu, also the tile scan of the soft silhouettes)
+void strip_scan(const int* cnt, int* off, int seg_len, long long seg_stride, int nseg, cudaStream_t stream);
+
 // FaceSrc / FaceGrad of a call from its ABI arguments; false = missing pointers for the chosen geometry form
 inline bool make_face_src(uint32_t flags, const float* faces, const float* vertices, const int32_t* indices, int F, int Nv,
                           nr::FaceSrc* s) {

@@ -1,0 +1,399 @@
+// nr_soft.cu -- soft silhouettes (nr_b200_soft_silhouettes / nr_b200_soft_silhouettes_backward, include/nr_b200.h).
+//
+// Every face gives every pixel within reach a probability D = sigmoid(+-d^2 / sigma) of the pixel's squared distance d^2
+// to the face (SoftRas), and alpha = 1 - prod_j (1 - D_j).  Both passes walk 16 x 16 pixel tiles:
+//
+//   k_soft_setup    one thread per face: the participation test (every vertex depth in [near, far]), the face record
+//                   (three edges {a, b - a, 1 / |b - a|^2}, 64 bytes) and the face's tile box -- its pixel box grown by the
+//                   cut-off reach plus one pixel -- and counts the face into each tile it overlaps (global atomics).
+//                   Faces spanning more than kWideTiles tiles are counted once, into the item's wide slot.
+//   k_strip_scan    the backward's segment scan (nr_backward.cu), one segment per item: tile counters -> list offsets.
+//   k_soft_fill     one thread per face: appends the face to the list of each tile it counted into (atomic cursors).
+//   k_soft_fwd      one CTA per (tile, item), one thread per pixel.  The tile's list, then the wide list with a box
+//                   test, are staged into shared memory 256 records at a time; every thread adds softplus(x_j) of its
+//                   pixel into a 64-bit fixed-point sum, so the list order the atomic fill left does not reach alpha: the
+//                   forward is bit-for-bit deterministic.  alpha = -expm1(-Lambda), one streaming store per pixel.
+//   k_soft_bwd      the same traversal with g (1 - alpha) per pixel: each face's 6 xy partials are reduced over the
+//                   warp (shuffles, only when a lane of the warp is within reach), then over the CTA (shared-memory
+//                   adds), and leave the CTA as one set of global atomics per face and tile through nr::FaceGrad.
+#include <cuda_runtime.h>
+#include <math.h>
+#include <stdint.h>
+#include <string.h>
+
+#include "nr_b200.h"
+#include "nr_internal.h"
+
+namespace {
+
+constexpr int kTile = 16;                   // tile side in pixels
+constexpr int kThreads = kTile * kTile;     // one thread per pixel of the tile
+constexpr int kWideTiles = 16;              // faces over more tiles go to the item's wide list (bounds the list storage)
+constexpr float kFix = 1099511627776.0f;    // 2^40: fixed-point scale of Lambda
+constexpr float kTermCap = 64.0f;           // softplus terms and Lambda saturate here: -expm1(-64) == 1.0f
+
+struct SoftParams {
+    nr::FaceSrc src;
+    nr::FaceGrad dst;
+    float4* rec;        // [B*F][4] face records: edge k = {ax, ay, ex, ey} in rec[k], rec[3] = {1/|e_0|^2, 1/|e_1|^2, 1/|e_2|^2, 0}
+    uint2* box;         // [B*F] tile box {tx_lo | tx_hi << 16, ty_lo | ty_hi << 16}; lo > hi = takes no part
+    int* cnt;           // [B*(ntiles+1)] faces per (item, tile); slot ntiles = the item's wide faces
+    int* cursor;        // [B*(ntiles+1)] fill cursors
+    int* off;           // [B*(ntiles+1)] list offsets (k_strip_scan)
+    int* list;          // [B*F*kWideTiles] face indices grouped by (item, tile)
+    float* alpha;       // [B,S,S]: written by the forward, read by the backward
+    const float* g;     // [B,S,S] upstream gradient
+    int B, F, S, ntx, ntiles;
+    float inv_sigma;    // 1 / sigma
+    float cut;          // sigma ln((1 - eps) / eps): an outside face contributes only when d^2 <= cut
+    float reach;        // sqrt(cut) S / 2 + 1: the cut-off reach in pixels with one pixel of rounding guard
+    float near_, far_;
+};
+
+__device__ __forceinline__ uint32_t pack16(int lo, int hi) { return ((uint32_t)lo & 0xFFFFu) | ((uint32_t)hi << 16); }
+__device__ __forceinline__ int lo16(uint32_t v) { return (int)(short)(v & 0xFFFFu); }
+__device__ __forceinline__ int hi16(uint32_t v) { return (int)(short)(v >> 16); }
+
+// the pixel centre of the hard rasterizer (nr_forward.cu): NDC of raster column / row i
+__device__ __forceinline__ float soft_centre(int i, int S) { return __fdiv_rn((float)(2 * i + 1 - S), (float)S); }
+
+// ------------------------------------------------------------------------------------------------ k_soft_setup
+template <bool kFill>
+__global__ void __launch_bounds__(256) k_soft_setup(const __grid_constant__ SoftParams p) {
+    const int b = blockIdx.y;
+    const int f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= p.F) return;
+    const size_t id = (size_t)b * p.F + f;
+    uint2 bb;
+    if (kFill) {
+        bb = __ldg(p.box + id);
+    } else {
+        float v[9];
+        nr::load_face(p.src, b, f, v);
+        bool part = true;
+#pragma unroll
+        for (int k = 0; k < 3; k++) {
+            part = part && v[3 * k + 2] >= p.near_ && v[3 * k + 2] <= p.far_;
+            part = part && isfinite(v[3 * k]) && isfinite(v[3 * k + 1]);
+        }
+        const float S = (float)p.S, lim = (float)(p.S - 1);
+        // column of x: (x S + S - 1) / 2; row of y: S - 1 - (y S + S - 1) / 2 (row 0 at the top)
+        const float xmin = fminf(v[0], fminf(v[3], v[6])), xmax = fmaxf(v[0], fmaxf(v[3], v[6]));
+        const float ymin = fminf(v[1], fminf(v[4], v[7])), ymax = fmaxf(v[1], fmaxf(v[4], v[7]));
+        const float c0 = fmaxf(floorf(__fmaf_rn(xmin, S, lim) * 0.5f - p.reach), 0.0f);
+        const float c1 = fminf(ceilf(__fmaf_rn(xmax, S, lim) * 0.5f + p.reach), lim);
+        const float r0 = fmaxf(floorf(lim - __fmaf_rn(ymax, S, lim) * 0.5f - p.reach), 0.0f);
+        const float r1 = fminf(ceilf(lim - __fmaf_rn(ymin, S, lim) * 0.5f + p.reach), lim);
+        bb = make_uint2(pack16(1, 0), pack16(1, 0));
+        if (part && c0 <= c1 && r0 <= r1) {
+            bb = make_uint2(pack16((int)c0 / kTile, (int)c1 / kTile), pack16((int)r0 / kTile, (int)r1 / kTile));
+            float4* r = p.rec + id * 4;
+            float il[3];
+#pragma unroll
+            for (int k = 0; k < 3; k++) {
+                const int n = k == 2 ? 0 : k + 1;
+                const float ax = v[3 * k], ay = v[3 * k + 1];
+                const float ex = __fsub_rn(v[3 * n], ax), ey = __fsub_rn(v[3 * n + 1], ay);
+                const float l2 = __fmaf_rn(ex, ex, ey * ey);
+                il[k] = l2 > 0.0f ? __frcp_rn(l2) : 0.0f;  // a zero-length edge: t = 0, the distance to its point
+                r[k] = make_float4(ax, ay, ex, ey);
+            }
+            r[3] = make_float4(il[0], il[1], il[2], 0.0f);
+        }
+        p.box[id] = bb;
+    }
+    const int tx0 = lo16(bb.x), tx1 = hi16(bb.x), ty0 = lo16(bb.y), ty1 = hi16(bb.y);
+    if (tx0 > tx1) return;
+    int* seg = (kFill ? p.cursor : p.cnt) + (size_t)b * (p.ntiles + 1);
+    const int* segoff = p.off + (size_t)b * (p.ntiles + 1);
+    const int w = tx1 - tx0 + 1, n = w * (ty1 - ty0 + 1);
+    for (int i = 0; i < (n > kWideTiles ? 1 : n); i++) {
+        const int t = n > kWideTiles ? p.ntiles : (ty0 + i / w) * p.ntx + tx0 + i % w;
+        const int pos = atomicAdd(seg + t, 1);
+        if (kFill) p.list[segoff[t] + pos] = f;
+    }
+}
+
+// ------------------------------------------------------------------------------------------------ per-pixel terms
+// x_j of face record r at pixel p, or false when the face does not contribute (outside and beyond the cut-off).  With
+// it: the nearest edge k, its segment parameter t and p - q (q the nearest point), for the backward.
+__device__ __forceinline__ bool soft_term(const float4* r, float px, float py, float inv_sigma, float cut, float& x,
+                                          int& kb, float& tb, float& qxb, float& qyb) {
+    const float il[3] = {r[3].x, r[3].y, r[3].z};
+    float best = INFINITY, c[3];
+    kb = 0; tb = 0.0f; qxb = 0.0f; qyb = 0.0f;
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        const float4 e = r[k];
+        const float dx = __fsub_rn(px, e.x), dy = __fsub_rn(py, e.y);
+        const float t = fminf(fmaxf(__fmaf_rn(dx, e.z, dy * e.w) * il[k], 0.0f), 1.0f);
+        const float qx = __fmaf_rn(-t, e.z, dx), qy = __fmaf_rn(-t, e.w, dy);
+        const float d2 = __fmaf_rn(qx, qx, qy * qy);
+        c[k] = __fmaf_rn(e.z, dy, -(e.w * dx));  // edge function of edge k at p
+        if (d2 < best) { best = d2; kb = k; tb = t; qxb = qx; qyb = qy; }
+    }
+    const bool inside = (c[0] > 0.0f && c[1] > 0.0f && c[2] > 0.0f) || (c[0] < 0.0f && c[1] < 0.0f && c[2] < 0.0f);
+    if (!inside && best > cut) return false;
+    const float a = best * inv_sigma;
+    x = inside ? a : -a;
+    return true;
+}
+
+// Stages the next <= kThreads faces of the tile (its own list, then the wide list with a box test) into shared memory;
+// returns how many were staged.  `next` is the position in the concatenated list, advanced by kThreads.
+__device__ __forceinline__ int stage_faces(const SoftParams& p, int b, int tile, int tx, int ty, int n_tile, int n_all,
+                                           int next, float4* s_rec, int* s_face, int* s_n) {
+    const int tid = threadIdx.x;
+    if (tid == 0) *s_n = 0;
+    __syncthreads();
+    const int i = next + tid;
+    const size_t seg = (size_t)b * (p.ntiles + 1);
+    int f = -1;
+    if (i < n_tile) {
+        f = p.list[p.off[seg + tile] + i];
+    } else if (i < n_all) {
+        f = p.list[p.off[seg + p.ntiles] + (i - n_tile)];
+        const uint2 bb = __ldg(p.box + (size_t)b * p.F + f);
+        if (tx < lo16(bb.x) || tx > hi16(bb.x) || ty < lo16(bb.y) || ty > hi16(bb.y)) f = -1;
+    }
+    const unsigned m = __ballot_sync(0xffffffffu, f >= 0);
+    int base = 0;
+    if ((tid & 31) == 0 && m) base = atomicAdd(s_n, __popc(m));
+    base = __shfl_sync(0xffffffffu, base, 0);
+    if (f >= 0) {
+        const int slot = base + __popc(m & ((1u << (tid & 31)) - 1u));
+        const float4* r = p.rec + ((size_t)b * p.F + f) * 4;
+#pragma unroll
+        for (int k = 0; k < 4; k++) s_rec[slot * 4 + k] = __ldg(r + k);
+        s_face[slot] = f;
+    }
+    __syncthreads();
+    return *s_n;
+}
+
+// ------------------------------------------------------------------------------------------------ k_soft_fwd
+__global__ void __launch_bounds__(kThreads) k_soft_fwd(const __grid_constant__ SoftParams p) {
+    __shared__ float4 s_rec[kThreads * 4];
+    __shared__ int s_face[kThreads];
+    __shared__ int s_n;
+    const int tile = blockIdx.x, b = blockIdx.y;
+    const int tx = tile % p.ntx, ty = tile / p.ntx;
+    const int col = tx * kTile + (threadIdx.x % kTile), row = ty * kTile + (threadIdx.x / kTile);
+    const int S = p.S;
+    const float px = soft_centre(col, S), py = soft_centre(S - 1 - row, S);
+    const size_t seg = (size_t)b * (p.ntiles + 1);
+    const int n_tile = p.cnt[seg + tile], n_all = n_tile + p.cnt[seg + p.ntiles];
+    const unsigned long long cap = (unsigned long long)(kTermCap * kFix);
+    unsigned long long acc = 0;  // Lambda in units of 2^-40: integer adds, so the order of the faces does not matter
+    for (int next = 0; next < n_all; next += kThreads) {
+        const int n = stage_faces(p, b, tile, tx, ty, n_tile, n_all, next, s_rec, s_face, &s_n);
+        for (int j = 0; j < n; j++) {
+            float x, t, qx, qy;
+            int k;
+            if (!soft_term(s_rec + 4 * j, px, py, p.inv_sigma, p.cut, x, k, t, qx, qy)) continue;
+            const float sp = fmaxf(x, 0.0f) + log1pf(expf(-fabsf(x)));  // softplus(x) >= 0
+            acc += (unsigned long long)__float2ll_rn(fminf(sp, kTermCap) * kFix);
+            acc = acc < cap ? acc : cap;
+        }
+        __syncthreads();
+    }
+    if (row < S && col < S) {
+        const float lam = __ull2float_rn(acc) * (1.0f / kFix);
+        __stcs(p.alpha + (size_t)b * S * S + (size_t)row * S + col, -expm1f(-lam));
+    }
+}
+
+// ------------------------------------------------------------------------------------------------ k_soft_bwd
+__global__ void __launch_bounds__(kThreads) k_soft_bwd(const __grid_constant__ SoftParams p) {
+    __shared__ float4 s_rec[kThreads * 4];
+    __shared__ int s_face[kThreads];
+    __shared__ float s_acc[kThreads * 6];
+    __shared__ int s_n;
+    const int tile = blockIdx.x, b = blockIdx.y;
+    const int tx = tile % p.ntx, ty = tile / p.ntx;
+    const int col = tx * kTile + (threadIdx.x % kTile), row = ty * kTile + (threadIdx.x / kTile);
+    const int S = p.S, lane = threadIdx.x & 31;
+    const float px = soft_centre(col, S), py = soft_centre(S - 1 - row, S);
+    const size_t seg = (size_t)b * (p.ntiles + 1);
+    const int n_tile = p.cnt[seg + tile], n_all = n_tile + p.cnt[seg + p.ntiles];
+    if (n_all == 0) return;  // CTA-uniform
+    float gp = 0.0f;  // d loss / d x_j = gp D_j with gp = g (1 - alpha) (-2 sign / sigma folded in below)
+    if (row < S && col < S) {
+        const size_t o = (size_t)b * S * S + (size_t)row * S + col;
+        gp = __ldg(p.g + o) * (1.0f - __ldg(p.alpha + o));
+    }
+    for (int i = threadIdx.x; i < kThreads * 6; i += kThreads) s_acc[i] = 0.0f;
+    for (int next = 0; next < n_all; next += kThreads) {
+        const int n = stage_faces(p, b, tile, tx, ty, n_tile, n_all, next, s_rec, s_face, &s_n);
+        for (int j = 0; j < n; j++) {
+            float x = 0.0f, t = 0.0f, qx = 0.0f, qy = 0.0f;
+            int k = 0;
+            const bool hit = gp != 0.0f && soft_term(s_rec + 4 * j, px, py, p.inv_sigma, p.cut, x, k, t, qx, qy);
+            if (!__any_sync(0xffffffffu, hit)) continue;  // warp-uniform
+            float v[6] = {0.0f, 0.0f, 0.0f, 0.0f, 0.0f, 0.0f};
+            if (hit) {
+                const float e = expf(-fabsf(x));
+                const float D = x >= 0.0f ? __frcp_rn(1.0f + e) : __fdiv_rn(e, 1.0f + e);
+                // d x / d(d^2) = +-1/sigma; d(d^2)/da = -2 (1 - t)(p - q), d(d^2)/db = -2 t (p - q) for edge (a, b)
+                const float s = gp * D * (x >= 0.0f ? -2.0f : 2.0f) * p.inv_sigma;
+                const float wa = s * (1.0f - t), wb = s * t;
+#pragma unroll
+                for (int m = 0; m < 3; m++) {
+                    const bool is_a = m == k, is_b = m == (k == 2 ? 0 : k + 1);
+                    v[2 * m] = is_a ? wa * qx : (is_b ? wb * qx : 0.0f);
+                    v[2 * m + 1] = is_a ? wa * qy : (is_b ? wb * qy : 0.0f);
+                }
+            }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1)
+#pragma unroll
+                for (int m = 0; m < 6; m++) v[m] += __shfl_xor_sync(0xffffffffu, v[m], o);
+            if (lane < 6) {
+                float mine = v[0];
+#pragma unroll
+                for (int m = 1; m < 6; m++) if (lane == m) mine = v[m];
+                atomicAdd(&s_acc[j * 6 + lane], mine);
+            }
+        }
+        __syncthreads();
+        // one set of global atomics per face of the round: thread (face slot, vertex)
+        for (int i = threadIdx.x; i < n * 3; i += kThreads) {
+            const int j = i / 3, m = i % 3;
+            const float gx = s_acc[j * 6 + 2 * m], gy = s_acc[j * 6 + 2 * m + 1];
+            s_acc[j * 6 + 2 * m] = 0.0f; s_acc[j * 6 + 2 * m + 1] = 0.0f;
+            if (gx == 0.0f && gy == 0.0f) continue;
+            float* gv = nr::face_grad_vertex(p.dst, b, s_face[j], m);
+            if (gv) { atomicAdd(gv, gx); atomicAdd(gv + 1, gy); }
+        }
+        __syncthreads();
+    }
+}
+
+// ------------------------------------------------------------------------------------------------ host
+// workspace = face records | tile boxes | counters | cursors (one memset covers both) | offsets | lists
+struct SoftLayout {
+    size_t rec, box, cnt, cursor, off, list, total;
+};
+
+inline size_t align256(size_t x) { return (x + 255) / 256 * 256; }
+
+inline int tiles_per_axis(int S) { return (S + kTile - 1) / kTile; }
+
+// false: sizes the kernels cannot index (grid.y = B, grid.x = tiles, 16-bit tile boxes, 32-bit list offsets)
+inline bool soft_sizes_ok(int B, int F, int S) {
+    if (B <= 0 || F <= 0 || S <= 0) return false;
+    if (B > 65535 || S > 32767) return false;
+    return (long long)B * F * kWideTiles <= 0x7FFFFFFFll;
+}
+
+inline SoftLayout soft_layout(int B, int F, int S) {
+    const size_t nt = (size_t)tiles_per_axis(S) * tiles_per_axis(S);
+    const size_t nseg = (size_t)B * (nt + 1);
+    SoftLayout L;
+    L.rec = 0;
+    L.box = L.rec + align256((size_t)B * F * 4 * sizeof(float4));
+    L.cnt = L.box + align256((size_t)B * F * sizeof(uint2));
+    L.cursor = L.cnt + nseg * sizeof(int);
+    L.off = L.cnt + align256(2 * nseg * sizeof(int));
+    L.list = L.off + align256(nseg * sizeof(int));
+    L.total = L.list + align256((size_t)B * F * kWideTiles * sizeof(int));
+    return L;
+}
+
+// the host checks of both entry points; fills `p` on success (NR_ERR_WORKSPACE after every NR_ERR_INVALID_ARG rule)
+int soft_setup(const nr_b200_soft_args* a, bool backward, SoftParams* p) {
+    nr_internal::launch_count() = 0;
+    if (!a || a->struct_size != sizeof(nr_b200_soft_args)) return NR_ERR_INVALID_ARG;
+    const uint32_t flags = a->flags;
+    const int B = a->batch_size, F = a->num_faces, S = a->image_size;
+    if (!soft_sizes_ok(B, F, S)) return NR_ERR_INVALID_ARG;
+    const float sigma = a->sigma;
+    if (!isfinite(sigma) || !(sigma > 0.0f)) return NR_ERR_INVALID_ARG;
+    if (!(a->near_ <= a->far_)) return NR_ERR_INVALID_ARG;
+    memset(p, 0, sizeof(*p));
+    if (!nr_internal::make_face_src(flags, a->faces, a->vertices, a->face_indices, F, a->num_vertices, &p->src))
+        return NR_ERR_INVALID_ARG;
+    if (!a->alpha) return NR_ERR_INVALID_ARG;
+    if (backward) {
+        const bool indexed = (flags & NR_FACES_INDEXED) != 0;
+        if (indexed ? a->grad_faces != nullptr : a->grad_vertices != nullptr) return NR_ERR_INVALID_ARG;
+        if (!nr_internal::make_face_grad(flags, a->grad_faces, a->grad_vertices, a->face_indices, F, a->num_vertices, &p->dst))
+            return NR_ERR_INVALID_ARG;
+    }
+    const SoftLayout L = soft_layout(B, F, S);
+    if (!a->workspace || a->workspace_bytes < L.total || ((uintptr_t)a->workspace & 15)) return NR_ERR_WORKSPACE;
+    char* ws = (char*)a->workspace;
+    p->rec = (float4*)(ws + L.rec); p->box = (uint2*)(ws + L.box);
+    p->cnt = (int*)(ws + L.cnt); p->cursor = (int*)(ws + L.cursor); p->off = (int*)(ws + L.off); p->list = (int*)(ws + L.list);
+    p->alpha = a->alpha; p->g = a->grad_alpha;
+    p->B = B; p->F = F; p->S = S;
+    p->ntx = tiles_per_axis(S); p->ntiles = p->ntx * p->ntx;
+    const double cut = (double)sigma * log((1.0 - NR_SOFT_EPS) / NR_SOFT_EPS);
+    p->inv_sigma = (float)(1.0 / (double)sigma);
+    p->cut = (float)cut;
+    p->reach = (float)(sqrt(cut) * S * 0.5) + 1.0f;
+    p->near_ = a->near_; p->far_ = a->far_;
+    return NR_OK;
+}
+
+// setup -> scan -> fill: the tile lists of every item
+int bin_faces(const SoftParams& p, cudaStream_t s) {
+    nr_internal::prof_begin("memset_soft_bins", s);
+    if (cudaMemsetAsync(p.cnt, 0, 2 * (size_t)p.B * (p.ntiles + 1) * sizeof(int), s) != cudaSuccess) return NR_ERR_CUDA;
+    nr_internal::prof_end(s);
+    const dim3 grid((unsigned)((p.F + 255) / 256), (unsigned)p.B);
+    {
+        nr_internal::LaunchScope ls("k_soft_setup", s);
+        k_soft_setup<false><<<grid, 256, 0, s>>>(p);
+    }
+    nr_internal::strip_scan(p.cnt, p.off, p.ntiles + 1, (long long)p.F * kWideTiles, p.B, s);
+    {
+        nr_internal::LaunchScope ls("k_soft_fill", s);
+        k_soft_setup<true><<<grid, 256, 0, s>>>(p);
+    }
+    return NR_OK;
+}
+
+}  // namespace
+
+extern "C" size_t nr_b200_soft_workspace_bytes(int32_t B, int32_t F, int32_t S, float sigma, uint32_t flags) {
+    (void)flags;
+    if (!soft_sizes_ok(B, F, S) || !isfinite(sigma) || !(sigma > 0.0f)) return 0;
+    return soft_layout(B, F, S).total;
+}
+
+extern "C" int nr_b200_soft_silhouettes(const nr_b200_soft_args* args, void* cuda_stream) {
+    SoftParams p;
+    const int rc = soft_setup(args, false, &p);
+    if (rc != NR_OK) return rc;
+    cudaStream_t s = (cudaStream_t)cuda_stream;
+    if (bin_faces(p, s) != NR_OK) return NR_ERR_CUDA;
+    {
+        nr_internal::LaunchScope ls("k_soft_fwd", s);
+        k_soft_fwd<<<dim3((unsigned)p.ntiles, (unsigned)p.B), kThreads, 0, s>>>(p);
+    }
+    return cudaGetLastError() == cudaSuccess ? NR_OK : NR_ERR_CUDA;
+}
+
+extern "C" int nr_b200_soft_silhouettes_backward(const nr_b200_soft_args* args, void* cuda_stream) {
+    SoftParams p;
+    const int rc = soft_setup(args, true, &p);
+    if (rc != NR_OK) return rc;
+    const nr_b200_soft_args* a = args;
+    const bool indexed = (a->flags & NR_FACES_INDEXED) != 0;
+    cudaStream_t s = (cudaStream_t)cuda_stream;
+    if (!(a->flags & NR_GRAD_ACCUMULATE)) {
+        nr_internal::prof_begin("memset_grads", s);
+        const cudaError_t e = indexed ? cudaMemsetAsync(a->grad_vertices, 0, (size_t)p.B * a->num_vertices * 3 * sizeof(float), s)
+                                      : cudaMemsetAsync(a->grad_faces, 0, (size_t)p.B * p.F * 9 * sizeof(float), s);
+        nr_internal::prof_end(s);
+        if (e != cudaSuccess) return NR_ERR_CUDA;
+    }
+    if (!a->grad_alpha) return cudaGetLastError() == cudaSuccess ? NR_OK : NR_ERR_CUDA;
+    if (bin_faces(p, s) != NR_OK) return NR_ERR_CUDA;
+    {
+        nr_internal::LaunchScope ls("k_soft_bwd", s);
+        k_soft_bwd<<<dim3((unsigned)p.ntiles, (unsigned)p.B), kThreads, 0, s>>>(p);
+    }
+    return cudaGetLastError() == cudaSuccess ? NR_OK : NR_ERR_CUDA;
+}

@@ -16,6 +16,7 @@ There is no CPU path (the reference raises NotImplementedError for CPU arrays as
 from __future__ import annotations
 
 import ctypes
+import math
 import os
 
 import torch
@@ -989,6 +990,118 @@ def rasterize_attributes(
     S = int(image_size) * 2 if anti_aliasing else int(image_size)
     image = _InterpolateFunction.apply(geom, attrs, fim, wmap, indices, flags, S)
     return (image, alpha) if return_alpha else image
+
+
+DEFAULT_SOFT_SIGMA = 1e-5
+
+
+class _SoftSilhouettesFunction(torch.autograd.Function):
+    """autograd node of the soft silhouettes: forward = nr_b200_soft_silhouettes, backward =
+    nr_b200_soft_silhouettes_backward from the saved alpha.  `geom` / `indices` as _RasterizeFunction."""
+
+    @staticmethod
+    def forward(ctx, geom, indices, S, sigma, near, far):
+        lib = _lib.load()
+        dev = geom.device
+        geom_c = geom.detach().contiguous()
+        with torch.cuda.device(dev):
+            alpha = torch.empty((geom_c.shape[0], S, S), dtype=torch.float32, device=dev)
+            a, ws = _soft_args(lib, geom_c, indices, S, sigma, near, far)
+            a.alpha = _ptr(alpha)
+            _lib.check(lib.nr_b200_soft_silhouettes(ctypes.byref(a), _stream_ptr(dev)))
+        ctx.cfg = (S, sigma, near, far)
+        ctx.save_for_backward(geom_c, indices, alpha)
+        return alpha
+
+    @staticmethod
+    def backward(ctx, g):
+        if g is None or not ctx.needs_input_grad[0]:
+            return None, None, None, None, None, None
+        lib = _lib.load()
+        geom_c, indices, alpha = ctx.saved_tensors
+        dev = geom_c.device
+        g = g.detach().to(torch.float32).contiguous()
+        with torch.cuda.device(dev):
+            grad_geom = torch.empty_like(geom_c)
+            a, ws = _soft_args(lib, geom_c, indices, *ctx.cfg)
+            a.alpha, a.grad_alpha = _ptr(alpha), _ptr(g)
+            if indices is not None:
+                a.grad_vertices = _ptr(grad_geom)
+            else:
+                a.grad_faces = _ptr(grad_geom)
+            _lib.check(lib.nr_b200_soft_silhouettes_backward(ctypes.byref(a), _stream_ptr(dev)))
+        return grad_geom, None, None, None, None, None
+
+
+def _soft_args(lib, geom_c, indices, S, sigma, near, far):
+    """nr_b200_soft_args of a call and its workspace (returned so that it lives until the launch is queued)"""
+    a = _lib.SoftArgs()
+    a.struct_size = ctypes.sizeof(_lib.SoftArgs)
+    B = geom_c.shape[0]
+    flags = 0
+    if indices is not None:
+        flags |= _lib.NR_FACES_INDEXED
+        if indices.dim() == 2 or (indices.shape[0] == 1 and B > 1):
+            flags |= _lib.NR_INDICES_SHARED
+        a.vertices, a.face_indices, a.num_vertices = _ptr(geom_c), _ptr(indices), geom_c.shape[1]
+        a.num_faces = indices.shape[-2]
+    else:
+        a.faces, a.num_faces = _ptr(geom_c), geom_c.shape[1]
+    a.flags = flags
+    a.batch_size, a.image_size = B, S
+    a.sigma, a.near_, a.far_ = sigma, near, far
+    n = lib.nr_b200_soft_workspace_bytes(B, a.num_faces, S, sigma, flags)
+    if n == 0:
+        raise ValueError("rasterize_soft_silhouettes: sizes out of range (batch %d, %d faces, image %d)" % (B, a.num_faces, S))
+    ws = torch.empty(n, dtype=torch.uint8, device=geom_c.device)
+    a.workspace, a.workspace_bytes = _ptr(ws), n
+    return a, ws
+
+
+def rasterize_soft_silhouettes(
+        faces,
+        image_size=DEFAULT_IMAGE_SIZE,
+        sigma=DEFAULT_SOFT_SIGMA,
+        near=DEFAULT_NEAR,
+        far=DEFAULT_FAR,
+        *,
+        vertices=None,
+):
+    """Soft silhouettes [B,H,W] (SoftRas, Liu et al. 2019): every face gives every pixel within reach the probability
+    sigmoid(+-d^2 / sigma) of the pixel's squared NDC distance d^2 to the face (+ inside, - outside), and
+    alpha = 1 - prod_j (1 - D_j) over the faces.  Unlike rasterize_silhouettes, the gradient reaches every vertex of every
+    face within reach of a pixel -- faces a few pixels off a target outline, and faces hidden behind others -- so it suits
+    fitting shapes to masks.  Not in the reference.
+
+    Geometry as rasterize_silhouettes: faces [B,F,3,3], or `vertices` [B,Nv,3] with integer faces [F,3] / [1|B,F,3] (an
+    expanded index set stays shared).  Winding does not matter: pass each face once (a fill_back copy would count twice).
+    A face takes part only when all three vertex depths lie in [near, far] (a per-face test, not the hard rasterizer's
+    per-pixel depth test).  sigma > 0 sets the softness: the reach is sqrt(sigma ln((1-eps)/eps)) image_size / 2 pixels
+    with eps = 1e-4, about 1.2 px at 256 x 256 for the default 1e-5.  No anti-aliasing; deterministic forward.  The exact
+    definition and its gradient are in include/nr_b200.h (nr_b200_soft_args)."""
+    try:
+        sigma = float(sigma)
+    except (TypeError, ValueError):
+        raise TypeError("sigma must be a number, got %r" % (sigma,))
+    if not math.isfinite(sigma) or sigma <= 0:
+        raise ValueError("sigma must be finite and > 0, got %r" % (sigma,))
+    if not (float(near) <= float(far)):
+        raise ValueError("near must be <= far, got near=%r far=%r" % (near, far))
+    if int(image_size) < 1:
+        raise ValueError("image_size must be >= 1, got %r" % (image_size,))
+    _check_inputs(faces, None, False, vertices=vertices)  # the geometry, then the device check
+    indices = None
+    if vertices is not None:
+        geom = vertices if vertices.dtype == torch.float32 else vertices.float()
+        indices = faces
+        if indices.dim() == 3 and indices.shape[0] > 1 and indices.stride(0) == 0:
+            indices = indices[:1]
+        indices = indices.to(torch.int32).contiguous()
+    else:
+        geom = faces if faces.dtype == torch.float32 else faces.float()
+        if not geom.is_cuda:
+            raise NotImplementedError("neural_renderer_b200 has no CPU implementation (inputs must be CUDA tensors)")
+    return _SoftSilhouettesFunction.apply(geom, indices, int(image_size), sigma, float(near), float(far))
 
 
 class Rasterize(object):

@@ -6,7 +6,8 @@ import math
 import torch
 
 from . import functional as F
-from .rasterize import rasterize, rasterize_attributes, rasterize_depth, rasterize_silhouettes
+from .rasterize import (DEFAULT_SOFT_SIGMA, rasterize, rasterize_attributes, rasterize_depth, rasterize_silhouettes,
+                        rasterize_soft_silhouettes)
 
 
 class Renderer(object):
@@ -101,6 +102,16 @@ class Renderer(object):
         faces = F.vertices_to_faces(vertices, faces)
         # renderer.py:52 -- near / far / rasterizer_eps are NOT forwarded (module defaults apply)
         return rasterize_silhouettes(faces, self.image_size, self.anti_aliasing)
+
+    def render_soft_silhouettes(self, vertices, faces, sigma=DEFAULT_SOFT_SIGMA):
+        """Soft silhouettes [B,H,W] (neural_renderer_b200.rasterize_soft_silhouettes) seen through this renderer's camera,
+        with near / far.  Winding does not matter to them, so fill_back adds no copies (a copy would count twice) and the
+        result is the same either way; anti_aliasing is ignored (the soft image needs no supersampling).  The gradient
+        reaches `vertices` through the camera from every face within reach of a pixel."""
+        vertices = self._transform(vertices)
+        if self.fused and self._fusable(vertices, faces):
+            return rasterize_soft_silhouettes(faces, self.image_size, sigma, self.near, self.far, vertices=vertices)
+        return rasterize_soft_silhouettes(F.vertices_to_faces(vertices, faces), self.image_size, sigma, self.near, self.far)
 
     def render_depth(self, vertices, faces):
         if self.fused and self._fusable(vertices, faces):
