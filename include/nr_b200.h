@@ -567,6 +567,80 @@ typedef struct nr_b200_soft_args {
     size_t workspace_bytes;
 } nr_b200_soft_args;
 
+/* Soft RGB (within ABI 4, additive): SoftRas colour aggregation over every face within reach, with gradients into the
+ * vertices (x, y and z), the per-face texture cubes and the face light.  Geometry, pixel centres, the participation
+ * test, d_j^2, inside_j, x_j, D_j, the cut-off and alpha are exactly those of the soft silhouettes above: alpha is
+ * bit-identical to nr_b200_soft_silhouettes on the same inputs.  For each contributing (pixel, face j):
+ *   A = (x1 - x0)(y2 - y0) - (y1 - y0)(x2 - x0), the doubled signed area (fp32, plain products: vertices exactly collinear
+ *     in x, y give exactly 0).  A face with A == 0 counts towards alpha but not towards rgb.
+ *   Screen barycentrics: with the edge functions c_k of the distance test (edge k from v_k to v_k+1,
+ *     c_k = (v_k+1 - v_k) x (p - v_k)), lam_k = c_{k+1 mod 3} / A; clipped lh = clamp(lam, 0, 1), l = lh / sum lh.
+ *   zp = 1 / sum_k l_k / z_k (perspective-correct depth).
+ *   C_j = the trilinear cube sample of texture_coords(l, zp, z_0, z_1, z_2) with ts and the clamp from eps, as
+ *     nr_b200_forward samples cubes (no fill_back reversal); with face_light every tap is multiplied by the face's light
+ *     first.
+ *   zn_j = (far - zp) / (far - near); the background sits at zn_b = NR_SOFT_BG_DEPTH.
+ *   zmax = max(zn_b, max_j zn_j), w_j = D_j exp((zn_j - zmax) / gamma), w_b = exp((zn_b - zmax) / gamma),
+ *   Z = sum_j w_j + w_b,  rgb = (sum_j w_j C_j + w_b background) / Z.
+ * The exponents are taken from depth differences, (zref - zp_j) / ((far - near) gamma), zref = far - zmax (far - near),
+ * not from differences of zn (whose fp32 rounding near far would dominate at a small gamma).  The forward takes the faces
+ * of each pixel in a fixed order (the tile's faces, then the item's wide faces, each by ascending face index: the lists
+ * are sorted) and accumulates a running-max softmax: zref starts at the background level far - NR_SOFT_BG_DEPTH (far -
+ * near) with Z = 1 and the background colour, and a nearer face rescales Z and the sum by exp((zp - zref) / ((far -
+ * near) gamma)).  A face whose weight against the running zref is exactly 0 in fp32 contributes nothing and its cube is
+ * not read.  rgb is therefore bit-for-bit repeatable; under a permutation of the faces it is equal only within fp32
+ * rounding.  state = {Z, zref} per pixel, written by the forward and read by the backward.
+ * Backward: the exact derivative of the above with subgradients at the branches (the nearest edge and its segment, the
+ * clamps of lh and of texture_coords, the cube cell and the cut-off held fixed; zref cancels and is held fixed).  With
+ * g = grad_rgb at the pixel, the saved rgb and Z (no division by D_j):
+ *   d L / d x_j  = (1 - alpha) D_j grad_alpha + w_j (1 - D_j) g . (C_j - rgb) / Z
+ *   d L / d zn_j = (w_j / gamma) g . (C_j - rgb) / Z      (through zp into l (x, y) and the vertex depths z_k)
+ *   d L / d C_j  = w_j g / Z   (into the 8 taps times the light: grad_textures; into grad_face_light by the unlit sample;
+ *                               through the cube's axis derivative and texture_coords into l, zp and z_k)
+ *   grad_faces / grad_vertices (as the silhouettes, now with z), grad_textures and grad_face_light are zero-filled first
+ *   unless NR_GRAD_ACCUMULATE.  fp32 atomics, not bit-pinned.  grad_rgb / grad_alpha NULL = zeros.
+ * Scratch: nr_b200_soft_rgb_workspace_bytes (both passes).  It includes the sort's scratch, which CUB sizes for the
+ * current device: the query needs one (0 without one, as nr_b200_vertex_normals_workspace_bytes).
+ * Host rejections (NR_ERR_INVALID_ARG, before any launch): every rejection of the silhouettes (struct_size !=
+ * sizeof(nr_b200_soft_rgb_args)), a non-finite or non-positive gamma, near >= far (strict: the normalisation divides by
+ * far - near) or a non-finite far - near or eps, ts < 2 or ts^3 3 > 2^31 - 1, NULL textures, rgb, alpha or state, and any flag outside
+ * NR_FACES_INDEXED | NR_INDICES_SHARED | NR_TEX_SHARED | NR_GRAD_ACCUMULATE (NR_TEX_UV, NR_TEX_MIPMAP and
+ * NR_TEX_FILL_BACK included).  Then NR_ERR_WORKSPACE for a missing, short or unaligned workspace. */
+#define NR_SOFT_BG_DEPTH 1e-3
+
+typedef struct nr_b200_soft_rgb_args {
+    uint32_t struct_size; /* sizeof(nr_b200_soft_rgb_args) */
+    uint32_t flags;       /* NR_FACES_INDEXED / NR_INDICES_SHARED, NR_TEX_SHARED, NR_GRAD_ACCUMULATE (backward) */
+    int32_t batch_size;   /* B */
+    int32_t num_faces;    /* F */
+    int32_t image_size;   /* S */
+    int32_t num_vertices; /* Nv (NR_FACES_INDEXED) */
+    int32_t texture_size; /* ts >= 2 */
+    float sigma;          /* > 0 */
+    float gamma;          /* > 0: the depth softmax temperature (in units of zn) */
+    float near_;          /* near < far; faces with a vertex depth outside [near, far] take no part */
+    float far_;
+    float eps;            /* texture_coords' clamp: t <= ts - 1 - eps */
+    float background[3];  /* RGB of the background term */
+    int32_t _pad0;
+    const float *faces;          /* [B,F,3,3], or NULL with NR_FACES_INDEXED */
+    const float *vertices;       /* [B,Nv,3], NR_FACES_INDEXED only */
+    const int32_t *face_indices; /* [B,F,3], or [F,3] with NR_INDICES_SHARED */
+    const float *textures;       /* [B,F,ts,ts,ts,3], or [F,ts,ts,ts,3] with NR_TEX_SHARED */
+    const float *face_light;     /* [B,F,3] or NULL = unlit */
+    float *rgb;                  /* [B,3,S,S]: written by the forward (row 0 at the top), read by the backward */
+    float *alpha;                /* [B,S,S]: likewise */
+    float *state;                /* [B,2,S,S]: {Z, zref}, likewise */
+    const float *grad_rgb;       /* backward: [B,3,S,S] or NULL (zeros) */
+    const float *grad_alpha;     /* backward: [B,S,S] or NULL (zeros) */
+    float *grad_faces;           /* backward: [B,F,3,3]; not with NR_FACES_INDEXED */
+    float *grad_vertices;        /* backward: [B,Nv,3]; only with NR_FACES_INDEXED */
+    float *grad_textures;        /* backward: layout of textures, or NULL = not wanted */
+    float *grad_face_light;      /* backward: [B,F,3], or NULL = not wanted */
+    void *workspace;             /* nr_b200_soft_rgb_workspace_bytes() bytes, 16-byte aligned */
+    size_t workspace_bytes;
+} nr_b200_soft_rgb_args;
+
 /* ABI version of the loaded library (== NR_B200_ABI_VERSION it was built with). */
 NR_B200_API int nr_b200_abi_version(void);
 NR_B200_API const char *nr_b200_error_string(int code);
@@ -633,6 +707,11 @@ NR_B200_API size_t nr_b200_soft_workspace_bytes(int32_t batch_size, int32_t num_
                                                 uint32_t flags);
 NR_B200_API int nr_b200_soft_silhouettes(const nr_b200_soft_args *args, void *cuda_stream);
 NR_B200_API int nr_b200_soft_silhouettes_backward(const nr_b200_soft_args *args, void *cuda_stream);
+/* Soft RGB (nr_b200_soft_rgb_args above): rgb [B,3,S,S], alpha [B,S,S] and state, and the backward into the geometry,
+ * grad_textures and grad_face_light.  The workspace size is 0 for sizes or flags the calls refuse, or without a device. */
+NR_B200_API size_t nr_b200_soft_rgb_workspace_bytes(int32_t batch_size, int32_t num_faces, int32_t image_size, uint32_t flags);
+NR_B200_API int nr_b200_soft_rgb(const nr_b200_soft_rgb_args *args, void *cuda_stream);
+NR_B200_API int nr_b200_soft_rgb_backward(const nr_b200_soft_rgb_args *args, void *cuda_stream);
 
 /* vertices_to_faces (reference vertices_to_faces.py:4-21), the step either side of the rasterizer:
  *   forward   out_faces[b,f,k,:] = vertices[b, faces[b,f,k], :]           ([B,Nv,3] x [B,Nf,3] int32 -> [B,Nf,3,3])

@@ -61,6 +61,9 @@ EXPORTED_SYMBOLS = (
     "nr_b200_soft_workspace_bytes",
     "nr_b200_soft_silhouettes",
     "nr_b200_soft_silhouettes_backward",
+    "nr_b200_soft_rgb_workspace_bytes",
+    "nr_b200_soft_rgb",
+    "nr_b200_soft_rgb_backward",
     "nr_b200_vertices_to_faces",
     "nr_b200_vertices_to_faces_backward",
     "nr_b200_camera_transform",
@@ -195,6 +198,26 @@ class SoftArgs(ctypes.Structure):
 SOFT_EPS = 1e-4  # NR_SOFT_EPS: an outside face contributes while its D >= SOFT_EPS
 
 
+class SoftRgbArgs(ctypes.Structure):
+    _fields_ = [
+        ("struct_size", ctypes.c_uint32), ("flags", ctypes.c_uint32),
+        ("batch_size", ctypes.c_int32), ("num_faces", ctypes.c_int32),
+        ("image_size", ctypes.c_int32), ("num_vertices", ctypes.c_int32), ("texture_size", ctypes.c_int32),
+        ("sigma", ctypes.c_float), ("gamma", ctypes.c_float), ("near_", ctypes.c_float), ("far_", ctypes.c_float),
+        ("eps", ctypes.c_float), ("background", ctypes.c_float * 3), ("_pad0", ctypes.c_int32),
+        ("faces", ctypes.c_void_p), ("vertices", ctypes.c_void_p), ("face_indices", ctypes.c_void_p),
+        ("textures", ctypes.c_void_p), ("face_light", ctypes.c_void_p),
+        ("rgb", ctypes.c_void_p), ("alpha", ctypes.c_void_p), ("state", ctypes.c_void_p),
+        ("grad_rgb", ctypes.c_void_p), ("grad_alpha", ctypes.c_void_p),
+        ("grad_faces", ctypes.c_void_p), ("grad_vertices", ctypes.c_void_p),
+        ("grad_textures", ctypes.c_void_p), ("grad_face_light", ctypes.c_void_p),
+        ("workspace", ctypes.c_void_p), ("workspace_bytes", ctypes.c_size_t),
+    ]
+
+
+SOFT_BG_DEPTH = 1e-3  # NR_SOFT_BG_DEPTH: the normalised depth of the soft RGB's background term
+
+
 _LIB = None
 
 
@@ -270,6 +293,12 @@ def load():
         fn = getattr(lib, name)
         fn.restype = ctypes.c_int
         fn.argtypes = [ctypes.POINTER(SoftArgs), ctypes.c_void_p]
+    lib.nr_b200_soft_rgb_workspace_bytes.restype = ctypes.c_size_t
+    lib.nr_b200_soft_rgb_workspace_bytes.argtypes = [ctypes.c_int32] * 3 + [ctypes.c_uint32]
+    for name in ("nr_b200_soft_rgb", "nr_b200_soft_rgb_backward"):
+        fn = getattr(lib, name)
+        fn.restype = ctypes.c_int
+        fn.argtypes = [ctypes.POINTER(SoftRgbArgs), ctypes.c_void_p]
     lib.nr_b200_vertices_to_faces.restype = ctypes.c_int
     lib.nr_b200_vertices_to_faces.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
                                               ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p]

@@ -1104,6 +1104,152 @@ def rasterize_soft_silhouettes(
     return _SoftSilhouettesFunction.apply(geom, indices, int(image_size), sigma, float(near), float(far))
 
 
+DEFAULT_SOFT_GAMMA = 1e-4
+
+
+class _SoftRgbFunction(torch.autograd.Function):
+    """autograd node of the soft RGB: forward = nr_b200_soft_rgb, backward = nr_b200_soft_rgb_backward from the saved
+    rgb, alpha and state.  `geom` / `indices` as _RasterizeFunction; `textures` [B|1,F,ts,ts,ts,3] (1 = shared)."""
+
+    @staticmethod
+    def forward(ctx, geom, textures, face_light, indices, cfg):
+        lib = _lib.load()
+        dev = geom.device
+        geom_c = geom.detach().contiguous()
+        tex_c = textures.detach().contiguous()
+        light_c = face_light.detach().contiguous() if face_light is not None else None
+        B, S = geom_c.shape[0], cfg[0]
+        with torch.cuda.device(dev):
+            rgb = torch.empty((B, 3, S, S), dtype=torch.float32, device=dev)
+            alpha = torch.empty((B, S, S), dtype=torch.float32, device=dev)
+            state = torch.empty((B, 2, S, S), dtype=torch.float32, device=dev)
+            a, ws = _soft_rgb_args(lib, geom_c, indices, tex_c, light_c, cfg)
+            a.rgb, a.alpha, a.state = _ptr(rgb), _ptr(alpha), _ptr(state)
+            _lib.check(lib.nr_b200_soft_rgb(ctypes.byref(a), _stream_ptr(dev)))
+        ctx.cfg = cfg
+        ctx.save_for_backward(geom_c, tex_c, light_c, indices, rgb, alpha, state)
+        return rgb, alpha
+
+    @staticmethod
+    def backward(ctx, g_rgb, g_alpha):
+        lib = _lib.load()
+        geom_c, tex_c, light_c, indices, rgb, alpha, state = ctx.saved_tensors
+        dev = geom_c.device
+        need_geom, need_tex, need_light = ctx.needs_input_grad[:3]
+        if not (need_geom or need_tex or need_light) or (g_rgb is None and g_alpha is None):
+            return None, None, None, None, None
+        g_rgb = g_rgb.detach().to(torch.float32).contiguous() if g_rgb is not None else None
+        g_alpha = g_alpha.detach().to(torch.float32).contiguous() if g_alpha is not None else None
+        with torch.cuda.device(dev):
+            grad_geom = torch.empty_like(geom_c)
+            grad_tex = torch.empty_like(tex_c) if need_tex else None
+            grad_light = torch.empty_like(light_c) if need_light and light_c is not None else None
+            a, ws = _soft_rgb_args(lib, geom_c, indices, tex_c, light_c, ctx.cfg)
+            a.rgb, a.alpha, a.state = _ptr(rgb), _ptr(alpha), _ptr(state)
+            a.grad_rgb, a.grad_alpha = _ptr(g_rgb), _ptr(g_alpha)
+            if indices is not None:
+                a.grad_vertices = _ptr(grad_geom)
+            else:
+                a.grad_faces = _ptr(grad_geom)
+            a.grad_textures, a.grad_face_light = _ptr(grad_tex), _ptr(grad_light)
+            _lib.check(lib.nr_b200_soft_rgb_backward(ctypes.byref(a), _stream_ptr(dev)))
+        return grad_geom if need_geom else None, grad_tex, grad_light, None, None
+
+
+def _soft_rgb_args(lib, geom_c, indices, tex_c, light_c, cfg):
+    """nr_b200_soft_rgb_args of a call and its workspace (returned so that it lives until the launch is queued)"""
+    S, sigma, gamma, near, far, eps, bg = cfg
+    a = _lib.SoftRgbArgs()
+    a.struct_size = ctypes.sizeof(_lib.SoftRgbArgs)
+    B = geom_c.shape[0]
+    flags = 0
+    if indices is not None:
+        flags |= _lib.NR_FACES_INDEXED
+        if indices.dim() == 2 or (indices.shape[0] == 1 and B > 1):
+            flags |= _lib.NR_INDICES_SHARED
+        a.vertices, a.face_indices, a.num_vertices = _ptr(geom_c), _ptr(indices), geom_c.shape[1]
+        a.num_faces = indices.shape[-2]
+    else:
+        a.faces, a.num_faces = _ptr(geom_c), geom_c.shape[1]
+    if tex_c.shape[0] == 1 and B > 1:
+        flags |= _lib.NR_TEX_SHARED
+    a.flags = flags
+    a.batch_size, a.image_size, a.texture_size = B, S, tex_c.shape[2]
+    a.sigma, a.gamma, a.near_, a.far_, a.eps = sigma, gamma, near, far, eps
+    a.background[:] = bg
+    a.textures, a.face_light = _ptr(tex_c), _ptr(light_c)
+    n = lib.nr_b200_soft_rgb_workspace_bytes(B, a.num_faces, S, flags)
+    if n == 0:
+        raise ValueError("rasterize_soft: sizes out of range (batch %d, %d faces, image %d)" % (B, a.num_faces, S))
+    ws = torch.empty(n, dtype=torch.uint8, device=geom_c.device)
+    a.workspace, a.workspace_bytes = _ptr(ws), n
+    return a, ws
+
+
+def rasterize_soft(
+        faces,
+        textures,
+        image_size=DEFAULT_IMAGE_SIZE,
+        sigma=DEFAULT_SOFT_SIGMA,
+        gamma=DEFAULT_SOFT_GAMMA,
+        near=DEFAULT_NEAR,
+        far=DEFAULT_FAR,
+        eps=DEFAULT_EPS,
+        background_color=DEFAULT_BACKGROUND_COLOR,
+        *,
+        vertices=None,
+        face_light=None,
+):
+    """Soft RGB images [B,3,H,W] and soft silhouettes [B,H,W] (SoftRas, Liu et al. 2019): every face within reach of a
+    pixel (the soft silhouettes' probability D_j, rasterize_soft_silhouettes) adds its texture colour with the weight
+    D_j exp((zn_j - zmax) / gamma) of its normalised depth zn_j = (far - zp) / (far - near), against a background term at
+    zn = 1e-3.  Unlike rasterize, the gradient reaches the vertices from every face within reach -- hidden faces and
+    faces a few pixels off their target included -- and reaches the vertex depths, so the depth order itself can be
+    learned.  Not in the reference.
+
+    Geometry as rasterize_soft_silhouettes (pass each face once; fill_back copies would count twice).  textures: per-face
+    cubes [B,F,ts,ts,ts,3], or [1,F,...] shared by every item (its gradient is the sum over the items), sampled at the
+    perspective-correct clipped barycentrics with the clamp from `eps` as rasterize samples them.  face_light [B,F,3]
+    (e.g. functional.face_light_from_vertices) multiplies every texel first; None = unlit.  gamma > 0 sets how sharply
+    the nearer face wins.  Returns (rgb, alpha); alpha is bit-identical to rasterize_soft_silhouettes.  Deterministic
+    forward.  Gradients into the geometry, the textures and face_light.  The exact definition is in include/nr_b200.h
+    (nr_b200_soft_rgb_args)."""
+    try:
+        sigma, gamma = float(sigma), float(gamma)
+    except (TypeError, ValueError):
+        raise TypeError("sigma and gamma must be numbers, got %r, %r" % (sigma, gamma))
+    if not math.isfinite(sigma) or sigma <= 0:
+        raise ValueError("sigma must be finite and > 0, got %r" % (sigma,))
+    if not math.isfinite(gamma) or gamma <= 0:
+        raise ValueError("gamma must be finite and > 0, got %r" % (gamma,))
+    if not (float(near) < float(far)):
+        raise ValueError("near must be < far, got near=%r far=%r" % (near, far))
+    if int(image_size) < 1:
+        raise ValueError("image_size must be >= 1, got %r" % (image_size,))
+    bg = [float(c) for c in background_color]
+    if len(bg) != 3:
+        raise ValueError("background_color must have 3 components, got %r" % (background_color,))
+    if face_light is not None and not isinstance(face_light, torch.Tensor):
+        raise TypeError("face_light must be a torch.Tensor")
+    _check_inputs(faces, textures, True, face_light=face_light, vertices=vertices)  # the shapes, then the device check
+    indices = None
+    if vertices is not None:
+        geom = vertices if vertices.dtype == torch.float32 else vertices.float()
+        indices = faces
+        if indices.dim() == 3 and indices.shape[0] > 1 and indices.stride(0) == 0:
+            indices = indices[:1]
+        indices = indices.to(torch.int32).contiguous()
+    else:
+        geom = faces if faces.dtype == torch.float32 else faces.float()
+    if textures.shape[0] > 1 and textures.stride(0) == 0:
+        textures = textures[:1]  # an expanded shared set stays one set
+    textures = textures if textures.dtype == torch.float32 else textures.float()
+    if face_light is not None and face_light.dtype != torch.float32:
+        face_light = face_light.float()
+    cfg = (int(image_size), sigma, gamma, float(near), float(far), float(eps), tuple(bg))
+    return _SoftRgbFunction.apply(geom, textures, face_light, indices, cfg)
+
+
 class Rasterize(object):
     """The reference's function object (rasterize.py:19-64): `Rasterize(image_size, near, far, eps,
     background_color, return_rgb, return_alpha, return_depth)(faces[, textures]) -> (rgb, alpha, depth)` with the

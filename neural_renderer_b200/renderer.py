@@ -6,8 +6,8 @@ import math
 import torch
 
 from . import functional as F
-from .rasterize import (DEFAULT_SOFT_SIGMA, rasterize, rasterize_attributes, rasterize_depth, rasterize_silhouettes,
-                        rasterize_soft_silhouettes)
+from .rasterize import (DEFAULT_SOFT_GAMMA, DEFAULT_SOFT_SIGMA, rasterize, rasterize_attributes, rasterize_depth,
+                        rasterize_silhouettes, rasterize_soft, rasterize_soft_silhouettes)
 
 
 class Renderer(object):
@@ -112,6 +112,29 @@ class Renderer(object):
         if self.fused and self._fusable(vertices, faces):
             return rasterize_soft_silhouettes(faces, self.image_size, sigma, self.near, self.far, vertices=vertices)
         return rasterize_soft_silhouettes(F.vertices_to_faces(vertices, faces), self.image_size, sigma, self.near, self.far)
+
+    def render_soft(self, vertices, faces, textures, sigma=DEFAULT_SOFT_SIGMA, gamma=DEFAULT_SOFT_GAMMA):
+        """Soft RGB images [B,3,H,W] and soft silhouettes [B,H,W] (neural_renderer_b200.rasterize_soft) seen through this
+        renderer's camera, with near / far, rasterizer_eps and background_color, lit by the flat light of the faces as
+        given (functional.face_light_from_vertices).  textures: per-face cubes [B,F,ts,ts,ts,3] or [1,F,...].  As for the
+        soft silhouettes, fill_back adds no copies (a copy would count twice), so a face seen from behind keeps its front
+        face's light; anti_aliasing is ignored.  Flat shading only.  The gradient reaches `vertices` through the camera and
+        the light, and the textures."""
+        if self.shading != 'flat':
+            raise ValueError("render_soft supports shading='flat' only, got shading=%r" % (self.shading,))
+        n_lights = self.lights.shape[-2] if isinstance(self.lights, torch.Tensor) else len(self.lights)
+        for name, unsupported in (("lights", n_lights), ("environment_sh", self.environment_sh is not None),
+                                  ("normal_map", self.normal_map is not None), ("specular_map", self.specular_map is not None)):
+            if unsupported:
+                raise ValueError("render_soft does not support %s (flat light only)" % name)
+        light_args = (self.light_intensity_ambient, self.light_intensity_directional, self.light_color_ambient,
+                      self.light_color_directional, self.light_direction)
+        args = (self.image_size, sigma, gamma, self.near, self.far, self.rasterizer_eps, self.background_color)
+        if self.fused and self._fusable(vertices, faces):
+            light = F.face_light_from_vertices(vertices, faces, *light_args)
+            return rasterize_soft(faces, textures, *args, vertices=self._transform(vertices), face_light=light)
+        light = F.face_light(F.vertices_to_faces(vertices, faces), *light_args)
+        return rasterize_soft(F.vertices_to_faces(self._transform(vertices), faces), textures, *args, face_light=light)
 
     def render_depth(self, vertices, faces):
         if self.fused and self._fusable(vertices, faces):
