@@ -641,6 +641,46 @@ typedef struct nr_b200_soft_rgb_args {
     size_t workspace_bytes;
 } nr_b200_soft_rgb_args;
 
+/* Soft RGB through a texture image (within ABI 4, additive): nr_b200_soft_rgb_uv / _backward take the soft RGB's
+ * arguments and this struct.  Everything up to the clipped, renormalised barycentrics l and zp, the participation test,
+ * D_j, the cut-off, alpha (bit-identical to nr_b200_soft_silhouettes), zero-area faces (alpha only), the softmax, the
+ * background term and the running-max order are exactly those of nr_b200_soft_rgb above.  Only the colour C_j of a
+ * contributing (pixel, face j) differs:
+ *   l'_k = l_k (zp / z_k)  (div.rn, not renormalised: the l_k of NR_TEX_UV with l in place of w),
+ *   uv = sum_k l'_k uv_k   with the face's own UV corners (the expression of NR_TEX_UV),
+ *   NR_TEX_UV:              the bilinear sample of NR_TEX_UV at uv (clamp to [0, 1], NaN -> 0, row 0 = top), every tap
+ *                           times face_light first;
+ *   NR_TEX_UV|NR_TEX_MIPMAP: `textures` is the packed pyramid of nr_b200_mip_build, sampled as NR_TEX_MIPMAP with the level
+ *                           of detail of NR_TEX_MIPMAP per (pixel, face) in image pixels, taking the face's screen-barycentric
+ *                           derivatives in place of K1's inverse: with lam_k = c_{k+1} / A, d lam_k / d column =
+ *                           -(2/S) e_{k+1,y} / A and d lam_k / d row = -(2/S) e_{k+1,x} / A (e_m = v_{m+1} - v_m), and
+ *                           l in place of w.  Level l1 is not read when f = 0.  No gradient flows through the LOD.
+ * Backward: the exact derivative of the above with the cells, the levels, the UV clamp (gated per axis), the nearest edge,
+ * the lh clamp and the cut-off held fixed.  With h = w_j g / Z (d L / d C_j of nr_b200_soft_rgb) and s the unlit sample:
+ *   grad_textures:  every tap of the image (pyramid: of the pyramid; collapse it with nr_b200_mip_collapse) gets
+ *                   a_l * tap weight * light_c * h_c;
+ *   grad_face_light: h_c s_c;
+ *   (gu, gv) = d L / d uv as NR_TEX_UV's face_uvs gradient with h_c light_c; grad_face_uvs[k] += l'_k (gu, gv) (summed over
+ *                   the items with NR_UV_SHARED);
+ *   vertices:       d L / d l'_k = gu u_k + gv v_k, on through l, zp and z_k, then as nr_b200_soft_rgb into x, y and z.
+ *   Every gradient output is zero-filled first unless NR_GRAD_ACCUMULATE.  fp32 atomics, not bit-pinned.
+ * uv NULL runs exactly nr_b200_soft_rgb / nr_b200_soft_rgb_backward.  With uv: NR_TEX_UV is required; NR_UV_SHARED,
+ * NR_TEX_MIPMAP, NR_TEX_SHARED (one image for every item), NR_FACES_INDEXED, NR_INDICES_SHARED and NR_GRAD_ACCUMULATE are
+ * allowed; `textures` is the image [Bt,Ht,Wt,3] or the pyramid [Bt,P,3]; texture_size and eps are ignored.
+ * Scratch: the cube call's, nr_b200_soft_rgb_workspace_bytes(B, F, S, flags & ~(NR_TEX_UV | NR_UV_SHARED | NR_TEX_MIPMAP)).
+ * Host rejections before any launch: every rejection of nr_b200_soft_rgb that still applies, a struct_size of either
+ * struct other than its sizeof, no NR_TEX_UV, NULL face_uvs, Ht or Wt < 1, NR_TEX_FILL_BACK, NR_GRAD_INTERIOR,
+ * NR_RETURN_*, NR_ANTI_ALIASING or any unknown flag (NR_ERR_INVALID_ARG); then image or UV offsets beyond 32 bits
+ * (NR_ERR_UNSUPPORTED); then the workspace as nr_b200_soft_rgb. */
+typedef struct nr_b200_soft_uv_args {
+    uint32_t struct_size;          /* sizeof(nr_b200_soft_uv_args) */
+    int32_t texture_height;        /* Ht >= 1 (level 0) */
+    int32_t texture_width;         /* Wt >= 1 */
+    int32_t _pad0;
+    const float *face_uvs;         /* [B,F,3,2], or [F,3,2] with NR_UV_SHARED */
+    float *grad_face_uvs;          /* backward: layout of face_uvs, or NULL = not wanted */
+} nr_b200_soft_uv_args;
+
 /* ABI version of the loaded library (== NR_B200_ABI_VERSION it was built with). */
 NR_B200_API int nr_b200_abi_version(void);
 NR_B200_API const char *nr_b200_error_string(int code);
@@ -712,6 +752,10 @@ NR_B200_API int nr_b200_soft_silhouettes_backward(const nr_b200_soft_args *args,
 NR_B200_API size_t nr_b200_soft_rgb_workspace_bytes(int32_t batch_size, int32_t num_faces, int32_t image_size, uint32_t flags);
 NR_B200_API int nr_b200_soft_rgb(const nr_b200_soft_rgb_args *args, void *cuda_stream);
 NR_B200_API int nr_b200_soft_rgb_backward(const nr_b200_soft_rgb_args *args, void *cuda_stream);
+/* Soft RGB through a texture image (nr_b200_soft_uv_args above); uv NULL runs exactly the two calls above. */
+NR_B200_API int nr_b200_soft_rgb_uv(const nr_b200_soft_rgb_args *args, const nr_b200_soft_uv_args *uv, void *cuda_stream);
+NR_B200_API int nr_b200_soft_rgb_uv_backward(const nr_b200_soft_rgb_args *args, const nr_b200_soft_uv_args *uv,
+                                             void *cuda_stream);
 
 /* vertices_to_faces (reference vertices_to_faces.py:4-21), the step either side of the rasterizer:
  *   forward   out_faces[b,f,k,:] = vertices[b, faces[b,f,k], :]           ([B,Nv,3] x [B,Nf,3] int32 -> [B,Nf,3,3])

@@ -64,6 +64,8 @@ EXPORTED_SYMBOLS = (
     "nr_b200_soft_rgb_workspace_bytes",
     "nr_b200_soft_rgb",
     "nr_b200_soft_rgb_backward",
+    "nr_b200_soft_rgb_uv",
+    "nr_b200_soft_rgb_uv_backward",
     "nr_b200_vertices_to_faces",
     "nr_b200_vertices_to_faces_backward",
     "nr_b200_camera_transform",
@@ -215,6 +217,13 @@ class SoftRgbArgs(ctypes.Structure):
     ]
 
 
+class SoftUvArgs(ctypes.Structure):
+    _fields_ = [
+        ("struct_size", ctypes.c_uint32), ("texture_height", ctypes.c_int32), ("texture_width", ctypes.c_int32),
+        ("_pad0", ctypes.c_int32), ("face_uvs", ctypes.c_void_p), ("grad_face_uvs", ctypes.c_void_p),
+    ]
+
+
 SOFT_BG_DEPTH = 1e-3  # NR_SOFT_BG_DEPTH: the normalised depth of the soft RGB's background term
 
 
@@ -299,6 +308,10 @@ def load():
         fn = getattr(lib, name)
         fn.restype = ctypes.c_int
         fn.argtypes = [ctypes.POINTER(SoftRgbArgs), ctypes.c_void_p]
+    for name in ("nr_b200_soft_rgb_uv", "nr_b200_soft_rgb_uv_backward"):
+        fn = getattr(lib, name)
+        fn.restype = ctypes.c_int
+        fn.argtypes = [ctypes.POINTER(SoftRgbArgs), ctypes.POINTER(SoftUvArgs), ctypes.c_void_p]
     lib.nr_b200_vertices_to_faces.restype = ctypes.c_int
     lib.nr_b200_vertices_to_faces.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
                                               ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p]

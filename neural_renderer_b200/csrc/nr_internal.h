@@ -28,6 +28,17 @@ struct LaunchScope {
 // nr_backward.cu, also the tile scan of the soft silhouettes)
 void strip_scan(const int* cnt, int* off, int seg_len, long long seg_stride, int nseg, cudaStream_t stream);
 
+// The soft RGB's host half (nr_soft_rgb.cu), shared by the cube and the texture-image units.  `params` / `layout` point
+// to nr_soft_rgb.cuh's SoftRgbParams / SoftRgbLayout, which each unit compiles in its own anonymous namespace (as its
+// kernels), so they pass by address.
+//   soft_rgb_check      the NR_ERR_INVALID_ARG rules of nr_b200_soft_rgb(_backward) with `allowed` flags; cubes = false
+//                       skips texture_size and eps (the caller fills params->tex); fills everything but the workspace
+//   soft_rgb_workspace  NR_ERR_WORKSPACE / NR_ERR_CUDA: the layout (soft_rgb_layout) and the workspace pointers
+//   soft_rgb_bin        the tile binning (bin_faces_rgb): setup, scan, depth records and keys, sorted when `sort`
+int soft_rgb_check(const nr_b200_soft_rgb_args* a, uint32_t allowed, bool cubes, bool backward, void* params);
+int soft_rgb_workspace(const nr_b200_soft_rgb_args* a, void* params, void* layout);
+int soft_rgb_bin(void* params, const void* layout, bool sort, cudaStream_t stream);
+
 // FaceSrc / FaceGrad of a call from its ABI arguments; false = missing pointers for the chosen geometry form
 inline bool make_face_src(uint32_t flags, const float* faces, const float* vertices, const int32_t* indices, int F, int Nv,
                           nr::FaceSrc* s) {

@@ -12,6 +12,8 @@
 //   k_soft_rgb_bwd    the same traversal of the unsorted lists: 12 partials per face (x, y, z of three vertices, three
 //                     light channels) reduced over the warp and the CTA; the 8-tap texture scatters of a warp merged in a
 //                     per-warp shared-memory cube when ts^3 3 <= kWarpCube, then flushed to global memory
+// The forward traversal is nr_soft_rgb.cuh's, with the cube sampler below.  The host checks, the workspace layout and
+// the binning are shared with nr_soft_uv.cu through nr_internal.h.
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
@@ -22,29 +24,12 @@
 #include "nr_b200.h"
 #include "nr_internal.h"
 #include "nr_soft.cuh"
+#include "nr_soft_rgb.cuh"
 #include "nr_texture.cuh"
 
 namespace {
 
 constexpr int kWarpCube = 384;   // floats of a warp's texture-gradient cube (ts <= 5)
-constexpr int kWarps = kThreads / 32;
-
-struct SoftRgbParams {
-    SoftParams s;          // the silhouettes' binning and alpha (s.g = grad_alpha)
-    float4* zrec;          // [B*F] {z0, z1, z2, A}: vertex depths and the doubled signed area
-    void* keys;            // [B*F*kWideTiles] composite keys (uint32_t or uint64_t)
-    nr::Texture tex;       // cubes [Bt,F,ts,ts,ts,3]
-    const float* light;    // [B,F,3] face_light or nullptr
-    float* rgb;            // [B,3,S,S]
-    float* state;          // [B,2,S,S]: Z, zref
-    const float* g_rgb;    // [B,3,S,S] or nullptr
-    float* grad_tex;       // like tex, or nullptr
-    float* grad_light;     // [B,F,3] or nullptr
-    int ts, fbits;
-    float bg[3];
-    float zp_bg;           // far - NR_SOFT_BG_DEPTH (far - near): the depth of the background level
-    float inv_fg;          // 1 / ((far - near) gamma)
-};
 
 template <typename K>
 __global__ void __launch_bounds__(256) k_soft_rgb_keys(const __grid_constant__ SoftRgbParams p) {
@@ -83,76 +68,17 @@ __global__ void __launch_bounds__(256) k_soft_rgb_fill(const __grid_constant__ S
     }
 }
 
-// Stages the next <= kThreads faces of the tile in list order (its own list, then the wide list with a box test): the
-// slots come from a block-wide scan of the ballots, so slot order is list order.  Returns how many were staged.
-template <typename K>
-__device__ __forceinline__ int stage_rgb(const SoftRgbParams& p, int b, int tile, int tx, int ty, int n_tile, int n_all,
-                                         int next, float4* s_rec, float4* s_z, int* s_face, int* s_wn) {
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int i = next + tid;
-    const size_t seg = (size_t)b * (p.s.ntiles + 1);
-    const K* keys = (const K*)p.keys;
-    const K mask = ((K)1 << p.fbits) - 1;
-    int f = -1;
-    if (i < n_tile) {
-        f = (int)(keys[p.s.off[seg + tile] + i] & mask);
-    } else if (i < n_all) {
-        f = (int)(keys[p.s.off[seg + p.s.ntiles] + (i - n_tile)] & mask);
-        const uint2 bb = __ldg(p.s.box + (size_t)b * p.s.F + f);
-        if (tx < lo16(bb.x) || tx > hi16(bb.x) || ty < lo16(bb.y) || ty > hi16(bb.y)) f = -1;
+// the forward colour of the per-face cubes: the trilinear sample at texture_coords(l, zp, z)
+struct CubeSampler {
+    __device__ __forceinline__ void color(const SoftRgbParams& p, int b, int f, const SoftBary& bc, const float4& z,
+                                          const float4*, float& r, float& g, float& bl) const {
+        const int ts = p.ts;
+        const nr::TexCoord tc = nr::texture_coords(bc.l, bc.zp, z.x, z.y, z.z, ts, p.tex.tex_cmp, p.tex.tex_val);
+        const float* cube = p.tex.tex + p.tex.cube_off(b, f, ts);
+        if (p.light) nr::cube_blend<true, true>(cube, tc, ts, false, p.light + ((size_t)b * p.s.F + f) * 3, r, g, bl);
+        else nr::cube_blend<false, true>(cube, tc, ts, false, nullptr, r, g, bl);
     }
-    const unsigned m = __ballot_sync(0xffffffffu, f >= 0);
-    if (lane == 0) s_wn[warp] = __popc(m);
-    __syncthreads();
-    int base = 0, n = 0;
-#pragma unroll
-    for (int w = 0; w < kWarps; w++) {
-        const int c = s_wn[w];
-        base += w < warp ? c : 0;
-        n += c;
-    }
-    if (f >= 0) {
-        const int slot = base + __popc(m & ((1u << lane) - 1u));
-        const size_t id = (size_t)b * p.s.F + f;
-        const float4* r = p.s.rec + id * 4;
-#pragma unroll
-        for (int k = 0; k < 4; k++) s_rec[slot * 4 + k] = __ldg(r + k);
-        s_z[slot] = __ldg(p.zrec + id);
-        s_face[slot] = f;
-    }
-    __syncthreads();
-    return n;
-}
-
-// the soft RGB barycentrics of a pixel (include/nr_b200.h): lam_k = c_{k+1} / A, clamped to [0, 1] (lh), renormalised
-// (l = lh / s), and the perspective-correct depth zp = 1 / sum_k l_k / z_k
-struct SoftBary {
-    float lam[3], l[3], s, zp;
 };
-__device__ __forceinline__ SoftBary soft_bary(const float c[3], const float4& z) {
-    SoftBary o;
-    const float zz[3] = {z.x, z.y, z.z};
-    float lh[3];
-#pragma unroll
-    for (int k = 0; k < 3; k++) {
-        o.lam[k] = __fdiv_rn(c[k == 2 ? 0 : k + 1], z.w);
-        lh[k] = fminf(fmaxf(o.lam[k], 0.0f), 1.0f);
-    }
-    o.s = __fadd_rn(__fadd_rn(lh[0], lh[1]), lh[2]);
-    float q = 0.0f;
-#pragma unroll
-    for (int k = 0; k < 3; k++) {
-        o.l[k] = __fdiv_rn(lh[k], o.s);
-        q = __fadd_rn(q, __fdiv_rn(o.l[k], zz[k]));
-    }
-    o.zp = __frcp_rn(q);
-    return o;
-}
-
-__device__ __forceinline__ float soft_sigmoid(float x) {
-    const float e = expf(-fabsf(x));
-    return x >= 0.0f ? __frcp_rn(1.0f + e) : __fdiv_rn(e, 1.0f + e);
-}
 
 // ------------------------------------------------------------------------------------------------ k_soft_rgb_fwd
 template <typename K>
@@ -161,63 +87,7 @@ __global__ void __launch_bounds__(kThreads) k_soft_rgb_fwd(const __grid_constant
     __shared__ float4 s_z[kThreads];
     __shared__ int s_face[kThreads];
     __shared__ int s_wn[kWarps];
-    const int tile = blockIdx.x, b = blockIdx.y;
-    const int tx = tile % p.s.ntx, ty = tile / p.s.ntx;
-    const int col = tx * kTile + (threadIdx.x % kTile), row = ty * kTile + (threadIdx.x / kTile);
-    const int S = p.s.S, ts = p.ts;
-    const float px = soft_centre(col, S), py = soft_centre(S - 1 - row, S);
-    const size_t seg = (size_t)b * (p.s.ntiles + 1);
-    const int n_tile = p.s.cnt[seg + tile], n_all = n_tile + p.s.cnt[seg + p.s.ntiles];
-    const unsigned long long cap = (unsigned long long)(kTermCap * kFix);
-    unsigned long long acc = 0;  // alpha exactly as k_soft_fwd
-    // running-max softmax: zref = the smallest depth so far (the background level first), Z and N relative to it
-    float zref = p.zp_bg, Z = 1.0f, N0 = p.bg[0], N1 = p.bg[1], N2 = p.bg[2];
-    for (int next = 0; next < n_all; next += kThreads) {
-        const int n = stage_rgb<K>(p, b, tile, tx, ty, n_tile, n_all, next, s_rec, s_z, s_face, s_wn);
-        for (int j = 0; j < n; j++) {
-            float x, t, qx, qy, c[3];
-            int k;
-            if (!soft_eval(s_rec + 4 * j, px, py, p.s.inv_sigma, p.s.cut, x, k, t, qx, qy, c)) continue;
-            const float sp = fmaxf(x, 0.0f) + log1pf(expf(-fabsf(x)));
-            acc += (unsigned long long)__float2ll_rn(fminf(sp, kTermCap) * kFix);
-            acc = acc < cap ? acc : cap;
-            const float4 z = s_z[j];
-            if (z.w == 0.0f) continue;  // a zero-area face: alpha only
-            const SoftBary bc = soft_bary(c, z);
-            const float D = soft_sigmoid(x);
-            float w;
-            if (bc.zp < zref) {
-                const float sc = expf(__fmul_rn(__fsub_rn(bc.zp, zref), p.inv_fg));
-                Z = __fmul_rn(Z, sc); N0 = __fmul_rn(N0, sc); N1 = __fmul_rn(N1, sc); N2 = __fmul_rn(N2, sc);
-                zref = bc.zp;
-                w = D;
-            } else {
-                w = __fmul_rn(D, expf(__fmul_rn(__fsub_rn(zref, bc.zp), p.inv_fg)));
-                if (w == 0.0f) continue;  // its cube is not read
-            }
-            const int f = s_face[j];
-            const nr::TexCoord tc = nr::texture_coords(bc.l, bc.zp, z.x, z.y, z.z, ts, p.tex.tex_cmp, p.tex.tex_val);
-            const float* cube = p.tex.tex + p.tex.cube_off(b, f, ts);
-            float r, g, bl;
-            if (p.light) nr::cube_blend<true, true>(cube, tc, ts, false, p.light + ((size_t)b * p.s.F + f) * 3, r, g, bl);
-            else nr::cube_blend<false, true>(cube, tc, ts, false, nullptr, r, g, bl);
-            Z = __fadd_rn(Z, w);
-            N0 = __fmaf_rn(w, r, N0); N1 = __fmaf_rn(w, g, N1); N2 = __fmaf_rn(w, bl, N2);
-        }
-        __syncthreads();
-    }
-    if (row < S && col < S) {
-        const size_t plane = (size_t)S * S, o = (size_t)row * S + col;
-        const float lam = __ull2float_rn(acc) * (1.0f / kFix);
-        __stcs(p.s.alpha + b * plane + o, -expm1f(-lam));
-        float* rgb = p.rgb + (size_t)b * 3 * plane + o;
-        __stcs(rgb, __fdiv_rn(N0, Z));
-        __stcs(rgb + plane, __fdiv_rn(N1, Z));
-        __stcs(rgb + 2 * plane, __fdiv_rn(N2, Z));
-        float* st = p.state + (size_t)b * 2 * plane + o;
-        __stcs(st, Z);
-        __stcs(st + plane, zref);
-    }
+    soft_rgb_fwd_body<K>(p, CubeSampler{}, s_rec, s_z, s_face, s_wn);
 }
 
 // ------------------------------------------------------------------------------------------------ k_soft_rgb_bwd
@@ -424,15 +294,6 @@ __global__ void __launch_bounds__(kThreads) k_soft_rgb_bwd(const __grid_constant
     }
 }
 
-// soft RGB workspace = the silhouettes' records, boxes, counters, cursors and offsets | depth records | keys | sorted
-// keys | CUB scratch.  The keys are 32-bit when (B (ntiles + 1)) << fbits fits, else 64-bit.
-struct SoftRgbLayout {
-    SoftLayout s;
-    size_t zrec, keys, keys_out, temp, temp_bytes, total;
-    int fbits, end_bit;
-    bool wide;
-};
-
 template <typename K>
 bool sort_temp_bytes(size_t n, int end_bit, size_t* bytes) {
     *bytes = 0;
@@ -464,62 +325,6 @@ bool soft_rgb_layout(int B, int F, int S, SoftRgbLayout* L) {
 }
 
 constexpr uint32_t kSoftRgbFlags = NR_FACES_INDEXED | NR_INDICES_SHARED | NR_TEX_SHARED | NR_GRAD_ACCUMULATE;
-
-// the host checks of both soft RGB entry points; fills `p` and `L` on success
-int soft_rgb_setup(const nr_b200_soft_rgb_args* a, bool backward, SoftRgbParams* p, SoftRgbLayout* L) {
-    nr_internal::launch_count() = 0;
-    if (!a || a->struct_size != sizeof(nr_b200_soft_rgb_args)) return NR_ERR_INVALID_ARG;
-    const uint32_t flags = a->flags;
-    if (flags & ~kSoftRgbFlags) return NR_ERR_INVALID_ARG;
-    const int B = a->batch_size, F = a->num_faces, S = a->image_size, ts = a->texture_size;
-    if (!soft_sizes_ok(B, F, S)) return NR_ERR_INVALID_ARG;
-    const float sigma = a->sigma, gamma = a->gamma;
-    if (!isfinite(sigma) || !(sigma > 0.0f) || !isfinite(gamma) || !(gamma > 0.0f)) return NR_ERR_INVALID_ARG;
-    if (!(a->near_ < a->far_) || !isfinite(a->far_ - a->near_) || !isfinite(a->eps)) return NR_ERR_INVALID_ARG;
-    memset(p, 0, sizeof(*p));
-    if (!nr_internal::make_face_src(flags, a->faces, a->vertices, a->face_indices, F, a->num_vertices, &p->s.src))
-        return NR_ERR_INVALID_ARG;
-    if (ts < 2 || (long long)ts * ts * ts * 3 > 0x7FFFFFFFll || !a->textures) return NR_ERR_INVALID_ARG;
-    if (!a->rgb || !a->alpha || !a->state) return NR_ERR_INVALID_ARG;
-    if (backward) {
-        const bool indexed = (flags & NR_FACES_INDEXED) != 0;
-        if (indexed ? a->grad_faces != nullptr : a->grad_vertices != nullptr) return NR_ERR_INVALID_ARG;
-        if (!nr_internal::make_face_grad(flags, a->grad_faces, a->grad_vertices, a->face_indices, F, a->num_vertices,
-                                         &p->s.dst))
-            return NR_ERR_INVALID_ARG;
-    }
-    if (!a->workspace || ((uintptr_t)a->workspace & 15)) return NR_ERR_WORKSPACE;
-    if (!soft_rgb_layout(B, F, S, L)) return NR_ERR_CUDA;
-    if (a->workspace_bytes < L->total) return NR_ERR_WORKSPACE;
-    char* ws = (char*)a->workspace;
-    SoftParams& s = p->s;
-    s.rec = (float4*)(ws + L->s.rec); s.box = (uint2*)(ws + L->s.box);
-    s.cnt = (int*)(ws + L->s.cnt); s.cursor = (int*)(ws + L->s.cursor); s.off = (int*)(ws + L->s.off);
-    s.alpha = a->alpha; s.g = a->grad_alpha;
-    s.B = B; s.F = F; s.S = S;
-    s.ntx = tiles_per_axis(S); s.ntiles = s.ntx * s.ntx;
-    const double cut = (double)sigma * log((1.0 - NR_SOFT_EPS) / NR_SOFT_EPS);
-    s.inv_sigma = (float)(1.0 / (double)sigma);
-    s.cut = (float)cut;
-    s.reach = (float)(sqrt(cut) * S * 0.5) + 1.0f;
-    s.near_ = a->near_; s.far_ = a->far_;
-    p->zrec = (float4*)(ws + L->zrec);
-    p->keys = ws + L->keys;
-    p->tex.tex = a->textures;
-    p->tex.cube_bstride = (flags & NR_TEX_SHARED) ? 0 : (size_t)F;
-    const double tmax = (double)(ts - 1) - a->eps;
-    p->tex.tex_cmp = nr_internal::float_le(tmax);
-    p->tex.tex_val = (float)tmax;
-    p->light = a->face_light;
-    p->rgb = a->rgb; p->state = a->state; p->g_rgb = a->grad_rgb;
-    p->grad_tex = a->grad_textures; p->grad_light = a->grad_face_light;
-    p->ts = ts; p->fbits = L->fbits;
-    for (int c = 0; c < 3; c++) p->bg[c] = a->background[c];
-    const double fn = (double)a->far_ - (double)a->near_;
-    p->zp_bg = (float)((double)a->far_ - NR_SOFT_BG_DEPTH * fn);
-    p->inv_fg = (float)(1.0 / (fn * (double)gamma));
-    return NR_OK;
-}
 
 // the silhouettes' setup and scan, then the depth records and keys (the forward: sentinels first, sorted after)
 template <typename K>
@@ -558,7 +363,7 @@ int bin_faces_rgb(SoftRgbParams& p, const SoftRgbLayout& L, bool sort, cudaStrea
 
 template <typename K>
 int soft_rgb_forward(SoftRgbParams& p, const SoftRgbLayout& L, cudaStream_t s) {
-    if (bin_faces_rgb<K>(p, L, true, s) != NR_OK) return NR_ERR_CUDA;
+    if (nr_internal::soft_rgb_bin(&p, &L, true, s) != NR_OK) return NR_ERR_CUDA;
     nr_internal::LaunchScope ls("k_soft_rgb_fwd", s);
     k_soft_rgb_fwd<K><<<dim3((unsigned)p.s.ntiles, (unsigned)p.s.B), kThreads, 0, s>>>(p);
     return NR_OK;
@@ -566,10 +371,95 @@ int soft_rgb_forward(SoftRgbParams& p, const SoftRgbLayout& L, cudaStream_t s) {
 
 template <typename K>
 int soft_rgb_backward(SoftRgbParams& p, const SoftRgbLayout& L, cudaStream_t s) {
-    if (bin_faces_rgb<K>(p, L, false, s) != NR_OK) return NR_ERR_CUDA;
+    if (nr_internal::soft_rgb_bin(&p, &L, false, s) != NR_OK) return NR_ERR_CUDA;
     nr_internal::LaunchScope ls("k_soft_rgb_bwd", s);
     k_soft_rgb_bwd<K><<<dim3((unsigned)p.s.ntiles, (unsigned)p.s.B), kThreads, 0, s>>>(p);
     return NR_OK;
+}
+
+}  // namespace
+
+namespace nr_internal {
+
+int soft_rgb_check(const nr_b200_soft_rgb_args* a, uint32_t allowed, bool cubes, bool backward, void* params) {
+    SoftRgbParams* p = (SoftRgbParams*)params;
+    if (!a || a->struct_size != sizeof(nr_b200_soft_rgb_args)) return NR_ERR_INVALID_ARG;
+    const uint32_t flags = a->flags;
+    if (flags & ~allowed) return NR_ERR_INVALID_ARG;
+    const int B = a->batch_size, F = a->num_faces, S = a->image_size, ts = a->texture_size;
+    if (!soft_sizes_ok(B, F, S)) return NR_ERR_INVALID_ARG;
+    const float sigma = a->sigma, gamma = a->gamma;
+    if (!isfinite(sigma) || !(sigma > 0.0f) || !isfinite(gamma) || !(gamma > 0.0f)) return NR_ERR_INVALID_ARG;
+    if (!(a->near_ < a->far_) || !isfinite(a->far_ - a->near_) || (cubes && !isfinite(a->eps))) return NR_ERR_INVALID_ARG;
+    memset(p, 0, sizeof(*p));
+    if (!make_face_src(flags, a->faces, a->vertices, a->face_indices, F, a->num_vertices, &p->s.src))
+        return NR_ERR_INVALID_ARG;
+    if (!a->textures || (cubes && (ts < 2 || (long long)ts * ts * ts * 3 > 0x7FFFFFFFll))) return NR_ERR_INVALID_ARG;
+    if (!a->rgb || !a->alpha || !a->state) return NR_ERR_INVALID_ARG;
+    if (backward) {
+        const bool indexed = (flags & NR_FACES_INDEXED) != 0;
+        if (indexed ? a->grad_faces != nullptr : a->grad_vertices != nullptr) return NR_ERR_INVALID_ARG;
+        if (!make_face_grad(flags, a->grad_faces, a->grad_vertices, a->face_indices, F, a->num_vertices, &p->s.dst))
+            return NR_ERR_INVALID_ARG;
+    }
+    SoftParams& s = p->s;
+    s.alpha = a->alpha; s.g = a->grad_alpha;
+    s.B = B; s.F = F; s.S = S;
+    s.ntx = tiles_per_axis(S); s.ntiles = s.ntx * s.ntx;
+    const double cut = (double)sigma * log((1.0 - NR_SOFT_EPS) / NR_SOFT_EPS);
+    s.inv_sigma = (float)(1.0 / (double)sigma);
+    s.cut = (float)cut;
+    s.reach = (float)(sqrt(cut) * S * 0.5) + 1.0f;
+    s.near_ = a->near_; s.far_ = a->far_;
+    if (cubes) {
+        p->tex.tex = a->textures;
+        p->tex.cube_bstride = (flags & NR_TEX_SHARED) ? 0 : (size_t)F;
+        const double tmax = (double)(ts - 1) - a->eps;
+        p->tex.tex_cmp = float_le(tmax);
+        p->tex.tex_val = (float)tmax;
+        p->ts = ts;
+    }
+    p->light = a->face_light;
+    p->rgb = a->rgb; p->state = a->state; p->g_rgb = a->grad_rgb;
+    p->grad_tex = a->grad_textures; p->grad_light = a->grad_face_light;
+    for (int c = 0; c < 3; c++) p->bg[c] = a->background[c];
+    const double fn = (double)a->far_ - (double)a->near_;
+    p->zp_bg = (float)((double)a->far_ - NR_SOFT_BG_DEPTH * fn);
+    p->inv_fg = (float)(1.0 / (fn * (double)gamma));
+    return NR_OK;
+}
+
+int soft_rgb_workspace(const nr_b200_soft_rgb_args* a, void* params, void* layout) {
+    SoftRgbParams* p = (SoftRgbParams*)params;
+    SoftRgbLayout* L = (SoftRgbLayout*)layout;
+    if (!a->workspace || ((uintptr_t)a->workspace & 15)) return NR_ERR_WORKSPACE;
+    if (!soft_rgb_layout(p->s.B, p->s.F, p->s.S, L)) return NR_ERR_CUDA;
+    if (a->workspace_bytes < L->total) return NR_ERR_WORKSPACE;
+    char* ws = (char*)a->workspace;
+    SoftParams& s = p->s;
+    s.rec = (float4*)(ws + L->s.rec); s.box = (uint2*)(ws + L->s.box);
+    s.cnt = (int*)(ws + L->s.cnt); s.cursor = (int*)(ws + L->s.cursor); s.off = (int*)(ws + L->s.off);
+    p->zrec = (float4*)(ws + L->zrec);
+    p->keys = ws + L->keys;
+    p->fbits = L->fbits;
+    return NR_OK;
+}
+
+int soft_rgb_bin(void* params, const void* layout, bool sort, cudaStream_t s) {
+    SoftRgbParams& p = *(SoftRgbParams*)params;
+    const SoftRgbLayout& L = *(const SoftRgbLayout*)layout;
+    return L.wide ? bin_faces_rgb<unsigned long long>(p, L, sort, s) : bin_faces_rgb<uint32_t>(p, L, sort, s);
+}
+
+}  // namespace nr_internal
+
+namespace {
+
+// the host checks of both soft RGB entry points; fills `p` and `L` on success
+int soft_rgb_setup(const nr_b200_soft_rgb_args* a, bool backward, SoftRgbParams* p, SoftRgbLayout* L) {
+    nr_internal::launch_count() = 0;
+    const int rc = nr_internal::soft_rgb_check(a, kSoftRgbFlags, true, backward, p);
+    return rc != NR_OK ? rc : nr_internal::soft_rgb_workspace(a, p, L);
 }
 
 }  // namespace

@@ -1186,6 +1186,75 @@ def _soft_rgb_args(lib, geom_c, indices, tex_c, light_c, cfg):
     return a, ws
 
 
+class _SoftUvFunction(torch.autograd.Function):
+    """autograd node of the soft RGB through a texture image: forward = nr_b200_soft_rgb_uv, backward =
+    nr_b200_soft_rgb_uv_backward.  `textures` is the image [B|1,Ht,Wt,3], or its packed pyramid [B|1,P,3] when `hw` =
+    (Ht, Wt) of level 0 is given (trilinear); `face_uvs` [B|1,F,3,2] (1 = shared)."""
+
+    @staticmethod
+    def forward(ctx, geom, textures, face_light, face_uvs, indices, cfg, hw):
+        lib = _lib.load()
+        dev = geom.device
+        geom_c = geom.detach().contiguous()
+        tex_c = textures.detach().contiguous()
+        uv_c = face_uvs.detach().contiguous()
+        light_c = face_light.detach().contiguous() if face_light is not None else None
+        B, S = geom_c.shape[0], cfg[0]
+        with torch.cuda.device(dev):
+            rgb = torch.empty((B, 3, S, S), dtype=torch.float32, device=dev)
+            alpha = torch.empty((B, S, S), dtype=torch.float32, device=dev)
+            state = torch.empty((B, 2, S, S), dtype=torch.float32, device=dev)
+            a, u, ws = _soft_uv_args(lib, geom_c, indices, tex_c, light_c, uv_c, cfg, hw)
+            a.rgb, a.alpha, a.state = _ptr(rgb), _ptr(alpha), _ptr(state)
+            _lib.check(lib.nr_b200_soft_rgb_uv(ctypes.byref(a), ctypes.byref(u), _stream_ptr(dev)))
+        ctx.cfg, ctx.hw = cfg, hw
+        ctx.save_for_backward(geom_c, tex_c, light_c, uv_c, indices, rgb, alpha, state)
+        return rgb, alpha
+
+    @staticmethod
+    def backward(ctx, g_rgb, g_alpha):
+        lib = _lib.load()
+        geom_c, tex_c, light_c, uv_c, indices, rgb, alpha, state = ctx.saved_tensors
+        dev = geom_c.device
+        need_geom, need_tex, need_light, need_uv = ctx.needs_input_grad[:4]
+        none = (None,) * 7
+        if not (need_geom or need_tex or need_light or need_uv) or (g_rgb is None and g_alpha is None):
+            return none
+        g_rgb = g_rgb.detach().to(torch.float32).contiguous() if g_rgb is not None else None
+        g_alpha = g_alpha.detach().to(torch.float32).contiguous() if g_alpha is not None else None
+        with torch.cuda.device(dev):
+            grad_geom = torch.empty_like(geom_c)
+            grad_tex = torch.empty_like(tex_c) if need_tex else None
+            grad_light = torch.empty_like(light_c) if need_light and light_c is not None else None
+            grad_uv = torch.empty_like(uv_c) if need_uv else None
+            a, u, ws = _soft_uv_args(lib, geom_c, indices, tex_c, light_c, uv_c, ctx.cfg, ctx.hw)
+            a.rgb, a.alpha, a.state = _ptr(rgb), _ptr(alpha), _ptr(state)
+            a.grad_rgb, a.grad_alpha = _ptr(g_rgb), _ptr(g_alpha)
+            if indices is not None:
+                a.grad_vertices = _ptr(grad_geom)
+            else:
+                a.grad_faces = _ptr(grad_geom)
+            a.grad_textures, a.grad_face_light = _ptr(grad_tex), _ptr(grad_light)
+            u.grad_face_uvs = _ptr(grad_uv)
+            _lib.check(lib.nr_b200_soft_rgb_uv_backward(ctypes.byref(a), ctypes.byref(u), _stream_ptr(dev)))
+        return grad_geom if need_geom else None, grad_tex, grad_light, grad_uv, None, None, None
+
+
+def _soft_uv_args(lib, geom_c, indices, tex_c, light_c, uv_c, cfg, hw):
+    """nr_b200_soft_rgb_args and nr_b200_soft_uv_args of a texture-image call, and the workspace (the cube call's)"""
+    a, ws = _soft_rgb_args(lib, geom_c, indices, tex_c, light_c, cfg)
+    a.flags |= _lib.NR_TEX_UV
+    if uv_c.shape[0] == 1 and geom_c.shape[0] > 1:
+        a.flags |= _lib.NR_UV_SHARED
+    if hw is not None:
+        a.flags |= _lib.NR_TEX_MIPMAP
+    u = _lib.SoftUvArgs()
+    u.struct_size = ctypes.sizeof(_lib.SoftUvArgs)
+    u.texture_height, u.texture_width = hw if hw is not None else (tex_c.shape[1], tex_c.shape[2])
+    u.face_uvs = _ptr(uv_c)
+    return a, u, ws
+
+
 def rasterize_soft(
         faces,
         textures,
@@ -1199,6 +1268,8 @@ def rasterize_soft(
         *,
         vertices=None,
         face_light=None,
+        face_uvs=None,
+        texture_filter='bilinear',
 ):
     """Soft RGB images [B,3,H,W] and soft silhouettes [B,H,W] (SoftRas, Liu et al. 2019): every face within reach of a
     pixel (the soft silhouettes' probability D_j, rasterize_soft_silhouettes) adds its texture colour with the weight
@@ -1213,7 +1284,12 @@ def rasterize_soft(
     (e.g. functional.face_light_from_vertices) multiplies every texel first; None = unlit.  gamma > 0 sets how sharply
     the nearer face wins.  Returns (rgb, alpha); alpha is bit-identical to rasterize_soft_silhouettes.  Deterministic
     forward.  Gradients into the geometry, the textures and face_light.  The exact definition is in include/nr_b200.h
-    (nr_b200_soft_rgb_args)."""
+    (nr_b200_soft_rgb_args).
+
+    With face_uvs [F,3,2] / [1|B,F,3,2] (UV of every face corner; an expanded set stays shared), `textures` is a texture
+    image [Ht,Wt,3] / [1|B,Ht,Wt,3] (row 0 = top) sampled at each face's perspective-correct UV: bilinearly, or through
+    a mip pyramid with texture_filter='trilinear' (as rasterize_rgbad samples images).  Gradients then also reach the
+    image and, when it requires grad, face_uvs (nr_b200_soft_uv_args)."""
     try:
         sigma, gamma = float(sigma), float(gamma)
     except (TypeError, ValueError):
@@ -1231,7 +1307,12 @@ def rasterize_soft(
         raise ValueError("background_color must have 3 components, got %r" % (background_color,))
     if face_light is not None and not isinstance(face_light, torch.Tensor):
         raise TypeError("face_light must be a torch.Tensor")
-    _check_inputs(faces, textures, True, face_light=face_light, vertices=vertices)  # the shapes, then the device check
+    if texture_filter not in TEXTURE_FILTERS:
+        raise ValueError("texture_filter must be one of %s, got %r" % (TEXTURE_FILTERS, texture_filter))
+    if texture_filter == 'trilinear' and face_uvs is None:
+        raise ValueError("texture_filter='trilinear' samples a texture image: it needs face_uvs")
+    # the shapes, then the device check
+    _check_inputs(faces, textures, True, face_light=face_light, vertices=vertices, face_uvs=face_uvs)
     indices = None
     if vertices is not None:
         geom = vertices if vertices.dtype == torch.float32 else vertices.float()
@@ -1241,12 +1322,21 @@ def rasterize_soft(
         indices = indices.to(torch.int32).contiguous()
     else:
         geom = faces if faces.dtype == torch.float32 else faces.float()
-    if textures.shape[0] > 1 and textures.stride(0) == 0:
-        textures = textures[:1]  # an expanded shared set stays one set
-    textures = textures if textures.dtype == torch.float32 else textures.float()
     if face_light is not None and face_light.dtype != torch.float32:
         face_light = face_light.float()
     cfg = (int(image_size), sigma, gamma, float(near), float(far), float(eps), tuple(bg))
+    if face_uvs is not None:
+        batch_size = geom.shape[0]
+        textures = _batched(textures, batch_size, 3)
+        face_uvs = _batched(face_uvs, batch_size, 3)
+        hw = None
+        if texture_filter == 'trilinear':
+            hw = (int(textures.shape[1]), int(textures.shape[2]))
+            textures = _MipPyramid.apply(textures)
+        return _SoftUvFunction.apply(geom, textures, face_light, face_uvs, indices, cfg, hw)
+    if textures.shape[0] > 1 and textures.stride(0) == 0:
+        textures = textures[:1]  # an expanded shared set stays one set
+    textures = textures if textures.dtype == torch.float32 else textures.float()
     return _SoftRgbFunction.apply(geom, textures, face_light, indices, cfg)
 
 

@@ -113,13 +113,15 @@ class Renderer(object):
             return rasterize_soft_silhouettes(faces, self.image_size, sigma, self.near, self.far, vertices=vertices)
         return rasterize_soft_silhouettes(F.vertices_to_faces(vertices, faces), self.image_size, sigma, self.near, self.far)
 
-    def render_soft(self, vertices, faces, textures, sigma=DEFAULT_SOFT_SIGMA, gamma=DEFAULT_SOFT_GAMMA):
+    def render_soft(self, vertices, faces, textures, sigma=DEFAULT_SOFT_SIGMA, gamma=DEFAULT_SOFT_GAMMA, face_uvs=None):
         """Soft RGB images [B,3,H,W] and soft silhouettes [B,H,W] (neural_renderer_b200.rasterize_soft) seen through this
         renderer's camera, with near / far, rasterizer_eps and background_color, lit by the flat light of the faces as
         given (functional.face_light_from_vertices).  textures: per-face cubes [B,F,ts,ts,ts,3] or [1,F,...].  As for the
         soft silhouettes, fill_back adds no copies (a copy would count twice), so a face seen from behind keeps its front
         face's light; anti_aliasing is ignored.  Flat shading only.  The gradient reaches `vertices` through the camera and
-        the light, and the textures."""
+        the light, and the textures.  With `face_uvs` [F,3,2] / [B,F,3,2], `textures` is a texture image [Ht,Wt,3] /
+        [1|B,Ht,Wt,3] sampled with `self.texture_filter` (as render), and a `face_uvs` with requires_grad gets a
+        gradient too."""
         if self.shading != 'flat':
             raise ValueError("render_soft supports shading='flat' only, got shading=%r" % (self.shading,))
         n_lights = self.lights.shape[-2] if isinstance(self.lights, torch.Tensor) else len(self.lights)
@@ -130,11 +132,12 @@ class Renderer(object):
         light_args = (self.light_intensity_ambient, self.light_intensity_directional, self.light_color_ambient,
                       self.light_color_directional, self.light_direction)
         args = (self.image_size, sigma, gamma, self.near, self.far, self.rasterizer_eps, self.background_color)
+        uv = dict(face_uvs=face_uvs, texture_filter=self.texture_filter if face_uvs is not None else 'bilinear')
         if self.fused and self._fusable(vertices, faces):
             light = F.face_light_from_vertices(vertices, faces, *light_args)
-            return rasterize_soft(faces, textures, *args, vertices=self._transform(vertices), face_light=light)
+            return rasterize_soft(faces, textures, *args, vertices=self._transform(vertices), face_light=light, **uv)
         light = F.face_light(F.vertices_to_faces(vertices, faces), *light_args)
-        return rasterize_soft(F.vertices_to_faces(self._transform(vertices), faces), textures, *args, face_light=light)
+        return rasterize_soft(F.vertices_to_faces(self._transform(vertices), faces), textures, *args, face_light=light, **uv)
 
     def render_depth(self, vertices, faces):
         if self.fused and self._fusable(vertices, faces):
