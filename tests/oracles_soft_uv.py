@@ -72,43 +72,21 @@ def lod(faces, l, zp, uvk, S, Ht, Wt, levels):
         return torch.nan_to_num(out, nan=0.0, neginf=0.0).clamp(0.0, levels - 1)
 
 
-def soft_uv(faces, tex, uvs, S, sigma, gamma, near=0.1, far=100.0, background=(0.0, 0.0, 0.0), face_light=None,
-            hw=None, cut_scale=1.0):
-    """(rgb [B,3,S,S], alpha [B,S,S]) in float64 of faces [B,F,3,3], uvs [1|B,F,3,2] and either an image
-    [1|B,Ht,Wt,3] (bilinear, hw None) or a packed pyramid [1|B,P,3] of an image of hw = (Ht, Wt) (trilinear)"""
-    faces = faces.to(torch.float64)
-    B, F = faces.shape[:2]
-    dev = faces.device
-    p = osoft.pixel_centres(S, device=dev)
-    P = p.shape[0]
-    part = osoft.participates(faces, near, far)
-    d2, inside = osoft.face_terms(faces, p)                               # [B,F,P]
-    x = torch.where(inside, d2 / sigma, -d2 / sigma)
-    on = part[..., None] & (inside | (d2 <= osoft.cut(sigma) * cut_scale))
-    alpha = osoft.alpha_from_x(x.transpose(1, 2), on.transpose(1, 2)).reshape(B, S, S)
-    D = torch.sigmoid(x)
-    A = orgb.doubled_area(faces)[..., None]                                # [B,F,1]
-    valid = on & (A != 0)
-    safeA = torch.where(A != 0, A, torch.ones_like(A))
-    c = orgb.edge_functions(faces, p)                                      # [B,F,3,P]
-    lam = c.roll(-1, dims=2) / safeA[:, :, None]                           # lam_k = c_{k+1} / A
-    lam = torch.where((A != 0)[:, :, None], lam, torch.full_like(lam, 1.0 / 3.0))
-    lh = lam.clamp(0.0, 1.0)
-    s = lh.sum(2, keepdim=True)
-    l = lh / torch.where(s > 0, s, torch.ones_like(s))
+def uv_terms(faces, tex, uvk, p, S, sigma, near, far, face_light, hw, cut_scale):
+    """(x, on, valid, zn, C) of soft_uv per (item, face, pixel) of faces [B,F,3,3] at p [P,2] / [B,P,2]; tex [B,...]
+    and uvk [B,F,3,2] float64 already expanded to the items"""
+    B = faces.shape[0]
+    x, on, valid, l, zp = orgb.bary_terms(faces, p, sigma, near, far, cut_scale)
     z = faces[..., 2][..., None]                                           # [B,F,3,1]
-    zp = 1.0 / (l / z).sum(2)                                              # [B,F,P]
     lp = l * zp[:, :, None] / z                                            # l'_k [B,F,3,P]
-    uvk = uvs.to(torch.float64).expand(B, -1, -1, -1)                      # [B,F,3,2]
     u = (lp * uvk[..., 0][..., None]).sum(2)
     v = (lp * uvk[..., 1][..., None]).sum(2)
-    tex = tex.to(torch.float64).expand(B, *tex.shape[1:])
     if hw is None:
         Ht, Wt = tex.shape[1:3]
         C = sample(tex.reshape(B, Ht * Wt, 3), 0, Ht, Wt, u, v)
     else:
         Ht, Wt = hw
-        off, hs, ws = level_table(Ht, Wt, dev)
+        off, hs, ws = level_table(Ht, Wt, faces.device)
         L = off.numel()
         ld = lod(faces, l, zp, uvk, S, Ht, Wt, L)
         l0 = ld.floor().long()
@@ -117,14 +95,30 @@ def soft_uv(faces, tex, uvs, S, sigma, gamma, near=0.1, far=100.0, background=(0
         C = (1 - f) * sample(tex, off[l0], hs[l0], ws[l0], u, v) + f * sample(tex, off[l1], hs[l1], ws[l1], u, v)
     if face_light is not None:
         C = C * face_light.to(torch.float64)[:, :, None, :]
-    zn = (far - zp) / (far - near)
-    neg = torch.full_like(zn, -math.inf)
-    zmax = torch.where(valid, zn, neg).amax(1).clamp_min(orgb.BG_DEPTH).detach()   # [B,P]
-    ex = torch.where(valid, (zn - zmax[:, None]) / gamma, neg)
-    w = torch.where(valid, D * torch.exp(ex), torch.zeros_like(D))        # [B,F,P]
-    wb = torch.exp((orgb.BG_DEPTH - zmax) / gamma)                         # [B,P]
-    bg = torch.tensor(background, dtype=torch.float64, device=dev)
-    num = (w[..., None] * torch.where(valid[..., None], C, torch.zeros_like(C))).sum(1) + wb[..., None] * bg
-    Z = w.sum(1) + wb
-    rgb = (num / Z[..., None]).reshape(B, S, S, 3).permute(0, 3, 1, 2)
-    return rgb, alpha
+    return x, on, valid, (far - zp) / (far - near), C
+
+
+def soft_uv(faces, tex, uvs, S, sigma, gamma, near=0.1, far=100.0, background=(0.0, 0.0, 0.0), face_light=None,
+            hw=None, cut_scale=1.0, pix=None):
+    """(rgb [B,3,S,S], alpha [B,S,S]) in float64 of faces [B,F,3,3], uvs [1|B,F,3,2] and either an image
+    [1|B,Ht,Wt,3] (bilinear, hw None) or a packed pyramid [1|B,P,3] of an image of hw = (Ht, Wt) (trilinear).  With pix
+    (flat pixel indices [P] or [B,P]): (rgb [B,3,P], alpha [B,P]) from the faces in reach only (osoft.sparse_eval)."""
+    tex = tex.to(torch.float64)
+    uvs = uvs.to(torch.float64)
+    if pix is not None:
+        def terms(b0, b1, idx, fc, p):
+            tc = tex[b0:b1] if tex.shape[0] > 1 else tex.expand(b1 - b0, *tex.shape[1:])
+            fl = None if face_light is None else osoft.take(face_light, b0, b1, idx)
+            return uv_terms(fc, tc, osoft.take(uvs, b0, b1, idx), p, S, sigma, near, far, fl, hw, cut_scale)
+        alpha, rgb = osoft.sparse_eval(faces, S, pix, sigma, near, far, cut_scale, terms,
+                                       orgb.softmax_blend(gamma, background))
+        return rgb, alpha
+    faces = faces.to(torch.float64)
+    B = faces.shape[0]
+    p = osoft.pixel_centres(S, device=faces.device)
+    x, on, valid, zn, C = uv_terms(faces, tex.expand(B, *tex.shape[1:]), uvs.expand(B, -1, -1, -1), p, S, sigma, near,
+                                   far, face_light, hw, cut_scale)
+    alpha = osoft.alpha_from_x(x.transpose(1, 2), on.transpose(1, 2)).reshape(B, S, S)
+    zmax = orgb.zmax_of(valid, zn).clamp_min(orgb.BG_DEPTH).detach()      # [B,P]
+    rgb = orgb.blend_finish(orgb.blend_sums(x, valid, zn, C, zmax, gamma), zmax, gamma, background)
+    return rgb.reshape(B, S, S, 3).permute(0, 3, 1, 2), alpha
