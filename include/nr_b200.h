@@ -681,6 +681,55 @@ typedef struct nr_b200_soft_uv_args {
     float *grad_face_uvs;          /* backward: layout of face_uvs, or NULL = not wanted */
 } nr_b200_soft_uv_args;
 
+/* Soft attribute images (within ABI 4, additive): nr_b200_soft_attributes / _backward take the soft RGB's arguments and
+ * this struct, and render C >= 1 arbitrary channels (per-vertex colours, soft depth, normals, positions, features) through
+ * the soft RGB's aggregation.  Geometry, pixel centres, the participation test, d_j^2, x_j, D_j, the cut-off, alpha
+ * (bit-identical to nr_b200_soft_silhouettes), zero-area faces (alpha only), l, zp, the weights w_j, the background level
+ * NR_SOFT_BG_DEPTH, the running-max softmax, its fixed face order and the rule that a face whose weight is exactly 0
+ * contributes nothing are exactly those of nr_b200_soft_rgb above.  Only the colour of a contributing (pixel, face j)
+ * differs: it is a C-vector A_j,
+ *   l'_k = l_k * (zp / z_k)  (div.rn: the l'_k of nr_b200_soft_rgb_uv),
+ *   A_jc = fma(l'_2, a_2c, fma(l'_1, a_1c, l'_0 * a_0c))  (the chain of nr_b200_interpolate), a_kc = corner k's attribute:
+ *   per corner [B,F,3,C] (corners in the face's own order), or with NR_ATTR_PER_VERTEX per vertex [B,Nv,C] through
+ *   face_indices (needs NR_FACES_INDEXED; an index outside [0, Nv) reads zeros).  NR_ATTR_SHARED: one set [F,3,C] /
+ *   [Nv,C] for every item.
+ *   out_c = (sum_j w_j A_jc + w_b bg_c) / Z, accumulated as the soft RGB's N_c (bg = background [C], or zeros when NULL).
+ * Every channel's arithmetic is independent of the others: channel c of a C-channel call is bit-identical to a C = 1 call
+ * with that channel alone.  state = {Z, zref} does not depend on the attributes: on the same geometry, sigma, gamma, near
+ * and far it is bit-identical to nr_b200_soft_rgb's.  A camera-z attribute (a_k = z_k) gives A_j = zp up to rounding: a
+ * soft depth map (its background is bg; far matches what the hard depth writes where nothing is covered).
+ * Backward: the exact derivative with the branches of nr_b200_soft_rgb held (the nearest edge and segment, the lh clamp,
+ * the cut-off, zref).  No gradient flows into the background.  With g_c = grad_out at the pixel, the saved out and Z, and
+ * h_c = w_j g_c / Z:
+ *   grad_attributes[corner k, or vertex face_indices[b,f,k], c] += l'_k h_c  (summed over the items with NR_ATTR_SHARED;
+ *                   out-of-range indices are skipped);
+ *   H = sum_c g_c (A_jc - out_c) / Z;   d L / d x_j = (1 - alpha) D_j grad_alpha + w_j (1 - D_j) H;
+ *   d L / d zp_j through the weight = -w_j H / ((far - near) gamma);
+ *   d L / d l'_k = sum_c h_c a_kc, on through l, zp, z_k and the edge functions into x, y and z exactly as
+ *                   nr_b200_soft_rgb_uv continues gu u_k + gv v_k.
+ *   grad_faces / grad_vertices and grad_attributes are zero-filled first unless NR_GRAD_ACCUMULATE.  fp32 atomics, not
+ *   bit-pinned.  grad_out / grad_alpha NULL = zeros; grad_attributes NULL = not wanted.
+ * From nr_b200_soft_rgb_args the calls read the geometry, sigma, gamma, near, far, alpha, state, grad_alpha,
+ * grad_faces / grad_vertices and the workspace; texture_size, eps and background[3] are ignored, and textures,
+ * face_light, rgb, grad_rgb, grad_textures and grad_face_light must be NULL.  Allowed flags: NR_FACES_INDEXED,
+ * NR_INDICES_SHARED, NR_ATTR_PER_VERTEX, NR_ATTR_SHARED, NR_GRAD_ACCUMULATE.
+ * Scratch: the soft RGB's, nr_b200_soft_rgb_workspace_bytes(B, F, S, flags & (NR_FACES_INDEXED | NR_INDICES_SHARED |
+ * NR_GRAD_ACCUMULATE)).
+ * Host rejections before any launch: NR_ERR_INVALID_ARG for a struct_size of either struct other than its sizeof, C < 1,
+ * a NULL attributes or out, NR_ATTR_PER_VERTEX without NR_FACES_INDEXED, any other flag, a non-NULL rgb-only pointer
+ * above, and every rejection of nr_b200_soft_rgb that still applies (NULL alpha or state included); then
+ * NR_ERR_UNSUPPORTED when the attribute set (or its gradient) holds more than 2^31 - 1 floats (32-bit offsets); then the
+ * workspace as nr_b200_soft_rgb. */
+typedef struct nr_b200_soft_attr_args {
+    uint32_t struct_size;          /* sizeof(nr_b200_soft_attr_args) */
+    int32_t channels;              /* C >= 1 */
+    const float *attributes;       /* [B,F,3,C] / [B,Nv,C] (no B with NR_ATTR_SHARED) */
+    const float *background;       /* [C], or NULL = zeros */
+    float *out;                    /* [B,C,S,S]: written by the forward (row 0 at the top), read by the backward */
+    const float *grad_out;         /* backward: [B,C,S,S] or NULL (zeros) */
+    float *grad_attributes;        /* backward: layout of attributes, or NULL = not wanted */
+} nr_b200_soft_attr_args;
+
 /* ABI version of the loaded library (== NR_B200_ABI_VERSION it was built with). */
 NR_B200_API int nr_b200_abi_version(void);
 NR_B200_API const char *nr_b200_error_string(int code);
@@ -756,6 +805,12 @@ NR_B200_API int nr_b200_soft_rgb_backward(const nr_b200_soft_rgb_args *args, voi
 NR_B200_API int nr_b200_soft_rgb_uv(const nr_b200_soft_rgb_args *args, const nr_b200_soft_uv_args *uv, void *cuda_stream);
 NR_B200_API int nr_b200_soft_rgb_uv_backward(const nr_b200_soft_rgb_args *args, const nr_b200_soft_uv_args *uv,
                                              void *cuda_stream);
+/* Soft attribute images (nr_b200_soft_attr_args above): out [B,C,S,S], alpha and state, and the backward into the
+ * geometry and grad_attributes. */
+NR_B200_API int nr_b200_soft_attributes(const nr_b200_soft_rgb_args *args, const nr_b200_soft_attr_args *attr,
+                                        void *cuda_stream);
+NR_B200_API int nr_b200_soft_attributes_backward(const nr_b200_soft_rgb_args *args, const nr_b200_soft_attr_args *attr,
+                                                 void *cuda_stream);
 
 /* vertices_to_faces (reference vertices_to_faces.py:4-21), the step either side of the rasterizer:
  *   forward   out_faces[b,f,k,:] = vertices[b, faces[b,f,k], :]           ([B,Nv,3] x [B,Nf,3] int32 -> [B,Nf,3,3])

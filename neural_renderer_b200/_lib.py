@@ -66,6 +66,8 @@ EXPORTED_SYMBOLS = (
     "nr_b200_soft_rgb_backward",
     "nr_b200_soft_rgb_uv",
     "nr_b200_soft_rgb_uv_backward",
+    "nr_b200_soft_attributes",
+    "nr_b200_soft_attributes_backward",
     "nr_b200_vertices_to_faces",
     "nr_b200_vertices_to_faces_backward",
     "nr_b200_camera_transform",
@@ -224,6 +226,14 @@ class SoftUvArgs(ctypes.Structure):
     ]
 
 
+class SoftAttrArgs(ctypes.Structure):
+    _fields_ = [
+        ("struct_size", ctypes.c_uint32), ("channels", ctypes.c_int32),
+        ("attributes", ctypes.c_void_p), ("background", ctypes.c_void_p), ("out", ctypes.c_void_p),
+        ("grad_out", ctypes.c_void_p), ("grad_attributes", ctypes.c_void_p),
+    ]
+
+
 SOFT_BG_DEPTH = 1e-3  # NR_SOFT_BG_DEPTH: the normalised depth of the soft RGB's background term
 
 
@@ -312,6 +322,10 @@ def load():
         fn = getattr(lib, name)
         fn.restype = ctypes.c_int
         fn.argtypes = [ctypes.POINTER(SoftRgbArgs), ctypes.POINTER(SoftUvArgs), ctypes.c_void_p]
+    for name in ("nr_b200_soft_attributes", "nr_b200_soft_attributes_backward"):
+        fn = getattr(lib, name)
+        fn.restype = ctypes.c_int
+        fn.argtypes = [ctypes.POINTER(SoftRgbArgs), ctypes.POINTER(SoftAttrArgs), ctypes.c_void_p]
     lib.nr_b200_vertices_to_faces.restype = ctypes.c_int
     lib.nr_b200_vertices_to_faces.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
                                               ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p]

@@ -31,11 +31,13 @@ void strip_scan(const int* cnt, int* off, int seg_len, long long seg_stride, int
 // The soft RGB's host half (nr_soft_rgb.cu), shared by the cube and the texture-image units.  `params` / `layout` point
 // to nr_soft_rgb.cuh's SoftRgbParams / SoftRgbLayout, which each unit compiles in its own anonymous namespace (as its
 // kernels), so they pass by address.
-//   soft_rgb_check      the NR_ERR_INVALID_ARG rules of nr_b200_soft_rgb(_backward) with `allowed` flags; cubes = false
-//                       skips texture_size and eps (the caller fills params->tex); fills everything but the workspace
+//   soft_rgb_check      the NR_ERR_INVALID_ARG rules of nr_b200_soft_rgb(_backward) with `allowed` flags for the colour
+//                       source `src`: kSoftImage skips texture_size and eps (the caller fills params->tex), kSoftAttributes
+//                       also textures and rgb (nr_soft_attr.cu has its own colour buffers); fills everything but the workspace
 //   soft_rgb_workspace  NR_ERR_WORKSPACE / NR_ERR_CUDA: the layout (soft_rgb_layout) and the workspace pointers
 //   soft_rgb_bin        the tile binning (bin_faces_rgb): setup, scan, depth records and keys, sorted when `sort`
-int soft_rgb_check(const nr_b200_soft_rgb_args* a, uint32_t allowed, bool cubes, bool backward, void* params);
+enum SoftColourSource { kSoftCubes, kSoftImage, kSoftAttributes };
+int soft_rgb_check(const nr_b200_soft_rgb_args* a, uint32_t allowed, SoftColourSource src, bool backward, void* params);
 int soft_rgb_workspace(const nr_b200_soft_rgb_args* a, void* params, void* layout);
 int soft_rgb_bin(void* params, const void* layout, bool sort, cudaStream_t stream);
 

@@ -381,8 +381,9 @@ int soft_rgb_backward(SoftRgbParams& p, const SoftRgbLayout& L, cudaStream_t s) 
 
 namespace nr_internal {
 
-int soft_rgb_check(const nr_b200_soft_rgb_args* a, uint32_t allowed, bool cubes, bool backward, void* params) {
+int soft_rgb_check(const nr_b200_soft_rgb_args* a, uint32_t allowed, SoftColourSource src, bool backward, void* params) {
     SoftRgbParams* p = (SoftRgbParams*)params;
+    const bool cubes = src == kSoftCubes, colour = src != kSoftAttributes;
     if (!a || a->struct_size != sizeof(nr_b200_soft_rgb_args)) return NR_ERR_INVALID_ARG;
     const uint32_t flags = a->flags;
     if (flags & ~allowed) return NR_ERR_INVALID_ARG;
@@ -394,8 +395,8 @@ int soft_rgb_check(const nr_b200_soft_rgb_args* a, uint32_t allowed, bool cubes,
     memset(p, 0, sizeof(*p));
     if (!make_face_src(flags, a->faces, a->vertices, a->face_indices, F, a->num_vertices, &p->s.src))
         return NR_ERR_INVALID_ARG;
-    if (!a->textures || (cubes && (ts < 2 || (long long)ts * ts * ts * 3 > 0x7FFFFFFFll))) return NR_ERR_INVALID_ARG;
-    if (!a->rgb || !a->alpha || !a->state) return NR_ERR_INVALID_ARG;
+    if ((colour && !a->textures) || (cubes && (ts < 2 || (long long)ts * ts * ts * 3 > 0x7FFFFFFFll))) return NR_ERR_INVALID_ARG;
+    if ((colour && !a->rgb) || !a->alpha || !a->state) return NR_ERR_INVALID_ARG;
     if (backward) {
         const bool indexed = (flags & NR_FACES_INDEXED) != 0;
         if (indexed ? a->grad_faces != nullptr : a->grad_vertices != nullptr) return NR_ERR_INVALID_ARG;
@@ -458,7 +459,7 @@ namespace {
 // the host checks of both soft RGB entry points; fills `p` and `L` on success
 int soft_rgb_setup(const nr_b200_soft_rgb_args* a, bool backward, SoftRgbParams* p, SoftRgbLayout* L) {
     nr_internal::launch_count() = 0;
-    const int rc = nr_internal::soft_rgb_check(a, kSoftRgbFlags, true, backward, p);
+    const int rc = nr_internal::soft_rgb_check(a, kSoftRgbFlags, nr_internal::kSoftCubes, backward, p);
     return rc != NR_OK ? rc : nr_internal::soft_rgb_workspace(a, p, L);
 }
 

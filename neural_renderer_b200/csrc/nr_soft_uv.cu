@@ -345,7 +345,7 @@ int soft_uv_setup(const nr_b200_soft_rgb_args* a, const nr_b200_soft_uv_args* uv
         return NR_ERR_INVALID_ARG;
     if (!(a->flags & NR_TEX_UV)) return NR_ERR_INVALID_ARG;
     memset(p, 0, sizeof(*p));
-    int rc = nr_internal::soft_rgb_check(a, kSoftUvFlags, false, backward, &p->r);
+    int rc = nr_internal::soft_rgb_check(a, kSoftUvFlags, nr_internal::kSoftImage, backward, &p->r);
     if (rc != NR_OK) return rc;
     const UvTexArgs t = {a->flags | NR_RETURN_RGB, a->batch_size, a->num_faces, 0, a->textures, 0.0f, uv->face_uvs,
                          uv->texture_height, uv->texture_width};

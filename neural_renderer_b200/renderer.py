@@ -7,7 +7,7 @@ import torch
 
 from . import functional as F
 from .rasterize import (DEFAULT_SOFT_GAMMA, DEFAULT_SOFT_SIGMA, rasterize, rasterize_attributes, rasterize_depth,
-                        rasterize_silhouettes, rasterize_soft, rasterize_soft_silhouettes)
+                        rasterize_silhouettes, rasterize_soft, rasterize_soft_attributes, rasterize_soft_silhouettes)
 
 
 class Renderer(object):
@@ -138,6 +138,50 @@ class Renderer(object):
             return rasterize_soft(faces, textures, *args, vertices=self._transform(vertices), face_light=light, **uv)
         light = F.face_light(F.vertices_to_faces(vertices, faces), *light_args)
         return rasterize_soft(F.vertices_to_faces(self._transform(vertices), faces), textures, *args, face_light=light, **uv)
+
+    def render_soft_attributes(self, vertices, faces, vertex_attributes=None, face_attributes=None,
+                               sigma=DEFAULT_SOFT_SIGMA, gamma=DEFAULT_SOFT_GAMMA, background=None):
+        """Soft attribute images [B,C,H,W] (neural_renderer_b200.rasterize_soft_attributes) seen through this renderer's
+        camera, with near / far: e.g. per-vertex colours, `render_soft_attributes(v, f, vertex_attributes=colours)`.
+        Exactly one of vertex_attributes [Nv,C] / [1|B,Nv,C] and face_attributes [F,3,C] / [1|B,F,3,C]; background: C
+        numbers or None (zeros).  As for render_soft, fill_back adds no copies (a copy would count twice) and
+        anti_aliasing is ignored.  No lighting.  The gradient reaches `vertices` through the camera from every face
+        within reach of a pixel, and the attributes."""
+        if (vertex_attributes is None) == (face_attributes is None):
+            raise TypeError("give exactly one of vertex_attributes= and face_attributes=")
+        args = (self.image_size, sigma, gamma, self.near, self.far)
+        transformed = self._transform(vertices)
+        if self.fused and self._fusable(vertices, faces):
+            return rasterize_soft_attributes(faces, *args, vertices=transformed, vertex_attributes=vertex_attributes,
+                                             face_attributes=face_attributes, background=background)
+        # op by op: materialised faces, per-vertex attributes gathered to the corners in torch (as render_attributes)
+        if vertex_attributes is not None:
+            va = vertex_attributes[None] if vertex_attributes.dim() == 2 else vertex_attributes
+            B, C = vertices.shape[0], va.shape[-1]
+            idx = faces.long().expand(B, -1, -1).reshape(B, -1, 1).expand(-1, -1, C)
+            face_attributes = torch.gather(va.expand(B, -1, -1), 1, idx).reshape(B, -1, 3, C)
+        return rasterize_soft_attributes(F.vertices_to_faces(transformed, faces), *args, face_attributes=face_attributes,
+                                         background=background)
+
+    def render_soft_depth(self, vertices, faces, sigma=DEFAULT_SOFT_SIGMA, gamma=DEFAULT_SOFT_GAMMA):
+        """Soft depth maps [B,H,W]: the camera z of the transformed vertices rendered by render_soft_attributes as a
+        one-channel per-vertex attribute, with the background at `far` (what render_depth writes where nothing is
+        covered).  Every face within reach of a pixel sends its depth a gradient -- hidden faces and faces just outside
+        a target outline included -- which the hard depth map does not.
+
+        SoftRas semantics: a pixel within reach of a face but outside it reads (nearly) that face's depth, not `far`.
+        The background sits at the normalised depth 1e-3, i.e. just in front of `far`, so its softmax weight is
+        exp(-zn / gamma) below that of any reached face at normalised depth zn; even a face's faint edge term D_j
+        outweighs it by far at a small gamma.  The soft depth map therefore spreads each silhouette by the cut-off reach
+        (about 1.2 px at sigma = 1e-5 and 256 x 256); compare it with a target only where the target is covered, or use
+        the soft silhouettes for the outline."""
+        transformed = self._transform(vertices)
+        args = (self.image_size, sigma, gamma, self.near, self.far)
+        if self.fused and self._fusable(vertices, faces):
+            return rasterize_soft_attributes(faces, *args, vertices=transformed, vertex_attributes=transformed[..., 2:3],
+                                             background=[self.far])[:, 0]
+        fv = F.vertices_to_faces(transformed, faces)
+        return rasterize_soft_attributes(fv, *args, face_attributes=fv[..., 2:3], background=[self.far])[:, 0]
 
     def render_depth(self, vertices, faces):
         if self.fused and self._fusable(vertices, faces):
