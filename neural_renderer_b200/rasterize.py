@@ -1422,6 +1422,19 @@ def _soft_attr_args(lib, geom_c, indices, attr_c, bg, per_vertex, cfg):
     return a, t, ws
 
 
+def _device_background(values, device):
+    """the background [C] float32 of a sequence of numbers on `device`: copied once per (values, device), then served
+    from the small-constant cache of the camera and light parameters, so later calls enqueue no host copy"""
+    from . import functional
+    import numpy as np
+    row = np.asarray(values, dtype=np.float32)
+    key = ("soft_background", row.tobytes(), str(device))
+    hit = functional._CAMERA_CACHE.get(key)
+    if hit is None:
+        hit = functional._cache_put(key, torch.from_numpy(row).to(device))
+    return hit
+
+
 def rasterize_soft_attributes(
         faces,
         image_size=DEFAULT_IMAGE_SIZE,
@@ -1449,7 +1462,13 @@ def rasterize_soft_attributes(
     item; its gradient is the sum over the items.  background: C numbers (or a tensor [C]) for the background term, None
     = zeros; it gets no gradient.  Each channel is computed on its own: channel c equals a one-channel render of it, bit
     for bit.  Deterministic forward.  Returns the image, or (image, alpha) with alpha bit-identical to
-    rasterize_soft_silhouettes.  The exact definition is in include/nr_b200.h (nr_b200_soft_attr_args)."""
+    rasterize_soft_silhouettes.  The exact definition is in include/nr_b200.h (nr_b200_soft_attr_args).
+
+    CUDA graphs: a background tensor on the geometry's device is read in place, so a call with one can be captured.  A
+    sequence of numbers is copied to the device on its first use and then cached per value and device, as the camera
+    and light constants are: the capture of a call with a sequence needs one eager call with the same values before it
+    (the usual warm-up does that), and a sequence first seen during a capture, or a background tensor on the host,
+    makes a synchronising host-to-device copy, which a capture refuses."""
     try:
         sigma, gamma = float(sigma), float(gamma)
     except (TypeError, ValueError):
@@ -1466,14 +1485,15 @@ def rasterize_soft_attributes(
     bg = None
     if background is not None:
         if isinstance(background, torch.Tensor):
-            bg = background.detach().reshape(-1).to(torch.float64).cpu()
+            bg = background.detach().reshape(-1)     # used where it lies: no host round trip
         else:
             try:
-                bg = torch.tensor([float(c) for c in background], dtype=torch.float64)
+                bg = tuple(float(c) for c in background)
             except (TypeError, ValueError):
                 raise TypeError("background must be a sequence of numbers or a tensor, got %r" % (background,))
-        if isinstance(attrs_in, torch.Tensor) and attrs_in.dim() >= 1 and bg.numel() != attrs_in.shape[-1]:
-            raise ValueError("background must have one value per channel (%d), got %d" % (attrs_in.shape[-1], bg.numel()))
+        n = bg.numel() if isinstance(bg, torch.Tensor) else len(bg)
+        if isinstance(attrs_in, torch.Tensor) and attrs_in.dim() >= 1 and n != attrs_in.shape[-1]:
+            raise ValueError("background must have one value per channel (%d), got %d" % (attrs_in.shape[-1], n))
     attrs, per_vertex = _check_attribute_inputs(faces, vertices, vertex_attributes, face_attributes)  # then the device
     indices = None
     if vertices is not None:
@@ -1485,8 +1505,10 @@ def rasterize_soft_attributes(
     else:
         geom = faces if faces.dtype == torch.float32 else faces.float()
     attrs = _batched(attrs, geom.shape[0], 2 if per_vertex else 3)  # an expanded shared set: NR_ATTR_SHARED
-    if bg is not None:
-        bg = bg.to(device=geom.device, dtype=torch.float32)
+    if isinstance(bg, torch.Tensor):
+        bg = bg.to(device=geom.device, dtype=torch.float32).contiguous()
+    elif bg is not None:
+        bg = _device_background(bg, geom.device)
     cfg = (int(image_size), sigma, gamma, float(near), float(far))
     image, alpha = _SoftAttrFunction.apply(geom, attrs, indices, bg, per_vertex, cfg)
     return (image, alpha) if return_alpha else image

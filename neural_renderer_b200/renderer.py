@@ -144,9 +144,10 @@ class Renderer(object):
         """Soft attribute images [B,C,H,W] (neural_renderer_b200.rasterize_soft_attributes) seen through this renderer's
         camera, with near / far: e.g. per-vertex colours, `render_soft_attributes(v, f, vertex_attributes=colours)`.
         Exactly one of vertex_attributes [Nv,C] / [1|B,Nv,C] and face_attributes [F,3,C] / [1|B,F,3,C]; background: C
-        numbers or None (zeros).  As for render_soft, fill_back adds no copies (a copy would count twice) and
-        anti_aliasing is ignored.  No lighting.  The gradient reaches `vertices` through the camera from every face
-        within reach of a pixel, and the attributes."""
+        numbers, a tensor [C] or None (zeros); rasterize_soft_attributes says which can be captured in a CUDA graph.
+        As for render_soft, fill_back adds no copies (a copy would count twice) and anti_aliasing is ignored.  No
+        lighting.  The gradient reaches `vertices` through the camera from every face within reach of a pixel, and the
+        attributes."""
         if (vertex_attributes is None) == (face_attributes is None):
             raise TypeError("give exactly one of vertex_attributes= and face_attributes=")
         args = (self.image_size, sigma, gamma, self.near, self.far)
@@ -177,11 +178,13 @@ class Renderer(object):
         the soft silhouettes for the outline."""
         transformed = self._transform(vertices)
         args = (self.image_size, sigma, gamma, self.near, self.far)
+        # the background made on the device: no host copy, so a step that calls this can be captured in a CUDA graph
+        far = torch.full((1,), float(self.far), dtype=torch.float32, device=transformed.device)
         if self.fused and self._fusable(vertices, faces):
             return rasterize_soft_attributes(faces, *args, vertices=transformed, vertex_attributes=transformed[..., 2:3],
-                                             background=[self.far])[:, 0]
+                                             background=far)[:, 0]
         fv = F.vertices_to_faces(transformed, faces)
-        return rasterize_soft_attributes(fv, *args, face_attributes=fv[..., 2:3], background=[self.far])[:, 0]
+        return rasterize_soft_attributes(fv, *args, face_attributes=fv[..., 2:3], background=far)[:, 0]
 
     def render_depth(self, vertices, faces):
         if self.fused and self._fusable(vertices, faces):

@@ -174,6 +174,11 @@ TOL_PARAMS_ELEM_259 = 6e-4
 # moves with the order of K5's fp32 atomics: 8.5e-5 and 7.6e-5 per element in two runs on one H100, and over TOL_GRAD in a
 # third whose value was not kept.  Held at TOL_GRAD_ELEM_229; the cause is case 214's, at a smaller size.
 TOL_GRAD_ELEM_229 = 1.5e-4
+# Case 273 (shared image and UVs, Phong with SH through a normal map, sigma 16, fill_back) has an image gradient whose
+# largest element is 41.1, summed by fp32 atomics whose order changes from run to run.  Six runs of the same input on
+# one H100 (700 W) gave 1.3e-4, 1.1e-4, 5.0e-5, 1.1e-4, 7.2e-6 and 5.0e-5 per element -- a few ulps of the largest
+# addend, 5e-6 absolute, on an element below 1e-3 of the maximum -- and 2.3e-7 to 4.5e-7 per tensor.  That one gradient is held at TOL_TEX_ELEM_273; every other row keeps TOL_GRAD.
+TOL_TEX_ELEM_273 = 2.5e-4
 PHONG_INPUTS = ("corner_shading", "params", "lights", "sh")
 MAP_INPUTS = ("normal_map", "corner_tangents", "specular_map")
 CASES = abi_cases.cases()
@@ -633,6 +638,8 @@ def run_case(c, metrics=None):
             tol_elem = TOL_GRAD_ELEM_214
         if (c["id"], k) == (229, "grad_faces"):
             tol_elem = TOL_GRAD_ELEM_229
+        if (c["id"], k) == (273, "grad_textures"):
+            tol_elem = TOL_TEX_ELEM_273
         if (c["id"], k) == (259, "grad_params"):
             tol_elem = TOL_PARAMS_ELEM_259
         note(k, "tensor_interior" if interior else "tensor", e1)

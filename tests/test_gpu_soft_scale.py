@@ -197,8 +197,8 @@ def _count_blend():
 
 
 def check_forward(scene, rgb, alpha, S, sigma, gamma, pix, what):
-    """rgb [B,3,S,S] / alpha [B,S,S] at the pixels pix [B,P] against the sparse oracle under the gates of the
-    docstring; returns the largest error / gate ratios seen, for the record"""
+    """rgb [B,3,S,S] (or an attribute image [B,C,S,S]) / alpha [B,S,S] at the pixels pix [B,P] against the sparse
+    oracle under the gates of the docstring; returns the largest error / gate ratios seen, for the record"""
     B = scene.faces.shape[0]
     leaves = [x.detach() for x in scene.leaves()]
     terms = scene.oracle_terms(leaves, S, sigma)
@@ -209,7 +209,7 @@ def check_forward(scene, rgb, alpha, S, sigma, gamma, pix, what):
         _, g = osoft.sparse_eval(leaves[0], S, pix, sigma, NEAR, FAR, 1.0,
                                  _gate_terms(scene, terms, sigma, gamma, scene.colour_sensitivity()),
                                  _gate_blend(gamma, scene.bg))
-    edge = g[..., 6] > 0
+    edge = g[..., -1] > 0
     assert edge.double().mean().item() <= 0.01, (what, edge.double().mean().item())
     flat = lambda t: t.reshape(B, *t.shape[1:-2], S * S)   # noqa: E731
     got_a = torch.gather(flat(alpha).double(), 1, pix)
@@ -223,9 +223,10 @@ def check_forward(scene, rgb, alpha, S, sigma, gamma, pix, what):
                                            for b, i in bad.nonzero()[:8]])
     worst["alpha"] = (err_a / gate_a).masked_fill(edge, 0).max().item()
     if rgb is not None:
-        got = torch.gather(flat(rgb).double(), 2, pix[:, None].expand(-1, 3, -1)).permute(0, 2, 1)
-        err = (got - g[..., :3]).abs()
-        gate = torch.where((n <= 5)[..., None], torch.full_like(err, tol_rgb(sigma)), SAFETY * g[..., 3:6])
+        nc = rgb.shape[1]                                   # 3, or the channels of an attribute image
+        got = torch.gather(flat(rgb).double(), 2, pix[:, None].expand(-1, nc, -1)).permute(0, 2, 1)
+        err = (got - g[..., :nc]).abs()
+        gate = torch.where((n <= 5)[..., None], torch.full_like(err, tol_rgb(sigma)), SAFETY * g[..., nc:2 * nc])
         bad = (err > gate) & ~edge[..., None]
         assert not bad.any(), (what, "rgb", [(int(b), int(pix[b, i]), int(n[b, i]), err[b, i, c].item(), gate[b, i, c].item())
                                              for b, i, c in bad.nonzero()[:8]])

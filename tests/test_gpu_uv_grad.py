@@ -136,7 +136,11 @@ def test_directional_derivative_vs_central_difference(tf, hw):
 @pytest.mark.parametrize("tf", ["bilinear", "trilinear"])
 def test_rest_of_the_backward_is_unchanged(tf):
     """image, light and vertex gradients with and without face_uvs.requires_grad: the same pixels reach the same
-    atomics (their order is not fixed from run to run, hence a gate at fp32 noise rather than equality)"""
+    atomics (their order is not fixed from run to run, hence a gate at fp32 noise rather than equality).  Six runs of
+    each on one H100 (700 W), bilinear: the same call twice differs by up to 4.2e-7 per tensor in the image gradient
+    (2.1e-7 light, 5.4e-8 vertices), with against without face_uvs by up to 5.8e-7, and a run of the suite once went
+    past 1e-6: the gate is 3e-6, about 25 ulps of each tensor's largest element.  A lost or doubled contribution moves
+    an element by a whole pixel's share, far more than that."""
     B, F, H = 2, 400, 64
     faces0 = _faces(B, F, seed=41)
     uvs0, img0 = _spread_uvs((F, 3, 2), 0, 1, seed=42), _rand((1, 96, 80, 3), seed=43)
@@ -152,9 +156,9 @@ def test_rest_of_the_backward_is_unchanged(tf):
     (rgb0, gf0, gt0, gl0, gu0), (rgb1, gf1, gt1, gl1, gu1) = out
     assert gu0 is None and gu1 is not None and (gu1 != 0).any()
     assert torch.equal(rgb0, rgb1)
-    assert rel_err(np_(gt1), np_(gt0)) <= 1e-6
-    assert rel_err(np_(gl1), np_(gl0)) <= 1e-6
-    assert rel_err(np_(gf1), np_(gf0)) <= 1e-6
+    assert rel_err(np_(gt1), np_(gt0)) <= 3e-6
+    assert rel_err(np_(gl1), np_(gl0)) <= 3e-6
+    assert rel_err(np_(gf1), np_(gf0)) <= 3e-6
 
 
 @pytest.mark.parametrize("tf", ["bilinear", "trilinear"])
