@@ -730,6 +730,55 @@ typedef struct nr_b200_soft_attr_args {
     float *grad_attributes;        /* backward: layout of attributes, or NULL = not wanted */
 } nr_b200_soft_attr_args;
 
+/* Soft fragments (within ABI 4, additive): nr_b200_soft_fragments / _backward take the soft RGB's arguments and this
+ * struct, and return for every pixel the K nearest faces within reach (PyTorch3D's MeshRasterizer with faces_per_pixel =
+ * K and a blur radius), to be shaded and blended by the caller.  Pixel centres, the participation test, d_j^2, inside_j,
+ * x_j, the cut-off, A, the barycentrics lam, lh, l and zp, and l'_k = l_k (zp / z_k) (div.rn) are exactly those of
+ * nr_b200_soft_rgb and nr_b200_soft_attributes above.
+ *   Candidate: a (pixel, face j) is one when the face takes part, is within reach (inside, or d_j^2 within the cut-off),
+ *     has A != 0 (a zero-area face is not a fragment, as it is not a colour of the soft RGB) and a finite fp32 zp.
+ *   Selection: candidates are ordered by the key (zp, f) -- the fp32 zp first, the face index within the item second, a
+ *     total order that does not depend on the order of the lists -- and the first n = min(K, #candidates) are kept.  The
+ *     result is deterministic, and invariant under a permutation of the faces up to exact zp ties.  The first K1 slots
+ *     of a call with K2 > K1 are the K1 call's.
+ *   Outputs, slot k < n nearest first, row 0 at the top:
+ *     pix_to_face [B,S,S,K] int64: the face index within its item, in [0, F) (not packed b F + f);
+ *     zbuf        [B,S,S,K] float: zp;
+ *     bary        [B,S,S,K,3] float: l'_0, l'_1, l'_2, clipped and renormalised exactly as the soft attributes
+ *                 interpolate, so sum_k l'_k a_k is A_j of nr_b200_soft_attributes;
+ *     dists       [B,S,S,K] float: +d_j^2 inside, -d_j^2 outside, in squared NDC units (the d_j^2 soft_eval minimises,
+ *                 i.e. sigma x_j before the scaling by 1 / sigma), so sigmoid(dists / sigma) is SoftRas's D_j.  The sign
+ *                 is the OPPOSITE of PyTorch3D's dists (negative inside there).
+ *   Slots k >= n hold -1 in every field (bary: all three), as in PyTorch3D.
+ * Backward: the exact derivative with the selection held fixed, and with it the nearest edge and its segment branch, the
+ * lh clamp and the cut-off.  grad_zbuf, grad_bary and grad_dists (each NULL = zeros) flow into x, y and z of the
+ * vertices; empty slots are ignored.  zbuf and bary go through the chain of nr_b200_soft_attributes_backward from l'_k
+ * and zp (d L / d l'_k = grad_bary, d L / d zp = grad_zbuf); dists through d(+-d^2)/d(a, b) of the nearest edge (a, b),
+ * sigma times the silhouettes' d x_j / d(a, b), and nothing into z.  grad_faces / grad_vertices are zero-filled first
+ * unless NR_GRAD_ACCUMULATE; shared indices reduce over the items, out-of-range indices are skipped.  fp32 atomics, not
+ * bit-pinned.  The backward reads pix_to_face (the forward's) and the upstream gradients; zbuf, bary and dists are not
+ * read and may be NULL there.
+ * From nr_b200_soft_rgb_args the calls read the geometry, sigma, near, far, grad_faces / grad_vertices and the
+ * workspace; gamma, texture_size, eps and background[3] are ignored, and textures, face_light, rgb, alpha, state,
+ * grad_rgb, grad_alpha, grad_textures and grad_face_light must be NULL.  Allowed flags: NR_FACES_INDEXED,
+ * NR_INDICES_SHARED, NR_GRAD_ACCUMULATE.  1 <= K <= 32.
+ * Scratch: the soft RGB's, nr_b200_soft_rgb_workspace_bytes(B, F, S, flags).
+ * Host rejections before any launch: NR_ERR_INVALID_ARG for a struct_size of either struct other than its sizeof, K
+ * outside [1, 32], a NULL pix_to_face (and, in the forward, a NULL zbuf, bary or dists), a non-NULL pointer of the list
+ * above, any other flag, and every rejection of nr_b200_soft_rgb that still applies; then the workspace as
+ * nr_b200_soft_rgb. */
+typedef struct nr_b200_soft_frag_args {
+    uint32_t struct_size;          /* sizeof(nr_b200_soft_frag_args) */
+    int32_t faces_per_pixel;       /* K, 1 <= K <= 32 */
+    int64_t *pix_to_face;          /* [B,S,S,K]: written by the forward, read by the backward */
+    float *zbuf;                   /* [B,S,S,K]: forward */
+    float *bary;                   /* [B,S,S,K,3]: forward */
+    float *dists;                  /* [B,S,S,K]: forward */
+    const float *grad_zbuf;        /* backward: [B,S,S,K] or NULL (zeros) */
+    const float *grad_bary;        /* backward: [B,S,S,K,3] or NULL (zeros) */
+    const float *grad_dists;       /* backward: [B,S,S,K] or NULL (zeros) */
+} nr_b200_soft_frag_args;
+
 /* ABI version of the loaded library (== NR_B200_ABI_VERSION it was built with). */
 NR_B200_API int nr_b200_abi_version(void);
 NR_B200_API const char *nr_b200_error_string(int code);
@@ -811,6 +860,12 @@ NR_B200_API int nr_b200_soft_attributes(const nr_b200_soft_rgb_args *args, const
                                         void *cuda_stream);
 NR_B200_API int nr_b200_soft_attributes_backward(const nr_b200_soft_rgb_args *args, const nr_b200_soft_attr_args *attr,
                                                  void *cuda_stream);
+/* Soft fragments (nr_b200_soft_frag_args above): pix_to_face, zbuf, bary and dists, and the backward into the
+ * geometry. */
+NR_B200_API int nr_b200_soft_fragments(const nr_b200_soft_rgb_args *args, const nr_b200_soft_frag_args *frag,
+                                       void *cuda_stream);
+NR_B200_API int nr_b200_soft_fragments_backward(const nr_b200_soft_rgb_args *args, const nr_b200_soft_frag_args *frag,
+                                                void *cuda_stream);
 
 /* vertices_to_faces (reference vertices_to_faces.py:4-21), the step either side of the rasterizer:
  *   forward   out_faces[b,f,k,:] = vertices[b, faces[b,f,k], :]           ([B,Nv,3] x [B,Nf,3] int32 -> [B,Nf,3,3])

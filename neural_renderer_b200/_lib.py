@@ -68,6 +68,8 @@ EXPORTED_SYMBOLS = (
     "nr_b200_soft_rgb_uv_backward",
     "nr_b200_soft_attributes",
     "nr_b200_soft_attributes_backward",
+    "nr_b200_soft_fragments",
+    "nr_b200_soft_fragments_backward",
     "nr_b200_vertices_to_faces",
     "nr_b200_vertices_to_faces_backward",
     "nr_b200_camera_transform",
@@ -234,6 +236,16 @@ class SoftAttrArgs(ctypes.Structure):
     ]
 
 
+class SoftFragArgs(ctypes.Structure):
+    _fields_ = [
+        ("struct_size", ctypes.c_uint32), ("faces_per_pixel", ctypes.c_int32),
+        ("pix_to_face", ctypes.c_void_p), ("zbuf", ctypes.c_void_p), ("bary", ctypes.c_void_p), ("dists", ctypes.c_void_p),
+        ("grad_zbuf", ctypes.c_void_p), ("grad_bary", ctypes.c_void_p), ("grad_dists", ctypes.c_void_p),
+    ]
+
+
+SOFT_MAX_FACES_PER_PIXEL = 32  # the largest K of nr_b200_soft_fragments
+
 SOFT_BG_DEPTH = 1e-3  # NR_SOFT_BG_DEPTH: the normalised depth of the soft RGB's background term
 
 
@@ -326,6 +338,10 @@ def load():
         fn = getattr(lib, name)
         fn.restype = ctypes.c_int
         fn.argtypes = [ctypes.POINTER(SoftRgbArgs), ctypes.POINTER(SoftAttrArgs), ctypes.c_void_p]
+    for name in ("nr_b200_soft_fragments", "nr_b200_soft_fragments_backward"):
+        fn = getattr(lib, name)
+        fn.restype = ctypes.c_int
+        fn.argtypes = [ctypes.POINTER(SoftRgbArgs), ctypes.POINTER(SoftFragArgs), ctypes.c_void_p]
     lib.nr_b200_vertices_to_faces.restype = ctypes.c_int
     lib.nr_b200_vertices_to_faces.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
                                               ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p]

@@ -16,7 +16,7 @@ CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libnr_b200.so")
 FLAGS_PATH = LIB_PATH + ".flags"  # the nvcc flags (target architecture) the library next to it was built with
 SOURCES = ["nr_api.cu", "nr_forward.cu", "nr_backward.cu", "nr_glue.cu", "nr_mip.cu", "nr_attr.cu", "nr_interior.cu", "nr_phong.cu",
-           "nr_soft.cu", "nr_soft_rgb.cu", "nr_soft_uv.cu", "nr_soft_attr.cu"]
+           "nr_soft.cu", "nr_soft_rgb.cu", "nr_soft_uv.cu", "nr_soft_attr.cu", "nr_soft_frag.cu"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

@@ -33,10 +33,11 @@ void strip_scan(const int* cnt, int* off, int seg_len, long long seg_stride, int
 // kernels), so they pass by address.
 //   soft_rgb_check      the NR_ERR_INVALID_ARG rules of nr_b200_soft_rgb(_backward) with `allowed` flags for the colour
 //                       source `src`: kSoftImage skips texture_size and eps (the caller fills params->tex), kSoftAttributes
-//                       also textures and rgb (nr_soft_attr.cu has its own colour buffers); fills everything but the workspace
+//                       also textures and rgb (nr_soft_attr.cu has its own colour buffers), kSoftFragments also gamma,
+//                       alpha and state (nr_soft_frag.cu has no softmax); fills everything but the workspace
 //   soft_rgb_workspace  NR_ERR_WORKSPACE / NR_ERR_CUDA: the layout (soft_rgb_layout) and the workspace pointers
 //   soft_rgb_bin        the tile binning (bin_faces_rgb): setup, scan, depth records and keys, sorted when `sort`
-enum SoftColourSource { kSoftCubes, kSoftImage, kSoftAttributes };
+enum SoftColourSource { kSoftCubes, kSoftImage, kSoftAttributes, kSoftFragments };
 int soft_rgb_check(const nr_b200_soft_rgb_args* a, uint32_t allowed, SoftColourSource src, bool backward, void* params);
 int soft_rgb_workspace(const nr_b200_soft_rgb_args* a, void* params, void* layout);
 int soft_rgb_bin(void* params, const void* layout, bool sort, cudaStream_t stream);

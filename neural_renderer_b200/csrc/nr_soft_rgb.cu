@@ -383,20 +383,21 @@ namespace nr_internal {
 
 int soft_rgb_check(const nr_b200_soft_rgb_args* a, uint32_t allowed, SoftColourSource src, bool backward, void* params) {
     SoftRgbParams* p = (SoftRgbParams*)params;
-    const bool cubes = src == kSoftCubes, colour = src != kSoftAttributes;
+    const bool cubes = src == kSoftCubes, colour = src != kSoftAttributes && src != kSoftFragments;
+    const bool softmax = src != kSoftFragments;
     if (!a || a->struct_size != sizeof(nr_b200_soft_rgb_args)) return NR_ERR_INVALID_ARG;
     const uint32_t flags = a->flags;
     if (flags & ~allowed) return NR_ERR_INVALID_ARG;
     const int B = a->batch_size, F = a->num_faces, S = a->image_size, ts = a->texture_size;
     if (!soft_sizes_ok(B, F, S)) return NR_ERR_INVALID_ARG;
     const float sigma = a->sigma, gamma = a->gamma;
-    if (!isfinite(sigma) || !(sigma > 0.0f) || !isfinite(gamma) || !(gamma > 0.0f)) return NR_ERR_INVALID_ARG;
+    if (!isfinite(sigma) || !(sigma > 0.0f) || (softmax && (!isfinite(gamma) || !(gamma > 0.0f)))) return NR_ERR_INVALID_ARG;
     if (!(a->near_ < a->far_) || !isfinite(a->far_ - a->near_) || (cubes && !isfinite(a->eps))) return NR_ERR_INVALID_ARG;
     memset(p, 0, sizeof(*p));
     if (!make_face_src(flags, a->faces, a->vertices, a->face_indices, F, a->num_vertices, &p->s.src))
         return NR_ERR_INVALID_ARG;
     if ((colour && !a->textures) || (cubes && (ts < 2 || (long long)ts * ts * ts * 3 > 0x7FFFFFFFll))) return NR_ERR_INVALID_ARG;
-    if ((colour && !a->rgb) || !a->alpha || !a->state) return NR_ERR_INVALID_ARG;
+    if ((colour && !a->rgb) || (softmax && (!a->alpha || !a->state))) return NR_ERR_INVALID_ARG;
     if (backward) {
         const bool indexed = (flags & NR_FACES_INDEXED) != 0;
         if (indexed ? a->grad_faces != nullptr : a->grad_vertices != nullptr) return NR_ERR_INVALID_ARG;
@@ -426,7 +427,7 @@ int soft_rgb_check(const nr_b200_soft_rgb_args* a, uint32_t allowed, SoftColourS
     for (int c = 0; c < 3; c++) p->bg[c] = a->background[c];
     const double fn = (double)a->far_ - (double)a->near_;
     p->zp_bg = (float)((double)a->far_ - NR_SOFT_BG_DEPTH * fn);
-    p->inv_fg = (float)(1.0 / (fn * (double)gamma));
+    p->inv_fg = softmax ? (float)(1.0 / (fn * (double)gamma)) : 0.0f;
     return NR_OK;
 }
 

@@ -920,3 +920,40 @@ def specular_map(color, shininess):
     except RuntimeError:
         raise ValueError("shininess must broadcast to %s, got %s" % (tuple(color.shape[:-1]), tuple(sig.shape))) from None
     return torch.cat((color, sig[..., None]), dim=-1)
+
+
+def interpolate_face_attributes(pix_to_face, bary_coords, face_attributes):
+    """Per-corner attributes interpolated at soft fragments (rasterize_soft_fragments): out[b,y,x,k] =
+    sum_m bary_coords[b,y,x,k,m] face_attributes[(b,) pix_to_face[b,y,x,k], m], [B,H,W,K,C], zeros in empty slots
+    (pix_to_face < 0).  face_attributes [F,3,C] (one set for every item) or [B,F,3,C] / [1,F,3,C].  With the fragments'
+    bary_coords this is A_j of rasterize_soft_attributes for every selected face; blend the slots in torch (e.g.
+    w = sigmoid(dists / sigma) times a depth softmax).  Torch glue, differentiable in bary_coords and face_attributes:
+    one gather per corner and a multiply-add, without a [..., 3, C] intermediate."""
+    if not isinstance(pix_to_face, torch.Tensor) or not isinstance(bary_coords, torch.Tensor) \
+            or not isinstance(face_attributes, torch.Tensor):
+        raise TypeError("pix_to_face, bary_coords and face_attributes must be torch.Tensors")
+    if pix_to_face.dtype.is_floating_point or pix_to_face.dim() != 4:
+        raise ValueError("pix_to_face must be an integer tensor [B,H,W,K], got %s %s"
+                         % (pix_to_face.dtype, tuple(pix_to_face.shape)))
+    if tuple(bary_coords.shape) != tuple(pix_to_face.shape) + (3,):
+        raise ValueError("bary_coords must have shape %s, got %s"
+                         % (tuple(pix_to_face.shape) + (3,), tuple(bary_coords.shape)))
+    B = pix_to_face.shape[0]
+    fa = face_attributes
+    if fa.dim() == 4 and fa.shape[0] == 1:
+        fa = fa[0]
+    if not (fa.dim() == 3 or (fa.dim() == 4 and fa.shape[0] == B)) or fa.shape[-2] != 3:
+        raise ValueError("face_attributes must have shape [F,3,C] or [B,F,3,C], got %s" % (tuple(face_attributes.shape),))
+    F_, C = fa.shape[-3], fa.shape[-1]
+    valid = pix_to_face >= 0
+    ids = torch.where(valid, pix_to_face, torch.zeros_like(pix_to_face)).long()
+    if fa.dim() == 4:
+        ids = ids + (torch.arange(B, device=ids.device) * F_).view(B, 1, 1, 1)
+        fa = fa.reshape(B * F_, 3, C)
+    ids = ids.reshape(-1)
+    out = None
+    for m in range(3):
+        a = fa[:, m].index_select(0, ids).reshape(*pix_to_face.shape, C)
+        w = bary_coords[..., m:m + 1].to(a.dtype)
+        out = a * w if out is None else torch.addcmul(out, a, w)
+    return torch.where(valid[..., None], out, torch.zeros((), dtype=out.dtype, device=out.device))

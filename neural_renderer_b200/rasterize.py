@@ -15,6 +15,7 @@ There is no CPU path (the reference raises NotImplementedError for CPU arrays as
 """
 from __future__ import annotations
 
+import collections
 import ctypes
 import math
 import os
@@ -1512,6 +1513,139 @@ def rasterize_soft_attributes(
     cfg = (int(image_size), sigma, gamma, float(near), float(far))
     image, alpha = _SoftAttrFunction.apply(geom, attrs, indices, bg, per_vertex, cfg)
     return (image, alpha) if return_alpha else image
+
+
+Fragments = collections.namedtuple("Fragments", ["pix_to_face", "zbuf", "bary_coords", "dists"])
+Fragments.__doc__ = """The K nearest faces within reach of every pixel (rasterize_soft_fragments): pix_to_face [B,H,W,K] int64
+(-1 = empty slot), zbuf [B,H,W,K], bary_coords [B,H,W,K,3] and dists [B,H,W,K] (+d^2 inside, -d^2 outside)."""
+
+
+class _SoftFragFunction(torch.autograd.Function):
+    """autograd node of the soft fragments: forward = nr_b200_soft_fragments, backward = nr_b200_soft_fragments_backward
+    from the saved pix_to_face.  `geom` / `indices` as _RasterizeFunction; cfg = (S, sigma, K, near, far)."""
+
+    @staticmethod
+    def forward(ctx, geom, indices, cfg):
+        lib = _lib.load()
+        dev = geom.device
+        geom_c = geom.detach().contiguous()
+        B, S, K = geom_c.shape[0], cfg[0], cfg[2]
+        with torch.cuda.device(dev):
+            p2f = torch.empty((B, S, S, K), dtype=torch.int64, device=dev)
+            zbuf = torch.empty((B, S, S, K), dtype=torch.float32, device=dev)
+            bary = torch.empty((B, S, S, K, 3), dtype=torch.float32, device=dev)
+            dists = torch.empty((B, S, S, K), dtype=torch.float32, device=dev)
+            a, t, ws = _soft_frag_args(lib, geom_c, indices, cfg)
+            t.pix_to_face, t.zbuf, t.bary, t.dists = _ptr(p2f), _ptr(zbuf), _ptr(bary), _ptr(dists)
+            _lib.check(lib.nr_b200_soft_fragments(ctypes.byref(a), ctypes.byref(t), _stream_ptr(dev)))
+        ctx.cfg = cfg
+        ctx.mark_non_differentiable(p2f)
+        ctx.save_for_backward(geom_c, indices, p2f)
+        return p2f, zbuf, bary, dists
+
+    @staticmethod
+    def backward(ctx, _g_p2f, g_zbuf, g_bary, g_dists):
+        if not ctx.needs_input_grad[0] or (g_zbuf is None and g_bary is None and g_dists is None):
+            return None, None, None
+        lib = _lib.load()
+        geom_c, indices, p2f = ctx.saved_tensors
+        dev = geom_c.device
+        prep = lambda g: g.detach().to(torch.float32).contiguous() if g is not None else None  # noqa: E731
+        g_zbuf, g_bary, g_dists = prep(g_zbuf), prep(g_bary), prep(g_dists)
+        with torch.cuda.device(dev):
+            grad_geom = torch.empty_like(geom_c)
+            a, t, ws = _soft_frag_args(lib, geom_c, indices, ctx.cfg)
+            t.pix_to_face = _ptr(p2f)
+            t.grad_zbuf, t.grad_bary, t.grad_dists = _ptr(g_zbuf), _ptr(g_bary), _ptr(g_dists)
+            if indices is not None:
+                a.grad_vertices = _ptr(grad_geom)
+            else:
+                a.grad_faces = _ptr(grad_geom)
+            _lib.check(lib.nr_b200_soft_fragments_backward(ctypes.byref(a), ctypes.byref(t), _stream_ptr(dev)))
+        return grad_geom, None, None
+
+
+def _soft_frag_args(lib, geom_c, indices, cfg):
+    """nr_b200_soft_rgb_args and nr_b200_soft_frag_args of a fragment call, and the workspace (the soft RGB's)"""
+    S, sigma, K, near, far = cfg
+    a = _lib.SoftRgbArgs()
+    a.struct_size = ctypes.sizeof(_lib.SoftRgbArgs)
+    B = geom_c.shape[0]
+    flags = 0
+    if indices is not None:
+        flags |= _lib.NR_FACES_INDEXED
+        if indices.dim() == 2 or (indices.shape[0] == 1 and B > 1):
+            flags |= _lib.NR_INDICES_SHARED
+        a.vertices, a.face_indices, a.num_vertices = _ptr(geom_c), _ptr(indices), geom_c.shape[1]
+        a.num_faces = indices.shape[-2]
+    else:
+        a.faces, a.num_faces = _ptr(geom_c), geom_c.shape[1]
+    n = lib.nr_b200_soft_rgb_workspace_bytes(B, a.num_faces, S, flags)
+    if n == 0:
+        raise ValueError("rasterize_soft_fragments: sizes out of range (batch %d, %d faces, image %d)" % (B, a.num_faces, S))
+    a.flags = flags
+    a.batch_size, a.image_size = B, S
+    a.sigma, a.near_, a.far_ = sigma, near, far
+    ws = torch.empty(n, dtype=torch.uint8, device=geom_c.device)
+    a.workspace, a.workspace_bytes = _ptr(ws), n
+    t = _lib.SoftFragArgs()
+    t.struct_size = ctypes.sizeof(_lib.SoftFragArgs)
+    t.faces_per_pixel = K
+    return a, t, ws
+
+
+def rasterize_soft_fragments(
+        faces,
+        image_size=DEFAULT_IMAGE_SIZE,
+        sigma=DEFAULT_SOFT_SIGMA,
+        faces_per_pixel=8,
+        near=DEFAULT_NEAR,
+        far=DEFAULT_FAR,
+        *,
+        vertices=None,
+):
+    """Soft fragments (PyTorch3D's MeshRasterizer with faces_per_pixel = K and a blur radius): for every pixel the K
+    nearest faces within reach of it -- inside, or within the soft silhouettes' cut-off reach sqrt(sigma ln((1-eps)/eps))
+    -- ordered by their perspective-correct depth (then by face index), each with its depth, its barycentrics and its
+    signed squared distance.  Shade and blend them in torch with any shader: functional.interpolate_face_attributes
+    interpolates per-corner attributes at them, and w = sigmoid(dists / sigma) is SoftRas's coverage probability.  Not in
+    the reference.
+
+    Geometry as rasterize_soft_silhouettes (faces [B,F,3,3], or `vertices` [B,Nv,3] with integer faces [F,3] /
+    [1|B,F,3]).  A face takes part when its three vertex depths lie in [near, far]; a zero-area face is no fragment.
+    1 <= faces_per_pixel <= 32.  Returns Fragments(pix_to_face [B,H,W,K] int64, the face index within its item;
+    zbuf [B,H,W,K]; bary_coords [B,H,W,K,3], perspective-correct, clipped and renormalised; dists [B,H,W,K], +d^2
+    inside and -d^2 outside in squared NDC units -- the opposite sign of PyTorch3D's).  Empty slots hold -1 in every
+    field.  Row 0 is at the top.  Deterministic.  Gradients flow from zbuf, bary_coords and dists into the vertices'
+    x, y and z with the selection held fixed.  The exact definition is in include/nr_b200.h (nr_b200_soft_frag_args)."""
+    try:
+        sigma = float(sigma)
+    except (TypeError, ValueError):
+        raise TypeError("sigma must be a number, got %r" % (sigma,))
+    if not math.isfinite(sigma) or sigma <= 0:
+        raise ValueError("sigma must be finite and > 0, got %r" % (sigma,))
+    if isinstance(faces_per_pixel, bool) or not hasattr(faces_per_pixel, "__index__"):
+        raise TypeError("faces_per_pixel must be an integer, got %r" % (faces_per_pixel,))
+    K = faces_per_pixel.__index__()
+    if not 1 <= K <= _lib.SOFT_MAX_FACES_PER_PIXEL:
+        raise ValueError("faces_per_pixel must be in [1, %d], got %r" % (_lib.SOFT_MAX_FACES_PER_PIXEL, faces_per_pixel))
+    if not (float(near) < float(far)):
+        raise ValueError("near must be < far, got near=%r far=%r" % (near, far))
+    if int(image_size) < 1:
+        raise ValueError("image_size must be >= 1, got %r" % (image_size,))
+    _check_inputs(faces, None, False, vertices=vertices)  # the geometry, then the device check
+    indices = None
+    if vertices is not None:
+        geom = vertices if vertices.dtype == torch.float32 else vertices.float()
+        indices = faces
+        if indices.dim() == 3 and indices.shape[0] > 1 and indices.stride(0) == 0:
+            indices = indices[:1]
+        indices = indices.to(torch.int32).contiguous()
+    else:
+        geom = faces if faces.dtype == torch.float32 else faces.float()
+        if not geom.is_cuda:
+            raise NotImplementedError("neural_renderer_b200 has no CPU implementation (inputs must be CUDA tensors)")
+    return Fragments(*_SoftFragFunction.apply(geom, indices, (int(image_size), sigma, K, float(near), float(far))))
 
 
 class Rasterize(object):

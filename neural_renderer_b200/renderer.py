@@ -7,7 +7,8 @@ import torch
 
 from . import functional as F
 from .rasterize import (DEFAULT_SOFT_GAMMA, DEFAULT_SOFT_SIGMA, rasterize, rasterize_attributes, rasterize_depth,
-                        rasterize_silhouettes, rasterize_soft, rasterize_soft_attributes, rasterize_soft_silhouettes)
+                        rasterize_silhouettes, rasterize_soft, rasterize_soft_attributes, rasterize_soft_fragments,
+                        rasterize_soft_silhouettes)
 
 
 class Renderer(object):
@@ -185,6 +186,18 @@ class Renderer(object):
                                              background=far)[:, 0]
         fv = F.vertices_to_faces(transformed, faces)
         return rasterize_soft_attributes(fv, *args, face_attributes=fv[..., 2:3], background=far)[:, 0]
+
+    def render_soft_fragments(self, vertices, faces, sigma=DEFAULT_SOFT_SIGMA, faces_per_pixel=8):
+        """Soft fragments (neural_renderer_b200.rasterize_soft_fragments) seen through this renderer's camera, with near /
+        far: for every pixel the faces_per_pixel nearest faces within reach, with their depth, barycentrics and signed
+        squared distance, to shade and blend in torch (functional.interpolate_face_attributes).  fill_back adds no copies
+        (a copy would take a second slot) and anti_aliasing is ignored.  The gradient reaches `vertices` through the
+        camera."""
+        transformed = self._transform(vertices)
+        args = (self.image_size, sigma, faces_per_pixel, self.near, self.far)
+        if self.fused and self._fusable(vertices, faces):
+            return rasterize_soft_fragments(faces, *args, vertices=transformed)
+        return rasterize_soft_fragments(F.vertices_to_faces(transformed, faces), *args)
 
     def render_depth(self, vertices, faces):
         if self.fused and self._fusable(vertices, faces):
