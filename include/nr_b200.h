@@ -779,6 +779,72 @@ typedef struct nr_b200_soft_frag_args {
     const float *grad_dists;       /* backward: [B,S,S,K] or NULL (zeros) */
 } nr_b200_soft_frag_args;
 
+/* Soft blend of fragments (within ABI 4, additive): nr_b200_blend_fragments / _backward blend per-slot colours of the
+ * soft fragments above (any shader's output, e.g. interpolate_face_attributes of the fragments) by SoftRas's depth
+ * softmax, and replace the torch expression
+ *   w = where(p2f >= 0, sigmoid(dists / sigma) exp((zref - zbuf) / ((far - near) gamma)), 0),
+ *   out = ((w[..., None] colors).sum(-2) + w_b bg) / (w.sum(-1) + w_b)[..., None], permuted to [B,C,H,W].
+ * Per item and pixel (row 0 at the top) with K slots of pix_to_face (a slot is valid when its value is >= 0), zbuf,
+ * dists and a colour c_k in R^C, for the valid slots k (the slots need not be sorted):
+ *   x_k  = dists_k * (1 / sigma)  (fp32 1 / sigma; dists +d^2 inside, -d^2 outside: the sign of nr_b200_soft_frag_args),
+ *   D_k  = sigmoid(x_k),
+ *   zb   = far - NR_SOFT_BG_DEPTH (far - near),   zref = min(zb, min_k zbuf_k),
+ *   w_k  = D_k exp((zref - zbuf_k) / ((far - near) gamma)),   w_b = exp((zref - zb) / ((far - near) gamma)),
+ *   Z    = w_b + sum_k w_k,
+ *   out_c = (w_b bg_c + sum_k w_k c_kc) / Z                     -> out [B,C,H,W] (planar),
+ *   alpha = 1 - prod_k (1 - D_k) = -expm1(-sum_k softplus(x_k)) -> alpha [B,H,W].
+ * Invalid slots contribute nothing, whatever they hold; a pixel with no valid slot gives out = bg and alpha = 0.  The
+ * exponents are depth differences, as nr_b200_soft_rgb's.  fp32 order: Z and sum softplus are summed from the first
+ * term shown in slot order, out_c as fma(w_k, c_kc, N) from N = w_b bg_c in slot order, then one division by Z; zref is
+ * a minimum.  So the results are bit-for-bit repeatable, appending empty slots (K -> K + p, all -1) changes no bit,
+ * channel c of a C-channel call is bit-identical to a C = 1 call on that channel alone, and a permutation of the slots
+ * changes only fp32 rounding.  Z is 0 (and out NaN) only when every weight underflows, which no slot within the
+ * fragments' reach can cause.  With every pixel's candidate count below K, the blend of interpolate_face_attributes of
+ * the fragments is nr_b200_soft_attributes up to fp32 rounding.
+ * Where it differs from PyTorch3D's softmax_rgb_blend: dists has the opposite sign (positive inside); the background
+ * sits at the normalised depth NR_SOFT_BG_DEPTH = 1e-3 (1e-10 there), with no max(delta, eps) clamp of the background
+ * weight; the output is planar [B,C,H,W] with a separate alpha (RGBA channels-last there).
+ * Backward: exact, with zref held fixed (it cancels).  With g = grad_out at the pixel, g_a = grad_alpha and
+ * H_k = g . (c_k - out) / Z (summed over the channels in order, from the forward's out):
+ *   grad_colors[k, c] = w_k g_c / Z,
+ *   grad_dists[k]     = ((1 - alpha) D_k g_a + w_k (1 - D_k) H_k) / sigma,
+ *   grad_zbuf[k]      = -w_k H_k / ((far - near) gamma).
+ * Invalid slots get exactly 0.  No gradient flows into the background, sigma, gamma, near or far.  Every gradient is
+ * written pixel-locally, with no atomics and no zero-fill: the backward is bit-for-bit deterministic.  The backward
+ * reads the forward's out and recomputes zref, Z and sum softplus from zbuf and dists with the forward's own arithmetic;
+ * it takes 1 - alpha as exp(-sum softplus), which keeps its precision where the saved alpha rounds to 1 (alpha is not
+ * read and may be NULL there).  No state buffer and no workspace.
+ * Host rejections before any launch (NR_ERR_INVALID_ARG): a NULL struct or a struct_size other than its sizeof, B, H,
+ * W or C < 1, K outside [1, 32], B H W K C past 4e18 (indices are 64-bit), a non-finite or non-positive sigma or gamma,
+ * near >= far or a non-finite near, far or far - near, 1 / sigma or 1 / ((far - near) gamma) beyond fp32, a NULL
+ * pix_to_face, zbuf, dists, colors or out (and alpha in the forward), in the backward all three gradient outputs NULL, and a pointer short
+ * of its element alignment (8 bytes for pix_to_face, 4 for the rest); wider loads are chosen at run time when the
+ * addresses allow. */
+typedef struct nr_b200_blend_args {
+    uint32_t struct_size;          /* sizeof(nr_b200_blend_args) */
+    int32_t batch_size;            /* B >= 1 */
+    int32_t height;                /* H >= 1 */
+    int32_t width;                 /* W >= 1 */
+    int32_t faces_per_pixel;       /* K, 1 <= K <= 32 */
+    int32_t channels;              /* C >= 1 */
+    float sigma;                   /* > 0 */
+    float gamma;                   /* > 0: the depth softmax temperature (in units of far - near) */
+    float near_;                   /* near < far */
+    float far_;
+    const int64_t *pix_to_face;    /* [B,H,W,K] */
+    const float *zbuf;             /* [B,H,W,K] */
+    const float *dists;            /* [B,H,W,K] */
+    const float *colors;           /* [B,H,W,K,C] (the layout of interpolate_face_attributes) */
+    const float *background;       /* [C], or NULL = zeros */
+    float *out;                    /* [B,C,H,W]: written by the forward, read by the backward */
+    float *alpha;                  /* [B,H,W]: written by the forward */
+    const float *grad_out;         /* backward: [B,C,H,W] or NULL (zeros) */
+    const float *grad_alpha;       /* backward: [B,H,W] or NULL (zeros) */
+    float *grad_colors;            /* backward: [B,H,W,K,C] or NULL = not wanted */
+    float *grad_zbuf;              /* backward: [B,H,W,K] or NULL = not wanted */
+    float *grad_dists;             /* backward: [B,H,W,K] or NULL = not wanted */
+} nr_b200_blend_args;
+
 /* ABI version of the loaded library (== NR_B200_ABI_VERSION it was built with). */
 NR_B200_API int nr_b200_abi_version(void);
 NR_B200_API const char *nr_b200_error_string(int code);
@@ -866,6 +932,10 @@ NR_B200_API int nr_b200_soft_fragments(const nr_b200_soft_rgb_args *args, const 
                                        void *cuda_stream);
 NR_B200_API int nr_b200_soft_fragments_backward(const nr_b200_soft_rgb_args *args, const nr_b200_soft_frag_args *frag,
                                                 void *cuda_stream);
+/* Soft blend of fragments (nr_b200_blend_args above): out and alpha, and the backward into the colours, zbuf and
+ * dists. */
+NR_B200_API int nr_b200_blend_fragments(const nr_b200_blend_args *args, void *cuda_stream);
+NR_B200_API int nr_b200_blend_fragments_backward(const nr_b200_blend_args *args, void *cuda_stream);
 
 /* vertices_to_faces (reference vertices_to_faces.py:4-21), the step either side of the rasterizer:
  *   forward   out_faces[b,f,k,:] = vertices[b, faces[b,f,k], :]           ([B,Nv,3] x [B,Nf,3] int32 -> [B,Nf,3,3])

@@ -927,8 +927,9 @@ def interpolate_face_attributes(pix_to_face, bary_coords, face_attributes):
     sum_m bary_coords[b,y,x,k,m] face_attributes[(b,) pix_to_face[b,y,x,k], m], [B,H,W,K,C], zeros in empty slots
     (pix_to_face < 0).  face_attributes [F,3,C] (one set for every item) or [B,F,3,C] / [1,F,3,C].  With the fragments'
     bary_coords this is A_j of rasterize_soft_attributes for every selected face; blend the slots in torch (e.g.
-    w = sigmoid(dists / sigma) times a depth softmax).  Torch glue, differentiable in bary_coords and face_attributes:
-    one gather per corner and a multiply-add, without a [..., 3, C] intermediate."""
+    w = sigmoid(dists / sigma) times a depth softmax), or hand them to rasterize.blend_soft_fragments, which blends
+    them by SoftRas's depth softmax in CUDA.  Torch glue, differentiable in bary_coords and face_attributes: one gather
+    per corner and a multiply-add, without a [..., 3, C] intermediate."""
     if not isinstance(pix_to_face, torch.Tensor) or not isinstance(bary_coords, torch.Tensor) \
             or not isinstance(face_attributes, torch.Tensor):
         raise TypeError("pix_to_face, bary_coords and face_attributes must be torch.Tensors")

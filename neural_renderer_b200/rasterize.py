@@ -1607,9 +1607,9 @@ def rasterize_soft_fragments(
     """Soft fragments (PyTorch3D's MeshRasterizer with faces_per_pixel = K and a blur radius): for every pixel the K
     nearest faces within reach of it -- inside, or within the soft silhouettes' cut-off reach sqrt(sigma ln((1-eps)/eps))
     -- ordered by their perspective-correct depth (then by face index), each with its depth, its barycentrics and its
-    signed squared distance.  Shade and blend them in torch with any shader: functional.interpolate_face_attributes
-    interpolates per-corner attributes at them, and w = sigmoid(dists / sigma) is SoftRas's coverage probability.  Not in
-    the reference.
+    signed squared distance.  Shade them in torch with any shader: functional.interpolate_face_attributes
+    interpolates per-corner attributes at them, and w = sigmoid(dists / sigma) is SoftRas's coverage probability;
+    blend_soft_fragments blends the shaded slots by SoftRas's depth softmax in CUDA.  Not in the reference.
 
     Geometry as rasterize_soft_silhouettes (faces [B,F,3,3], or `vertices` [B,Nv,3] with integer faces [F,3] /
     [1|B,F,3]).  A face takes part when its three vertex depths lie in [near, far]; a zero-area face is no fragment.
@@ -1646,6 +1646,139 @@ def rasterize_soft_fragments(
         if not geom.is_cuda:
             raise NotImplementedError("neural_renderer_b200 has no CPU implementation (inputs must be CUDA tensors)")
     return Fragments(*_SoftFragFunction.apply(geom, indices, (int(image_size), sigma, K, float(near), float(far))))
+
+
+class _BlendFunction(torch.autograd.Function):
+    """autograd node of the soft blend: forward = nr_b200_blend_fragments, backward = nr_b200_blend_fragments_backward
+    from the saved inputs and out.  cfg = (sigma, gamma, near, far)."""
+
+    @staticmethod
+    def forward(ctx, zbuf, dists, colors, p2f, bg, cfg):
+        lib = _lib.load()
+        dev = colors.device
+        B, H, W, K, C = colors.shape
+        with torch.cuda.device(dev):
+            out = torch.empty((B, C, H, W), dtype=torch.float32, device=dev)
+            alpha = torch.empty((B, H, W), dtype=torch.float32, device=dev)
+            a = _blend_args(zbuf, dists, colors, p2f, bg, cfg)
+            a.out, a.alpha = _ptr(out), _ptr(alpha)
+            _lib.check(lib.nr_b200_blend_fragments(ctypes.byref(a), _stream_ptr(dev)))
+        ctx.cfg = cfg
+        ctx.save_for_backward(zbuf, dists, colors, p2f, bg, out)
+        return out, alpha
+
+    @staticmethod
+    def backward(ctx, g_out, g_alpha):
+        want = ctx.needs_input_grad[:3]
+        if not any(want) or (g_out is None and g_alpha is None):
+            return None, None, None, None, None, None
+        lib = _lib.load()
+        zbuf, dists, colors, p2f, bg, out = ctx.saved_tensors
+        dev = colors.device
+        prep = lambda g: g.detach().to(torch.float32).contiguous() if g is not None else None  # noqa: E731
+        g_out, g_alpha = prep(g_out), prep(g_alpha)
+        with torch.cuda.device(dev):
+            gz = torch.empty_like(zbuf) if want[0] else None
+            gd = torch.empty_like(dists) if want[1] else None
+            gc = torch.empty_like(colors) if want[2] else None
+            a = _blend_args(zbuf, dists, colors, p2f, bg, ctx.cfg)
+            a.out, a.grad_out, a.grad_alpha = _ptr(out), _ptr(g_out), _ptr(g_alpha)
+            a.grad_zbuf, a.grad_dists, a.grad_colors = _ptr(gz), _ptr(gd), _ptr(gc)
+            _lib.check(lib.nr_b200_blend_fragments_backward(ctypes.byref(a), _stream_ptr(dev)))
+        return gz, gd, gc, None, None, None
+
+
+def _blend_args(zbuf, dists, colors, p2f, bg, cfg):
+    B, H, W, K, C = colors.shape
+    a = _lib.BlendArgs()
+    a.struct_size = ctypes.sizeof(_lib.BlendArgs)
+    a.batch_size, a.height, a.width, a.faces_per_pixel, a.channels = B, H, W, K, C
+    a.sigma, a.gamma, a.near_, a.far_ = cfg
+    a.pix_to_face, a.zbuf, a.dists, a.colors = _ptr(p2f), _ptr(zbuf), _ptr(dists), _ptr(colors)
+    a.background = _ptr(bg) if bg.numel() else None
+    return a
+
+
+def _positive_number(name, v):
+    try:
+        v = float(v)
+    except (TypeError, ValueError):
+        raise TypeError("%s must be a number, got %r" % (name, v))
+    if not math.isfinite(v) or v <= 0:
+        raise ValueError("%s must be finite and > 0, got %r" % (name, v))
+    return v
+
+
+def blend_soft_fragments(fragments, colors, sigma, gamma, near=DEFAULT_NEAR, far=DEFAULT_FAR, background=None):
+    """SoftRas's depth-softmax blend of per-slot colours over soft fragments, in CUDA: the step a fragment pipeline ends
+    with ("shade in torch, blend on the GPU").  fragments: a Fragments of rasterize_soft_fragments (pix_to_face, zbuf
+    and dists are read; bary_coords is not), colors [B,H,W,K,C] the colour of every slot (any torch shader's output,
+    e.g. functional.interpolate_face_attributes of the fragments).  Per pixel, over the valid slots (pix_to_face >= 0,
+    in any order), with D_k = sigmoid(dists_k / sigma), zb = far - 1e-3 (far - near) and zref = min(zb, min_k zbuf_k):
+      w_k = D_k exp((zref - zbuf_k) / ((far - near) gamma)),  w_b = exp((zref - zb) / ((far - near) gamma)),
+      image_c = (sum_k w_k colors_kc + w_b background_c) / (sum_k w_k + w_b),  alpha = 1 - prod_k (1 - D_k).
+    sigma and gamma are required: sigma must be the one the fragments were rasterized with (dists / sigma is their
+    coverage), and no default could know it.  Returns (image [B,C,H,W], alpha [B,H,W]).  With the fragments' sigma and
+    every pixel's candidate count below K,
+    blend_soft_fragments(frag, interpolate_face_attributes(frag.pix_to_face, frag.bary_coords, a)) is
+    rasterize_soft_attributes(..., face_attributes=a) up to fp32 rounding.  background: C numbers or a [C] tensor
+    (default zeros; no gradient).  Gradients flow into colors and, through zbuf and dists, on into the fragments'
+    vertices.  Deterministic, forward and backward.  Not in the reference; PyTorch3D's softmax_rgb_blend differs in the
+    sign of dists, the background level (1e-10 there) and the layout (RGBA channels-last there).  The exact definition is
+    in include/nr_b200.h (nr_b200_blend_args)."""
+    if not isinstance(fragments, tuple) or len(fragments) != 4:
+        raise TypeError("fragments must be a Fragments (pix_to_face, zbuf, bary_coords, dists)")
+    p2f, zbuf, _, dists = fragments
+    for name, t in (("pix_to_face", p2f), ("zbuf", zbuf), ("dists", dists), ("colors", colors)):
+        if not isinstance(t, torch.Tensor):
+            raise TypeError("%s must be a torch.Tensor, got %s" % (name, type(t).__name__))
+    if p2f.dtype != torch.int64 or p2f.dim() != 4:
+        raise ValueError("pix_to_face must be an int64 tensor [B,H,W,K], got %s %s" % (p2f.dtype, tuple(p2f.shape)))
+    for name, t in (("zbuf", zbuf), ("dists", dists)):
+        if not t.dtype.is_floating_point or tuple(t.shape) != tuple(p2f.shape):
+            raise ValueError("%s must be a floating tensor of shape %s, got %s %s"
+                             % (name, tuple(p2f.shape), t.dtype, tuple(t.shape)))
+    if not colors.dtype.is_floating_point or colors.dim() != 5 or tuple(colors.shape[:4]) != tuple(p2f.shape):
+        raise ValueError("colors must be a floating tensor [B,H,W,K,C] with [B,H,W,K] = %s, got %s %s"
+                         % (tuple(p2f.shape), colors.dtype, tuple(colors.shape)))
+    B, H, W, K, C = colors.shape
+    if min(B, H, W, K, C) < 1:
+        raise ValueError("every size of colors must be >= 1, got %s" % (tuple(colors.shape),))
+    if K > _lib.SOFT_MAX_FACES_PER_PIXEL:
+        raise ValueError("at most %d slots per pixel, got %d" % (_lib.SOFT_MAX_FACES_PER_PIXEL, K))
+    sigma = _positive_number("sigma", sigma)
+    gamma = _positive_number("gamma", gamma)
+    near, far = float(near), float(far)
+    if not (math.isfinite(near) and math.isfinite(far) and near < far):
+        raise ValueError("near and far must be finite with near < far, got near=%r far=%r" % (near, far))
+    bg = background
+    if bg is not None:
+        if isinstance(bg, torch.Tensor):
+            if bg.dim() != 1 or bg.shape[0] != C or not bg.dtype.is_floating_point:
+                raise ValueError("background must be a floating tensor [%d], got %s %s" % (C, bg.dtype, tuple(bg.shape)))
+        else:
+            try:
+                bg = [float(v) for v in bg]
+            except (TypeError, ValueError):
+                raise TypeError("background must be a sequence of %d numbers or a tensor, got %r" % (C, background))
+            if len(bg) != C:
+                raise ValueError("background must have %d values, got %d" % (C, len(bg)))
+    dev = colors.device
+    for name, t in (("pix_to_face", p2f), ("zbuf", zbuf), ("dists", dists)):
+        if t.device != dev:
+            raise ValueError("%s is on %s, colors on %s" % (name, t.device, dev))
+    if isinstance(bg, torch.Tensor) and bg.device != dev:
+        raise ValueError("background is on %s, colors on %s" % (bg.device, dev))
+    if not colors.is_cuda:
+        raise NotImplementedError("neural_renderer_b200 has no CPU implementation (inputs must be CUDA tensors)")
+    if bg is None:
+        bg = torch.zeros(0, dtype=torch.float32, device=dev)
+    elif isinstance(bg, torch.Tensor):
+        bg = bg.detach().to(torch.float32).contiguous()
+    else:
+        bg = _device_background(bg, dev)
+    f32 = lambda t: t.to(torch.float32).contiguous()  # noqa: E731
+    return _BlendFunction.apply(f32(zbuf), f32(dists), f32(colors), p2f.contiguous(), bg, (sigma, gamma, near, far))
 
 
 class Rasterize(object):
