@@ -845,6 +845,55 @@ typedef struct nr_b200_blend_args {
     float *grad_dists;             /* backward: [B,H,W,K] or NULL = not wanted */
 } nr_b200_blend_args;
 
+/* Soft interpolation of fragments (within ABI 4, additive): nr_b200_interpolate_fragments / _backward interpolate C >= 1
+ * per-corner or per-vertex attributes at the slots of one fragment set (the soft fragments above, or any caller's
+ * pix_to_face and bary of the same layout), and replace the torch gather-and-multiply-add of interpolate_face_attributes.
+ * Per slot (b, y, x, k) with f = pix_to_face[b,y,x,k] and l_m = bary[b,y,x,k,m]:
+ *   the slot is valid when 0 <= f < F (an unsigned compare: -1, any other negative value and f >= F are empty slots, so
+ *   an edited pix_to_face never reads out of bounds);
+ *   a_mc = corner m's attribute: per corner attributes[(b,) f, m, c] ([B,F,3,C], or [F,3,C] with NR_ATTR_SHARED), or with
+ *   NR_ATTR_PER_VERTEX per vertex attributes[(b,) i, c] ([B,Nv,C], or [Nv,C] with NR_ATTR_SHARED) through the index
+ *   i = face_indices[(b,) f, m] ([B,F,3], or [F,3] with NR_INDICES_SHARED); an index outside [0, Nv) reads zeros;
+ *   out[b,y,x,k,c] = fma(l_2, a_2c, fma(l_1, a_1c, l_0 * a_0c))  (the chain of nr_b200_interpolate and of
+ *   nr_b200_soft_attributes), exactly 0 in an empty slot.  Layout [B,H,W,K,C], the one nr_b200_blend_fragments reads.
+ * Every channel's arithmetic is independent of the others.  So, bit for bit: a per-vertex call equals a per-corner call on
+ * the materialised attributes (nr_b200_vertices_to_faces of the vertex set); channel c of a C-channel call equals a C = 1
+ * call on that channel alone; a shared set (NR_ATTR_SHARED, NR_INDICES_SHARED) equals the same set expanded per item.
+ * Backward, with g_c = grad_out[b,y,x,k,c] (grad_out NULL = zeros):
+ *   grad_bary[b,y,x,k,m] = sum_c g_c a_mc, in fp32 from the first product s = g_0 a_m0, then s = fma(g_c, a_mc, s) for
+ *     c = 1, 2, ... in order; written pixel-locally, bit-for-bit deterministic; exactly 0 in an empty slot;
+ *   grad_attributes[corner m of f, or vertex face_indices[(b,) f, m], c] += l_m g_c  (summed over the items with
+ *     NR_ATTR_SHARED; out-of-range indices get nothing).  fp32 atomics, not bit-pinned.
+ *   Each gradient output may be NULL (not wanted), and each is zero-filled first unless NR_GRAD_ACCUMULATE, which adds
+ *   into it (grad_bary as prev + sum, one rounding).
+ * No workspace and no state: the backward reads pix_to_face, bary, face_indices, attributes and grad_out.
+ * Host rejections before any launch (NR_ERR_INVALID_ARG): a NULL struct or a struct_size other than its sizeof, B, H, W,
+ * C or F < 1, K outside [1, 32], Nv < 1 with NR_ATTR_PER_VERTEX, a flag other than NR_ATTR_PER_VERTEX, NR_ATTR_SHARED,
+ * NR_INDICES_SHARED and (backward) NR_GRAD_ACCUMULATE, NR_ATTR_PER_VERTEX without face_indices, a NULL pix_to_face, bary
+ * or attributes (and out in the forward), in the backward both gradient outputs NULL, a pointer short of its element
+ * alignment (8 bytes for pix_to_face, 4 for the rest), and sizes past the kernels' index width: B H W K or the attribute
+ * set past 4e18 elements, B H W K / 256 or B H W / 32 CTAs past 2^31 - 1, or C past 2^20.  Wider loads and stores are
+ * chosen at run time when C % 4 == 0 and the addresses allow them. */
+typedef struct nr_b200_frag_interp_args {
+    uint32_t struct_size;          /* sizeof(nr_b200_frag_interp_args) */
+    uint32_t flags;                /* NR_ATTR_PER_VERTEX, NR_ATTR_SHARED, NR_INDICES_SHARED, NR_GRAD_ACCUMULATE (backward) */
+    int32_t batch_size;            /* B >= 1 */
+    int32_t height;                /* H >= 1 */
+    int32_t width;                 /* W >= 1 */
+    int32_t faces_per_pixel;       /* K, 1 <= K <= 32 */
+    int32_t channels;              /* C >= 1 */
+    int32_t num_faces;             /* F >= 1: the valid range of pix_to_face */
+    int32_t num_vertices;          /* Nv >= 1 with NR_ATTR_PER_VERTEX (else ignored) */
+    const int64_t *pix_to_face;    /* [B,H,W,K] */
+    const float *bary;             /* [B,H,W,K,3] */
+    const int32_t *face_indices;   /* NR_ATTR_PER_VERTEX: [B,F,3], or [F,3] with NR_INDICES_SHARED (else ignored) */
+    const float *attributes;       /* [B,F,3,C] / [B,Nv,C] (no B with NR_ATTR_SHARED) */
+    float *out;                    /* forward: [B,H,W,K,C] */
+    const float *grad_out;         /* backward: [B,H,W,K,C] or NULL (zeros) */
+    float *grad_attributes;        /* backward: layout of attributes, or NULL = not wanted */
+    float *grad_bary;              /* backward: [B,H,W,K,3], or NULL = not wanted */
+} nr_b200_frag_interp_args;
+
 /* ABI version of the loaded library (== NR_B200_ABI_VERSION it was built with). */
 NR_B200_API int nr_b200_abi_version(void);
 NR_B200_API const char *nr_b200_error_string(int code);
@@ -936,6 +985,10 @@ NR_B200_API int nr_b200_soft_fragments_backward(const nr_b200_soft_rgb_args *arg
  * dists. */
 NR_B200_API int nr_b200_blend_fragments(const nr_b200_blend_args *args, void *cuda_stream);
 NR_B200_API int nr_b200_blend_fragments_backward(const nr_b200_blend_args *args, void *cuda_stream);
+/* Soft interpolation of fragments (nr_b200_frag_interp_args above): out, and the backward into the attributes and the
+ * barycentrics. */
+NR_B200_API int nr_b200_interpolate_fragments(const nr_b200_frag_interp_args *args, void *cuda_stream);
+NR_B200_API int nr_b200_interpolate_fragments_backward(const nr_b200_frag_interp_args *args, void *cuda_stream);
 
 /* vertices_to_faces (reference vertices_to_faces.py:4-21), the step either side of the rasterizer:
  *   forward   out_faces[b,f,k,:] = vertices[b, faces[b,f,k], :]           ([B,Nv,3] x [B,Nf,3] int32 -> [B,Nf,3,3])

@@ -72,6 +72,8 @@ EXPORTED_SYMBOLS = (
     "nr_b200_soft_fragments_backward",
     "nr_b200_blend_fragments",
     "nr_b200_blend_fragments_backward",
+    "nr_b200_interpolate_fragments",
+    "nr_b200_interpolate_fragments_backward",
     "nr_b200_vertices_to_faces",
     "nr_b200_vertices_to_faces_backward",
     "nr_b200_camera_transform",
@@ -258,6 +260,17 @@ class BlendArgs(ctypes.Structure):
     ]
 
 
+class FragInterpArgs(ctypes.Structure):
+    _fields_ = [
+        ("struct_size", ctypes.c_uint32), ("flags", ctypes.c_uint32), ("batch_size", ctypes.c_int32),
+        ("height", ctypes.c_int32), ("width", ctypes.c_int32), ("faces_per_pixel", ctypes.c_int32),
+        ("channels", ctypes.c_int32), ("num_faces", ctypes.c_int32), ("num_vertices", ctypes.c_int32),
+        ("pix_to_face", ctypes.c_void_p), ("bary", ctypes.c_void_p), ("face_indices", ctypes.c_void_p),
+        ("attributes", ctypes.c_void_p), ("out", ctypes.c_void_p), ("grad_out", ctypes.c_void_p),
+        ("grad_attributes", ctypes.c_void_p), ("grad_bary", ctypes.c_void_p),
+    ]
+
+
 SOFT_MAX_FACES_PER_PIXEL = 32  # the largest K of nr_b200_soft_fragments
 
 SOFT_BG_DEPTH = 1e-3  # NR_SOFT_BG_DEPTH: the normalised depth of the soft RGB's background term
@@ -360,6 +373,10 @@ def load():
         fn = getattr(lib, name)
         fn.restype = ctypes.c_int
         fn.argtypes = [ctypes.POINTER(BlendArgs), ctypes.c_void_p]
+    for name in ("nr_b200_interpolate_fragments", "nr_b200_interpolate_fragments_backward"):
+        fn = getattr(lib, name)
+        fn.restype = ctypes.c_int
+        fn.argtypes = [ctypes.POINTER(FragInterpArgs), ctypes.c_void_p]
     lib.nr_b200_vertices_to_faces.restype = ctypes.c_int
     lib.nr_b200_vertices_to_faces.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int32, ctypes.c_int32,
                                               ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p]

@@ -929,7 +929,9 @@ def interpolate_face_attributes(pix_to_face, bary_coords, face_attributes):
     bary_coords this is A_j of rasterize_soft_attributes for every selected face; blend the slots in torch (e.g.
     w = sigmoid(dists / sigma) times a depth softmax), or hand them to rasterize.blend_soft_fragments, which blends
     them by SoftRas's depth softmax in CUDA.  Torch glue, differentiable in bary_coords and face_attributes: one gather
-    per corner and a multiply-add, without a [..., 3, C] intermediate."""
+    per corner and a multiply-add, without a [..., 3, C] intermediate.  rasterize.interpolate_soft_fragments computes
+    the same in CUDA (per corner or per vertex), and is the one to use on the GPU; this one serves any dtype and device,
+    float64 included."""
     if not isinstance(pix_to_face, torch.Tensor) or not isinstance(bary_coords, torch.Tensor) \
             or not isinstance(face_attributes, torch.Tensor):
         raise TypeError("pix_to_face, bary_coords and face_attributes must be torch.Tensors")

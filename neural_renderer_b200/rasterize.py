@@ -1607,9 +1607,10 @@ def rasterize_soft_fragments(
     """Soft fragments (PyTorch3D's MeshRasterizer with faces_per_pixel = K and a blur radius): for every pixel the K
     nearest faces within reach of it -- inside, or within the soft silhouettes' cut-off reach sqrt(sigma ln((1-eps)/eps))
     -- ordered by their perspective-correct depth (then by face index), each with its depth, its barycentrics and its
-    signed squared distance.  Shade them in torch with any shader: functional.interpolate_face_attributes
-    interpolates per-corner attributes at them, and w = sigmoid(dists / sigma) is SoftRas's coverage probability;
-    blend_soft_fragments blends the shaded slots by SoftRas's depth softmax in CUDA.  Not in the reference.
+    signed squared distance.  Shade them in torch with any shader: interpolate_soft_fragments interpolates per-corner
+    or per-vertex attributes at them in CUDA (functional.interpolate_face_attributes in torch), and
+    w = sigmoid(dists / sigma) is SoftRas's coverage probability; blend_soft_fragments blends the shaded slots by
+    SoftRas's depth softmax in CUDA.  Not in the reference.
 
     Geometry as rasterize_soft_silhouettes (faces [B,F,3,3], or `vertices` [B,Nv,3] with integer faces [F,3] /
     [1|B,F,3]).  A face takes part when its three vertex depths lie in [near, far]; a zero-area face is no fragment.
@@ -1713,7 +1714,7 @@ def blend_soft_fragments(fragments, colors, sigma, gamma, near=DEFAULT_NEAR, far
     """SoftRas's depth-softmax blend of per-slot colours over soft fragments, in CUDA: the step a fragment pipeline ends
     with ("shade in torch, blend on the GPU").  fragments: a Fragments of rasterize_soft_fragments (pix_to_face, zbuf
     and dists are read; bary_coords is not), colors [B,H,W,K,C] the colour of every slot (any torch shader's output,
-    e.g. functional.interpolate_face_attributes of the fragments).  Per pixel, over the valid slots (pix_to_face >= 0,
+    e.g. interpolate_soft_fragments or functional.interpolate_face_attributes of the fragments).  Per pixel, over the valid slots (pix_to_face >= 0,
     in any order), with D_k = sigmoid(dists_k / sigma), zb = far - 1e-3 (far - near) and zref = min(zb, min_k zbuf_k):
       w_k = D_k exp((zref - zbuf_k) / ((far - near) gamma)),  w_b = exp((zref - zb) / ((far - near) gamma)),
       image_c = (sum_k w_k colors_kc + w_b background_c) / (sum_k w_k + w_b),  alpha = 1 - prod_k (1 - D_k).
@@ -1779,6 +1780,137 @@ def blend_soft_fragments(fragments, colors, sigma, gamma, near=DEFAULT_NEAR, far
         bg = _device_background(bg, dev)
     f32 = lambda t: t.to(torch.float32).contiguous()  # noqa: E731
     return _BlendFunction.apply(f32(zbuf), f32(dists), f32(colors), p2f.contiguous(), bg, (sigma, gamma, near, far))
+
+
+class _FragInterpFunction(torch.autograd.Function):
+    """autograd node of the soft interpolation of fragments: forward = nr_b200_interpolate_fragments, backward =
+    nr_b200_interpolate_fragments_backward from the saved inputs.  `attributes` [B|1,F,3,C] per corner or [B|1,Nv,C]
+    per vertex (1 = shared), `indices` int32 [F,3] / [B|1,F,3] or None; cfg = (flags, F)."""
+
+    @staticmethod
+    def forward(ctx, bary, attributes, p2f, indices, cfg):
+        lib = _lib.load()
+        dev = bary.device
+        B, H, W, K = p2f.shape
+        with torch.cuda.device(dev):
+            out = torch.empty((B, H, W, K, attributes.shape[-1]), dtype=torch.float32, device=dev)
+            a = _frag_interp_args(bary, attributes, p2f, indices, cfg)
+            a.out = _ptr(out)
+            _lib.check(lib.nr_b200_interpolate_fragments(ctypes.byref(a), _stream_ptr(dev)))
+        ctx.cfg = cfg
+        ctx.save_for_backward(bary, attributes, p2f, indices)
+        return out
+
+    @staticmethod
+    def backward(ctx, g_out):
+        want_bary, want_attr = ctx.needs_input_grad[:2]
+        if not (want_bary or want_attr) or g_out is None:
+            return None, None, None, None, None
+        lib = _lib.load()
+        bary, attributes, p2f, indices = ctx.saved_tensors
+        dev = bary.device
+        g_out = g_out.detach().to(torch.float32).contiguous()
+        with torch.cuda.device(dev):
+            gb = torch.empty_like(bary) if want_bary else None
+            ga = torch.empty_like(attributes) if want_attr else None
+            a = _frag_interp_args(bary, attributes, p2f, indices, ctx.cfg)
+            a.grad_out, a.grad_bary, a.grad_attributes = _ptr(g_out), _ptr(gb), _ptr(ga)
+            _lib.check(lib.nr_b200_interpolate_fragments_backward(ctypes.byref(a), _stream_ptr(dev)))
+        return gb, ga, None, None, None
+
+
+def _frag_interp_args(bary, attributes, p2f, indices, cfg):
+    flags, F = cfg
+    B, H, W, K = p2f.shape
+    a = _lib.FragInterpArgs()
+    a.struct_size = ctypes.sizeof(_lib.FragInterpArgs)
+    a.flags = flags
+    a.batch_size, a.height, a.width, a.faces_per_pixel, a.channels = B, H, W, K, attributes.shape[-1]
+    a.num_faces = F
+    a.pix_to_face, a.bary, a.attributes = _ptr(p2f), _ptr(bary), _ptr(attributes)
+    if indices is not None:
+        a.face_indices, a.num_vertices = _ptr(indices), attributes.shape[-2]
+    return a
+
+
+def interpolate_soft_fragments(fragments, face_attributes=None, *, vertex_attributes=None, faces=None):
+    """Per-corner or per-vertex attributes interpolated at soft fragments, in CUDA: the step every shader over fragments
+    starts with (colours, normals, positions, UVs, features).  fragments: a Fragments of rasterize_soft_fragments
+    (pix_to_face and bary_coords are read).  Exactly one of face_attributes [F,3,C] / [1|B,F,3,C] (per corner) and
+    vertex_attributes [Nv,C] / [1|B,Nv,C] (per vertex, with the integer faces [F,3] / [1|B,F,3] that index them; a
+    corner whose index lies outside [0, Nv) reads zeros).  A batch of 1 (or an expanded stride-0 batch) is one set
+    shared by every item; its gradient is the sum over the items.  Per slot with f = pix_to_face in [0, F) and
+    l = bary_coords: out[b,y,x,k,c] = fma(l_2, a_2c, fma(l_1, a_1c, l_0 a_0c)); any other f (-1 included) is an empty
+    slot and gets exactly 0.  Returns [B,H,W,K,C] float32, the layout blend_soft_fragments reads.
+
+    The same values as functional.interpolate_face_attributes (on the gathered corners, for per-vertex attributes) up
+    to fp32 rounding, without its [B,H,W,K,C] temporaries and index_select backward, and without materialising
+    [B,F,3,C] corners for per-vertex attributes.  Gradients flow into the attributes and into fragments.bary_coords,
+    and through bary_coords on into the vertices of rasterize_soft_fragments.  Each channel is computed on its own
+    (channel c equals a one-channel call on it, bit for bit), a per-vertex call equals the per-corner call on the
+    gathered corners and a shared set equals the same set expanded, bit for bit; the forward and the barycentric
+    gradient are deterministic.  Not in the reference.  The exact definition is in include/nr_b200.h
+    (nr_b200_frag_interp_args)."""
+    if not isinstance(fragments, tuple) or len(fragments) != 4:
+        raise TypeError("fragments must be a Fragments (pix_to_face, zbuf, bary_coords, dists)")
+    p2f, _, bary, _ = fragments
+    for name, t in (("pix_to_face", p2f), ("bary_coords", bary)):
+        if not isinstance(t, torch.Tensor):
+            raise TypeError("%s must be a torch.Tensor, got %s" % (name, type(t).__name__))
+    if p2f.dtype != torch.int64 or p2f.dim() != 4:
+        raise ValueError("pix_to_face must be an int64 tensor [B,H,W,K], got %s %s" % (p2f.dtype, tuple(p2f.shape)))
+    if not bary.dtype.is_floating_point or tuple(bary.shape) != tuple(p2f.shape) + (3,):
+        raise ValueError("bary_coords must be a floating tensor of shape %s, got %s %s"
+                         % (tuple(p2f.shape) + (3,), bary.dtype, tuple(bary.shape)))
+    B, H, W, K = p2f.shape
+    if min(B, H, W, K) < 1:
+        raise ValueError("every size of pix_to_face must be >= 1, got %s" % (tuple(p2f.shape),))
+    if K > _lib.SOFT_MAX_FACES_PER_PIXEL:
+        raise ValueError("at most %d slots per pixel, got %d" % (_lib.SOFT_MAX_FACES_PER_PIXEL, K))
+    if (face_attributes is None) == (vertex_attributes is None):
+        raise TypeError("give exactly one of face_attributes and vertex_attributes=")
+    per_vertex = vertex_attributes is not None
+    attrs = vertex_attributes if per_vertex else face_attributes
+    name = "vertex_attributes" if per_vertex else "face_attributes"
+    if not isinstance(attrs, torch.Tensor) or not attrs.is_floating_point():
+        raise TypeError("%s must be a floating point torch.Tensor" % name)
+    rows = 1 if per_vertex else 2                                    # [Nv] or [F,3] before the channels
+    if attrs.dim() not in (rows + 1, rows + 2) or (attrs.dim() == rows + 2 and attrs.shape[0] not in (1, B)) \
+            or (not per_vertex and attrs.shape[-2] != 3) or attrs.shape[-1] < 1 or attrs.shape[-rows - 1] < 1:
+        want = "[Nv,C] or [1|B,Nv,C]" if per_vertex else "[F,3,C] or [1|B,F,3,C]"
+        raise ValueError("%s must have shape %s with C >= 1 (B = %d), got %s" % (name, want, B, tuple(attrs.shape)))
+    if per_vertex:
+        if faces is None:
+            raise ValueError("vertex_attributes need the integer faces [F,3] / [1|B,F,3] that index them")
+        if not isinstance(faces, torch.Tensor) or faces.dtype.is_floating_point or faces.dtype == torch.bool:
+            raise TypeError("faces must be an integer torch.Tensor")
+        if faces.dim() not in (2, 3) or faces.shape[-1] != 3 or faces.shape[-2] < 1 \
+                or (faces.dim() == 3 and faces.shape[0] not in (1, B)):
+            raise ValueError("faces must have shape [F,3] or [1|B,F,3] (B = %d), got %s" % (B, tuple(faces.shape)))
+        F = faces.shape[-2]
+    else:
+        if faces is not None:
+            raise TypeError("faces is only read with vertex_attributes")
+        F = attrs.shape[-3]
+    dev = bary.device
+    for n, t in (("pix_to_face", p2f), (name, attrs), ("faces", faces)):
+        if t is not None and t.device != dev:
+            raise ValueError("%s is on %s, bary_coords on %s" % (n, t.device, dev))
+    if not bary.is_cuda:
+        raise NotImplementedError("neural_renderer_b200 has no CPU implementation (inputs must be CUDA tensors)")
+    attrs = _batched(attrs, B, rows + 1)                              # an expanded shared set: NR_ATTR_SHARED
+    flags = _lib.NR_ATTR_SHARED if attrs.shape[0] == 1 and B > 1 else 0
+    indices = None
+    if per_vertex:
+        flags |= _lib.NR_ATTR_PER_VERTEX
+        indices = faces
+        if indices.dim() == 3 and indices.shape[0] > 1 and indices.stride(0) == 0:
+            indices = indices[:1]
+        if indices.dim() == 2 or (indices.shape[0] == 1 and B > 1):
+            flags |= _lib.NR_INDICES_SHARED
+        indices = indices.to(torch.int32).contiguous()
+    return _FragInterpFunction.apply(bary.to(torch.float32).contiguous(), attrs.contiguous(), p2f.contiguous(), indices,
+                                     (flags, F))
 
 
 class Rasterize(object):
