@@ -196,20 +196,26 @@ def _count_blend():
             lambda sums, ref: torch.stack(sums, -1))
 
 
-def check_forward(scene, rgb, alpha, S, sigma, gamma, pix, what):
+def check_forward(scene, rgb, alpha, S, sigma, gamma, pix, what, terms=None, cull=1.0):
     """rgb [B,3,S,S] (or an attribute image [B,C,S,S]) / alpha [B,S,S] at the pixels pix [B,P] against the sparse
-    oracle under the gates of the docstring; returns the largest error / gate ratios seen, for the record"""
+    oracle under the gates of the docstring; returns the largest error / gate ratios seen, for the record.  terms: the
+    oracle's terms at the kernel's own selection (tests/soft_selection.py), culled at the cut-off scale `cull`; the
+    fp32 cut-off decision is then the oracle's too, so the pixels near the cut-off are checked like every other."""
     B = scene.faces.shape[0]
     leaves = [x.detach() for x in scene.leaves()]
-    terms = scene.oracle_terms(leaves, S, sigma)
+    selected = terms is not None
+    if not selected:
+        terms = scene.oracle_terms(leaves, S, sigma)
     with torch.no_grad():
-        a_or, ac = osoft.sparse_eval(leaves[0], S, pix, sigma, NEAR, FAR, 1.0, _alpha_terms(terms, sigma),
+        a_or, ac = osoft.sparse_eval(leaves[0], S, pix, sigma, NEAR, FAR, cull, _alpha_terms(terms, sigma),
                                      _count_blend())
         n, sdx = ac[..., 0], ac[..., 1]
-        _, g = osoft.sparse_eval(leaves[0], S, pix, sigma, NEAR, FAR, 1.0,
+        _, g = osoft.sparse_eval(leaves[0], S, pix, sigma, NEAR, FAR, cull,
                                  _gate_terms(scene, terms, sigma, gamma, scene.colour_sensitivity()),
                                  _gate_blend(gamma, scene.bg))
     edge = g[..., -1] > 0
+    if selected:
+        edge = torch.zeros_like(edge)
     assert edge.double().mean().item() <= 0.01, (what, edge.double().mean().item())
     flat = lambda t: t.reshape(B, *t.shape[1:-2], S * S)   # noqa: E731
     got_a = torch.gather(flat(alpha).double(), 1, pix)
