@@ -5,6 +5,7 @@
 #include <math.h>
 
 #include <atomic>
+#include <initializer_list>
 
 #include "nr_b200.h"
 #include "nr_geom.cuh"
@@ -28,13 +29,37 @@ struct LaunchScope {
 // nr_backward.cu, also the tile scan of the soft silhouettes)
 void strip_scan(const int* cnt, int* off, int seg_len, long long seg_stride, int nseg, cudaStream_t stream);
 
-// The soft RGB's host half (nr_soft_rgb.cu), shared by the cube and the texture-image units.  `params` / `layout` point
-// to nr_soft_rgb.cuh's SoftRgbParams / SoftRgbLayout, which each unit compiles in its own anonymous namespace (as its
-// kernels), so they pass by address.
+// A gradient buffer to zero-fill: `bytes` from `ptr`, or nothing when `ptr` is NULL
+struct GradBuf {
+    void* ptr;
+    size_t bytes;
+};
+
+// Zero-fills `bufs` in order inside one "memset_grads" profile range; returns the first CUDA error
+inline cudaError_t zero_grads(std::initializer_list<GradBuf> bufs, cudaStream_t stream) {
+    prof_begin("memset_grads", stream);
+    cudaError_t e = cudaSuccess;
+    for (const GradBuf& b : bufs)
+        if (e == cudaSuccess && b.ptr) e = cudaMemsetAsync(b.ptr, 0, b.bytes, stream);
+    prof_end(stream);
+    return e;
+}
+
+// The geometry gradient of a call: grad_vertices [B,Nv,3] with NR_FACES_INDEXED, else grad_faces [B,F,3,3]
+template <class Args>
+inline GradBuf geometry_grad(const Args* a) {
+    if (a->flags & NR_FACES_INDEXED) return {a->grad_vertices, (size_t)a->batch_size * a->num_vertices * 3 * sizeof(float)};
+    return {a->grad_faces, (size_t)a->batch_size * a->num_faces * 9 * sizeof(float)};
+}
+
+// The soft RGB's host half (nr_soft_rgb.cu), shared by the cube, texture-image, attribute and fragment units.
+// `params` / `layout` point to nr_soft_rgb.cuh's SoftRgbParams / SoftRgbLayout, which each unit compiles in its own
+// anonymous namespace (as its kernels), so they pass by address.
 //   soft_rgb_check      the NR_ERR_INVALID_ARG rules of nr_b200_soft_rgb(_backward) with `allowed` flags for the colour
-//                       source `src`: kSoftImage skips texture_size and eps (the caller fills params->tex), kSoftAttributes
-//                       also textures and rgb (nr_soft_attr.cu has its own colour buffers), kSoftFragments also gamma,
-//                       alpha and state (nr_soft_frag.cu has no softmax); fills everything but the workspace
+//                       source `src`, on top of the silhouettes' (fill_soft_params, nr_soft.cuh): kSoftImage skips
+//                       texture_size and eps (the caller fills params->tex), kSoftAttributes also textures and rgb
+//                       (nr_soft_attr.cu has its own colour buffers), kSoftFragments also gamma, alpha and state
+//                       (nr_soft_frag.cu has no softmax); fills everything but the workspace
 //   soft_rgb_workspace  NR_ERR_WORKSPACE / NR_ERR_CUDA: the layout (soft_rgb_layout) and the workspace pointers
 //   soft_rgb_bin        the tile binning (bin_faces_rgb): setup, scan, depth records and keys, sorted when `sort`
 enum SoftColourSource { kSoftCubes, kSoftImage, kSoftAttributes, kSoftFragments };

@@ -161,53 +161,29 @@ __global__ void __launch_bounds__(kThreads) k_soft_bwd(const __grid_constant__ S
 int soft_setup(const nr_b200_soft_args* a, bool backward, SoftParams* p) {
     nr_internal::launch_count() = 0;
     if (!a || a->struct_size != sizeof(nr_b200_soft_args)) return NR_ERR_INVALID_ARG;
-    const uint32_t flags = a->flags;
-    const int B = a->batch_size, F = a->num_faces, S = a->image_size;
-    if (!soft_sizes_ok(B, F, S)) return NR_ERR_INVALID_ARG;
-    const float sigma = a->sigma;
-    if (!isfinite(sigma) || !(sigma > 0.0f)) return NR_ERR_INVALID_ARG;
-    if (!(a->near_ <= a->far_)) return NR_ERR_INVALID_ARG;
+    if (!(a->near_ <= a->far_) || !a->alpha) return NR_ERR_INVALID_ARG;
     memset(p, 0, sizeof(*p));
-    if (!nr_internal::make_face_src(flags, a->faces, a->vertices, a->face_indices, F, a->num_vertices, &p->src))
-        return NR_ERR_INVALID_ARG;
-    if (!a->alpha) return NR_ERR_INVALID_ARG;
-    if (backward) {
-        const bool indexed = (flags & NR_FACES_INDEXED) != 0;
-        if (indexed ? a->grad_faces != nullptr : a->grad_vertices != nullptr) return NR_ERR_INVALID_ARG;
-        if (!nr_internal::make_face_grad(flags, a->grad_faces, a->grad_vertices, a->face_indices, F, a->num_vertices, &p->dst))
-            return NR_ERR_INVALID_ARG;
-    }
-    const SoftLayout L = soft_layout(B, F, S);
+    if (!fill_soft_params(a, backward, p)) return NR_ERR_INVALID_ARG;
+    const SoftLayout L = soft_layout(p->B, p->F, p->S);
     if (!a->workspace || a->workspace_bytes < L.total || ((uintptr_t)a->workspace & 15)) return NR_ERR_WORKSPACE;
     char* ws = (char*)a->workspace;
     p->rec = (float4*)(ws + L.rec); p->box = (uint2*)(ws + L.box);
     p->cnt = (int*)(ws + L.cnt); p->cursor = (int*)(ws + L.cursor); p->off = (int*)(ws + L.off); p->list = (int*)(ws + L.list);
-    p->alpha = a->alpha; p->g = a->grad_alpha;
-    p->B = B; p->F = F; p->S = S;
-    p->ntx = tiles_per_axis(S); p->ntiles = p->ntx * p->ntx;
-    const double cut = (double)sigma * log((1.0 - NR_SOFT_EPS) / NR_SOFT_EPS);
-    p->inv_sigma = (float)(1.0 / (double)sigma);
-    p->cut = (float)cut;
-    p->reach = (float)(sqrt(cut) * S * 0.5) + 1.0f;
-    p->near_ = a->near_; p->far_ = a->far_;
     return NR_OK;
+}
+
+// A template, as bin_prefix is: k_soft_setup<true> is then instantiated after k_soft_setup<false>, so the object lists
+// its kernels in the order of earlier builds and its SASS compares with theirs line for line
+template <typename = void>
+void fill_lists(const SoftParams& p, cudaStream_t s) {
+    nr_internal::LaunchScope ls("k_soft_fill", s);
+    k_soft_setup<true><<<dim3((unsigned)((p.F + 255) / 256), (unsigned)p.B), 256, 0, s>>>(p);
 }
 
 // setup -> scan -> fill: the tile lists of every item
 int bin_faces(const SoftParams& p, cudaStream_t s) {
-    nr_internal::prof_begin("memset_soft_bins", s);
-    if (cudaMemsetAsync(p.cnt, 0, 2 * (size_t)p.B * (p.ntiles + 1) * sizeof(int), s) != cudaSuccess) return NR_ERR_CUDA;
-    nr_internal::prof_end(s);
-    const dim3 grid((unsigned)((p.F + 255) / 256), (unsigned)p.B);
-    {
-        nr_internal::LaunchScope ls("k_soft_setup", s);
-        k_soft_setup<false><<<grid, 256, 0, s>>>(p);
-    }
-    nr_internal::strip_scan(p.cnt, p.off, p.ntiles + 1, (long long)p.F * kWideTiles, p.B, s);
-    {
-        nr_internal::LaunchScope ls("k_soft_fill", s);
-        k_soft_setup<true><<<grid, 256, 0, s>>>(p);
-    }
+    if (bin_prefix(p, s) != NR_OK) return NR_ERR_CUDA;
+    fill_lists(p, s);
     return NR_OK;
 }
 
@@ -237,15 +213,9 @@ extern "C" int nr_b200_soft_silhouettes_backward(const nr_b200_soft_args* args, 
     const int rc = soft_setup(args, true, &p);
     if (rc != NR_OK) return rc;
     const nr_b200_soft_args* a = args;
-    const bool indexed = (a->flags & NR_FACES_INDEXED) != 0;
     cudaStream_t s = (cudaStream_t)cuda_stream;
-    if (!(a->flags & NR_GRAD_ACCUMULATE)) {
-        nr_internal::prof_begin("memset_grads", s);
-        const cudaError_t e = indexed ? cudaMemsetAsync(a->grad_vertices, 0, (size_t)p.B * a->num_vertices * 3 * sizeof(float), s)
-                                      : cudaMemsetAsync(a->grad_faces, 0, (size_t)p.B * p.F * 9 * sizeof(float), s);
-        nr_internal::prof_end(s);
-        if (e != cudaSuccess) return NR_ERR_CUDA;
-    }
+    if (!(a->flags & NR_GRAD_ACCUMULATE) && nr_internal::zero_grads({nr_internal::geometry_grad(a)}, s) != cudaSuccess)
+        return NR_ERR_CUDA;
     if (!a->grad_alpha) return cudaGetLastError() == cudaSuccess ? NR_OK : NR_ERR_CUDA;
     if (bin_faces(p, s) != NR_OK) return NR_ERR_CUDA;
     {

@@ -1,5 +1,6 @@
 // nr_soft.cuh -- what the soft silhouettes (nr_soft.cu) and the soft RGB (nr_soft_rgb.cu) share: the tile binning's
-// parameters, the per-face setup / fill kernel k_soft_setup, the per-pixel distance test and the workspace layout.
+// parameters, the per-face setup / fill kernel k_soft_setup, the per-pixel distance test, the workspace layout, the
+// host fill of the parameters and the start of the binning.
 // Everything is in an anonymous namespace: each translation unit compiles its own copy of what it uses.
 #pragma once
 #include <cuda_runtime.h>
@@ -159,6 +160,49 @@ inline SoftLayout soft_layout(int B, int F, int S) {
     L.list = L.off + align256(nseg * sizeof(int));
     L.total = L.list + align256((size_t)B * F * kWideTiles * sizeof(int));
     return L;
+}
+
+// The rules and fields of a zeroed SoftParams that nr_b200_soft_args and nr_b200_soft_rgb_args share: sizes the kernels
+// can index, a finite sigma > 0, the geometry and (backward) its gradient in the same form -- the other form's gradient
+// NULL -- and the tile grid, the cut-off, near / far, alpha and its gradient.  false = NR_ERR_INVALID_ARG; the caller
+// sets the workspace pointers.
+template <class Args>
+inline bool fill_soft_params(const Args* a, bool backward, SoftParams* p) {
+    const uint32_t flags = a->flags;
+    const int B = a->batch_size, F = a->num_faces, S = a->image_size;
+    const float sigma = a->sigma;
+    if (!soft_sizes_ok(B, F, S) || !isfinite(sigma) || !(sigma > 0.0f)) return false;
+    if (!nr_internal::make_face_src(flags, a->faces, a->vertices, a->face_indices, F, a->num_vertices, &p->src)) return false;
+    if (backward) {
+        const bool indexed = (flags & NR_FACES_INDEXED) != 0;
+        if (indexed ? a->grad_faces != nullptr : a->grad_vertices != nullptr) return false;
+        if (!nr_internal::make_face_grad(flags, a->grad_faces, a->grad_vertices, a->face_indices, F, a->num_vertices, &p->dst))
+            return false;
+    }
+    p->alpha = a->alpha; p->g = a->grad_alpha;
+    p->B = B; p->F = F; p->S = S;
+    p->ntx = tiles_per_axis(S); p->ntiles = p->ntx * p->ntx;
+    const double cut = (double)sigma * log((1.0 - NR_SOFT_EPS) / NR_SOFT_EPS);
+    p->inv_sigma = (float)(1.0 / (double)sigma);
+    p->cut = (float)cut;
+    p->reach = (float)(sqrt(cut) * S * 0.5) + 1.0f;
+    p->near_ = a->near_; p->far_ = a->far_;
+    return true;
+}
+
+// The start of every tile binning: the counters zeroed, k_soft_setup (face records, tile boxes, counts) and the scan
+// (list offsets).  A template so that only the units that call it instantiate k_soft_setup.
+template <typename = void>
+int bin_prefix(const SoftParams& p, cudaStream_t s) {
+    nr_internal::prof_begin("memset_soft_bins", s);
+    if (cudaMemsetAsync(p.cnt, 0, 2 * (size_t)p.B * (p.ntiles + 1) * sizeof(int), s) != cudaSuccess) return NR_ERR_CUDA;
+    nr_internal::prof_end(s);
+    {
+        nr_internal::LaunchScope ls("k_soft_setup", s);
+        k_soft_setup<false><<<dim3((unsigned)((p.F + 255) / 256), (unsigned)p.B), 256, 0, s>>>(p);
+    }
+    nr_internal::strip_scan(p.cnt, p.off, p.ntiles + 1, (long long)p.F * kWideTiles, p.B, s);
+    return NR_OK;
 }
 
 }  // namespace

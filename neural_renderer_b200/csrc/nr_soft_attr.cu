@@ -2,8 +2,8 @@
 // include/nr_b200.h): the soft RGB's aggregation with a C-channel colour A_jc = sum_k l'_k a_kc interpolated from
 // per-corner or per-vertex attributes (per-vertex colours, soft depth, normals, features).
 //
-// The host checks, the workspace and the binning (setup, scan, keys, sort) are nr_soft_rgb.cu's (nr_internal.h); the
-// face staging, the barycentrics and the sigmoid are nr_soft_rgb.cuh's; the chain from l'_k into the vertices is
+// The host checks, the workspace and the binning (keys, sort) are nr_soft_rgb.cu's (nr_internal.h), on the parameter
+// fill and the binning start (setup, scan) of nr_soft.cuh; the gradient zero-fill is nr_internal.h's; the face staging, the barycentrics and the sigmoid are nr_soft_rgb.cuh's; the chain from l'_k into the vertices is
 // k_soft_uv_bwd's (a copy, soft_lprime_chain).  New kernels, each for 32- and 64-bit keys and
 // for channel blocks of kCB = 4 or 16:
 //   k_soft_attr_fwd<K, kCB>  the traversal of k_soft_rgb_fwd with kCB numerators per pixel in registers; grid.z runs the
@@ -476,16 +476,10 @@ extern "C" int nr_b200_soft_attributes_backward(const nr_b200_soft_rgb_args* arg
     const int rc = soft_attr_setup(args, attr, true, &p, &L, &attr_floats);
     if (rc != NR_OK) return rc;
     const nr_b200_soft_rgb_args* a = args;
-    const bool indexed = (a->flags & NR_FACES_INDEXED) != 0;
     cudaStream_t s = (cudaStream_t)cuda_stream;
-    if (!(a->flags & NR_GRAD_ACCUMULATE)) {
-        nr_internal::prof_begin("memset_grads", s);
-        cudaError_t e = indexed ? cudaMemsetAsync(a->grad_vertices, 0, (size_t)p.r.s.B * a->num_vertices * 3 * sizeof(float), s)
-                                : cudaMemsetAsync(a->grad_faces, 0, (size_t)p.r.s.B * p.r.s.F * 9 * sizeof(float), s);
-        if (e == cudaSuccess && p.gattr) e = cudaMemsetAsync(p.gattr, 0, attr_floats * sizeof(float), s);
-        nr_internal::prof_end(s);
-        if (e != cudaSuccess) return NR_ERR_CUDA;
-    }
+    if (!(a->flags & NR_GRAD_ACCUMULATE) &&
+        nr_internal::zero_grads({nr_internal::geometry_grad(a), {p.gattr, attr_floats * sizeof(float)}}, s) != cudaSuccess)
+        return NR_ERR_CUDA;
     if (!a->grad_alpha && !attr->grad_out) return cudaGetLastError() == cudaSuccess ? NR_OK : NR_ERR_CUDA;
     return soft_attr_run(p, L, true, s);
 }

@@ -367,15 +367,9 @@ extern "C" int nr_b200_soft_fragments_backward(const nr_b200_soft_rgb_args* args
     const int rc = soft_frag_setup(args, frag, true, &p, &L);
     if (rc != NR_OK) return rc;
     const nr_b200_soft_rgb_args* a = args;
-    const bool indexed = (a->flags & NR_FACES_INDEXED) != 0;
     cudaStream_t s = (cudaStream_t)cuda_stream;
-    if (!(a->flags & NR_GRAD_ACCUMULATE)) {
-        nr_internal::prof_begin("memset_grads", s);
-        const cudaError_t e = indexed ? cudaMemsetAsync(a->grad_vertices, 0, (size_t)p.r.s.B * a->num_vertices * 3 * sizeof(float), s)
-                                      : cudaMemsetAsync(a->grad_faces, 0, (size_t)p.r.s.B * p.r.s.F * 9 * sizeof(float), s);
-        nr_internal::prof_end(s);
-        if (e != cudaSuccess) return NR_ERR_CUDA;
-    }
+    if (!(a->flags & NR_GRAD_ACCUMULATE) && nr_internal::zero_grads({nr_internal::geometry_grad(a)}, s) != cudaSuccess)
+        return NR_ERR_CUDA;
     if (!frag->grad_zbuf && !frag->grad_bary && !frag->grad_dists)
         return cudaGetLastError() == cudaSuccess ? NR_OK : NR_ERR_CUDA;
     // the records and depth records of the binning; its lists are not read

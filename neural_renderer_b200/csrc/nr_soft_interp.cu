@@ -312,12 +312,8 @@ extern "C" int nr_b200_interpolate_fragments_backward(const nr_b200_frag_interp_
     const int rc = interp_setup(args, true, &p, &nattr);
     if (rc != NR_OK) return rc;
     cudaStream_t s = (cudaStream_t)cuda_stream;
-    if (p.gattr && !p.accumulate) {
-        nr_internal::prof_begin("memset_grads", s);
-        const cudaError_t e = cudaMemsetAsync(p.gattr, 0, nattr * sizeof(float), s);
-        nr_internal::prof_end(s);
-        if (e != cudaSuccess) return NR_ERR_CUDA;
-    }
+    if (p.gattr && !p.accumulate && nr_internal::zero_grads({{p.gattr, nattr * sizeof(float)}}, s) != cudaSuccess)
+        return NR_ERR_CUDA;
     // without an upstream gradient the attribute gradient stays as it is; grad_bary still gets its zeros
     if (!p.gbary && !p.g) return cudaGetLastError() == cudaSuccess ? NR_OK : NR_ERR_CUDA;
     p.G = p.K >= kWarpsB ? 1 : (kWarpsB + p.K - 1) / p.K;

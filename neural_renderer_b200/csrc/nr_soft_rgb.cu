@@ -13,7 +13,7 @@
 //                     light channels) reduced over the warp and the CTA; the 8-tap texture scatters of a warp merged in a
 //                     per-warp shared-memory cube when ts^3 3 <= kWarpCube, then flushed to global memory
 // The forward traversal is nr_soft_rgb.cuh's, with the cube sampler below.  The host checks, the workspace layout and
-// the binning are shared with nr_soft_uv.cu through nr_internal.h.
+// the binning below serve the texture-image, attribute and fragment units too (nr_internal.h).
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
@@ -330,15 +330,8 @@ constexpr uint32_t kSoftRgbFlags = NR_FACES_INDEXED | NR_INDICES_SHARED | NR_TEX
 template <typename K>
 int bin_faces_rgb(SoftRgbParams& p, const SoftRgbLayout& L, bool sort, cudaStream_t s) {
     const SoftParams& q = p.s;
-    nr_internal::prof_begin("memset_soft_bins", s);
-    if (cudaMemsetAsync(q.cnt, 0, 2 * (size_t)q.B * (q.ntiles + 1) * sizeof(int), s) != cudaSuccess) return NR_ERR_CUDA;
-    nr_internal::prof_end(s);
+    if (bin_prefix(q, s) != NR_OK) return NR_ERR_CUDA;
     const dim3 grid((unsigned)((q.F + 255) / 256), (unsigned)q.B);
-    {
-        nr_internal::LaunchScope ls("k_soft_setup", s);
-        k_soft_setup<false><<<grid, 256, 0, s>>>(q);
-    }
-    nr_internal::strip_scan(q.cnt, q.off, q.ntiles + 1, (long long)q.F * kWideTiles, q.B, s);
     const size_t cap = (size_t)q.B * q.F * kWideTiles;
     if (sort) {
         nr_internal::LaunchScope ls("k_soft_rgb_keys", s);
@@ -388,34 +381,17 @@ int soft_rgb_check(const nr_b200_soft_rgb_args* a, uint32_t allowed, SoftColourS
     if (!a || a->struct_size != sizeof(nr_b200_soft_rgb_args)) return NR_ERR_INVALID_ARG;
     const uint32_t flags = a->flags;
     if (flags & ~allowed) return NR_ERR_INVALID_ARG;
-    const int B = a->batch_size, F = a->num_faces, S = a->image_size, ts = a->texture_size;
-    if (!soft_sizes_ok(B, F, S)) return NR_ERR_INVALID_ARG;
-    const float sigma = a->sigma, gamma = a->gamma;
-    if (!isfinite(sigma) || !(sigma > 0.0f) || (softmax && (!isfinite(gamma) || !(gamma > 0.0f)))) return NR_ERR_INVALID_ARG;
+    const int ts = a->texture_size;
+    const float gamma = a->gamma;
+    if (softmax && (!isfinite(gamma) || !(gamma > 0.0f))) return NR_ERR_INVALID_ARG;
     if (!(a->near_ < a->far_) || !isfinite(a->far_ - a->near_) || (cubes && !isfinite(a->eps))) return NR_ERR_INVALID_ARG;
-    memset(p, 0, sizeof(*p));
-    if (!make_face_src(flags, a->faces, a->vertices, a->face_indices, F, a->num_vertices, &p->s.src))
-        return NR_ERR_INVALID_ARG;
     if ((colour && !a->textures) || (cubes && (ts < 2 || (long long)ts * ts * ts * 3 > 0x7FFFFFFFll))) return NR_ERR_INVALID_ARG;
     if ((colour && !a->rgb) || (softmax && (!a->alpha || !a->state))) return NR_ERR_INVALID_ARG;
-    if (backward) {
-        const bool indexed = (flags & NR_FACES_INDEXED) != 0;
-        if (indexed ? a->grad_faces != nullptr : a->grad_vertices != nullptr) return NR_ERR_INVALID_ARG;
-        if (!make_face_grad(flags, a->grad_faces, a->grad_vertices, a->face_indices, F, a->num_vertices, &p->s.dst))
-            return NR_ERR_INVALID_ARG;
-    }
-    SoftParams& s = p->s;
-    s.alpha = a->alpha; s.g = a->grad_alpha;
-    s.B = B; s.F = F; s.S = S;
-    s.ntx = tiles_per_axis(S); s.ntiles = s.ntx * s.ntx;
-    const double cut = (double)sigma * log((1.0 - NR_SOFT_EPS) / NR_SOFT_EPS);
-    s.inv_sigma = (float)(1.0 / (double)sigma);
-    s.cut = (float)cut;
-    s.reach = (float)(sqrt(cut) * S * 0.5) + 1.0f;
-    s.near_ = a->near_; s.far_ = a->far_;
+    memset(p, 0, sizeof(*p));
+    if (!fill_soft_params(a, backward, &p->s)) return NR_ERR_INVALID_ARG;
     if (cubes) {
         p->tex.tex = a->textures;
-        p->tex.cube_bstride = (flags & NR_TEX_SHARED) ? 0 : (size_t)F;
+        p->tex.cube_bstride = (flags & NR_TEX_SHARED) ? 0 : (size_t)a->num_faces;
         const double tmax = (double)(ts - 1) - a->eps;
         p->tex.tex_cmp = float_le(tmax);
         p->tex.tex_val = (float)tmax;
@@ -489,20 +465,15 @@ extern "C" int nr_b200_soft_rgb_backward(const nr_b200_soft_rgb_args* args, void
     const int rc = soft_rgb_setup(args, true, &p, &L);
     if (rc != NR_OK) return rc;
     const nr_b200_soft_rgb_args* a = args;
-    const bool indexed = (a->flags & NR_FACES_INDEXED) != 0;
     cudaStream_t s = (cudaStream_t)cuda_stream;
     if (!(a->flags & NR_GRAD_ACCUMULATE)) {
-        nr_internal::prof_begin("memset_grads", s);
-        cudaError_t e = indexed ? cudaMemsetAsync(a->grad_vertices, 0, (size_t)p.s.B * a->num_vertices * 3 * sizeof(float), s)
-                                : cudaMemsetAsync(a->grad_faces, 0, (size_t)p.s.B * p.s.F * 9 * sizeof(float), s);
         const size_t cube = (size_t)p.ts * p.ts * p.ts * 3;
         const size_t tex_items = (a->flags & NR_TEX_SHARED) ? 1 : (size_t)p.s.B;
-        if (e == cudaSuccess && a->grad_textures)
-            e = cudaMemsetAsync(a->grad_textures, 0, tex_items * p.s.F * cube * sizeof(float), s);
-        if (e == cudaSuccess && a->grad_face_light)
-            e = cudaMemsetAsync(a->grad_face_light, 0, (size_t)p.s.B * p.s.F * 3 * sizeof(float), s);
-        nr_internal::prof_end(s);
-        if (e != cudaSuccess) return NR_ERR_CUDA;
+        if (nr_internal::zero_grads({nr_internal::geometry_grad(a),
+                                     {a->grad_textures, tex_items * p.s.F * cube * sizeof(float)},
+                                     {a->grad_face_light, (size_t)p.s.B * p.s.F * 3 * sizeof(float)}},
+                                    s) != cudaSuccess)
+            return NR_ERR_CUDA;
     }
     if (!a->grad_alpha && !a->grad_rgb) return cudaGetLastError() == cudaSuccess ? NR_OK : NR_ERR_CUDA;
     if ((L.wide ? soft_rgb_backward<unsigned long long>(p, L, s) : soft_rgb_backward<uint32_t>(p, L, s)) != NR_OK)

@@ -397,19 +397,13 @@ extern "C" int nr_b200_soft_rgb_uv_backward(const nr_b200_soft_rgb_args* args, c
     const int rc = soft_uv_setup(args, uv, true, &p, &L, &tex_floats, &uv_floats);
     if (rc != NR_OK) return rc;
     const nr_b200_soft_rgb_args* a = args;
-    const bool indexed = (a->flags & NR_FACES_INDEXED) != 0;
     cudaStream_t s = (cudaStream_t)cuda_stream;
-    if (!(a->flags & NR_GRAD_ACCUMULATE)) {
-        nr_internal::prof_begin("memset_grads", s);
-        cudaError_t e = indexed ? cudaMemsetAsync(a->grad_vertices, 0, (size_t)p.r.s.B * a->num_vertices * 3 * sizeof(float), s)
-                                : cudaMemsetAsync(a->grad_faces, 0, (size_t)p.r.s.B * p.r.s.F * 9 * sizeof(float), s);
-        if (e == cudaSuccess && a->grad_textures) e = cudaMemsetAsync(a->grad_textures, 0, tex_floats * sizeof(float), s);
-        if (e == cudaSuccess && a->grad_face_light)
-            e = cudaMemsetAsync(a->grad_face_light, 0, (size_t)p.r.s.B * p.r.s.F * 3 * sizeof(float), s);
-        if (e == cudaSuccess && p.grad_uvs) e = cudaMemsetAsync(p.grad_uvs, 0, uv_floats * sizeof(float), s);
-        nr_internal::prof_end(s);
-        if (e != cudaSuccess) return NR_ERR_CUDA;
-    }
+    if (!(a->flags & NR_GRAD_ACCUMULATE) &&
+        nr_internal::zero_grads({nr_internal::geometry_grad(a), {a->grad_textures, tex_floats * sizeof(float)},
+                                 {a->grad_face_light, (size_t)p.r.s.B * p.r.s.F * 3 * sizeof(float)},
+                                 {p.grad_uvs, uv_floats * sizeof(float)}},
+                                s) != cudaSuccess)
+        return NR_ERR_CUDA;
     if (!a->grad_alpha && !a->grad_rgb) return cudaGetLastError() == cudaSuccess ? NR_OK : NR_ERR_CUDA;
     return soft_uv_run(p, L, true, s);
 }

@@ -310,6 +310,42 @@ def _stream_ptr(device):
     return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
+def _index_set(indices):
+    """integer faces [F,3] / [1|B,F,3] as int32; an expanded [F,3] index set (Mesh.get_batch) stays one shared set and is
+    not materialised"""
+    if indices.dim() == 3 and indices.shape[0] > 1 and indices.stride(0) == 0:
+        indices = indices[:1]
+    return indices.to(torch.int32).contiguous()
+
+
+def _geometry(faces, vertices):
+    """(geom, indices) of a call: vertices as float32 with faces as its index set, or faces as float32 and None"""
+    if vertices is None:
+        return (faces if faces.dtype == torch.float32 else faces.float()), None
+    return (vertices if vertices.dtype == torch.float32 else vertices.float()), _index_set(faces)
+
+
+def _set_geometry(a, geom_c, indices):
+    """the geometry fields of an args struct (faces, or vertices / face_indices / num_vertices, and num_faces); returns
+    its geometry flags (a 2-D index set is shared, as is a batch of 1 with a larger geometry batch)"""
+    if indices is None:
+        a.faces, a.num_faces = _ptr(geom_c), geom_c.shape[1]
+        return 0
+    a.vertices, a.face_indices, a.num_vertices = _ptr(geom_c), _ptr(indices), geom_c.shape[1]
+    a.num_faces = indices.shape[-2]
+    if indices.dim() == 2 or (indices.shape[0] == 1 and geom_c.shape[0] > 1):
+        return _lib.NR_FACES_INDEXED | _lib.NR_INDICES_SHARED
+    return _lib.NR_FACES_INDEXED
+
+
+def _set_geometry_grad(a, indices, grad_geom):
+    """the geometry gradient field of an args struct: grad_vertices when indexed, else grad_faces"""
+    if indices is not None:
+        a.grad_vertices = _ptr(grad_geom)
+    else:
+        a.grad_faces = _ptr(grad_geom)
+
+
 class _RasterizeFunction(torch.autograd.Function):
     """autograd node of the hot path: forward = nr_b200_forward, backward = nr_b200_backward.
 
@@ -449,13 +485,10 @@ class _RasterizeFunction(torch.autograd.Function):
             ws = torch.empty((max(ws_bytes, 16),), dtype=torch.uint8, device=dev)
             a = _lib.BackwardArgs()
             a.struct_size = ctypes.sizeof(_lib.BackwardArgs)
-            a.batch_size, a.num_faces, a.raster_size, a.texture_size = B, F, cfg.S, ctx.ts
+            a.batch_size, a.raster_size, a.texture_size = B, cfg.S, ctx.ts
             a.eps = cfg.eps
-            if indices is not None:
-                a.vertices, a.face_indices, a.num_vertices = _ptr(geom_c), _ptr(indices), geom_c.shape[1]
-                a.grad_vertices = _ptr(grad_geom)
-            else:
-                a.faces, a.grad_faces = _ptr(geom_c), _ptr(grad_geom)
+            _set_geometry(a, geom_c, indices)  # and num_faces = F
+            _set_geometry_grad(a, indices, grad_geom)
             a.textures = _ptr(tex_c)
             a.face_uvs, (a.texture_height, a.texture_width) = _ptr(uv_c), ctx.tex_hw
             a.face_light, a.grad_face_light = _ptr(light_c), _ptr(grad_light)
@@ -613,15 +646,7 @@ def _run(faces, textures, image_size, anti_aliasing, near, far, eps, background_
     _check_inputs(faces, textures, return_rgb, face_light, textures_fill_back, vertices, face_uvs, corner_light,
                   corner_shading, shading_params, lights, environment_sh, normal_map, corner_tangents, specular_map)
     phong = [corner_shading, shading_params, lights, environment_sh, normal_map, corner_tangents, specular_map]
-    indices = None
-    if vertices is not None:
-        geom = vertices if vertices.dtype == torch.float32 else vertices.float()
-        indices = faces
-        if indices.dim() == 3 and indices.shape[0] > 1 and indices.stride(0) == 0:
-            indices = indices[:1]  # an expanded [F,3] index set (Mesh.get_batch): keep it shared, do not materialise
-        indices = indices.to(torch.int32).contiguous()
-    else:
-        geom = faces if faces.dtype == torch.float32 else faces.float()
+    geom, indices = _geometry(faces, vertices)
     batch_size = geom.shape[0]
     if not return_rgb:
         face_uvs = None
@@ -882,10 +907,7 @@ class _InterpolateFunction(torch.autograd.Function):
             grad_attr = torch.empty_like(attr_c) if want_attr else None
             a = _interpolate_args(geom_c, attr_c, fim, wmap, indices, ctx.flags, ctx.S)
             a.grad_out, a.grad_attributes = _ptr(g), _ptr(grad_attr)
-            if indices is not None:
-                a.grad_vertices = _ptr(grad_geom)
-            else:
-                a.grad_faces = _ptr(grad_geom)
+            _set_geometry_grad(a, indices, grad_geom)
             _lib.check(lib.nr_b200_interpolate_backward(ctypes.byref(a), _stream_ptr(dev)))
         return grad_geom, grad_attr, None, None, None, None, None
 
@@ -894,14 +916,7 @@ def _interpolate_args(geom_c, attr_c, fim, wmap, indices, flags, S):
     a = _lib.InterpolateArgs()
     a.struct_size = ctypes.sizeof(_lib.InterpolateArgs)
     B = geom_c.shape[0]
-    if indices is not None:
-        flags |= _lib.NR_FACES_INDEXED
-        if indices.dim() == 2 or (indices.shape[0] == 1 and B > 1):
-            flags |= _lib.NR_INDICES_SHARED
-        a.vertices, a.face_indices, a.num_vertices = _ptr(geom_c), _ptr(indices), geom_c.shape[1]
-        a.num_faces = indices.shape[-2]
-    else:
-        a.faces, a.num_faces = _ptr(geom_c), geom_c.shape[1]
+    flags |= _set_geometry(a, geom_c, indices)
     if attr_c.shape[0] == 1 and B > 1:
         flags |= _lib.NR_ATTR_SHARED
     a.flags = flags
@@ -974,15 +989,7 @@ def rasterize_attributes(
     alpha image of `return_alpha=True`, which is the rasterizer's and carries its usual silhouette gradient.  Returns
     the image, or (image, alpha)."""
     attrs, per_vertex = _check_attribute_inputs(faces, vertices, vertex_attributes, face_attributes)
-    indices = None
-    if vertices is not None:
-        geom = vertices if vertices.dtype == torch.float32 else vertices.float()
-        indices = faces
-        if indices.dim() == 3 and indices.shape[0] > 1 and indices.stride(0) == 0:
-            indices = indices[:1]
-        indices = indices.to(torch.int32).contiguous()
-    else:
-        geom = faces if faces.dtype == torch.float32 else faces.float()
+    geom, indices = _geometry(faces, vertices)
     batch_size = geom.shape[0]
     attrs = _batched(attrs, batch_size, 2 if per_vertex else 3)  # an expanded shared set: NR_ATTR_SHARED
     _, alpha, _, fim, wmap = _run(indices if indices is not None else geom, None, image_size, anti_aliasing, near, far,
@@ -994,6 +1001,16 @@ def rasterize_attributes(
 
 
 DEFAULT_SOFT_SIGMA = 1e-5
+
+
+def _positive_number(name, v):
+    try:
+        v = float(v)
+    except (TypeError, ValueError):
+        raise TypeError("%s must be a number, got %r" % (name, v))
+    if not math.isfinite(v) or v <= 0:
+        raise ValueError("%s must be finite and > 0, got %r" % (name, v))
+    return v
 
 
 class _SoftSilhouettesFunction(torch.autograd.Function):
@@ -1026,10 +1043,7 @@ class _SoftSilhouettesFunction(torch.autograd.Function):
             grad_geom = torch.empty_like(geom_c)
             a, ws = _soft_args(lib, geom_c, indices, *ctx.cfg)
             a.alpha, a.grad_alpha = _ptr(alpha), _ptr(g)
-            if indices is not None:
-                a.grad_vertices = _ptr(grad_geom)
-            else:
-                a.grad_faces = _ptr(grad_geom)
+            _set_geometry_grad(a, indices, grad_geom)
             _lib.check(lib.nr_b200_soft_silhouettes_backward(ctypes.byref(a), _stream_ptr(dev)))
         return grad_geom, None, None, None, None, None
 
@@ -1039,19 +1053,10 @@ def _soft_args(lib, geom_c, indices, S, sigma, near, far):
     a = _lib.SoftArgs()
     a.struct_size = ctypes.sizeof(_lib.SoftArgs)
     B = geom_c.shape[0]
-    flags = 0
-    if indices is not None:
-        flags |= _lib.NR_FACES_INDEXED
-        if indices.dim() == 2 or (indices.shape[0] == 1 and B > 1):
-            flags |= _lib.NR_INDICES_SHARED
-        a.vertices, a.face_indices, a.num_vertices = _ptr(geom_c), _ptr(indices), geom_c.shape[1]
-        a.num_faces = indices.shape[-2]
-    else:
-        a.faces, a.num_faces = _ptr(geom_c), geom_c.shape[1]
-    a.flags = flags
+    a.flags = _set_geometry(a, geom_c, indices)
     a.batch_size, a.image_size = B, S
     a.sigma, a.near_, a.far_ = sigma, near, far
-    n = lib.nr_b200_soft_workspace_bytes(B, a.num_faces, S, sigma, flags)
+    n = lib.nr_b200_soft_workspace_bytes(B, a.num_faces, S, sigma, a.flags)
     if n == 0:
         raise ValueError("rasterize_soft_silhouettes: sizes out of range (batch %d, %d faces, image %d)" % (B, a.num_faces, S))
     ws = torch.empty(n, dtype=torch.uint8, device=geom_c.device)
@@ -1080,28 +1085,13 @@ def rasterize_soft_silhouettes(
     per-pixel depth test).  sigma > 0 sets the softness: the reach is sqrt(sigma ln((1-eps)/eps)) image_size / 2 pixels
     with eps = 1e-4, about 1.2 px at 256 x 256 for the default 1e-5.  No anti-aliasing; deterministic forward.  The exact
     definition and its gradient are in include/nr_b200.h (nr_b200_soft_args)."""
-    try:
-        sigma = float(sigma)
-    except (TypeError, ValueError):
-        raise TypeError("sigma must be a number, got %r" % (sigma,))
-    if not math.isfinite(sigma) or sigma <= 0:
-        raise ValueError("sigma must be finite and > 0, got %r" % (sigma,))
+    sigma = _positive_number("sigma", sigma)
     if not (float(near) <= float(far)):
         raise ValueError("near must be <= far, got near=%r far=%r" % (near, far))
     if int(image_size) < 1:
         raise ValueError("image_size must be >= 1, got %r" % (image_size,))
     _check_inputs(faces, None, False, vertices=vertices)  # the geometry, then the device check
-    indices = None
-    if vertices is not None:
-        geom = vertices if vertices.dtype == torch.float32 else vertices.float()
-        indices = faces
-        if indices.dim() == 3 and indices.shape[0] > 1 and indices.stride(0) == 0:
-            indices = indices[:1]
-        indices = indices.to(torch.int32).contiguous()
-    else:
-        geom = faces if faces.dtype == torch.float32 else faces.float()
-        if not geom.is_cuda:
-            raise NotImplementedError("neural_renderer_b200 has no CPU implementation (inputs must be CUDA tensors)")
+    geom, indices = _geometry(faces, vertices)
     return _SoftSilhouettesFunction.apply(geom, indices, int(image_size), sigma, float(near), float(far))
 
 
@@ -1109,88 +1099,11 @@ DEFAULT_SOFT_GAMMA = 1e-4
 
 
 class _SoftRgbFunction(torch.autograd.Function):
-    """autograd node of the soft RGB: forward = nr_b200_soft_rgb, backward = nr_b200_soft_rgb_backward from the saved
-    rgb, alpha and state.  `geom` / `indices` as _RasterizeFunction; `textures` [B|1,F,ts,ts,ts,3] (1 = shared)."""
-
-    @staticmethod
-    def forward(ctx, geom, textures, face_light, indices, cfg):
-        lib = _lib.load()
-        dev = geom.device
-        geom_c = geom.detach().contiguous()
-        tex_c = textures.detach().contiguous()
-        light_c = face_light.detach().contiguous() if face_light is not None else None
-        B, S = geom_c.shape[0], cfg[0]
-        with torch.cuda.device(dev):
-            rgb = torch.empty((B, 3, S, S), dtype=torch.float32, device=dev)
-            alpha = torch.empty((B, S, S), dtype=torch.float32, device=dev)
-            state = torch.empty((B, 2, S, S), dtype=torch.float32, device=dev)
-            a, ws = _soft_rgb_args(lib, geom_c, indices, tex_c, light_c, cfg)
-            a.rgb, a.alpha, a.state = _ptr(rgb), _ptr(alpha), _ptr(state)
-            _lib.check(lib.nr_b200_soft_rgb(ctypes.byref(a), _stream_ptr(dev)))
-        ctx.cfg = cfg
-        ctx.save_for_backward(geom_c, tex_c, light_c, indices, rgb, alpha, state)
-        return rgb, alpha
-
-    @staticmethod
-    def backward(ctx, g_rgb, g_alpha):
-        lib = _lib.load()
-        geom_c, tex_c, light_c, indices, rgb, alpha, state = ctx.saved_tensors
-        dev = geom_c.device
-        need_geom, need_tex, need_light = ctx.needs_input_grad[:3]
-        if not (need_geom or need_tex or need_light) or (g_rgb is None and g_alpha is None):
-            return None, None, None, None, None
-        g_rgb = g_rgb.detach().to(torch.float32).contiguous() if g_rgb is not None else None
-        g_alpha = g_alpha.detach().to(torch.float32).contiguous() if g_alpha is not None else None
-        with torch.cuda.device(dev):
-            grad_geom = torch.empty_like(geom_c)
-            grad_tex = torch.empty_like(tex_c) if need_tex else None
-            grad_light = torch.empty_like(light_c) if need_light and light_c is not None else None
-            a, ws = _soft_rgb_args(lib, geom_c, indices, tex_c, light_c, ctx.cfg)
-            a.rgb, a.alpha, a.state = _ptr(rgb), _ptr(alpha), _ptr(state)
-            a.grad_rgb, a.grad_alpha = _ptr(g_rgb), _ptr(g_alpha)
-            if indices is not None:
-                a.grad_vertices = _ptr(grad_geom)
-            else:
-                a.grad_faces = _ptr(grad_geom)
-            a.grad_textures, a.grad_face_light = _ptr(grad_tex), _ptr(grad_light)
-            _lib.check(lib.nr_b200_soft_rgb_backward(ctypes.byref(a), _stream_ptr(dev)))
-        return grad_geom if need_geom else None, grad_tex, grad_light, None, None
-
-
-def _soft_rgb_args(lib, geom_c, indices, tex_c, light_c, cfg):
-    """nr_b200_soft_rgb_args of a call and its workspace (returned so that it lives until the launch is queued)"""
-    S, sigma, gamma, near, far, eps, bg = cfg
-    a = _lib.SoftRgbArgs()
-    a.struct_size = ctypes.sizeof(_lib.SoftRgbArgs)
-    B = geom_c.shape[0]
-    flags = 0
-    if indices is not None:
-        flags |= _lib.NR_FACES_INDEXED
-        if indices.dim() == 2 or (indices.shape[0] == 1 and B > 1):
-            flags |= _lib.NR_INDICES_SHARED
-        a.vertices, a.face_indices, a.num_vertices = _ptr(geom_c), _ptr(indices), geom_c.shape[1]
-        a.num_faces = indices.shape[-2]
-    else:
-        a.faces, a.num_faces = _ptr(geom_c), geom_c.shape[1]
-    if tex_c.shape[0] == 1 and B > 1:
-        flags |= _lib.NR_TEX_SHARED
-    a.flags = flags
-    a.batch_size, a.image_size, a.texture_size = B, S, tex_c.shape[2]
-    a.sigma, a.gamma, a.near_, a.far_, a.eps = sigma, gamma, near, far, eps
-    a.background[:] = bg
-    a.textures, a.face_light = _ptr(tex_c), _ptr(light_c)
-    n = lib.nr_b200_soft_rgb_workspace_bytes(B, a.num_faces, S, flags)
-    if n == 0:
-        raise ValueError("rasterize_soft: sizes out of range (batch %d, %d faces, image %d)" % (B, a.num_faces, S))
-    ws = torch.empty(n, dtype=torch.uint8, device=geom_c.device)
-    a.workspace, a.workspace_bytes = _ptr(ws), n
-    return a, ws
-
-
-class _SoftUvFunction(torch.autograd.Function):
-    """autograd node of the soft RGB through a texture image: forward = nr_b200_soft_rgb_uv, backward =
-    nr_b200_soft_rgb_uv_backward.  `textures` is the image [B|1,Ht,Wt,3], or its packed pyramid [B|1,P,3] when `hw` =
-    (Ht, Wt) of level 0 is given (trilinear); `face_uvs` [B|1,F,3,2] (1 = shared)."""
+    """autograd node of the soft RGB: forward = nr_b200_soft_rgb_uv, backward = nr_b200_soft_rgb_uv_backward from the
+    saved rgb, alpha and state.  `geom` / `indices` as _RasterizeFunction.  Cubes: `textures` [B|1,F,ts,ts,ts,3]
+    (1 = shared) and `face_uvs` None, the NULL nr_b200_soft_uv_args of the cube call.  Texture image: `textures` is the
+    image [B|1,Ht,Wt,3], or its packed pyramid [B|1,P,3] when `hw` = (Ht, Wt) of level 0 is given (trilinear), and
+    `face_uvs` [B|1,F,3,2] (1 = shared)."""
 
     @staticmethod
     def forward(ctx, geom, textures, face_light, face_uvs, indices, cfg, hw):
@@ -1198,16 +1111,16 @@ class _SoftUvFunction(torch.autograd.Function):
         dev = geom.device
         geom_c = geom.detach().contiguous()
         tex_c = textures.detach().contiguous()
-        uv_c = face_uvs.detach().contiguous()
+        uv_c = face_uvs.detach().contiguous() if face_uvs is not None else None
         light_c = face_light.detach().contiguous() if face_light is not None else None
         B, S = geom_c.shape[0], cfg[0]
         with torch.cuda.device(dev):
             rgb = torch.empty((B, 3, S, S), dtype=torch.float32, device=dev)
             alpha = torch.empty((B, S, S), dtype=torch.float32, device=dev)
             state = torch.empty((B, 2, S, S), dtype=torch.float32, device=dev)
-            a, u, ws = _soft_uv_args(lib, geom_c, indices, tex_c, light_c, uv_c, cfg, hw)
+            a, u, ws = _soft_tex_args(lib, geom_c, indices, tex_c, light_c, uv_c, cfg, hw)
             a.rgb, a.alpha, a.state = _ptr(rgb), _ptr(alpha), _ptr(state)
-            _lib.check(lib.nr_b200_soft_rgb_uv(ctypes.byref(a), ctypes.byref(u), _stream_ptr(dev)))
+            _lib.check(lib.nr_b200_soft_rgb_uv(ctypes.byref(a), u, _stream_ptr(dev)))
         ctx.cfg, ctx.hw = cfg, hw
         ctx.save_for_backward(geom_c, tex_c, light_c, uv_c, indices, rgb, alpha, state)
         return rgb, alpha
@@ -1228,22 +1141,43 @@ class _SoftUvFunction(torch.autograd.Function):
             grad_tex = torch.empty_like(tex_c) if need_tex else None
             grad_light = torch.empty_like(light_c) if need_light and light_c is not None else None
             grad_uv = torch.empty_like(uv_c) if need_uv else None
-            a, u, ws = _soft_uv_args(lib, geom_c, indices, tex_c, light_c, uv_c, ctx.cfg, ctx.hw)
+            a, u, ws = _soft_tex_args(lib, geom_c, indices, tex_c, light_c, uv_c, ctx.cfg, ctx.hw, grad_uv)
             a.rgb, a.alpha, a.state = _ptr(rgb), _ptr(alpha), _ptr(state)
             a.grad_rgb, a.grad_alpha = _ptr(g_rgb), _ptr(g_alpha)
-            if indices is not None:
-                a.grad_vertices = _ptr(grad_geom)
-            else:
-                a.grad_faces = _ptr(grad_geom)
+            _set_geometry_grad(a, indices, grad_geom)
             a.grad_textures, a.grad_face_light = _ptr(grad_tex), _ptr(grad_light)
-            u.grad_face_uvs = _ptr(grad_uv)
-            _lib.check(lib.nr_b200_soft_rgb_uv_backward(ctypes.byref(a), ctypes.byref(u), _stream_ptr(dev)))
+            _lib.check(lib.nr_b200_soft_rgb_uv_backward(ctypes.byref(a), u, _stream_ptr(dev)))
         return grad_geom if need_geom else None, grad_tex, grad_light, grad_uv, None, None, None
 
 
-def _soft_uv_args(lib, geom_c, indices, tex_c, light_c, uv_c, cfg, hw):
-    """nr_b200_soft_rgb_args and nr_b200_soft_uv_args of a texture-image call, and the workspace (the cube call's)"""
-    a, ws = _soft_rgb_args(lib, geom_c, indices, tex_c, light_c, cfg)
+def _soft_rgb_args(lib, geom_c, indices, S, sigma, near, far, gamma=0.0, flags=0, name="rasterize_soft"):
+    """nr_b200_soft_rgb_args with the fields every soft RGB-family call sets (the geometry with its flags and `flags`,
+    the sizes, sigma, gamma, near and far) and its workspace (returned so that it lives until the launch is queued)"""
+    a = _lib.SoftRgbArgs()
+    a.struct_size = ctypes.sizeof(_lib.SoftRgbArgs)
+    B = geom_c.shape[0]
+    a.flags = flags | _set_geometry(a, geom_c, indices)
+    a.batch_size, a.image_size = B, S
+    a.sigma, a.gamma, a.near_, a.far_ = sigma, gamma, near, far
+    n = lib.nr_b200_soft_rgb_workspace_bytes(B, a.num_faces, S, a.flags)
+    if n == 0:
+        raise ValueError("%s: sizes out of range (batch %d, %d faces, image %d)" % (name, B, a.num_faces, S))
+    ws = torch.empty(n, dtype=torch.uint8, device=geom_c.device)
+    a.workspace, a.workspace_bytes = _ptr(ws), n
+    return a, ws
+
+
+def _soft_tex_args(lib, geom_c, indices, tex_c, light_c, uv_c, cfg, hw, grad_uv=None):
+    """nr_b200_soft_rgb_args of a soft RGB call, a reference to its nr_b200_soft_uv_args (None for cubes) and the
+    workspace"""
+    S, sigma, gamma, near, far, eps, bg = cfg
+    tex_shared = _lib.NR_TEX_SHARED if tex_c.shape[0] == 1 and geom_c.shape[0] > 1 else 0
+    a, ws = _soft_rgb_args(lib, geom_c, indices, S, sigma, near, far, gamma, tex_shared)
+    a.texture_size, a.eps = tex_c.shape[2], eps
+    a.background[:] = bg
+    a.textures, a.face_light = _ptr(tex_c), _ptr(light_c)
+    if uv_c is None:
+        return a, None, ws
     a.flags |= _lib.NR_TEX_UV
     if uv_c.shape[0] == 1 and geom_c.shape[0] > 1:
         a.flags |= _lib.NR_UV_SHARED
@@ -1252,8 +1186,8 @@ def _soft_uv_args(lib, geom_c, indices, tex_c, light_c, uv_c, cfg, hw):
     u = _lib.SoftUvArgs()
     u.struct_size = ctypes.sizeof(_lib.SoftUvArgs)
     u.texture_height, u.texture_width = hw if hw is not None else (tex_c.shape[1], tex_c.shape[2])
-    u.face_uvs = _ptr(uv_c)
-    return a, u, ws
+    u.face_uvs, u.grad_face_uvs = _ptr(uv_c), _ptr(grad_uv)
+    return a, ctypes.byref(u), ws
 
 
 def rasterize_soft(
@@ -1291,14 +1225,7 @@ def rasterize_soft(
     image [Ht,Wt,3] / [1|B,Ht,Wt,3] (row 0 = top) sampled at each face's perspective-correct UV: bilinearly, or through
     a mip pyramid with texture_filter='trilinear' (as rasterize_rgbad samples images).  Gradients then also reach the
     image and, when it requires grad, face_uvs (nr_b200_soft_uv_args)."""
-    try:
-        sigma, gamma = float(sigma), float(gamma)
-    except (TypeError, ValueError):
-        raise TypeError("sigma and gamma must be numbers, got %r, %r" % (sigma, gamma))
-    if not math.isfinite(sigma) or sigma <= 0:
-        raise ValueError("sigma must be finite and > 0, got %r" % (sigma,))
-    if not math.isfinite(gamma) or gamma <= 0:
-        raise ValueError("gamma must be finite and > 0, got %r" % (gamma,))
+    sigma, gamma = _positive_number("sigma", sigma), _positive_number("gamma", gamma)
     if not (float(near) < float(far)):
         raise ValueError("near must be < far, got near=%r far=%r" % (near, far))
     if int(image_size) < 1:
@@ -1314,31 +1241,23 @@ def rasterize_soft(
         raise ValueError("texture_filter='trilinear' samples a texture image: it needs face_uvs")
     # the shapes, then the device check
     _check_inputs(faces, textures, True, face_light=face_light, vertices=vertices, face_uvs=face_uvs)
-    indices = None
-    if vertices is not None:
-        geom = vertices if vertices.dtype == torch.float32 else vertices.float()
-        indices = faces
-        if indices.dim() == 3 and indices.shape[0] > 1 and indices.stride(0) == 0:
-            indices = indices[:1]
-        indices = indices.to(torch.int32).contiguous()
-    else:
-        geom = faces if faces.dtype == torch.float32 else faces.float()
+    geom, indices = _geometry(faces, vertices)
     if face_light is not None and face_light.dtype != torch.float32:
         face_light = face_light.float()
     cfg = (int(image_size), sigma, gamma, float(near), float(far), float(eps), tuple(bg))
+    hw = None
     if face_uvs is not None:
         batch_size = geom.shape[0]
         textures = _batched(textures, batch_size, 3)
         face_uvs = _batched(face_uvs, batch_size, 3)
-        hw = None
         if texture_filter == 'trilinear':
             hw = (int(textures.shape[1]), int(textures.shape[2]))
             textures = _MipPyramid.apply(textures)
-        return _SoftUvFunction.apply(geom, textures, face_light, face_uvs, indices, cfg, hw)
-    if textures.shape[0] > 1 and textures.stride(0) == 0:
-        textures = textures[:1]  # an expanded shared set stays one set
-    textures = textures if textures.dtype == torch.float32 else textures.float()
-    return _SoftRgbFunction.apply(geom, textures, face_light, indices, cfg)
+    else:
+        if textures.shape[0] > 1 and textures.stride(0) == 0:
+            textures = textures[:1]  # an expanded shared set stays one set
+        textures = textures if textures.dtype == torch.float32 else textures.float()
+    return _SoftRgbFunction.apply(geom, textures, face_light, face_uvs, indices, cfg, hw)
 
 
 class _SoftAttrFunction(torch.autograd.Function):
@@ -1381,10 +1300,7 @@ class _SoftAttrFunction(torch.autograd.Function):
             a, t, ws = _soft_attr_args(lib, geom_c, indices, attr_c, bg, ctx.per_vertex, ctx.cfg)
             a.alpha, a.state, a.grad_alpha = _ptr(alpha), _ptr(state), _ptr(g_alpha)
             t.out, t.grad_out, t.grad_attributes = _ptr(out), _ptr(g_out), _ptr(grad_attr)
-            if indices is not None:
-                a.grad_vertices = _ptr(grad_geom)
-            else:
-                a.grad_faces = _ptr(grad_geom)
+            _set_geometry_grad(a, indices, grad_geom)
             _lib.check(lib.nr_b200_soft_attributes_backward(ctypes.byref(a), ctypes.byref(t), _stream_ptr(dev)))
         return grad_geom if need_geom else None, grad_attr, None, None, None, None
 
@@ -1392,30 +1308,11 @@ class _SoftAttrFunction(torch.autograd.Function):
 def _soft_attr_args(lib, geom_c, indices, attr_c, bg, per_vertex, cfg):
     """nr_b200_soft_rgb_args and nr_b200_soft_attr_args of an attribute call, and the workspace (the soft RGB's)"""
     S, sigma, gamma, near, far = cfg
-    a = _lib.SoftRgbArgs()
-    a.struct_size = ctypes.sizeof(_lib.SoftRgbArgs)
-    B = geom_c.shape[0]
-    flags = 0
-    if indices is not None:
-        flags |= _lib.NR_FACES_INDEXED
-        if indices.dim() == 2 or (indices.shape[0] == 1 and B > 1):
-            flags |= _lib.NR_INDICES_SHARED
-        a.vertices, a.face_indices, a.num_vertices = _ptr(geom_c), _ptr(indices), geom_c.shape[1]
-        a.num_faces = indices.shape[-2]
-    else:
-        a.faces, a.num_faces = _ptr(geom_c), geom_c.shape[1]
-    n = lib.nr_b200_soft_rgb_workspace_bytes(B, a.num_faces, S, flags)
-    if n == 0:
-        raise ValueError("rasterize_soft_attributes: sizes out of range (batch %d, %d faces, image %d)" % (B, a.num_faces, S))
+    a, ws = _soft_rgb_args(lib, geom_c, indices, S, sigma, near, far, gamma, name="rasterize_soft_attributes")
     if per_vertex:
-        flags |= _lib.NR_ATTR_PER_VERTEX
-    if attr_c.shape[0] == 1 and B > 1:
-        flags |= _lib.NR_ATTR_SHARED
-    a.flags = flags
-    a.batch_size, a.image_size = B, S
-    a.sigma, a.gamma, a.near_, a.far_ = sigma, gamma, near, far
-    ws = torch.empty(n, dtype=torch.uint8, device=geom_c.device)
-    a.workspace, a.workspace_bytes = _ptr(ws), n
+        a.flags |= _lib.NR_ATTR_PER_VERTEX
+    if attr_c.shape[0] == 1 and geom_c.shape[0] > 1:
+        a.flags |= _lib.NR_ATTR_SHARED
     t = _lib.SoftAttrArgs()
     t.struct_size = ctypes.sizeof(_lib.SoftAttrArgs)
     t.channels = attr_c.shape[-1]
@@ -1470,14 +1367,7 @@ def rasterize_soft_attributes(
     and light constants are: the capture of a call with a sequence needs one eager call with the same values before it
     (the usual warm-up does that), and a sequence first seen during a capture, or a background tensor on the host,
     makes a synchronising host-to-device copy, which a capture refuses."""
-    try:
-        sigma, gamma = float(sigma), float(gamma)
-    except (TypeError, ValueError):
-        raise TypeError("sigma and gamma must be numbers, got %r, %r" % (sigma, gamma))
-    if not math.isfinite(sigma) or sigma <= 0:
-        raise ValueError("sigma must be finite and > 0, got %r" % (sigma,))
-    if not math.isfinite(gamma) or gamma <= 0:
-        raise ValueError("gamma must be finite and > 0, got %r" % (gamma,))
+    sigma, gamma = _positive_number("sigma", sigma), _positive_number("gamma", gamma)
     if not (float(near) < float(far)):
         raise ValueError("near must be < far, got near=%r far=%r" % (near, far))
     if int(image_size) < 1:
@@ -1496,15 +1386,7 @@ def rasterize_soft_attributes(
         if isinstance(attrs_in, torch.Tensor) and attrs_in.dim() >= 1 and n != attrs_in.shape[-1]:
             raise ValueError("background must have one value per channel (%d), got %d" % (attrs_in.shape[-1], n))
     attrs, per_vertex = _check_attribute_inputs(faces, vertices, vertex_attributes, face_attributes)  # then the device
-    indices = None
-    if vertices is not None:
-        geom = vertices if vertices.dtype == torch.float32 else vertices.float()
-        indices = faces
-        if indices.dim() == 3 and indices.shape[0] > 1 and indices.stride(0) == 0:
-            indices = indices[:1]
-        indices = indices.to(torch.int32).contiguous()
-    else:
-        geom = faces if faces.dtype == torch.float32 else faces.float()
+    geom, indices = _geometry(faces, vertices)
     attrs = _batched(attrs, geom.shape[0], 2 if per_vertex else 3)  # an expanded shared set: NR_ATTR_SHARED
     if isinstance(bg, torch.Tensor):
         bg = bg.to(device=geom.device, dtype=torch.float32).contiguous()
@@ -1557,10 +1439,7 @@ class _SoftFragFunction(torch.autograd.Function):
             a, t, ws = _soft_frag_args(lib, geom_c, indices, ctx.cfg)
             t.pix_to_face = _ptr(p2f)
             t.grad_zbuf, t.grad_bary, t.grad_dists = _ptr(g_zbuf), _ptr(g_bary), _ptr(g_dists)
-            if indices is not None:
-                a.grad_vertices = _ptr(grad_geom)
-            else:
-                a.grad_faces = _ptr(grad_geom)
+            _set_geometry_grad(a, indices, grad_geom)
             _lib.check(lib.nr_b200_soft_fragments_backward(ctypes.byref(a), ctypes.byref(t), _stream_ptr(dev)))
         return grad_geom, None, None
 
@@ -1568,26 +1447,7 @@ class _SoftFragFunction(torch.autograd.Function):
 def _soft_frag_args(lib, geom_c, indices, cfg):
     """nr_b200_soft_rgb_args and nr_b200_soft_frag_args of a fragment call, and the workspace (the soft RGB's)"""
     S, sigma, K, near, far = cfg
-    a = _lib.SoftRgbArgs()
-    a.struct_size = ctypes.sizeof(_lib.SoftRgbArgs)
-    B = geom_c.shape[0]
-    flags = 0
-    if indices is not None:
-        flags |= _lib.NR_FACES_INDEXED
-        if indices.dim() == 2 or (indices.shape[0] == 1 and B > 1):
-            flags |= _lib.NR_INDICES_SHARED
-        a.vertices, a.face_indices, a.num_vertices = _ptr(geom_c), _ptr(indices), geom_c.shape[1]
-        a.num_faces = indices.shape[-2]
-    else:
-        a.faces, a.num_faces = _ptr(geom_c), geom_c.shape[1]
-    n = lib.nr_b200_soft_rgb_workspace_bytes(B, a.num_faces, S, flags)
-    if n == 0:
-        raise ValueError("rasterize_soft_fragments: sizes out of range (batch %d, %d faces, image %d)" % (B, a.num_faces, S))
-    a.flags = flags
-    a.batch_size, a.image_size = B, S
-    a.sigma, a.near_, a.far_ = sigma, near, far
-    ws = torch.empty(n, dtype=torch.uint8, device=geom_c.device)
-    a.workspace, a.workspace_bytes = _ptr(ws), n
+    a, ws = _soft_rgb_args(lib, geom_c, indices, S, sigma, near, far, name="rasterize_soft_fragments")
     t = _lib.SoftFragArgs()
     t.struct_size = ctypes.sizeof(_lib.SoftFragArgs)
     t.faces_per_pixel = K
@@ -1619,12 +1479,7 @@ def rasterize_soft_fragments(
     inside and -d^2 outside in squared NDC units -- the opposite sign of PyTorch3D's).  Empty slots hold -1 in every
     field.  Row 0 is at the top.  Deterministic.  Gradients flow from zbuf, bary_coords and dists into the vertices'
     x, y and z with the selection held fixed.  The exact definition is in include/nr_b200.h (nr_b200_soft_frag_args)."""
-    try:
-        sigma = float(sigma)
-    except (TypeError, ValueError):
-        raise TypeError("sigma must be a number, got %r" % (sigma,))
-    if not math.isfinite(sigma) or sigma <= 0:
-        raise ValueError("sigma must be finite and > 0, got %r" % (sigma,))
+    sigma = _positive_number("sigma", sigma)
     if isinstance(faces_per_pixel, bool) or not hasattr(faces_per_pixel, "__index__"):
         raise TypeError("faces_per_pixel must be an integer, got %r" % (faces_per_pixel,))
     K = faces_per_pixel.__index__()
@@ -1635,17 +1490,7 @@ def rasterize_soft_fragments(
     if int(image_size) < 1:
         raise ValueError("image_size must be >= 1, got %r" % (image_size,))
     _check_inputs(faces, None, False, vertices=vertices)  # the geometry, then the device check
-    indices = None
-    if vertices is not None:
-        geom = vertices if vertices.dtype == torch.float32 else vertices.float()
-        indices = faces
-        if indices.dim() == 3 and indices.shape[0] > 1 and indices.stride(0) == 0:
-            indices = indices[:1]
-        indices = indices.to(torch.int32).contiguous()
-    else:
-        geom = faces if faces.dtype == torch.float32 else faces.float()
-        if not geom.is_cuda:
-            raise NotImplementedError("neural_renderer_b200 has no CPU implementation (inputs must be CUDA tensors)")
+    geom, indices = _geometry(faces, vertices)
     return Fragments(*_SoftFragFunction.apply(geom, indices, (int(image_size), sigma, K, float(near), float(far))))
 
 
@@ -1698,16 +1543,6 @@ def _blend_args(zbuf, dists, colors, p2f, bg, cfg):
     a.pix_to_face, a.zbuf, a.dists, a.colors = _ptr(p2f), _ptr(zbuf), _ptr(dists), _ptr(colors)
     a.background = _ptr(bg) if bg.numel() else None
     return a
-
-
-def _positive_number(name, v):
-    try:
-        v = float(v)
-    except (TypeError, ValueError):
-        raise TypeError("%s must be a number, got %r" % (name, v))
-    if not math.isfinite(v) or v <= 0:
-        raise ValueError("%s must be finite and > 0, got %r" % (name, v))
-    return v
 
 
 def blend_soft_fragments(fragments, colors, sigma, gamma, near=DEFAULT_NEAR, far=DEFAULT_FAR, background=None):
@@ -1903,12 +1738,9 @@ def interpolate_soft_fragments(fragments, face_attributes=None, *, vertex_attrib
     indices = None
     if per_vertex:
         flags |= _lib.NR_ATTR_PER_VERTEX
-        indices = faces
-        if indices.dim() == 3 and indices.shape[0] > 1 and indices.stride(0) == 0:
-            indices = indices[:1]
+        indices = _index_set(faces)
         if indices.dim() == 2 or (indices.shape[0] == 1 and B > 1):
             flags |= _lib.NR_INDICES_SHARED
-        indices = indices.to(torch.int32).contiguous()
     return _FragInterpFunction.apply(bary.to(torch.float32).contiguous(), attrs.contiguous(), p2f.contiguous(), indices,
                                      (flags, F))
 
